@@ -2,6 +2,7 @@
 """bench.py -- images/sec of the end-to-end VGG16 Faster R-CNN forward path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--precision bf16x3|bf16] [--impl b200|reference]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (config #2): synthetic 600x1000 image (uniform(0,255) - BGR means), random-init weights
@@ -21,6 +22,9 @@ Prints ONE JSON line (rank 0).  `value`   : device-timed (CUDA events) images/s,
                                             peak), a >= 200-image sustained run (vs the sustained peak), DRAM traffic and
                                             per-kernel HBM fractions from the committed ncu pass of this binary.
                                 `cpu_baseline`: the CPU oracle pipeline on this box's host cores (rank 0, N=1).
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step returned to its caller (count, prob, boxes,
+rois, scores, per-class keep lists) as DIR/<name>.npy (float32 / float64); the inputs are seeded, so two builds can be
+compared output for output.
 `--impl reference` times the reference-equivalent CPU pipeline instead (torch-CPU fp32 dense ops standing in for
 Chainer-NumPy -- Chainer is not installable offline -- plus the reference's own compiled cpu_nms.pyx when
 oracle/_ref holds it, else the C restatement).
@@ -34,7 +38,7 @@ import sys
 import threading
 import time
 
-# More hardware work queues than the default 8: the B200 arm keeps 4 lane streams, a copy stream and, in the reference-interface
+# More hardware work queues than the default 8: the device arm keeps 4 lane streams, a copy stream and, in the reference-interface
 # leg, a graph stream + a host-NMS stream per caller thread; with 8 queues unrelated streams alias onto one queue and a 30 us NMS
 # kernel can sit behind another thread's 1.4 ms graph (must be set before the CUDA context exists).
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
@@ -56,8 +60,8 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1421.6), d.get("hbm_gbs", 6571.9), "measured"
-    return 1590.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 3350.0, "fallback"
 
 
 class ClockSampler(object):
@@ -108,7 +112,7 @@ class ClockSampler(object):
 def cpu_pipeline_once(orc, params, x, info, ref_nms=None, raw=None):
     """One image through the reference-equivalent CPU path.  Returns (seconds, nms_seconds).
     raw: optional uint8 (h0,w0,3) BGR image -- then forward.py's img_preprocessing (34-45) is part of the timed work
-    and replaces `x`, like the B200 arm's e2e."""
+    and replaces `x`, like the device arm's e2e."""
     t0 = time.perf_counter()
     if raw is not None:
         x = orc.img_preprocessing(raw)[0][None]
@@ -175,7 +179,7 @@ def run_reference_arm(args, rank):
     x = None
     raw = np.random.default_rng(7).integers(0, 256, (375, 625, 3), dtype=np.uint8)     # resizes to 600x1000
     info = np.array([[H_IMG, W_IMG]], np.int32)
-    warm = max(args.warmup, 3)               # the same warm-up count as the B200 arm
+    warm = max(args.warmup, 3)               # the same warm-up count as the device arm
     for _ in range(warm):
         t_probe, _ = cpu_pipeline_once(orc, params, x, info, ref_nms, raw=raw)
     steps = args.steps
@@ -206,7 +210,7 @@ def run_reference_arm(args, rank):
     print(json.dumps(line), flush=True)
 
 
-# ----------------------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------------------- device arm
 def hbm_fractions(tj, table, peak_hbm):
     """Per-kernel HBM fractions (VERDICT r01 item 3): DRAM bytes of each launch from the ncu pass of this binary
     (profiles/r02_conv_stack_dram.json) over the launch's LIVE CUDA-event time where bench.py times it (the GEMM launches:
@@ -287,7 +291,7 @@ WORKLOAD = ("VGG16 Faster R-CNN forward + the caller's per-class NMS (forward.py
 def bench_config():
     """The SAME `config` object in both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "image": [H_IMG, W_IMG], "proposals": 300, "num_classes": 21,
-            "l2": "no L2 flush needed: the per-step working set (activations + weights, ~1.5 GB) exceeds the 126 MB L2 and 4 "
+            "l2": "no L2 flush needed: the per-step working set (activations + weights, ~1.5 GB) exceeds the 50 MB L2 and 4 "
                   "input images are rotated"}
 
 
@@ -345,6 +349,17 @@ def reference_api_image(model, x_var, info_var, nms, np_):
         dets = dets[keep, :]
         n_det += int((dets[:, -1] >= 0.8).sum())
     return prob.shape[0], n_det
+
+
+def dump_outputs(out_dir, plan):
+    """What the caller of the timed path receives for one image (ForwardPlan.unpack_result of its result block), as
+    float32 (values) / float64 (counts and indices) .npy files."""
+    os.makedirs(out_dir, exist_ok=True)
+    res = plan.unpack_result(plan.result.cpu().numpy())
+    for name, v in res.items():
+        a = np.asarray(v)
+        a = a.astype(np.float32) if a.dtype == np.float32 else a.astype(np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_b200_arm(args, rank, local_rank, world):
@@ -405,6 +420,8 @@ def run_b200_arm(args, rank, local_rank, world):
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pool.plans[(args.steps - 1) % len(pool)])
     R_last = int(plan.prop.count.item())
     n_conf_last = int(plan.det[2].sum().item())
     # tie-free-ness of the run (SURVEY 8d): distinct fg scores among the anchors of the last image
@@ -418,8 +435,8 @@ def run_b200_arm(args, rank, local_rank, world):
     e1.record()
     barrier()
     ms_single = e0.elapsed_time(e1)
-    # a sustained run (>= 200 images, whatever --steps says): the number to hold against bf16_tflops_sustained
-    n_sus = max(200, args.steps)
+    # a sustained run of the same length: the number to hold against bf16_tflops_sustained
+    n_sus = args.steps
     barrier()
     e0.record()
     pool.fork()
@@ -434,7 +451,7 @@ def run_b200_arm(args, rank, local_rank, world):
     table = conv_layer_table(plan, torch) if rank == 0 else None
     ms_max = shard.max_over_ranks(ms, device="cuda")          # slowest rank decides
     value = world * args.steps / (ms_max / 1e3)
-    # seeds 0-4 (SURVEY 8d): one image in flight, 20 images per seed, this rank
+    # seeds 0-4 (SURVEY 8d): one image in flight, --steps images per seed, this rank
     seed_rates = {}
     if rank == 0:
         for sd in range(5):
@@ -442,16 +459,16 @@ def run_b200_arm(args, rank, local_rank, world):
             plan.forward(xi)
             torch.cuda.synchronize()
             e0.record()
-            for _ in range(20):
+            for _ in range(args.steps):
                 plan.forward(xi)
             e1.record()
             torch.cuda.synchronize()
-            seed_rates[str(sd)] = {"images_per_s": 20e3 / e0.elapsed_time(e1), "proposals": int(plan.prop.count.item())}
+            seed_rates[str(sd)] = {"images_per_s": args.steps * 1e3 / e0.elapsed_time(e1), "proposals": int(plan.prop.count.item())}
     barrier()
 
     # The e2e legs run Python per image.  A full (generation-2) garbage collection in a process that has imported torch walks
-    # ~1M objects and takes 70-80 ms (measured: the "periodic stall" of round 1 and the 81 ms outliers of
-    # profiles/r02_host_api_profile.txt); a serving process moves its start-up objects out of the collector's way once.
+    # ~1M objects and stalls the caller for tens of milliseconds; a serving process moves its start-up objects out of the
+    # collector's way once.
     import gc
     gc.collect()
     gc.freeze()
@@ -560,7 +577,7 @@ def run_b200_arm(args, rank, local_rank, world):
     import sys as _sys
     old_switch = _sys.getswitchinterval()
     _sys.setswitchinterval(1e-4)
-    n_thr = max(args.steps, 6 * T)           # at least 6 images per caller thread, whatever --steps says (reported: e2e.images_timed)
+    n_thr = max(args.steps, T)               # at least 1 image per caller thread (reported: e2e.images_timed)
     per = [(n_thr + T - 1 - k) // T for k in range(T)]
 
     def threads_leg():
@@ -628,10 +645,10 @@ def run_b200_arm(args, rank, local_rank, world):
     if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")):
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             pk = json.load(f)
-    peak_burst = pk.get("bf16_tflops", 1590.0)
-    peak_sus = pk.get("bf16_tflops_sustained", 1421.6)
-    peak_hbm = pk.get("hbm_gbs", 6571.9)
-    peak_src = "MEASURED_PEAKS.json" if pk else "fallback (B200_PROFILING.md)"
+    peak_burst = pk.get("bf16_tflops", 989.0)
+    peak_sus = pk.get("bf16_tflops_sustained", 989.0)
+    peak_hbm = pk.get("hbm_gbs", 3350.0)
+    peak_src = "MEASURED_PEAKS.json" if pk else "fallback (H100 SXM data sheet: dense bf16 989 TFLOP/s, HBM3 3.35 TB/s at 700 W)"
     conv_rows = [r for r in table if " k3" in r[0] or "->64 k1" in r[0]]   # trunk + RPN convs (3x3 incl. conv1_1, the twin 1x1)
     conv_ms = sum(r[1] for r in conv_rows)
     all_ms = sum(r[1] for r in table)
@@ -646,7 +663,7 @@ def run_b200_arm(args, rank, local_rank, world):
     achieved = CONV_STACK_GFLOP / conv_ms          # GFLOP/ms == TFLOP/s (algorithmic flops)
     sus_ips = n_sus / (ms_sus / 1e3)               # per rank set: all ranks ran n_sus images in ms_sus
     roofline = {
-        "bound": "tensor", "kernel": "conv_gemm_kernel (tcgen05 implicit-GEMM; %d GEMM launches/step)" % len(table),
+        "bound": "tensor", "kernel": "conv_gemm_kernel (wgmma implicit-GEMM; %d GEMM launches/step)" % len(table),
         # isolated per-launch timings (a spin kernel ahead of every launch, clocks near max) -> the BURST peak applies
         "achieved": achieved, "peak": peak_burst, "unit": "TFLOP/s", "frac": achieved / peak_burst,
         "peak_source": "%s bf16_tflops (burst: every launch timed alone between CUDA events)" % peak_src,
@@ -658,7 +675,7 @@ def run_b200_arm(args, rank, local_rank, world):
                       "achieved": sus_ips * CONV_STACK_GFLOP / 1e3, "peak": peak_sus, "unit": "TFLOP/s",
                       "frac": sus_ips * CONV_STACK_GFLOP / 1e3 / peak_sus,
                       "executed_frac": sus_ips * CONV_STACK_GFLOP * exec_mult / 1e3 / peak_sus,
-                      "note": "whole forward steps (3 images in flight), conv-stack flops only in the numerator; "
+                      "note": "whole forward steps (--in-flight images in flight), conv-stack flops only in the numerator; "
                               "peak = bf16_tflops_sustained"},
         "traffic": traffic,     # DRAM read+write bytes of the conv-stack launches of one step (ncu pass of this binary)
         "traffic_source": traffic_src,
@@ -691,7 +708,7 @@ def run_b200_arm(args, rank, local_rank, world):
         "metric": "images/sec end-to-end VGG16 Faster R-CNN forward @600x1000",
         "value": value, "unit": "images/s", "n_gpus": world, "steps": args.steps, "warmup": warm,
         "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "bf16x3 (bf16 hi/lo split operands, 3 tcgen05 MMAs per product, fp32 accumulate)"
+        "dtype": "bf16x3 (bf16 hi/lo split operands, 3 wgmma products per product, fp32 accumulate)"
                  if args.precision == "bf16x3" else "bf16 (fp32 accumulate)",
         "data": "synthetic",
         "config": bench_config(),
@@ -958,6 +975,8 @@ def main():
     ap.add_argument("--smem-reserve-kb", type=int, default=0,
                     help="shared memory per SM the conv kernels leave to other streams' small kernels (tuning experiment)")
     ap.add_argument("--api-threads", type=int, default=8, help="caller threads of the reference-interface e2e leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="forward workload: write the last timed step's outputs as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--workload", default="forward", choices=["forward", "train_rpn", "train_rcnn", "resnet101"],
                     help="forward = the headline metric (default); train_rpn / resnet101 = secondary workloads (configs #5 / #4)")
     args = ap.parse_args()

@@ -38,7 +38,7 @@ void set_error(const char* fmt, ...);
 // ------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  The forward path is a chain of ~35 dependent kernels; launched with the
 // programmatic-stream-serialization attribute a kernel's CTAs may become resident while the previous kernel drains
-// (its CTAs exit one by one), run their prologue (barrier init, TMEM allocation, tensor-map prefetch, argument setup)
+// (its CTAs exit one by one), run their prologue (barrier init, tensor-map prefetch, argument setup)
 // and then block in grid_dep_wait() until the previous grid has completed and its writes are visible.  EVERY kernel
 // launched through launch_pdl() must call grid_dep_wait() before its first global-memory access.  Inside a stream
 // capture the attribute becomes a programmatic edge of the CUDA graph.  frcnn_set_programmatic_launch(0) turns the

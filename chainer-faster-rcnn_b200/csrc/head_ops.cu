@@ -5,7 +5,7 @@
 //   frcnn_head_decode     : softmax + per-class decode + clip    (models/faster_rcnn.py:175-178)
 //   frcnn_detect          : per-class NMS + confidence filter    (forward.py:48-57)
 // All are HBM/L2-bound: 16-byte vector accesses along the channel axis (NHWC), grids sized to
-// cover the tensor with >= 2 waves of 148 SMs where the tensor is large enough.
+// cover the tensor with >= 2 waves of 132 SMs where the tensor is large enough.
 #include <stdarg.h>
 #include <string.h>
 
@@ -510,7 +510,7 @@ __global__ void head_decode_kernel(const float* scores, const float* deltas, int
 // second pass for R > 2048/... never needed: R <= 2048 = 32 words) -- the greedy chain costs a shuffle + a few ALU ops per
 // row instead of a block-wide barrier per kept box (the first version: 85 us for 300 rows x 20 classes; this one: 40 us).
 constexpr int kDetThreads = 256;                      // detect_barrier_kernel
-constexpr int kDetMaskThreads = 1024;                 // detect_kernel: 20 CTAs on 148 SMs -- the rank and mask phases scale with the CTA
+constexpr int kDetMaskThreads = 1024;                 // detect_kernel: 20 CTAs on 132 SMs -- the rank and mask phases scale with the CTA
 constexpr int kDetMaxR = 2048;
 
 __device__ __forceinline__ float det_iou(const float4 a, const float4 b) {
@@ -701,7 +701,7 @@ __global__ void __launch_bounds__(kDetThreads) detect_barrier_kernel(const float
 
 static int grid_for(long total, int block) {
     long g = (total + block - 1) / block;
-    const long cap = 148l * 16;
+    const long cap = 132l * 16;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -714,9 +714,8 @@ extern "C" const char* frcnn_last_error(void) { return g_err; }
 
 namespace frcnn {
 static int pdl_default() {
-    // off unless FRCNN_PDL=1: measured on B200 (profiles/r02_bench_pdl_on_off.txt) the attribute changes neither the one-image
-    // latency (1.584 vs 1.592 ms) nor the throughput (844 vs 847 img/s) of the replayed graph -- the persistent conv CTAs own
-    // every SM's shared memory until they exit, so a dependent kernel cannot become resident early anyway
+    // off unless FRCNN_PDL=1: the persistent conv CTAs own every SM's shared memory until they exit, so a dependent kernel
+    // cannot become resident early anyway
     const char* e = getenv("FRCNN_PDL");
     return (e != nullptr && e[0] == '1') ? 1 : 0;
 }
@@ -852,7 +851,7 @@ extern "C" int frcnn_roi_pool(const void* feat_hi, const void* feat_lo, int H, i
     const int slices = (C / 8 + c8_per_cta - 1) / c8_per_cta;
     const int threads = ((outw * c8_per_cta + 31) / 32) * 32;
     const long ctas = (long)R_cap * slices;
-    const dim3 grid((unsigned)(ctas < 148l * 64 ? ctas : 148l * 64));
+    const dim3 grid((unsigned)(ctas < 132l * 64 ? ctas : 132l * 64));
     if (feat_lo) {
         FRCNN_CUDA_OK(launch_pdl(roi_pool_col_kernel<true>, grid, dim3(threads), 0, (cudaStream_t)stream, (const __nv_bfloat16*)feat_hi,
                                  (const __nv_bfloat16*)feat_lo, H, W, C, rois, count, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,

@@ -2,12 +2,12 @@
 //
 // Replaces L.Linear + F.relu at /root/reference models/faster_rcnn.py:33-36,127-134 (fc6, fc7, cls_score | bbox_pred).
 //
-// Why not the convolution's orientation (RoIs = pixel rows of the 128 x CG tile): 300 rows occupy 512 rows of CTA-pair
-// tiles (41 % of the tensor work multiplies zeros -- wasted energy on a power-capped part) and the 64 tiles of fc6 walk
-// K = 25,088 serially.  Here the operands are swapped: the WEIGHT rows are the M side (4096 = 16 full pair tiles), the RoIs
-// are the N side (300 -> 320 = 2 tiles of N = 160: 6.7 % padding), and K is split so that every SM pair has one unit of
-// work; each split additionally rotates its k-blocks over two TMEM accumulators (the tensor core's fp32 accumulator
-// truncates on every add, DESIGN.md 2).  Per split the GEMM (conv_gemm_kernel in split-K "NT" mode) writes an fp32 slab
+// Why not the convolution's orientation (RoIs = pixel rows of the 128-row tile): 300 rows occupy 384 tile rows (22 % of
+// the tensor work multiplies zeros) and the 3 tiles of fc6 walk K = 25,088 serially.  Here the operands are swapped: the
+// WEIGHT rows are the M side (4096 = 32 full tiles), the RoIs are the N side (300 -> 320 = 5 tiles of N = 64: 6.7 %
+// padding), and K is split so that every SM has about one unit of work; a long split additionally promotes its
+// tensor-core partial sums into a register total every 8 k-blocks (the tensor core's fp32 accumulator truncates on
+// every add, DESIGN.md 2).  Per split the GEMM (conv_gemm_kernel in split-K "NT" mode) writes an fp32 slab
 // parts[split][channel][roi]; `linear_reduce_kernel` sums the slabs in fixed order (deterministic), adds the bias, applies
 // ReLU, zeroes the rows past the device-side RoI count, transposes through shared memory and writes [roi][channel] as
 // bf16 hi/lo planes (the next layer's operand) and/or fp32.
@@ -112,7 +112,7 @@ static LinearPlan plan_linear(int R_cap, int K, int Cout) {
     LinearPlan lp;
     lp.ld = (R_cap + 31) / 32 * 32;
     // N tile: least padding, then the wider tile
-    const int cand[4] = {256, 160, 128, 64};
+    const int cand[3] = {256, 128, 64};
     long best = -1;
     lp.bn = 128;
     for (int bn : cand) {
@@ -121,15 +121,14 @@ static LinearPlan plan_linear(int R_cap, int K, int Cout) {
     }
     const int kb = K / 64;
     const int m_tiles = cdiv(Cout, 128);
-    const int cg = m_tiles >= 2 ? 2 : 1;                     // conv2d_impl's rule
-    const int base = cdiv(m_tiles, cg) * cdiv(lp.ld, lp.bn);
-    int sms = 148;
+    const int base = m_tiles * cdiv(lp.ld, lp.bn);
+    int sms = 132;
     {
         int dev = 0;
         if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 148;
+        if (sms <= 0) sms = 132;
     }
-    const int slots = sms / cg > 0 ? sms / cg : 1;
+    const int slots = sms;
     // splits: minimise (waves x k-blocks per unit) + the reduction's traffic; a unit keeps >= 2 k-blocks
     const double red_cost = (double)cdiv(Cout, 128) * 128 * lp.ld * 8.0 / 5e6 / 0.75;       // one slab written + read, in k-block times
     double best_cost = 0;
@@ -141,7 +140,7 @@ static LinearPlan plan_linear(int R_cap, int K, int Cout) {
         if (s == 1 || cost < best_cost) { best_cost = cost; lp.splits = s; }
     }
     const int per = cdiv(kb, lp.splits);
-    // a second accumulator per split for long K, when TMEM has room for it next to the correction accumulator
+    // long K per split: promote the tensor-core partial sums (conv2d_impl then narrows the N tile to fit the registers)
     lp.nacc = (per >= 64) ? 2 : 1;
     lp.m_rows = Cout;
     lp.parts_bytes = (size_t)lp.splits * Cout * lp.ld * sizeof(float);

@@ -280,9 +280,8 @@ __global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortAr
 }
 
 // Ordering step: rank-by-counting across the whole chip.  The composites are unique (they contain the
-// index), so rank(i) = #{j : comp[j] < comp[i]} is a permutation; 6000^2 64-bit compares are ~3 us on 148
-// SMs, where a single-CTA bitonic network of the same 6000 elements took 50-170 us (instruction-issue
-// bound on one SM).  Each block ranks 32 elements (8 threads per element, each scanning 1/8 of the list from
+// index), so rank(i) = #{j : comp[j] < comp[i]} is a permutation; 6000^2 64-bit compares spread over the
+// whole chip, where a single-CTA bitonic network of the same 6000 elements is instruction-issue bound on one SM.  Each block ranks 32 elements (8 threads per element, each scanning 1/8 of the list from
 // a shared-memory copy) and scatters box / score / index straight to the sorted position.
 constexpr int kRankThreads = 256, kRankPerBlock = 32;
 __global__ void __launch_bounds__(kRankThreads) rank_scatter_kernel(const SortArgs a) {

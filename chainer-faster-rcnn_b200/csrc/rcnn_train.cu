@@ -316,7 +316,7 @@ int frcnn_roi_pool_backward(const void* feat_hi, const void* feat_lo, int H, int
     FRCNN_CUDA_OK(cudaMemsetAsync(workspace, 0, n * sizeof(long long), st));
     const long total = (long)R_cap * outh * outw * (C / 8);
     long grid = (total + 255) / 256;
-    if (grid > 148l * 16) grid = 148l * 16;
+    if (grid > 132l * 16) grid = 132l * 16;
     roi_pool_backward_kernel<<<(unsigned)grid, 256, 0, st>>>((const __nv_bfloat16*)feat_hi, (const __nv_bfloat16*)feat_lo, H, W, C, rois,
                                                             count, R_cap, outh, outw, scale, (const __nv_bfloat16*)g_hi,
                                                             (const __nv_bfloat16*)g_lo, (long long*)workspace);

@@ -125,7 +125,7 @@ __global__ void subsample2x_kernel(const __nv_bfloat16* __restrict__ xh, const _
 
 static int grid_cover(long total, int block) {
     long g = (total + block - 1) / block;
-    const long cap = 148l * 16;
+    const long cap = 132l * 16;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

@@ -1,6 +1,6 @@
 // train_backward.cu -- the memory-bound kernels of the conv backward pass (SURVEY.md 8f rank 1, train_rpn.py step).
 //
-// The dense parts of backward run on the SAME tcgen05 kernel as forward (conv_gemm_sm100.cu):
+// The dense parts of backward run on the SAME wgmma kernel as forward (conv_gemm_sm90.cu):
 //   data gradient    dX = conv(dY, W rotated 180 deg, in/out swapped)      -> frcnn_conv2d with frcnn_pack_conv_weights_dgrad
 //   weight gradient  dW[r][s] = sum_pixels dY[p] (x) X[p + (r-1, s-1)]      -> frcnn_gemm_nt_splitk over a zero-padded,
 //                                                                            pixel-contiguous ("transposed") copy of dY and X

@@ -282,7 +282,7 @@ def set_conv_tile(block_n=0, tile_h=0, tile_w=0):
 
 
 def set_conv_cta_group(cta_group=0):
-    """0 = automatic, 1 = single-CTA MMAs only, 2 = CTA pairs (cta_group::2) wherever the tile allows."""
+    """0 = automatic (single CTAs), 1 = single CTAs, 2 = CTA pairs (a 2-CTA cluster sharing the weight tile) wherever the layer allows."""
     _lib.load().frcnn_conv2d_set_cta_group(cta_group)
 
 

@@ -1,5 +1,5 @@
 /*
- * frcnn_b200.h -- C ABI of libfrcnn_b200.so: the Blackwell (sm_100a) Faster R-CNN forward
+ * frcnn_b200.h -- C ABI of libfrcnn_b200.so: the Hopper (sm_90a) Faster R-CNN forward
  * detection path, a from-scratch replacement for the hot path of mitmul/chainer-faster-rcnn.
  *
  * Conventions (differences from the reference's only FFI, models/gpu_nms.hpp:9-10, are deliberate):
@@ -16,7 +16,7 @@
  *
  * Dense operands are NHWC bf16.  "bf16x3" precision: a tensor is a pair of bf16 planes (hi, lo)
  * with value = hi + lo (16 significant bits); the contraction computes hi*hi + lo*hi + hi*lo
- * with fp32 accumulation in TMEM.  Passing NULL for the lo planes selects single-pass bf16.
+ * with fp32 accumulation in registers.  Passing NULL for the lo planes selects single-pass bf16.
  */
 #ifndef FRCNN_B200_H_
 #define FRCNN_B200_H_
@@ -104,7 +104,7 @@ int frcnn_proposals(const float* cls, long cls_chan_stride, long cls_pix_stride,
                     int* dbg_num_sorted, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Dense contraction on tcgen05 tensor cores (TMA -> smem -> tcgen05.mma -> TMEM -> epilogue):
+ * Dense contraction on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue):
  * 3x3 stride-1 pad-1 convolution or 1x1 convolution / GEMM over NHWC bf16, fused bias (+ReLU).
  * Replaces L.Convolution2D (models/vgg16.py:39-67, models/region_proposal_network.py:53-57) and
  * L.Linear (models/faster_rcnn.py:33-36; a Linear over R rows is the 1x1 case with H=1, W=R).
@@ -126,8 +126,9 @@ int frcnn_conv2d(const void* x_hi, const void* x_lo, int H, int W, int Cin, cons
 /* Tuning override for tests / benchmarks: force the N tile (64/128/256) and the pixel tile
  * (tile_h*tile_w == 128); 0 = automatic. Process-wide. */
 void frcnn_conv2d_set_tile(int block_n, int tile_h, int tile_w);
-/* 0 = automatic (CTA pairs / cta_group::2 for N tiles >= 128), 1 = force single-CTA MMAs, 2 = force pairs
- * where the tile allows it.  Process-wide; for tests and A/B timing. */
+/* 0 = automatic (single CTAs, the faster choice measured on an H100), 1 = single CTAs, 2 = CTA pairs where the layer
+ * allows it (64-channel K blocks).  A pair is a cluster of 2 CTAs on neighbouring pixel tiles of the same N tile:
+ * each loads half of the weight tile and multicasts it to both.  Per calling thread; for tests and A/B timing. */
 void frcnn_conv2d_set_cta_group(int cta_group);
 /* Host staging for callers that hold HOST arrays (forward.py:88-99 uploads a float32 image and reads the results back):
  * pinned blocks owned by the library and explicit asynchronous copies on the caller's stream.  frcnn_host_alloc returns
@@ -152,7 +153,7 @@ void frcnn_set_programmatic_launch(int on);
 
 /* Cap on the persistent grid of subsequent frcnn_conv2d launches (0 = all SMs).  With several independent images in
  * flight on different streams, launches that each take a share of the SMs run side by side instead of queueing behind
- * each other's 148-CTA grids, and a smaller grid quantises a layer's tile count into fuller waves.  The value is baked
+ * each other's one-CTA-per-SM grids, and a smaller grid quantises a layer's tile count into fuller waves.  The value is baked
  * into a CUDA graph at capture time. */
 void frcnn_conv2d_set_max_ctas(int max_ctas);
 /* Shared memory (bytes, 0..96 KB) that subsequent frcnn_conv2d launches of the calling thread leave unused on every SM

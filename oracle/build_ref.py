@@ -24,7 +24,7 @@ rich-compare).
 
 No reference source is copied into the repository: the patched text only ever
 exists under a temporary directory, and only the compiled ``.so`` lands in
-``oracle/_ref/`` (git-ignored, but it travels to the GPU box with gpurun).
+``oracle/_ref/`` (git-ignored build product).
 
 ``build_bbox()`` / ``load_bbox()`` do the same for models/bbox.pyx (``bbox_overlaps``, the IoU matrix of
 the training path, anchor_target_layer.py:181-185) into ``oracle/_ref/ref_bbox*.so``; its alias patch is
@@ -32,7 +32,7 @@ the training path, anchor_target_layer.py:181-185) into ``oracle/_ref/ref_bbox*.
     DTYPE = np.float -> DTYPE = np.float64   (bbox.pyx:12)
     np.float_t       -> np.float64_t         (bbox.pyx:13; the same C double)
 
-If /root/reference is absent (the GPU box) this script is a no-op and the
+If the reference checkout is absent this script is a no-op and the
 pre-built ``.so`` -- if any -- is used as is.
 """
 import os

@@ -1,6 +1,6 @@
 """pytest configuration: registers the `gpu` marker and puts the oracle and the
-B200 package directory on sys.path.  GPU tests are skipped (not failed) when no CUDA device
-is visible, so `-m "not gpu"` and a plain run both work in the CPU-only build container."""
+package directory on sys.path.  GPU tests are skipped (not failed) when no CUDA device
+is visible, so `-m "not gpu"` and a plain run both work on a machine without a GPU."""
 import os
 import sys
 
@@ -14,7 +14,7 @@ for p in (os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests"), PKG, ROOT):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (runs on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -7,7 +7,7 @@
 //   * the 7.2 MB copy split in 1 MB chunks, and split over 2 / 4 streams
 //   * an SM copy kernel reading MAPPED pinned host memory directly (zero-copy, no copy engine)
 //   * pageable memcpy for reference
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o h2d_probe h2d_probe.cu      Run: ./h2d_probe
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o h2d_probe h2d_probe.cu      Run: ./h2d_probe
 #include <cuda_runtime.h>
 
 #include <algorithm>

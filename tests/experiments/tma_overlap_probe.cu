@@ -6,13 +6,13 @@
 // Map: dims {32, W, H}, strides {16 B, (W+2)*16 B}, box {32, TW, TH}, SWIZZLE_64B.  Tile at (0, w0, h0) must hold, at smem row
 // (y*TW + x), chunk j (16 B, XOR-swizzled with ((row>>1)&3)), the 8 channels of padded pixel (h0+y, w0+x+j); rows with
 // h0+y outside [0,H) must be zero.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -I ../../chainer-faster-rcnn_b200/csrc -o tma_overlap_probe tma_overlap_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -I ../../chainer-faster-rcnn_b200/csrc -o tma_overlap_probe tma_overlap_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 constexpr int TW = 16, TH = 8;
 

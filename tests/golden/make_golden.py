@@ -16,7 +16,7 @@ Imports the reference's own modules from /root/reference:
                                              (oracle/build_ref.py -> oracle/_ref/).
 `np.float` (removed NumPy alias used at models/proposal_layer.py:66) is aliased to `float`.
 
-The vectors are committed; the GPU box never needs /root/reference.
+The vectors are committed; the tests never need the reference itself.
 Inputs that are large are NOT stored: they are regenerated from the seed by
 tests/golden_inputs.py (same code used here), and a checksum of the input is stored instead.
 """
@@ -35,7 +35,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import build_ref          # noqa: E402
 import golden_inputs as gi  # noqa: E402
 
-REF = "/root/reference"
+REF = build_ref.REF
 
 
 def install_chainer_standin():
@@ -91,6 +91,17 @@ def import_reference():
     return Variable, ref_nms, ga, bt, pl
 
 
+def make_cpu_nms_clustered(ref_nms):
+    """The reference's cpu_nms on 1500 clustered boxes (5 seeds x 3 thresholds) -> cpu_nms_clustered.npz."""
+    out = {}
+    for seed in range(5):
+        dets = gi._clustered_dets(1500, 100 + seed)
+        out["s%d_checksum" % seed] = gi.checksum(dets)
+        for thr in (0.3, 0.5, 0.7):
+            out["s%d_t%02d_keep" % (seed, round(thr * 10))] = np.asarray(ref_nms.cpu_nms(dets, thr), dtype=np.int64)
+    np.savez_compressed(os.path.join(HERE, "cpu_nms_clustered.npz"), **out)
+
+
 def main():
     Variable, ref_nms, ga, bt, pl = import_reference()
     out = {}
@@ -124,6 +135,7 @@ def main():
         out[name + "_thr"] = np.float64(thr)
         out[name + "_checksum"] = gi.checksum(dets)
     np.savez(os.path.join(HERE, "cpu_nms.npz"), **out)
+    make_cpu_nms_clustered(ref_nms)
 
     # ---- 4. ProposalLayer.__call__
     out = {}

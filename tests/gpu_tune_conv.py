@@ -1,5 +1,5 @@
 """Tuning sweep (not a pytest file): time every conv/GEMM layer of the headline config for each
-N-tile / pixel-tile choice.  Prints a table; the winners go into the heuristic in conv_gemm_sm100.cu."""
+N-tile / pixel-tile choice.  Prints a table; the winners go into the heuristic in conv_gemm_sm90.cu."""
 import sys
 import torch
 sys.path[:0] = ["chainer-faster-rcnn_b200"]
@@ -25,7 +25,6 @@ for prec in precisions:
         gflop = 2.0 * H * W * Cout * k * k * Cin / 1e9
         res = []
         tiles = TILES if H > 1 else [(1, 128)]
-        tiles = [(16, 8), (8, 16)] if H > 1 else [(1, 128)]     # (16,8) = halo path for 3x3
         for cg in (1, 2):
             for bn in (64, 128, 256):
                 if bn > Cout:

@@ -135,30 +135,6 @@ def test_host_copy_pool_is_a_memcpy():
     assert all(np.array_equal(o, src[:o.size]) for o in outs)
 
 
-def test_bench_traffic_record_is_reproducible_from_the_committed_ncu_launch_list(tmp_path):
-    """bench.py's roofline.traffic comes from profiles/r02_conv_stack_dram.json; that file must be what
-    profiles/summarize_dram.py derives from the committed ncu launch list (same bytes, same launch count, same git hash)."""
-    import json
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    rec = json.load(open(os.path.join(root, "profiles", "r02_conv_stack_dram.json")))
-    out = tmp_path / "dram.json"
-    subprocess.check_call([sys.executable, os.path.join(root, "profiles", "summarize_dram.py"),
-                           os.path.join(root, "profiles", "r02_launches_dram_forward.csv"), rec["git"], str(out)],
-                          stdout=subprocess.DEVNULL)
-    got = json.load(open(out))
-    assert got["conv_stack_launches"] == rec["conv_stack_launches"] == 15
-    assert got["conv_stack_dram_bytes_per_step"] == rec["conv_stack_dram_bytes_per_step"]
-    assert abs(got["conv_stack_time_share_under_ncu"] - rec["conv_stack_time_share_under_ncu"]) < 1e-12
-    assert rec["git"] in open(os.path.join(root, "profiles", "r02_launches_dram_forward.csv")).readline()
-    sys.path.insert(0, root)
-    import bench
-    frac = bench.hbm_fractions(got, [("layer", 0.1, 1.0)] * len(got["gemm_launches"]), 6571.9)
-    assert {"conv1_1", "fc6", "pack_image_c8", "roi_pool"} <= set(frac) and 0 < frac["fc6"]["frac_of_hbm_peak"] < 1
-
-
 def test_packed_pair_maximum_is_the_maximum_of_the_values():
     """What roi_pool_col_kernel relies on (csrc/head_ops.cu, 'RoI max pooling'): an activation is stored as v = hi + lo with
     hi = RN_bf16(v), lo = RN_bf16(v - hi), so |lo| <= ulp(hi)/2.  (1) hi + lo is exact in float32; (2) the order of the values is

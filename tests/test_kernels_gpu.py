@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): every CUDA kernel, called through the C ABI, against the
+"""GPU parity tests (run on an H100): every CUDA kernel, called through the C ABI, against the
 CPU oracle on the same seeded inputs.  Integer / index / box results must be BIT-EXACT; dense
 contractions must be within the stated tolerance of the oracle evaluated on identical inputs."""
 import os
@@ -138,7 +138,7 @@ def test_proposals_all_filtered_and_tiny(ops):
     assert R == len(want_rois) and np.array_equal(work.rois.cpu().numpy()[:R], want_rois)
 
 
-# ------------------------------------------------------------------------------- dense: conv / GEMM on tcgen05
+# ------------------------------------------------------------------------------- dense: conv / GEMM on wgmma
 def _quant16(a):
     """Value representable as bf16 hi + bf16 lo (what a bf16x3 operand holds)."""
     t = torch.from_numpy(np.ascontiguousarray(a, dtype=f32))
@@ -214,7 +214,8 @@ def test_conv2d_tile_shapes(ops, tile):
                                    (16, 8, 64, 128, 3),       # a single pixel tile (pairs not applicable)
                                    (1, 300, 512, 256, 1)])    # GEMM rows, 3 tiles
 def test_conv2d_single_cta_and_cta_pair_agree_with_oracle(ops, precision, cta_group, shape):
-    """cta_group::1 and cta_group::2 (CTA pairs, M = 256 MMAs, half of B per CTA) must both match the oracle."""
+    """Single CTAs and CTA pairs (a 2-CTA cluster, each CTA loading half of the weight tile and multicasting it to both)
+    must both match the oracle."""
     H, W, Cin, Cout, k = shape
     ops.set_conv_cta_group(cta_group)
     try:
@@ -432,7 +433,7 @@ def test_detections_assembly_matches_forward_py_loop(ops):
 
 @pytest.mark.parametrize("x3", [True, False])
 def test_long_k_gemm_rotating_accumulators_exact(ops, x3):
-    """K = 25,088 (fc6) runs with three rotating TMEM accumulators (ConvParams::nacc): on small-integer operands every
+    """K = 25,088 (fc6) runs with its tensor-core partial sums promoted every 8 k-blocks: on small-integer operands every
     partial sum is exactly representable, so the result must equal the integer GEMM exactly -- in both precision modes --
     and a K just below the switch-over (one accumulator) must agree too."""
     g = torch.Generator(device="cuda").manual_seed(3)

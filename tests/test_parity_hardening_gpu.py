@@ -6,7 +6,7 @@
     probability errors PER ELEMENT (not only max-norm), printed and asserted;
   * the reference's interface: models.faster_rcnn.FasterRCNN.__call__ fed HOST float32 arrays (one pinned upload, one
     download) returns bit for bit what the device path returns, also from several caller threads at once;
-  * the reference's own test files executed unchanged (when /root/reference is present -- it is not on the GPU box);
+  * the reference's own test files executed unchanged (where the reference's sources are present, see oracle/build_ref.py);
   * the training path's NCCL all-reduce as a pytest (skipped under 2 GPUs).
 
 Tolerance readings ("within 1e-4 relative", BASELINE north_star):
@@ -27,6 +27,7 @@ import numpy as np
 import pytest
 import torch
 
+import build_ref
 import frcnn_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -355,11 +356,11 @@ def test_cpu_nms_host_small_and_large_paths_and_threads():
 
 
 # ------------------------------------------------------------------------------- the reference's own test files, unchanged
-REF = "/root/reference"
+REF = build_ref.REF          # the reference checkout (FRCNN_REFERENCE_ROOT)
 
 
 def _run_reference_test_file(rel, only=None):
-    """Load /root/reference/<rel> as a module (unchanged source) after dropin.install() and run its unittest cases."""
+    """Load <reference>/<rel> as a module (unchanged source) after dropin.install() and run its unittest cases."""
     import importlib.util
     import unittest
     from frcnn_b200 import dropin
@@ -386,7 +387,7 @@ def _run_reference_test_file(rel, only=None):
     return len(tests)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="/root/reference is not present on this box (it never is on the GPU box)")
+@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference's sources are not present")
 @pytest.mark.parametrize("rel,only", [("tests/test_proposal_layer.py", None), ("tests/test_region_proposal_network.py", None),
                                       ("tests/test_generate_anchors.py", None), ("tests/test_faster_rcnn.py", "test_forward_whole")])
 def test_reference_test_files_run_unchanged(rel, only):
@@ -396,7 +397,7 @@ def test_reference_test_files_run_unchanged(rel, only):
 
 
 def test_reference_test_faster_rcnn_statements_with_the_voc_stand_in():
-    """tests/test_faster_rcnn.py:29-62 re-typed (the file itself cannot travel to the GPU box): setUp with VOC('train')[1] from the
+    """tests/test_faster_rcnn.py:29-62 re-typed (the file itself is not part of this repository): setUp with VOC('train')[1] from the
     synthetic stand-in, then test_forward_whole for both trunks and the three train switches."""
     import chainer
     import cupy as cp
