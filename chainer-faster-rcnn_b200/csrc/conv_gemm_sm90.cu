@@ -562,22 +562,40 @@ static int device_sm_count() {
     return sms;
 }
 
+// The plan of the calling thread's last conv / GEMM launch (frcnn_conv2d_last_plan), in the order
+// BN, BK, x3, promote, CG, TH, TW, stages, grid, num_tiles, n_parts, splits.
+constexpr int kPlanFields = 12;
+static thread_local int g_last_plan[kPlanFields] = {};
+
+// Bytes of one ring stage and of the stage-independent part of the dynamic shared memory (alignment slack, barriers, the
+// epilogue's transpose tiles and, with resident weights, every weight tile of the layer).
+static void conv_smem_layout(int BN, int BK, bool x3, int bres_kblocks, int* stage_bytes, int* fixed) {
+    const int planes = x3 ? 2 : 1;
+    const int a_bytes = kTileM * BK * 2, b_bytes = BN * BK * 2;
+    *stage_bytes = bres_kblocks > 0 ? planes * a_bytes : planes * (a_bytes + b_bytes);
+    *fixed = 1024 /*align slack*/ + kBarrierBytes + kScratchBytes + bres_kblocks * planes * b_bytes;
+}
+
+// Pipeline stages that fit the shared-memory budget (at most 20).  The budget is the whole SM by default;
+// frcnn_conv2d_set_smem_reserve leaves a slice of every SM to other kernels, so that the small kernels of ANOTHER image in
+// flight (decode, NMS, RoI pooling, a host caller's per-class NMS) can become resident next to a convolution instead of
+// waiting for one of its CTAs to retire.
+static int conv_stages(int BN, int BK, bool x3, int bres_kblocks) {
+    int stage_bytes, fixed;
+    conv_smem_layout(BN, BK, x3, bres_kblocks, &stage_bytes, &fixed);
+    const int stages = (227 * 1024 - g_smem_reserve - fixed) / stage_bytes;
+    return stages > 20 ? 20 : stages;
+}
+
 template <int BN, int BK, bool X3, bool PROMOTE, int CG>
 static int launch_conv(const CUtensorMap* tm, ConvParams p, cudaStream_t stream) {
-    using C = Cfg<BN, BK>;
     p.fd_tiles_w = make_fastdiv(p.tiles_w);
     p.fd_n_tiles = make_fastdiv(p.n_tiles);
     p.fd_tiles_per_part = make_fastdiv(p.tiles_per_part);
-    const int planes = X3 ? 2 : 1;
-    const int bres_bytes = p.b_res ? p.taps * p.cin_blocks * planes * C::B_BYTES : 0;
-    const int stage_bytes = p.b_res ? planes * C::A_BYTES : planes * (C::A_BYTES + C::B_BYTES);
-    const int fixed = 1024 /*align slack*/ + kBarrierBytes + kScratchBytes + bres_bytes;
-    // shared-memory budget of the persistent CTA: everything by default; frcnn_conv2d_set_smem_reserve leaves a slice of
-    // every SM to other kernels, so that the small kernels of ANOTHER image in flight (decode, NMS, RoI pooling, a host
-    // caller's per-class NMS) can become resident next to a convolution instead of waiting for one of its CTAs to retire
-    const int smem_budget = 227 * 1024 - g_smem_reserve;
-    int stages = (smem_budget - fixed) / stage_bytes;
-    if (stages > 20) stages = 20;
+    const int bres_kblocks = p.b_res ? p.taps * p.cin_blocks : 0;
+    int stage_bytes, fixed;
+    conv_smem_layout(BN, BK, X3, bres_kblocks, &stage_bytes, &fixed);
+    const int stages = conv_stages(BN, BK, X3, bres_kblocks);
     if (stages < 2) {
         set_error("conv tile BN=%d BK=%d x3=%d does not fit 2 pipeline stages", BN, BK, (int)X3);
         return FRCNN_ERR_ARG;
@@ -590,6 +608,9 @@ static int launch_conv(const CUtensorMap* tm, ConvParams p, cudaStream_t stream)
     if (g_max_ctas > 0 && g_max_ctas < ctas) ctas = g_max_ctas;      // several images in flight: each launch takes a share of the SMs
     const int units = ctas / CG > 0 ? ctas / CG : 1;     // CTAs (CG = 1) or CTA pairs (CG = 2) resident at once
     const int grid = CG * (p.num_tiles < units ? p.num_tiles : units);
+    const int plan[kPlanFields] = {BN, BK, X3 ? 1 : 0, PROMOTE ? 1 : 0, CG, p.TH, p.TW, stages, grid, p.num_tiles, p.n_parts,
+                                   p.splits};
+    for (int i = 0; i < kPlanFields; ++i) g_last_plan[i] = plan[i];
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(kNumThreads);
@@ -632,6 +653,11 @@ extern "C" void frcnn_conv2d_set_tile(int block_n, int tile_h, int tile_w) {
     g_force_tw = tile_w;
 }
 
+extern "C" int frcnn_conv2d_last_plan(int* out, int n) {
+    for (int i = 0; out != nullptr && i < n && i < kPlanFields; ++i) out[i] = g_last_plan[i];
+    return kPlanFields;
+}
+
 namespace {
 struct GemmExtra {          // split-K GEMM mode of the same kernel (frcnn_gemm_nt_splitk)
     int groups, row_stride, splits;
@@ -652,6 +678,7 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
                        void* y_hi, void* y_lo, float* y_f32, int ld_f32, const int* m_valid, void* stream_,
                        const GemmExtra* ge, const ResExtra* re = nullptr, const WinExtra* we = nullptr) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    for (int& v : g_last_plan) v = 0;          // a call that launches nothing leaves an empty record
     FRCNN_REQUIRE(x_hi && w_hi && (bias || ge), "frcnn_conv2d: x_hi, w_hi and bias are required");
     FRCNN_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "frcnn_conv2d: x_lo and w_lo must both be given (bf16x3) or both NULL");
     FRCNN_REQUIRE(ksize == 1 || ksize == 3, "frcnn_conv2d: ksize must be 1 or 3 (got %d)", ksize);
@@ -718,6 +745,15 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     }
     while (BN > bn_cap) BN /= 2;
     if (BN != 64 && BN != 128 && BN != 256) BN = 128;      // an N tile without a kernel (160): the nearest smaller one
+    // a shared-memory reserve (frcnn_conv2d_set_smem_reserve) can leave less than two pipeline stages of a wide N tile
+    // (bf16x3 BN = 128 above 81,408 B): narrow the tile until two fit; launch_conv reports the case where BN = 64 does not
+    {
+        const int kblocks = (we != nullptr ? 3 : ksize * ksize) * cdiv(Cin, BK);
+        auto bres_kblocks = [&](int bn) {
+            return (we != nullptr && cdiv(cout_cover, bn) == 1 && ge == nullptr && kblocks <= 16) ? kblocks : 0;
+        };
+        while (BN > 64 && conv_stages(BN, BK, x3, bres_kblocks(BN)) < 2) BN /= 2;
+    }
 
     ConvParams p;
     p.H = H; p.W = W; p.Cout = Cout;

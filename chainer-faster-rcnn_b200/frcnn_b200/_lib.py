@@ -44,6 +44,7 @@ SIGNATURES = {
     "frcnn_conv2d_set_cta_group": (None, [c_int]),
     "frcnn_conv2d_set_max_ctas": (None, [c_int]),
     "frcnn_conv2d_set_smem_reserve": (None, [c_int]),
+    "frcnn_conv2d_last_plan": (c_int, [c_void_p, c_int]),
     "frcnn_set_programmatic_launch": (None, [c_int]),
     "frcnn_host_alloc": (c_void_p, [c_size_t]),
     "frcnn_host_free": (c_int, [c_void_p]),

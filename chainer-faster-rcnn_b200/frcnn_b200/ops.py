@@ -362,6 +362,18 @@ def set_conv_max_ctas(max_ctas=0):
     _lib.load().frcnn_conv2d_set_max_ctas(int(max_ctas))
 
 
+CONV_PLAN_FIELDS = ("BN", "BK", "x3", "promote", "CG", "TH", "TW", "stages", "grid", "num_tiles", "n_parts", "splits")
+
+
+def conv_last_plan():
+    """The plan of this thread's last conv / GEMM launch (frcnn_conv2d_last_plan) as a dict of CONV_PLAN_FIELDS."""
+    buf = (ctypes.c_int * len(CONV_PLAN_FIELDS))()
+    n = _lib.load().frcnn_conv2d_last_plan(buf, len(buf))
+    if n != len(CONV_PLAN_FIELDS):
+        raise FrcnnError("frcnn_conv2d_last_plan: %d fields, expected %d" % (n, len(CONV_PLAN_FIELDS)))
+    return dict(zip(CONV_PLAN_FIELDS, buf))
+
+
 def maxpool2x2_ceil(x, out=None):
     H, W, C = x.hi.shape
     if out is None:

@@ -158,8 +158,14 @@ void frcnn_set_programmatic_launch(int on);
 void frcnn_conv2d_set_max_ctas(int max_ctas);
 /* Shared memory (bytes, 0..96 KB) that subsequent frcnn_conv2d launches of the calling thread leave unused on every SM
  * (fewer pipeline stages), so that small kernels of other streams can be resident beside the persistent convolution CTAs.
+ * Where fewer than two stages of the planned N tile would fit, a narrower N tile is used.
  * Read at launch time (fixed inside a captured graph). */
 void frcnn_conv2d_set_smem_reserve(int bytes);
+/* The plan of the calling thread's last frcnn_conv2d / frcnn_conv2d_res / frcnn_conv3x3_c8 / frcnn_gemm_nt_splitk /
+ * frcnn_linear GEMM launch: copies min(n, 12) ints to out in the order BN, BK, x3, promote (long-K partial sums), CTA
+ * group, tile_h, tile_w, pipeline stages, grid (CTAs), tiles (pair-tiles for CTA pairs, all split-K parts included),
+ * split-K parts, splits; all zero when the last call launched nothing.  Returns the number of fields (12). */
+int frcnn_conv2d_last_plan(int* out, int n);
 
 /* OIHW fp32 weights (Chainer layout, e.g. trunk/conv1_1/W) -> [kh*kw, Cout, Cin_pad] bf16 hi/lo.
  * For Linear weights (Cout, K) pass kh=kw=1.  `perm_chw_to_hwc` != 0 with (c,h,w) = (pc,ph,pw)

@@ -41,6 +41,22 @@ def test_library_loads_and_exports_every_declared_symbol(lib):
         assert re.search(r"\sT\s+%s$" % re.escape(s), out, flags=re.M), s
 
 
+def test_every_conv_gemm_instantiation_has_a_dispatch_matrix_case():
+    """The FRCNN_DISPATCH(...) lines of conv_gemm_sm90.cu are exactly the parameter list of the GPU dispatch-matrix test
+    (tests/test_conv_gemm_coverage_gpu.py), in the same order: an instantiation cannot be added without a test."""
+    import test_conv_gemm_coverage_gpu as cov
+    table = cov.parse_dispatch_table()
+    assert len(table) == 25 and len(set(table)) == len(table)
+    assert table == cov.DISPATCH
+    assert set(cov.MATRIX_SHAPE) == set(cov.DISPATCH)
+
+
+def test_conv_last_plan_reports_every_field(lib):
+    from frcnn_b200 import ops
+    assert lib.frcnn_conv2d_last_plan(None, 0) == len(ops.CONV_PLAN_FIELDS) == 12
+    assert list(ops.conv_last_plan()) == list(ops.CONV_PLAN_FIELDS)
+
+
 def test_no_hard_dependency_on_libcuda(lib):
     from frcnn_b200 import _lib
     out = subprocess.run(["ldd", _lib.LIB_PATH], capture_output=True, text=True).stdout

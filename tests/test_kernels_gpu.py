@@ -193,7 +193,7 @@ def _conv_case(ops, H, W, Cin, Cout, ksize, precision, seed, relu=True, ld_f32=0
 @pytest.mark.parametrize("shape", [
     (24, 40, 64, 64, 3),      # BK=64, BN=64, exact tiles
     (19, 33, 64, 128, 3),     # ragged H/W (TMA zero fill + store predicates)
-    (13, 21, 128, 256, 3),    # BN=256 path
+    (13, 21, 128, 256, 3),    # wide Cout, few pixel tiles: plans BN=64 (BN=256: test_conv_gemm_coverage_gpu.py)
     (38, 63, 512, 512, 3),    # conv5 / RPN 3x3 real shape
     (11, 17, 16, 64, 3),      # BK=16 (SWIZZLE_32B) -- conv1_1 with the image padded to 16 channels
     (10, 12, 64, 96, 1),      # 1x1
@@ -453,7 +453,7 @@ def test_long_k_gemm_rotating_accumulators_exact(ops, x3):
 @pytest.mark.parametrize("precision", ["bf16", "bf16x3"])
 @pytest.mark.parametrize("shape", [(300, 1024, 105, 171, False),      # cls_score|bbox_pred: one 128-row weight tile, fp32 out
                                    (300, 4096, 4096, 300, True),       # fc7
-                                   (300, 25088, 512, 233, True),       # fc6's K (392 k-blocks: 2 splits x 2 accumulators)
+                                   (300, 25088, 4096, 233, True),      # fc6: 4 splits of 98 k-blocks, each promoting its sums
                                    (77, 192, 96, 50, True),            # ragged everything: R_cap < one N tile, 3 k-blocks
                                    (1000, 512, 256, 999, True)])       # config #4's RoI count (N tiles of 256)
 def test_linear_swapab_vs_float64(ops, precision, shape):
@@ -465,7 +465,7 @@ def test_linear_swapab_vs_float64(ops, precision, shape):
     w = (rng.standard_normal((N, K)) * (1.0 / K) ** 0.5).astype(f32)
     b = (rng.standard_normal(N) * 0.1).astype(f32)
     q = _quant16 if precision == "bf16x3" else _bf16
-    ref = q(x).astype(np.float64) @ q(w).astype(np.float64).T + b
+    ref = (dev(q(x)).double() @ dev(q(w)).double().T).cpu().numpy() + b      # float64, on the GPU for fc6's size
     if relu:
         ref = np.maximum(ref, 0)
     xt = dev(x)[None]                                         # [1,R,K]
@@ -491,11 +491,11 @@ def test_linear_swapab_vs_float64(ops, precision, shape):
 
 @pytest.mark.parametrize("x3", [True, False])
 def test_linear_swapab_long_k_exact_on_integers(ops, x3):
-    """Small-integer operands: every partial sum is exact in fp32, so split-K + rotating accumulators + the fixed-order
-    reduction must reproduce the integer GEMM exactly (fc6's K = 25,088 and a short K)."""
+    """Small-integer operands: every partial sum is exact in fp32, so split-K + promoted partial sums + the fixed-order
+    reduction must reproduce the integer GEMM exactly (fc6: 4 splits of 98 promoted k-blocks; short K without promotion)."""
     g = torch.Generator(device="cuda").manual_seed(5)
-    for K in (25088, 4096, 128):
-        R, N = 300, 256
+    for K, N in ((25088, 4096), (4096, 256), (128, 256)):
+        R = 300
         x = torch.randint(-2, 3, (1, R, K), device="cuda", generator=g).float()
         w = torch.randint(-2, 3, (N, K), device="cuda", generator=g).float()
         b = torch.randint(-5, 6, (N,), device="cuda", generator=g).float()

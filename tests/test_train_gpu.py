@@ -319,7 +319,7 @@ def _ref_gemm_parts(A, B, groups, row_stride, S_eff, K):
 
 @pytest.mark.parametrize("M,N,K,groups,splits,x3", [
     (64, 64, 64 * 37, 9, 5, True),        # conv1_2-like: half-empty M tile, single-CTA path, ragged last split
-    (512, 512, 64 * 40, 9, 3, True),      # CTA pairs, wide N
+    (512, 512, 64 * 40, 9, 3, True),      # wide N (BN = 128), several pixel tiles
     (256, 128, 64 * 16, 1, 1, True),      # plain GEMM, no split
     (128, 64, 64 * 9, 9, 9, False),       # single-pass bf16
     (54, 512, 64 * 12, 1, 4, True),       # RPN heads: M not a multiple of anything
