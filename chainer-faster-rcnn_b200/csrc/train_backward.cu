@@ -31,7 +31,7 @@ struct PrepArgs {
     __nv_bfloat16 *o_hi, *o_lo;      // NHWC [H][W][C] out (optional)
     __nv_bfloat16 *t_hi, *t_lo;      // transposed [planes][C][Kp] out (optional)
     int planes;                      // 1: plane at q; 3: planes shifted by -1/0/+1 pixel
-    int times2;                      // multiply the result by 2 (the 1/(1-ratio) of a ratio-0.5 dropout): exponent + 1, exact
+    int times2;                      // multiply the result by 2 (the 1/(1-ratio) of a ratio-0.5 dropout), correctly rounded
 };
 
 constexpr int PAD_LEFT = 8;          // zero columns left of pixel 0 in the transposed layout: every 8-pixel group starts 16-B aligned
@@ -64,30 +64,45 @@ __device__ __forceinline__ void pack8(const float v[8], uint32_t hw[4], uint32_t
     }
 }
 
+// per-halfword mask of y > 0 for packed bf16 words read as int16: (0, +inf] -- +0, negatives and every NaN are excluded, as
+// Chainer's `y > 0` excludes them
+__device__ __forceinline__ uint32_t positive_mask(uint32_t y) { return __vcmpgts2(y, 0u) & __vcmplts2(y, 0x7F817F81u); }
+
+// x2 on each bf16 of a packed pair, correctly rounded: exact for finite values (subnormals included), +-inf for an overflow,
+// inf stays inf and NaN stays NaN
+__device__ __forceinline__ uint32_t times2_bf16x2(uint32_t x) {
+    __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&x);
+    v = __hmul2(v, __floats2bfloat162_rn(2.f, 2.f));
+    return *reinterpret_cast<const uint32_t*>(&v);
+}
+
 // The (masked / routed) gradient of 8 channels (chunk c8) at pixel (h, w) as packed bf16 words -- integer SIMD only:
-//   * a value is the pair (hi, lo) with hi = bf16(v), lo = bf16(v - hi): v > 0 iff hi > 0 (read as int16); equality of
-//     two values is tested on the exact float sums (eq_values);
+//   * a value is the pair (hi, lo) with hi = bf16(v), lo = bf16(v - hi): v > 0 iff hi > 0 (read as int16, NaN excluded);
+//     equality of two values is tested on the exact float sums (eq_values);
 //   * F.max_pooling_2d backward: the incoming gradient goes to the FIRST element of the 2x2 ceil-mode window (scan order)
 //     whose value equals the pooled maximum;  F.relu backward: gy where y > 0.
-// Masked elements become +0 in both planes; kept elements keep the source's (hi, lo) words untouched.
+// Masked elements become +0 in both planes; kept elements keep the source's (hi, lo) words untouched (an fp32 source is
+// split into (hi, lo) first).
 __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int c8, uint32_t hw[4], uint32_t lw[4]) {
+    const long off = ((long)h * a.W + w) * a.C + c8 * 8;
+    uint32_t keep[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+    uint32_t yh[4], yl[4] = {0u, 0u, 0u, 0u};
+    if (a.y_hi != nullptr) {
+        ld4(a.y_hi, off, yh);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) keep[m] = positive_mask(yh[m]);          // y > 0
+    }
     if (a.g_f32 != nullptr) {
         const float* g = a.g_f32 + ((long)h * a.W + w) * a.ld_f32 + c8 * 8;
         float v[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = (c8 * 8 + j < a.ld_f32) ? g[j] : 0.f;
         pack8(v, hw, lw);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) { hw[m] &= keep[m]; lw[m] &= keep[m]; }
         return;
     }
-    const long off = ((long)h * a.W + w) * a.C + c8 * 8;
-    uint32_t keep[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-    uint32_t yh[4], yl[4] = {0u, 0u, 0u, 0u};
-    if (a.y_hi != nullptr) {
-        ld4(a.y_hi, off, yh);
-        if (a.y_lo) ld4(a.y_lo, off, yl);
-#pragma unroll
-        for (int m = 0; m < 4; ++m) keep[m] = __vcmpgts2(yh[m], 0u);          // y > 0
-    }
+    if (a.y_hi != nullptr && a.y_lo) ld4(a.y_lo, off, yl);
     long goff = off;
     if (a.p_hi != nullptr) {
         const int Wq = (a.W + 1) / 2;
@@ -117,12 +132,8 @@ __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int 
 #pragma unroll
     for (int m = 0; m < 4; ++m) { hw[m] &= keep[m]; lw[m] &= keep[m]; }
     if (a.times2) {
-        // x2 on a bf16 = exponent field + 1 (halves with a zero exponent field -- zero / subnormal -- are left alone)
 #pragma unroll
-        for (int m = 0; m < 4; ++m) {
-            hw[m] += 0x00800080u & __vcmpne2(hw[m] & 0x7F807F80u, 0u);
-            lw[m] += 0x00800080u & __vcmpne2(lw[m] & 0x7F807F80u, 0u);
-        }
+        for (int m = 0; m < 4; ++m) { hw[m] = times2_bf16x2(hw[m]); lw[m] = times2_bf16x2(lw[m]); }
     }
 }
 

@@ -434,13 +434,14 @@ long frcnn_padded_pixels(int H, int W, int* row_pitch);
 
 /* Gradient / activation re-layout with the element-wise backward ops fused:
  *   source  : bf16 hi(/lo) NHWC planes g [H][W][C] -- or [ceil(H/2)][ceil(W/2)][C] when p_hi is given -- or fp32 [H*W][ld_f32]
- *   y (opt) : the forward post-ReLU activation [H][W][C]: value *= (y > 0)                 (F.relu backward)
+ *   y (opt) : the forward post-ReLU activation [H][W][C]: value *= (y > 0), false for NaN  (F.relu backward)
  *   p (opt) : the 2x2/2 ceil-mode max-pooled y: the source is routed to the FIRST maximum of each window in scan order
  *             (F.max_pooling_2d backward), zero elsewhere
  *   outputs : o (opt) NHWC hi/lo [H][W][C]; t (opt) transposed padded planes [planes][C][Kp], planes = 1 (at k) or 3
  *             (plane j at k holds pixel k + j - 1: the pre-shifted B operand of frcnn_gemm_nt_splitk groups = 9).
- * With y = p = NULL and planes = 3 this is the plain activation transposer.  times2 != 0 doubles the result exactly
- * (exponent + 1): the backward factor 1/(1-ratio) of a ratio-0.5 F.dropout whose kept set is {y > 0}. */
+ * With y = p = NULL and planes = 3 this is the plain activation transposer.  times2 != 0 (bf16 source only) doubles each
+ * plane as bf16(2 x), exact for finite values, +-inf on overflow, NaN stays NaN: the backward factor 1/(1-ratio) of a
+ * ratio-0.5 F.dropout whose kept set is {y > 0}. */
 int frcnn_grad_prepare(const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi, const void* y_lo,
                        const void* p_hi, const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo,
                        int planes, int times2, void* stream);

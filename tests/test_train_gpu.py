@@ -396,29 +396,13 @@ def _route_reference(g_in, y, p):
     return np.where(y > 0, v, 0).astype(f32)
 
 
-def test_rpn_train_step_layerwise_and_end_to_end():
-    """The whole train_rpn.py step: forward + AnchorTargetLayer + losses + backward (15 convs: weight gradient, data
-    gradient, ReLU / max-pool backward) + WeightDecay + MomentumSGD.
-
-    ReLU and max-pool make the end-to-end gradient DISCONTINUOUS in the forward activations: one pre-activation whose
-    sign differs between two correct implementations changes every upstream gradient by ~1e-3 of its max-norm (the
-    float32 and float64 runs of the oracle itself differ by 4e-4 from conv3_3 down for exactly this reason).  So:
-      (1) layer by layer, on the DEVICE's own tensors: the masked/routed gradient is exactly the restated rule, and each
-          layer's dW / db / dX match float64 conv gradients of the same inputs within 5e-5 of max-norm (continuous
-          functions: bf16x3 precision only);
-      (2) end to end against the float64 autograd oracle: losses 1e-4, every gradient within 1e-2 of max-norm (flips),
-          and the optimizer update rule over two steps (momentum)."""
-    from frcnn_b200.train_engine import RpnTrainer
+def _rpn_layerwise_errors(tr, params, x, dbg, dev="cpu"):
+    """Part (1) of the RPN step check, on the trainer's own tensors after tr.backward(debug=dbg): per layer the masked /
+    routed gradient equals the restated rule exactly, and dW / db / dX against float64 conv gradients (computed on `dev`)
+    of the same inputs.  Returns the worst dW/db and dX errors relative to max-norm."""
     import torch.nn.grad as tg
-    H, W = 296, 392                        # ragged pooled sizes: 296->148->74->37->19, 392->196->98->49->25
-    params, x, gt, info = _train_case(H, W, 3)
-    tr = RpnTrainer(params, H, W, ANCHORS, precision="bf16x3", subsample="none")
-    losses = tr.forward(_dev(x[0]), _dev(gt[0]))
-    dbg = {}
-    tr.backward(debug=dbg)
-    torch.cuda.synchronize()
-    # ---- (1) layer-wise, float64 on the device's own activations / gradients
-    f64 = lambda a: torch.from_numpy(np.asarray(a, np.float64))
+    f64 = lambda a: torch.from_numpy(np.asarray(a, np.float64)).to(dev)
+    host = lambda t: t.cpu().numpy()
     worst_w = worst_x = 0.0
     for i, L in enumerate(tr.layers):
         name = L["name"]
@@ -433,12 +417,12 @@ def test_rpn_train_step_layerwise_and_end_to_end():
             xin = f64(x)                                                                  # conv1_1 sees the image itself
         else:
             xin = f64(tr._input_of(L).to_chw_f32().cpu().numpy())[None]
-        dw_ref = tg.conv2d_weight(xin, Wt.shape, dy, padding=1).numpy()
+        dw_ref = host(tg.conv2d_weight(xin, Wt.shape, dy, padding=1))
         e_w = _rel(tr.grads(name + "/W").cpu().numpy(), dw_ref)
-        e_b = _rel(tr.grads(name + "/b").cpu().numpy(), dy.sum((0, 2, 3)).numpy())
+        e_b = _rel(tr.grads(name + "/b").cpu().numpy(), host(dy.sum((0, 2, 3))))
         e_x = 0.0
         if i > 0:
-            dx_ref = tg.conv2d_input(xin.shape, Wt, dy, padding=1).numpy()[0]
+            dx_ref = host(tg.conv2d_input(xin.shape, Wt, dy, padding=1))[0]
             e_x = _rel(d["g_out"].cpu().numpy(), dx_ref)
         print("  %-22s dW %.2e  db %.2e  dX %.2e" % (name, e_w, e_b, e_x))
         worst_w, worst_x = max(worst_w, e_w, e_b), max(worst_x, e_x)
@@ -446,14 +430,39 @@ def test_rpn_train_step_layerwise_and_end_to_end():
     dyh = f64(dbg["heads"]["dy"].cpu().numpy())[None][:, :54]
     mid = f64(tr.layers[13]["y"].to_chw_f32().cpu().numpy())[None]
     Wh = f64(np.concatenate([params["RPN/rpn_cls_score/W"], params["RPN/rpn_bbox_pred/W"]], 0))
-    dwh = tg.conv2d_weight(mid, Wh.shape, dyh).numpy()
+    dwh = host(tg.conv2d_weight(mid, Wh.shape, dyh))
     got_wh = np.concatenate([tr.grads("RPN/rpn_cls_score/W").cpu().numpy(), tr.grads("RPN/rpn_bbox_pred/W").cpu().numpy()], 0)
     got_bh = np.concatenate([tr.grads("RPN/rpn_cls_score/b").cpu().numpy(), tr.grads("RPN/rpn_bbox_pred/b").cpu().numpy()], 0)
-    e_w, e_b = _rel(got_wh, dwh), _rel(got_bh, dyh.sum((0, 2, 3)).numpy())
-    e_x = _rel(dbg["heads"]["g_out"].cpu().numpy(), tg.conv2d_input(mid.shape, Wh, dyh).numpy()[0])
+    e_w, e_b = _rel(got_wh, dwh), _rel(got_bh, host(dyh.sum((0, 2, 3))))
+    e_x = _rel(dbg["heads"]["g_out"].cpu().numpy(), host(tg.conv2d_input(mid.shape, Wh, dyh))[0])
     print("  %-22s dW %.2e  db %.2e  dX %.2e" % ("RPN heads", e_w, e_b, e_x))
     worst_w, worst_x = max(worst_w, e_w, e_b), max(worst_x, e_x)
     print("layer-wise worst: dW/db %.2e, dX %.2e" % (worst_w, worst_x))
+    return worst_w, worst_x
+
+
+def test_rpn_train_step_layerwise_and_end_to_end():
+    """The whole train_rpn.py step: forward + AnchorTargetLayer + losses + backward (15 convs: weight gradient, data
+    gradient, ReLU / max-pool backward) + WeightDecay + MomentumSGD.
+
+    ReLU and max-pool make the end-to-end gradient DISCONTINUOUS in the forward activations: one pre-activation whose
+    sign differs between two correct implementations changes every upstream gradient by ~1e-3 of its max-norm (the
+    float32 and float64 runs of the oracle itself differ by 4e-4 from conv3_3 down for exactly this reason).  So:
+      (1) layer by layer, on the DEVICE's own tensors: the masked/routed gradient is exactly the restated rule, and each
+          layer's dW / db / dX match float64 conv gradients of the same inputs within 5e-5 of max-norm (continuous
+          functions: bf16x3 precision only);
+      (2) end to end against the float64 autograd oracle: losses 1e-4, every gradient within 1e-2 of max-norm (flips),
+          and the optimizer update rule over two steps (momentum)."""
+    from frcnn_b200.train_engine import RpnTrainer
+    H, W = 296, 392                        # ragged pooled sizes: 296->148->74->37->19, 392->196->98->49->25
+    params, x, gt, info = _train_case(H, W, 3)
+    tr = RpnTrainer(params, H, W, ANCHORS, precision="bf16x3", subsample="none")
+    losses = tr.forward(_dev(x[0]), _dev(gt[0]))
+    dbg = {}
+    tr.backward(debug=dbg)
+    torch.cuda.synchronize()
+    # ---- (1) layer-wise, float64 on the device's own activations / gradients
+    worst_w, worst_x = _rpn_layerwise_errors(tr, params, x, dbg)
     assert worst_w <= 5e-5 and worst_x <= 5e-5
     # ---- (2) end to end
     n_in = int(tr.targets.counts[0].item())
@@ -502,6 +511,21 @@ def test_rpn_train_step_layerwise_and_end_to_end():
     l3 = tr.forward(_dev(x[0]), _dev(gt[0])).cpu().numpy()
     print("loss after 0/2 updates: %.5f -> %.5f" % (Lv[3], l3[3]))
     assert l3[3] < Lv[3]
+
+
+def test_rpn_train_step_layerwise_600x1000():
+    """Part (1) of the step check above at the benchmarked 600x1000 image: every layer's routing / masking exact and its
+    dW / db / dX within 5e-5 of max-norm of float64 references (computed on the GPU at this size)."""
+    from frcnn_b200.train_engine import RpnTrainer
+    H, W = 600, 1000
+    params, x, gt, info = _train_case(H, W, 3)
+    tr = RpnTrainer(params, H, W, ANCHORS, precision="bf16x3", subsample="none")
+    tr.forward(_dev(x[0]), _dev(gt[0]))
+    dbg = {}
+    tr.backward(debug=dbg)
+    torch.cuda.synchronize()
+    worst_w, worst_x = _rpn_layerwise_errors(tr, params, x, dbg, dev="cuda")
+    assert worst_w <= 5e-5 and worst_x <= 5e-5
 
 
 # ------------------------------------------------------------------ RCNN-head training (train_rcnn.py)
