@@ -113,17 +113,6 @@ __device__ __forceinline__ float det_expf(float x) {
     return __fmul_rn(__fmul_rn(p, pow2i(h)), pow2i(ni - h));
 }
 
-// Order-preserving map float -> uint32 (larger float => larger key) that encodes the project's one score order (DESIGN §2):
-// -0.0 and +0.0 get the same key, and every NaN, whatever its sign and payload, gets key 1, below -inf's 0x007FFFFF.  Key 0
-// is never produced: it marks "filtered out" entries.  Rank-by-counting with (key desc, index asc) is therefore the same
-// total order as the oracle's orc_cmp_desc.
-__device__ __forceinline__ uint32_t float_to_ordered(float f) {
-    if (f != f) return 1u;
-    uint32_t b = __float_as_uint(f);
-    if (b == 0x80000000u) b = 0u;
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-
 // bf16 hi/lo split of an fp32 value: v ~= hi + lo with 16 significant bits ("bf16x3" operands).
 __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(v);

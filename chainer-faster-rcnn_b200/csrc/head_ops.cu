@@ -10,6 +10,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "nms_math.cuh"
 
 namespace frcnn {
 
@@ -504,25 +505,14 @@ __global__ void head_decode_kernel(const float* scores, const float* deltas, int
 }
 
 // ------------------------------------------------------------------------------------------ per-class detection
-// One CTA per foreground class, R <= 2048 rows.  Rank-by-counting sort (the score order of DESIGN §2 on float_to_ordered
-// keys: descending, -0.0 == +0.0, NaN last, ties to the lower index), then the suppression as
-// a bitmask: every thread fills rows of the R x R/64 "i suppresses j" matrix in shared memory (upper triangle, exact
-// cpu_nms arithmetic), and ONE warp walks the rows in rank order keeping `removed` in registers (lane w owns word w, a
-// second pass for R > 2048/... never needed: R <= 2048 = 32 words) -- the greedy chain costs a shuffle + a few ALU ops per
-// row instead of a block-wide barrier per kept box (the first version: 85 us for 300 rows x 20 classes; this one: 40 us).
+// One CTA per foreground class, R <= 2048 rows: rank by counting in the score order of nms_math.cuh, then the greedy
+// suppression with cpu_nms's exact decision.  detect_kernel builds the R x R/64 "i suppresses j" bitmask in shared memory
+// (upper triangle), and ONE warp walks its rows in rank order keeping `removed` in registers (lane w owns word w; R <= 2048
+// = 32 words) -- the greedy chain costs a shuffle + a few ALU ops per row instead of a block-wide barrier per kept box (the
+// barrier version: 85 us for 300 rows x 20 classes; the bitmask: 40 us).
 constexpr int kDetThreads = 256;                      // detect_barrier_kernel
 constexpr int kDetMaskThreads = 1024;                 // detect_kernel: 20 CTAs on 132 SMs -- the rank and mask phases scale with the CTA
 constexpr int kDetMaxR = 2048;
-
-__device__ __forceinline__ float det_iou(const float4 a, const float4 b) {
-    const float area_a = __fmul_rn(__fadd_rn(__fsub_rn(a.z, a.x), 1.0f), __fadd_rn(__fsub_rn(a.w, a.y), 1.0f));
-    const float area_b = __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.0f), __fadd_rn(__fsub_rn(b.w, b.y), 1.0f));
-    const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y), xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-    const float w = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-    const float h = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-    const float inter = __fmul_rn(w, h);
-    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
-}
 
 __global__ void __launch_bounds__(kDetMaskThreads) detect_kernel(const float* prob, const float* boxes, const int* count,
                                                              int R_cap, int NC, double thr, float conf,
@@ -550,32 +540,26 @@ __global__ void __launch_bounds__(kDetMaskThreads) detect_kernel(const float* pr
         if (nge) atomicAdd(&s_nge, nge);
     }
     __syncthreads();
-    // rank = position in the score order of DESIGN §2 (descending; -0.0 == +0.0; NaN last; ties: lower roi first): a
-    // permutation of [0, R), and the rows with score >= conf come first whatever else the rows hold
+    // rank: a permutation of [0, R), and the rows with score >= conf come first whatever else the rows hold.  (The same
+    // prologue as detect_barrier_kernel's; as a shared function it cost this kernel 2%: R left the uniform registers.)
     for (int r = tid; r < R; r += kDetMaskThreads) {
         const uint32_t s = skey[r];
         int rank = 0;
-        for (int q = 0; q < R; ++q) {
-            const uint32_t t = skey[q];
-            rank += (t > s) || (t == s && q < r);
-        }
+        for (int q = 0; q < R; ++q) rank += ahead(skey[q], q, s, r);
         order[rank] = r;
         const float4 b = reinterpret_cast<const float4*>(boxes)[(long)r * NC + cls];
         sbox[rank] = b;
-        sarea[rank] = __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.0f), __fadd_rn(__fsub_rn(b.w, b.y), 1.0f));
+        sarea[rank] = box_area(b);
     }
     __syncthreads();
     // mask rows: item = (word w, row i) with w >= i/64 (upper triangle), i fastest: the lanes of a warp work on consecutive
     // rows i against the SAME 64 columns, so sbox[j] is a broadcast read and sbox[i] a conflict-free one (with w fastest the
-    // lanes read 5 different boxes 1 KB apart = the same banks: measured 4x slower).  The 64-pair loop is straight-line code
-    // (as in nms_mask_kernel): the decision "iou >= thr" is taken with products wherever that is provably the same decision
-    // as the reference's divide + double compare (models/cpu_nms.pyx:64-65); the pairs the products cannot decide (within
-    // 1e-5 of the threshold, a non-positive union) are recorded in a second word and take the exact sequence after the loop.
-    // Columns past R hold whatever the shared memory held: their bits are masked off, never used.
+    // lanes read 5 different boxes 1 KB apart = the same banks: measured 4x slower).
+    // The pair loop of suppress_word64(), written out: at this kernel's 64-register cap the shared routine needs 8 more bytes
+    // of stack; with the `pt.on` select the compiler specialises the loop for the common case instead.
     const int nw = (R + 63) >> 6;
     const float thr_f = (float)thr;
-    const float thr_lo = thr_f * (1.0f - 1e-5f), thr_hi = thr_f * (1.0f + 1e-5f);
-    const bool fast_ok = thr_f > 1e-3f;
+    const PreTest pt = pretest_bounds(thr_f);
     for (int it = tid; it < R * nw; it += kDetMaskThreads) {
         const int w = it / R, i = it - w * R;
         unsigned long long bits = 0ull;
@@ -586,28 +570,20 @@ __global__ void __launch_bounds__(kDetMaskThreads) detect_kernel(const float* pr
             uint32_t sup_w[2] = {0u, 0u}, und_w[2] = {0u, 0u};
 #pragma unroll
             for (int j = 0; j < 64; ++j) {
-                const float4 b = sbox[j0 + j];
-                const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y), xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-                const float ww = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-                const float hh = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-                const float inter = __fmul_rn(ww, hh);
-                const float uni = __fsub_rn(__fadd_rn(area_a, sarea[j0 + j]), inter);
-                const bool pos = uni > 0.0f;
-                const bool yes = pos && inter > thr_hi * uni, no = pos && inter < thr_lo * uni;
-                sup_w[j >> 5] |= (uint32_t)yes << (j & 31);
-                und_w[j >> 5] |= (uint32_t)!(yes || no) << (j & 31);
+                float inter, uni;
+                inter_union(a, area_a, sbox[j0 + j], sarea[j0 + j], inter, uni);
+                uint32_t sure, und;
+                pretest(inter, uni, pt, sure, und);
+                sup_w[j >> 5] |= sure << (j & 31);
+                und_w[j >> 5] |= und << (j & 31);
             }
             const int lo = max(i + 1 - j0, 0), hi = min(R - j0, 64);              // live columns [lo, hi) of this word
             unsigned long long live = hi < 64 ? (1ull << hi) - 1ull : ~0ull;
             live = lo < 64 ? (live >> lo) << lo : 0ull;
             bits = ((unsigned long long)sup_w[0] | ((unsigned long long)sup_w[1] << 32)) & live;
-            unsigned long long und = fast_ok ? ((unsigned long long)und_w[0] | ((unsigned long long)und_w[1] << 32)) & live : live;
-            while (und != 0ull) {                                                 // rare: the reference's exact sequence
-                const int j = __ffsll((long long)und) - 1;
-                und &= und - 1ull;
-                const bool sup = (double)det_iou(a, sbox[j0 + j]) >= thr;
-                bits = sup ? (bits | (1ull << j)) : (bits & ~(1ull << j));
-            }
+            const unsigned long long und = pt.on ? ((unsigned long long)und_w[0] | ((unsigned long long)und_w[1] << 32)) & live : live;
+            bits = resolve_undecided(bits, und, [&](int j) { const float4 b = sbox[j0 + j]; return iou(a, box_area(a), b, box_area(b)); },
+                                     thr, thr_f, FRCNN_NMS_GE_DOUBLE);
         }
         mask[(size_t)i * words + w] = bits;
     }
@@ -679,10 +655,7 @@ __global__ void __launch_bounds__(kDetThreads) detect_barrier_kernel(const float
     for (int r = tid; r < R; r += kDetThreads) {             // the order of detect_kernel
         const uint32_t s = skey[r];
         int rank = 0;
-        for (int q = 0; q < R; ++q) {
-            const uint32_t t = skey[q];
-            rank += (t > s) || (t == s && q < r);
-        }
+        for (int q = 0; q < R; ++q) rank += ahead(skey[q], q, s, r);
         order[rank] = r;
         sbox[rank] = reinterpret_cast<const float4*>(boxes)[(long)r * NC + cls];
         dead[rank] = 0;
@@ -700,7 +673,9 @@ __global__ void __launch_bounds__(kDetThreads) detect_barrier_kernel(const float
         }
         ++nk;
         for (int j = i + 1 + tid; j < R; j += kDetThreads) {
-            if (!dead[j] && (double)det_iou(a, sbox[j]) >= thr) dead[j] = 1;
+            const float4 b = sbox[j];
+            // box_area(a) stays in the loop: hoisted, it would sit on the serial path of every pivot
+            if (!dead[j] && suppresses(iou(a, box_area(a), b, box_area(b)), thr, (float)thr, FRCNN_NMS_GE_DOUBLE)) dead[j] = 1;
         }
         __syncthreads();
     }

@@ -7,10 +7,9 @@
 // keeps one context: a stream, a MAPPED pinned staging block (dets in, keep list + completion flag out) and a device
 // workspace -- nothing is allocated or freed per call (the reference mallocs and frees its device scratch on every call,
 // nms_kernel.cu:100-108,142-143).  n <= 2048: ONE single-CTA kernel reads the boxes straight from the mapped host block
-// (zero-copy over PCIe), ranks them by counting (the score order of DESIGN §2: descending, -0.0 == +0.0, NaN last, ties:
-// lower index first), resolves the greedy suppression with a lazily built IoU bitmask (cpu_nms.pyx's exact float32 IoU /
-// double compare, or `_nms`'s float `>`), writes the keep list into the mapped block and raises a flag the host thread
-// polls: no cudaMemcpy, no cudaStreamSynchronize on this path.
+// (zero-copy over PCIe), ranks them by counting (the score order of nms_math.cuh), resolves the greedy suppression with a
+// lazily built IoU bitmask (cpu_nms.pyx's decision, or `_nms`'s float `>`), writes the keep list into the mapped block and
+// raises a flag the host thread polls: no cudaMemcpy, no cudaStreamSynchronize on this path.
 // n > 2048: the chip-wide pipeline of frcnn_nms (sort, 64x64 IoU bitmask, device-side scan) on the context's buffers.
 #include <stdint.h>
 #include <string.h>
@@ -22,6 +21,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "nms_math.cuh"
 
 namespace frcnn {
 
@@ -37,50 +37,32 @@ constexpr int kSmallMax = 2048;
 // the results straight into the `removed` words.
 // Phases: (1) the dense rows, coalesced 16-byte reads of the mapped host block; (2) rank by counting, all threads;
 // (3) diagonal blocks; (4) per 64-rank block: resolve, then kept rows x later columns; (5) keep list + count to the mapped
-// block in wide writes, fence, flag.  IoU arithmetic: cpu_nms.pyx's exact float32 expression / double compare wherever the
-// product pre-test cannot decide.
+// block in wide writes, fence, flag.
 constexpr int kFastThreadsMax = 1024;
 
-// bits[k] = box `i` (rank) suppresses box j0 + k, k < 16 (columns >= n read box n - 1; the caller masks them).
-// Branch-free inner loop (the compiler turned `if (decided) ... else divide` into three divergent branches per pair, which
-// ran at a third of the issue rate): the product pre-test fills `sb` (surely suppressed) and `ub` (undecided: |IoU - thr| <=
-// 1e-5 thr, a degenerate union, or thr <= 1e-3 where thr_hi / thr_lo are +-inf); the rare undecided pairs take
-// cpu_nms.pyx's exact division / double compare afterwards.
+// bits[k] = box `i` (rank) suppresses box j0 + k, k < 16 (columns >= n read box n - 1; the caller masks them): the pairs of
+// suppress_word64() in a rolled loop, for code size.  (With `if (decided) ... else divide` in the loop the compiler made
+// three divergent branches per pair, which ran at a third of the issue rate.)
 __device__ __forceinline__ unsigned sup_bits16(const float4* __restrict__ sbox, const float* __restrict__ area, int i, int j0, int n,
-                                               float thr_f, float thr_lo, float thr_hi, double thr_d, int mode) {
+                                               const PreTest pt, double thr_d, float thr_f, int mode) {
     const float4 a = sbox[i];
     const float area_a = area[i];
     unsigned sb = 0u, ub = 0u;
 #pragma unroll 4
     for (int k = 0; k < 16; ++k) {
         const int j = min(j0 + k, n - 1);
-        const float4 b = sbox[j];
-        const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y), xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-        const float ww = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-        const float hh = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-        const float inter = __fmul_rn(ww, hh);
-        const float uni = __fsub_rn(__fadd_rn(area_a, area[j]), inter);
-        const unsigned pos = uni > 0.0f;
-        const unsigned yes = inter > __fmul_rn(thr_hi, uni);
-        const unsigned no = inter < __fmul_rn(thr_lo, uni);
-        sb |= (pos & yes) << k;
-        ub |= ((pos & (yes | no)) ^ 1u) << k;
+        float inter, uni;
+        inter_union(a, area_a, sbox[j], area[j], inter, uni);
+        uint32_t sure, und;
+        pretest(inter, uni, pt, sure, und);
+        sb |= sure << k;
+        ub |= und << k;
     }
-    while (ub) {                                        // rare
-        const int k = __ffs((int)ub) - 1;
-        ub &= ub - 1u;
+    auto iou_of = [&](int k) {
         const int j = min(j0 + k, n - 1);
-        const float4 b = sbox[j];
-        const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y), xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-        const float ww = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-        const float hh = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-        const float inter = __fmul_rn(ww, hh);
-        const float uni = __fsub_rn(__fadd_rn(area_a, area[j]), inter);
-        const float ovr = __fdiv_rn(inter, uni);
-        const bool sup = mode == FRCNN_NMS_GE_DOUBLE ? ((double)ovr >= thr_d) : (ovr > thr_f);
-        sb = (sb & ~(1u << k)) | ((unsigned)sup << k);
-    }
-    return sb;
+        return iou(a, area_a, sbox[j], area[j]);
+    };
+    return resolve_undecided(sb, ub, iou_of, thr_d, thr_f, mode);
 }
 
 __global__ void __launch_bounds__(kFastThreadsMax) nms_small_fast_kernel(const float* __restrict__ dets, int n, int sd, int presorted,
@@ -114,10 +96,8 @@ __global__ void __launch_bounds__(kFastThreadsMax) nms_small_fast_kernel(const f
     }
     __syncthreads();
     FRCNN_NMS_STAMP(1);
-    // (2) rank by counting with ALL threads: `parts` threads per row, each compares its row's score key (float_to_ordered:
-    // the total order of DESIGN §2) against a slice of the densely re-packed keys, four per 16-byte broadcast load; the
-    // partial counts meet in shared-memory atomics.  Every real key is >= 1, so a row's count is the number of rows ahead
-    // of it in that order: a permutation of [0, n).
+    // (2) rank by counting with ALL threads: `parts` threads per row, each counts the rows ahead() of its own in a slice of
+    // the densely re-packed keys, four per 16-byte broadcast load; the partial counts meet in shared-memory atomics.
     if (!presorted) {
         for (int r = tid; r < n4; r += T) {
             skey[r] = r < n ? float_to_ordered(flat[r * sd + 4]) : 0u;   // padding never counts: key 0 is below every row's
@@ -135,10 +115,7 @@ __global__ void __launch_bounds__(kFastThreadsMax) nms_small_fast_kernel(const f
             for (int g = g0; g < g1; ++g) {
                 const uint4 t = reinterpret_cast<const uint4*>(skey)[g];
                 const int q = g << 2;
-                cnt += (int)(t.x > s) | ((int)(t.x == s) & (int)(q + 0 < r));
-                cnt += (int)(t.y > s) | ((int)(t.y == s) & (int)(q + 1 < r));
-                cnt += (int)(t.z > s) | ((int)(t.z == s) & (int)(q + 2 < r));
-                cnt += (int)(t.w > s) | ((int)(t.w == s) & (int)(q + 3 < r));
+                cnt += ahead(t.x, q + 0, s, r) + ahead(t.y, q + 1, s, r) + ahead(t.z, q + 2, s, r) + ahead(t.w, q + 3, s, r);
             }
             if (cnt) atomicAdd(&order[r], cnt);
         }
@@ -160,20 +137,19 @@ __global__ void __launch_bounds__(kFastThreadsMax) nms_small_fast_kernel(const f
                 const float4 bx = make_float4(d[0], d[1], d[2], d[3]);
                 order[my_rank[u]] = r;
                 sbox[my_rank[u]] = bx;
-                area[my_rank[u]] = __fmul_rn(__fadd_rn(__fsub_rn(bx.z, bx.x), 1.0f), __fadd_rn(__fsub_rn(bx.w, bx.y), 1.0f));
+                area[my_rank[u]] = box_area(bx);
             }
         }
     }
     __syncthreads();
     FRCNN_NMS_STAMP(2);
-    const bool fast_ok = thr_f > 1e-3f;                  // else: every pair takes the exact path
-    const float thr_lo = fast_ok ? thr_f * (1.0f - 1e-5f) : -INFINITY, thr_hi = fast_ok ? thr_f * (1.0f + 1e-5f) : INFINITY;
+    const PreTest pt = pretest_bounds(thr_f);
     // (3) diagonal blocks: item = (block b, 16-column quarter qd, local row il), il fastest
     for (int it = tid; it < nw * 256; it += T) {
         const int b = it >> 8, qd = (it >> 6) & 3, il = it & 63;
         const int i = (b << 6) + il, j0 = (b << 6) + (qd << 4);
         if (i >= n || j0 >= n || (qd << 4) + 15 <= il) continue;
-        unsigned bits = sup_bits16(sbox, area, i, j0, n, thr_f, thr_lo, thr_hi, thr_d, mode);
+        unsigned bits = sup_bits16(sbox, area, i, j0, n, pt, thr_d, thr_f, mode);
         // keep j > i and j < n
         const int lo = il + 1 - (qd << 4);                                   // first valid k
         if (lo > 0) bits &= ~((1u << lo) - 1u);
@@ -237,7 +213,7 @@ __global__ void __launch_bounds__(kFastThreadsMax) nms_small_fast_kernel(const f
             for (int it = tid; it < kb * ncq; it += T) {
                 const int cq = it / kb, k = it - cq * kb;       // k fastest: a warp = different kept rows, same columns
                 const int i = r0 + s_kl[k], j0 = c0 + (cq << 4);
-                unsigned bits = sup_bits16(sbox, area, i, j0, n, thr_f, thr_lo, thr_hi, thr_d, mode);
+                unsigned bits = sup_bits16(sbox, area, i, j0, n, pt, thr_d, thr_f, mode);
                 const int hi = n - j0;
                 if (hi < 16) bits &= (1u << hi) - 1u;
                 if (bits) atomicOr(&removed32[j0 >> 5], bits << (j0 & 16));

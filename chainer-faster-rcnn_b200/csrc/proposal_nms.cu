@@ -19,6 +19,7 @@
 //   5. nms_scan_kernel     ONE CTA walks the mask (device-side; the reference copies it to the host,
 //                          nms_kernel.cu:124-139), stops at post_nms_top_n, gathers the output rows
 #include "common.cuh"
+#include "nms_math.cuh"
 
 namespace frcnn {
 
@@ -317,31 +318,10 @@ __global__ void __launch_bounds__(kRankThreads) rank_scatter_kernel(const SortAr
 
 
 // ------------------------------------------------------------------------------------------ 3. IoU bitmask
-// IoU exactly as models/cpu_nms.pyx:58-65 (float32, one rounding per op, true division).
-__device__ __forceinline__ float iou_plus1(const float4 a, const float area_a, const float4 b) {
-    const float area_b = __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.0f), __fadd_rn(__fsub_rn(b.w, b.y), 1.0f));
-    const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-    const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-    const float w = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-    const float h = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-    const float inter = __fmul_rn(w, h);
-    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
-}
-__device__ __forceinline__ bool suppresses(float ovr, double thr_d, float thr_f, int mode) {
-    return mode == FRCNN_NMS_GE_DOUBLE ? ((double)ovr >= thr_d) : (ovr > thr_f);
-}
-
 // grid (col_blocks, col_blocks); only blocks with col >= row do work.  mask[row_box][col_block].
-// Thread = one row box against the block's 64 column boxes (shared memory, broadcast reads, areas precomputed).  The pair loop
-// is fully unrolled and branch-free: the first version skipped disjoint pairs with `continue` and chose between three decision
-// paths per pair, so the lanes of a warp (different row boxes) diverged on almost every column and the warp paid for the sum
-// of the paths (38 us for 6000 boxes, ~4x the instruction-issue bound).  Here every pair costs the same ~25 instructions, the
-// bit position is a compile-time constant (32-bit words, no 64-bit variable shift), and the pairs the fast test cannot decide
-// are only RECORDED in the loop; the exact sequence runs for them afterwards.
-// Fast exact-safe test: with u = area_a + area_b - inter, the decision "inter/u >= thr" is certain whenever u > 0 and inter is
-// outside [thr*u*(1-1e-5), thr*u*(1+1e-5)] (the float roundings involved are < 1e-6 relative); a disjoint pair has
-// inter == 0 < thr_lo*u.  Everything else -- within 1e-5 of the threshold, u <= 0 or NaN (degenerate boxes), thr <= 1e-3 --
-// takes the reference's own sequence: float divide, then the compare of models/cpu_nms.pyx:64-65 / nms_kernel.cu's '>'.
+// Thread = one row box against the block's 64 column boxes (shared memory, broadcast reads, areas precomputed): one
+// branch-free suppress_word64() per thread, ~25 instructions a pair.  (Pairs that branched on their decision path
+// diverged the warp on almost every column: 38 us for 6000 boxes, ~4x the instruction-issue bound.)
 __global__ void __launch_bounds__(64) nms_mask_kernel(const float4* boxes, const int* n_ptr, int n_cap,
                                                       double thr_d, float thr_f, int mode,
                                                       unsigned long long* mask, int col_blocks) {
@@ -356,41 +336,16 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const float4* boxes, const
     {
         const float4 b = t < ccount ? boxes[cb * 64 + t] : make_float4(0.f, 0.f, 0.f, 0.f);
         cbox[t] = b;
-        carea[t] = __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.0f), __fadd_rn(__fsub_rn(b.w, b.y), 1.0f));
+        carea[t] = box_area(b);
     }
     __syncthreads();
     const int ri = rb * 64 + t;
     if (ri >= n) return;
     const float4 a = boxes[ri];
-    const float area_a = __fmul_rn(__fadd_rn(__fsub_rn(a.z, a.x), 1.0f), __fadd_rn(__fsub_rn(a.w, a.y), 1.0f));
     const int start = (rb == cb) ? t + 1 : 0;               // the diagonal block: pairs (i, j > i) only
-    const float thr_lo = thr_f * (1.0f - 1e-5f), thr_hi = thr_f * (1.0f + 1e-5f);
-    uint32_t sup_w[2] = {0u, 0u}, und_w[2] = {0u, 0u};     // bit j: "suppresses" by the fast test / the fast test cannot say
-#pragma unroll
-    for (int j = 0; j < 64; ++j) {
-        const float4 b = cbox[j];
-        const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-        const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-        const float w = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-        const float h = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
-        const float inter = __fmul_rn(w, h);
-        const float uni = __fsub_rn(__fadd_rn(area_a, carea[j]), inter);
-        const bool pos = uni > 0.0f;
-        const bool yes = pos && inter > thr_hi * uni, no = pos && inter < thr_lo * uni;
-        sup_w[j >> 5] |= (uint32_t)yes << (j & 31);
-        und_w[j >> 5] |= (uint32_t)!(yes || no) << (j & 31);
-    }
     unsigned long long live = ccount < 64 ? (1ull << ccount) - 1ull : ~0ull;       // columns [start, ccount)
     live = start < 64 ? (live >> start) << start : 0ull;
-    unsigned long long bits = ((unsigned long long)sup_w[0] | ((unsigned long long)sup_w[1] << 32)) & live;
-    unsigned long long und = thr_f > 1e-3f ? ((unsigned long long)und_w[0] | ((unsigned long long)und_w[1] << 32)) & live : live;
-    while (und != 0ull) {                                   // rare: the reference's exact sequence, pair by pair
-        const int j = __ffsll((long long)und) - 1;
-        und &= und - 1ull;
-        const bool sup = suppresses(iou_plus1(a, area_a, cbox[j]), thr_d, thr_f, mode);
-        bits = sup ? (bits | (1ull << j)) : (bits & ~(1ull << j));
-    }
-    mask[(long)ri * col_blocks + cb] = bits;
+    mask[(long)ri * col_blocks + cb] = suppress_word64(a, box_area(a), cbox, carea, live, pretest_bounds(thr_f), thr_d, thr_f, mode);
 }
 
 // ------------------------------------------------------------------------------------------ 4. mask scan

@@ -13,21 +13,9 @@
 //                                           64-bit fixed-point atomics (order independent: bit-reproducible), then converted
 // Small latency-bound kernels (<= 300 RoIs): no tensor cores by design.
 #include "common.cuh"
+#include "nms_math.cuh"
 
 namespace frcnn {
-
-// bbox.pyx:32-55 on (double)proposal x (double)gt row
-__device__ __forceinline__ double roi_iou(const float4 b, const float* q) {
-    const double b0 = b.x, b1 = b.y, b2 = b.z, b3 = b.w, q0 = q[0], q1 = q[1], q2 = q[2], q3 = q[3];
-    const double qa = __dmul_rn(__dadd_rn(__dsub_rn(q2, q0), 1.0), __dadd_rn(__dsub_rn(q3, q1), 1.0));
-    const double iw = __dadd_rn(__dsub_rn(fmin(b2, q2), fmax(b0, q0)), 1.0);
-    if (!(iw > 0.0)) return 0.0;
-    const double ih = __dadd_rn(__dsub_rn(fmin(b3, q3), fmax(b1, q1)), 1.0);
-    if (!(ih > 0.0)) return 0.0;
-    const double ba = __dmul_rn(__dadd_rn(__dsub_rn(b2, b0), 1.0), __dadd_rn(__dsub_rn(b3, b1), 1.0));
-    const double inter = __dmul_rn(iw, ih);
-    return __ddiv_rn(inter, __dsub_rn(__dadd_rn(ba, qa), inter));
-}
 
 __global__ void roi_overlaps_kernel(const float* __restrict__ rois, const int* __restrict__ count, int R_cap,
                                     const float* __restrict__ gt, int n_gt, double* __restrict__ max_ov, int* __restrict__ argmax) {
@@ -37,9 +25,12 @@ __global__ void roi_overlaps_kernel(const float* __restrict__ rois, const int* _
     double best = -1.0;
     int bi = -1;
     if (r < R) {
-        const float4 b = reinterpret_cast<const float4*>(rois)[r];
+        const float4 rb = reinterpret_cast<const float4*>(rois)[r];
+        const double b[4] = {rb.x, rb.y, rb.z, rb.w};
         for (int g = 0; g < n_gt; ++g) {
-            const double ov = roi_iou(b, gt + (size_t)g * 5);
+            const float* gr = gt + (size_t)g * 5;
+            const double q[4] = {gr[0], gr[1], gr[2], gr[3]};
+            const double ov = iou_f64(b, q, box_area_f64(q[0], q[1], q[2], q[3]));   // bbox.pyx on (double)proposal x (double)gt row
             if (ov > best) { best = ov; bi = g; }          // first maximum (numpy argmax)
         }
     }

@@ -17,6 +17,7 @@
 // the device offers (0) none, (1) a counter-hash selection (deterministic in (seed, anchor index), no host sync), and
 // (2) explicit index sets (how parity with a recorded reference run is pinned).
 #include "common.cuh"
+#include "nms_math.cuh"
 
 namespace frcnn {
 
@@ -36,22 +37,6 @@ __device__ __forceinline__ bool anchor_box(const AnchorGeom& g, int i, double b[
     return b[0] >= 0.0 && b[1] >= 0.0 && b[2] < (double)g.im_w && b[3] < (double)g.im_h;
 }
 
-// bbox.pyx:32-55, same operation order.  q_area = (q2-q0+1)*(q3-q1+1) is hoisted like the reference does (:33-36).
-__device__ __forceinline__ double iou_f64(const double b[4], double q0, double q1, double q2, double q3, double q_area) {
-    double iw = __dadd_rn(__dsub_rn(fmin(b[2], q2), fmax(b[0], q0)), 1.0);
-    if (!(iw > 0.0)) return 0.0;
-    double ih = __dadd_rn(__dsub_rn(fmin(b[3], q3), fmax(b[1], q1)), 1.0);
-    if (!(ih > 0.0)) return 0.0;
-    double b_area = __dmul_rn(__dadd_rn(__dsub_rn(b[2], b[0]), 1.0), __dadd_rn(__dsub_rn(b[3], b[1]), 1.0));
-    double inter = __dmul_rn(iw, ih);
-    double ua = __dsub_rn(__dadd_rn(b_area, q_area), inter);
-    return __ddiv_rn(inter, ua);
-}
-
-__device__ __forceinline__ double gt_area(const float* q) {
-    return __dmul_rn(__dadd_rn(__dsub_rn((double)q[2], (double)q[0]), 1.0), __dadd_rn(__dsub_rn((double)q[3], (double)q[1]), 1.0));
-}
-
 // ------------------------------------------------------------------------------------------ bbox_overlaps (generic)
 __global__ void bbox_overlaps_kernel(const double* __restrict__ boxes, int N, const double* __restrict__ query, int K,
                                      double* __restrict__ out) {
@@ -59,9 +44,8 @@ __global__ void bbox_overlaps_kernel(const double* __restrict__ boxes, int N, co
     if (t >= (long)N * K) return;
     int n = (int)(t / K), k = (int)(t % K);
     double b[4] = {boxes[n * 4], boxes[n * 4 + 1], boxes[n * 4 + 2], boxes[n * 4 + 3]};
-    double q0 = query[k * 4], q1 = query[k * 4 + 1], q2 = query[k * 4 + 2], q3 = query[k * 4 + 3];
-    double qa = __dmul_rn(__dadd_rn(__dsub_rn(q2, q0), 1.0), __dadd_rn(__dsub_rn(q3, q1), 1.0));
-    out[t] = iou_f64(b, q0, q1, q2, q3, qa);
+    double q[4] = {query[k * 4], query[k * 4 + 1], query[k * 4 + 2], query[k * 4 + 3]};
+    out[t] = iou_f64(b, q, box_area_f64(q[0], q[1], q[2], q[3]));
 }
 
 // ------------------------------------------------------------------------------------------ 1. overlaps: row max / arg-max, column max
@@ -84,14 +68,14 @@ __global__ void __launch_bounds__(256) anchor_overlap_kernel(AnchorGeom g, int n
         for (int t = threadIdx.x; t < gc; t += blockDim.x) {
             const float* q = gt + (size_t)(g0 + t) * 5;
             s_gt[t * 4 + 0] = q[0]; s_gt[t * 4 + 1] = q[1]; s_gt[t * 4 + 2] = q[2]; s_gt[t * 4 + 3] = q[3];
-            s_area[t] = gt_area(q);
+            s_area[t] = box_area_f64(q[0], q[1], q[2], q[3]);
             s_max[t] = 0ull;
         }
         __syncthreads();
         if (inside) {
             for (int t = 0; t < gc; ++t) {
-                double ov = iou_f64(b, (double)s_gt[t * 4], (double)s_gt[t * 4 + 1], (double)s_gt[t * 4 + 2],
-                                    (double)s_gt[t * 4 + 3], s_area[t]);
+                const double q[4] = {s_gt[t * 4], s_gt[t * 4 + 1], s_gt[t * 4 + 2], s_gt[t * 4 + 3]};
+                double ov = iou_f64(b, q, s_area[t]);
                 if (ov > best) { best = ov; best_g = g0 + t; }          // strict: first maximum wins (numpy argmax)
                 unsigned long long bits = (unsigned long long)__double_as_longlong(ov);   // ov >= 0: bit order == value order
                 if (bits > s_max[t]) atomicMax(&s_max[t], bits);
@@ -123,8 +107,9 @@ __global__ void __launch_bounds__(256) anchor_label_kernel(AnchorGeom g, int n_a
         double mo = max_ov[i];
         bool is_gt_best = false;                       // np.where(overlaps == gt_max_overlaps)[0]: every tie, any gt (:196)
         for (int t = 0; t < n_gt && !is_gt_best; ++t) {
-            const float* q = gt + (size_t)t * 5;
-            double ov = iou_f64(b, (double)q[0], (double)q[1], (double)q[2], (double)q[3], gt_area(q));
+            const float* gr = gt + (size_t)t * 5;
+            const double q[4] = {gr[0], gr[1], gr[2], gr[3]};
+            double ov = iou_f64(b, q, box_area_f64(q[0], q[1], q[2], q[3]));
             is_gt_best = (unsigned long long)__double_as_longlong(ov) == gt_max_bits[t];
         }
         // :137-146 in order: bg, per-gt best, >= pos_thr, bg again (clobbers)
