@@ -84,7 +84,26 @@ struct ConvParams {
     // y_f32 + part*part_stride.  n_parts == 1: an ordinary convolution.
     int n_parts, tiles_per_part, splits, kb_per_split, kb_total, g_row_stride;
     long part_stride;
+    // batch: n_img images of one H x W shape, [n_img][H][W][C] (A through a 4-D tensor map {C, W, H, image} when n_img > 1).
+    // Pixel tile mt is tile mt % img_tiles of image mt / img_tiles; each image keeps the one-image plan, and every output
+    // (bf16, pooled bf16, fp32, residual) is addressed in its own image at img_pix (img_opix pooled) pixels per image.
+    int n_img, img_tiles;
+    FastDiv fd_img_tiles;
+    long img_pix, img_opix;
 };
+
+// Pixel tile mt -> (image, first row, first column).  Past the last tile (odd count, CTA pairs) the row lies below the
+// last image: loads read zeros and nothing is stored.
+__device__ __forceinline__ void tile_origin(const ConvParams& p, int mt, int& img, int& h0, int& w0) {
+    img = 0;
+    if (p.n_img > 1) {
+        img = min(fd_div(mt, p.fd_img_tiles), p.n_img - 1);
+        mt -= img * p.img_tiles;
+    }
+    const int th_i = fd_div(mt, p.fd_tiles_w);
+    h0 = th_i * p.TH;
+    w0 = (mt - th_i * p.tiles_w) * p.TW;
+}
 
 constexpr int kNumThreads = 384;          // warpgroup 0 producer, warpgroups 1-2 MMA + epilogue
 constexpr int kTileM = 128;
@@ -128,11 +147,12 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b, float& ra, flo
 }
 
 // One 16-channel run of one pixel: bias, residual, ReLU, validity, fp32 and bf16 (hi / lo, optionally 2x2-pooled) stores.
-__device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16], int part, int h, int w, int n, int lane,
-                                             int m_valid) {
+__device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16], int part, int img, int h, int w, int n,
+                                             int lane, int m_valid) {
     const bool in_img = (h < p.H) && (w < p.W);
-    const long pix = (long)h * p.W + w;
-    const bool live = in_img && pix < m_valid;
+    const long ipix = (long)h * p.W + w;
+    const long pix = img * p.img_pix + ipix;
+    const bool live = in_img && ipix < m_valid;
     if (p.bias != nullptr) {                    // split-K partial sums carry no bias (the reduction adds it once)
         const float4* b4 = reinterpret_cast<const float4*>(p.bias + n);
 #pragma unroll
@@ -188,7 +208,7 @@ __device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16]
                 v[j] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, tw_mask));
             }
             writer = in_img && (lane & (1 | tw_mask)) == 0;
-            opix = (long)(h >> 1) * ((p.W + 1) >> 1) + (w >> 1);
+            opix = img * p.img_opix + (long)(h >> 1) * ((p.W + 1) >> 1) + (w >> 1);
         }
         if (writer) {
             uint4 hv[2], lv[2];
@@ -301,10 +321,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                 const int part = fd_div(tile, p.fd_tiles_per_part), t2 = tile - part * p.tiles_per_part;
                 const int mq = fd_div(t2, p.fd_n_tiles), nt = t2 - mq * p.n_tiles;
                 const int mt = mq * CG + (int)rank;      // past the last pixel tile (odd count): loads zeros, stores nothing
-                const int th_i = fd_div(mt, p.fd_tiles_w);
-                const int h0 = th_i * p.TH;
-                const int w0 = (mt - th_i * p.tiles_w) * p.TW;
+                int img, h0, w0;
+                tile_origin(p, mt, img, h0, w0);
                 const int n0 = nt * BN;
+                // one image: the 3-D map; a batch: the 4-D map, whose out-of-bounds fill pads every image on its own
+                auto load_a = [&](uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int k, int w, int h) {
+                    if (p.n_img > 1) ptx::tma_load_4d(dst, tm, bar, k, w, h, img);
+                    else ptx::tma_load_3d(dst, tm, bar, k, w, h);
+                };
                 const int nkb = part_kblocks(p, part, num_kb);
                 const int ka = part_k0(p, part) * BK, kboff = ka + part_b_shift(p, part);
                 const int bplane = part_b_plane(p, part);
@@ -317,11 +341,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                     else ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t* st = ring + (size_t)stage * stage_bytes;
                     ptx::mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
-                    ptx::tma_load_3d(st, &tm_a_hi, &full_bar[stage], ka + cb * BK, w0 + s - p.pad_w, h0 + r - p.pad_h);
+                    load_a(st, &tm_a_hi, &full_bar[stage], ka + cb * BK, w0 + s - p.pad_w, h0 + r - p.pad_h);
                     if (!bres) load_b(st + C::A_BYTES, &tm_b_hi, &full_bar[stage], kboff + cb * BK, n0, btap);
                     if (X3) {
                         uint8_t* st2 = st + a_lo_off;
-                        ptx::tma_load_3d(st2, &tm_a_lo, &full_bar[stage], ka + cb * BK, w0 + s - p.pad_w, h0 + r - p.pad_h);
+                        load_a(st2, &tm_a_lo, &full_bar[stage], ka + cb * BK, w0 + s - p.pad_w, h0 + r - p.pad_h);
                         if (!bres) load_b(st2 + C::A_BYTES, &tm_b_lo, &full_bar[stage], kboff + cb * BK, n0, btap);
                     }
                     if (++stage == S) { stage = 0; phase ^= 1; }
@@ -360,8 +384,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             const int part = fd_div(tile, p.fd_tiles_per_part), t2 = tile - part * p.tiles_per_part;
             const int mq = fd_div(t2, p.fd_n_tiles), nt = t2 - mq * p.n_tiles;
             const int mt = mq * CG + (int)rank;
-            const int th_i = fd_div(mt, p.fd_tiles_w);
-            const int h0 = th_i * p.TH, w0 = (mt - th_i * p.tiles_w) * p.TW;
+            int img, h0, w0;
+            tile_origin(p, mt, img, h0, w0);
             const int n0 = nt * BN;
             const int nkb = part_kblocks(p, part, num_kb);
     #pragma unroll
@@ -452,7 +476,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                     v[4 * q + 2] = f.z;
                     v[4 * q + 3] = f.w;
                 }
-                epilogue_run(p, v, part, h0 + row_h, w0 + row_w, n0 + ch * 32 + 16 * eh, lane, m_valid);
+                epilogue_run(p, v, part, img, h0 + row_h, w0 + row_w, n0 + ch * 32 + 16 * eh, lane, m_valid);
             }
         }
     }
@@ -485,10 +509,11 @@ static EncodeTiledFn get_encode_fn() {
 // nothing after its first image (six driver calls per conv launch otherwise); graph replay never comes here.
 struct TmapKey {
     const void* base;
-    uint64_t d0, d1, d2;
+    uint64_t d0, d1, d2, d3, s3;
     uint32_t b0, b1, b2;
     bool operator==(const TmapKey& o) const {
-        return base == o.base && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && b0 == o.b0 && b1 == o.b1 && b2 == o.b2;
+        return base == o.base && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && d3 == o.d3 && s3 == o.s3 && b0 == o.b0 &&
+               b1 == o.b1 && b2 == o.b2;
     }
 };
 constexpr int kTmapCacheSlots = 512;
@@ -504,12 +529,14 @@ static TmapCache* tmap_cache() {
 }
 
 static int make_tmap_3d(CUtensorMap* tm, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0,
-                        uint32_t b1, uint32_t b2, uint64_t stride1_bytes = 0, uint64_t stride2_bytes = 0) {
+                        uint32_t b1, uint32_t b2, uint64_t stride1_bytes = 0, uint64_t stride2_bytes = 0, uint64_t d3 = 0,
+                        uint64_t stride3_bytes = 0) {
     // stride1_bytes / stride2_bytes != 0: explicit byte strides of dimensions 1 and 2 (a SLIDING-WINDOW map when stride1 is
     // smaller than the dimension-0 extent: neighbouring "rows" overlap in memory, tests/experiments/tma_overlap_probe.cu); the cache key folds them into d1 / d2's upper bits
-    const TmapKey key{base, d0, d1 | (stride1_bytes << 32), d2 | (stride2_bytes << 32), b0, b1, b2};
+    // d3 > 0: a 4-D map (a batch of d3 images, stride3_bytes apart, box extent 1 along it)
+    const TmapKey key{base, d0, d1 | (stride1_bytes << 32), d2 | (stride2_bytes << 32), d3, stride3_bytes, b0, b1, b2};
     uint64_t hsh = reinterpret_cast<uintptr_t>(base) * 0x9E3779B97F4A7C15ull;
-    hsh ^= (d0 * 31 + d1) * 0xC2B2AE3D27D4EB4Full + d2 * 0x165667B19E3779F9ull + b0 * 131 + b1 * 17 + b2;
+    hsh ^= (d0 * 31 + d1) * 0xC2B2AE3D27D4EB4Full + d2 * 0x165667B19E3779F9ull + b0 * 131 + b1 * 17 + b2 + d3 * 0x27D4EB2Full;
     const int slot = (int)((hsh >> 20) % kTmapCacheSlots);
     TmapCache* cache = tmap_cache();
     if (cache->used[slot] && cache->key[slot] == key) {
@@ -521,13 +548,14 @@ static int make_tmap_3d(CUtensorMap* tm, const void* base, uint64_t d0, uint64_t
         set_error("cuTensorMapEncodeTiled not available from the driver");
         return FRCNN_ERR_CUDA;
     }
-    cuuint64_t dims[3] = {d0, d1, d2};
-    cuuint64_t strides[2] = {stride1_bytes ? stride1_bytes : d0 * 2, stride2_bytes ? stride2_bytes : d0 * d1 * 2};
-    cuuint32_t box[3] = {b0, b1, b2};
-    cuuint32_t estr[3] = {1, 1, 1};
+    cuuint64_t dims[4] = {d0, d1, d2, d3};
+    cuuint64_t strides[3] = {stride1_bytes ? stride1_bytes : d0 * 2, stride2_bytes ? stride2_bytes : d0 * d1 * 2,
+                             stride3_bytes ? stride3_bytes : d0 * d1 * d2 * 2};
+    cuuint32_t box[4] = {b0, b1, b2, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
     CUtensorMapSwizzle sw = (b0 * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B
                                             : (b0 * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, d3 > 0 ? 4 : 3, const_cast<void*>(base), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -592,6 +620,7 @@ static int launch_conv(const CUtensorMap* tm, ConvParams p, cudaStream_t stream)
     p.fd_tiles_w = make_fastdiv(p.tiles_w);
     p.fd_n_tiles = make_fastdiv(p.n_tiles);
     p.fd_tiles_per_part = make_fastdiv(p.tiles_per_part);
+    p.fd_img_tiles = make_fastdiv(p.img_tiles);
     const int bres_kblocks = p.b_res ? p.taps * p.cin_blocks : 0;
     int stage_bytes, fixed;
     conv_smem_layout(BN, BK, X3, bres_kblocks, &stage_bytes, &fixed);
@@ -670,15 +699,19 @@ struct ResExtra {           // residual input of frcnn_conv2d_res
 };
 struct WinExtra {           // frcnn_conv3x3_c8: 3x3 convolution over a compact [H][W+2][8] image through a sliding-window map
     int row_pixels;         // pixels per stored row (W + 2: one zero column on each side)
+    long image_elems;       // elements per image of a batch (frcnn_image_c8_elems)
 };
 }  // namespace
 
+// n_img > 1: a batch of n_img images of the same shape, [n_img][H][W][C] (compact first layer: n_img planes of
+// frcnn_image_c8_elems), every image planned, tiled and computed exactly as a one-image launch would.
 static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin, const void* w_hi,
                        const void* w_lo, const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2,
                        void* y_hi, void* y_lo, float* y_f32, int ld_f32, const int* m_valid, void* stream_,
-                       const GemmExtra* ge, const ResExtra* re = nullptr, const WinExtra* we = nullptr) {
+                       const GemmExtra* ge, const ResExtra* re = nullptr, const WinExtra* we = nullptr, int n_img = 1) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     for (int& v : g_last_plan) v = 0;          // a call that launches nothing leaves an empty record
+    FRCNN_REQUIRE(n_img >= 1 && (n_img == 1 || (!ge && !m_valid && !re)), "frcnn_conv2d: bad batch of %d images", n_img);
     FRCNN_REQUIRE(x_hi && w_hi && (bias || ge), "frcnn_conv2d: x_hi, w_hi and bias are required");
     FRCNN_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "frcnn_conv2d: x_lo and w_lo must both be given (bf16x3) or both NULL");
     FRCNN_REQUIRE(ksize == 1 || ksize == 3, "frcnn_conv2d: ksize must be 1 or 3 (got %d)", ksize);
@@ -770,8 +803,13 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     // CTA pairs (a cluster of 2 sharing each weight tile through TMA multicast) only on request: on an H100 the pair's
     // lockstep over one stage ring made the whole 600x1000 forward 1.9x slower than single CTAs (5.55 vs 2.96 ms / image)
     const int CG = (g_force_cg == 2 && BK == 64 && we == nullptr) ? 2 : 1;
-    FRCNN_REQUIRE(m_tiles * p.n_tiles < (1l << 30), "frcnn_conv2d: too many tiles");
-    p.num_tiles = (int)(cdiv((int)m_tiles, CG) * p.n_tiles);     // tiles (CG = 1) or pair-tiles (CG = 2)
+    FRCNN_REQUIRE(n_img * m_tiles * p.n_tiles < (1l << 30), "frcnn_conv2d: too many tiles");
+    // a batch only multiplies the pixel tiles: the tile shape and N tile above are the one-image plan
+    p.n_img = n_img;
+    p.img_tiles = (int)m_tiles;
+    p.img_pix = (long)H * W;
+    p.img_opix = (long)((H + 1) / 2) * ((W + 1) / 2);
+    p.num_tiles = (int)(cdiv((int)(n_img * m_tiles), CG) * p.n_tiles);     // tiles (CG = 1) or pair-tiles (CG = 2)
     p.tiles_per_part = p.num_tiles;
     p.n_parts = 1; p.splits = 1; p.kb_per_split = p.kb_total = p.taps * p.cin_blocks; p.g_row_stride = 0; p.part_stride = 0;
     if (ge != nullptr) {
@@ -807,11 +845,12 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     CUtensorMap tm[4];
     int rc;
     const uint64_t as1 = we ? 16 : 0, as2 = we ? (uint64_t)we->row_pixels * 16 : 0;     // sliding window: one pixel (8 ch) per step
-    if ((rc = make_tmap_3d(&tm[0], x_hi, Cin, W, H, BK, TW, TH, as1, as2)) != FRCNN_OK) return rc;
+    const uint64_t an = n_img > 1 ? n_img : 0, as3 = (n_img > 1 && we) ? (uint64_t)we->image_elems * 2 : 0;
+    if ((rc = make_tmap_3d(&tm[0], x_hi, Cin, W, H, BK, TW, TH, as1, as2, an, as3)) != FRCNN_OK) return rc;
     const int b_planes = (ge != nullptr && ge->groups == 9) ? 3 : p.taps;
     if ((rc = make_tmap_3d(&tm[2], w_hi, Cin, Cout, b_planes, BK, BN / CG, 1)) != FRCNN_OK) return rc;
     if (x3) {
-        if ((rc = make_tmap_3d(&tm[1], x_lo, Cin, W, H, BK, TW, TH, as1, as2)) != FRCNN_OK) return rc;
+        if ((rc = make_tmap_3d(&tm[1], x_lo, Cin, W, H, BK, TW, TH, as1, as2, an, as3)) != FRCNN_OK) return rc;
         if ((rc = make_tmap_3d(&tm[3], w_lo, Cin, Cout, b_planes, BK, BN / CG, 1)) != FRCNN_OK) return rc;
     } else {
         tm[1] = tm[0];
@@ -871,9 +910,28 @@ extern "C" int frcnn_conv2d_res(const void* x_hi, const void* x_lo, int H, int W
 extern "C" int frcnn_conv3x3_c8(const void* x_hi, const void* x_lo, int H, int W, const void* w_hi, const void* w_lo,
                                 const float* bias, int Cout, int relu, void* y_hi, void* y_lo, void* stream_) {
     FRCNN_ENTRY();
-    WinExtra we{W + 2};
+    WinExtra we{W + 2, 0};
     return conv2d_impl(x_hi, x_lo, H, W, 32, w_hi, w_lo, bias, Cout, 3, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_, nullptr,
                        nullptr, &we);
+}
+
+extern "C" int frcnn_conv2d_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi,
+                                  const void* w_lo, const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2,
+                                  void* y_hi, void* y_lo, float* y_f32, int ld_f32, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1, "frcnn_conv2d_batch: N must be >= 1 (got %d)", N);
+    return conv2d_impl(x_hi, x_lo, H, W, Cin, w_hi, w_lo, bias, Cout, ksize, relu, fuse_pool2x2, y_hi, y_lo, y_f32, ld_f32,
+                       nullptr, stream_, nullptr, nullptr, nullptr, N);
+}
+
+extern "C" int frcnn_conv3x3_c8_batch(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi,
+                                      const void* w_lo, const float* bias, int Cout, int relu, void* y_hi, void* y_lo,
+                                      void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && H > 0 && W > 0, "frcnn_conv3x3_c8_batch: bad shape N=%d H=%d W=%d", N, H, W);
+    WinExtra we{W + 2, (long)frcnn_image_c8_elems(H, W)};
+    return conv2d_impl(x_hi, x_lo, H, W, 32, w_hi, w_lo, bias, Cout, 3, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_, nullptr,
+                       nullptr, &we, N);
 }
 
 extern "C" int frcnn_gemm_nt_splitk_splits(int K, int splits) {

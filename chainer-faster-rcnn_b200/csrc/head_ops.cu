@@ -155,8 +155,12 @@ __global__ void pack_image_im2col_kernel(const float* x, int C, int H, int W, lo
 // zero pixel left and right of every row.  conv1_1 (models/vgg16.py:39) then reads, for output pixel (h, w) and kernel row
 // r, the 32 contiguous values of stored pixels w .. w+3 of row h+r-1 through a SLIDING-WINDOW tensor map (frcnn_conv3x3_c8):
 // 19 MB written here instead of the 77 MB of the [H][W][32] im2col copy, and nothing re-read from HBM four times.
+// A batch: image blockIdx.y reads x + blockIdx.y * sn and writes its own plane, out_elems elements further on.
 __global__ void pack_image_c8_kernel(const float* x, int C, int H, int W, long sc, long sh, long sw, __nv_bfloat16* hi,
-                                     __nv_bfloat16* lo, long slack_pixels) {
+                                     __nv_bfloat16* lo, long slack_pixels, long sn, long out_elems) {
+    x += blockIdx.y * sn;
+    hi += blockIdx.y * out_elems;
+    if (lo) lo += blockIdx.y * out_elems;
     const int WP = W + 2;
     const long total = (long)H * WP + slack_pixels;
     for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < total; p += (long)gridDim.x * blockDim.x) {
@@ -775,7 +779,21 @@ extern "C" int frcnn_pack_image_c8(const float* x, int C, int H, int W, long str
     FRCNN_REQUIRE(stride_c > 0 && stride_h > 0 && stride_w > 0, "frcnn_pack_image_c8: strides must be positive");
     const long total = (long)H * (W + 2) + 8;
     pack_image_c8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x, C, H, W, stride_c, stride_h, stride_w,
-                                                                                (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, 8);
+                                                                                (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, 8, 0, 0);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+extern "C" int frcnn_pack_image_c8_batch(const float* x, int N, int C, int H, int W, long stride_n, long stride_c, long stride_h,
+                                         long stride_w, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(x && y_hi && N >= 1 && N <= 65535 && C > 0 && C <= 3 && H > 0 && W > 0,
+                  "frcnn_pack_image_c8_batch: needs 1 <= N <= 65535 and 1 <= C <= 3 (got N=%d C=%d)", N, C);
+    FRCNN_REQUIRE(stride_n > 0 && stride_c > 0 && stride_h > 0 && stride_w > 0, "frcnn_pack_image_c8_batch: strides must be positive");
+    const long total = (long)H * (W + 2) + 8;
+    const dim3 grid(grid_for(total, 256), N);
+    pack_image_c8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, C, H, W, stride_c, stride_h, stride_w, (__nv_bfloat16*)y_hi,
+                                                                 (__nv_bfloat16*)y_lo, 8, stride_n, (long)frcnn_image_c8_elems(H, W));
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }

@@ -20,16 +20,24 @@ int gemm_nt_splitk_parts(const void* a_hi, const void* a_lo, int M, int K, const
 
 constexpr int kRedC = 64, kRedR = 32, kRedThreads = 256;
 
-// parts [S][Mrows][ld] fp32 (row = output channel, column = RoI)  ->  y[r][c], r < R_cap, c < Cout
+// parts [S][Mrows][ld] fp32 (row = output channel, column = RoI)  ->  y[r][c], r < seg_rows, c < Cout (rows >= R_cap are 0).
+// A batch of images: blockIdx.y = image * rblocks + row block; image i owns parts columns [i*seg_rows, (i+1)*seg_rows), output
+// rows [i*seg_rows, (i+1)*seg_rows) and RoI count m_valid[i * count_stride].  One image: rblocks = gridDim.y, seg_rows = R_cap.
 __global__ void __launch_bounds__(kRedThreads) linear_reduce_kernel(const float* __restrict__ parts, int S, long part_stride, int ld,
                                                                     const float* __restrict__ bias, int Cout, int R_cap,
                                                                     const int* __restrict__ m_valid, int relu,
                                                                     __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo,
-                                                                    float* __restrict__ y_f32, int ld_f32) {
+                                                                    float* __restrict__ y_f32, int ld_f32, int seg_rows, int rblocks,
+                                                                    int count_stride) {
     __shared__ float tile[kRedC][kRedR + 1];
     grid_dep_wait();
-    const int c0 = blockIdx.x * kRedC, r0 = blockIdx.y * kRedR;
-    const int R = m_valid ? min(*m_valid, R_cap) : R_cap;
+    const int img = blockIdx.y / rblocks;
+    const int c0 = blockIdx.x * kRedC, r0 = (blockIdx.y - img * rblocks) * kRedR;
+    parts += (long)img * seg_rows;
+    if (y_hi != nullptr) y_hi += (long)img * seg_rows * Cout;
+    if (y_lo != nullptr) y_lo += (long)img * seg_rows * Cout;
+    if (y_f32 != nullptr) y_f32 += (long)img * seg_rows * ld_f32;
+    const int R = m_valid ? min(m_valid[(long)img * count_stride], R_cap) : R_cap;
     // load phase: thread = (channel row, 4 consecutive RoI columns): one 16-byte load per split (ld % 32 == 0 keeps every row
     // 128-byte aligned), all splits' loads of a thread independent; summed in split order (deterministic)
     {
@@ -75,7 +83,7 @@ __global__ void __launch_bounds__(kRedThreads) linear_reduce_kernel(const float*
 #pragma unroll
         for (int k = 0; k < kRedR / 8; ++k) {
             const int r = r0 + rl + 8 * k;
-            if (r >= R_cap) continue;
+            if (r >= seg_rows) continue;
             const float v0 = tile[cp][rl + 8 * k], v1 = tile[cp + 1][rl + 8 * k];
             if (y_hi != nullptr && c < Cout) {
                 __nv_bfloat16 h0, l0, h1, l1;
@@ -182,6 +190,47 @@ extern "C" int frcnn_linear(const void* x_hi, const void* x_lo, int R_cap, int K
     dim3 grid(cdiv(cols, kRedC), cdiv(R_cap, kRedR));
     FRCNN_CUDA_OK(launch_pdl(linear_reduce_kernel, grid, dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream_),
                              (const float*)parts, S, (long)Cout * lp.ld, lp.ld, bias, Cout, R_cap, m_valid, relu,
-                             (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, y_f32, ld_f32));
+                             (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, y_f32, ld_f32, R_cap, (int)grid.y, 0));
+    return FRCNN_OK;
+}
+
+extern "C" size_t frcnn_linear_batch_workspace_bytes(int N, int R_cap, int K, int Cout) {
+    FRCNN_ENTRY();
+    if (N <= 0 || R_cap <= 0 || K <= 0 || Cout <= 0 || K % 64 != 0) return 0;
+    return align_up((size_t)N * plan_linear(R_cap, K, Cout).parts_bytes, 256);
+}
+
+extern "C" int frcnn_linear_batch(const void* x_hi, const void* x_lo, int N, int R_cap, int K, const void* w_hi, const void* w_lo,
+                                  const float* bias, int Cout, int relu, const int* counts, int count_stride, void* y_hi, void* y_lo,
+                                  float* y_f32, int ld_f32, void* workspace, size_t workspace_bytes, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(x_hi && w_hi && bias && workspace, "frcnn_linear_batch: x_hi, w_hi, bias and workspace are required");
+    FRCNN_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "frcnn_linear_batch: x_lo and w_lo must both be given (bf16x3) or both NULL");
+    FRCNN_REQUIRE(N >= 1 && R_cap > 0 && Cout > 0 && K > 0 && K % 64 == 0,
+                  "frcnn_linear_batch: bad shape N=%d R_cap=%d K=%d Cout=%d (K %% 64 == 0)", N, R_cap, K, Cout);
+    FRCNN_REQUIRE(y_hi || y_f32, "frcnn_linear_batch: no output requested");
+    FRCNN_REQUIRE(!y_lo || y_hi, "frcnn_linear_batch: y_lo without y_hi");
+    FRCNN_REQUIRE(!y_f32 || ld_f32 >= Cout, "frcnn_linear_batch: ld_f32 must be >= Cout");
+    FRCNN_REQUIRE(count_stride >= 0, "frcnn_linear_batch: count_stride must be >= 0");
+    // the one-image plan (N tile, splits, partial-sum promotion): every image's sums are those of frcnn_linear
+    const LinearPlan lp = plan_linear(R_cap, K, Cout);
+    const int rows = N * lp.ld;
+    FRCNN_REQUIRE((long)N * lp.ld < (1l << 30), "frcnn_linear_batch: too many rows");
+    const size_t need = (size_t)N * lp.parts_bytes;
+    if (workspace_bytes < need) {
+        set_error("frcnn_linear_batch: workspace %zu < required %zu", workspace_bytes, need);
+        return FRCNN_ERR_WORKSPACE;
+    }
+    float* parts = static_cast<float*>(workspace);
+    int S = 0;
+    // the N side is all images' segments of lp.ld rows back to back: parts[split][Cout][N * lp.ld]
+    int rc = gemm_nt_splitk_parts(w_hi, w_lo, Cout, K, x_hi, x_lo, rows, lp.splits, lp.bn, lp.nacc, parts, rows, &S, stream_);
+    if (rc != FRCNN_OK) return rc;
+    const int cols = y_f32 ? (ld_f32 > Cout ? ld_f32 : Cout) : Cout;
+    const int rblocks = lp.ld / kRedR;
+    dim3 grid(cdiv(cols, kRedC), N * rblocks);
+    FRCNN_CUDA_OK(launch_pdl(linear_reduce_kernel, grid, dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream_),
+                             (const float*)parts, S, (long)Cout * rows, rows, bias, Cout, R_cap, counts, relu,
+                             (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, y_f32, ld_f32, lp.ld, rblocks, count_stride));
     return FRCNN_OK;
 }

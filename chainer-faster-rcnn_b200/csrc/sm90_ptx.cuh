@@ -103,6 +103,14 @@ __device__ __forceinline__ void tma_load_3d(void* smem, const void* desc, uint64
         "r"(c2)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(void* smem, const void* desc, uint64_t* bar, int c0, int c1, int c2, int c3) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2];"
+        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "r"(c2), "r"(c3)
+        : "memory");
+}
 
 // ----------------------------------------------------------------------------- clusters (CTA pairs)
 __device__ __forceinline__ uint32_t cluster_ctarank() {

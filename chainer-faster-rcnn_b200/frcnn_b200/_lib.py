@@ -37,6 +37,15 @@ SIGNATURES = {
                                 c_void_p]),
     "frcnn_conv2d": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "frcnn_conv2d_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                   c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "frcnn_linear_batch_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "frcnn_linear_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                   c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
+    "frcnn_pack_image_c8_batch": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_long, c_long, c_long, c_long, c_void_p, c_void_p,
+                                          c_void_p]),
+    "frcnn_conv3x3_c8_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p]),
     "frcnn_linear_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "frcnn_linear": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),

@@ -95,6 +95,31 @@ class PackedWeights(object):
         return hi, lo, ops.pad_bias(b, max(n_bias, b.numel()))
 
 
+def _result_layout(post_n, NC):
+    """Every per-image result lives in ONE device block (4-byte words) so that a host caller gets all of it with a single
+    D2H transfer: [count | prob | boxes | rois | scores | keep_count | conf_count | keep_idx].  Returns ({name: (offset,
+    words)}, block words)."""
+    sizes = [("count", 4), ("prob", post_n * NC), ("boxes", post_n * 4 * NC), ("rois", post_n * 4), ("scores", post_n),
+             ("keep_count", NC - 1), ("conf_count", NC - 1), ("keep_idx", (NC - 1) * post_n)]
+    layout, off = {}, 0
+    for name, n_ in sizes:
+        layout[name] = (off, n_)
+        off += (n_ + 3) // 4 * 4
+    return layout, off
+
+
+def _unpack_block(words, L, post_n, NC, with_detect):
+    f = words.view(np.float32)
+    R = int(words[L["count"][0]])
+    sl = lambda a, name: a[L[name][0]: L[name][0] + L[name][1]]          # noqa: E731
+    out = dict(count=R, prob=sl(f, "prob").reshape(post_n, NC)[:R], boxes=sl(f, "boxes").reshape(post_n, 4 * NC)[:R],
+               rois=sl(f, "rois").reshape(post_n, 4)[:R], scores=sl(f, "scores")[:R])
+    if with_detect:
+        out.update(keep_idx=sl(words, "keep_idx").reshape(NC - 1, post_n), keep_count=sl(words, "keep_count"),
+                   conf_count=sl(words, "conf_count"))
+    return out
+
+
 class ForwardPlan(object):
     """Buffers + launch sequence for one image shape."""
 
@@ -129,15 +154,8 @@ class ForwardPlan(object):
         self.fh, self.fw = h, w_
         self.rpn_mid = act(h, w_, weights.rpn3[0].shape[1])
         self.rpn_out = torch.empty((h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
-        # every per-image result lives in ONE device block (4-byte words) so that a host caller gets all of it with a
-        # single D2H transfer: [count | prob | boxes | rois | scores | keep_count | conf_count | keep_idx]
         NC = weights.num_classes
-        sizes = [("count", 4), ("prob", post_n * NC), ("boxes", post_n * 4 * NC), ("rois", post_n * 4), ("scores", post_n),
-                 ("keep_count", NC - 1), ("conf_count", NC - 1), ("keep_idx", (NC - 1) * post_n)]
-        self.result_layout, off = {}, 0
-        for name, n_ in sizes:
-            self.result_layout[name] = (off, n_)
-            off += (n_ + 3) // 4 * 4
+        self.result_layout, off = _result_layout(post_n, NC)
         self.result_words_nodetect = self.result_layout["keep_count"][0]
         self.result = torch.zeros((off,), dtype=torch.int32, device=dev)
         rf = self.result.view(torch.float32)
@@ -293,37 +311,205 @@ class ForwardPlan(object):
 
     def unpack_result(self, words):
         """numpy int32 words of a result block -> dict of views (count int, prob [R,NC], boxes [R,4NC], rois, scores, detect lists)."""
-        L, post_n, NC = self.result_layout, self.post_n, self.w.num_classes
-        f = words.view(np.float32)
-        R = int(words[L["count"][0]])
-        sl = lambda a, name: a[L[name][0]: L[name][0] + L[name][1]]          # noqa: E731
-        out = dict(count=R, prob=sl(f, "prob").reshape(post_n, NC)[:R], boxes=sl(f, "boxes").reshape(post_n, 4 * NC)[:R],
-                   rois=sl(f, "rois").reshape(post_n, 4)[:R], scores=sl(f, "scores")[:R])
-        if self.with_detect:
-            out.update(keep_idx=sl(words, "keep_idx").reshape(NC - 1, post_n), keep_count=sl(words, "keep_count"),
-                       conf_count=sl(words, "conf_count"))
-        return out
+        return _unpack_block(words, self.result_layout, self.post_n, self.w.num_classes, self.with_detect)
 
     def forward(self, x_chw=None):
         """Run one image.  x_chw: (3,H,W) float32 CUDA tensor (copied into the static input) or None
         to reuse the current contents of `self.x_in`.  Returns (prob, boxes, count) device tensors."""
         if x_chw is not None:
             self.x_in.copy_(x_chw, non_blocking=True)
-        if not self.use_graph:
-            self._run()
-        else:
-            if self.graph is None:
-                # one capture at a time in the process (torch's capture stream is shared), and thread-local capture mode so
-                # that other host threads (each running its own plan) may keep calling CUDA meanwhile
-                with _CAPTURE_LOCK:
-                    self._run()                   # warm-up outside capture (func attributes, lazy init)
-                    torch.cuda.current_stream().synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        self._run()
-                    self.graph = g
-            self.graph.replay()
+        _launch(self)
         return self.prob, self.boxes, self.prop.count
+
+
+def _launch(plan):
+    """Runs plan._run(): eagerly, or by replaying its CUDA graph (captured on first use)."""
+    if not plan.use_graph:
+        plan._run()
+        return
+    if plan.graph is None:
+        # one capture at a time in the process (torch's capture stream is shared), and thread-local capture mode so
+        # that other host threads (each running its own plan) may keep calling CUDA meanwhile
+        with _CAPTURE_LOCK:
+            plan._run()                   # warm-up outside capture (func attributes, lazy init)
+            torch.cuda.current_stream().synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                plan._run()
+            plan.graph = g
+    plan.graph.replay()
+
+
+class BatchPlan(object):
+    """Buffers + launch sequence for N images of one shape (VGG16 trunk), all in ONE CUDA graph.
+
+    The trunk, the RPN convolutions and the fc6 / fc7 / head GEMMs each run once over all N images (frcnn_conv2d_batch,
+    frcnn_conv3x3_c8_batch, frcnn_linear_batch: the one-image plan with N times the tiles); ProposalLayer, RoI pooling,
+    the head decode and the per-class NMS run once per image at pointer offsets.  Every image's results are bit-identical
+    to a ForwardPlan's on that image.  The result buffer holds N consecutive blocks in ForwardPlan's layout, so the host
+    gets everything with one D2H.  Takes ForwardPlan's keyword options."""
+
+    def __init__(self, weights, N, H, W, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
+                 anchors=None, with_detect=False, det_nms_thresh=0.3, det_conf=0.8, use_graph=True, keep_rpn_debug=False,
+                 fuse_pool=True, hwc_input=False):
+        if int(N) != N or N < 1:
+            raise FrcnnError("BatchPlan needs N >= 1 images (got %r)" % (N,))
+        if anchors is None:
+            raise FrcnnError("BatchPlan needs the [A,4] float64 anchor table")
+        if "conv1_1" not in weights.convs:
+            raise FrcnnError("BatchPlan runs the VGG16 trunk only")
+        N = int(N)
+        self.w, self.N, self.H, self.W = weights, N, H, W
+        self._ctor = dict(pre_n=pre_n, post_n=post_n, nms_thresh=nms_thresh, min_size=min_size, feat_stride=feat_stride,
+                          anchors=anchors, with_detect=with_detect, det_nms_thresh=det_nms_thresh, det_conf=det_conf,
+                          use_graph=use_graph, keep_rpn_debug=keep_rpn_debug, fuse_pool=fuse_pool, hwc_input=hwc_input)
+        self.hwc_input = bool(hwc_input)       # x_in holds the bytes of dense (N,H,W,3) images
+        self.pre_n, self.post_n, self.nms_thresh, self.min_size, self.feat_stride = pre_n, post_n, nms_thresh, min_size, feat_stride
+        self.with_detect, self.det_nms_thresh, self.det_conf = with_detect, det_nms_thresh, det_conf
+        dev = weights.device
+        x3 = weights.precision == "bf16x3"
+        A, NC = weights.n_anchors, weights.num_classes
+        self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
+
+        def act(*shape, zero=False):
+            hi = (torch.zeros if zero else torch.empty)(shape, dtype=torch.bfloat16, device=dev)
+            return ops.Act(hi, torch.zeros_like(hi) if (x3 and zero) else (torch.empty_like(hi) if x3 else None))
+
+        self.x_in = torch.zeros((N, 3, H, W), dtype=torch.float32, device=dev)
+        self.acts = [act(N, ops._lib.load().frcnn_image_c8_elems(H, W))]
+        h, w_ = H, W
+        self.trunk_steps = []          # as ForwardPlan._alloc_trunk
+        for i, item in enumerate(VGG16_LAYERS):
+            if item == "pool":
+                continue
+            pooled = i + 1 < len(VGG16_LAYERS) and VGG16_LAYERS[i + 1] == "pool"
+            fuse = fuse_pool and pooled
+            if fuse:
+                h, w_ = (h + 1) // 2, (w_ + 1) // 2
+            self.acts.append(act(N, h, w_, item[2]))
+            self.trunk_steps.append((item[0], fuse, pooled and not fuse))
+            if pooled and not fuse:
+                h, w_ = (h + 1) // 2, (w_ + 1) // 2
+                self.acts.append(act(N, h, w_, item[2]))
+        self.fh, self.fw = h, w_
+        self.rpn_mid = act(N, h, w_, weights.rpn3[0].shape[1])
+        self.rpn_out = torch.empty((N * h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
+        self.result_layout, self.block_words = _result_layout(post_n, NC)
+        self.result_words_nodetect = self.result_layout["keep_count"][0]
+        self.result = torch.zeros((N * self.block_words,), dtype=torch.int32, device=dev)
+        # the RoI counts for frcnn_linear_batch: word `count` of every block, block_words apart
+        self.counts = self.result[self.result_layout["count"][0]:]
+        # head activations: one segment of ld1 rows per image; rows [post_n, ld1) of pool5 stay zero
+        self.ld1 = ops.round_up(post_n, 32)
+        C = self.acts[-1].hi.shape[-1]
+        self.pool5 = act(N, self.ld1, 49 * C, zero=True)
+        self.fc6 = act(N, self.ld1, 4096)
+        self.fc7 = act(N, self.ld1, 4096)
+        self.head_out = torch.empty((N, self.ld1, weights.head_ld), dtype=torch.float32, device=dev)
+        self.fc_work = max((ops.linear_batch_workspace(N, post_n, k_, c_, dev) for k_, c_ in
+                            ((49 * C, 4096), (4096, 4096), (4096, 5 * NC))), key=lambda t: t.numel())
+        self.images = []
+        for n in range(N):
+            blk = self.result[n * self.block_words:(n + 1) * self.block_words]
+            rf = blk.view(torch.float32)
+            seg = lambda t, name: t[self.result_layout[name][0]: self.result_layout[name][0] + self.result_layout[name][1]]   # noqa: E731
+            prop = ops.ProposalWorkspace(A, h, w_, pre_n, post_n, dev, debug=keep_rpn_debug,
+                                         outputs=(seg(rf, "rois").view(post_n, 4), seg(rf, "scores"), seg(blk, "count")[:1]))
+            self.images.append(dict(prop=prop, prob=seg(rf, "prob").view(post_n, NC), boxes=seg(rf, "boxes").view(post_n, 4 * NC),
+                                    det=(seg(blk, "keep_idx").view(NC - 1, post_n), seg(blk, "keep_count"), seg(blk, "conf_count"))))
+        self._host = None
+        self.graph = None
+        self.use_graph = use_graph
+        self.im_h, self.im_w = H, W
+        self.n_launches = 0
+
+    @staticmethod
+    def _image(a, n):
+        return ops.Act(a.hi[n], None if a.lo is None else a.lo[n])
+
+    def _run(self):
+        w, N, post_n = self.w, self.N, self.post_n
+        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input)
+        n = 1
+        i = 0
+        for name, fused, pool_after in self.trunk_steps:
+            hi, lo, b = w.convs[name]
+            if i == 0:
+                ops.conv3x3_c8_batch(self.acts[0], N, self.H, self.W, hi, lo, b, True, out=self.acts[1])
+            else:
+                ops.conv2d_batch(self.acts[i], hi, lo, b, 3, True, out=self.acts[i + 1], fuse_pool=fused)
+            n += 1
+            i += 1
+            if pool_after:
+                for k in range(N):
+                    ops.maxpool2x2_ceil(self._image(self.acts[i], k), out=self._image(self.acts[i + 1], k))
+                n += N
+                i += 1
+        feat = self.feat = self.acts[-1]
+        hi, lo, b = w.rpn3
+        ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid)
+        hi, lo, b = w.rpn_heads
+        ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out)
+        n += 2
+        hw = self.fh * self.fw
+        for k, im in enumerate(self.images):
+            ops.proposals(self.rpn_out[k * hw:(k + 1) * hw], None, self.anchors, w.n_anchors, self.fh, self.fw, self.feat_stride,
+                          self.im_h, self.im_w, self.min_size, self.pre_n, post_n, self.nms_thresh,
+                          layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=im["prop"], debug=im["prop"].dbg_dets is not None)
+            p5 = self.pool5
+            ops.roi_pool(self._image(feat, k), im["prop"].rois, im["prop"].count, 7, 7, 1.0 / self.feat_stride,
+                         out=ops.Act(p5.hi[k, :post_n], None if p5.lo is None else p5.lo[k, :post_n]))
+            n += 5 + 1
+        cnt, bw = self.counts, self.block_words
+        hi, lo, b = w.fc6
+        ops.linear_batch(self.pool5, hi, lo, b, True, post_n, counts=cnt, count_stride=bw, out=self.fc6, work=self.fc_work)
+        hi, lo, b = w.fc7
+        ops.linear_batch(self.fc6, hi, lo, b, True, post_n, counts=cnt, count_stride=bw, out=self.fc7, work=self.fc_work)
+        hi, lo, b = w.head
+        ops.linear_batch(self.fc7, hi, lo, b, False, post_n, counts=cnt, count_stride=bw, out_f32=self.head_out,
+                         ld_f32=w.head_ld, work=self.fc_work, want_act=False)
+        n += 3 * 2
+        for k, im in enumerate(self.images):
+            ops.head_decode(self.head_out[k, :post_n], w.head_ld, im["prop"].rois, im["prop"].count, w.num_classes,
+                            self.im_h, self.im_w, out_prob=im["prob"], out_boxes=im["boxes"])
+            n += 5
+            if self.with_detect:
+                ops.detect(im["prob"], im["boxes"], im["prop"].count, self.det_nms_thresh, self.det_conf, out=im["det"])
+                n += 1
+        self.n_launches = n
+
+    def clone(self):
+        """A second set of buffers (and its own graph) over the SAME packed weights: lets another batch be in flight."""
+        p = type(self)(self.w, self.N, self.H, self.W, **self._ctor)
+        p.set_clip(self.im_h, self.im_w)
+        return p
+
+    set_clip = ForwardPlan.set_clip
+    host_io = ForwardPlan.host_io
+    forward_host = ForwardPlan.forward_host       # x_np: float32 (N,3,H,W); returns unpack_result's list
+
+    def result_words(self):
+        """Words of the result buffer a host caller needs: every block, the last one without the NMS lists when they are off."""
+        last = self.block_words if self.with_detect else self.result_words_nodetect
+        return (self.N - 1) * self.block_words + last
+
+    def unpack_result(self, words):
+        """numpy int32 words of the result buffer -> list of N dicts as ForwardPlan.unpack_result returns them."""
+        bw = self.block_words
+        return [_unpack_block(words[k * bw:(k + 1) * bw], self.result_layout, self.post_n, self.w.num_classes, self.with_detect)
+                for k in range(self.N)]
+
+    def forward(self, x_nchw=None):
+        """Run the batch.  x_nchw: (N,3,H,W) float32 CUDA tensor (copied into the static input) or None to reuse the
+        current contents of `self.x_in`.  Returns (list of prob [post_n,NC], list of boxes [post_n,4NC], counts [N] int32
+        device view); rows past an image's count are zero."""
+        if x_nchw is not None:
+            if tuple(x_nchw.shape) != tuple(self.x_in.shape):
+                raise FrcnnError("BatchPlan: input of shape %s, the plan is for %s" % (tuple(x_nchw.shape), tuple(self.x_in.shape)))
+            self.x_in.copy_(x_nchw, non_blocking=True)
+        _launch(self)
+        counts = self.result.view(self.N, self.block_words)[:, self.result_layout["count"][0]]
+        return [im["prob"] for im in self.images], [im["boxes"] for im in self.images], counts
 
 
 class LanePool(object):
@@ -549,6 +735,28 @@ class Engine(object):
         prob, boxes, count = p.forward(x_chw)
         R = int(count.item())           # the one documented D2H sync (SURVEY.md Q11)
         return prob[:R], boxes[:R], p
+
+    def batch_plan(self, N, H, W, **overrides):
+        """The BatchPlan for N images of H x W (cached per shape and options)."""
+        kw = dict(self.plan_kwargs)
+        kw.update(overrides)
+        key = ("batch", N, H, W, tuple(sorted(kw.items())))
+        if key not in self.plans:
+            self.plans[key] = BatchPlan(self.weights, N, H, W, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
+        return self.plans[key]
+
+    def forward_batch(self, x_nchw, img_info=None, **overrides):
+        """N same-size images (N,3,H,W) float32 CUDA -> list of per-image (prob [R_n,NC], boxes [R_n,4NC]) device tensors,
+        after one sync for the N counts."""
+        if x_nchw.dim() != 4 or x_nchw.shape[1] != 3:
+            raise FrcnnError("forward_batch: expected (N,3,H,W) images, got %s" % (tuple(x_nchw.shape),))
+        N, _, H, W = x_nchw.shape
+        p = self.batch_plan(N, H, W, **overrides)
+        if img_info is not None:
+            p.set_clip(int(img_info[0]), int(img_info[1]))
+        probs, boxes, counts = p.forward(x_nchw)
+        R = counts.cpu().tolist()
+        return [(pr[:r], bx[:r]) for pr, bx, r in zip(probs, boxes, R)]
 
 
 class CForward(object):

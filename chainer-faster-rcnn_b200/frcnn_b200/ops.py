@@ -218,6 +218,104 @@ def linear(x, w_hi, w_lo, bias, relu, m_valid=None, out=None, out_f32=None, ld_f
     return y, y32
 
 
+def pack_image_c8_batch(x_nchw, precision="bf16x3", out=None, hwc_memory=False):
+    """(N,C<=3,H,W) float32 CUDA images -> Act of planes [N, frcnn_image_c8_elems(H,W)]: pack_image_c8 of every image.
+    hwc_memory: the buffer's BYTES are dense (N,H,W,C) images."""
+    _need_cuda(x_nchw)
+    x = x_nchw.contiguous().float()
+    N, C, H, W = x.shape
+    lib = _lib.load()
+    n = lib.frcnn_image_c8_elems(H, W)
+    if out is None:
+        hi = torch.empty((N, n), dtype=torch.bfloat16, device=x.device)
+        out = Act(hi, torch.empty_like(hi) if precision == "bf16x3" else None)
+    if out.hi.numel() < N * n:
+        raise FrcnnError("pack_image_c8_batch: output holds %d elements, needs %d" % (out.hi.numel(), N * n))
+    sc, sh, sw = (1, W * C, C) if hwc_memory else (H * W, W, 1)
+    check(lib.frcnn_pack_image_c8_batch(_p(x), N, C, H, W, C * H * W, sc, sh, sw, _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_pack_image_c8_batch")
+    return out
+
+
+def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None):
+    """frcnn_conv3x3_c8_batch: conv1_1 over N compact images (pack_image_c8_batch) -> Act [N,H,W,Cout]."""
+    taps, Cout, k = w_hi.shape
+    if (taps, k) != (3, 32):
+        raise FrcnnError("conv3x3_c8_batch: weights must be [3, Cout, 32] (pack_conv_weights_c8)")
+    if (x_c8.lo is None) != (w_lo is None):
+        raise FrcnnError("conv3x3_c8_batch: activation and weight precision modes differ")
+    if x_c8.hi.numel() < N * _lib.load().frcnn_image_c8_elems(H, W):
+        raise FrcnnError("conv3x3_c8_batch: input holds fewer than %d compact images of %dx%d" % (N, H, W))
+    if out is None:
+        yh = torch.empty((N, H, W, Cout), dtype=torch.bfloat16, device=x_c8.hi.device)
+        out = Act(yh, torch.empty_like(yh) if x_c8.lo is not None else None)
+    check(_lib.load().frcnn_conv3x3_c8_batch(_p(x_c8.hi), _p(x_c8.lo), N, H, W, _p(w_hi), _p(w_lo), _p(bias), Cout,
+                                             1 if relu else 0, _p(out.hi), _p(out.lo), _stream()), "frcnn_conv3x3_c8_batch")
+    return out
+
+
+def conv2d_batch(x, w_hi, w_lo, bias, ksize, relu, out_act=True, ld_f32=0, out=None, out_f32=None, fuse_pool=False):
+    """frcnn_conv2d_batch: x Act [N,H,W,Cin]; returns (Act [N,H,W,Cout] (pooled: [N,ceil(H/2),ceil(W/2),Cout]) or None,
+    fp32 [N*H*W, ld_f32] or None).  Each image's output equals conv2d on that image, bit for bit."""
+    N, H, W, Cin = x.hi.shape
+    taps, Cout, cin_w = w_hi.shape
+    if cin_w != Cin or taps != ksize * ksize:
+        raise FrcnnError("conv2d_batch: weight shape %s does not match input channels %d / ksize %d" % (tuple(w_hi.shape), Cin, ksize))
+    if (x.lo is None) != (w_lo is None):
+        raise FrcnnError("conv2d_batch: activation and weight precision modes differ")
+    y = out
+    if out_act and y is None:
+        oh, ow = ((H + 1) // 2, (W + 1) // 2) if fuse_pool else (H, W)
+        yh = torch.empty((N, oh, ow, Cout), dtype=torch.bfloat16, device=x.hi.device)
+        y = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    y32 = out_f32
+    if ld_f32 and y32 is None:
+        y32 = torch.empty((N * H * W, ld_f32), dtype=torch.float32, device=x.hi.device)
+    need = round_up(max(Cout, ld_f32), 32)
+    if bias.numel() < need:
+        raise FrcnnError("conv2d_batch: bias has %d entries, needs %d (use pad_bias)" % (bias.numel(), need))
+    check(_lib.load().frcnn_conv2d_batch(_p(x.hi), _p(x.lo), N, H, W, Cin, _p(w_hi), _p(w_lo), _p(bias), Cout, ksize,
+                                         1 if relu else 0, 1 if fuse_pool else 0, _p(y.hi) if y else None,
+                                         _p(y.lo) if y else None, _p(y32), ld_f32, _stream()), "frcnn_conv2d_batch")
+    return y, y32
+
+
+def linear_batch_workspace(N, R_cap, K, Cout, device):
+    n = _lib.load().frcnn_linear_batch_workspace_bytes(int(N), int(R_cap), int(K), int(Cout))
+    if n == 0:
+        raise FrcnnError("frcnn_linear_batch_workspace_bytes: bad shape N=%d R_cap=%d K=%d Cout=%d" % (N, R_cap, K, Cout))
+    return torch.empty((n,), dtype=torch.uint8, device=device)
+
+
+def linear_batch(x, w_hi, w_lo, bias, relu, R_cap, counts=None, count_stride=1, out=None, out_f32=None, ld_f32=0, work=None,
+                 want_act=True):
+    """frcnn_linear_batch: x Act [N, ld1, K] with ld1 = round_up(R_cap, 32) rows per image; counts: device int32 holding image
+    n's RoI count at counts[n * count_stride] (None: R_cap each).  Returns (Act [N, ld1, Cout] or None, fp32 [N, ld1, ld_f32] or
+    None); each image's rows equal linear on that image, bit for bit, and rows past its count are zero."""
+    N, ld1, K = x.hi.shape
+    taps, Cout, kw = w_hi.shape
+    if taps != 1 or kw != K:
+        raise FrcnnError("linear_batch: weight shape %s does not match K = %d" % (tuple(w_hi.shape), K))
+    if ld1 != round_up(R_cap, 32):
+        raise FrcnnError("linear_batch: %d rows per image, expected round_up(R_cap=%d, 32)" % (ld1, R_cap))
+    if (x.lo is None) != (w_lo is None):
+        raise FrcnnError("linear_batch: activation and weight precision modes differ")
+    dev = x.hi.device
+    y = out
+    if want_act and y is None:
+        yh = torch.empty((N, ld1, Cout), dtype=torch.bfloat16, device=dev)
+        y = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    y32 = out_f32
+    if ld_f32 and y32 is None:
+        y32 = torch.empty((N, ld1, ld_f32), dtype=torch.float32, device=dev)
+    if work is None:
+        work = linear_batch_workspace(N, R_cap, K, Cout, dev)
+    check(_lib.load().frcnn_linear_batch(_p(x.hi), _p(x.lo), N, R_cap, K, _p(w_hi), _p(w_lo), _p(bias), Cout, 1 if relu else 0,
+                                         _p(counts), int(count_stride), _p(y.hi) if y else None, _p(y.lo) if y else None,
+                                         _p(y32), int(ld_f32), _p(work), work.numel(), _stream()), "frcnn_linear_batch")
+    return y, y32
+
+
 def conv2d_res(x, w_hi, w_lo, bias, ksize, relu, res, out=None):
     """frcnn_conv2d_res: y = act(conv(x) + bias + res); res an Act of the output shape (ResNet shortcut add)."""
     H, W, Cin = x.hi.shape

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import ops
+from ._lib import FrcnnError
 from .engine import Engine, ForwardPlan, PackedWeights, _t
 
 RESNET_BLOCKS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
@@ -143,6 +144,9 @@ class ResNetEngine(Engine):
         if key not in self.plans:
             self.plans[key] = ResNetForwardPlan(self.weights, H, W, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
         return self.plans[key]
+
+    def batch_plan(self, N, H, W, **overrides):
+        raise FrcnnError("ResNetEngine runs one image at a time: batches (BatchPlan) need the VGG16 trunk")
 
 
 class TrunkOnly(object):

@@ -123,6 +123,13 @@ int frcnn_proposals(const float* cls, long cls_chan_stride, long cls_pix_stride,
 int frcnn_conv2d(const void* x_hi, const void* x_lo, int H, int W, int Cin, const void* w_hi, const void* w_lo,
                  const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2, void* y_hi, void* y_lo, float* y_f32,
                  int ld_f32, const int* m_valid, void* stream);
+/* frcnn_conv2d over a batch of N >= 1 images of one shape in one launch: x [N,H,W,Cin], y [N,H,W,Cout] (pooled:
+ * [N,ceil(H/2),ceil(W/2),Cout]), y_f32 [N*H*W, ld_f32].  The input is read through a 4-D tensor map, so each image is
+ * zero-padded on its own; the tile shape and N tile are the one-image plan, so every image's output is bit-identical to
+ * frcnn_conv2d on that image.  No m_valid. */
+int frcnn_conv2d_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi, const void* w_lo,
+                       const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2, void* y_hi, void* y_lo, float* y_f32,
+                       int ld_f32, void* stream);
 /* Tuning override for tests / benchmarks: force the N tile (64/128/256) and the pixel tile
  * (tile_h*tile_w == 128); 0 = automatic. Process-wide. */
 void frcnn_conv2d_set_tile(int block_n, int tile_h, int tile_w);
@@ -162,8 +169,9 @@ void frcnn_conv2d_set_max_ctas(int max_ctas);
  * Read at launch time (fixed inside a captured graph). */
 void frcnn_conv2d_set_smem_reserve(int bytes);
 /* The plan of the calling thread's last frcnn_conv2d / frcnn_conv2d_res / frcnn_conv3x3_c8 / frcnn_gemm_nt_splitk /
- * frcnn_linear GEMM launch: copies min(n, 12) ints to out in the order BN, BK, x3, promote (long-K partial sums), CTA
- * group, tile_h, tile_w, pipeline stages, grid (CTAs), tiles (pair-tiles for CTA pairs, all split-K parts included),
+ * frcnn_linear GEMM launch (or their _batch forms): copies min(n, 12) ints to out in the order BN, BK, x3, promote (long-K
+ * partial sums), CTA group, tile_h, tile_w, pipeline stages, grid (CTAs), tiles (pair-tiles for CTA pairs, all split-K
+ * parts and all images of a batch included),
  * split-K parts, splits; all zero when the last call launched nothing.  Returns the number of fields (12). */
 int frcnn_conv2d_last_plan(int* out, int n);
 
@@ -200,6 +208,13 @@ int frcnn_pack_image_c8(const float* x, int C, int H, int W, long stride_c, long
 int frcnn_pack_conv_weights_c8(const float* w_oihw, int Cout, int Cin, void* w_hi, void* w_lo, void* stream);
 int frcnn_conv3x3_c8(const void* x_hi, const void* x_lo, int H, int W, const void* w_hi, const void* w_lo, const float* bias,
                      int Cout, int relu, void* y_hi, void* y_lo, void* stream);
+/* The same for a batch of N images of one shape: image n's source is x + n*stride_n, its compact planes start
+ * n * frcnn_image_c8_elems(H, W) elements into y_hi / y_lo, and frcnn_conv3x3_c8_batch writes y [N,H,W,Cout], each image
+ * bit-identical to frcnn_conv3x3_c8 on it. */
+int frcnn_pack_image_c8_batch(const float* x, int N, int C, int H, int W, long stride_n, long stride_c, long stride_h,
+                              long stride_w, void* y_hi, void* y_lo, void* stream);
+int frcnn_conv3x3_c8_batch(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo,
+                           const float* bias, int Cout, int relu, void* y_hi, void* y_lo, void* stream);
 
 /* Same with an explicit source layout: element (c, h, w) is x[c*stride_c + h*stride_h + w*stride_w] (in floats).
  * (H*W, W, 1) = dense (C,H,W); (1, W*C, C) = dense (H,W,C) memory, which is what forward.py:45's
@@ -234,6 +249,15 @@ size_t frcnn_linear_workspace_bytes(int R_cap, int K, int Cout);
 int frcnn_linear(const void* x_hi, const void* x_lo, int R_cap, int K, const void* w_hi, const void* w_lo,
                  const float* bias, int Cout, int relu, const int* m_valid, void* y_hi, void* y_lo, float* y_f32,
                  int ld_f32, void* workspace, size_t workspace_bytes, void* stream);
+/* frcnn_linear over the RoIs of N images in one GEMM.  Every image owns a segment of ld1 = round_up(R_cap, 32) rows:
+ * x [N][ld1][K] (rows past R_cap should be zero; they only reach their own, discarded, output rows), y_hi/y_lo
+ * [N][ld1][Cout] and y_f32 [N][ld1][ld_f32], rows >= image n's count written as 0.  counts (optional, device): image n
+ * has min(counts[n * count_stride], R_cap) RoIs.  The N tile, split count and partial-sum promotion are those
+ * frcnn_linear picks for one image, so each image's rows are bit-identical to frcnn_linear on that image. */
+size_t frcnn_linear_batch_workspace_bytes(int N, int R_cap, int K, int Cout);
+int frcnn_linear_batch(const void* x_hi, const void* x_lo, int N, int R_cap, int K, const void* w_hi, const void* w_lo,
+                       const float* bias, int Cout, int relu, const int* counts, int count_stride, void* y_hi, void* y_lo,
+                       float* y_f32, int ld_f32, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Head tail (models/faster_rcnn.py:175-178): softmax over num_classes scores + per-class
  * bbox_transform_inv + clip_boxes.  scores element (r,c) at scores[r*ld + c], deltas (r,j) at
