@@ -1,10 +1,12 @@
-// forward_graph.cu -- frcnn_forward_vgg16: the whole forward detection path behind ONE C-ABI call.
+// forward_graph.cu -- frcnn_forward_vgg16(_batch): the whole forward detection path of one image, or of N same-size images,
+// behind ONE C-ABI call.
 //
 // FasterRCNN.__call__, inference branch (/root/reference models/faster_rcnn.py:92-134,175-178): trunk (models/vgg16.py:38-82)
 // -> RPN (models/region_proposal_network.py:117-124) -> ProposalLayer (models/proposal_layer.py:102-198) -> RoI pooling ->
 // fc6 / fc7 -> cls_score | bbox_pred -> softmax + decode + clip.  This is pure host orchestration: it carves the caller's
-// workspace and enqueues the same kernels, in the same order, as frcnn_b200/engine.py -- for callers that have no Python
-// (the launch sequence is static, so the caller may capture it into a CUDA graph).  No allocation, no synchronisation.
+// workspace and enqueues the same kernels, in the same order, as frcnn_b200/engine.py's BatchPlan -- for callers that have no
+// Python (the launch sequence is static, so the caller may capture it into a CUDA graph).  No allocation, no synchronisation.
+// One image is the batch of N = 1; every stage is one launch for all N images.
 #include "common.cuh"
 
 using namespace frcnn;
@@ -39,37 +41,41 @@ struct Layout {
     float *rpn_out, *head_out, *rois, *scores;
     void *prop_ws, *fc_ws;
     size_t prop_ws_bytes, fc_ws_bytes;
-    int fh, fw, rpn_ld, head_ld;
+    int fh, fw, rpn_ld, head_ld, ld1;
     size_t total;
 };
 
 int round32(int v) { return (v + 31) / 32 * 32; }
 
-Layout carve(const frcnn_forward_config& c, void* workspace) {
+// The workspace of N images: every activation is [N][...] (image n's block right after image n-1's), the head
+// activations hold ld1 = round_up(post_nms_top_n, 32) rows per image (frcnn_linear_batch's segments).
+Layout carve(const frcnn_forward_config& c, int N, void* workspace) {
     Layout L;
     Carver k{(char*)workspace, 0, c.x3 != 0};
-    L.x_col = k.act((long)frcnn_image_c8_elems(c.H, c.W));          // compact first-layer input [H][W+2][8]
+    L.x_col = k.act((long)N * frcnn_image_c8_elems(c.H, c.W));    // compact first-layer input [N][H][W+2][8]
     int h = c.H, w = c.W;
     for (int i = 0; i < 13; ++i) {
         if (kVgg[i][2]) { h = (h + 1) / 2; w = (w + 1) / 2; }          // the pool is fused into this conv's epilogue
-        L.act[i] = k.act((long)h * w * kVgg[i][1]);
+        L.act[i] = k.act((long)N * h * w * kVgg[i][1]);
     }
     L.fh = h; L.fw = w;
     L.rpn_ld = round32(6 * c.n_anchors);
     L.head_ld = round32(5 * c.num_classes);
-    L.rpn_mid = k.act((long)h * w * 512);
-    L.rpn_out = (float*)k.take((size_t)h * w * L.rpn_ld * 4);
-    L.prop_ws_bytes = frcnn_proposals_workspace_bytes(c.n_anchors, h, w, c.pre_nms_top_n);
+    L.ld1 = round32(c.post_nms_top_n);
+    const long rows = (long)N * L.ld1;
+    L.rpn_mid = k.act((long)N * h * w * 512);
+    L.rpn_out = (float*)k.take((size_t)N * h * w * L.rpn_ld * 4);
+    L.prop_ws_bytes = frcnn_proposals_batch_workspace_bytes(N, c.n_anchors, h, w, c.pre_nms_top_n);
     L.prop_ws = k.take(L.prop_ws_bytes);
-    L.rois = (float*)k.take((size_t)c.post_nms_top_n * 4 * 4);
-    L.scores = (float*)k.take((size_t)c.post_nms_top_n * 4);
-    L.pool5 = k.act((long)c.post_nms_top_n * 49 * 512);
-    L.fc6 = k.act((long)c.post_nms_top_n * 4096);
-    L.fc7 = k.act((long)c.post_nms_top_n * 4096);
-    L.head_out = (float*)k.take((size_t)c.post_nms_top_n * L.head_ld * 4);
-    L.fc_ws_bytes = frcnn_linear_workspace_bytes(c.post_nms_top_n, 49 * 512, 4096);
-    const size_t b7 = frcnn_linear_workspace_bytes(c.post_nms_top_n, 4096, 4096);
-    const size_t bh = frcnn_linear_workspace_bytes(c.post_nms_top_n, 4096, 5 * c.num_classes);
+    L.rois = (float*)k.take((size_t)N * c.post_nms_top_n * 4 * 4);
+    L.scores = (float*)k.take((size_t)N * c.post_nms_top_n * 4);
+    L.pool5 = k.act(rows * 49 * 512);
+    L.fc6 = k.act(rows * 4096);
+    L.fc7 = k.act(rows * 4096);
+    L.head_out = (float*)k.take((size_t)rows * L.head_ld * 4);
+    L.fc_ws_bytes = frcnn_linear_batch_workspace_bytes(N, c.post_nms_top_n, 49 * 512, 4096);
+    const size_t b7 = frcnn_linear_batch_workspace_bytes(N, c.post_nms_top_n, 4096, 4096);
+    const size_t bh = frcnn_linear_batch_workspace_bytes(N, c.post_nms_top_n, 4096, 5 * c.num_classes);
     if (b7 > L.fc_ws_bytes) L.fc_ws_bytes = b7;
     if (bh > L.fc_ws_bytes) L.fc_ws_bytes = bh;
     L.fc_ws = k.take(L.fc_ws_bytes);
@@ -85,25 +91,21 @@ int check_config(const frcnn_forward_config* c) {
     return FRCNN_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t frcnn_forward_workspace_bytes(const frcnn_forward_config* config) {
-    FRCNN_ENTRY();
-    if (check_config(config) != FRCNN_OK) return 0;
-    return carve(*config, nullptr).total;
+int check_batch(int N) {
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "frcnn_forward: N must be in [1,65535] (got %d)", N);
+    return FRCNN_OK;
 }
 
-int frcnn_forward_vgg16(const frcnn_forward_config* config, const frcnn_vgg16_weights* wts, const float* image_chw, int im_h,
-                        int im_w, void* workspace, size_t workspace_bytes, float* out_prob, float* out_boxes, int* out_count,
-                        void* stream) {
-    FRCNN_ENTRY();
+// The forward path over N images of one shape: every stage is one launch sequence for the whole batch.
+int forward_n(const frcnn_forward_config* config, const frcnn_vgg16_weights* wts, int N, const float* images_nchw, int im_h,
+              int im_w, void* workspace, size_t workspace_bytes, float* out_prob, float* out_boxes, int* out_count,
+              cudaStream_t stream) {
     int rc = check_config(config);
     if (rc != FRCNN_OK) return rc;
+    if ((rc = check_batch(N)) != FRCNN_OK) return rc;
     const frcnn_forward_config& c = *config;
-    FRCNN_REQUIRE(wts && image_chw && workspace && out_prob && out_boxes && out_count, "frcnn_forward: null pointer");
-    const Layout L = carve(c, workspace);
+    FRCNN_REQUIRE(wts && images_nchw && workspace && out_prob && out_boxes && out_count, "frcnn_forward: null pointer");
+    const Layout L = carve(c, N, workspace);
     if (workspace_bytes < L.total) {
         set_error("frcnn_forward: workspace %zu < %zu bytes", workspace_bytes, L.total);
         return FRCNN_ERR_WORKSPACE;
@@ -111,43 +113,79 @@ int frcnn_forward_vgg16(const frcnn_forward_config* config, const frcnn_vgg16_we
     const bool x3 = c.x3 != 0;
     for (int i = 0; i < 13; ++i)
         FRCNN_REQUIRE(wts->conv[i].hi && wts->conv[i].bias && (!x3 || wts->conv[i].lo), "frcnn_forward: trunk layer %d weights missing", i);
-    // ---- trunk: conv1_1 as a K = 3 x 32 GEMM over the compact image (sliding-window tensor map), then 12 shared-halo 3x3 convs
-    if ((rc = frcnn_pack_image_c8(image_chw, 3, c.H, c.W, (long)c.H * c.W, c.W, 1, L.x_col.hi, L.x_col.lo, stream)) != FRCNN_OK) return rc;
+    // ---- trunk: conv1_1 as a K = 3 x 32 GEMM over the compact images (sliding-window tensor map), then 12 shared-halo 3x3 convs
+    const long hw = (long)c.H * c.W;
+    if ((rc = frcnn_pack_image_c8_batch(images_nchw, N, 3, c.H, c.W, 3 * hw, hw, c.W, 1, L.x_col.hi, L.x_col.lo, stream)) != FRCNN_OK)
+        return rc;
     Plane x = L.x_col;
     int h = c.H, w = c.W, cin = 32;
     for (int i = 0; i < 13; ++i) {
         const frcnn_packed_layer& l = wts->conv[i];
         if (i == 0)
-            rc = frcnn_conv3x3_c8(x.hi, x.lo, h, w, l.hi, l.lo, l.bias, kVgg[0][1], 1, L.act[0].hi, L.act[0].lo, stream);
+            rc = frcnn_conv3x3_c8_batch(x.hi, x.lo, N, h, w, l.hi, l.lo, l.bias, kVgg[0][1], 1, L.act[0].hi, L.act[0].lo, stream);
         else
-            rc = frcnn_conv2d(x.hi, x.lo, h, w, cin, l.hi, l.lo, l.bias, kVgg[i][1], 3, 1, kVgg[i][2], L.act[i].hi, L.act[i].lo, nullptr,
-                              0, nullptr, stream);
+            rc = frcnn_conv2d_batch(x.hi, x.lo, N, h, w, cin, l.hi, l.lo, l.bias, kVgg[i][1], 3, 1, kVgg[i][2], L.act[i].hi, L.act[i].lo,
+                                    nullptr, 0, stream);
         if (rc != FRCNN_OK) return rc;
         if (kVgg[i][2]) { h = (h + 1) / 2; w = (w + 1) / 2; }
         x = L.act[i];
         cin = kVgg[i][1];
     }
     const Plane feat = x;
-    // ---- RPN: 3x3 conv + ReLU, the merged twin 1x1 heads (fp32 [H*W, rpn_ld]), ProposalLayer with the 2A-way softmax fused
-    if ((rc = frcnn_conv2d(feat.hi, feat.lo, h, w, 512, wts->rpn3.hi, wts->rpn3.lo, wts->rpn3.bias, 512, 3, 1, 0, L.rpn_mid.hi,
-                           L.rpn_mid.lo, nullptr, 0, nullptr, stream)) != FRCNN_OK) return rc;
-    if ((rc = frcnn_conv2d(L.rpn_mid.hi, L.rpn_mid.lo, h, w, 512, wts->rpn_heads.hi, wts->rpn_heads.lo, wts->rpn_heads.bias,
-                           6 * c.n_anchors, 1, 0, 0, nullptr, nullptr, L.rpn_out, L.rpn_ld, nullptr, stream)) != FRCNN_OK) return rc;
-    if ((rc = frcnn_proposals(L.rpn_out, 1, L.rpn_ld, 1, L.rpn_out + 2 * c.n_anchors, 1, L.rpn_ld, wts->anchors, c.n_anchors, h, w,
-                              c.feat_stride, im_h, im_w, c.min_size, c.pre_nms_top_n, c.post_nms_top_n, c.nms_thresh, L.rois,
-                              L.scores, out_count, nullptr, nullptr, nullptr, L.prop_ws, L.prop_ws_bytes, stream)) != FRCNN_OK) return rc;
-    // ---- RoI pooling + head (rows past *out_count are zero)
-    const int R = c.post_nms_top_n;
-    if ((rc = frcnn_roi_pool(feat.hi, feat.lo, h, w, 512, L.rois, out_count, R, 7, 7, 1.0f / (float)c.feat_stride, L.pool5.hi,
-                             L.pool5.lo, nullptr, stream)) != FRCNN_OK) return rc;
-    if ((rc = frcnn_linear(L.pool5.hi, L.pool5.lo, R, 49 * 512, wts->fc6.hi, wts->fc6.lo, wts->fc6.bias, 4096, 1, out_count, L.fc6.hi,
-                           L.fc6.lo, nullptr, 0, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
-    if ((rc = frcnn_linear(L.fc6.hi, L.fc6.lo, R, 4096, wts->fc7.hi, wts->fc7.lo, wts->fc7.bias, 4096, 1, out_count, L.fc7.hi, L.fc7.lo,
-                           nullptr, 0, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
-    if ((rc = frcnn_linear(L.fc7.hi, L.fc7.lo, R, 4096, wts->head.hi, wts->head.lo, wts->head.bias, 5 * c.num_classes, 0, out_count,
-                           nullptr, nullptr, L.head_out, L.head_ld, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
-    return frcnn_head_decode(L.head_out, L.head_out + c.num_classes, L.head_ld, L.rois, out_count, R, c.num_classes, im_h, im_w,
-                             out_prob, out_boxes, stream);
+    // ---- RPN: 3x3 conv + ReLU, the merged twin 1x1 heads (fp32 [N*H*W, rpn_ld]), ProposalLayer with the 2A-way softmax fused
+    if ((rc = frcnn_conv2d_batch(feat.hi, feat.lo, N, h, w, 512, wts->rpn3.hi, wts->rpn3.lo, wts->rpn3.bias, 512, 3, 1, 0, L.rpn_mid.hi,
+                                 L.rpn_mid.lo, nullptr, 0, stream)) != FRCNN_OK) return rc;
+    if ((rc = frcnn_conv2d_batch(L.rpn_mid.hi, L.rpn_mid.lo, N, h, w, 512, wts->rpn_heads.hi, wts->rpn_heads.lo, wts->rpn_heads.bias,
+                                 6 * c.n_anchors, 1, 0, 0, nullptr, nullptr, L.rpn_out, L.rpn_ld, stream)) != FRCNN_OK) return rc;
+    const int R = c.post_nms_top_n, NC = c.num_classes;
+    const long rpn_is = (long)h * w * L.rpn_ld;
+    if ((rc = frcnn_proposals_batch(N, L.rpn_out, 1, L.rpn_ld, rpn_is, 1, L.rpn_out + 2 * c.n_anchors, 1, L.rpn_ld, rpn_is, wts->anchors,
+                                    c.n_anchors, h, w, c.feat_stride, im_h, im_w, c.min_size, c.pre_nms_top_n, R, c.nms_thresh, L.rois,
+                                    4l * R, L.scores, R, out_count, 1, nullptr, 0, nullptr, 0, nullptr, 0, L.prop_ws, L.prop_ws_bytes,
+                                    stream)) != FRCNN_OK) return rc;
+    // ---- RoI pooling + head (rows past out_count[n] are zero)
+    if ((rc = frcnn_roi_pool_batch(feat.hi, feat.lo, N, h, w, 512, L.rois, 4l * R, out_count, 1, R, 7, 7, 1.0f / (float)c.feat_stride,
+                                   L.pool5.hi, L.pool5.lo, nullptr, (long)L.ld1 * 49 * 512, stream)) != FRCNN_OK) return rc;
+    if ((rc = frcnn_linear_batch(L.pool5.hi, L.pool5.lo, N, R, 49 * 512, wts->fc6.hi, wts->fc6.lo, wts->fc6.bias, 4096, 1, out_count, 1,
+                                 L.fc6.hi, L.fc6.lo, nullptr, 0, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
+    if ((rc = frcnn_linear_batch(L.fc6.hi, L.fc6.lo, N, R, 4096, wts->fc7.hi, wts->fc7.lo, wts->fc7.bias, 4096, 1, out_count, 1, L.fc7.hi,
+                                 L.fc7.lo, nullptr, 0, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
+    if ((rc = frcnn_linear_batch(L.fc7.hi, L.fc7.lo, N, R, 4096, wts->head.hi, wts->head.lo, wts->head.bias, 5 * NC, 0, out_count, 1,
+                                 nullptr, nullptr, L.head_out, L.head_ld, L.fc_ws, L.fc_ws_bytes, stream)) != FRCNN_OK) return rc;
+    return frcnn_head_decode_batch(N, L.head_out, L.head_out + NC, L.head_ld, (long)L.ld1 * L.head_ld, L.rois, 4l * R, out_count, 1, R,
+                                   NC, im_h, im_w, out_prob, (long)R * NC, out_boxes, 4l * R * NC, stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t frcnn_forward_workspace_bytes(const frcnn_forward_config* config) {
+    FRCNN_ENTRY();
+    if (check_config(config) != FRCNN_OK) return 0;
+    return carve(*config, 1, nullptr).total;
+}
+
+size_t frcnn_forward_batch_workspace_bytes(const frcnn_forward_config* config, int N) {
+    FRCNN_ENTRY();
+    if (check_config(config) != FRCNN_OK || check_batch(N) != FRCNN_OK) return 0;
+    return carve(*config, N, nullptr).total;
+}
+
+int frcnn_forward_vgg16(const frcnn_forward_config* config, const frcnn_vgg16_weights* wts, const float* image_chw, int im_h,
+                        int im_w, void* workspace, size_t workspace_bytes, float* out_prob, float* out_boxes, int* out_count,
+                        void* stream) {
+    FRCNN_ENTRY();
+    return forward_n(config, wts, 1, image_chw, im_h, im_w, workspace, workspace_bytes, out_prob, out_boxes, out_count,
+                     static_cast<cudaStream_t>(stream));
+}
+
+int frcnn_forward_vgg16_batch(const frcnn_forward_config* config, const frcnn_vgg16_weights* wts, int N, const float* images_nchw,
+                              int im_h, int im_w, void* workspace, size_t workspace_bytes, float* out_prob, float* out_boxes,
+                              int* out_count, void* stream) {
+    FRCNN_ENTRY();
+    return forward_n(config, wts, N, images_nchw, im_h, im_w, workspace, workspace_bytes, out_prob, out_boxes, out_count,
+                     static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

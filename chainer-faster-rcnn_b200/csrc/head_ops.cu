@@ -263,9 +263,20 @@ __global__ void unpack_nhwc_kernel(const __nv_bfloat16* hi, const __nv_bfloat16*
 }
 
 // ------------------------------------------------------------------------------------------ max-pool 2x2/2 ceil
+// A batch [N][H][W][C]: image blockIdx.y reads x + blockIdx.y * H*W*C and writes y + blockIdx.y * Ho*Wo*C.
+// Every kernel of this file with a kBatch parameter takes the image from blockIdx.y when it is true; the one-image entry
+// points launch the kBatch = false instantiation, where the image is the constant 0 and the offsets fold away.
+template <bool kBatch>
 __global__ void maxpool_kernel(const __nv_bfloat16* xh, const __nv_bfloat16* xl, int H, int W, int C,
                                __nv_bfloat16* yh, __nv_bfloat16* yl) {
     grid_dep_wait();
+    if (kBatch) {
+        const long xo = blockIdx.y * ((long)H * W * C), yo = blockIdx.y * ((long)((H + 1) / 2) * ((W + 1) / 2) * C);
+        xh += xo;
+        yh += yo;
+        if (xl) xl += xo;
+        if (yl) yl += yo;
+    }
     const int Ho = (H + 1) / 2, Wo = (W + 1) / 2, C8 = C / 8;
     const long total = (long)Ho * Wo * C8;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -363,13 +374,25 @@ __device__ __forceinline__ Pair8 pair8_neg_inf() {
 }
 
 constexpr int kRoiColMaxThreads = 448;        // 7 output columns x 64 channel groups; two CTAs of 72 registers per SM
-template <bool LO>
+template <bool LO, bool kBatch>
 __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(const __nv_bfloat16* __restrict__ fh, const __nv_bfloat16* __restrict__ fl,
                                                                          int H, int W, int C, const float* __restrict__ rois,
                                                                          const int* __restrict__ count, int R_cap, int PH, int PW, float scale,
                                                                          __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol,
-                                                                         float* __restrict__ of32, int c8_per_cta, int slices) {
+                                                                         float* __restrict__ of32, int c8_per_cta, int slices,
+                                                                         long rois_is, long count_is, long out_is) {
     grid_dep_wait();
+    if (kBatch) {                      // image blockIdx.y: its feature map [H][W][C], RoIs, count and output rows
+        const long img = blockIdx.y;
+        const long fo = img * ((long)H * W * C), oo = img * out_is;
+        fh += fo;
+        if (LO) fl += fo;
+        rois += img * rois_is;
+        if (count) count += img * count_is;
+        if (oh) oh += oo;
+        if (ol) ol += oo;
+        if (of32) of32 += oo;
+    }
     __shared__ int s_ws[kRoiMaxBins], s_we[kRoiMaxBins], s_hs[kRoiMaxBins], s_he[kRoiMaxBins];
     const int C8 = C / 8;
     const int R = count ? min(*count, R_cap) : R_cap;
@@ -470,13 +493,25 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
 
 // ------------------------------------------------------------------------------------------ head decode
 // One thread per (roi, class): softmax over classes (every thread recomputes max/sum of its row --
-// 21 values, L1-resident) and bbox_transform_inv + clip_boxes for its class's 4 deltas.
+// 21 values, L1-resident) and bbox_transform_inv + clip_boxes for its class's 4 deltas.  Image blockIdx.y of a batch
+// reads and writes its own rows, (image) * (the array's image stride) elements on.
+struct DecodeStrides { long in, rois, count, prob, boxes; };
+template <bool kBatch>
 __global__ void head_decode_kernel(const float* scores, const float* deltas, int ld, const float* rois,
                                    const int* count, int R_cap, int NC, int im_h, int im_w, float* prob,
-                                   float* boxes) {
+                                   float* boxes, const DecodeStrides is) {
     grid_dep_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= R_cap * NC) return;
+    if (kBatch) {
+        const long img = blockIdx.y;
+        scores += img * is.in;
+        deltas += img * is.in;
+        rois += img * is.rois;
+        if (count) count += img * is.count;
+        prob += img * is.prob;
+        boxes += img * is.boxes;
+    }
     const int r = i / NC, c = i - r * NC;
     const int R = count ? min(*count, R_cap) : R_cap;
     float p = 0.0f;
@@ -518,10 +553,27 @@ constexpr int kDetThreads = 256;                      // detect_barrier_kernel
 constexpr int kDetMaskThreads = 1024;                 // detect_kernel: 20 CTAs on 132 SMs -- the rank and mask phases scale with the CTA
 constexpr int kDetMaxR = 2048;
 
+// Image blockIdx.y of a batch: its prob / boxes rows, count and keep_idx / keep_count / conf_count outputs lie
+// (image) * (the array's image stride) elements on.  Applied to the base pointers once, here at entry.
+struct DetectStrides { long prob, boxes, count, keep_idx, keep_count, conf_count; };
+__device__ __forceinline__ void detect_image_bases(const DetectStrides& is, const float*& prob, const float*& boxes,
+                                                   const int*& count, int*& keep_idx, int*& keep_count, int*& conf_count) {
+    const long img = blockIdx.y;
+    prob += img * is.prob;
+    boxes += img * is.boxes;
+    if (count) count += img * is.count;
+    keep_idx += img * is.keep_idx;
+    keep_count += img * is.keep_count;
+    conf_count += img * is.conf_count;
+}
+
+template <bool kBatch>
 __global__ void __launch_bounds__(kDetMaskThreads) detect_kernel(const float* prob, const float* boxes, const int* count,
                                                              int R_cap, int NC, double thr, float conf,
-                                                             int* keep_idx, int* keep_count, int* conf_count) {
+                                                             int* keep_idx, int* keep_count, int* conf_count,
+                                                             const DetectStrides is) {
     grid_dep_wait();
+    if (kBatch) detect_image_bases(is, prob, boxes, count, keep_idx, keep_count, conf_count);
     extern __shared__ __align__(16) unsigned char dsm[];
     const int R = count ? min(*count, R_cap) : R_cap;
     const int words = (R_cap + 63) >> 6;                             // uint64 words per mask row
@@ -632,10 +684,13 @@ __global__ void __launch_bounds__(kDetMaskThreads) detect_kernel(const float* pr
 
 // Fallback for R_cap too large for the bitmask to fit in shared memory (R_cap > ~1100): survivors are resolved with one
 // block-wide barrier per kept box.
+template <bool kBatch>
 __global__ void __launch_bounds__(kDetThreads) detect_barrier_kernel(const float* prob, const float* boxes, const int* count,
                                                              int R_cap, int NC, double thr, float conf,
-                                                             int* keep_idx, int* keep_count, int* conf_count) {
+                                                             int* keep_idx, int* keep_count, int* conf_count,
+                                                             const DetectStrides is) {
     grid_dep_wait();
+    if (kBatch) detect_image_bases(is, prob, boxes, count, keep_idx, keep_count, conf_count);
     extern __shared__ __align__(16) unsigned char dsm[];
     const int R = count ? min(*count, R_cap) : R_cap;
     float4* sbox = reinterpret_cast<float4*>(dsm);                   // [R_cap] boxes by rank
@@ -831,55 +886,152 @@ extern "C" int frcnn_unpack_nhwc(const void* x_hi, const void* x_lo, int H, int 
     return FRCNN_OK;
 }
 
+namespace frcnn {
+static int maxpool2x2_n(const char* fn, const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo,
+                        cudaStream_t stream) {
+    FRCNN_REQUIRE(x_hi && y_hi && H > 0 && W > 0 && C > 0 && C % 8 == 0, "%s: bad arguments (C=%d)", fn, C);
+    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "%s: lo planes must both be given or both NULL", fn);
+    const long total = (long)((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
+    FRCNN_CUDA_OK(launch_pdl(N > 1 ? maxpool_kernel<true> : maxpool_kernel<false>, dim3(grid_for(total, 256), N), dim3(256), 0, stream, (const __nv_bfloat16*)x_hi,
+                             (const __nv_bfloat16*)x_lo, H, W, C, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo));
+    return FRCNN_OK;
+}
+
+static int roi_pool_n(const char* fn, const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                      long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale, void* out_hi,
+                      void* out_lo, float* out_f32, long out_stride, cudaStream_t stream) {
+    FRCNN_REQUIRE(feat_hi && rois && (out_hi || out_f32) && H > 0 && W > 0 && C > 0 && C % 8 == 0 && R_cap > 0 &&
+                      outh > 0 && outw > 0,
+                  "%s: bad arguments", fn);
+    FRCNN_REQUIRE(!out_lo || out_hi, "%s: out_lo without out_hi", fn);
+    FRCNN_REQUIRE(outw < kRoiMaxBins && outh < kRoiMaxBins, "%s: outh and outw must be < %d", fn, kRoiMaxBins);
+    if (N > 1) {
+        const long rows = (long)R_cap * outh * outw * C;
+        FRCNN_REQUIRE(rois_stride >= 0 && rois_stride % 4 == 0, "%s: rois image stride must be a multiple of 4 and >= 0", fn);
+        FRCNN_REQUIRE(!counts || count_stride >= 0, "%s: count image stride must be >= 0", fn);
+        FRCNN_REQUIRE(out_stride >= rows && out_stride % 8 == 0, "%s: output image stride %ld overlaps (needs a multiple of 8, >= %ld)",
+                      fn, out_stride, rows);
+    }
+    int c8_per_cta = 1;                                      // a power of two: the slice's channel groups are contiguous
+    while (2 * c8_per_cta <= C / 8 && 2 * c8_per_cta * outw <= kRoiColMaxThreads) c8_per_cta *= 2;
+    const int slices = (C / 8 + c8_per_cta - 1) / c8_per_cta;
+    const int threads = ((outw * c8_per_cta + 31) / 32) * 32;
+    const long ctas = (long)R_cap * slices;
+    const dim3 grid((unsigned)(ctas < 132l * 64 ? ctas : 132l * 64), N);
+    if (feat_lo) {
+        FRCNN_CUDA_OK(launch_pdl(N > 1 ? roi_pool_col_kernel<true, true> : roi_pool_col_kernel<true, false>, grid, dim3(threads), 0, stream, (const __nv_bfloat16*)feat_hi,
+                                 (const __nv_bfloat16*)feat_lo, H, W, C, rois, counts, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
+                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride));
+    } else {
+        FRCNN_CUDA_OK(launch_pdl(N > 1 ? roi_pool_col_kernel<false, true> : roi_pool_col_kernel<false, false>, grid, dim3(threads), 0, stream, (const __nv_bfloat16*)feat_hi,
+                                 (const __nv_bfloat16*)feat_lo, H, W, C, rois, counts, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
+                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride));
+    }
+    return FRCNN_OK;
+}
+
+static int head_decode_n(const char* fn, int N, const float* scores, const float* deltas, int ld, const float* rois,
+                         const int* counts, int R_cap, int num_classes, int im_h, int im_w, float* out_prob, float* out_boxes,
+                         const DecodeStrides& is, cudaStream_t stream) {
+    FRCNN_REQUIRE(scores && deltas && rois && out_prob && out_boxes && R_cap > 0 && num_classes > 0 && ld >= num_classes,
+                  "%s: bad arguments", fn);
+    if (N > 1) {
+        FRCNN_REQUIRE(is.in >= 0 && is.rois >= 0 && is.rois % 4 == 0 && (!counts || is.count >= 0),
+                      "%s: input image strides must be >= 0 (rois: a multiple of 4)", fn);
+        FRCNN_REQUIRE(is.prob >= (long)R_cap * num_classes, "%s: prob image stride %ld overlaps (needs >= %ld)", fn, is.prob,
+                      (long)R_cap * num_classes);
+        FRCNN_REQUIRE(is.boxes >= 4l * R_cap * num_classes && is.boxes % 4 == 0,
+                      "%s: boxes image stride %ld overlaps (needs a multiple of 4, >= %ld)", fn, is.boxes, 4l * R_cap * num_classes);
+    }
+    const int total = R_cap * num_classes;
+    FRCNN_CUDA_OK(launch_pdl(N > 1 ? head_decode_kernel<true> : head_decode_kernel<false>, dim3(cdiv(total, 128), N), dim3(128), 0, stream, scores, deltas, ld, rois, counts, R_cap,
+                             num_classes, im_h, im_w, out_prob, out_boxes, is));
+    return FRCNN_OK;
+}
+
+static int detect_n(const char* fn, int N, const float* prob, const float* boxes, const int* counts, int R_cap, int num_classes,
+                    double nms_thresh, float conf, int* keep_idx, int* keep_count, int* conf_count, const DetectStrides& is,
+                    cudaStream_t stream) {
+    FRCNN_REQUIRE(prob && boxes && keep_idx && keep_count && conf_count && num_classes > 1, "%s: bad arguments", fn);
+    FRCNN_REQUIRE(R_cap > 0 && R_cap <= kDetMaxR, "%s: R_cap must be in [1,%d] (got %d)", fn, kDetMaxR, R_cap);
+    if (N > 1) {
+        FRCNN_REQUIRE(is.prob >= 0 && is.boxes >= 0 && is.boxes % 4 == 0 && (!counts || is.count >= 0),
+                      "%s: input image strides must be >= 0 (boxes: a multiple of 4)", fn);
+        FRCNN_REQUIRE(is.keep_idx >= (long)(num_classes - 1) * R_cap, "%s: keep_idx image stride %ld overlaps (needs >= %ld)", fn,
+                      is.keep_idx, (long)(num_classes - 1) * R_cap);
+        FRCNN_REQUIRE(is.keep_count >= num_classes - 1 && is.conf_count >= num_classes - 1,
+                      "%s: keep_count / conf_count image strides %ld / %ld overlap (need >= %d)", fn, is.keep_count, is.conf_count,
+                      num_classes - 1);
+    }
+    const size_t words = (size_t)(R_cap + 63) / 64;
+    size_t smem = (size_t)R_cap * (sizeof(float) + sizeof(int) + 8 * words) + 64 * words * (sizeof(float4) + sizeof(float)) + 16;
+    const dim3 grid(num_classes - 1, N);
+    if (smem > 200 * 1024) {
+        smem = (size_t)R_cap * (sizeof(float) + sizeof(int) + sizeof(float4) + 1) + 16;
+        auto kern = N > 1 ? detect_barrier_kernel<true> : detect_barrier_kernel<false>;
+        FRCNN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        FRCNN_CUDA_OK(launch_pdl(kern, grid, dim3(kDetThreads), smem, stream, prob, boxes, counts, R_cap, num_classes,
+                                 nms_thresh, conf, keep_idx, keep_count, conf_count, is));
+        return FRCNN_OK;
+    }
+    auto kern = N > 1 ? detect_kernel<true> : detect_kernel<false>;
+    FRCNN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FRCNN_CUDA_OK(launch_pdl(kern, grid, dim3(kDetMaskThreads), smem, stream, prob, boxes, counts, R_cap, num_classes,
+                             nms_thresh, conf, keep_idx, keep_count, conf_count, is));
+    return FRCNN_OK;
+}
+}  // namespace frcnn
+
+#define FRCNN_REQUIRE_BATCH(fn, N) FRCNN_REQUIRE((N) >= 1 && (N) <= 65535, "%s: N must be in [1,65535] (got %d)", fn, (int)(N))
+
 extern "C" int frcnn_maxpool2x2_ceil(const void* x_hi, const void* x_lo, int H, int W, int C, void* y_hi, void* y_lo,
                                      void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(x_hi && y_hi && H > 0 && W > 0 && C > 0 && C % 8 == 0, "frcnn_maxpool2x2_ceil: bad arguments (C=%d)", C);
-    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "frcnn_maxpool2x2_ceil: lo planes must both be given or both NULL");
-    const long total = (long)((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
-    FRCNN_CUDA_OK(launch_pdl(maxpool_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream,
-                             (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, H, W, C, (__nv_bfloat16*)y_hi,
-                             (__nv_bfloat16*)y_lo));
-    return FRCNN_OK;
+    return maxpool2x2_n("frcnn_maxpool2x2_ceil", x_hi, x_lo, 1, H, W, C, y_hi, y_lo, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_maxpool2x2_ceil_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo,
+                                           void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_maxpool2x2_ceil_batch", N);
+    return maxpool2x2_n("frcnn_maxpool2x2_ceil_batch", x_hi, x_lo, N, H, W, C, y_hi, y_lo, (cudaStream_t)stream);
 }
 
 extern "C" int frcnn_roi_pool(const void* feat_hi, const void* feat_lo, int H, int W, int C, const float* rois,
                               const int* count, int R_cap, int outh, int outw, float scale, void* out_hi, void* out_lo,
                               float* out_f32, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(feat_hi && rois && (out_hi || out_f32) && H > 0 && W > 0 && C > 0 && C % 8 == 0 && R_cap > 0 &&
-                      outh > 0 && outw > 0,
-                  "frcnn_roi_pool: bad arguments");
-    FRCNN_REQUIRE(!out_lo || out_hi, "frcnn_roi_pool: out_lo without out_hi");
-    FRCNN_REQUIRE(outw < kRoiMaxBins && outh < kRoiMaxBins, "frcnn_roi_pool: outh and outw must be < %d", kRoiMaxBins);
-    int c8_per_cta = 1;                                      // a power of two: the slice's channel groups are contiguous
-    while (2 * c8_per_cta <= C / 8 && 2 * c8_per_cta * outw <= kRoiColMaxThreads) c8_per_cta *= 2;
-    const int slices = (C / 8 + c8_per_cta - 1) / c8_per_cta;
-    const int threads = ((outw * c8_per_cta + 31) / 32) * 32;
-    const long ctas = (long)R_cap * slices;
-    const dim3 grid((unsigned)(ctas < 132l * 64 ? ctas : 132l * 64));
-    if (feat_lo) {
-        FRCNN_CUDA_OK(launch_pdl(roi_pool_col_kernel<true>, grid, dim3(threads), 0, (cudaStream_t)stream, (const __nv_bfloat16*)feat_hi,
-                                 (const __nv_bfloat16*)feat_lo, H, W, C, rois, count, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
-                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices));
-    } else {
-        FRCNN_CUDA_OK(launch_pdl(roi_pool_col_kernel<false>, grid, dim3(threads), 0, (cudaStream_t)stream, (const __nv_bfloat16*)feat_hi,
-                                 (const __nv_bfloat16*)feat_lo, H, W, C, rois, count, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
-                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices));
-    }
-    return FRCNN_OK;
+    return roi_pool_n("frcnn_roi_pool", feat_hi, feat_lo, 1, H, W, C, rois, 0, count, 0, R_cap, outh, outw, scale, out_hi, out_lo,
+                      out_f32, 0, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_roi_pool_batch(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                                    long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale,
+                                    void* out_hi, void* out_lo, float* out_f32, long out_stride, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_roi_pool_batch", N);
+    return roi_pool_n("frcnn_roi_pool_batch", feat_hi, feat_lo, N, H, W, C, rois, rois_stride, counts, count_stride, R_cap, outh, outw,
+                      scale, out_hi, out_lo, out_f32, out_stride, (cudaStream_t)stream);
 }
 
 extern "C" int frcnn_head_decode(const float* scores, const float* deltas, int ld, const float* rois, const int* count,
                                  int R_cap, int num_classes, int im_h, int im_w, float* out_prob, float* out_boxes,
                                  void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(scores && deltas && rois && out_prob && out_boxes && R_cap > 0 && num_classes > 0 && ld >= num_classes,
-                  "frcnn_head_decode: bad arguments");
-    const int total = R_cap * num_classes;
-    FRCNN_CUDA_OK(launch_pdl(head_decode_kernel, dim3(cdiv(total, 128)), dim3(128), 0, (cudaStream_t)stream, scores, deltas, ld,
-                             rois, count, R_cap, num_classes, im_h, im_w, out_prob, out_boxes));
-    return FRCNN_OK;
+    const DecodeStrides is = {0, 0, 0, 0, 0};
+    return head_decode_n("frcnn_head_decode", 1, scores, deltas, ld, rois, count, R_cap, num_classes, im_h, im_w, out_prob, out_boxes,
+                         is, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_head_decode_batch(int N, const float* scores, const float* deltas, int ld, long in_stride, const float* rois,
+                                       long rois_stride, const int* counts, long count_stride, int R_cap, int num_classes, int im_h,
+                                       int im_w, float* out_prob, long prob_stride, float* out_boxes, long boxes_stride,
+                                       void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_head_decode_batch", N);
+    const DecodeStrides is = {in_stride, rois_stride, count_stride, prob_stride, boxes_stride};
+    return head_decode_n("frcnn_head_decode_batch", N, scores, deltas, ld, rois, counts, R_cap, num_classes, im_h, im_w, out_prob,
+                         out_boxes, is, (cudaStream_t)stream);
 }
 
 namespace frcnn {
@@ -935,19 +1087,18 @@ extern "C" int frcnn_detect(const float* prob, const float* boxes, const int* co
                             double nms_thresh, float conf, int* keep_idx, int* keep_count, int* conf_count,
                             void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(prob && boxes && keep_idx && keep_count && conf_count && num_classes > 1, "frcnn_detect: bad arguments");
-    FRCNN_REQUIRE(R_cap > 0 && R_cap <= kDetMaxR, "frcnn_detect: R_cap must be in [1,%d] (got %d)", kDetMaxR, R_cap);
-    const size_t words = (size_t)(R_cap + 63) / 64;
-    size_t smem = (size_t)R_cap * (sizeof(float) + sizeof(int) + 8 * words) + 64 * words * (sizeof(float4) + sizeof(float)) + 16;
-    if (smem > 200 * 1024) {
-        smem = (size_t)R_cap * (sizeof(float) + sizeof(int) + sizeof(float4) + 1) + 16;
-        FRCNN_CUDA_OK(cudaFuncSetAttribute(detect_barrier_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        FRCNN_CUDA_OK(launch_pdl(detect_barrier_kernel, dim3(num_classes - 1), dim3(kDetThreads), smem, (cudaStream_t)stream, prob,
-                                 boxes, count, R_cap, num_classes, nms_thresh, conf, keep_idx, keep_count, conf_count));
-        return FRCNN_OK;
-    }
-    FRCNN_CUDA_OK(cudaFuncSetAttribute(detect_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FRCNN_CUDA_OK(launch_pdl(detect_kernel, dim3(num_classes - 1), dim3(kDetMaskThreads), smem, (cudaStream_t)stream, prob, boxes,
-                             count, R_cap, num_classes, nms_thresh, conf, keep_idx, keep_count, conf_count));
-    return FRCNN_OK;
+    const DetectStrides is = {0, 0, 0, 0, 0, 0};
+    return detect_n("frcnn_detect", 1, prob, boxes, count, R_cap, num_classes, nms_thresh, conf, keep_idx, keep_count, conf_count, is,
+                    (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_detect_batch(int N, const float* prob, long prob_stride, const float* boxes, long boxes_stride,
+                                  const int* counts, long count_stride, int R_cap, int num_classes, double nms_thresh, float conf,
+                                  int* keep_idx, long keep_idx_stride, int* keep_count, long keep_count_stride, int* conf_count,
+                                  long conf_count_stride, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_detect_batch", N);
+    const DetectStrides is = {prob_stride, boxes_stride, count_stride, keep_idx_stride, keep_count_stride, conf_count_stride};
+    return detect_n("frcnn_detect_batch", N, prob, boxes, counts, R_cap, num_classes, nms_thresh, conf, keep_idx, keep_count, conf_count,
+                    is, (cudaStream_t)stream);
 }

@@ -18,10 +18,25 @@
 //   4. nms_mask_kernel     upper-triangular 64x64 IoU tiles -> uint64 suppression bitmask
 //   5. nms_scan_kernel     ONE CTA walks the mask (device-side; the reference copies it to the host,
 //                          nms_kernel.cu:124-139), stops at post_nms_top_n, gathers the output rows
+//
+// A batch of N images runs the same five launches: the image is grid dimension y (decode, rank/scatter), z (IoU mask) or
+// the CTA index (select, scan: one CTA per image).  Image n's scratch is the NmsWs slice n * ws_stride bytes into the
+// workspace, and its inputs / outputs sit n * (their image stride) elements further on.  Every kernel moves its base
+// pointers once, at entry.  One image is the case n = 0, compiled as its own instantiation (kBatch = false: the image index
+// is the constant 0 and every offset folds away), so that the one-image kernels keep their code and their time.
 #include "common.cuh"
 #include "nms_math.cuh"
 
 namespace frcnn {
+
+// a workspace pointer moved `bytes` on (to the image's slice)
+template <typename T>
+__device__ __forceinline__ T* ws_at(T* p, long bytes) {
+    return reinterpret_cast<T*>(reinterpret_cast<char*>(const_cast<void*>(static_cast<const void*>(p))) + bytes);
+}
+// an optional output moved `elems` on; NULL stays NULL
+template <typename T>
+__device__ __forceinline__ T* opt_at(T* p, long elems) { return p ? p + elems : p; }
 
 // ------------------------------------------------------------------------------------------ 1. decode
 struct DecodeArgs {
@@ -30,13 +45,19 @@ struct DecodeArgs {
     const double* anchors;
     int A, H, W, feat_stride, im_h, im_w, min_size;
     float4* boxes; float* scores; uint32_t* keys;
+    long cls_is, bbox_is, ws_stride;      // image strides: cls / bbox in floats, the workspace slice in bytes
 };
 
+template <bool kBatch>
 __global__ void rpn_decode_kernel(const DecodeArgs a) {
     grid_dep_wait();
     const int n = a.A * a.H * a.W;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const int img = kBatch ? blockIdx.y : 0;
+    const float* cls = a.cls + img * a.cls_is;
+    const float* bbox = a.bbox + img * a.bbox_is;
+    const long ws_off = img * a.ws_stride;
     const int pix = i / a.A, an = i - pix * a.A;
     const int h = pix / a.W, w = pix - h * a.W;
 
@@ -45,7 +66,7 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     if (a.cls_is_logits) {
         // F.softmax over ALL 2A channels (models/region_proposal_network.py:119, SURVEY Q1):
         // y = x - max; e = exp(y); e / sum(e), sum in ascending channel order.
-        const float* c = a.cls + (long)pix * a.cls_ps;
+        const float* c = cls + (long)pix * a.cls_ps;
         float m = c[0];
         for (int k = 1; k < 2 * a.A; ++k) m = fmaxf(m, c[(long)k * a.cls_cs]);
         float s = 0.0f, mine = 0.0f;
@@ -56,7 +77,7 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
         }
         score = __fdiv_rn(mine, s);
     } else {
-        score = a.cls[(long)(a.A + an) * a.cls_cs + (long)pix * a.cls_ps];
+        score = cls[(long)(a.A + an) * a.cls_cs + (long)pix * a.cls_ps];
     }
 
     // anchor (models/proposal_layer.py:207-221): float64 base + integer shift, cast to float32
@@ -66,7 +87,7 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     const float ax2 = (float)(a.anchors[4 * an + 2] + sx);
     const float ay2 = (float)(a.anchors[4 * an + 3] + sy);
     // deltas: bbox_trans[(h*W+w)*A + an, j] = rpn_bbox_pred[4*an + j, h, w]  (:138)
-    const float* d = a.bbox + (long)pix * a.bbox_ps + (long)(4 * an) * a.bbox_cs;
+    const float* d = bbox + (long)pix * a.bbox_ps + (long)(4 * an) * a.bbox_cs;
     const float dx = d[0], dy = d[a.bbox_cs], dw = d[2 * a.bbox_cs], dh = d[3 * a.bbox_cs];
 
     // bbox_transform_inv (models/bbox_transform.py:51-74)
@@ -93,9 +114,9 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     const float hs = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
     const bool ok = (ws >= (float)a.min_size) && (hs >= (float)a.min_size) && (score == score);
 
-    a.boxes[i] = make_float4(x1, y1, x2, y2);
-    a.scores[i] = score;
-    a.keys[i] = ok ? float_to_ordered(score) : 0u;
+    ws_at(a.boxes, ws_off)[i] = make_float4(x1, y1, x2, y2);
+    ws_at(a.scores, ws_off)[i] = score;
+    ws_at(a.keys, ws_off)[i] = ok ? float_to_ordered(score) : 0u;
 }
 
 __global__ void dets_keys_kernel(const float* dets, int n, float4* boxes, float* scores, uint32_t* keys) {
@@ -147,14 +168,18 @@ struct SortArgs {
     const float4* boxes; const float* scores;
     float4* sorted_boxes; float* sorted_scores; int* sorted_idx; int* num_sorted;
     float* dbg_dets; int* dbg_idx; int* dbg_num;
-    long long* dbg_clocks;     // optional: 8 phase timestamps (clock64 of thread 0)
+    long long* dbg_clocks;     // optional: 8 phase timestamps (clock64 of thread 0 of image 0)
     unsigned long long* comp_out;   // [k_cap] selected composites (key desc | index), unordered
 };
+// Image strides of a batched select / rank-scatter: the workspace slice (bytes) and the debug outputs (elements).  A
+// parameter of its own: in SortArgs the larger argument block changed the one-image topk_sort_kernel's code.
+struct SortStrides { long ws, dbg_dets, dbg_idx, dbg_num; };
 
-// Selection step (ONE CTA): count, 4-pass radix select of the top_k-th key, order-preserving compaction.
+// Selection step (ONE CTA per image): count, 4-pass radix select of the top_k-th key, order-preserving compaction.
 // dynamic smem: uint64 comp[P] (P >= min(top_k, n)) followed, when it fits, by a copy of the n keys
 // (the select passes then never touch global memory again).
-__global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortArgs a, const int P, const int cache_keys) {
+template <bool kBatch>
+__global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortArgs a, const int P, const int cache_keys, const SortStrides is) {
     grid_dep_wait();
     extern __shared__ unsigned long long comp[];
     __shared__ unsigned int hist[256];
@@ -164,15 +189,17 @@ __global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortAr
     const int tid = threadIdx.x, lane = tid & 31;
     const int n = a.n;
     const int n_pad = (n + 31) & ~31;                 // whole warps iterate together (warp-aggregated atomics)
+    const int img = kBatch ? blockIdx.x : 0;
+    const long ws_off = img * is.ws;
     uint32_t* skeys = reinterpret_cast<uint32_t*>(comp + P);
-    const uint32_t* keys = a.keys;
-#define SORT_MARK(i) do { if (a.dbg_clocks && tid == 0) a.dbg_clocks[i] = clock64(); } while (0)
+    const uint32_t* keys = ws_at(a.keys, ws_off);
+#define SORT_MARK(i) do { if (a.dbg_clocks && tid == 0 && img == 0) a.dbg_clocks[i] = clock64(); } while (0)
     SORT_MARK(0);
 
     // ---- count candidates (key != 0), filling the smem copy on the way
     unsigned int cnt = 0;
     for (int i = tid; i < n; i += kSortThreads) {
-        const uint32_t k = a.keys[i];
+        const uint32_t k = ws_at(a.keys, ws_off)[i];
         if (cache_keys) skeys[i] = k;
         cnt += k != 0u;
     }
@@ -269,13 +296,14 @@ __global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortAr
     __syncthreads();
     SORT_MARK(3);
     // ---- hand the K selected composites (unordered) to the chip-wide rank kernel
-    for (int r = tid; r < K; r += kSortThreads) a.comp_out[r] = comp[r];
+    unsigned long long* comp_out = ws_at(a.comp_out, ws_off);
+    for (int r = tid; r < K; r += kSortThreads) comp_out[r] = comp[r];
     SORT_MARK(4);
     SORT_MARK(5);
 #undef SORT_MARK
     if (tid == 0) {
-        *a.num_sorted = K;
-        if (a.dbg_num) *a.dbg_num = K;
+        *ws_at(a.num_sorted, ws_off) = K;
+        if (a.dbg_num) a.dbg_num[img * is.dbg_num] = K;
     }
 }
 
@@ -284,13 +312,17 @@ __global__ void __launch_bounds__(kSortThreads, 1) topk_sort_kernel(const SortAr
 // whole chip, where a single-CTA bitonic network of the same 6000 elements is instruction-issue bound on one SM.  Each block ranks 32 elements (8 threads per element, each scanning 1/8 of the list from
 // a shared-memory copy) and scatters box / score / index straight to the sorted position.
 constexpr int kRankThreads = 256, kRankPerBlock = 32;
-__global__ void __launch_bounds__(kRankThreads) rank_scatter_kernel(const SortArgs a) {
+template <bool kBatch>
+__global__ void __launch_bounds__(kRankThreads) rank_scatter_kernel(const SortArgs a, const SortStrides is) {
     grid_dep_wait();
     extern __shared__ unsigned long long scomp[];
-    const int K = *a.num_sorted;
+    const int img = kBatch ? blockIdx.y : 0;
+    const long ws_off = img * is.ws;
+    const int K = *ws_at(a.num_sorted, ws_off);
     const int e0 = blockIdx.x * kRankPerBlock;
     if (e0 >= K) return;
-    for (int i = threadIdx.x; i < K; i += kRankThreads) scomp[i] = a.comp_out[i];
+    const unsigned long long* comp_in = ws_at(a.comp_out, ws_off);
+    for (int i = threadIdx.x; i < K; i += kRankThreads) scomp[i] = comp_in[i];
     __syncthreads();
     const int e = e0 + (threadIdx.x >> 3), part = threadIdx.x & 7;
     const bool live = e < K;
@@ -303,30 +335,35 @@ __global__ void __launch_bounds__(kRankThreads) rank_scatter_kernel(const SortAr
     if (live && part == 0) {
         const int r = cnt;
         const int idx = (int)(mine & 0xFFFFFFFFull);
-        const float4 b = a.boxes[idx];
-        const float s = a.scores[idx];
-        a.sorted_boxes[r] = b;
-        a.sorted_scores[r] = s;
-        a.sorted_idx[r] = idx;
+        const float4 b = ws_at(a.boxes, ws_off)[idx];
+        const float s = ws_at(a.scores, ws_off)[idx];
+        ws_at(a.sorted_boxes, ws_off)[r] = b;
+        ws_at(a.sorted_scores, ws_off)[r] = s;
+        ws_at(a.sorted_idx, ws_off)[r] = idx;
         if (a.dbg_dets) {
-            float* o = a.dbg_dets + 5l * r;
+            float* o = a.dbg_dets + img * is.dbg_dets + 5l * r;
             o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w; o[4] = s;
         }
-        if (a.dbg_idx) a.dbg_idx[r] = idx;
+        if (a.dbg_idx) a.dbg_idx[img * is.dbg_idx + r] = idx;
     }
 }
 
 
 // ------------------------------------------------------------------------------------------ 3. IoU bitmask
-// grid (col_blocks, col_blocks); only blocks with col >= row do work.  mask[row_box][col_block].
+// grid (col_blocks, col_blocks, images); only blocks with col >= row do work.  mask[row_box][col_block].
 // Thread = one row box against the block's 64 column boxes (shared memory, broadcast reads, areas precomputed): one
 // branch-free suppress_word64() per thread, ~25 instructions a pair.  (Pairs that branched on their decision path
 // diverged the warp on almost every column: 38 us for 6000 boxes, ~4x the instruction-issue bound.)
+// boxes, n_ptr and mask lie in the image's workspace slice, blockIdx.z * ws_stride bytes on.
+template <bool kBatch>
 __global__ void __launch_bounds__(64) nms_mask_kernel(const float4* boxes, const int* n_ptr, int n_cap,
                                                       double thr_d, float thr_f, int mode,
-                                                      unsigned long long* mask, int col_blocks) {
+                                                      unsigned long long* mask, int col_blocks, long ws_stride) {
     grid_dep_wait();
-    const int n = n_ptr ? min(*n_ptr, n_cap) : n_cap;
+    const long ws_off = kBatch ? blockIdx.z * ws_stride : 0;
+    boxes = ws_at(boxes, ws_off);
+    mask = ws_at(mask, ws_off);
+    const int n = n_ptr ? min(*ws_at(n_ptr, ws_off), n_cap) : n_cap;
     const int rb = blockIdx.y, cb = blockIdx.x;
     if (cb < rb || rb * 64 >= n || cb * 64 >= n) return;
     __shared__ float4 cbox[64];
@@ -357,8 +394,12 @@ struct ScanArgs {
     const float4* sorted_boxes; const float* sorted_scores;   // optional gather
     float* out_rois; float* out_scores; int out_cap;
     int diag_in_smem;
+    long ws_stride;                                   // image stride of the workspace slice (bytes)
+    long rois_is, scores_is, count_is;                // image strides of out_rois / out_scores / num_out (elements)
 };
 
+// ONE CTA per image (blockIdx.x).  keep_out (frcnn_nms only) is never batched.
+template <bool kBatch>
 __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
     grid_dep_wait();
     extern __shared__ unsigned long long removed[];   // [col_blocks]
@@ -367,7 +408,10 @@ __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
     __shared__ int s_nk, s_total;
     __shared__ int s_keep_all[2048];                  // positions of the first 2048 survivors (for the gather)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n = a.n_ptr ? min(*a.n_ptr, a.n_cap) : a.n_cap;
+    const int img = kBatch ? blockIdx.x : 0;
+    const long ws_off = img * a.ws_stride;
+    const unsigned long long* const mask = ws_at(a.mask, ws_off);
+    const int n = a.n_ptr ? min(*ws_at(a.n_ptr, ws_off), a.n_cap) : a.n_cap;
     const int nb = (n + 63) / 64;
     const int nsb = (nb + 3) / 4;
     const int limit = a.max_keep > 0 ? a.max_keep : 0x7fffffff;
@@ -384,7 +428,7 @@ __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int w = 4 * sb + j;
-            pf[j] = (row < n && w < nb) ? a.mask[row * a.col_blocks + w] : 0ull;
+            pf[j] = (row < n && w < nb) ? mask[row * a.col_blocks + w] : 0ull;
         }
     };
     if (nsb > 0) request(0);
@@ -408,7 +452,7 @@ __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
                     if (lane == 0) {
                         s_keep[nk] = lr;
                         const int pos = blk * 64 + i;
-                        if (a.keep_out) a.keep_out[total] = a.index_map ? a.index_map[pos] : pos;
+                        if (a.keep_out) a.keep_out[total] = a.index_map ? ws_at(a.index_map, ws_off)[pos] : pos;
                         if (total < 2048) s_keep_all[total] = pos;
                     }
                     ++nk;
@@ -429,7 +473,7 @@ __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
         const int w0 = 4 * (sb + 1);
         const int W = nb - w0;
         const int items = W > 0 ? nk * W : 0;
-        const unsigned long long* base = a.mask + (long)(sb * 256) * a.col_blocks + w0;
+        const unsigned long long* base = mask + (long)(sb * 256) * a.col_blocks + w0;
         for (int it0 = tid; it0 < items; it0 += 8 * 256) {
             unsigned long long m[8];
             int wv[8];
@@ -452,18 +496,22 @@ __global__ void __launch_bounds__(256, 1) nms_scan_kernel(const ScanArgs a) {
     }
     __syncthreads();
     const int total = s_total;
-    if (tid == 0 && a.num_out) *a.num_out = total;
+    if (tid == 0 && a.num_out) a.num_out[img * a.count_is] = total;
     if (a.out_rois) {
+        const float4* sorted_boxes = ws_at(a.sorted_boxes, ws_off);
+        const float* sorted_scores = ws_at(a.sorted_scores, ws_off);
+        float4* out_rois = reinterpret_cast<float4*>(a.out_rois + img * a.rois_is);
+        float* out_scores = opt_at(a.out_scores, img * a.scores_is);
         for (int r = tid; r < a.out_cap; r += blockDim.x) {
             float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
             float s = 0.f;
             if (r < total && r < 2048) {
                 const int pos = s_keep_all[r];
-                b = a.sorted_boxes[pos];
-                s = a.sorted_scores[pos];
+                b = sorted_boxes[pos];
+                s = sorted_scores[pos];
             }
-            reinterpret_cast<float4*>(a.out_rois)[r] = b;
-            if (a.out_scores) a.out_scores[r] = s;
+            out_rois[r] = b;
+            if (out_scores) out_scores[r] = s;
         }
     }
 }
@@ -515,9 +563,15 @@ static int next_pow2(int v) {
     return p;
 }
 
-// sort (top-k) + mask + scan, shared by frcnn_proposals and frcnn_nms
-static int run_sort_nms(const NmsWs& w, int n_all, int top_k, double thresh, int mode, int max_keep,
-                        int* keep_out, int* num_out, float* out_rois, float* out_scores, int out_cap,
+// Image strides (elements) of the per-image outputs of a batched run; all zero for one image.
+struct OutStrides {
+    long rois, scores, count, dbg_dets, dbg_idx, dbg_num;
+};
+
+// sort (top-k) + mask + scan over N images (workspace slices ws_stride bytes apart), shared by frcnn_proposals(_batch)
+// and frcnn_nms
+static int run_sort_nms(const NmsWs& w, int N, long ws_stride, const OutStrides& os, int n_all, int top_k, double thresh,
+                        int mode, int max_keep, int* keep_out, int* num_out, float* out_rois, float* out_scores, int out_cap,
                         float* dbg_dets, int* dbg_idx, int* dbg_num, bool map_to_original, cudaStream_t stream) {
     const int k_cap = top_k < n_all ? top_k : n_all;
     const int P = next_pow2(k_cap < 2 ? 2 : k_cap);
@@ -529,20 +583,25 @@ static int run_sort_nms(const NmsWs& w, int n_all, int top_k, double thresh, int
     sa.dbg_dets = dbg_dets; sa.dbg_idx = dbg_idx; sa.dbg_num = dbg_num;
     sa.dbg_clocks = g_sort_clocks;
     sa.comp_out = w.comp;
+    const SortStrides ss = {ws_stride, os.dbg_dets, os.dbg_idx, os.dbg_num};
     size_t sort_smem = sizeof(unsigned long long) * (size_t)P;
     const size_t keys_bytes = sizeof(uint32_t) * (size_t)n_all;
     const int cache_keys = sort_smem + keys_bytes <= 188 * 1024;     // smem copy of the keys when it fits (34 KB of static smem on top)
     if (cache_keys) sort_smem += keys_bytes;
-    FRCNN_CUDA_OK(cudaFuncSetAttribute(topk_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sort_smem));
-    FRCNN_CUDA_OK(launch_pdl(topk_sort_kernel, dim3(1), dim3(kSortThreads), sort_smem, stream, sa, P, cache_keys));
+    const bool batch = N > 1;
+    auto topk = batch ? topk_sort_kernel<true> : topk_sort_kernel<false>;
+    FRCNN_CUDA_OK(cudaFuncSetAttribute(topk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sort_smem));
+    FRCNN_CUDA_OK(launch_pdl(topk, dim3(N), dim3(kSortThreads), sort_smem, stream, sa, P, cache_keys, ss));
     const size_t rank_smem = sizeof(unsigned long long) * (size_t)k_cap;
-    FRCNN_CUDA_OK(cudaFuncSetAttribute(rank_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rank_smem));
-    FRCNN_CUDA_OK(launch_pdl(rank_scatter_kernel, dim3(cdiv(k_cap, kRankPerBlock)), dim3(kRankThreads), rank_smem, stream, sa));
+    auto rank = batch ? rank_scatter_kernel<true> : rank_scatter_kernel<false>;
+    FRCNN_CUDA_OK(cudaFuncSetAttribute(rank, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rank_smem));
+    FRCNN_CUDA_OK(launch_pdl(rank, dim3(cdiv(k_cap, kRankPerBlock), N), dim3(kRankThreads), rank_smem, stream, sa, ss));
 
     const int cbs = cdiv(k_cap, 64);
-    dim3 grid(cbs, cbs);
-    FRCNN_CUDA_OK(launch_pdl(nms_mask_kernel, grid, dim3(64), 0, stream, (const float4*)w.sorted_boxes, (const int*)w.num_sorted,
-                             k_cap, thresh, (float)thresh, mode, w.mask, w.col_blocks));
+    dim3 grid(cbs, cbs, N);
+    FRCNN_CUDA_OK(launch_pdl(batch ? nms_mask_kernel<true> : nms_mask_kernel<false>, grid, dim3(64), 0, stream,
+                             (const float4*)w.sorted_boxes, (const int*)w.num_sorted, k_cap, thresh, (float)thresh, mode, w.mask,
+                             w.col_blocks, ws_stride));
 
     ScanArgs sc;
     sc.mask = w.mask; sc.col_blocks = w.col_blocks;
@@ -551,10 +610,57 @@ static int run_sort_nms(const NmsWs& w, int n_all, int top_k, double thresh, int
     sc.keep_out = keep_out; sc.num_out = num_out;
     sc.sorted_boxes = w.sorted_boxes; sc.sorted_scores = w.sorted_scores;
     sc.out_rois = out_rois; sc.out_scores = out_scores; sc.out_cap = out_cap;
+    sc.ws_stride = ws_stride;
+    sc.rois_is = os.rois; sc.scores_is = os.scores; sc.count_is = os.count;
     const size_t scan_smem = sizeof(unsigned long long) * (size_t)w.col_blocks;
     sc.diag_in_smem = 0;
-    FRCNN_CUDA_OK(launch_pdl(nms_scan_kernel, dim3(1), dim3(256), scan_smem, stream, sc));
+    FRCNN_CUDA_OK(launch_pdl(batch ? nms_scan_kernel<true> : nms_scan_kernel<false>, dim3(N), dim3(256), scan_smem, stream, sc));
     return FRCNN_OK;
+}
+
+// The ProposalLayer over N images: shape checks, workspace carving, decode + run_sort_nms.
+static int proposals_n(const char* fn, int N, const float* cls, long cls_cs, long cls_ps, long cls_is, int cls_is_logits,
+                       const float* bbox, long bbox_cs, long bbox_ps, long bbox_is, const double* anchors, int A, int H, int W,
+                       int feat_stride, int im_h, int im_w, int min_size, int pre_nms_top_n, int post_nms_top_n, double nms_thresh,
+                       float* out_rois, float* out_scores, int* out_count, float* dbg_dets, int* dbg_idx, int* dbg_num,
+                       const OutStrides& os, void* ws, size_t ws_bytes, cudaStream_t stream) {
+    FRCNN_REQUIRE(cls && bbox && anchors && out_rois && out_count && ws, "%s: NULL argument", fn);
+    FRCNN_REQUIRE(A > 0 && A <= 32 && H > 0 && W > 0, "%s: bad shape A=%d H=%d W=%d", fn, A, H, W);
+    FRCNN_REQUIRE(pre_nms_top_n > 0 && pre_nms_top_n <= 16384, "%s: pre_nms_top_n must be in [1,16384] (got %d)", fn, pre_nms_top_n);
+    FRCNN_REQUIRE(post_nms_top_n > 0 && post_nms_top_n <= 2048, "%s: post_nms_top_n must be in [1,2048] (got %d)", fn, post_nms_top_n);
+    const long n_all_l = (long)A * H * W;
+    FRCNN_REQUIRE(n_all_l < (1l << 24), "%s: too many anchors (%ld)", fn, n_all_l);
+    const int n_all = (int)n_all_l;
+    const int k_cap = pre_nms_top_n < n_all ? pre_nms_top_n : n_all;
+    if (N > 1) {      // every image's outputs must be disjoint from the next one's
+        FRCNN_REQUIRE(cls_is >= 0 && bbox_is >= 0, "%s: input image strides must be >= 0", fn);
+        FRCNN_REQUIRE(os.rois >= 4l * post_nms_top_n && os.rois % 4 == 0,
+                      "%s: rois image stride %ld overlaps (needs a multiple of 4, >= %d)", fn, os.rois, 4 * post_nms_top_n);
+        FRCNN_REQUIRE(!out_scores || os.scores >= post_nms_top_n, "%s: scores image stride %ld overlaps (needs >= %d)", fn, os.scores,
+                      post_nms_top_n);
+        FRCNN_REQUIRE(os.count >= 1, "%s: count image stride %ld overlaps (needs >= 1)", fn, os.count);
+        FRCNN_REQUIRE(!dbg_dets || os.dbg_dets >= 5l * k_cap, "%s: debug dets image stride %ld overlaps (needs >= %d)", fn, os.dbg_dets,
+                      5 * k_cap);
+        FRCNN_REQUIRE(!dbg_idx || os.dbg_idx >= k_cap, "%s: debug index image stride %ld overlaps (needs >= %d)", fn, os.dbg_idx, k_cap);
+        FRCNN_REQUIRE(!dbg_num || os.dbg_num >= 1, "%s: debug count image stride %ld overlaps (needs >= 1)", fn, os.dbg_num);
+    }
+    NmsWs w = carve(ws, n_all, k_cap);
+    const size_t need = (size_t)N * w.total;       // w.total is a multiple of 256: the slices stay 256-byte aligned
+    if (ws_bytes < need) {
+        set_error("%s: workspace %zu < required %zu", fn, ws_bytes, need);
+        return FRCNN_ERR_WORKSPACE;
+    }
+    DecodeArgs da;
+    da.cls = cls; da.cls_cs = cls_cs; da.cls_ps = cls_ps; da.cls_is_logits = cls_is_logits;
+    da.bbox = bbox; da.bbox_cs = bbox_cs; da.bbox_ps = bbox_ps;
+    da.anchors = anchors;
+    da.A = A; da.H = H; da.W = W; da.feat_stride = feat_stride; da.im_h = im_h; da.im_w = im_w; da.min_size = min_size;
+    da.boxes = w.boxes; da.scores = w.scores; da.keys = w.keys;
+    da.cls_is = cls_is; da.bbox_is = bbox_is; da.ws_stride = (long)w.total;
+    FRCNN_CUDA_OK(launch_pdl(N > 1 ? rpn_decode_kernel<true> : rpn_decode_kernel<false>, dim3(cdiv(n_all, 128), N), dim3(128), 0,
+                             stream, da));
+    return run_sort_nms(w, N, (long)w.total, os, n_all, pre_nms_top_n, nms_thresh, FRCNN_NMS_GE_DOUBLE, post_nms_top_n, nullptr,
+                        out_count, out_rois, out_scores, post_nms_top_n, dbg_dets, dbg_idx, dbg_num, false, stream);
 }
 
 }  // namespace frcnn
@@ -569,6 +675,12 @@ extern "C" size_t frcnn_proposals_workspace_bytes(int A, int H, int W, int pre_n
     return carve(nullptr, (int)n_all, k_cap).total;
 }
 
+extern "C" size_t frcnn_proposals_batch_workspace_bytes(int N, int A, int H, int W, int pre_nms_top_n) {
+    FRCNN_ENTRY();
+    if (N < 1 || N > 65535) return 0;
+    return (size_t)N * frcnn_proposals_workspace_bytes(A, H, W, pre_nms_top_n);
+}
+
 extern "C" int frcnn_proposals(const float* cls, long cls_chan_stride, long cls_pix_stride, int cls_is_logits,
                                const float* bbox, long bbox_chan_stride, long bbox_pix_stride, const double* anchors,
                                int A, int H, int W, int feat_stride, int im_h, int im_w, int min_size,
@@ -576,30 +688,29 @@ extern "C" int frcnn_proposals(const float* cls, long cls_chan_stride, long cls_
                                float* out_scores, int* out_count, float* dbg_sorted_dets, int* dbg_sorted_anchor_idx,
                                int* dbg_num_sorted, void* ws, size_t ws_bytes, void* stream_) {
     FRCNN_ENTRY();
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    FRCNN_REQUIRE(cls && bbox && anchors && out_rois && out_count && ws, "frcnn_proposals: NULL argument");
-    FRCNN_REQUIRE(A > 0 && A <= 32 && H > 0 && W > 0, "frcnn_proposals: bad shape A=%d H=%d W=%d", A, H, W);
-    FRCNN_REQUIRE(pre_nms_top_n > 0 && pre_nms_top_n <= 16384, "frcnn_proposals: pre_nms_top_n must be in [1,16384] (got %d)", pre_nms_top_n);
-    FRCNN_REQUIRE(post_nms_top_n > 0 && post_nms_top_n <= 2048, "frcnn_proposals: post_nms_top_n must be in [1,2048] (got %d)", post_nms_top_n);
-    const long n_all_l = (long)A * H * W;
-    FRCNN_REQUIRE(n_all_l < (1l << 24), "frcnn_proposals: too many anchors (%ld)", n_all_l);
-    const int n_all = (int)n_all_l;
-    const int k_cap = pre_nms_top_n < n_all ? pre_nms_top_n : n_all;
-    NmsWs w = carve(ws, n_all, k_cap);
-    if (ws_bytes < w.total) {
-        set_error("frcnn_proposals: workspace %zu < required %zu", ws_bytes, w.total);
-        return FRCNN_ERR_WORKSPACE;
-    }
-    DecodeArgs da;
-    da.cls = cls; da.cls_cs = cls_chan_stride; da.cls_ps = cls_pix_stride; da.cls_is_logits = cls_is_logits;
-    da.bbox = bbox; da.bbox_cs = bbox_chan_stride; da.bbox_ps = bbox_pix_stride;
-    da.anchors = anchors;
-    da.A = A; da.H = H; da.W = W; da.feat_stride = feat_stride; da.im_h = im_h; da.im_w = im_w; da.min_size = min_size;
-    da.boxes = w.boxes; da.scores = w.scores; da.keys = w.keys;
-    FRCNN_CUDA_OK(launch_pdl(rpn_decode_kernel, dim3(cdiv(n_all, 128)), dim3(128), 0, stream, da));
-    return run_sort_nms(w, n_all, pre_nms_top_n, nms_thresh, FRCNN_NMS_GE_DOUBLE, post_nms_top_n, nullptr, out_count,
-                        out_rois, out_scores, post_nms_top_n, dbg_sorted_dets, dbg_sorted_anchor_idx, dbg_num_sorted,
-                        false, stream);
+    const OutStrides os = {0, 0, 0, 0, 0, 0};
+    return proposals_n("frcnn_proposals", 1, cls, cls_chan_stride, cls_pix_stride, 0, cls_is_logits, bbox, bbox_chan_stride,
+                       bbox_pix_stride, 0, anchors, A, H, W, feat_stride, im_h, im_w, min_size, pre_nms_top_n, post_nms_top_n,
+                       nms_thresh, out_rois, out_scores, out_count, dbg_sorted_dets, dbg_sorted_anchor_idx, dbg_num_sorted, os, ws,
+                       ws_bytes, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int frcnn_proposals_batch(int N, const float* cls, long cls_chan_stride, long cls_pix_stride, long cls_image_stride,
+                                     int cls_is_logits, const float* bbox, long bbox_chan_stride, long bbox_pix_stride,
+                                     long bbox_image_stride, const double* anchors, int A, int H, int W, int feat_stride, int im_h,
+                                     int im_w, int min_size, int pre_nms_top_n, int post_nms_top_n, double nms_thresh,
+                                     float* out_rois, long rois_image_stride, float* out_scores, long scores_image_stride,
+                                     int* out_count, long count_image_stride, float* dbg_sorted_dets, long dbg_dets_image_stride,
+                                     int* dbg_sorted_anchor_idx, long dbg_idx_image_stride, int* dbg_num_sorted,
+                                     long dbg_num_image_stride, void* ws, size_t ws_bytes, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "frcnn_proposals_batch: N must be in [1,65535] (got %d)", N);
+    const OutStrides os = {rois_image_stride, scores_image_stride, count_image_stride, dbg_dets_image_stride, dbg_idx_image_stride,
+                           dbg_num_image_stride};
+    return proposals_n("frcnn_proposals_batch", N, cls, cls_chan_stride, cls_pix_stride, cls_image_stride, cls_is_logits, bbox,
+                       bbox_chan_stride, bbox_pix_stride, bbox_image_stride, anchors, A, H, W, feat_stride, im_h, im_w, min_size,
+                       pre_nms_top_n, post_nms_top_n, nms_thresh, out_rois, out_scores, out_count, dbg_sorted_dets,
+                       dbg_sorted_anchor_idx, dbg_num_sorted, os, ws, ws_bytes, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" size_t frcnn_nms_workspace_bytes(int n) {
@@ -626,7 +737,8 @@ extern "C" int frcnn_nms(const float* dets, int n, double thresh, int mode, int 
         return FRCNN_ERR_WORKSPACE;
     }
     FRCNN_CUDA_OK(launch_pdl(dets_keys_kernel, dim3(cdiv(n, 256)), dim3(256), 0, stream, dets, n, w.boxes, w.scores, w.keys));
-    return run_sort_nms(w, n, n, thresh, mode, max_keep, keep_out, num_out, nullptr, nullptr, 0, nullptr, nullptr,
+    const OutStrides os = {0, 0, 0, 0, 0, 0};
+    return run_sort_nms(w, 1, 0, os, n, n, thresh, mode, max_keep, keep_out, num_out, nullptr, nullptr, 0, nullptr, nullptr,
                         nullptr, true, stream);
 }
 

@@ -124,6 +124,21 @@ SIGNATURES = {
     "frcnn_forward_vgg16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
     "frcnn_debug_sort_clocks": (None, [c_void_p]),
+    "frcnn_proposals_batch_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "frcnn_proposals_batch": (c_int, [c_int, c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_long, c_long, c_long, c_void_p,
+                                      c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double,
+                                      c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long,
+                                      c_void_p, c_long, c_void_p, c_size_t, c_void_p]),
+    "frcnn_maxpool2x2_ceil_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "frcnn_roi_pool_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_long, c_int, c_int,
+                                     c_int, c_float, c_void_p, c_void_p, c_void_p, c_long, c_void_p]),
+    "frcnn_head_decode_batch": (c_int, [c_int, c_void_p, c_void_p, c_int, c_long, c_void_p, c_long, c_void_p, c_long, c_int, c_int,
+                                        c_int, c_int, c_void_p, c_long, c_void_p, c_long, c_void_p]),
+    "frcnn_detect_batch": (c_int, [c_int, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_int, c_int, c_double, c_float,
+                                   c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p]),
+    "frcnn_forward_batch_workspace_bytes": (c_size_t, [c_void_p, c_int]),
+    "frcnn_forward_vgg16_batch": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p,
+                                          c_void_p, c_void_p]),
     "frcnn_detect": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double, c_float, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
 }

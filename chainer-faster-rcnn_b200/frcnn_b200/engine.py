@@ -343,11 +343,14 @@ def _launch(plan):
 class BatchPlan(object):
     """Buffers + launch sequence for N images of one shape (VGG16 trunk), all in ONE CUDA graph.
 
-    The trunk, the RPN convolutions and the fc6 / fc7 / head GEMMs each run once over all N images (frcnn_conv2d_batch,
-    frcnn_conv3x3_c8_batch, frcnn_linear_batch: the one-image plan with N times the tiles); ProposalLayer, RoI pooling,
-    the head decode and the per-class NMS run once per image at pointer offsets.  Every image's results are bit-identical
-    to a ForwardPlan's on that image.  The result buffer holds N consecutive blocks in ForwardPlan's layout, so the host
-    gets everything with one D2H.  Takes ForwardPlan's keyword options."""
+    Every stage runs once over all N images: the trunk, the RPN convolutions and the fc6 / fc7 / head GEMMs
+    (frcnn_conv2d_batch, frcnn_conv3x3_c8_batch, frcnn_linear_batch: the one-image plan with N times the tiles), and
+    ProposalLayer, RoI pooling, the head decode, the per-class NMS and the stand-alone max-pools (frcnn_proposals_batch,
+    frcnn_roi_pool_batch, frcnn_head_decode_batch, frcnn_detect_batch, frcnn_maxpool2x2_ceil_batch: the image is a grid
+    dimension), so the number of launches does not grow with N.  Every image's results are bit-identical to a
+    ForwardPlan's on that image.  The result buffer holds N consecutive blocks in ForwardPlan's layout, so the host gets
+    everything with one D2H; the batched post-processing reads and writes those blocks in place at a stride of one block.
+    Takes ForwardPlan's keyword options."""
 
     def __init__(self, weights, N, H, W, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
                  anchors=None, with_detect=False, det_nms_thresh=0.3, det_conf=0.8, use_graph=True, keep_rpn_debug=False,
@@ -408,24 +411,22 @@ class BatchPlan(object):
         self.head_out = torch.empty((N, self.ld1, weights.head_ld), dtype=torch.float32, device=dev)
         self.fc_work = max((ops.linear_batch_workspace(N, post_n, k_, c_, dev) for k_, c_ in
                             ((49 * C, 4096), (4096, 4096), (4096, 5 * NC))), key=lambda t: t.numel())
-        self.images = []
-        for n in range(N):
-            blk = self.result[n * self.block_words:(n + 1) * self.block_words]
-            rf = blk.view(torch.float32)
-            seg = lambda t, name: t[self.result_layout[name][0]: self.result_layout[name][0] + self.result_layout[name][1]]   # noqa: E731
-            prop = ops.ProposalWorkspace(A, h, w_, pre_n, post_n, dev, debug=keep_rpn_debug,
-                                         outputs=(seg(rf, "rois").view(post_n, 4), seg(rf, "scores"), seg(blk, "count")[:1]))
-            self.images.append(dict(prop=prop, prob=seg(rf, "prob").view(post_n, NC), boxes=seg(rf, "boxes").view(post_n, 4 * NC),
-                                    det=(seg(blk, "keep_idx").view(NC - 1, post_n), seg(blk, "keep_count"), seg(blk, "conf_count"))))
+        # every per-image result as ONE [N, ...] view of the N blocks (image stride = block_words): the batched entries
+        # write straight into the blocks
+        blocks = self.result.view(N, self.block_words)
+        seg = lambda t, name: t[:, self.result_layout[name][0]: self.result_layout[name][0] + self.result_layout[name][1]]   # noqa: E731
+        bf = blocks.view(torch.float32)
+        self.prop = ops.ProposalBatchWorkspace(N, A, h, w_, pre_n, post_n, dev, debug=keep_rpn_debug,
+                                               outputs=(seg(bf, "rois").view(N, post_n, 4), seg(bf, "scores"), seg(blocks, "count")[:, 0]))
+        self.prob = seg(bf, "prob").view(N, post_n, NC)
+        self.boxes = seg(bf, "boxes").view(N, post_n, 4 * NC)
+        self.det = (seg(blocks, "keep_idx").view(N, NC - 1, post_n), seg(blocks, "keep_count"), seg(blocks, "conf_count"))
+        self.images = [dict(prob=self.prob[n], boxes=self.boxes[n], det=tuple(t[n] for t in self.det)) for n in range(N)]
         self._host = None
         self.graph = None
         self.use_graph = use_graph
         self.im_h, self.im_w = H, W
         self.n_launches = 0
-
-    @staticmethod
-    def _image(a, n):
-        return ops.Act(a.hi[n], None if a.lo is None else a.lo[n])
 
     def _run(self):
         w, N, post_n = self.w, self.N, self.post_n
@@ -441,9 +442,8 @@ class BatchPlan(object):
             n += 1
             i += 1
             if pool_after:
-                for k in range(N):
-                    ops.maxpool2x2_ceil(self._image(self.acts[i], k), out=self._image(self.acts[i + 1], k))
-                n += N
+                ops.maxpool2x2_ceil_batch(self.acts[i], out=self.acts[i + 1])
+                n += 1
                 i += 1
         feat = self.feat = self.acts[-1]
         hi, lo, b = w.rpn3
@@ -451,15 +451,13 @@ class BatchPlan(object):
         hi, lo, b = w.rpn_heads
         ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out)
         n += 2
-        hw = self.fh * self.fw
-        for k, im in enumerate(self.images):
-            ops.proposals(self.rpn_out[k * hw:(k + 1) * hw], None, self.anchors, w.n_anchors, self.fh, self.fw, self.feat_stride,
-                          self.im_h, self.im_w, self.min_size, self.pre_n, post_n, self.nms_thresh,
-                          layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=im["prop"], debug=im["prop"].dbg_dets is not None)
-            p5 = self.pool5
-            ops.roi_pool(self._image(feat, k), im["prop"].rois, im["prop"].count, 7, 7, 1.0 / self.feat_stride,
-                         out=ops.Act(p5.hi[k, :post_n], None if p5.lo is None else p5.lo[k, :post_n]))
-            n += 5 + 1
+        ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, w.rpn_ld), None, self.anchors, w.n_anchors, self.fh, self.fw,
+                            self.feat_stride, self.im_h, self.im_w, self.min_size, self.pre_n, post_n, self.nms_thresh,
+                            layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=self.prop, debug=self.prop.dbg_dets is not None)
+        p5 = self.pool5
+        ops.roi_pool_batch(feat, self.prop.rois, self.prop.count, 7, 7, 1.0 / self.feat_stride,
+                           out=ops.Act(p5.hi[:, :post_n], None if p5.lo is None else p5.lo[:, :post_n]))
+        n += 5 + 1          # decode, select, rank/scatter, IoU mask, mask scan; RoI pool
         cnt, bw = self.counts, self.block_words
         hi, lo, b = w.fc6
         ops.linear_batch(self.pool5, hi, lo, b, True, post_n, counts=cnt, count_stride=bw, out=self.fc6, work=self.fc_work)
@@ -469,13 +467,12 @@ class BatchPlan(object):
         ops.linear_batch(self.fc7, hi, lo, b, False, post_n, counts=cnt, count_stride=bw, out_f32=self.head_out,
                          ld_f32=w.head_ld, work=self.fc_work, want_act=False)
         n += 3 * 2
-        for k, im in enumerate(self.images):
-            ops.head_decode(self.head_out[k, :post_n], w.head_ld, im["prop"].rois, im["prop"].count, w.num_classes,
-                            self.im_h, self.im_w, out_prob=im["prob"], out_boxes=im["boxes"])
-            n += 5
-            if self.with_detect:
-                ops.detect(im["prob"], im["boxes"], im["prop"].count, self.det_nms_thresh, self.det_conf, out=im["det"])
-                n += 1
+        ops.head_decode_batch(self.head_out[:, :post_n], w.head_ld, self.prop.rois, self.prop.count, w.num_classes,
+                              self.im_h, self.im_w, out_prob=self.prob, out_boxes=self.boxes)
+        n += 1
+        if self.with_detect:
+            ops.detect_batch(self.prob, self.boxes, self.prop.count, self.det_nms_thresh, self.det_conf, out=self.det)
+            n += 1
         self.n_launches = n
 
     def clone(self):
@@ -761,14 +758,16 @@ class Engine(object):
 
 class CForward(object):
     """frcnn_forward_vgg16: the whole forward path behind the single C-ABI entry (include/frcnn_b200.h) -- what a caller
-    without Python binds.  Same kernels, same order as ForwardPlan._run; this wrapper only fills the C structs from a
-    PackedWeights and owns the workspace / output tensors."""
+    without Python binds.  Same kernels, same order as BatchPlan._run; this wrapper only fills the C structs from a
+    PackedWeights and owns the workspace / output tensors.  N > 1: frcnn_forward_vgg16_batch over N images per call."""
 
-    def __init__(self, weights, H, W, anchors, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16):
+    def __init__(self, weights, H, W, anchors, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16, N=1):
         import ctypes
         from . import _lib
+        if int(N) != N or N < 1:
+            raise FrcnnError("CForward needs N >= 1 images (got %r)" % (N,))
         self._lib, self._ct = _lib.load(), ctypes
-        self.w, self.H, self.W, self.post_n = weights, H, W, post_n
+        self.w, self.H, self.W, self.post_n, self.N = weights, H, W, post_n, int(N)
         dev = weights.device
         self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
         cfg = _lib.ForwardConfig(H, W, weights.num_classes, weights.n_anchors, feat_stride, pre_n, post_n, min_size,
@@ -782,22 +781,34 @@ class CForward(object):
         wt.fc6, wt.fc7, wt.head = layer(*weights.fc6), layer(*weights.fc7), layer(*weights.head)
         wt.anchors = self.anchors.data_ptr()
         self.cfg, self.wt = cfg, wt
-        nbytes = self._lib.frcnn_forward_workspace_bytes(ctypes.byref(cfg))
+        if self.N == 1:
+            nbytes = self._lib.frcnn_forward_workspace_bytes(ctypes.byref(cfg))
+        else:
+            nbytes = self._lib.frcnn_forward_batch_workspace_bytes(ctypes.byref(cfg), self.N)
         if nbytes == 0:
             raise FrcnnError("frcnn_forward_workspace_bytes: %s" % _lib.last_error())
         self.ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
-        self.prob = torch.empty((post_n, weights.num_classes), dtype=torch.float32, device=dev)
-        self.boxes = torch.empty((post_n, 4 * weights.num_classes), dtype=torch.float32, device=dev)
-        self.count = torch.zeros((1,), dtype=torch.int32, device=dev)
+        lead = () if self.N == 1 else (self.N,)
+        self.prob = torch.empty(lead + (post_n, weights.num_classes), dtype=torch.float32, device=dev)
+        self.boxes = torch.empty(lead + (post_n, 4 * weights.num_classes), dtype=torch.float32, device=dev)
+        self.count = torch.zeros((self.N,), dtype=torch.int32, device=dev)
 
-    def forward(self, x_chw, im_info=None):
-        """x_chw (3,H,W) float32 CUDA.  Returns (prob, boxes, count) device tensors (rows past count are zero)."""
+    def forward(self, x, im_info=None):
+        """x: (3,H,W) float32 CUDA for N = 1, (N,3,H,W) otherwise.  Returns (prob, boxes, count) device tensors
+        ([N, ...] for N > 1; rows past an image's count are zero)."""
         from . import _lib
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
-        x = x_chw.contiguous().float()
+        want = (3, self.H, self.W) if self.N == 1 else (self.N, 3, self.H, self.W)
+        if tuple(x.shape) != want:
+            raise FrcnnError("CForward: input of shape %s, expected %s" % (tuple(x.shape), want))
+        x = x.contiguous().float()
         ct = self._ct
-        _lib.check(self._lib.frcnn_forward_vgg16(ct.byref(self.cfg), ct.byref(self.wt), ct.c_void_p(x.data_ptr()), im_h, im_w,
-                                                 ct.c_void_p(self.ws.data_ptr()), self.ws.numel(), ct.c_void_p(self.prob.data_ptr()),
-                                                 ct.c_void_p(self.boxes.data_ptr()), ct.c_void_p(self.count.data_ptr()),
-                                                 ct.c_void_p(torch.cuda.current_stream().cuda_stream)), "frcnn_forward_vgg16")
+        args = (ct.c_void_p(x.data_ptr()), im_h, im_w, ct.c_void_p(self.ws.data_ptr()), self.ws.numel(),
+                ct.c_void_p(self.prob.data_ptr()), ct.c_void_p(self.boxes.data_ptr()), ct.c_void_p(self.count.data_ptr()),
+                ct.c_void_p(torch.cuda.current_stream().cuda_stream))
+        if self.N == 1:
+            _lib.check(self._lib.frcnn_forward_vgg16(ct.byref(self.cfg), ct.byref(self.wt), *args), "frcnn_forward_vgg16")
+        else:
+            _lib.check(self._lib.frcnn_forward_vgg16_batch(ct.byref(self.cfg), ct.byref(self.wt), self.N, *args),
+                       "frcnn_forward_vgg16_batch")
         return self.prob, self.boxes, self.count

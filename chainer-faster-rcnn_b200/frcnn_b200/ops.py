@@ -582,6 +582,182 @@ def proposals(cls, bbox, anchors, A, H, W, feat_stride, im_h, im_w, min_size, pr
     return work
 
 
+# ---- batched post-processing: N images in one launch per kernel.  Every per-image array is a tensor whose dim 0 is the
+# image: each image's block must be dense, the blocks may sit any distance apart (e.g. views of BatchPlan's result blocks),
+# and that distance -- the tensor's stride(0) -- is the image stride handed to the library.
+def _image_stride(t, inner, what):
+    """t: [N, *inner] with each image's block dense (row-major); returns the image stride in elements."""
+    if t is None:
+        return 0
+    _need_cuda(t)
+    if tuple(t.shape[1:]) != tuple(inner):
+        raise FrcnnError("%s: per-image shape %s, expected %s" % (what, tuple(t.shape[1:]), tuple(inner)))
+    want = 1
+    for d, st in zip(reversed(inner), reversed(t.stride()[1:])):
+        if d > 1 and st != want:
+            raise FrcnnError("%s: each image's block must be dense (strides %s)" % (what, tuple(t.stride())))
+        want *= d
+    return int(t.stride(0))
+
+
+def _counts_stride(counts, N, what):
+    """counts: None (R_cap each) or an int32 tensor whose dim 0 is the image (e.g. one word of every result block)."""
+    if counts is None:
+        return 0
+    _need_cuda(counts)
+    if counts.dtype != torch.int32 or counts.shape[0] != N:
+        raise FrcnnError("%s: counts must be int32 with one entry per image" % what)
+    return int(counts.stride(0))
+
+
+def maxpool2x2_ceil_batch(x, out=None):
+    """frcnn_maxpool2x2_ceil_batch: Act [N,H,W,C] -> Act [N,ceil(H/2),ceil(W/2),C], one launch."""
+    N, H, W, C = x.hi.shape
+    if out is None:
+        yh = torch.empty((N, (H + 1) // 2, (W + 1) // 2, C), dtype=torch.bfloat16, device=x.hi.device)
+        out = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    for t in (x.hi, x.lo, out.hi, out.lo):
+        if t is not None and not t.is_contiguous():
+            raise FrcnnError("maxpool2x2_ceil_batch: planes must be dense [N,H,W,C]")
+    check(_lib.load().frcnn_maxpool2x2_ceil_batch(_p(x.hi), _p(x.lo), N, H, W, C, _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_maxpool2x2_ceil_batch")
+    return out
+
+
+def roi_pool_batch(feat, rois, counts=None, outh=7, outw=7, scale=1.0 / 16, want_f32=False, out=None, out_f32=None):
+    """frcnn_roi_pool_batch: feat Act [N,H,W,C] (dense); rois [N,R_cap,4]; counts [N] int32 (or None).  Returns (Act
+    [N,R_cap,outh*outw*C], fp32 [N,R_cap,outh*outw,C] or None).  `out` / `out_f32` may be strided views (image blocks
+    apart); the library takes one image stride for all outputs, so given both, their strides must agree."""
+    N, H, W, C = feat.hi.shape
+    R_cap = rois.shape[1]
+    K = outh * outw * C
+    if not feat.hi.is_contiguous() or (feat.lo is not None and not feat.lo.is_contiguous()):
+        raise FrcnnError("roi_pool_batch: feature planes must be dense [N,H,W,C]")
+    rs = _image_stride(rois, (R_cap, 4), "roi_pool_batch rois")
+    cs = _counts_stride(counts, N, "roi_pool_batch")
+    if out is None:
+        oh = torch.empty((N, R_cap, K), dtype=torch.bfloat16, device=rois.device)
+        out = Act(oh, torch.empty_like(oh) if feat.lo is not None else None)
+    os_ = _image_stride(out.hi, (R_cap, K), "roi_pool_batch out")
+    if out.lo is not None and _image_stride(out.lo, (R_cap, K), "roi_pool_batch out") != os_:
+        raise FrcnnError("roi_pool_batch: hi and lo outputs need the same image stride")
+    o32 = out_f32
+    if want_f32 and o32 is None:          # image blocks as far apart as the bf16 output's
+        o32 = torch.empty((N, os_), dtype=torch.float32, device=rois.device)[:, :K].view(N, R_cap, outh * outw, C)
+    if o32 is not None and _image_stride(o32, (R_cap, outh * outw, C), "roi_pool_batch out_f32") != os_ and N > 1:
+        raise FrcnnError("roi_pool_batch: the bf16 and fp32 outputs need the same image stride")
+    check(_lib.load().frcnn_roi_pool_batch(_p(feat.hi), _p(feat.lo), N, H, W, C, _p(rois), rs, _p(counts), cs, R_cap, outh, outw,
+                                           ctypes.c_float(scale), _p(out.hi), _p(out.lo), _p(o32), os_, _stream()),
+          "frcnn_roi_pool_batch")
+    return out, o32
+
+
+def head_decode_batch(scores_deltas, ld, rois, counts, num_classes, im_h, im_w, out_prob=None, out_boxes=None):
+    """frcnn_head_decode_batch: scores_deltas fp32 [N,R_cap,ld] (columns [0,NC) scores, [NC,5NC) deltas), rois [N,R_cap,4],
+    counts [N] int32 or None; out_prob [N,R_cap,NC], out_boxes [N,R_cap,4NC] (may be strided views)."""
+    N, R_cap = rois.shape[0], rois.shape[1]
+    dev = rois.device
+    if out_prob is None:
+        out_prob = torch.empty((N, R_cap, num_classes), dtype=torch.float32, device=dev)
+    if out_boxes is None:
+        out_boxes = torch.empty((N, R_cap, 4 * num_classes), dtype=torch.float32, device=dev)
+    ins = _image_stride(scores_deltas, (R_cap, ld), "head_decode_batch scores")
+    rs = _image_stride(rois, (R_cap, 4), "head_decode_batch rois")
+    cs = _counts_stride(counts, N, "head_decode_batch")
+    ps = _image_stride(out_prob, (R_cap, num_classes), "head_decode_batch out_prob")
+    bs = _image_stride(out_boxes, (R_cap, 4 * num_classes), "head_decode_batch out_boxes")
+    deltas_ptr = ctypes.c_void_p(scores_deltas.data_ptr() + 4 * num_classes)
+    check(_lib.load().frcnn_head_decode_batch(N, _p(scores_deltas), deltas_ptr, ld, ins, _p(rois), rs, _p(counts), cs, R_cap, num_classes,
+                                              int(im_h), int(im_w), _p(out_prob), ps, _p(out_boxes), bs, _stream()),
+          "frcnn_head_decode_batch")
+    return out_prob, out_boxes
+
+
+def detect_batch(prob, boxes, counts=None, nms_thresh=0.3, conf=0.8, out=None):
+    """frcnn_detect_batch: prob [N,R_cap,NC], boxes [N,R_cap,4NC], counts [N] int32 or None.  out: optional (keep_idx
+    [N,NC-1,R_cap], keep_count [N,NC-1], conf_count [N,NC-1]) int32, possibly strided views."""
+    N, R_cap, NC = prob.shape
+    dev = prob.device
+    if out is not None:
+        keep_idx, keep_count, conf_count = out
+    else:
+        keep_idx = torch.empty((N, NC - 1, R_cap), dtype=torch.int32, device=dev)
+        keep_count = torch.empty((N, NC - 1), dtype=torch.int32, device=dev)
+        conf_count = torch.empty((N, NC - 1), dtype=torch.int32, device=dev)
+    ps = _image_stride(prob, (R_cap, NC), "detect_batch prob")
+    bs = _image_stride(boxes, (R_cap, 4 * NC), "detect_batch boxes")
+    cs = _counts_stride(counts, N, "detect_batch")
+    ks = _image_stride(keep_idx, (NC - 1, R_cap), "detect_batch keep_idx")
+    kc = _image_stride(keep_count, (NC - 1,), "detect_batch keep_count")
+    cc = _image_stride(conf_count, (NC - 1,), "detect_batch conf_count")
+    check(_lib.load().frcnn_detect_batch(N, _p(prob), ps, _p(boxes), bs, _p(counts), cs, R_cap, NC, float(nms_thresh),
+                                         ctypes.c_float(conf), _p(keep_idx), ks, _p(keep_count), kc, _p(conf_count), cc, _stream()),
+          "frcnn_detect_batch")
+    return keep_idx, keep_count, conf_count
+
+
+class ProposalBatchWorkspace(object):
+    """Scratch + outputs of frcnn_proposals_batch for N images of one (A,H,W,pre,post) shape: N workspace slices in one
+    buffer, rois [N,post_n,4], scores [N,post_n], count [N] int32 and, with debug, dbg_dets [N,k,5], dbg_idx [N,k],
+    dbg_num [N] (k = min(pre_n, A*H*W))."""
+
+    def __init__(self, N, A, H, W, pre_n, post_n, device, debug=False, outputs=None):
+        """outputs: optional pre-allocated (rois [N,post_n,4], scores [N,post_n], count [N]) -- e.g. strided views of N result
+        blocks."""
+        lib = _lib.load()
+        self.N, self.shape = int(N), (A, H, W, pre_n, post_n)
+        nbytes = lib.frcnn_proposals_batch_workspace_bytes(int(N), A, H, W, pre_n)
+        if nbytes == 0:
+            raise FrcnnError("frcnn_proposals_batch_workspace_bytes: bad shape N=%r A=%d H=%d W=%d pre=%d" % (N, A, H, W, pre_n))
+        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        if outputs is not None:
+            self.rois, self.scores, self.count = outputs
+        else:
+            self.rois = torch.zeros((N, post_n, 4), dtype=torch.float32, device=device)
+            self.scores = torch.zeros((N, post_n), dtype=torch.float32, device=device)
+            self.count = torch.zeros((N,), dtype=torch.int32, device=device)
+        k_cap = min(pre_n, A * H * W)
+        self.dbg_dets = torch.zeros((N, k_cap, 5), dtype=torch.float32, device=device) if debug else None
+        self.dbg_idx = torch.zeros((N, k_cap), dtype=torch.int32, device=device) if debug else None
+        self.dbg_num = torch.zeros((N,), dtype=torch.int32, device=device) if debug else None
+
+
+def proposals_batch(cls, bbox, anchors, A, H, W, feat_stride, im_h, im_w, min_size, pre_n, post_n, nms_thresh,
+                    layout="nchw", ld=0, cls_is_logits=False, work=None, debug=False):
+    """frcnn_proposals_batch over N images (one clip bound for all).  layout "nchw": cls (N,2A,H,W), bbox (N,4A,H,W) planar;
+    layout "nhwc": cls one fp32 tensor [N,H*W,ld] with cls in columns [0,2A) and bbox in [2A,6A) (bbox None).  Returns the
+    ProposalBatchWorkspace holding the outputs."""
+    _need_cuda(cls)
+    N = cls.shape[0]
+    dev = cls.device
+    if work is None or work.N != N or work.shape != (A, H, W, pre_n, post_n) or (debug and work.dbg_dets is None):
+        work = ProposalBatchWorkspace(N, A, H, W, pre_n, post_n, dev, debug)
+    if layout == "nchw":
+        cs, ps, bcs, bps = H * W, 1, H * W, 1
+        cis = _image_stride(cls, (2 * A, H, W), "proposals_batch cls")
+        bis = _image_stride(bbox, (4 * A, H, W), "proposals_batch bbox")
+        bbox_ptr = _p(bbox)
+    else:
+        cs, ps, bcs, bps = 1, ld, 1, ld
+        cis = _image_stride(cls, (H * W, ld), "proposals_batch cls")
+        bis = cis if bbox is None else _image_stride(bbox, (H * W, ld), "proposals_batch bbox")
+        bbox_ptr = ctypes.c_void_p(cls.data_ptr() + 4 * 2 * A) if bbox is None else _p(bbox)
+    k_cap = min(pre_n, A * H * W)
+    rs = _image_stride(work.rois, (post_n, 4), "proposals_batch rois")
+    ss = _image_stride(work.scores, (post_n,), "proposals_batch scores")
+    cnt = _counts_stride(work.count, N, "proposals_batch")
+    dd = _image_stride(work.dbg_dets, (k_cap, 5), "proposals_batch dbg_dets") if debug else 0
+    di = _image_stride(work.dbg_idx, (k_cap,), "proposals_batch dbg_idx") if debug else 0
+    dn = _counts_stride(work.dbg_num, N, "proposals_batch dbg_num") if debug else 0
+    check(_lib.load().frcnn_proposals_batch(N, _p(cls), cs, ps, cis, 1 if cls_is_logits else 0, bbox_ptr, bcs, bps, bis, _p(anchors),
+                                            A, H, W, feat_stride, int(im_h), int(im_w), int(min_size), pre_n, post_n,
+                                            float(nms_thresh), _p(work.rois), rs, _p(work.scores), ss, _p(work.count), cnt,
+                                            _p(work.dbg_dets) if debug else None, dd, _p(work.dbg_idx) if debug else None, di,
+                                            _p(work.dbg_num) if debug else None, dn, _p(work.ws), work.ws.numel(), _stream()),
+          "frcnn_proposals_batch")
+    return work
+
+
 def nms(dets, thresh, mode=_lib.NMS_GE_DOUBLE, max_keep=0):
     """Device greedy NMS over unsorted dets [n,5] (CUDA fp32).  Returns (keep int32[n], count int32[1])."""
     _need_cuda(dets)

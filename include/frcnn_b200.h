@@ -102,6 +102,25 @@ int frcnn_proposals(const float* cls, long cls_chan_stride, long cls_pix_stride,
                     int pre_nms_top_n, int post_nms_top_n, double nms_thresh, float* out_rois,
                     float* out_scores, int* out_count, float* dbg_sorted_dets, int* dbg_sorted_anchor_idx,
                     int* dbg_num_sorted, void* ws, size_t ws_bytes, void* stream);
+/* frcnn_proposals over N same-size images in one launch per kernel (five launches for the whole batch).  Image n reads
+ * cls + n*cls_image_stride and bbox + n*bbox_image_stride (floats) and writes out_rois + n*rois_image_stride,
+ * out_scores + n*scores_image_stride, out_count + n*count_image_stride and the optional debug outputs at their image
+ * strides (elements): dense [N][post][4] arrays and result blocks some words apart both fit.  The anchors and the clip
+ * bounds (im_h, im_w) are shared by all images.  Each image's scratch is its own slice of `ws`
+ * (frcnn_proposals_batch_workspace_bytes = N slices at a 256-byte-aligned stride).  Every image's outputs are
+ * bit-identical to frcnn_proposals on that image.  frcnn_debug_sort_clocks records image 0 only.
+ * Errors: N outside [1,65535], a NULL required pointer, or (N > 1) an output stride smaller than one image's output
+ * (rois: 4*post_nms_top_n, a multiple of 4; scores: post_nms_top_n; count: 1; dbg dets: 5*k, dbg index: k with
+ * k = min(pre_nms_top_n, A*H*W)) -> FRCNN_ERR_ARG; a workspace below the query -> FRCNN_ERR_WORKSPACE. */
+size_t frcnn_proposals_batch_workspace_bytes(int N, int A, int H, int W, int pre_nms_top_n);
+int frcnn_proposals_batch(int N, const float* cls, long cls_chan_stride, long cls_pix_stride, long cls_image_stride,
+                          int cls_is_logits, const float* bbox, long bbox_chan_stride, long bbox_pix_stride,
+                          long bbox_image_stride, const double* anchors, int A, int H, int W, int feat_stride, int im_h,
+                          int im_w, int min_size, int pre_nms_top_n, int post_nms_top_n, double nms_thresh,
+                          float* out_rois, long rois_image_stride, float* out_scores, long scores_image_stride,
+                          int* out_count, long count_image_stride, float* dbg_sorted_dets, long dbg_dets_image_stride,
+                          int* dbg_sorted_anchor_idx, long dbg_idx_image_stride, int* dbg_num_sorted,
+                          long dbg_num_image_stride, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Dense contraction on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue):
@@ -229,6 +248,9 @@ int frcnn_unpack_nhwc(const void* x_hi, const void* x_lo, int H, int W, int C, f
  * [H,W,C] -> [ceil(H/2),ceil(W/2),C], C % 8 == 0. */
 int frcnn_maxpool2x2_ceil(const void* x_hi, const void* x_lo, int H, int W, int C, void* y_hi, void* y_lo,
                           void* stream);
+/* The same over a batch in one launch: [N,H,W,C] -> [N,ceil(H/2),ceil(W/2),C], 1 <= N <= 65535. */
+int frcnn_maxpool2x2_ceil_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo,
+                                void* stream);
 
 /* F.roi_pooling_2d(feature_map, [0|rois], outh, outw, scale) (models/faster_rcnn.py:123-126), Caffe
  * semantics.  feat [H,W,C] bf16 hi(/lo); rois [R_cap,4] fp32; *count valid rows (NULL = R_cap).
@@ -237,6 +259,13 @@ int frcnn_maxpool2x2_ceil(const void* x_hi, const void* x_lo, int H, int W, int 
 int frcnn_roi_pool(const void* feat_hi, const void* feat_lo, int H, int W, int C, const float* rois,
                    const int* count, int R_cap, int outh, int outw, float scale, void* out_hi, void* out_lo,
                    float* out_f32, void* stream);
+/* frcnn_roi_pool over N images in one launch: feat [N,H,W,C]; image n's RoIs at rois + n*rois_stride (floats, a multiple
+ * of 4), its count at counts[n*count_stride] (counts NULL = R_cap each), its output rows at n*out_stride elements into
+ * out_hi / out_lo / out_f32 (out_stride >= R_cap*outh*outw*C and a multiple of 8 when N > 1).  Each image's rows are
+ * bit-identical to frcnn_roi_pool on it. */
+int frcnn_roi_pool_batch(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                         long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale,
+                         void* out_hi, void* out_lo, float* out_f32, long out_stride, void* stream);
 
 /* L.Linear (+ F.relu) for a small number of rows: fc6 / fc7 / cls_score|bbox_pred over the R <= post_nms_top_n RoIs
  * (models/faster_rcnn.py:33-36,127-134).  y[r, c] = act(sum_k x[r,k] * w[c,k] + bias[c]) for r < R_cap, c < Cout.
@@ -266,6 +295,13 @@ int frcnn_linear_batch(const void* x_hi, const void* x_lo, int N, int R_cap, int
 int frcnn_head_decode(const float* scores, const float* deltas, int ld, const float* rois, const int* count,
                       int R_cap, int num_classes, int im_h, int im_w, float* out_prob, float* out_boxes,
                       void* stream);
+/* frcnn_head_decode over N images in one launch.  Image n: scores / deltas rows at n*in_stride floats on, rois at
+ * n*rois_stride (a multiple of 4), count at counts[n*count_stride] (NULL = R_cap), out_prob at n*prob_stride
+ * (>= R_cap*num_classes), out_boxes at n*boxes_stride (>= 4*R_cap*num_classes, a multiple of 4).  One clip bound for all.
+ * Each image's outputs are bit-identical to frcnn_head_decode on it. */
+int frcnn_head_decode_batch(int N, const float* scores, const float* deltas, int ld, long in_stride, const float* rois,
+                            long rois_stride, const int* counts, long count_stride, int R_cap, int num_classes, int im_h,
+                            int im_w, float* out_prob, long prob_stride, float* out_boxes, long boxes_stride, void* stream);
 
 /* Stand-alone box algebra, the array-level helpers of models/bbox_transform.py:
  *   out[n, 4k..4k+3] = bbox_transform_inv(boxes[n], trans[n, 4k..4k+3])   (:41-76), k < K
@@ -283,6 +319,14 @@ int frcnn_bbox_decode(const float* boxes, const float* trans, int N, int K, int 
  * R_cap <= 2048. */
 int frcnn_detect(const float* prob, const float* boxes, const int* count, int R_cap, int num_classes,
                  double nms_thresh, float conf, int* keep_idx, int* keep_count, int* conf_count, void* stream);
+/* frcnn_detect over N images in one launch (grid: num_classes-1 CTAs per image).  Image n reads prob / boxes at
+ * n*prob_stride / n*boxes_stride floats on (boxes: a multiple of 4) and its count at counts[n*count_stride] (NULL = R_cap),
+ * and writes keep_idx, keep_count, conf_count at their image strides (>= (num_classes-1)*R_cap, num_classes-1,
+ * num_classes-1 when N > 1).  Each image's outputs are bit-identical to frcnn_detect on it. */
+int frcnn_detect_batch(int N, const float* prob, long prob_stride, const float* boxes, long boxes_stride, const int* counts,
+                       long count_stride, int R_cap, int num_classes, double nms_thresh, float conf, int* keep_idx,
+                       long keep_idx_stride, int* keep_count, long keep_count_stride, int* conf_count,
+                       long conf_count_stride, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The whole forward path behind one call (forward_graph.cu): FasterRCNN.__call__, inference branch
@@ -319,6 +363,16 @@ size_t frcnn_forward_workspace_bytes(const frcnn_forward_config* config);      /
 int frcnn_forward_vgg16(const frcnn_forward_config* config, const frcnn_vgg16_weights* weights, const float* image_chw,
                         int im_h, int im_w, void* workspace, size_t workspace_bytes, float* out_prob, float* out_boxes,
                         int* out_count, void* stream);
+/* The same forward path over N images of config->H x config->W in one call: every stage is one launch sequence for the
+ * whole batch (frcnn_forward_vgg16 is the case N = 1).  images_nchw: (N,3,H,W) float32 device images; one clip bound
+ * (im_h, im_w) for all.  Outputs: out_prob [N][post_nms_top_n][num_classes], out_boxes [N][post_nms_top_n][4*num_classes],
+ * out_count [N].  Image n's outputs are bit-identical to frcnn_forward_vgg16 on image n.  N outside [1,65535] ->
+ * FRCNN_ERR_ARG (and frcnn_forward_batch_workspace_bytes returns 0); a workspace below
+ * frcnn_forward_batch_workspace_bytes(config, N) -> FRCNN_ERR_WORKSPACE.  Static launch sequence: capturable. */
+size_t frcnn_forward_batch_workspace_bytes(const frcnn_forward_config* config, int N);
+int frcnn_forward_vgg16_batch(const frcnn_forward_config* config, const frcnn_vgg16_weights* weights, int N,
+                              const float* images_nchw, int im_h, int im_w, void* workspace, size_t workspace_bytes,
+                              float* out_prob, float* out_boxes, int* out_count, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * ResNet trunk support (SURVEY.md 8f rank 2; chainer ResNetLayers as used by models/resnet.py:11-45).
@@ -495,7 +549,8 @@ int frcnn_pack_conv_weights_dgrad(const float* w_oihw, int Cout, int Cin, int kh
                                   void* stream);
 
 /* Profiling hook (not part of the drop-in surface): a device buffer of 8 int64 that receives the
- * per-phase clock64() stamps of subsequent top-k sort launches; NULL disables. */
+ * per-phase clock64() stamps of subsequent top-k sort launches; NULL disables.  A batched launch
+ * (frcnn_proposals_batch) records image 0 only. */
 void frcnn_debug_sort_clocks(long long* dev_buf);
 
 #ifdef __cplusplus
