@@ -113,6 +113,14 @@ __device__ __forceinline__ float det_expf(float x) {
     return __fmul_rn(__fmul_rn(p, pow2i(h)), pow2i(ni - h));
 }
 
+// clip_boxes (models/bbox_transform.py:87-98): max(min(v, bound), 0) for one coordinate, the clip of every decode kernel.
+// NumPy's minimum / maximum propagate NaN, CUDA's fminf / fmaxf return the other operand, so NaN is passed through
+// explicitly: a NaN coordinate stays NaN, and its box then fails every min-size test and suppresses nothing, as in the
+// oracle.
+__device__ __forceinline__ float clip_coord(float v, float bound) {
+    return v != v ? v : fmaxf(fminf(v, bound), 0.0f);
+}
+
 // bf16 hi/lo split of an fp32 value: v ~= hi + lo with 16 significant bits ("bf16x3" operands).
 __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(v);

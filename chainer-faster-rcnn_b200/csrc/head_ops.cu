@@ -534,10 +534,10 @@ __global__ void head_decode_kernel(const float* scores, const float* deltas, int
         const float pcx = __fadd_rn(__fmul_rn(d[0], bw), cx), pcy = __fadd_rn(__fmul_rn(d[1], bh), cy);
         const float pw = __fmul_rn(det_expf(d[2]), bw), ph = __fmul_rn(det_expf(d[3]), bh);
         const float wmax = (float)(im_w - 1), hmax = (float)(im_h - 1);
-        box.x = fmaxf(fminf(__fsub_rn(pcx, __fmul_rn(0.5f, pw)), wmax), 0.0f);
-        box.y = fmaxf(fminf(__fsub_rn(pcy, __fmul_rn(0.5f, ph)), hmax), 0.0f);
-        box.z = fmaxf(fminf(__fadd_rn(pcx, __fmul_rn(0.5f, pw)), wmax), 0.0f);
-        box.w = fmaxf(fminf(__fadd_rn(pcy, __fmul_rn(0.5f, ph)), hmax), 0.0f);
+        box.x = clip_coord(__fsub_rn(pcx, __fmul_rn(0.5f, pw)), wmax);
+        box.y = clip_coord(__fsub_rn(pcy, __fmul_rn(0.5f, ph)), hmax);
+        box.z = clip_coord(__fadd_rn(pcx, __fmul_rn(0.5f, pw)), wmax);
+        box.w = clip_coord(__fadd_rn(pcy, __fmul_rn(0.5f, ph)), hmax);
     }
     prob[i] = p;
     reinterpret_cast<float4*>(boxes)[i] = box;
@@ -1057,10 +1057,10 @@ __global__ void bbox_decode_kernel(const float* boxes, const float* trans, int N
     }
     if (clip) {
         const float wmax = (float)(im_w - 1), hmax = (float)(im_h - 1);
-        o.x = fmaxf(fminf(o.x, wmax), 0.0f);
-        o.y = fmaxf(fminf(o.y, hmax), 0.0f);
-        o.z = fmaxf(fminf(o.z, wmax), 0.0f);
-        o.w = fmaxf(fminf(o.w, hmax), 0.0f);
+        o.x = clip_coord(o.x, wmax);
+        o.y = clip_coord(o.y, hmax);
+        o.z = clip_coord(o.z, wmax);
+        o.w = clip_coord(o.w, hmax);
     }
     reinterpret_cast<float4*>(out)[i] = o;
     if (ok_flags) {

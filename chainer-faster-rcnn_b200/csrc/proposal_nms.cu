@@ -103,16 +103,17 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     float y1 = __fsub_rn(pcy, __fmul_rn(0.5f, ph));
     float x2 = __fadd_rn(pcx, __fmul_rn(0.5f, pw));
     float y2 = __fadd_rn(pcy, __fmul_rn(0.5f, ph));
-    // clip_boxes (models/bbox_transform.py:87-98): max(min(v, bound), 0)
+    // clip_boxes (models/bbox_transform.py:87-98)
     const float wmax = (float)(a.im_w - 1), hmax = (float)(a.im_h - 1);
-    x1 = fmaxf(fminf(x1, wmax), 0.0f);
-    y1 = fmaxf(fminf(y1, hmax), 0.0f);
-    x2 = fmaxf(fminf(x2, wmax), 0.0f);
-    y2 = fmaxf(fminf(y2, hmax), 0.0f);
-    // filter_boxes (models/bbox_transform.py:105-108)
+    x1 = clip_coord(x1, wmax);
+    y1 = clip_coord(y1, hmax);
+    x2 = clip_coord(x2, wmax);
+    y2 = clip_coord(y2, hmax);
+    // filter_boxes (models/bbox_transform.py:105-108): the only filter.  A NaN box fails it; a NaN score does not, and
+    // its key 1 ranks the row after every number (nms_math.cuh).
     const float ws = __fadd_rn(__fsub_rn(x2, x1), 1.0f);
     const float hs = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
-    const bool ok = (ws >= (float)a.min_size) && (hs >= (float)a.min_size) && (score == score);
+    const bool ok = (ws >= (float)a.min_size) && (hs >= (float)a.min_size);
 
     ws_at(a.boxes, ws_off)[i] = make_float4(x1, y1, x2, y2);
     ws_at(a.scores, ws_off)[i] = score;
