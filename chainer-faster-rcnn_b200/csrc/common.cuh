@@ -127,4 +127,23 @@ __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bflo
     lo = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
+// The value a split pair stands for in RoI pooling: hi + lo, or hi itself when hi is +-inf or NaN (split_bf16 of +-inf
+// leaves lo = NaN, and inf + NaN would turn an infinite feature into a NaN one).
+__device__ __forceinline__ float pool_pair_value(float hi, float lo) { return isfinite(hi) ? __fadd_rn(hi, lo) : hi; }
+
+// RoI-pooling bins, the one rule of the forward (roi_pool_col_kernel) and the backward (roi_pool_backward_kernel), restated
+// by the oracle's orc_roi_pool and tests/backward_ref.py (DESIGN §2).  A RoI coordinate becomes roundf(coord * scale) in
+// float32, converted to int32 with NaN -> 0 and saturation (cvt.rzi.s32.f32, as Chainer's GPU kernel converts it).  The
+// extent, the bin bounds and the shift by the start are 64-bit integers, then clamped to [0, L]: no step overflows, and a
+// RoI far larger than the map pools the whole map into its first bins.
+__device__ __forceinline__ int roi_coord(float c, float scale) { return __float2int_rz(roundf(__fmul_rn(c, scale))); }
+
+// [x, y) of bin i of P over the scaled RoI extent [s, e] along an axis of L pixels; empty when y <= x.
+__device__ __forceinline__ int2 roi_bin(int s, int e, int P, int i, int L) {
+    const long long ext = max((long long)e - s + 1, 1ll);
+    const float b = __fdiv_rn(__ll2float_rn(ext), (float)P);
+    const long long lo = (long long)floorf(__fmul_rn((float)i, b)) + s, hi = (long long)ceilf(__fmul_rn((float)(i + 1), b)) + s;
+    return make_int2((int)min(max(lo, 0ll), (long long)L), (int)min(max(hi, 0ll), (long long)L));
+}
+
 }  // namespace frcnn

@@ -305,7 +305,9 @@ __global__ void maxpool_kernel(const __nv_bfloat16* xh, const __nv_bfloat16* xl,
 
 // ------------------------------------------------------------------------------------------ RoI max pooling
 // Caffe / Chainer-v1 GPU semantics (see the oracle's orc_roi_pool): round() half away from zero, float32 bin sizes, empty
-// bin -> 0.  The bounds of the PH row bands and the PW column bins are computed ONCE per RoI.
+// bin -> 0; the bins of any RoI, NaN and infinite coordinates included, follow roi_coord / roi_bin (common.cuh).  The bounds
+// of the PH row bands and the PW column bins are computed ONCE per RoI.  NaN features are ignored (max.bf16x2 returns the
+// other operand, set.gt / set.eq are false), so a non-empty window with no number above -inf keeps its start, -inf.
 //
 // The maximum is taken on the PACKED bf16 pairs, not on converted floats.  A feature value is v = hi + lo with hi = RN_bf16(v)
 // and |lo| <= ulp(hi)/2 (split_bf16), and rounding is monotone, so v_a > v_b  <=>  hi_a > hi_b, or hi_a == hi_b and lo_a > lo_b:
@@ -401,22 +403,17 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
     for (int blk = blockIdx.x; blk < R_cap * slices; blk += gridDim.x) {
         const int r = blk / slices, c8 = (blk - r * slices) * c8_per_cta + c8l;
         const bool valid = r < R;                            // CTA-uniform
-        if (valid && tid < max(PH, PW)) {                    // the rounding chain of the oracle (orc_roi_pool)
+        if (valid && tid < max(PH, PW)) {                    // the bin rule of common.cuh (roi_coord / roi_bin)
             const float4 roi = reinterpret_cast<const float4*>(rois)[r];
-            const int sw = (int)roundf(__fmul_rn(roi.x, scale)), sh = (int)roundf(__fmul_rn(roi.y, scale));
-            const int ew = (int)roundf(__fmul_rn(roi.z, scale)), eh = (int)roundf(__fmul_rn(roi.w, scale));
-            const int rw = max(ew - sw + 1, 1), rh = max(eh - sh + 1, 1);
             if (tid < PH) {
-                const float bh = __fdiv_rn((float)rh, (float)PH);
-                const int hs = (int)floorf(__fmul_rn((float)tid, bh)) + sh, he = (int)ceilf(__fmul_rn((float)(tid + 1), bh)) + sh;
-                s_hs[tid] = min(max(hs, 0), H);
-                s_he[tid] = min(max(he, 0), H);
+                const int2 b = roi_bin(roi_coord(roi.y, scale), roi_coord(roi.w, scale), PH, tid, H);
+                s_hs[tid] = b.x;
+                s_he[tid] = b.y;
             }
             if (tid < PW) {
-                const float bw = __fdiv_rn((float)rw, (float)PW);
-                const int ws = (int)floorf(__fmul_rn((float)tid, bw)) + sw, we = (int)ceilf(__fmul_rn((float)(tid + 1), bw)) + sw;
-                s_ws[tid] = min(max(ws, 0), W);
-                s_we[tid] = min(max(we, 0), W);
+                const int2 b = roi_bin(roi_coord(roi.x, scale), roi_coord(roi.z, scale), PW, tid, W);
+                s_ws[tid] = b.x;
+                s_we[tid] = b.y;
             }
         }
         __syncthreads();
@@ -478,8 +475,8 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
                     float v[8];
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {
-                        v[2 * j] = __uint_as_float(hw[j] << 16) + __uint_as_float(lw[j] << 16);
-                        v[2 * j + 1] = __uint_as_float(hw[j] & 0xFFFF0000u) + __uint_as_float(lw[j] & 0xFFFF0000u);
+                        v[2 * j] = pool_pair_value(__uint_as_float(hw[j] << 16), __uint_as_float(lw[j] << 16));
+                        v[2 * j + 1] = pool_pair_value(__uint_as_float(hw[j] & 0xFFFF0000u), __uint_as_float(lw[j] & 0xFFFF0000u));
                     }
                     float4* d = reinterpret_cast<float4*>(of32 + off);
                     d[0] = make_float4(v[0], v[1], v[2], v[3]);

@@ -154,8 +154,9 @@ __global__ void dropout_kernel(__nv_bfloat16* __restrict__ hi, __nv_bfloat16* __
 // ------------------------------------------------------------------------------------------ RoI pooling backward
 constexpr double FIX_SCALE = 17592186044416.0;              // 2^44: sums of |g| up to 2^19 with a 5.7e-14 quantum
 
-// One thread per (roi, bin, 8 channels): rescans its window exactly like the forward kernel (strict '>' : first maximum in
-// (y, x) order) and adds the bin's gradient to the arg-max position of a 64-bit fixed-point map (integer atomics commute:
+// One thread per (roi, bin, 8 channels): rescans its window with the forward kernel's bins (roi_bin) and pair values
+// (pool_pair_value), from -inf with a strict '>' (the first maximum in (y, x) order; a window with no number above -inf
+// routes nothing) and adds the bin's gradient to the arg-max position of a 64-bit fixed-point map (integer atomics commute:
 // the result does not depend on the order of arrival).
 __global__ void roi_pool_backward_kernel(const __nv_bfloat16* __restrict__ fh, const __nv_bfloat16* __restrict__ fl, int H, int W,
                                          int C, const float* __restrict__ rois, const int* __restrict__ count, int R_cap, int PH,
@@ -172,19 +173,14 @@ __global__ void roi_pool_backward_kernel(const __nv_bfloat16* __restrict__ fh, c
         const int r = (int)(t / PH);
         if (r >= R) continue;
         const float4 roi = reinterpret_cast<const float4*>(rois)[r];
-        const int sw = (int)roundf(__fmul_rn(roi.x, scale)), sh = (int)roundf(__fmul_rn(roi.y, scale));
-        const int ew = (int)roundf(__fmul_rn(roi.z, scale)), eh = (int)roundf(__fmul_rn(roi.w, scale));
-        const int rw = max(ew - sw + 1, 1), rh = max(eh - sh + 1, 1);
-        const float bh = __fdiv_rn((float)rh, (float)PH), bw = __fdiv_rn((float)rw, (float)PW);
-        int hs = (int)floorf(__fmul_rn((float)ph, bh)) + sh, he = (int)ceilf(__fmul_rn((float)(ph + 1), bh)) + sh;
-        int ws = (int)floorf(__fmul_rn((float)pw, bw)) + sw, we = (int)ceilf(__fmul_rn((float)(pw + 1), bw)) + sw;
-        hs = min(max(hs, 0), H); he = min(max(he, 0), H);
-        ws = min(max(ws, 0), W); we = min(max(we, 0), W);
+        const int2 bh = roi_bin(roi_coord(roi.y, scale), roi_coord(roi.w, scale), PH, ph, H);
+        const int2 bw = roi_bin(roi_coord(roi.x, scale), roi_coord(roi.z, scale), PW, pw, W);
+        const int hs = bh.x, he = bh.y, ws = bw.x, we = bw.y;
         if (!(he > hs && we > ws)) continue;
         float m[8];
         int am[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { m[j] = -1e37f; am[j] = -1; }
+        for (int j = 0; j < 8; ++j) { m[j] = -INFINITY; am[j] = -1; }       // NaN and -inf never win: no gradient
         for (int y = hs; y < he; ++y)
             for (int x = ws; x < we; ++x) {
                 const long off = ((long)y * W + x) * C + 8 * c8;
@@ -195,7 +191,7 @@ __global__ void roi_pool_backward_kernel(const __nv_bfloat16* __restrict__ fh, c
                 const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    const float v = __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
+                    const float v = pool_pair_value(__bfloat162float(hb[j]), __bfloat162float(lb[j]));
                     if (v > m[j]) { m[j] = v; am[j] = y * W + x; }
                 }
             }

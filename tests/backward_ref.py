@@ -5,6 +5,8 @@ restated on the GPU, the CPU tests (test_backward_ref_cpu.py) check the restatem
 
 Rounding primitive: torch's float32 -> bfloat16 conversion (round to nearest, ties to even, subnormals kept, overflow to
 inf, NaN stays NaN); test_backward_ref_cpu.py pins that on hand-picked bit patterns."""
+import math
+
 import numpy as np
 import torch
 
@@ -166,41 +168,58 @@ def sgd_momentum(w, v, g, lr, momentum, weight_decay):
 
 
 # ---------------------------------------------------------------------------------------------- RoI pooling (NumPy)
-def _roundf(x32):
-    """C roundf on float32 values: half away from zero (float64 holds x + 0.5 exactly)."""
-    x = x32.astype(np.float64)
-    return (np.sign(x) * np.floor(np.abs(x) + 0.5)).astype(np.int64)
+def pool_value(hi, lo):
+    """float32 value of a (hi, lo) pair in RoI pooling (common.cuh pool_pair_value): hi + lo, or hi itself when hi is
+    +-inf or NaN (the split of +-inf has lo = NaN).  A missing lo plane is zero, as in the kernels: -0.0 becomes +0.0."""
+    h = hi.float()
+    return torch.where(torch.isfinite(h), h + (0.0 if lo is None else lo.float()), h)
+
+
+def roi_coord(coord, scale):
+    """int32 of roundf(float32(coord * scale)) as the kernels convert it (common.cuh roi_coord): half away from zero,
+    NaN -> 0, saturated to the int32 range."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        x = float(np.float32(coord) * np.float32(scale))
+    if x != x:
+        return 0
+    r = x if math.isinf(x) else math.copysign(math.floor(abs(x) + 0.5), x)    # float64 holds |x| + 0.5 exactly
+    return int(min(max(r, -2 ** 31), 2 ** 31 - 1))
+
+
+def roi_bin(s, e, P, i, L):
+    """[lo, hi) of bin i of P over the scaled extent [s, e], clamped to [0, L] (common.cuh roi_bin; Python ints do not
+    overflow, float32 for the bin size and the products)."""
+    f32 = np.float32
+    b = f32(max(e - s + 1, 1)) / f32(P)
+    lo = int(np.floor(f32(i) * b)) + s
+    hi = int(np.ceil(f32(i + 1) * b)) + s
+    return min(max(lo, 0), L), min(max(hi, 0), L)
 
 
 def roi_pool_argmax(feat, rois, outh, outw, scale):
-    """F.roi_pooling_2d forward with arg-max, float32 bin arithmetic of orc_roi_pool / roi_pool_backward_kernel.
-    feat [H,W,C] float32, rois [R,4] float32 (x1,y1,x2,y2).  Returns (max [R,outh,outw,C] float32 (0 for an empty bin),
-    argmax [R,outh,outw,C] int64 = y*W + x of the first maximum in (y, x) order, -1 for an empty bin)."""
-    f32 = np.float32
+    """F.roi_pooling_2d forward with arg-max under the rule of orc_roi_pool / roi_pool_backward_kernel (DESIGN §2).
+    feat [H,W,C] float32, rois [R,4] float32 (x1,y1,x2,y2).  Returns (max [R,outh,outw,C] float32: 0 for an empty bin,
+    -inf for a window with no number above -inf (NaN is ignored); argmax [R,outh,outw,C] int64 = y*W + x of the first
+    maximum in (y, x) order, -1 for an empty bin and where the maximum is -inf)."""
     H, W, C = feat.shape
     R = rois.shape[0]
-    mx = np.zeros((R, outh, outw, C), f32)
+    mx = np.zeros((R, outh, outw, C), np.float32)
     am = np.full((R, outh, outw, C), -1, np.int64)
-    sc = f32(scale)
     for r in range(R):
-        sw, sh, ew, eh = (int(_roundf(np.array(rois[r, j] * sc, f32))) for j in range(4))
-        rw, rh = max(ew - sw + 1, 1), max(eh - sh + 1, 1)
-        bh, bw = f32(rh) / f32(outh), f32(rw) / f32(outw)
+        sw, sh, ew, eh = (roi_coord(rois[r, j], scale) for j in range(4))
         for ph in range(outh):
-            hs = int(np.floor(f32(ph) * bh)) + sh
-            he = int(np.ceil(f32(ph + 1) * bh)) + sh
-            hs, he = min(max(hs, 0), H), min(max(he, 0), H)
+            hs, he = roi_bin(sh, eh, outh, ph, H)
             for pw in range(outw):
-                ws = int(np.floor(f32(pw) * bw)) + sw
-                we = int(np.ceil(f32(pw + 1) * bw)) + sw
-                ws, we = min(max(ws, 0), W), min(max(we, 0), W)
+                ws, we = roi_bin(sw, ew, outw, pw, W)
                 if he <= hs or we <= ws:
                     continue
                 win = feat[hs:he, ws:we].reshape(-1, C)
+                win = np.where(np.isnan(win), np.float32(-np.inf), win)
                 k = np.argmax(win, 0)                                   # first maximum in (y, x) order
-                mx[r, ph, pw] = win[k, np.arange(C)]
+                m = win[k, np.arange(C)]
+                mx[r, ph, pw] = m
                 ww = we - ws
-                am[r, ph, pw] = (hs + k // ww) * W + ws + k % ww
+                am[r, ph, pw] = np.where(m > -np.inf, (hs + k // ww) * W + ws + k % ww, -1)
     return mx, am
 
 

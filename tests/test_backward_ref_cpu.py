@@ -12,6 +12,7 @@ import torch
 
 import backward_ref as br
 import frcnn_oracle as orc
+import roi_pool_cases as rpc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
@@ -184,6 +185,37 @@ def test_roi_pool_argmax_max_equals_oracle(outh, outw, scale):
     r, ph, pw, c = np.argwhere(ok & (mx == 0))[0]
     y0, x0 = divmod(int(am[r, ph, pw, c]), W)
     assert feat[y0, x0, c] == 0
+
+
+@pytest.mark.parametrize("scale", rpc.SCALES)
+@pytest.mark.parametrize("outh,outw", rpc.OUT_SIZES)
+def test_roi_pool_argmax_equals_oracle_on_the_edge_matrix(outh, outw, scale):
+    """The restatement equals frcnn_oracle.roi_pool bit for bit on every edge geometry, non-finite and out-of-range RoIs
+    included, over features holding NaN, +-inf and values <= -1e37; its arg-max holds the maximum, and it is -1 exactly
+    where the maximum is 0 of an empty bin or -inf."""
+    rng = np.random.default_rng(outh * 64 + outw)
+    rois = np.vstack([rpc.geometry_rois(rpc.H, rpc.W, scale, outh, outw, rng, n_random=4),
+                      rpc.nonfinite_rois(rpc.H, rpc.W, scale)])
+    feat = np.concatenate([rpc.features(k, rpc.H, rpc.W, 1, outh + outw) for k in ("nan", "pos_inf", "huge_neg", "relu")], 2)
+    mx, am = br.roi_pool_argmax(feat, rois, outh, outw, scale)
+    want = rpc.oracle(feat, rois, outh, outw, scale)
+    assert np.array_equal(mx.view(np.uint32), want.view(np.uint32))
+    ok = am >= 0
+    C = feat.shape[2]
+    held = np.take_along_axis(feat.reshape(-1, C), np.where(ok, am, 0).reshape(-1, C), 0).reshape(am.shape)
+    assert np.array_equal(held[ok], mx[ok])
+    assert ((mx == 0) | (mx == -np.inf))[~ok].all() and (mx > -np.inf)[ok].all()
+
+
+def test_roi_pool_restatement_rule_known_answers():
+    """roi_coord: half away from zero, NaN -> 0, saturation; roi_bin: no overflow past the int32 range."""
+    assert [br.roi_coord(v, 1.0) for v in (2.5, -2.5, 0.49999997, -0.0, rpc.QNAN, rpc.NQNAN)] == [3, -3, 0, 0, 0, 0]
+    assert [br.roi_coord(v, 1.0) for v in (np.inf, -np.inf, 1e12, -1e12, 2147483520.0)] == \
+        [2 ** 31 - 1, -2 ** 31, 2 ** 31 - 1, -2 ** 31, 2147483520]
+    assert br.roi_bin(0, 2 ** 31 - 1, 2, 0, 5) == (0, 5) and br.roi_bin(0, 2 ** 31 - 1, 2, 1, 5) == (5, 5)
+    assert br.roi_bin(-2 ** 31, 2 ** 31 - 1, 7, 3, 9) == (0, 9)        # bin 3 of 2^32 pixels: about [-3.1e8, 3.1e8)
+    mx, am = br.roi_pool_argmax(np.array([[[np.nan]], [[-np.inf]]], f32), np.array([[0, 0, 0, 1]], f32), 1, 1, 1.0)
+    assert mx[0, 0, 0, 0] == -np.inf and am[0, 0, 0, 0] == -1
 
 
 def test_roi_pool_backward_scatter():
