@@ -146,4 +146,14 @@ __device__ __forceinline__ int2 roi_bin(int s, int e, int P, int i, int L) {
     return make_int2((int)min(max(lo, 0ll), (long long)L), (int)min(max(hi, 0ll), (long long)L));
 }
 
+// Canvas batches (the *_ext entries): image n of N sits at the top-left of its [Hc][Wc] slot and its true size is
+// extents[2n] x extents[2n+1] (device memory, read at run time, so one captured graph serves any mix of sizes).  After
+// `halvings` ceil-mode 2x2 pools the extent is ceil(e / 2^halvings) (repeated ceil-halving).  Every extent is clamped to
+// [0, limit] (the canvas at that resolution): a bad extent can never move a read or write outside the buffers.
+__device__ __forceinline__ int canvas_extent(const int* extents, int img, int axis, int halvings, int limit) {
+    long long e = max(__ldg(extents + 2 * img + axis), 0);
+    e = (e + (1ll << halvings) - 1) >> halvings;
+    return (int)min(e, (long long)limit);
+}
+
 }  // namespace frcnn

@@ -90,6 +90,11 @@ struct ConvParams {
     int n_img, img_tiles;
     FastDiv fd_img_tiles;
     long img_pix, img_opix;
+    // canvas batch (frcnn_*_batch_ext): image n's true size at this layer's input resolution is canvas_extent(extents, n,
+    // ., ext_halvings, H / W); every output pixel outside it is written as 0, the zero padding the next convolution reads.
+    // NULL: every pixel of the H x W image is live.
+    const int* extents;
+    int ext_halvings;
 };
 
 // Pixel tile mt -> (image, first row, first column).  Past the last tile (odd count, CTA pairs) the row lies below the
@@ -147,12 +152,13 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b, float& ra, flo
 }
 
 // One 16-channel run of one pixel: bias, residual, ReLU, validity, fp32 and bf16 (hi / lo, optionally 2x2-pooled) stores.
+// (ext_h, ext_w): the image's extent (H, W without a canvas); pixels outside it are stored as 0.
 __device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16], int part, int img, int h, int w, int n,
-                                             int lane, int m_valid) {
+                                             int lane, int m_valid, int ext_h, int ext_w) {
     const bool in_img = (h < p.H) && (w < p.W);
     const long ipix = (long)h * p.W + w;
     const long pix = img * p.img_pix + ipix;
-    const bool live = in_img && ipix < m_valid;
+    const bool live = in_img && h < ext_h && w < ext_w && ipix < m_valid;
     if (p.bias != nullptr) {                    // split-K partial sums carry no bias (the reduction adds it once)
         const float4* b4 = reinterpret_cast<const float4*>(p.bias + n);
 #pragma unroll
@@ -388,6 +394,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             tile_origin(p, mt, img, h0, w0);
             const int n0 = nt * BN;
             const int nkb = part_kblocks(p, part, num_kb);
+            const int ext_h = p.extents ? canvas_extent(p.extents, img, 0, p.ext_halvings, p.H) : p.H;
+            const int ext_w = p.extents ? canvas_extent(p.extents, img, 1, p.ext_halvings, p.W) : p.W;
     #pragma unroll
             for (int i = 0; i < NACC; ++i) {
                 acc[i] = 0.0f;
@@ -476,7 +484,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                     v[4 * q + 2] = f.z;
                     v[4 * q + 3] = f.w;
                 }
-                epilogue_run(p, v, part, img, h0 + row_h, w0 + row_w, n0 + ch * 32 + 16 * eh, lane, m_valid);
+                epilogue_run(p, v, part, img, h0 + row_h, w0 + row_w, n0 + ch * 32 + 16 * eh, lane, m_valid, ext_h, ext_w);
             }
         }
     }
@@ -708,10 +716,13 @@ struct WinExtra {           // frcnn_conv3x3_c8: 3x3 convolution over a compact 
 static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin, const void* w_hi,
                        const void* w_lo, const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2,
                        void* y_hi, void* y_lo, float* y_f32, int ld_f32, const int* m_valid, void* stream_,
-                       const GemmExtra* ge, const ResExtra* re = nullptr, const WinExtra* we = nullptr, int n_img = 1) {
+                       const GemmExtra* ge, const ResExtra* re = nullptr, const WinExtra* we = nullptr, int n_img = 1,
+                       const int* extents = nullptr, int ext_halvings = 0) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     for (int& v : g_last_plan) v = 0;          // a call that launches nothing leaves an empty record
     FRCNN_REQUIRE(n_img >= 1 && (n_img == 1 || (!ge && !m_valid && !re)), "frcnn_conv2d: bad batch of %d images", n_img);
+    FRCNN_REQUIRE(!extents || (!ge && !m_valid && !re && ext_halvings >= 0 && ext_halvings <= 30),
+                  "frcnn_conv2d: extents need a plain convolution and 0 <= halvings <= 30 (got %d)", ext_halvings);
     FRCNN_REQUIRE(x_hi && w_hi && (bias || ge), "frcnn_conv2d: x_hi, w_hi and bias are required");
     FRCNN_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "frcnn_conv2d: x_lo and w_lo must both be given (bf16x3) or both NULL");
     FRCNN_REQUIRE(ksize == 1 || ksize == 3, "frcnn_conv2d: ksize must be 1 or 3 (got %d)", ksize);
@@ -840,6 +851,8 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     p.m_valid = m_valid;
     p.res_hi = re ? (const __nv_bfloat16*)re->hi : nullptr;
     p.res_lo = re ? (const __nv_bfloat16*)re->lo : nullptr;
+    p.extents = extents;
+    p.ext_halvings = ext_halvings;
     FRCNN_REQUIRE(!re || (re->hi && !fuse_pool2x2 && Cout % 32 == 0), "frcnn_conv2d_res: residual needs res_hi, Cout %% 32 == 0 and no fused pool");
 
     CUtensorMap tm[4];
@@ -932,6 +945,27 @@ extern "C" int frcnn_conv3x3_c8_batch(const void* x_hi, const void* x_lo, int N,
     WinExtra we{W + 2, (long)frcnn_image_c8_elems(H, W)};
     return conv2d_impl(x_hi, x_lo, H, W, 32, w_hi, w_lo, bias, Cout, 3, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_, nullptr,
                        nullptr, &we, N);
+}
+
+extern "C" int frcnn_conv2d_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi,
+                                      const void* w_lo, const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2,
+                                      void* y_hi, void* y_lo, float* y_f32, int ld_f32, const int* extents, int halvings,
+                                      void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && extents, "frcnn_conv2d_batch_ext: needs N >= 1 (got %d) and the device extents", N);
+    return conv2d_impl(x_hi, x_lo, H, W, Cin, w_hi, w_lo, bias, Cout, ksize, relu, fuse_pool2x2, y_hi, y_lo, y_f32, ld_f32,
+                       nullptr, stream_, nullptr, nullptr, nullptr, N, extents, halvings);
+}
+
+extern "C" int frcnn_conv3x3_c8_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi,
+                                          const void* w_lo, const float* bias, int Cout, int relu, const int* extents,
+                                          void* y_hi, void* y_lo, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && H > 0 && W > 0 && extents, "frcnn_conv3x3_c8_batch_ext: bad shape N=%d H=%d W=%d or NULL extents",
+                  N, H, W);
+    WinExtra we{W + 2, (long)frcnn_image_c8_elems(H, W)};
+    return conv2d_impl(x_hi, x_lo, H, W, 32, w_hi, w_lo, bias, Cout, 3, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_, nullptr,
+                       nullptr, &we, N, extents, 0);
 }
 
 extern "C" int frcnn_gemm_nt_splitk_splits(int K, int splits) {

@@ -155,12 +155,15 @@ __global__ void pack_image_im2col_kernel(const float* x, int C, int H, int W, lo
 // zero pixel left and right of every row.  conv1_1 (models/vgg16.py:39) then reads, for output pixel (h, w) and kernel row
 // r, the 32 contiguous values of stored pixels w .. w+3 of row h+r-1 through a SLIDING-WINDOW tensor map (frcnn_conv3x3_c8):
 // 19 MB written here instead of the 77 MB of the [H][W][32] im2col copy, and nothing re-read from HBM four times.
-// A batch: image blockIdx.y reads x + blockIdx.y * sn and writes its own plane, out_elems elements further on.
+// A batch: image blockIdx.y reads x + blockIdx.y * sn and writes its own plane, out_elems elements further on.  A canvas
+// batch (extents != NULL): only the image's own eh x ew pixels are read, every other stored pixel of its plane is 0.
 __global__ void pack_image_c8_kernel(const float* x, int C, int H, int W, long sc, long sh, long sw, __nv_bfloat16* hi,
-                                     __nv_bfloat16* lo, long slack_pixels, long sn, long out_elems) {
+                                     __nv_bfloat16* lo, long slack_pixels, long sn, long out_elems, const int* extents) {
     x += blockIdx.y * sn;
     hi += blockIdx.y * out_elems;
     if (lo) lo += blockIdx.y * out_elems;
+    const int eh = extents ? canvas_extent(extents, blockIdx.y, 0, 0, H) : H;
+    const int ew = extents ? canvas_extent(extents, blockIdx.y, 1, 0, W) : W;
     const int WP = W + 2;
     const long total = (long)H * WP + slack_pixels;
     for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < total; p += (long)gridDim.x * blockDim.x) {
@@ -169,7 +172,7 @@ __global__ void pack_image_c8_kernel(const float* x, int C, int H, int W, long s
         for (int j = 0; j < 8; ++j) f.v[j] = 0.0f;
         if (p < (long)H * WP) {
             const int h = (int)(p / WP), wp = (int)(p % WP);
-            if (wp >= 1 && wp <= W) {
+            if (h < eh && wp >= 1 && wp <= ew) {
                 const long o = h * sh + (long)(wp - 1) * sw;
                 for (int c = 0; c < C; ++c) f.v[c] = x[c * sc + o];
             }
@@ -382,8 +385,12 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
                                                                          const int* __restrict__ count, int R_cap, int PH, int PW, float scale,
                                                                          __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol,
                                                                          float* __restrict__ of32, int c8_per_cta, int slices,
-                                                                         long rois_is, long count_is, long out_is) {
+                                                                         long rois_is, long count_is, long out_is,
+                                                                         const int* __restrict__ extents, int halvings) {
     grid_dep_wait();
+    // a canvas batch: the bins are clamped to the image's own map (bh x bw), the addressing keeps the canvas width W
+    const int bh = extents ? canvas_extent(extents, blockIdx.y, 0, halvings, H) : H;
+    const int bw = extents ? canvas_extent(extents, blockIdx.y, 1, halvings, W) : W;
     if (kBatch) {                      // image blockIdx.y: its feature map [H][W][C], RoIs, count and output rows
         const long img = blockIdx.y;
         const long fo = img * ((long)H * W * C), oo = img * out_is;
@@ -406,12 +413,12 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
         if (valid && tid < max(PH, PW)) {                    // the bin rule of common.cuh (roi_coord / roi_bin)
             const float4 roi = reinterpret_cast<const float4*>(rois)[r];
             if (tid < PH) {
-                const int2 b = roi_bin(roi_coord(roi.y, scale), roi_coord(roi.w, scale), PH, tid, H);
+                const int2 b = roi_bin(roi_coord(roi.y, scale), roi_coord(roi.w, scale), PH, tid, bh);
                 s_hs[tid] = b.x;
                 s_he[tid] = b.y;
             }
             if (tid < PW) {
-                const int2 b = roi_bin(roi_coord(roi.x, scale), roi_coord(roi.z, scale), PW, tid, W);
+                const int2 b = roi_bin(roi_coord(roi.x, scale), roi_coord(roi.z, scale), PW, tid, bw);
                 s_ws[tid] = b.x;
                 s_we[tid] = b.y;
             }
@@ -491,15 +498,20 @@ __global__ void __launch_bounds__(kRoiColMaxThreads, 2) roi_pool_col_kernel(cons
 // ------------------------------------------------------------------------------------------ head decode
 // One thread per (roi, class): softmax over classes (every thread recomputes max/sum of its row --
 // 21 values, L1-resident) and bbox_transform_inv + clip_boxes for its class's 4 deltas.  Image blockIdx.y of a batch
-// reads and writes its own rows, (image) * (the array's image stride) elements on.
+// reads and writes its own rows, (image) * (the array's image stride) elements on.  im_info (optional, device [N][2]):
+// image n's clip bounds (im_h, im_w), in place of the launch's one pair.
 struct DecodeStrides { long in, rois, count, prob, boxes; };
 template <bool kBatch>
 __global__ void head_decode_kernel(const float* scores, const float* deltas, int ld, const float* rois,
                                    const int* count, int R_cap, int NC, int im_h, int im_w, float* prob,
-                                   float* boxes, const DecodeStrides is) {
+                                   float* boxes, const DecodeStrides is, const int* im_info) {
     grid_dep_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= R_cap * NC) return;
+    if (im_info) {
+        im_h = __ldg(im_info + 2 * blockIdx.y);
+        im_w = __ldg(im_info + 2 * blockIdx.y + 1);
+    }
     if (kBatch) {
         const long img = blockIdx.y;
         scores += img * is.in;
@@ -831,23 +843,41 @@ extern "C" int frcnn_pack_image_c8(const float* x, int C, int H, int W, long str
     FRCNN_REQUIRE(stride_c > 0 && stride_h > 0 && stride_w > 0, "frcnn_pack_image_c8: strides must be positive");
     const long total = (long)H * (W + 2) + 8;
     pack_image_c8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x, C, H, W, stride_c, stride_h, stride_w,
-                                                                                (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, 8, 0, 0);
+                                                                                (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, 8, 0, 0,
+                                                                                nullptr);
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }
 
+namespace frcnn {
+static int pack_image_c8_n(const char* fn, const float* x, int N, int C, int H, int W, long stride_n, long stride_c, long stride_h,
+                           long stride_w, const int* extents, void* y_hi, void* y_lo, cudaStream_t stream) {
+    FRCNN_REQUIRE(x && y_hi && N >= 1 && N <= 65535 && C > 0 && C <= 3 && H > 0 && W > 0,
+                  "%s: needs 1 <= N <= 65535 and 1 <= C <= 3 (got N=%d C=%d)", fn, N, C);
+    FRCNN_REQUIRE(stride_n > 0 && stride_c > 0 && stride_h > 0 && stride_w > 0, "%s: strides must be positive", fn);
+    const long total = (long)H * (W + 2) + 8;
+    const dim3 grid(grid_for(total, 256), N);
+    pack_image_c8_kernel<<<grid, 256, 0, stream>>>(x, C, H, W, stride_c, stride_h, stride_w, (__nv_bfloat16*)y_hi,
+                                                   (__nv_bfloat16*)y_lo, 8, stride_n, (long)frcnn_image_c8_elems(H, W), extents);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+}  // namespace frcnn
+
 extern "C" int frcnn_pack_image_c8_batch(const float* x, int N, int C, int H, int W, long stride_n, long stride_c, long stride_h,
                                          long stride_w, void* y_hi, void* y_lo, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(x && y_hi && N >= 1 && N <= 65535 && C > 0 && C <= 3 && H > 0 && W > 0,
-                  "frcnn_pack_image_c8_batch: needs 1 <= N <= 65535 and 1 <= C <= 3 (got N=%d C=%d)", N, C);
-    FRCNN_REQUIRE(stride_n > 0 && stride_c > 0 && stride_h > 0 && stride_w > 0, "frcnn_pack_image_c8_batch: strides must be positive");
-    const long total = (long)H * (W + 2) + 8;
-    const dim3 grid(grid_for(total, 256), N);
-    pack_image_c8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, C, H, W, stride_c, stride_h, stride_w, (__nv_bfloat16*)y_hi,
-                                                                 (__nv_bfloat16*)y_lo, 8, stride_n, (long)frcnn_image_c8_elems(H, W));
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return pack_image_c8_n("frcnn_pack_image_c8_batch", x, N, C, H, W, stride_n, stride_c, stride_h, stride_w, nullptr, y_hi, y_lo,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_pack_image_c8_batch_ext(const float* x, int N, int C, int H, int W, long stride_n, long stride_c,
+                                             long stride_h, long stride_w, const int* extents, void* y_hi, void* y_lo,
+                                             void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(extents, "frcnn_pack_image_c8_batch_ext: extents is NULL");
+    return pack_image_c8_n("frcnn_pack_image_c8_batch_ext", x, N, C, H, W, stride_n, stride_c, stride_h, stride_w, extents, y_hi,
+                           y_lo, (cudaStream_t)stream);
 }
 
 extern "C" int frcnn_pack_conv_weights_c8(const float* w_oihw, int Cout, int Cin, void* w_hi, void* w_lo, void* stream) {
@@ -896,7 +926,9 @@ static int maxpool2x2_n(const char* fn, const void* x_hi, const void* x_lo, int 
 
 static int roi_pool_n(const char* fn, const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
                       long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale, void* out_hi,
-                      void* out_lo, float* out_f32, long out_stride, cudaStream_t stream) {
+                      void* out_lo, float* out_f32, long out_stride, cudaStream_t stream, const int* extents = nullptr,
+                      int halvings = 0) {
+    FRCNN_REQUIRE(halvings >= 0 && halvings <= 30, "%s: halvings must be in [0,30] (got %d)", fn, halvings);
     FRCNN_REQUIRE(feat_hi && rois && (out_hi || out_f32) && H > 0 && W > 0 && C > 0 && C % 8 == 0 && R_cap > 0 &&
                       outh > 0 && outw > 0,
                   "%s: bad arguments", fn);
@@ -918,18 +950,20 @@ static int roi_pool_n(const char* fn, const void* feat_hi, const void* feat_lo, 
     if (feat_lo) {
         FRCNN_CUDA_OK(launch_pdl(N > 1 ? roi_pool_col_kernel<true, true> : roi_pool_col_kernel<true, false>, grid, dim3(threads), 0, stream, (const __nv_bfloat16*)feat_hi,
                                  (const __nv_bfloat16*)feat_lo, H, W, C, rois, counts, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
-                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride));
+                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride,
+                                 extents, halvings));
     } else {
         FRCNN_CUDA_OK(launch_pdl(N > 1 ? roi_pool_col_kernel<false, true> : roi_pool_col_kernel<false, false>, grid, dim3(threads), 0, stream, (const __nv_bfloat16*)feat_hi,
                                  (const __nv_bfloat16*)feat_lo, H, W, C, rois, counts, R_cap, outh, outw, scale, (__nv_bfloat16*)out_hi,
-                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride));
+                                 (__nv_bfloat16*)out_lo, out_f32, c8_per_cta, slices, rois_stride, count_stride, out_stride,
+                                 extents, halvings));
     }
     return FRCNN_OK;
 }
 
 static int head_decode_n(const char* fn, int N, const float* scores, const float* deltas, int ld, const float* rois,
                          const int* counts, int R_cap, int num_classes, int im_h, int im_w, float* out_prob, float* out_boxes,
-                         const DecodeStrides& is, cudaStream_t stream) {
+                         const DecodeStrides& is, cudaStream_t stream, const int* im_info = nullptr) {
     FRCNN_REQUIRE(scores && deltas && rois && out_prob && out_boxes && R_cap > 0 && num_classes > 0 && ld >= num_classes,
                   "%s: bad arguments", fn);
     if (N > 1) {
@@ -942,7 +976,7 @@ static int head_decode_n(const char* fn, int N, const float* scores, const float
     }
     const int total = R_cap * num_classes;
     FRCNN_CUDA_OK(launch_pdl(N > 1 ? head_decode_kernel<true> : head_decode_kernel<false>, dim3(cdiv(total, 128), N), dim3(128), 0, stream, scores, deltas, ld, rois, counts, R_cap,
-                             num_classes, im_h, im_w, out_prob, out_boxes, is));
+                             num_classes, im_h, im_w, out_prob, out_boxes, is, im_info));
     return FRCNN_OK;
 }
 
@@ -1029,6 +1063,29 @@ extern "C" int frcnn_head_decode_batch(int N, const float* scores, const float* 
     const DecodeStrides is = {in_stride, rois_stride, count_stride, prob_stride, boxes_stride};
     return head_decode_n("frcnn_head_decode_batch", N, scores, deltas, ld, rois, counts, R_cap, num_classes, im_h, im_w, out_prob,
                          out_boxes, is, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_roi_pool_batch_ext(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                                        long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw,
+                                        float scale, const int* extents, int halvings, void* out_hi, void* out_lo, float* out_f32,
+                                        long out_stride, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_roi_pool_batch_ext", N);
+    FRCNN_REQUIRE(extents, "frcnn_roi_pool_batch_ext: extents is NULL");
+    return roi_pool_n("frcnn_roi_pool_batch_ext", feat_hi, feat_lo, N, H, W, C, rois, rois_stride, counts, count_stride, R_cap, outh,
+                      outw, scale, out_hi, out_lo, out_f32, out_stride, (cudaStream_t)stream, extents, halvings);
+}
+
+extern "C" int frcnn_head_decode_batch_ext(int N, const float* scores, const float* deltas, int ld, long in_stride, const float* rois,
+                                           long rois_stride, const int* counts, long count_stride, int R_cap, int num_classes,
+                                           const int* im_info, float* out_prob, long prob_stride, float* out_boxes,
+                                           long boxes_stride, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE_BATCH("frcnn_head_decode_batch_ext", N);
+    FRCNN_REQUIRE(im_info, "frcnn_head_decode_batch_ext: im_info is NULL");
+    const DecodeStrides is = {in_stride, rois_stride, count_stride, prob_stride, boxes_stride};
+    return head_decode_n("frcnn_head_decode_batch_ext", N, scores, deltas, ld, rois, counts, R_cap, num_classes, 0, 0, out_prob,
+                         out_boxes, is, (cudaStream_t)stream, im_info);
 }
 
 namespace frcnn {

@@ -46,6 +46,12 @@ struct DecodeArgs {
     int A, H, W, feat_stride, im_h, im_w, min_size;
     float4* boxes; float* scores; uint32_t* keys;
     long cls_is, bbox_is, ws_stride;      // image strides: cls / bbox in floats, the workspace slice in bytes
+    // canvas batch (frcnn_proposals_batch_ext): cells outside image n's feature-map extent (canvas_extent after
+    // ext_halvings) are filtered (key 0), and im_info[2n], im_info[2n+1] are its clip bounds.  NULL: the whole H x W map
+    // and (im_h, im_w) for every image.  The canvas anchor index ((h*W + w)*A + a) is monotone in the image's own index
+    // ((h*fw + w)*A + a), so the selection, the rank order and its lower-index tie rule are those of the image alone.
+    const int* extents; int ext_halvings;
+    const int* im_info;
 };
 
 template <bool kBatch>
@@ -60,6 +66,13 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     const long ws_off = img * a.ws_stride;
     const int pix = i / a.A, an = i - pix * a.A;
     const int h = pix / a.W, w = pix - h * a.W;
+    if (a.extents && (h >= canvas_extent(a.extents, img, 0, a.ext_halvings, a.H) ||
+                      w >= canvas_extent(a.extents, img, 1, a.ext_halvings, a.W))) {
+        ws_at(a.keys, ws_off)[i] = 0u;
+        return;
+    }
+    const int im_h = a.im_info ? __ldg(a.im_info + 2 * img) : a.im_h;
+    const int im_w = a.im_info ? __ldg(a.im_info + 2 * img + 1) : a.im_w;
 
     // fg score: channel A+an of rpn_cls_prob (models/proposal_layer.py:152-154)
     float score;
@@ -104,7 +117,7 @@ __global__ void rpn_decode_kernel(const DecodeArgs a) {
     float x2 = __fadd_rn(pcx, __fmul_rn(0.5f, pw));
     float y2 = __fadd_rn(pcy, __fmul_rn(0.5f, ph));
     // clip_boxes (models/bbox_transform.py:87-98)
-    const float wmax = (float)(a.im_w - 1), hmax = (float)(a.im_h - 1);
+    const float wmax = (float)(im_w - 1), hmax = (float)(im_h - 1);
     x1 = clip_coord(x1, wmax);
     y1 = clip_coord(y1, hmax);
     x2 = clip_coord(x2, wmax);
@@ -624,8 +637,10 @@ static int proposals_n(const char* fn, int N, const float* cls, long cls_cs, lon
                        const float* bbox, long bbox_cs, long bbox_ps, long bbox_is, const double* anchors, int A, int H, int W,
                        int feat_stride, int im_h, int im_w, int min_size, int pre_nms_top_n, int post_nms_top_n, double nms_thresh,
                        float* out_rois, float* out_scores, int* out_count, float* dbg_dets, int* dbg_idx, int* dbg_num,
-                       const OutStrides& os, void* ws, size_t ws_bytes, cudaStream_t stream) {
+                       const OutStrides& os, void* ws, size_t ws_bytes, cudaStream_t stream, const int* extents = nullptr,
+                       int ext_halvings = 0, const int* im_info = nullptr) {
     FRCNN_REQUIRE(cls && bbox && anchors && out_rois && out_count && ws, "%s: NULL argument", fn);
+    FRCNN_REQUIRE(ext_halvings >= 0 && ext_halvings <= 30, "%s: halvings must be in [0,30] (got %d)", fn, ext_halvings);
     FRCNN_REQUIRE(A > 0 && A <= 32 && H > 0 && W > 0, "%s: bad shape A=%d H=%d W=%d", fn, A, H, W);
     FRCNN_REQUIRE(pre_nms_top_n > 0 && pre_nms_top_n <= 16384, "%s: pre_nms_top_n must be in [1,16384] (got %d)", fn, pre_nms_top_n);
     FRCNN_REQUIRE(post_nms_top_n > 0 && post_nms_top_n <= 2048, "%s: post_nms_top_n must be in [1,2048] (got %d)", fn, post_nms_top_n);
@@ -658,6 +673,7 @@ static int proposals_n(const char* fn, int N, const float* cls, long cls_cs, lon
     da.A = A; da.H = H; da.W = W; da.feat_stride = feat_stride; da.im_h = im_h; da.im_w = im_w; da.min_size = min_size;
     da.boxes = w.boxes; da.scores = w.scores; da.keys = w.keys;
     da.cls_is = cls_is; da.bbox_is = bbox_is; da.ws_stride = (long)w.total;
+    da.extents = extents; da.ext_halvings = ext_halvings; da.im_info = im_info;
     FRCNN_CUDA_OK(launch_pdl(N > 1 ? rpn_decode_kernel<true> : rpn_decode_kernel<false>, dim3(cdiv(n_all, 128), N), dim3(128), 0,
                              stream, da));
     return run_sort_nms(w, N, (long)w.total, os, n_all, pre_nms_top_n, nms_thresh, FRCNN_NMS_GE_DOUBLE, post_nms_top_n, nullptr,
@@ -712,6 +728,23 @@ extern "C" int frcnn_proposals_batch(int N, const float* cls, long cls_chan_stri
                        bbox_chan_stride, bbox_pix_stride, bbox_image_stride, anchors, A, H, W, feat_stride, im_h, im_w, min_size,
                        pre_nms_top_n, post_nms_top_n, nms_thresh, out_rois, out_scores, out_count, dbg_sorted_dets,
                        dbg_sorted_anchor_idx, dbg_num_sorted, os, ws, ws_bytes, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int frcnn_proposals_batch_ext(int N, const float* cls, long cls_chan_stride, long cls_pix_stride, long cls_image_stride,
+                                         int cls_is_logits, const float* bbox, long bbox_chan_stride, long bbox_pix_stride,
+                                         long bbox_image_stride, const double* anchors, int A, int H, int W, int feat_stride,
+                                         const int* extents, int halvings, const int* im_info, int min_size, int pre_nms_top_n,
+                                         int post_nms_top_n, double nms_thresh, float* out_rois, long rois_image_stride,
+                                         float* out_scores, long scores_image_stride, int* out_count, long count_image_stride,
+                                         void* ws, size_t ws_bytes, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "frcnn_proposals_batch_ext: N must be in [1,65535] (got %d)", N);
+    FRCNN_REQUIRE(extents && im_info, "frcnn_proposals_batch_ext: extents and im_info are required");
+    const OutStrides os = {rois_image_stride, scores_image_stride, count_image_stride, 0, 0, 0};
+    return proposals_n("frcnn_proposals_batch_ext", N, cls, cls_chan_stride, cls_pix_stride, cls_image_stride, cls_is_logits, bbox,
+                       bbox_chan_stride, bbox_pix_stride, bbox_image_stride, anchors, A, H, W, feat_stride, 0, 0, min_size,
+                       pre_nms_top_n, post_nms_top_n, nms_thresh, out_rois, out_scores, out_count, nullptr, nullptr, nullptr, os, ws,
+                       ws_bytes, static_cast<cudaStream_t>(stream_), extents, halvings, im_info);
 }
 
 extern "C" size_t frcnn_nms_workspace_bytes(int n) {

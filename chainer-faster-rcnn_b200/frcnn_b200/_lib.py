@@ -139,6 +139,19 @@ SIGNATURES = {
     "frcnn_forward_batch_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "frcnn_forward_vgg16_batch": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p,
                                           c_void_p, c_void_p]),
+    "frcnn_proposals_batch_ext": (c_int, [c_int, c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_long, c_long, c_long, c_void_p,
+                                          c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_double,
+                                          c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_size_t, c_void_p]),
+    "frcnn_conv2d_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                       c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "frcnn_pack_image_c8_batch_ext": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_long, c_long, c_long, c_long, c_void_p,
+                                              c_void_p, c_void_p, c_void_p]),
+    "frcnn_conv3x3_c8_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                           c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_roi_pool_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_long, c_int,
+                                         c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_long, c_void_p]),
+    "frcnn_head_decode_batch_ext": (c_int, [c_int, c_void_p, c_void_p, c_int, c_long, c_void_p, c_long, c_void_p, c_long, c_int,
+                                            c_int, c_void_p, c_void_p, c_long, c_void_p, c_long, c_void_p]),
     "frcnn_detect": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double, c_float, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
 }

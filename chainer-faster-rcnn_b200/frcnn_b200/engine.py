@@ -422,6 +422,9 @@ class BatchPlan(object):
         self.boxes = seg(bf, "boxes").view(N, post_n, 4 * NC)
         self.det = (seg(blocks, "keep_idx").view(N, NC - 1, post_n), seg(blocks, "keep_count"), seg(blocks, "conf_count"))
         self.images = [dict(prob=self.prob[n], boxes=self.boxes[n], det=tuple(t[n] for t in self.det)) for n in range(N)]
+        # per-image device int32 [N, 2] extents (height, width) and clip bounds (im_h, im_w) of a canvas batch
+        # (CanvasBatchPlan); None: every image fills the H x W slot and (im_h, im_w) clips all of them
+        self.extents = self.im_info = None
         self._host = None
         self.graph = None
         self.use_graph = use_graph
@@ -430,33 +433,39 @@ class BatchPlan(object):
 
     def _run(self):
         w, N, post_n = self.w, self.N, self.post_n
-        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input)
+        ext = self.extents
+        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input, extents=ext)
         n = 1
         i = 0
+        k = 0           # 2x2 pools before the current layer: its extents are ceil(extent / 2^k)
         for name, fused, pool_after in self.trunk_steps:
             hi, lo, b = w.convs[name]
             if i == 0:
-                ops.conv3x3_c8_batch(self.acts[0], N, self.H, self.W, hi, lo, b, True, out=self.acts[1])
+                ops.conv3x3_c8_batch(self.acts[0], N, self.H, self.W, hi, lo, b, True, out=self.acts[1], extents=ext)
             else:
-                ops.conv2d_batch(self.acts[i], hi, lo, b, 3, True, out=self.acts[i + 1], fuse_pool=fused)
+                ops.conv2d_batch(self.acts[i], hi, lo, b, 3, True, out=self.acts[i + 1], fuse_pool=fused, extents=ext, halvings=k)
             n += 1
             i += 1
+            k += 1 if fused else 0
             if pool_after:
                 ops.maxpool2x2_ceil_batch(self.acts[i], out=self.acts[i + 1])
                 n += 1
                 i += 1
+                k += 1
         feat = self.feat = self.acts[-1]
         hi, lo, b = w.rpn3
-        ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid)
+        ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid, extents=ext, halvings=k)
         hi, lo, b = w.rpn_heads
-        ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out)
+        ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out, extents=ext,
+                         halvings=k)
         n += 2
         ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, w.rpn_ld), None, self.anchors, w.n_anchors, self.fh, self.fw,
                             self.feat_stride, self.im_h, self.im_w, self.min_size, self.pre_n, post_n, self.nms_thresh,
-                            layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=self.prop, debug=self.prop.dbg_dets is not None)
+                            layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=self.prop, debug=self.prop.dbg_dets is not None,
+                            extents=ext, halvings=k, im_info=self.im_info)
         p5 = self.pool5
         ops.roi_pool_batch(feat, self.prop.rois, self.prop.count, 7, 7, 1.0 / self.feat_stride,
-                           out=ops.Act(p5.hi[:, :post_n], None if p5.lo is None else p5.lo[:, :post_n]))
+                           out=ops.Act(p5.hi[:, :post_n], None if p5.lo is None else p5.lo[:, :post_n]), extents=ext, halvings=k)
         n += 5 + 1          # decode, select, rank/scatter, IoU mask, mask scan; RoI pool
         cnt, bw = self.counts, self.block_words
         hi, lo, b = w.fc6
@@ -468,7 +477,7 @@ class BatchPlan(object):
                          ld_f32=w.head_ld, work=self.fc_work, want_act=False)
         n += 3 * 2
         ops.head_decode_batch(self.head_out[:, :post_n], w.head_ld, self.prop.rois, self.prop.count, w.num_classes,
-                              self.im_h, self.im_w, out_prob=self.prob, out_boxes=self.boxes)
+                              self.im_h, self.im_w, out_prob=self.prob, out_boxes=self.boxes, im_info=self.im_info)
         n += 1
         if self.with_detect:
             ops.detect_batch(self.prob, self.boxes, self.prop.count, self.det_nms_thresh, self.det_conf, out=self.det)
@@ -504,6 +513,53 @@ class BatchPlan(object):
             if tuple(x_nchw.shape) != tuple(self.x_in.shape):
                 raise FrcnnError("BatchPlan: input of shape %s, the plan is for %s" % (tuple(x_nchw.shape), tuple(self.x_in.shape)))
             self.x_in.copy_(x_nchw, non_blocking=True)
+        _launch(self)
+        counts = self.result.view(self.N, self.block_words)[:, self.result_layout["count"][0]]
+        return [im["prob"] for im in self.images], [im["boxes"] for im in self.images], counts
+
+
+class CanvasBatchPlan(BatchPlan):
+    """A BatchPlan whose N images may have different sizes: each sits at the top-left of its Hc x Wc canvas slot, and its
+    true size and clip bounds are int32 [N, 2] device arrays that every kernel reads at run time (the *_batch_ext entries:
+    pixels outside an image are computed as zeros, its proposals, RoI bins and clips are its own).  So ONE captured graph
+    serves any mix of sizes up to the canvas, and an unused slot (extent 0 x 0) costs nothing but its share of the tiles.
+    Every image's results are bit-identical to a ForwardPlan's on that image alone.  Takes ForwardPlan's keyword options
+    except keep_rpn_debug (the debug rows would carry canvas anchor indices) and hwc_input."""
+
+    def __init__(self, weights, N, Hc, Wc, **kw):
+        if kw.get("keep_rpn_debug"):
+            raise FrcnnError("CanvasBatchPlan has no RPN debug outputs (keep_rpn_debug=True)")
+        if kw.get("hwc_input"):
+            raise FrcnnError("CanvasBatchPlan takes (3,H,W) images (hwc_input=True)")
+        super(CanvasBatchPlan, self).__init__(weights, N, Hc, Wc, **kw)
+        # rows 0 / 1: extents and clip bounds, written with one upload per forward
+        self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=weights.device)
+        self.extents, self.im_info = self._sizes[0], self._sizes[1]
+        self.image_sizes = [(0, 0)] * self.N
+
+    def forward(self, images=None, img_infos=None):
+        """images: a list of at most N (3,H_n,W_n) float32 CUDA tensors with H_n <= Hc and W_n <= Wc, copied into the
+        top-left of slots 0, 1, ...; the remaining slots are empty (count 0).  img_infos: optional per-image clip bounds
+        (im_h, im_w) (forward.py passes (H, H), SURVEY.md Q7); default (H_n, W_n).  None reuses the current slots, sizes and
+        clip bounds.  Returns BatchPlan.forward's (list of prob, list of boxes, counts)."""
+        if images is not None:
+            images = list(images)
+            if len(images) > self.N:
+                raise FrcnnError("CanvasBatchPlan: %d images for %d slots" % (len(images), self.N))
+            if img_infos is not None and len(img_infos) != len(images):
+                raise FrcnnError("CanvasBatchPlan: %d img_infos for %d images" % (len(img_infos), len(images)))
+            sizes = np.zeros((2, self.N, 2), dtype=np.int32)
+            for n, x in enumerate(images):
+                if x.dim() != 3 or x.shape[0] != 3 or not (0 < x.shape[1] <= self.H and 0 < x.shape[2] <= self.W):
+                    raise FrcnnError("CanvasBatchPlan: image %d of shape %s does not fit a (3,%d,%d) canvas" %
+                                     (n, tuple(x.shape), self.H, self.W))
+                sizes[0, n] = x.shape[1:]
+                sizes[1, n] = x.shape[1:] if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
+            for n, x in enumerate(images):
+                self.x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
+            # a pageable source: the copy is staged before copy_ returns, so `sizes` may go out of scope at once
+            self._sizes.copy_(torch.from_numpy(sizes), non_blocking=True)
+            self.image_sizes = [tuple(int(v) for v in sizes[0, n]) for n in range(self.N)]
         _launch(self)
         counts = self.result.view(self.N, self.block_words)[:, self.result_layout["count"][0]]
         return [im["prob"] for im in self.images], [im["boxes"] for im in self.images], counts
@@ -754,6 +810,40 @@ class Engine(object):
         probs, boxes, counts = p.forward(x_nchw)
         R = counts.cpu().tolist()
         return [(pr[:r], bx[:r]) for pr, bx, r in zip(probs, boxes, R)]
+
+    def canvas_plan(self, N, Hc, Wc, **overrides):
+        """The CanvasBatchPlan of N slots of Hc x Wc (cached per canvas and options)."""
+        kw = dict(self.plan_kwargs)
+        kw.update(overrides)
+        key = ("canvas", N, Hc, Wc, tuple(sorted(kw.items())))
+        if key not in self.plans:
+            self.plans[key] = CanvasBatchPlan(self.weights, N, Hc, Wc, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
+        return self.plans[key]
+
+    def forward_images(self, images, img_infos=None, N=None, canvas=None, **overrides):
+        """Images of any sizes, a list of (3,H_n,W_n) float32 CUDA tensors -> list of per-image (prob [R_n,NC], boxes
+        [R_n,4NC]) device tensors, N images per graph replay (default: all of them) on a canvas of (Hc, Wc) (default: the
+        largest H and W, each rounded up to a multiple of 64, so that a stream of photos reuses a few canvases).
+        img_infos: optional per-image clip bounds (im_h, im_w).  With more than N images the results are copies; otherwise
+        views into the plan's buffers, valid until its next call."""
+        images = list(images)
+        if not images:
+            return []
+        for x in images:
+            if x.dim() != 3 or x.shape[0] != 3:
+                raise FrcnnError("forward_images: expected (3,H,W) images, got %s" % (tuple(x.shape),))
+        N = len(images) if N is None else int(N)
+        if canvas is None:
+            canvas = (ops.round_up(max(int(x.shape[1]) for x in images), 64), ops.round_up(max(int(x.shape[2]) for x in images), 64))
+        p = self.canvas_plan(N, int(canvas[0]), int(canvas[1]), **overrides)
+        out = []
+        for s in range(0, len(images), N):
+            chunk = images[s:s + N]
+            probs, boxes, counts = p.forward(chunk, None if img_infos is None else img_infos[s:s + N])
+            R = counts.cpu().tolist()
+            res = [(probs[n][:R[n]], boxes[n][:R[n]]) for n in range(len(chunk))]
+            out += [(a.clone(), b.clone()) for a, b in res] if len(images) > N else res
+        return out
 
 
 class CForward(object):

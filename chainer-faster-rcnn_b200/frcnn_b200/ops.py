@@ -218,9 +218,18 @@ def linear(x, w_hi, w_lo, bias, relu, m_valid=None, out=None, out_f32=None, ld_f
     return y, y32
 
 
-def pack_image_c8_batch(x_nchw, precision="bf16x3", out=None, hwc_memory=False):
+def _per_image_pairs(t, N, what):
+    """A canvas batch's per-image (height, width) extents or (im_h, im_w) clip bounds: dense int32 CUDA [N, 2]."""
+    _need_cuda(t)
+    if t.dtype != torch.int32 or tuple(t.shape) != (N, 2) or not t.is_contiguous():
+        raise FrcnnError("%s: expected a dense int32 [%d, 2] CUDA tensor, got %s %s" % (what, N, t.dtype, tuple(t.shape)))
+    return _p(t)
+
+
+def pack_image_c8_batch(x_nchw, precision="bf16x3", out=None, hwc_memory=False, extents=None):
     """(N,C<=3,H,W) float32 CUDA images -> Act of planes [N, frcnn_image_c8_elems(H,W)]: pack_image_c8 of every image.
-    hwc_memory: the buffer's BYTES are dense (N,H,W,C) images."""
+    hwc_memory: the buffer's BYTES are dense (N,H,W,C) images.  extents: int32 [N, 2] device (height, width) of each image
+    in its H x W canvas slot (frcnn_pack_image_c8_batch_ext: everything outside is packed as 0)."""
     _need_cuda(x_nchw)
     x = x_nchw.contiguous().float()
     N, C, H, W = x.shape
@@ -232,13 +241,18 @@ def pack_image_c8_batch(x_nchw, precision="bf16x3", out=None, hwc_memory=False):
     if out.hi.numel() < N * n:
         raise FrcnnError("pack_image_c8_batch: output holds %d elements, needs %d" % (out.hi.numel(), N * n))
     sc, sh, sw = (1, W * C, C) if hwc_memory else (H * W, W, 1)
+    if extents is not None:
+        check(lib.frcnn_pack_image_c8_batch_ext(_p(x), N, C, H, W, C * H * W, sc, sh, sw, _per_image_pairs(extents, N, "extents"),
+                                                _p(out.hi), _p(out.lo), _stream()), "frcnn_pack_image_c8_batch_ext")
+        return out
     check(lib.frcnn_pack_image_c8_batch(_p(x), N, C, H, W, C * H * W, sc, sh, sw, _p(out.hi), _p(out.lo), _stream()),
           "frcnn_pack_image_c8_batch")
     return out
 
 
-def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None):
-    """frcnn_conv3x3_c8_batch: conv1_1 over N compact images (pack_image_c8_batch) -> Act [N,H,W,Cout]."""
+def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None, extents=None):
+    """frcnn_conv3x3_c8_batch: conv1_1 over N compact images (pack_image_c8_batch) -> Act [N,H,W,Cout].  extents: int32
+    [N, 2] device image sizes in H x W canvas slots (frcnn_conv3x3_c8_batch_ext: pixels outside are written as 0)."""
     taps, Cout, k = w_hi.shape
     if (taps, k) != (3, 32):
         raise FrcnnError("conv3x3_c8_batch: weights must be [3, Cout, 32] (pack_conv_weights_c8)")
@@ -249,14 +263,22 @@ def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None):
     if out is None:
         yh = torch.empty((N, H, W, Cout), dtype=torch.bfloat16, device=x_c8.hi.device)
         out = Act(yh, torch.empty_like(yh) if x_c8.lo is not None else None)
+    if extents is not None:
+        check(_lib.load().frcnn_conv3x3_c8_batch_ext(_p(x_c8.hi), _p(x_c8.lo), N, H, W, _p(w_hi), _p(w_lo), _p(bias), Cout,
+                                                     1 if relu else 0, _per_image_pairs(extents, N, "extents"), _p(out.hi),
+                                                     _p(out.lo), _stream()), "frcnn_conv3x3_c8_batch_ext")
+        return out
     check(_lib.load().frcnn_conv3x3_c8_batch(_p(x_c8.hi), _p(x_c8.lo), N, H, W, _p(w_hi), _p(w_lo), _p(bias), Cout,
                                              1 if relu else 0, _p(out.hi), _p(out.lo), _stream()), "frcnn_conv3x3_c8_batch")
     return out
 
 
-def conv2d_batch(x, w_hi, w_lo, bias, ksize, relu, out_act=True, ld_f32=0, out=None, out_f32=None, fuse_pool=False):
+def conv2d_batch(x, w_hi, w_lo, bias, ksize, relu, out_act=True, ld_f32=0, out=None, out_f32=None, fuse_pool=False,
+                 extents=None, halvings=0):
     """frcnn_conv2d_batch: x Act [N,H,W,Cin]; returns (Act [N,H,W,Cout] (pooled: [N,ceil(H/2),ceil(W/2),Cout]) or None,
-    fp32 [N*H*W, ld_f32] or None).  Each image's output equals conv2d on that image, bit for bit."""
+    fp32 [N*H*W, ld_f32] or None).  Each image's output equals conv2d on that image, bit for bit.
+    extents: int32 [N, 2] device image sizes (input pixels) in H x W canvas slots, ceil(extent / 2^halvings) at this layer
+    (frcnn_conv2d_batch_ext: every output pixel outside is written as 0)."""
     N, H, W, Cin = x.hi.shape
     taps, Cout, cin_w = w_hi.shape
     if cin_w != Cin or taps != ksize * ksize:
@@ -274,6 +296,12 @@ def conv2d_batch(x, w_hi, w_lo, bias, ksize, relu, out_act=True, ld_f32=0, out=N
     need = round_up(max(Cout, ld_f32), 32)
     if bias.numel() < need:
         raise FrcnnError("conv2d_batch: bias has %d entries, needs %d (use pad_bias)" % (bias.numel(), need))
+    if extents is not None:
+        check(_lib.load().frcnn_conv2d_batch_ext(_p(x.hi), _p(x.lo), N, H, W, Cin, _p(w_hi), _p(w_lo), _p(bias), Cout, ksize,
+                                                 1 if relu else 0, 1 if fuse_pool else 0, _p(y.hi) if y else None,
+                                                 _p(y.lo) if y else None, _p(y32), ld_f32, _per_image_pairs(extents, N, "extents"),
+                                                 int(halvings), _stream()), "frcnn_conv2d_batch_ext")
+        return y, y32
     check(_lib.load().frcnn_conv2d_batch(_p(x.hi), _p(x.lo), N, H, W, Cin, _p(w_hi), _p(w_lo), _p(bias), Cout, ksize,
                                          1 if relu else 0, 1 if fuse_pool else 0, _p(y.hi) if y else None,
                                          _p(y.lo) if y else None, _p(y32), ld_f32, _stream()), "frcnn_conv2d_batch")
@@ -624,10 +652,13 @@ def maxpool2x2_ceil_batch(x, out=None):
     return out
 
 
-def roi_pool_batch(feat, rois, counts=None, outh=7, outw=7, scale=1.0 / 16, want_f32=False, out=None, out_f32=None):
+def roi_pool_batch(feat, rois, counts=None, outh=7, outw=7, scale=1.0 / 16, want_f32=False, out=None, out_f32=None,
+                   extents=None, halvings=0):
     """frcnn_roi_pool_batch: feat Act [N,H,W,C] (dense); rois [N,R_cap,4]; counts [N] int32 (or None).  Returns (Act
     [N,R_cap,outh*outw*C], fp32 [N,R_cap,outh*outw,C] or None).  `out` / `out_f32` may be strided views (image blocks
-    apart); the library takes one image stride for all outputs, so given both, their strides must agree."""
+    apart); the library takes one image stride for all outputs, so given both, their strides must agree.
+    extents: int32 [N, 2] device image sizes (input pixels); image n's map is the top-left ceil(extent / 2^halvings) of
+    its slot and its bins are clamped to it (frcnn_roi_pool_batch_ext)."""
     N, H, W, C = feat.hi.shape
     R_cap = rois.shape[1]
     K = outh * outw * C
@@ -646,15 +677,22 @@ def roi_pool_batch(feat, rois, counts=None, outh=7, outw=7, scale=1.0 / 16, want
         o32 = torch.empty((N, os_), dtype=torch.float32, device=rois.device)[:, :K].view(N, R_cap, outh * outw, C)
     if o32 is not None and _image_stride(o32, (R_cap, outh * outw, C), "roi_pool_batch out_f32") != os_ and N > 1:
         raise FrcnnError("roi_pool_batch: the bf16 and fp32 outputs need the same image stride")
+    if extents is not None:
+        check(_lib.load().frcnn_roi_pool_batch_ext(_p(feat.hi), _p(feat.lo), N, H, W, C, _p(rois), rs, _p(counts), cs, R_cap, outh,
+                                                   outw, ctypes.c_float(scale), _per_image_pairs(extents, N, "extents"),
+                                                   int(halvings), _p(out.hi), _p(out.lo), _p(o32), os_, _stream()),
+              "frcnn_roi_pool_batch_ext")
+        return out, o32
     check(_lib.load().frcnn_roi_pool_batch(_p(feat.hi), _p(feat.lo), N, H, W, C, _p(rois), rs, _p(counts), cs, R_cap, outh, outw,
                                            ctypes.c_float(scale), _p(out.hi), _p(out.lo), _p(o32), os_, _stream()),
           "frcnn_roi_pool_batch")
     return out, o32
 
 
-def head_decode_batch(scores_deltas, ld, rois, counts, num_classes, im_h, im_w, out_prob=None, out_boxes=None):
+def head_decode_batch(scores_deltas, ld, rois, counts, num_classes, im_h, im_w, out_prob=None, out_boxes=None, im_info=None):
     """frcnn_head_decode_batch: scores_deltas fp32 [N,R_cap,ld] (columns [0,NC) scores, [NC,5NC) deltas), rois [N,R_cap,4],
-    counts [N] int32 or None; out_prob [N,R_cap,NC], out_boxes [N,R_cap,4NC] (may be strided views)."""
+    counts [N] int32 or None; out_prob [N,R_cap,NC], out_boxes [N,R_cap,4NC] (may be strided views).
+    im_info: int32 [N, 2] device clip bounds (im_h, im_w) per image, in place of (im_h, im_w) (frcnn_head_decode_batch_ext)."""
     N, R_cap = rois.shape[0], rois.shape[1]
     dev = rois.device
     if out_prob is None:
@@ -667,6 +705,11 @@ def head_decode_batch(scores_deltas, ld, rois, counts, num_classes, im_h, im_w, 
     ps = _image_stride(out_prob, (R_cap, num_classes), "head_decode_batch out_prob")
     bs = _image_stride(out_boxes, (R_cap, 4 * num_classes), "head_decode_batch out_boxes")
     deltas_ptr = ctypes.c_void_p(scores_deltas.data_ptr() + 4 * num_classes)
+    if im_info is not None:
+        check(_lib.load().frcnn_head_decode_batch_ext(N, _p(scores_deltas), deltas_ptr, ld, ins, _p(rois), rs, _p(counts), cs, R_cap,
+                                                      num_classes, _per_image_pairs(im_info, N, "im_info"), _p(out_prob), ps,
+                                                      _p(out_boxes), bs, _stream()), "frcnn_head_decode_batch_ext")
+        return out_prob, out_boxes
     check(_lib.load().frcnn_head_decode_batch(N, _p(scores_deltas), deltas_ptr, ld, ins, _p(rois), rs, _p(counts), cs, R_cap, num_classes,
                                               int(im_h), int(im_w), _p(out_prob), ps, _p(out_boxes), bs, _stream()),
           "frcnn_head_decode_batch")
@@ -723,10 +766,13 @@ class ProposalBatchWorkspace(object):
 
 
 def proposals_batch(cls, bbox, anchors, A, H, W, feat_stride, im_h, im_w, min_size, pre_n, post_n, nms_thresh,
-                    layout="nchw", ld=0, cls_is_logits=False, work=None, debug=False):
+                    layout="nchw", ld=0, cls_is_logits=False, work=None, debug=False, extents=None, halvings=0, im_info=None):
     """frcnn_proposals_batch over N images (one clip bound for all).  layout "nchw": cls (N,2A,H,W), bbox (N,4A,H,W) planar;
     layout "nhwc": cls one fp32 tensor [N,H*W,ld] with cls in columns [0,2A) and bbox in [2A,6A) (bbox None).  Returns the
-    ProposalBatchWorkspace holding the outputs."""
+    ProposalBatchWorkspace holding the outputs.
+    A canvas batch (frcnn_proposals_batch_ext): extents int32 [N, 2] device image sizes in input pixels, the feature-map
+    extent being ceil(extent / 2^halvings) of the H x W slot; im_info int32 [N, 2] device clip bounds per image, in place of
+    (im_h, im_w).  Both are required together; no debug outputs."""
     _need_cuda(cls)
     N = cls.shape[0]
     dev = cls.device
@@ -749,6 +795,16 @@ def proposals_batch(cls, bbox, anchors, A, H, W, feat_stride, im_h, im_w, min_si
     dd = _image_stride(work.dbg_dets, (k_cap, 5), "proposals_batch dbg_dets") if debug else 0
     di = _image_stride(work.dbg_idx, (k_cap,), "proposals_batch dbg_idx") if debug else 0
     dn = _counts_stride(work.dbg_num, N, "proposals_batch dbg_num") if debug else 0
+    if extents is not None or im_info is not None:
+        if extents is None or im_info is None or debug:
+            raise FrcnnError("proposals_batch: a canvas batch needs both extents and im_info, and has no debug outputs")
+        check(_lib.load().frcnn_proposals_batch_ext(N, _p(cls), cs, ps, cis, 1 if cls_is_logits else 0, bbox_ptr, bcs, bps, bis,
+                                                    _p(anchors), A, H, W, feat_stride, _per_image_pairs(extents, N, "extents"),
+                                                    int(halvings), _per_image_pairs(im_info, N, "im_info"), int(min_size), pre_n,
+                                                    post_n, float(nms_thresh), _p(work.rois), rs, _p(work.scores), ss,
+                                                    _p(work.count), cnt, _p(work.ws), work.ws.numel(), _stream()),
+              "frcnn_proposals_batch_ext")
+        return work
     check(_lib.load().frcnn_proposals_batch(N, _p(cls), cs, ps, cis, 1 if cls_is_logits else 0, bbox_ptr, bcs, bps, bis, _p(anchors),
                                             A, H, W, feat_stride, int(im_h), int(im_w), int(min_size), pre_n, post_n,
                                             float(nms_thresh), _p(work.rois), rs, _p(work.scores), ss, _p(work.count), cnt,

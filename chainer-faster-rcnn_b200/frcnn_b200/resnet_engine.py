@@ -148,6 +148,9 @@ class ResNetEngine(Engine):
     def batch_plan(self, N, H, W, **overrides):
         raise FrcnnError("ResNetEngine runs one image at a time: batches (BatchPlan) need the VGG16 trunk")
 
+    def canvas_plan(self, N, Hc, Wc, **overrides):
+        raise FrcnnError("ResNetEngine runs one image at a time: canvas batches (CanvasBatchPlan) need the VGG16 trunk")
+
 
 class TrunkOnly(object):
     """The trunk alone (models.resnet.ResNet.__call__): packs only trunk/* and runs ResNetForwardPlan's trunk hooks."""

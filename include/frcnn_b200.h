@@ -121,6 +121,20 @@ int frcnn_proposals_batch(int N, const float* cls, long cls_chan_stride, long cl
                           int* out_count, long count_image_stride, float* dbg_sorted_dets, long dbg_dets_image_stride,
                           int* dbg_sorted_anchor_idx, long dbg_idx_image_stride, int* dbg_num_sorted,
                           long dbg_num_image_stride, void* ws, size_t ws_bytes, void* stream);
+/* frcnn_proposals_batch over a CANVAS batch: N images of different sizes, each at the top-left of its H x W slot of the
+ * feature map.  extents (device, int32 [N][2]): image n's size (height, width) in INPUT pixels; its feature-map extent is
+ * ceil(extent / 2^halvings) (4 for VGG16), clamped to [0, H] x [0, W].  Cells outside it propose nothing.  im_info (device,
+ * int32 [N][2]): image n's clip bounds (im_h, im_w).  Both are read at run time, so a captured graph serves any mix of
+ * sizes.  Image n's rois, scores and count are bit-identical to frcnn_proposals on its own extent-sized map with its own
+ * clip bounds.  Other arguments as frcnn_proposals_batch (workspace: frcnn_proposals_batch_workspace_bytes of the canvas);
+ * no debug outputs.  Errors: NULL extents / im_info, N outside [1,65535], halvings outside [0,30] -> FRCNN_ERR_ARG. */
+int frcnn_proposals_batch_ext(int N, const float* cls, long cls_chan_stride, long cls_pix_stride, long cls_image_stride,
+                              int cls_is_logits, const float* bbox, long bbox_chan_stride, long bbox_pix_stride,
+                              long bbox_image_stride, const double* anchors, int A, int H, int W, int feat_stride,
+                              const int* extents, int halvings, const int* im_info, int min_size, int pre_nms_top_n,
+                              int post_nms_top_n, double nms_thresh, float* out_rois, long rois_image_stride, float* out_scores,
+                              long scores_image_stride, int* out_count, long count_image_stride, void* ws, size_t ws_bytes,
+                              void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Dense contraction on Hopper tensor cores (TMA -> smem -> wgmma -> register accumulators -> epilogue):
@@ -149,6 +163,15 @@ int frcnn_conv2d(const void* x_hi, const void* x_lo, int H, int W, int Cin, cons
 int frcnn_conv2d_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi, const void* w_lo,
                        const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2, void* y_hi, void* y_lo, float* y_f32,
                        int ld_f32, void* stream);
+/* frcnn_conv2d_batch over a CANVAS batch: image n sits at the top-left of its H x W slot and is extents[2n] x extents[2n+1]
+ * input pixels (device int32 [N][2], read at run time), i.e. ceil(extent / 2^halvings) pixels at this layer's input
+ * resolution, clamped to [0, H] x [0, W].  Every output pixel outside that extent (bf16 hi / lo, pooled, fp32) is written
+ * as 0 -- the zero padding the next 3x3 convolution then reads, as the one-image launch gets it from the TMA
+ * out-of-bounds fill -- so each image's pixels equal frcnn_conv2d on the image alone.  The input outside the extent must be
+ * zero (what this entry writes).  extents NULL, N < 1 or halvings outside [0,30] -> FRCNN_ERR_ARG. */
+int frcnn_conv2d_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi, const void* w_lo,
+                           const float* bias, int Cout, int ksize, int relu, int fuse_pool2x2, void* y_hi, void* y_lo,
+                           float* y_f32, int ld_f32, const int* extents, int halvings, void* stream);
 /* Tuning override for tests / benchmarks: force the N tile (64/128/256) and the pixel tile
  * (tile_h*tile_w == 128); 0 = automatic. Process-wide. */
 void frcnn_conv2d_set_tile(int block_n, int tile_h, int tile_w);
@@ -234,6 +257,14 @@ int frcnn_pack_image_c8_batch(const float* x, int N, int C, int H, int W, long s
                               long stride_w, void* y_hi, void* y_lo, void* stream);
 int frcnn_conv3x3_c8_batch(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo,
                            const float* bias, int Cout, int relu, void* y_hi, void* y_lo, void* stream);
+/* The same over a CANVAS batch of N H x W slots, image n of extents[2n] x extents[2n+1] pixels at the top-left of its slot
+ * (device int32 [N][2], clamped to [0, H] x [0, W]).  frcnn_pack_image_c8_batch_ext reads only the image's own pixels and
+ * writes zeros everywhere else in its plane; frcnn_conv3x3_c8_batch_ext writes 0 at every output pixel outside the extent
+ * (frcnn_conv2d_batch_ext with halvings 0).  NULL extents -> FRCNN_ERR_ARG. */
+int frcnn_pack_image_c8_batch_ext(const float* x, int N, int C, int H, int W, long stride_n, long stride_c, long stride_h,
+                                  long stride_w, const int* extents, void* y_hi, void* y_lo, void* stream);
+int frcnn_conv3x3_c8_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo,
+                               const float* bias, int Cout, int relu, const int* extents, void* y_hi, void* y_lo, void* stream);
 
 /* Same with an explicit source layout: element (c, h, w) is x[c*stride_c + h*stride_h + w*stride_w] (in floats).
  * (H*W, W, 1) = dense (C,H,W); (1, W*C, C) = dense (H,W,C) memory, which is what forward.py:45's
@@ -266,6 +297,14 @@ int frcnn_roi_pool(const void* feat_hi, const void* feat_lo, int H, int W, int C
 int frcnn_roi_pool_batch(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
                          long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale,
                          void* out_hi, void* out_lo, float* out_f32, long out_stride, void* stream);
+/* frcnn_roi_pool_batch over a CANVAS batch: image n's map is the top-left ceil(extent / 2^halvings) pixels of its H x W slot
+ * (extents: device int32 [N][2] in input pixels, clamped to [0, H] x [0, W]), and its bins are clamped to that map, not to
+ * the slot.  Each image's rows are bit-identical to frcnn_roi_pool on its own map.  NULL extents, halvings outside [0,30]
+ * -> FRCNN_ERR_ARG. */
+int frcnn_roi_pool_batch_ext(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                             long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw, float scale,
+                             const int* extents, int halvings, void* out_hi, void* out_lo, float* out_f32, long out_stride,
+                             void* stream);
 
 /* L.Linear (+ F.relu) for a small number of rows: fc6 / fc7 / cls_score|bbox_pred over the R <= post_nms_top_n RoIs
  * (models/faster_rcnn.py:33-36,127-134).  y[r, c] = act(sum_k x[r,k] * w[c,k] + bias[c]) for r < R_cap, c < Cout.
@@ -302,6 +341,12 @@ int frcnn_head_decode(const float* scores, const float* deltas, int ld, const fl
 int frcnn_head_decode_batch(int N, const float* scores, const float* deltas, int ld, long in_stride, const float* rois,
                             long rois_stride, const int* counts, long count_stride, int R_cap, int num_classes, int im_h,
                             int im_w, float* out_prob, long prob_stride, float* out_boxes, long boxes_stride, void* stream);
+/* frcnn_head_decode_batch with a clip bound per image: im_info (device int32 [N][2]) holds image n's (im_h, im_w), read at
+ * run time.  NULL im_info -> FRCNN_ERR_ARG. */
+int frcnn_head_decode_batch_ext(int N, const float* scores, const float* deltas, int ld, long in_stride, const float* rois,
+                                long rois_stride, const int* counts, long count_stride, int R_cap, int num_classes,
+                                const int* im_info, float* out_prob, long prob_stride, float* out_boxes, long boxes_stride,
+                                void* stream);
 
 /* Stand-alone box algebra, the array-level helpers of models/bbox_transform.py:
  *   out[n, 4k..4k+3] = bbox_transform_inv(boxes[n], trans[n, 4k..4k+3])   (:41-76), k < K
