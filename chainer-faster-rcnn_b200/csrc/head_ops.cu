@@ -206,36 +206,91 @@ struct PreArgs {
     int H, W;
     float* out;
 };
+
+// One axis of the resize: output index o of a source axis of n pixels -> the two source indices and the weight of the
+// second.  Whatever inv_scale holds, i0 and i1 end up inside [0, n - 1] (the conversion to int saturates, NaN gives 0).
+struct BilinearTap { int i0, i1; float t; };
+__device__ __forceinline__ BilinearTap bilinear_tap(int o, double inv_scale, int n) {
+    const double f = ((double)o + 0.5) * inv_scale - 0.5;
+    BilinearTap r;
+    r.i0 = (int)floor(f);
+    r.t = (float)(f - (double)r.i0);
+    if (r.i0 < 0) { r.i0 = 0; r.t = 0.0f; }
+    if (r.i0 >= n - 1) { r.i0 = n - 1; r.t = 0.0f; }
+    r.i1 = min(r.i0 + 1, n - 1);
+    return r;
+}
+
+// The resized, mean-subtracted pixel at taps (y, x) of a dense uint8 (h0, w0, 3) image: out[c], c = B, G, R.  The one
+// statement of the arithmetic for preprocess_bgr8_kernel and preprocess_bgr8_canvas_kernel.
+__device__ __forceinline__ void bilinear_bgr8(const unsigned char* src, int w0, const BilinearTap& y, const BilinearTap& x,
+                                              double m0, double m1, double m2, float out[3]) {
+    const unsigned char* r0 = src + (long)y.i0 * w0 * 3;
+    const unsigned char* r1 = src + (long)y.i1 * w0 * 3;
+    const double mean[3] = {m0, m1, m2};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float p00 = (float)((double)r0[x.i0 * 3 + c] - mean[c]);
+        const float p01 = (float)((double)r0[x.i1 * 3 + c] - mean[c]);
+        const float p10 = (float)((double)r1[x.i0 * 3 + c] - mean[c]);
+        const float p11 = (float)((double)r1[x.i1 * 3 + c] - mean[c]);
+        const float ha = __fmaf_rn(__fsub_rn(p01, p00), x.t, p00);
+        const float hb = __fmaf_rn(__fsub_rn(p11, p10), x.t, p10);
+        out[c] = __fmaf_rn(__fsub_rn(hb, ha), y.t, ha);
+    }
+}
+
 __global__ void preprocess_bgr8_kernel(const PreArgs a) {
     const long total = (long)a.H * a.W;
     for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < total; p += (long)gridDim.x * blockDim.x) {
         const int y = (int)(p / a.W), x = (int)(p % a.W);
-        const double fyd = ((double)y + 0.5) * a.sy - 0.5;
-        int y0 = (int)floor(fyd);
-        float ty = (float)(fyd - (double)y0);
-        if (y0 < 0) { y0 = 0; ty = 0.0f; }
-        if (y0 >= a.h0 - 1) { y0 = a.h0 - 1; ty = 0.0f; }
-        const int y1 = min(y0 + 1, a.h0 - 1);
-        const double fxd = ((double)x + 0.5) * a.sx - 0.5;
-        int x0 = (int)floor(fxd);
-        float tx = (float)(fxd - (double)x0);
-        if (x0 < 0) { x0 = 0; tx = 0.0f; }
-        if (x0 >= a.w0 - 1) { x0 = a.w0 - 1; tx = 0.0f; }
-        const int x1 = min(x0 + 1, a.w0 - 1);
-        const unsigned char* r0 = a.src + (long)y0 * a.w0 * 3;
-        const unsigned char* r1 = a.src + (long)y1 * a.w0 * 3;
-        const double mean[3] = {a.m0, a.m1, a.m2};
+        float v[3];
+        bilinear_bgr8(a.src, a.w0, bilinear_tap(y, a.sy, a.h0), bilinear_tap(x, a.sx, a.w0), a.m0, a.m1, a.m2, v);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float p00 = (float)((double)r0[x0 * 3 + c] - mean[c]);
-            const float p01 = (float)((double)r0[x1 * 3 + c] - mean[c]);
-            const float p10 = (float)((double)r1[x0 * 3 + c] - mean[c]);
-            const float p11 = (float)((double)r1[x1 * 3 + c] - mean[c]);
-            const float ha = __fmaf_rn(__fsub_rn(p01, p00), tx, p00);
-            const float hb = __fmaf_rn(__fsub_rn(p11, p10), tx, p10);
-            a.out[((long)c * a.H + y) * a.W + x] = __fmaf_rn(__fsub_rn(hb, ha), ty, ha);
-        }
+        for (int c = 0; c < 3; ++c) a.out[((long)c * a.H + y) * a.W + x] = v[c];
     }
+}
+
+// Raw photos straight into a canvas batch's first-layer planes: preprocess_bgr8_kernel + pack_image_c8_kernel(extents) for
+// all N slots in one launch, without the float32 image in between.  Image blockIdx.y is the dense uint8 (h0, w0, 3) block at
+// arena + src_off[n]; its resized extent, source size, offset and 1 / im_scale are device arrays read here, so a captured
+// launch serves any mix of sizes.  One block per stored row [Wc+2][8] of the slot (the last one also zeroes the 8 slack
+// pixels): the row's y taps are computed once per thread, and every stored pixel outside the extent is written as 0.  A
+// slot whose source does not lie inside [0, arena_bytes) or whose source size is not positive is an empty slot.
+struct PreCanvasArgs {
+    const unsigned char* arena; long long arena_bytes;
+    const long long* src_off; const int* src_hw; const double* inv_scale; const int* extents;
+    int Hc, Wc;
+    double m0, m1, m2;
+    __nv_bfloat16 *hi, *lo;
+    long out_elems;
+};
+__global__ void preprocess_bgr8_canvas_kernel(const PreCanvasArgs a) {
+    const int n = blockIdx.y, h = blockIdx.x, WP = a.Wc + 2;
+    __nv_bfloat16* hi = a.hi + n * a.out_elems;
+    __nv_bfloat16* lo = a.lo ? a.lo + n * a.out_elems : nullptr;
+    const int h0 = __ldg(a.src_hw + 2 * n), w0 = __ldg(a.src_hw + 2 * n + 1);
+    const long long off = __ldg(a.src_off + n);
+    const bool live = h0 > 0 && w0 > 0 && off >= 0 && off <= a.arena_bytes && (long long)h0 * w0 <= (a.arena_bytes - off) / 3;
+    const int eh = live ? canvas_extent(a.extents, n, 0, 0, a.Hc) : 0;
+    const int ew = live ? canvas_extent(a.extents, n, 1, 0, a.Wc) : 0;
+    F8 f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f.v[j] = 0.0f;
+    const long row = (long)h * WP;
+    if (h < eh) {
+        const unsigned char* src = a.arena + off;
+        const double inv = __ldg(a.inv_scale + n);
+        const BilinearTap ty = bilinear_tap(h, inv, h0);
+        for (int wp = threadIdx.x; wp < WP; wp += blockDim.x) {
+            F8 g = f;
+            if (wp >= 1 && wp <= ew) bilinear_bgr8(src, w0, ty, bilinear_tap(wp - 1, inv, w0), a.m0, a.m1, a.m2, g.v);
+            store8(hi, lo, (row + wp) * 8, g);
+        }
+    } else {
+        for (int wp = threadIdx.x; wp < WP; wp += blockDim.x) store8(hi, lo, (row + wp) * 8, f);
+    }
+    if (h == a.Hc - 1 && threadIdx.x < 8) store8(hi, lo, (row + WP + threadIdx.x) * 8, f);
 }
 
 // OIHW 3x3 weights (Cin <= 3) -> [1][Cout][32] bf16 hi/lo with the same K order as pack_image_im2col_kernel.
@@ -878,6 +933,33 @@ extern "C" int frcnn_pack_image_c8_batch_ext(const float* x, int N, int C, int H
     FRCNN_REQUIRE(extents, "frcnn_pack_image_c8_batch_ext: extents is NULL");
     return pack_image_c8_n("frcnn_pack_image_c8_batch_ext", x, N, C, H, W, stride_n, stride_c, stride_h, stride_w, extents, y_hi,
                            y_lo, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_preprocess_bgr8_canvas(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                             const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc,
+                                             int Wc, double mean_b, double mean_g, double mean_r, void* y_hi, void* y_lo,
+                                             void* stream) {
+    FRCNN_ENTRY();
+    const char* fn = "frcnn_preprocess_bgr8_canvas";
+    FRCNN_REQUIRE(arena, "%s: arena is NULL", fn);
+    FRCNN_REQUIRE(arena_bytes > 0, "%s: arena_bytes must be positive (got %lld)", fn, arena_bytes);
+    FRCNN_REQUIRE(src_off, "%s: src_off is NULL", fn);
+    FRCNN_REQUIRE(src_hw, "%s: src_hw is NULL", fn);
+    FRCNN_REQUIRE(inv_scale, "%s: inv_scale is NULL", fn);
+    FRCNN_REQUIRE(extents, "%s: extents is NULL", fn);
+    FRCNN_REQUIRE(y_hi, "%s: y_hi is NULL", fn);
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "%s: needs 1 <= N <= 65535 (got N=%d)", fn, N);
+    FRCNN_REQUIRE(Hc > 0 && Wc > 0, "%s: the canvas must be positive (got Hc=%d Wc=%d)", fn, Hc, Wc);
+    PreCanvasArgs a;
+    a.arena = arena; a.arena_bytes = arena_bytes;
+    a.src_off = src_off; a.src_hw = src_hw; a.inv_scale = inv_scale; a.extents = extents;
+    a.Hc = Hc; a.Wc = Wc;
+    a.m0 = mean_b; a.m1 = mean_g; a.m2 = mean_r;
+    a.hi = (__nv_bfloat16*)y_hi; a.lo = (__nv_bfloat16*)y_lo;
+    a.out_elems = (long)frcnn_image_c8_elems(Hc, Wc);
+    preprocess_bgr8_canvas_kernel<<<dim3(Hc, N), 128, 0, (cudaStream_t)stream>>>(a);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
 }
 
 extern "C" int frcnn_pack_conv_weights_c8(const float* w_oihw, int Cout, int Cin, void* w_hi, void* w_lo, void* stream) {

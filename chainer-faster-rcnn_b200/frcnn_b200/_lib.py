@@ -146,6 +146,8 @@ SIGNATURES = {
                                        c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "frcnn_pack_image_c8_batch_ext": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_long, c_long, c_long, c_long, c_void_p,
                                               c_void_p, c_void_p, c_void_p]),
+    "frcnn_preprocess_bgr8_canvas": (c_int, [c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                             c_double, c_double, c_double, c_void_p, c_void_p, c_void_p]),
     "frcnn_conv3x3_c8_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                            c_void_p, c_void_p, c_void_p, c_void_p]),
     "frcnn_roi_pool_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_long, c_int,

@@ -378,7 +378,7 @@ class BatchPlan(object):
             hi = (torch.zeros if zero else torch.empty)(shape, dtype=torch.bfloat16, device=dev)
             return ops.Act(hi, torch.zeros_like(hi) if (x3 and zero) else (torch.empty_like(hi) if x3 else None))
 
-        self.x_in = torch.zeros((N, 3, H, W), dtype=torch.float32, device=dev)
+        self._alloc_input(dev)
         self.acts = [act(N, ops._lib.load().frcnn_image_c8_elems(H, W))]
         h, w_ = H, W
         self.trunk_steps = []          # as ForwardPlan._alloc_trunk
@@ -431,10 +431,18 @@ class BatchPlan(object):
         self.im_h, self.im_w = H, W
         self.n_launches = 0
 
+    def _alloc_input(self, dev):
+        """The static input that the first launch reads: (N,3,H,W) float32 images."""
+        self.x_in = torch.zeros((self.N, 3, self.H, self.W), dtype=torch.float32, device=dev)
+
+    def _pack_input(self):
+        """The first launch: the static input -> the compact first-layer planes acts[0]."""
+        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input, extents=self.extents)
+
     def _run(self):
         w, N, post_n = self.w, self.N, self.post_n
         ext = self.extents
-        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input, extents=ext)
+        self._pack_input()
         n = 1
         i = 0
         k = 0           # 2x2 pools before the current layer: its extents are ceil(extent / 2^k)
@@ -524,24 +532,117 @@ class CanvasBatchPlan(BatchPlan):
     pixels outside an image are computed as zeros, its proposals, RoI bins and clips are its own).  So ONE captured graph
     serves any mix of sizes up to the canvas, and an unused slot (extent 0 x 0) costs nothing but its share of the tiles.
     Every image's results are bit-identical to a ForwardPlan's on that image alone.  Takes ForwardPlan's keyword options
-    except keep_rpn_debug (the debug rows would carry canvas anchor indices) and hwc_input."""
+    except keep_rpn_debug (the debug rows would carry canvas anchor indices) and hwc_input.
 
-    def __init__(self, weights, N, Hc, Wc, **kw):
+    raw_input=True: the plan takes RAW uint8 (h0,w0,3) BGR photos (forward_raw) instead of preprocessed float32 tensors.  Its
+    static input is one device block [descriptor header | pixels] (preprocess.raw_header_layout): the header holds every
+    slot's extents, clip bounds, source size, pixel offset and 1 / im_scale, the pixel area of arena_bytes (default: N
+    sources of up to Hc x Wc pixels) the photos themselves.  The first launch (frcnn_preprocess_bgr8_canvas) resizes,
+    subtracts pixel_means and packs all slots straight into the first-layer planes, so the plan holds no float32 images and
+    one host-to-device copy of that block delivers a whole batch."""
+
+    def __init__(self, weights, N, Hc, Wc, raw_input=False, pixel_means=None, arena_bytes=None, **kw):
         if kw.get("keep_rpn_debug"):
             raise FrcnnError("CanvasBatchPlan has no RPN debug outputs (keep_rpn_debug=True)")
         if kw.get("hwc_input"):
             raise FrcnnError("CanvasBatchPlan takes (3,H,W) images (hwc_input=True)")
+        from . import preprocess
+        self.raw_input = bool(raw_input)
+        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
+                                                              dtype=np.float64).reshape(-1)[:3])
+        self.arena_bytes = int(N) * 3 * int(Hc) * int(Wc) if arena_bytes is None else int(arena_bytes)
+        if self.raw_input and self.arena_bytes < 1:
+            raise FrcnnError("CanvasBatchPlan: arena_bytes must be positive (got %d)" % self.arena_bytes)
         super(CanvasBatchPlan, self).__init__(weights, N, Hc, Wc, **kw)
-        # rows 0 / 1: extents and clip bounds, written with one upload per forward
-        self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=weights.device)
-        self.extents, self.im_info = self._sizes[0], self._sizes[1]
+        if self.raw_input:
+            self._ctor.update(raw_input=True, pixel_means=self.pixel_means, arena_bytes=self.arena_bytes)
+            self.extents, self.im_info = self._hdr["extents"], self._hdr["im_info"]
+        else:
+            # rows 0 / 1: extents and clip bounds, written with one upload per forward
+            self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=weights.device)
+            self.extents, self.im_info = self._sizes[0], self._sizes[1]
         self.image_sizes = [(0, 0)] * self.N
+        self._res_host = None       # pinned mirror of the result blocks (fetch_result)
+
+    def _alloc_input(self, dev):
+        if not self.raw_input:
+            return super(CanvasBatchPlan, self)._alloc_input(dev)
+        from . import preprocess
+        layout, self.header_bytes = preprocess.raw_header_layout(self.N)
+        self.x_in = None
+        self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=dev)
+        self.arena = self.block[self.header_bytes:]
+        tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64}
+        self._hdr = {name: self.block[off:off + 8 * self.N].view(tdt[dt]).view((self.N, 2) if items == 2 else (self.N,))
+                     for name, (off, dt, items) in layout.items()}
+        self._stage = None          # pinned host mirror of the block + the event of its last upload (forward_raw)
+
+    def _pack_input(self):
+        if not self.raw_input:
+            return super(CanvasBatchPlan, self)._pack_input()
+        h = self._hdr
+        ops.preprocess_pack_canvas(self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"], self.H, self.W,
+                                   self.pixel_means, out=self.acts[0])
+
+    def raw_batch_header(self, shapes, img_infos=None):
+        """preprocess.raw_batch_header for this plan's slots, canvas and arena (raises FrcnnError when something does not fit)."""
+        from . import preprocess
+        if not self.raw_input:
+            raise FrcnnError("CanvasBatchPlan: raw photos need a plan built with raw_input=True")
+        return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
+
+    def forward_raw(self, images, img_infos=None):
+        """images: a list of at most N RAW uint8 (h0,w0,3) BGR photos of any sizes -- all numpy arrays (copied into a pinned
+        mirror of the block and uploaded with ONE host-to-device copy, header included) or all CUDA tensors (copied into the
+        arena on the device).  Each is resized as forward.py:34-45 does (preprocess.plan_size) inside the first launch.
+        img_infos: optional per-image clip bounds, default the resized (H_n, W_n); forward.py passes (H_n, H_n) (SURVEY.md
+        Q7).  Raises FrcnnError before anything is queued if a resized image does not fit the canvas or the photos do not
+        fit the arena.  Returns BatchPlan.forward's (list of prob, list of boxes, counts) and the list of im_scale."""
+        from . import preprocess
+        images = list(images)
+        on_host = all(isinstance(x, np.ndarray) for x in images)
+        if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
+            raise FrcnnError("forward_raw: the images must be all numpy arrays or all CUDA tensors")
+        for n, x in enumerate(images):
+            if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
+                raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
+        hdr, scales, used = self.raw_batch_header([x.shape[:2] for x in images], img_infos)
+        offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
+        cur = torch.cuda.current_stream()
+        if self._stage is None:
+            self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
+        pin, done = self._stage
+        done.synchronize()                    # the previous upload has left the pinned mirror
+        pin.np[:hdr.size] = hdr
+        if on_host:
+            for n, x in enumerate(images):
+                ops.host_copy(pin.ptr + self.header_bytes + int(offs[n]), np.ascontiguousarray(x))
+            pin.h2d(self.block, cur, nbytes=self.header_bytes + used)
+        else:
+            pin.h2d(self.block, cur, nbytes=self.header_bytes)
+            for n, x in enumerate(images):
+                self.arena[int(offs[n]):int(offs[n]) + x.numel()].copy_(x.contiguous().view(-1), non_blocking=True)
+        done.record(cur)
+        self.image_sizes = [tuple(int(v) for v in e) for e in preprocess.raw_header_views(hdr, self.N)["extents"]]
+        return self.forward(None) + (scales,)
+
+    def fetch_result(self):
+        """ONE device-to-host copy of all N result blocks on the current stream, waited for: unpack_result's list (numpy
+        views into a pinned block, valid until the next fetch)."""
+        if self._res_host is None:
+            self._res_host = ops.PinnedBlock((int(self.result.numel()),), np.int32)
+        cur = torch.cuda.current_stream()
+        self._res_host.d2h(self.result, cur, nbytes=4 * self.result_words())
+        ops.stream_synchronize(cur)
+        return self.unpack_result(self._res_host.np)
 
     def forward(self, images=None, img_infos=None):
         """images: a list of at most N (3,H_n,W_n) float32 CUDA tensors with H_n <= Hc and W_n <= Wc, copied into the
         top-left of slots 0, 1, ...; the remaining slots are empty (count 0).  img_infos: optional per-image clip bounds
         (im_h, im_w) (forward.py passes (H, H), SURVEY.md Q7); default (H_n, W_n).  None reuses the current slots, sizes and
         clip bounds.  Returns BatchPlan.forward's (list of prob, list of boxes, counts)."""
+        if images is not None and self.raw_input:
+            raise FrcnnError("CanvasBatchPlan(raw_input=True) takes raw photos through forward_raw")
         if images is not None:
             images = list(images)
             if len(images) > self.N:
@@ -574,7 +675,7 @@ class LanePool(object):
 
     def __init__(self, plan, lanes=3):
         self.plans = [plan] + [plan.clone() for _ in range(max(1, int(lanes)) - 1)]
-        dev = plan.x_in.device
+        dev = plan.w.device
         self.streams = [torch.cuda.Stream(device=dev) for _ in self.plans]
         for p, st in zip(self.plans, self.streams):
             if p.use_graph and p.graph is None:
@@ -693,6 +794,86 @@ class StreamRunner(object):
         self.pool.join()
         return counts
 
+
+class CanvasStreamRunner(object):
+    """Host-to-host streaming front end of a CanvasBatchPlan(raw_input=True, with_detect=True): RAW uint8 photos of mixed
+    sizes come from host memory, N per graph replay, and every image's detections (preprocess.result_detections, boxes in
+    source-image coordinates) go back to the host.  A ring of `depth` slots, each a pinned mirror of the plan's [header |
+    pixels] block and a pinned result block.  Per batch the host copies the photos and the header into the mirror, and the
+    GPU gets ONE H2D copy on the copy stream (straight into the lane plan's block, once that lane's previous replay is
+    over: the header is read throughout the graph), the graph on the lane's compute stream and ONE D2H of the result blocks.
+    With lanes > 1 a batch's upload and graph overlap the other lanes' graphs.  The host blocks only when it reuses a slot."""
+
+    def __init__(self, plan, depth=2, lanes=1):
+        base = plan.plans[0] if isinstance(plan, LanePool) else plan
+        if not (isinstance(base, CanvasBatchPlan) and base.raw_input and base.with_detect):
+            raise FrcnnError("CanvasStreamRunner needs a CanvasBatchPlan(raw_input=True, with_detect=True)")
+        self.pool = plan if isinstance(plan, LanePool) else LanePool(plan, lanes)
+        self.plan = plan = base
+        self.depth = D = max(2, int(depth), 2 * len(self.pool))
+        self.copy_stream = torch.cuda.Stream(device=plan.w.device)
+        self.stage = [ops.PinnedBlock((plan.block.numel(),), np.uint8) for _ in range(D)]
+        self.n_words = plan.result_words()
+        self.res = [ops.PinnedBlock((self.n_words,), np.int32) for _ in range(D)]
+        self.h2d_done = [torch.cuda.Event() for _ in range(D)]
+        self.step_done = [torch.cuda.Event() for _ in range(D)]
+        self.lane_done = [torch.cuda.Event() for _ in self.pool.plans]
+        self.h2d_copies = self.h2d_bytes = 0          # totals over run() calls
+
+    def _deliver(self, b, batches, results, on_result):
+        s, N = b % self.depth, self.plan.N
+        self.step_done[s].synchronize()
+        from . import preprocess
+        res = self.plan.unpack_result(self.res[s].np)
+        for n, im_scale in enumerate(batches[b][1]):
+            dets = preprocess.result_detections(res[n], im_scale)
+            results.append(dets)
+            if on_result is not None:
+                on_result(b * N + n, dets, im_scale)
+
+    def run(self, raw_images, on_result=None, img_infos=None):
+        """raw_images: sequence of uint8 (h0,w0,3) numpy arrays (pageable or pinned).  Every batch is checked against the
+        canvas and the arena first: FrcnnError is raised before anything is queued.  Calls on_result(i, detections,
+        im_scale) in image order and returns the list of detections; a last partial batch runs with its other slots empty."""
+        plan, D, L, N = self.plan, self.depth, len(self.pool), self.plan.N
+        raw_images = list(raw_images)
+        for i, x in enumerate(raw_images):
+            if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or x.ndim != 3 or x.shape[2] != 3:
+                raise FrcnnError("CanvasStreamRunner: image %d is not a uint8 (h, w, 3) numpy array" % i)
+        from . import preprocess
+        batches = []
+        for s0 in range(0, len(raw_images), N):
+            chunk = raw_images[s0:s0 + N]
+            batches.append(plan.raw_batch_header([x.shape[:2] for x in chunk], None if img_infos is None else img_infos[s0:s0 + N]))
+        results = []
+        self.pool.fork()
+        self.copy_stream.wait_stream(torch.cuda.current_stream())
+        for b, (hdr, scales, used) in enumerate(batches):
+            s, k = b % D, b % L
+            lane, cur = self.pool.plans[k], self.pool.streams[k]
+            if b >= D:
+                self._deliver(b - D, batches, results, on_result)         # slot reuse: batch b-D is finished and handed over
+            pin = self.stage[s]
+            pin.np[:hdr.size] = hdr
+            offs = preprocess.raw_header_views(hdr, N)["src_off"]
+            for n in range(len(scales)):
+                ops.host_copy(pin.ptr + plan.header_bytes + int(offs[n]), np.ascontiguousarray(raw_images[b * N + n]))
+            if b >= L:
+                self.copy_stream.wait_event(self.lane_done[k])            # the lane's previous replay no longer reads its block
+            pin.h2d(lane.block, self.copy_stream, nbytes=plan.header_bytes + used)
+            self.h2d_done[s].record(self.copy_stream)
+            self.h2d_copies += 1
+            self.h2d_bytes += plan.header_bytes + used
+            with torch.cuda.stream(cur):
+                cur.wait_event(self.h2d_done[s])
+                lane.forward(None)
+                self.lane_done[k].record(cur)
+                self.res[s].d2h(lane.result, cur, nbytes=4 * self.n_words)
+                self.step_done[s].record(cur)
+        for b in range(max(0, len(batches) - D), len(batches)):
+            self._deliver(b, batches, results, on_result)
+        self.pool.join()
+        return results
 
 
 class _PlanLease(object):
@@ -843,6 +1024,40 @@ class Engine(object):
             R = counts.cpu().tolist()
             res = [(probs[n][:R[n]], boxes[n][:R[n]]) for n in range(len(chunk))]
             out += [(a.clone(), b.clone()) for a, b in res] if len(images) > N else res
+        return out
+
+    def raw_canvas_plan(self, raw_images, N=None, canvas=None, nms_thresh=0.3, conf=0.8, **overrides):
+        """The CanvasBatchPlan(raw_input=True, with_detect=True) that serves `raw_images` N per replay: the canvas defaults
+        to the largest resized H and W, each rounded up to a multiple of 64, and the arena to N times the largest photo,
+        rounded up to 1 MiB."""
+        from . import preprocess
+        shapes = [tuple(int(v) for v in x.shape[:2]) for x in raw_images]
+        N = len(shapes) if N is None else int(N)
+        if canvas is None:
+            sizes = [preprocess.plan_size(h0, w0)[1:] for h0, w0 in shapes]
+            canvas = (ops.round_up(max(s[0] for s in sizes), 64), ops.round_up(max(s[1] for s in sizes), 64))
+        arena = N * ops.round_up(max(3 * h0 * w0 for h0, w0 in shapes), preprocess.RAW_ALIGN)
+        kw = dict(raw_input=True, arena_bytes=ops.round_up(arena, 1 << 20), with_detect=True, det_nms_thresh=nms_thresh,
+                  det_conf=conf)
+        kw.update(overrides)
+        return self.canvas_plan(N, int(canvas[0]), int(canvas[1]), **kw)
+
+    def detect_images(self, raw_images, N=None, canvas=None, nms_thresh=0.3, conf=0.8, img_infos=None, **overrides):
+        """forward.py's whole loop on RAW photos of any sizes: a list of uint8 (h0,w0,3) BGR arrays -> for each image the list
+        preprocess.detections gives, (cls_id, x1, y1, x2, y2, score) in source-image coordinates.  N images per graph
+        replay (default: all of them), one upload and one download per replay; the canvas as raw_canvas_plan picks it.
+        img_infos: optional per-image clip bounds (forward.py passes the resized (H, H))."""
+        from . import preprocess
+        raw_images = list(raw_images)
+        if not raw_images:
+            return []
+        p = self.raw_canvas_plan(raw_images, N, canvas, nms_thresh, conf, **overrides)
+        out = []
+        for s in range(0, len(raw_images), p.N):
+            chunk = raw_images[s:s + p.N]
+            scales = p.forward_raw(chunk, None if img_infos is None else img_infos[s:s + p.N])[3]
+            res = p.fetch_result()
+            out += [preprocess.result_detections(res[n], scales[n]) for n in range(len(chunk))]
         return out
 
 

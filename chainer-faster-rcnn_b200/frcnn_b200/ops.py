@@ -250,6 +250,34 @@ def pack_image_c8_batch(x_nchw, precision="bf16x3", out=None, hwc_memory=False, 
     return out
 
 
+def preprocess_pack_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc, pixel_means, precision="bf16x3", out=None):
+    """frcnn_preprocess_bgr8_canvas: raw uint8 BGR photos -> the compact first-layer planes of an N-slot Hc x Wc canvas, Act
+    [N, frcnn_image_c8_elems(Hc,Wc)], in one launch (resize + mean subtraction + pack; 0 outside every image).  arena: dense
+    uint8 CUDA tensor holding image n's (h0,w0,3) pixels at byte src_off[n] (int64 [N]); src_hw: int32 [N, 2] (h0, w0), <= 0
+    = empty slot; inv_scale: float64 [N] = 1 / im_scale; extents: int32 [N, 2] resized (H, W).  All of them device tensors
+    read when the kernel runs."""
+    _need_cuda(arena, src_off, src_hw, inv_scale, extents)
+    N = int(extents.shape[0])
+    if arena.dtype != torch.uint8 or not arena.is_contiguous():
+        raise FrcnnError("preprocess_pack_canvas: arena must be a dense uint8 CUDA tensor")
+    for t, dt, what in ((src_off, torch.int64, "src_off"), (inv_scale, torch.float64, "inv_scale")):
+        if t.dtype != dt or tuple(t.shape) != (N,) or not t.is_contiguous():
+            raise FrcnnError("preprocess_pack_canvas: %s must be a dense %s [%d] CUDA tensor" % (what, dt, N))
+    lib = _lib.load()
+    n = lib.frcnn_image_c8_elems(Hc, Wc)
+    if out is None:
+        hi = torch.empty((N, n), dtype=torch.bfloat16, device=arena.device)
+        out = Act(hi, torch.empty_like(hi) if precision == "bf16x3" else None)
+    if out.hi.numel() < N * n:
+        raise FrcnnError("preprocess_pack_canvas: output holds %d elements, needs %d" % (out.hi.numel(), N * n))
+    m = np.asarray(pixel_means, dtype=np.float64).reshape(-1)
+    check(lib.frcnn_preprocess_bgr8_canvas(_p(arena), arena.numel(), _p(src_off), _per_image_pairs(src_hw, N, "src_hw"),
+                                           _p(inv_scale), _per_image_pairs(extents, N, "extents"), N, int(Hc), int(Wc),
+                                           float(m[0]), float(m[1]), float(m[2]), _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_preprocess_bgr8_canvas")
+    return out
+
+
 def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None, extents=None):
     """frcnn_conv3x3_c8_batch: conv1_1 over N compact images (pack_image_c8_batch) -> Act [N,H,W,Cout].  extents: int32
     [N, 2] device image sizes in H x W canvas slots (frcnn_conv3x3_c8_batch_ext: pixels outside are written as 0)."""
@@ -460,6 +488,13 @@ class PinnedBlock(object):
                 self.ptr = None
         except Exception:          # noqa: BLE001  (interpreter shutdown)
             pass
+
+
+def host_copy(dst_ptr, arr):
+    """frcnn_host_copy: a C-contiguous numpy array -> host memory at address dst_ptr (e.g. inside a PinnedBlock)."""
+    if not arr.flags.c_contiguous:
+        raise FrcnnError("host_copy: need a C-contiguous array")
+    check(_lib.load().frcnn_host_copy(ctypes.c_void_p(int(dst_ptr)), ctypes.c_void_p(arr.ctypes.data), arr.nbytes), "frcnn_host_copy")
 
 
 def memcpy_h2d_async(dst, src_ptr, nbytes, stream):

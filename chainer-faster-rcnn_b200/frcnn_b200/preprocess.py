@@ -44,16 +44,78 @@ def img_preprocessing(orig_img, pixel_means=PIXEL_MEANS, max_size=1000, scale=60
     return out, im_scale
 
 
-def detections(cls_prob, pred_boxes, im_scale, nms_thresh=0.3, conf=0.8, count=None):
-    """forward.py:48-59 without the drawing: for every foreground class, per-class NMS (device), confidence
-    filter, boxes divided by im_scale and truncated to int like `map(int, dets[i, :4] / im_scale)`.
-    Returns a list of (cls_id, x1, y1, x2, y2, score) in the reference's iteration order."""
-    keep_idx, keep_count, conf_count = ops.detect(cls_prob, pred_boxes, count, nms_thresh, conf)
-    keep_idx, conf_count = keep_idx.cpu().numpy(), conf_count.cpu().numpy()
-    prob, boxes = cls_prob.detach().cpu().numpy(), pred_boxes.detach().cpu().numpy()
+def result_detections(res, im_scale):
+    """The list forward.py:50-59 draws, from host arrays: res holds prob [R,NC], boxes [R,4NC] and the per-class NMS lists
+    keep_idx [NC-1, >=R] / conf_count [NC-1] (an unpacked result block of a with_detect plan, or detections() below).
+    Boxes are divided by im_scale and truncated like `map(int, dets[i, :4] / im_scale)`; (cls_id, x1, y1, x2, y2, score)
+    in the reference's iteration order."""
+    prob, boxes, keep_idx, conf_count = res["prob"], res["boxes"], res["keep_idx"], res["conf_count"]
     out = []
     for c in range(1, prob.shape[1]):
         for r in keep_idx[c - 1, :conf_count[c - 1]]:
             x1, y1, x2, y2 = map(int, boxes[r, 4 * c:4 * c + 4] / im_scale)
             out.append((c, x1, y1, x2, y2, float(prob[r, c])))
     return out
+
+
+def detections(cls_prob, pred_boxes, im_scale, nms_thresh=0.3, conf=0.8, count=None):
+    """forward.py:48-59 without the drawing: for every foreground class, per-class NMS (device), confidence
+    filter, boxes divided by im_scale and truncated to int like `map(int, dets[i, :4] / im_scale)`.
+    Returns a list of (cls_id, x1, y1, x2, y2, score) in the reference's iteration order."""
+    keep_idx, keep_count, conf_count = ops.detect(cls_prob, pred_boxes, count, nms_thresh, conf)
+    return result_detections(dict(prob=cls_prob.detach().cpu().numpy(), boxes=pred_boxes.detach().cpu().numpy(),
+                                  keep_idx=keep_idx.cpu().numpy(), conf_count=conf_count.cpu().numpy()), im_scale)
+
+
+# ---- raw photos into a canvas batch (engine.CanvasBatchPlan(raw_input=True)): one block [descriptor header | pixels]
+# The header holds, for the N slots, the five arrays frcnn_preprocess_bgr8_canvas and the later *_batch_ext kernels read;
+# the pixels follow at header_bytes.  Host and device copies share the layout, so one H2D copy delivers a whole batch.
+RAW_FIELDS = (("extents", np.int32, 2), ("im_info", np.int32, 2), ("src_hw", np.int32, 2), ("src_off", np.int64, 1),
+              ("inv_scale", np.float64, 1))
+RAW_ALIGN = 64          # images start on 64-byte boundaries of the pixel area (the kernel itself reads single bytes)
+
+
+def raw_header_layout(N):
+    """({name: (byte offset, dtype, per-slot items)}, header_bytes): every array takes 8 * N bytes, and the pixels start at
+    header_bytes, a multiple of 256."""
+    return ({name: (8 * N * k, dt, items) for k, (name, dt, items) in enumerate(RAW_FIELDS)},
+            ops.round_up(8 * N * len(RAW_FIELDS), 256))
+
+
+def raw_header_views(buf, N):
+    """numpy views of the header arrays inside `buf`, a uint8 array that starts with a header for N slots."""
+    layout, _ = raw_header_layout(N)
+    return {name: buf[off:off + 8 * N].view(dt).reshape((N, 2) if items == 2 else (N,)) for name, (off, dt, items) in layout.items()}
+
+
+def raw_batch_header(shapes, N, Hc, Wc, arena_bytes, img_infos=None, scale=600, max_size=1000):
+    """The header of one batch of raw images: shapes = the (h0, w0) of at most N uint8 BGR images, laid out one after the
+    other (RAW_ALIGN) in a pixel area of arena_bytes; the remaining slots are empty.  img_infos: per-image clip bounds,
+    default the resized (H, W).  Returns (uint8 header array, [im_scale], pixel bytes used).  Raises FrcnnError when there
+    are too many images, a resized image does not fit the Hc x Wc canvas, or the pixels do not fit the arena."""
+    shapes = [(int(h0), int(w0)) for h0, w0 in shapes]
+    if len(shapes) > N:
+        raise _lib.FrcnnError("raw batch: %d images for %d slots" % (len(shapes), N))
+    if img_infos is not None and len(img_infos) != len(shapes):
+        raise _lib.FrcnnError("raw batch: %d img_infos for %d images" % (len(img_infos), len(shapes)))
+    hdr = np.zeros((raw_header_layout(N)[1],), dtype=np.uint8)
+    v = raw_header_views(hdr, N)
+    scales, used = [], 0
+    for n, (h0, w0) in enumerate(shapes):
+        if h0 < 1 or w0 < 1:
+            raise _lib.FrcnnError("raw batch: image %d has no pixels (%d x %d)" % (n, h0, w0))
+        im_scale, H, W = plan_size(h0, w0, scale, max_size)
+        if not (0 < H <= Hc and 0 < W <= Wc):
+            raise _lib.FrcnnError("raw batch: image %d (%d x %d) resizes to %d x %d, which does not fit a %d x %d canvas" %
+                                  (n, h0, w0, H, W, Hc, Wc))
+        off = ops.round_up(used, RAW_ALIGN)
+        used = off + 3 * h0 * w0
+        if used > arena_bytes:
+            raise _lib.FrcnnError("raw batch: images 0..%d need %d bytes, the arena holds %d" % (n, used, arena_bytes))
+        v["extents"][n] = (H, W)
+        v["im_info"][n] = (H, W) if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
+        v["src_hw"][n] = (h0, w0)
+        v["src_off"][n] = off
+        v["inv_scale"][n] = 1.0 / im_scale
+        scales.append(im_scale)
+    return hdr, scales, used

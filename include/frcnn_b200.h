@@ -265,6 +265,22 @@ int frcnn_pack_image_c8_batch_ext(const float* x, int N, int C, int H, int W, lo
                                   long stride_w, const int* extents, void* y_hi, void* y_lo, void* stream);
 int frcnn_conv3x3_c8_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo,
                                const float* bias, int Cout, int relu, const int* extents, void* y_hi, void* y_lo, void* stream);
+/* Raw photos into a canvas batch in ONE launch: frcnn_preprocess_bgr8 + frcnn_pack_image_c8_batch_ext for all N slots,
+ * without the float32 image in between.  Image n is the dense uint8 [h0,w0,3] BGR block at arena + src_off[n]; the planes
+ * y_hi / y_lo (frcnn_image_c8_elems(Hc, Wc) elements per slot, y_lo may be NULL) receive, inside the image's resized extent,
+ * bit for bit what frcnn_preprocess_bgr8 followed by the pack writes, and 0 at every other stored pixel (pad columns and
+ * slack included).  Everything per image is DEVICE memory read when the kernel runs, so a launch captured in a CUDA graph
+ * serves any mix of sizes:
+ *   src_off   int64  [N]     byte offset of the image inside the arena
+ *   src_hw    int32  [N][2]  (h0, w0); a component <= 0 marks an empty slot
+ *   inv_scale double [N]     1.0 / im_scale, divided on the host in double as frcnn_preprocess_bgr8 does
+ *   extents   int32  [N][2]  the resized (H, W), the array the other *_batch_ext entries read, clamped to the canvas
+ * A slot whose source does not lie inside [0, arena_bytes) (negative offset, offset + 3*h0*w0 > arena_bytes in 64-bit
+ * arithmetic) is treated as empty, and a clamped extent only shrinks what is written: no value of these arrays moves an
+ * access outside the arena or the planes.  NULL pointers, N outside 1..65535 or a non-positive canvas -> FRCNN_ERR_ARG. */
+int frcnn_preprocess_bgr8_canvas(const unsigned char* arena, long long arena_bytes, const long long* src_off, const int* src_hw,
+                                 const double* inv_scale, const int* extents, int N, int Hc, int Wc, double mean_b,
+                                 double mean_g, double mean_r, void* y_hi, void* y_lo, void* stream);
 
 /* Same with an explicit source layout: element (c, h, w) is x[c*stride_c + h*stride_h + w*stride_w] (in floats).
  * (H*W, W, 1) = dense (C,H,W); (1, W*C, C) = dense (H,W,C) memory, which is what forward.py:45's
