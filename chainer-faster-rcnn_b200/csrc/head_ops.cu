@@ -4,6 +4,7 @@
 //   frcnn_roi_pool        : F.roi_pooling_2d(.., 7, 7, 1/16)     (models/faster_rcnn.py:123-126)
 //   frcnn_head_decode     : softmax + per-class decode + clip    (models/faster_rcnn.py:175-178)
 //   frcnn_detect          : per-class NMS + confidence filter    (forward.py:48-57)
+//   frcnn_detection_lists_batch : the detection lists drawn     (forward.py:50-59)
 // All are HBM/L2-bound: 16-byte vector accesses along the channel axis (NHWC), grids sized to
 // cover the tensor with >= 2 waves of 132 SMs where the tensor is large enough.
 #include <stdarg.h>
@@ -810,6 +811,86 @@ __global__ void __launch_bounds__(kDetThreads) detect_barrier_kernel(const float
     }
 }
 
+// ------------------------------------------------------------------------------------------ detection lists
+// The list forward.py:50-59 draws (preprocess.result_detections) from the per-class NMS lists of frcnn_detect: for class
+// c = 1 .. NC-1 in order, the first conf_count[c-1] entries r of its keep list give the row
+//     (c, int(x1 / im_scale), int(y1 / im_scale), int(x2 / im_scale), int(y2 / im_scale)),  score prob[r, c].
+// `boxes[r, 4c:4c+4] / im_scale` divides a float32 row by a Python float; under NumPy >= 2 (NEP 50, the repository's NumPy)
+// the Python float is a weak scalar, so the quotient is the float32 division by float32(im_scale) -- __fdiv_rn by the
+// round-to-nearest float of the double -- and int() truncates it toward zero.  (Multiplying by a float reciprocal, or dividing
+// in double, gives different bits.)  The one deviation: NaN and +-inf make int() raise and a quotient outside the int32
+// range has no int32 value; here they convert as cvt.rzi.s32.f32 does (NaN -> 0, saturation to the int32 range), the rule
+// of roi_coord (DESIGN.md 2).  The graph's boxes are clipped to the image, so it never gets there.
+// One CTA per image: the classes go in chunks of kListThreads, a block scan over the chunk's counts gives every class its
+// output offset, and then the chunk's rows are written in parallel (row t finds its class by a binary search of the offsets).
+constexpr int kListThreads = 256;
+struct ListStrides { long prob, boxes, keep_idx, conf_count; };
+
+__global__ void __launch_bounds__(kListThreads) detection_lists_kernel(const float* prob, const float* boxes, const int* keep_idx,
+                                                                     const int* conf_count, const double* im_scale, int R_cap,
+                                                                     int NC, const ListStrides is, int* dets, float* scores,
+                                                                     int* det_count) {
+    grid_dep_wait();
+    const long img = blockIdx.x;
+    prob += img * is.prob;
+    boxes += img * is.boxes;
+    keep_idx += img * is.keep_idx;
+    conf_count += img * is.conf_count;
+    const long cap = (long)(NC - 1) * R_cap;
+    dets += img * cap * 5;
+    scores += img * cap;
+    const float s = __double2float_rn(im_scale[img]);
+    __shared__ int s_rel[kListThreads];                  // output offset of the chunk's classes, relative to the chunk
+    __shared__ int s_warp[kListThreads / 32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int carry = 0;                                       // rows of the classes before the chunk
+    for (int c0 = 0; c0 < NC - 1; c0 += kListThreads) {
+        const int k = c0 + tid;
+        const int n = k < NC - 1 ? min(max(conf_count[k], 0), R_cap) : 0;
+        int incl = n;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        int before = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kListThreads / 32; ++w) {
+            before += w < warp ? s_warp[w] : 0;
+            total += s_warp[w];
+        }
+        s_rel[tid] = before + incl - n;
+        __syncthreads();
+        const int nc = min(kListThreads, NC - 1 - c0);
+        for (int t = tid; t < total; t += kListThreads) {
+            int lo = 0, hi = nc;                         // the last class j with s_rel[j] <= t (it holds row t: t < s_rel[j+1])
+            while (hi - lo > 1) {
+                const int mid = (lo + hi) >> 1;
+                if (s_rel[mid] <= t) lo = mid; else hi = mid;
+            }
+            const int c = c0 + lo + 1;
+            const int r = keep_idx[(long)(c - 1) * R_cap + (t - s_rel[lo])];
+            int* d = dets + (long)(carry + t) * 5;
+            d[0] = c;
+            if (r >= 0 && r < R_cap) {
+                const float* b = boxes + (long)r * 4 * NC + 4 * c;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) d[1 + q] = __float2int_rz(__fdiv_rn(b[q], s));
+                scores[carry + t] = prob[(long)r * NC + c];
+            } else {                                     // not an index frcnn_detect writes: nothing is read
+#pragma unroll
+                for (int q = 0; q < 4; ++q) d[1 + q] = 0;
+                scores[carry + t] = 0.0f;
+            }
+        }
+        carry += total;
+        __syncthreads();                                 // s_rel / s_warp are rewritten by the next chunk
+    }
+    if (tid == 0) det_count[img] = carry;
+}
+
 static int grid_for(long total, int block) {
     long g = (total + block - 1) / block;
     const long cap = 132l * 16;
@@ -1237,4 +1318,31 @@ extern "C" int frcnn_detect_batch(int N, const float* prob, long prob_stride, co
     const DetectStrides is = {prob_stride, boxes_stride, count_stride, keep_idx_stride, keep_count_stride, conf_count_stride};
     return detect_n("frcnn_detect_batch", N, prob, boxes, counts, R_cap, num_classes, nms_thresh, conf, keep_idx, keep_count, conf_count,
                     is, (cudaStream_t)stream);
+}
+
+extern "C" int frcnn_detection_lists_batch(int N, const float* prob, long prob_stride, const float* boxes, long boxes_stride,
+                                           const int* keep_idx, long keep_idx_stride, const int* conf_count, long conf_count_stride,
+                                           const double* im_scale, int R_cap, int num_classes, int* out_dets, float* out_scores,
+                                           int* out_det_count, void* stream) {
+    FRCNN_ENTRY();
+    const char* fn = "frcnn_detection_lists_batch";
+    FRCNN_REQUIRE(prob, "%s: prob is NULL", fn);
+    FRCNN_REQUIRE(boxes, "%s: boxes is NULL", fn);
+    FRCNN_REQUIRE(keep_idx, "%s: keep_idx is NULL", fn);
+    FRCNN_REQUIRE(conf_count, "%s: conf_count is NULL", fn);
+    FRCNN_REQUIRE(im_scale, "%s: im_scale is NULL", fn);
+    FRCNN_REQUIRE(out_dets, "%s: out_dets is NULL", fn);
+    FRCNN_REQUIRE(out_scores, "%s: out_scores is NULL", fn);
+    FRCNN_REQUIRE(out_det_count, "%s: out_det_count is NULL", fn);
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "%s: N must be in [1,65535] (got N=%d)", fn, N);
+    FRCNN_REQUIRE(R_cap >= 1, "%s: R_cap must be >= 1 (got R_cap=%d)", fn, R_cap);
+    FRCNN_REQUIRE(num_classes >= 2, "%s: num_classes must be >= 2 (got num_classes=%d)", fn, num_classes);
+    FRCNN_REQUIRE((long)(num_classes - 1) * R_cap * 5 <= 0x7fffffffl, "%s: (num_classes-1) * R_cap = %ld rows is too large", fn,
+                  (long)(num_classes - 1) * R_cap);
+    FRCNN_REQUIRE(prob_stride >= 0 && boxes_stride >= 0 && keep_idx_stride >= 0 && conf_count_stride >= 0,
+                  "%s: image strides must be >= 0", fn);
+    const ListStrides is = {prob_stride, boxes_stride, keep_idx_stride, conf_count_stride};
+    FRCNN_CUDA_OK(launch_pdl(detection_lists_kernel, dim3(N), dim3(kListThreads), 0, (cudaStream_t)stream, prob, boxes, keep_idx,
+                             conf_count, im_scale, R_cap, num_classes, is, out_dets, out_scores, out_det_count));
+    return FRCNN_OK;
 }

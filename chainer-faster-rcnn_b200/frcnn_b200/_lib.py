@@ -156,6 +156,15 @@ SIGNATURES = {
                                             c_int, c_void_p, c_void_p, c_long, c_void_p, c_long, c_void_p]),
     "frcnn_detect": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double, c_float, c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "frcnn_detection_lists_batch": (c_int, [c_int, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p,
+                                            c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_forward_vgg16_canvas_workspace_bytes": (c_size_t, [c_void_p, c_int]),
+    "frcnn_forward_vgg16_canvas": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
+                                           c_void_p, c_void_p, c_void_p]),
+    "frcnn_raw_header_bytes": (c_size_t, [c_int]),
+    "frcnn_detect_vgg16_raw": (c_int, [c_void_p, c_void_p, c_int, c_void_p, ctypes.c_longlong, c_double, c_double, c_double, c_void_p,
+                                       c_double, c_float, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -1061,6 +1061,24 @@ class Engine(object):
         return out
 
 
+def _c_structs(weights, H, W, anchors, pre_n, post_n, nms_thresh, min_size, feat_stride):
+    """(device anchor table, frcnn_forward_config, frcnn_vgg16_weights) of the whole-graph C entries, filled from a
+    PackedWeights; the structs point into the weights' and the anchor table's device memory."""
+    from . import _lib
+    anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(weights.device)
+    cfg = _lib.ForwardConfig(H, W, weights.num_classes, weights.n_anchors, feat_stride, pre_n, post_n, min_size,
+                             float(nms_thresh), 1 if weights.precision == "bf16x3" else 0)
+    p = lambda t: None if t is None else t.data_ptr()                     # noqa: E731
+    layer = lambda hi, lo, b: _lib.PackedLayer(p(hi), p(lo), p(b))         # noqa: E731
+    wt = _lib.Vgg16Weights()
+    for i, item in enumerate([it for it in VGG16_LAYERS if it != "pool"]):
+        wt.conv[i] = layer(*weights.convs[item[0]])
+    wt.rpn3, wt.rpn_heads = layer(*weights.rpn3), layer(*weights.rpn_heads)
+    wt.fc6, wt.fc7, wt.head = layer(*weights.fc6), layer(*weights.fc7), layer(*weights.head)
+    wt.anchors = anchors.data_ptr()
+    return anchors, cfg, wt
+
+
 class CForward(object):
     """frcnn_forward_vgg16: the whole forward path behind the single C-ABI entry (include/frcnn_b200.h) -- what a caller
     without Python binds.  Same kernels, same order as BatchPlan._run; this wrapper only fills the C structs from a
@@ -1074,18 +1092,8 @@ class CForward(object):
         self._lib, self._ct = _lib.load(), ctypes
         self.w, self.H, self.W, self.post_n, self.N = weights, H, W, post_n, int(N)
         dev = weights.device
-        self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
-        cfg = _lib.ForwardConfig(H, W, weights.num_classes, weights.n_anchors, feat_stride, pre_n, post_n, min_size,
-                                 float(nms_thresh), 1 if weights.precision == "bf16x3" else 0)
-        p = lambda t: None if t is None else t.data_ptr()                     # noqa: E731
-        layer = lambda hi, lo, b: _lib.PackedLayer(p(hi), p(lo), p(b))         # noqa: E731
-        wt = _lib.Vgg16Weights()
-        for i, item in enumerate([it for it in VGG16_LAYERS if it != "pool"]):
-            wt.conv[i] = layer(*weights.convs[item[0]])
-        wt.rpn3, wt.rpn_heads = layer(*weights.rpn3), layer(*weights.rpn_heads)
-        wt.fc6, wt.fc7, wt.head = layer(*weights.fc6), layer(*weights.fc7), layer(*weights.head)
-        wt.anchors = self.anchors.data_ptr()
-        self.cfg, self.wt = cfg, wt
+        self.anchors, self.cfg, self.wt = _c_structs(weights, H, W, anchors, pre_n, post_n, nms_thresh, min_size, feat_stride)
+        cfg = self.cfg
         if self.N == 1:
             nbytes = self._lib.frcnn_forward_workspace_bytes(ctypes.byref(cfg))
         else:
@@ -1117,3 +1125,159 @@ class CForward(object):
             _lib.check(self._lib.frcnn_forward_vgg16_batch(ct.byref(self.cfg), ct.byref(self.wt), self.N, *args),
                        "frcnn_forward_vgg16_batch")
         return self.prob, self.boxes, self.count
+
+
+class CCanvasForward(object):
+    """frcnn_forward_vgg16_canvas / frcnn_detect_vgg16_raw: a canvas batch -- N images of different sizes, each at the top-left
+    of its Hc x Wc slot -- behind the single C-ABI call a caller without Python binds.  Same kernels, same order as
+    CanvasBatchPlan._run; this wrapper fills the C structs from a PackedWeights and owns the workspace, the static inputs and
+    the outputs, so launch() can be captured into a CUDA graph and replayed for any mix of sizes.
+
+    raw_input=False: the input is (N,3,Hc,Wc) float32 images plus the int32 [N, 2] extents and clip bounds (forward).
+    raw_input=True: the input is the device block [header | pixels] of raw uint8 BGR photos (preprocess.raw_header_layout,
+    arena_bytes of pixels, default N sources of up to Hc x Wc) and the float64 [N] im_scale; the call also runs the per-class
+    NMS (det_nms_thresh, det_conf) and writes forward.py's detection lists into ONE int32 buffer `lists`
+    [det_count (N, padded to 64 words) | dets [N][cap][5] | scores [N][cap] (float32)], cap = (NC-1) * post_n, so a host
+    caller gets them with one device-to-host copy (detect_raw)."""
+
+    def __init__(self, weights, N, Hc, Wc, anchors, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
+                 raw_input=False, pixel_means=None, arena_bytes=None, det_nms_thresh=0.3, det_conf=0.8):
+        import ctypes
+        from . import _lib, preprocess
+        if int(N) != N or N < 1:
+            raise FrcnnError("CCanvasForward needs N >= 1 images (got %r)" % (N,))
+        self._lib, self._ct = _lib.load(), ctypes
+        self.w, self.N, self.H, self.W, self.post_n = weights, int(N), int(Hc), int(Wc), post_n
+        self.raw_input = bool(raw_input)
+        self.det_nms_thresh, self.det_conf = float(det_nms_thresh), float(det_conf)
+        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
+                                                              dtype=np.float64).reshape(-1)[:3])
+        dev = weights.device
+        self.anchors, self.cfg, self.wt = _c_structs(weights, self.H, self.W, anchors, pre_n, post_n, nms_thresh, min_size,
+                                                     feat_stride)
+        nbytes = self._lib.frcnn_forward_vgg16_canvas_workspace_bytes(ctypes.byref(self.cfg), self.N)
+        if nbytes == 0:
+            raise FrcnnError("frcnn_forward_vgg16_canvas_workspace_bytes: %s" % _lib.last_error())
+        self.ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        NC = weights.num_classes
+        self.prob = torch.zeros((self.N, post_n, NC), dtype=torch.float32, device=dev)
+        self.boxes = torch.zeros((self.N, post_n, 4 * NC), dtype=torch.float32, device=dev)
+        self.count = torch.zeros((self.N,), dtype=torch.int32, device=dev)
+        if not self.raw_input:
+            self.x_in = torch.zeros((self.N, 3, self.H, self.W), dtype=torch.float32, device=dev)
+            self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=dev)     # rows: extents, clip bounds
+            self.extents, self.im_info = self._sizes[0], self._sizes[1]
+            return
+        self.arena_bytes = self.N * 3 * self.H * self.W if arena_bytes is None else int(arena_bytes)
+        if self.arena_bytes < 1:
+            raise FrcnnError("CCanvasForward: arena_bytes must be positive (got %d)" % self.arena_bytes)
+        self.header_bytes = int(self._lib.frcnn_raw_header_bytes(self.N))
+        self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=dev)
+        self.im_scale = torch.zeros((self.N,), dtype=torch.float64, device=dev)
+        self.cap = (NC - 1) * post_n
+        self.lists_layout = dict(det_count=0, dets=ops.round_up(self.N, 64), scores=ops.round_up(self.N, 64) + self.N * self.cap * 5)
+        self.lists = torch.zeros((self.lists_layout["scores"] + self.N * self.cap,), dtype=torch.int32, device=dev)
+        L = self.lists_layout
+        self.det_count = self.lists[:self.N]
+        self.dets = self.lists[L["dets"]:L["scores"]].view(self.N, self.cap, 5)
+        self.scores = self.lists[L["scores"]:].view(torch.float32).view(self.N, self.cap)
+        self._stage = None          # pinned mirrors of the block and of im_scale (stage_raw)
+        self._res_host = None       # pinned mirror of `lists` (fetch_detections)
+
+    def launch(self):
+        """Enqueue the C call on the current stream over the current contents of the static inputs (capturable)."""
+        from . import _lib
+        ct, p = self._ct, lambda t: self._ct.c_void_p(t.data_ptr())          # noqa: E731
+        st = ct.c_void_p(torch.cuda.current_stream().cuda_stream)
+        if self.raw_input:
+            m = self.pixel_means
+            _lib.check(self._lib.frcnn_detect_vgg16_raw(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(self.block), self.arena_bytes,
+                                                        m[0], m[1], m[2], p(self.im_scale), self.det_nms_thresh,
+                                                        ct.c_float(self.det_conf), p(self.ws), self.ws.numel(), p(self.prob),
+                                                        p(self.boxes), p(self.count), p(self.dets), p(self.scores),
+                                                        p(self.det_count), st), "frcnn_detect_vgg16_raw")
+        else:
+            _lib.check(self._lib.frcnn_forward_vgg16_canvas(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(self.x_in), p(self.extents),
+                                                            p(self.im_info), p(self.ws), self.ws.numel(), p(self.prob),
+                                                            p(self.boxes), p(self.count), st), "frcnn_forward_vgg16_canvas")
+
+    def set_images(self, images, img_infos=None):
+        """Float input: at most N (3,H_n,W_n) float32 CUDA tensors with H_n <= Hc and W_n <= Wc into the top-left of slots
+        0, 1, ...; the other slots are empty.  img_infos: optional per-image clip bounds (im_h, im_w), default (H_n, W_n)."""
+        if self.raw_input:
+            raise FrcnnError("CCanvasForward(raw_input=True) takes raw photos (stage_raw / detect_raw)")
+        images = list(images)
+        if len(images) > self.N or (img_infos is not None and len(img_infos) != len(images)):
+            raise FrcnnError("CCanvasForward: %d images (%s img_infos) for %d slots" %
+                             (len(images), "no" if img_infos is None else len(img_infos), self.N))
+        sizes = np.zeros((2, self.N, 2), dtype=np.int32)
+        for n, x in enumerate(images):
+            if x.dim() != 3 or x.shape[0] != 3 or not (0 < x.shape[1] <= self.H and 0 < x.shape[2] <= self.W):
+                raise FrcnnError("CCanvasForward: image %d of shape %s does not fit a (3,%d,%d) canvas" %
+                                 (n, tuple(x.shape), self.H, self.W))
+            sizes[0, n] = x.shape[1:]
+            sizes[1, n] = x.shape[1:] if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
+        for n, x in enumerate(images):
+            self.x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
+        self._sizes.copy_(torch.from_numpy(sizes), non_blocking=True)        # pageable: staged before copy_ returns
+
+    def forward(self, images, img_infos=None):
+        """set_images + launch.  Returns (prob [N,post_n,NC], boxes [N,post_n,4NC], count [N]) device tensors; rows past an
+        image's count are zero."""
+        self.set_images(images, img_infos)
+        self.launch()
+        return self.prob, self.boxes, self.count
+
+    def stage_raw(self, photos, img_infos=None):
+        """Raw input: at most N uint8 (h0,w0,3) BGR numpy photos and their header (preprocess.raw_batch_header) into the block
+        with one host-to-device copy, and their im_scale into `im_scale`.  Returns the list of im_scale."""
+        from . import preprocess
+        if not self.raw_input:
+            raise FrcnnError("CCanvasForward: raw photos need raw_input=True")
+        photos = list(photos)
+        for n, x in enumerate(photos):
+            if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or x.ndim != 3 or x.shape[2] != 3:
+                raise FrcnnError("CCanvasForward: photo %d is not a uint8 (h, w, 3) numpy array" % n)
+        hdr, scales, used = preprocess.raw_batch_header([x.shape[:2] for x in photos], self.N, self.H, self.W, self.arena_bytes,
+                                                        img_infos)
+        cur = torch.cuda.current_stream()
+        if self._stage is None:
+            self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), ops.PinnedBlock((self.N,), np.float64),
+                           torch.cuda.Event())
+        pin, pin_scale, done = self._stage
+        done.synchronize()                    # the previous upload has left the pinned mirrors
+        pin.np[:hdr.size] = hdr
+        offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
+        for n, x in enumerate(photos):
+            ops.host_copy(pin.ptr + self.header_bytes + int(offs[n]), np.ascontiguousarray(x))
+        pin_scale.np[:] = 0.0
+        pin_scale.np[:len(scales)] = scales
+        pin.h2d(self.block, cur, nbytes=self.header_bytes + used)
+        pin_scale.h2d(self.im_scale, cur)
+        done.record(cur)
+        return scales
+
+    def fetch_detections(self, n_images=None):
+        """ONE device-to-host copy of `lists` on the current stream, waited for: for each of the first n_images slots (default
+        N) its list of (cls_id, x1, y1, x2, y2, score), preprocess.result_detections' tuples."""
+        if self._res_host is None:
+            self._res_host = ops.PinnedBlock((int(self.lists.numel()),), np.int32)
+        cur = torch.cuda.current_stream()
+        self._res_host.d2h(self.lists, cur)
+        ops.stream_synchronize(cur)
+        return self.unpack_lists(self._res_host.np, n_images)
+
+    def unpack_lists(self, words, n_images=None):
+        """Host int32 words of `lists` -> for each of the first n_images slots (default N) its list of detections."""
+        L = self.lists_layout
+        dets = words[L["dets"]:L["scores"]].reshape(self.N, self.cap, 5)
+        scores = words[L["scores"]:].view(np.float32).reshape(self.N, self.cap)
+        return [[(*(int(v) for v in dets[n, k]), float(scores[n, k])) for k in range(int(words[n]))]
+                for n in range(self.N if n_images is None else int(n_images))]
+
+    def detect_raw(self, photos, img_infos=None):
+        """forward.py's whole loop on at most N raw photos in one C call: stage_raw + launch + fetch_detections."""
+        photos = list(photos)
+        self.stage_raw(photos, img_infos)
+        self.launch()
+        return self.fetch_detections(len(photos))

@@ -774,6 +774,33 @@ def detect_batch(prob, boxes, counts=None, nms_thresh=0.3, conf=0.8, out=None):
     return keep_idx, keep_count, conf_count
 
 
+def detection_lists_batch(prob, boxes, keep_idx, conf_count, im_scale, out=None):
+    """frcnn_detection_lists_batch: the lists forward.py:50-59 draws (preprocess.result_detections), built on the device.
+    prob [N,R_cap,NC], boxes [N,R_cap,4NC] fp32 and keep_idx [N,NC-1,R_cap] / conf_count [N,NC-1] int32 (detect_batch's
+    outputs), each possibly a strided view; im_scale float64 [N] device.  out: optional dense (dets int32 [N,cap,5], scores
+    fp32 [N,cap], det_count int32 [N]), cap = (NC-1)*R_cap.  Returns that triple; rows past det_count[n] are not written."""
+    N, R_cap, NC = prob.shape
+    dev = prob.device
+    cap = (NC - 1) * R_cap
+    if out is None:
+        out = (torch.empty((N, cap, 5), dtype=torch.int32, device=dev), torch.empty((N, cap), dtype=torch.float32, device=dev),
+               torch.empty((N,), dtype=torch.int32, device=dev))
+    dets, scores, det_count = out
+    _need_cuda(im_scale, dets, scores, det_count)
+    for t, dt, shape, what in ((im_scale, torch.float64, (N,), "im_scale"), (dets, torch.int32, (N, cap, 5), "dets"),
+                               (scores, torch.float32, (N, cap), "scores"), (det_count, torch.int32, (N,), "det_count")):
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise FrcnnError("detection_lists_batch: %s must be a dense %s %s CUDA tensor" % (what, dt, list(shape)))
+    ps = _image_stride(prob, (R_cap, NC), "detection_lists_batch prob")
+    bs = _image_stride(boxes, (R_cap, 4 * NC), "detection_lists_batch boxes")
+    ks = _image_stride(keep_idx, (NC - 1, R_cap), "detection_lists_batch keep_idx")
+    cc = _image_stride(conf_count, (NC - 1,), "detection_lists_batch conf_count")
+    check(_lib.load().frcnn_detection_lists_batch(N, _p(prob), ps, _p(boxes), bs, _p(keep_idx), ks, _p(conf_count), cc, _p(im_scale),
+                                                  R_cap, NC, _p(dets), _p(scores), _p(det_count), _stream()),
+          "frcnn_detection_lists_batch")
+    return dets, scores, det_count
+
+
 class ProposalBatchWorkspace(object):
     """Scratch + outputs of frcnn_proposals_batch for N images of one (A,H,W,pre,post) shape: N workspace slices in one
     buffer, rois [N,post_n,4], scores [N,post_n], count [N] int32 and, with debug, dbg_dets [N,k,5], dbg_idx [N,k],

@@ -388,6 +388,19 @@ int frcnn_detect_batch(int N, const float* prob, long prob_stride, const float* 
                        long count_stride, int R_cap, int num_classes, double nms_thresh, float conf, int* keep_idx,
                        long keep_idx_stride, int* keep_count, long keep_count_stride, int* conf_count,
                        long conf_count_stride, void* stream);
+/* The detection list forward.py:50-59 draws, on the device (one CTA per image): for class c = 1 .. num_classes-1 in order and
+ * the first conf_count[c-1] entries r of its keep_idx row (frcnn_detect_batch's outputs, read at their image strides, as are
+ * prob and boxes), the row out_dets = (c, x1, y1, x2, y2) int32 and out_scores = prob[r][c].  Each coordinate is
+ * `int(boxes[r][4c+j] / im_scale[n])` as NumPy >= 2 computes it: the float32 quotient by (float)im_scale[n], truncated toward
+ * zero.  Where Python's int() would raise or leave the int32 range, the quotient converts as cvt.rzi.s32.f32 does: NaN -> 0,
+ * saturation to [INT32_MIN, INT32_MAX].  Image n's list is at out_dets + n*cap*5 / out_scores + n*cap, cap =
+ * (num_classes-1) * R_cap (enough for every list), its length at out_det_count[n]; rows past it are NOT written.  conf_count
+ * is clamped to [0, R_cap]; a keep_idx entry outside [0, R_cap) gives the row (c, 0, 0, 0, 0), score 0, and reads nothing.
+ * NULL pointers, N outside [1,65535], R_cap < 1, num_classes < 2 or a negative stride -> FRCNN_ERR_ARG. */
+int frcnn_detection_lists_batch(int N, const float* prob, long prob_stride, const float* boxes, long boxes_stride,
+                                const int* keep_idx, long keep_idx_stride, const int* conf_count, long conf_count_stride,
+                                const double* im_scale, int R_cap, int num_classes, int* out_dets, float* out_scores,
+                                int* out_det_count, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The whole forward path behind one call (forward_graph.cu): FasterRCNN.__call__, inference branch
@@ -434,6 +447,49 @@ size_t frcnn_forward_batch_workspace_bytes(const frcnn_forward_config* config, i
 int frcnn_forward_vgg16_batch(const frcnn_forward_config* config, const frcnn_vgg16_weights* weights, int N,
                               const float* images_nchw, int im_h, int im_w, void* workspace, size_t workspace_bytes,
                               float* out_prob, float* out_boxes, int* out_count, void* stream);
+/* The same forward path over a CANVAS batch: N images of DIFFERENT sizes, each at the top-left of its config->H x config->W
+ * slot (the canvas Hc x Wc).  images_nchw: (N,3,Hc,Wc) float32 device images (pixels outside an image are never read);
+ * extents: device int32 [N][2], image n's (height, width), (0, 0) = an empty slot; im_info: device int32 [N][2], image n's
+ * clip bounds (im_h, im_w).  Both are read when the kernels run, so the static launch sequence, captured once into a CUDA
+ * graph, serves any mix of sizes.  The launches are those of the *_batch_ext entries, in the order of
+ * frcnn_forward_vgg16_batch; image n's outputs are bit-identical to frcnn_forward_vgg16 on that image alone.  Outputs as
+ * frcnn_forward_vgg16_batch.  The workspace (frcnn_forward_vgg16_canvas_workspace_bytes, 0 on a bad config or N) also serves
+ * frcnn_detect_vgg16_raw.  NULL pointers or N outside [1,65535] -> FRCNN_ERR_ARG; a short workspace -> FRCNN_ERR_WORKSPACE. */
+size_t frcnn_forward_vgg16_canvas_workspace_bytes(const frcnn_forward_config* config, int N);
+int frcnn_forward_vgg16_canvas(const frcnn_forward_config* config, const frcnn_vgg16_weights* weights, int N,
+                               const float* images_nchw, const int* extents, const int* im_info, void* workspace,
+                               size_t workspace_bytes, float* out_prob, float* out_boxes, int* out_count, void* stream);
+
+/* The device block [header | pixels] of raw photos (frcnn_detect_vgg16_raw, frcnn_b200.preprocess.raw_header_layout).  The
+ * header holds FRCNN_RAW_FIELDS arrays of 8 * N bytes each; array f starts at byte 8 * N * f:
+ *   FRCNN_RAW_EXTENTS   int32  [N][2]  the resized (H, W) of image n, (0, 0) = an empty slot
+ *   FRCNN_RAW_IM_INFO   int32  [N][2]  its clip bounds (im_h, im_w) (forward.py passes (H, H))
+ *   FRCNN_RAW_SRC_HW    int32  [N][2]  its source size (h0, w0)
+ *   FRCNN_RAW_SRC_OFF   int64  [N]     byte offset of its uint8 (h0, w0, 3) BGR pixels in the pixel area
+ *   FRCNN_RAW_INV_SCALE double [N]     1.0 / im_scale
+ * (see frcnn_preprocess_bgr8_canvas).  The pixel area starts at frcnn_raw_header_bytes(N), a multiple of 256 (0 for N outside
+ * [1,65535]). */
+#define FRCNN_RAW_EXTENTS 0
+#define FRCNN_RAW_IM_INFO 1
+#define FRCNN_RAW_SRC_HW 2
+#define FRCNN_RAW_SRC_OFF 3
+#define FRCNN_RAW_INV_SCALE 4
+#define FRCNN_RAW_FIELDS 5
+size_t frcnn_raw_header_bytes(int N);
+
+/* forward.py's whole loop on RAW photos of different sizes behind one call: frcnn_preprocess_bgr8_canvas (resize, mean
+ * subtraction (mean_b, mean_g, mean_r) and first-layer pack of every slot), the launch sequence of frcnn_forward_vgg16_canvas,
+ * frcnn_detect_batch (per-class NMS det_nms_thresh, score >= det_conf; forward.py uses 0.3 and 0.8) and
+ * frcnn_detection_lists_batch.  block: the device block [header | arena_bytes bytes of pixels] (8-byte aligned); im_scale:
+ * device double [N], image n's im_scale (the divisor of its boxes).  Outputs: out_prob / out_boxes / out_count as
+ * frcnn_forward_vgg16_canvas, and image n's detection list at out_dets + n*cap*5 / out_scores + n*cap, its length in
+ * out_det_count[n], cap = (num_classes-1) * post_nms_top_n.  Workspace: frcnn_forward_vgg16_canvas_workspace_bytes.  Static
+ * launch sequence: captured once, it serves any batch that fits the canvas and the arena.  Errors as
+ * frcnn_forward_vgg16_canvas, and a non-positive arena_bytes -> FRCNN_ERR_ARG. */
+int frcnn_detect_vgg16_raw(const frcnn_forward_config* config, const frcnn_vgg16_weights* weights, int N, const void* block,
+                           long long arena_bytes, double mean_b, double mean_g, double mean_r, const double* im_scale,
+                           double det_nms_thresh, float det_conf, void* workspace, size_t workspace_bytes, float* out_prob,
+                           float* out_boxes, int* out_count, int* out_dets, float* out_scores, int* out_det_count, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * ResNet trunk support (SURVEY.md 8f rank 2; chainer ResNetLayers as used by models/resnet.py:11-45).
