@@ -19,14 +19,15 @@ Mirrors FasterRCNN.__call__ (inference branch, /root/reference models/faster_rcn
 All buffers are allocated once per (image shape, mode); the data-dependent RoI count stays on the
 device (rows past it are zero) so the launch sequence is static and is captured into a CUDA graph.
 """
+import collections
+import threading
+import time
+
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, preprocess
 from ._lib import FrcnnError
-
-import threading
-import time
 
 _CAPTURE_LOCK = threading.Lock()
 # diagnostic hook: a list that receives, per ForwardPlan.forward_host call, the host-side milliseconds of
@@ -40,6 +41,28 @@ VGG16_LAYERS = [
     ("conv4_1", 256, 512), ("conv4_2", 512, 512), ("conv4_3", 512, 512), "pool",
     ("conv5_1", 512, 512), ("conv5_2", 512, 512), ("conv5_3", 512, 512),
 ]
+
+# one VGG16 conv layer of a plan: `halvings` 2x2 pools precede its input, fused_pool = the following pool runs in its
+# epilogue, pool_after = it runs as a stand-alone max-pool; (out_h, out_w) is the layer's output (after a fused pool)
+TrunkStep = collections.namedtuple("TrunkStep", "name cin cout halvings fused_pool pool_after out_h out_w")
+
+
+def vgg16_schedule(H, W, fuse_pool):
+    """The VGG16 trunk on an H x W image: ([TrunkStep] per conv layer, feature-map (h, w)).  Every 2x2 pool is ceil-mode."""
+    steps, h, w, k = [], H, W, 0
+    for i, item in enumerate(VGG16_LAYERS):
+        if item == "pool":
+            continue
+        pooled = i + 1 < len(VGG16_LAYERS) and VGG16_LAYERS[i + 1] == "pool"
+        fused = fuse_pool and pooled
+        if fused:
+            h, w = (h + 1) // 2, (w + 1) // 2
+        steps.append(TrunkStep(item[0], item[1], item[2], k, fused, pooled and not fused, h, w))
+        if pooled:
+            k += 1
+            if not fused:
+                h, w = (h + 1) // 2, (w + 1) // 2
+    return steps, (h, w)
 
 
 def _t(a, device):
@@ -120,150 +143,67 @@ def _unpack_block(words, L, post_n, NC, with_detect):
     return out
 
 
-class ForwardPlan(object):
-    """Buffers + launch sequence for one image shape."""
+class _PlanBase(object):
+    """What ForwardPlan (one image) and BatchPlan (N images of one shape) share: the keyword options, the VGG16 trunk's
+    activations, the result blocks and the host-array front end.  Each keeps its own launch sequence (_run)."""
+    _lead = ()          # leading dimensions of every activation and of the result blocks: (N,) in a BatchPlan
 
-    def __init__(self, weights, H, W, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
-                 anchors=None, with_detect=False, det_nms_thresh=0.3, det_conf=0.8, use_graph=True, keep_rpn_debug=False,
-                 fuse_pool=True, hwc_input=False):
+    def __init__(self, weights, H, W, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16, anchors=None,
+                 with_detect=False, det_nms_thresh=0.3, det_conf=0.8, use_graph=True, keep_rpn_debug=False, fuse_pool=True,
+                 hwc_input=False):
+        if anchors is None:
+            raise FrcnnError("%s needs the [A,4] float64 anchor table" % type(self).__name__)
         self.w, self.H, self.W = weights, H, W
         self._ctor = dict(pre_n=pre_n, post_n=post_n, nms_thresh=nms_thresh, min_size=min_size, feat_stride=feat_stride,
                           anchors=anchors, with_detect=with_detect, det_nms_thresh=det_nms_thresh, det_conf=det_conf,
                           use_graph=use_graph, keep_rpn_debug=keep_rpn_debug, fuse_pool=fuse_pool, hwc_input=hwc_input)
-        # hwc_input: the static input buffer holds the bytes of a dense (H,W,3) float32 image (what a forward.py-style caller's
-        # `img.transpose(2,0,1).astype(np.float32)` really is in memory); the first kernel reads it with HWC strides
-        self.hwc_input = bool(hwc_input)
-        dev = weights.device
-        x3 = weights.precision == "bf16x3"
         self.pre_n, self.post_n, self.nms_thresh, self.min_size, self.feat_stride = pre_n, post_n, nms_thresh, min_size, feat_stride
         self.with_detect, self.det_nms_thresh, self.det_conf = with_detect, det_nms_thresh, det_conf
-        A = weights.n_anchors
-        if anchors is None:
-            raise FrcnnError("ForwardPlan needs the [A,4] float64 anchor table")
-        self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
-
-        def act(h, w, c):
-            hi = torch.empty((h, w, c), dtype=torch.bfloat16, device=dev)
-            return ops.Act(hi, torch.empty_like(hi) if x3 else None)
-
-        self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)      # static input (C,H,W)
-        self.img_info = torch.tensor([H, W], dtype=torch.int32, device=dev)      # clip bounds (h, w): static in the graph
-        self._act = act
-        self.fuse_pool = fuse_pool
-        h, w_ = self._alloc_trunk(H, W)
-        self.fh, self.fw = h, w_
-        self.rpn_mid = act(h, w_, weights.rpn3[0].shape[1])
-        self.rpn_out = torch.empty((h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
-        NC = weights.num_classes
-        self.result_layout, off = _result_layout(post_n, NC)
-        self.result_words_nodetect = self.result_layout["keep_count"][0]
-        self.result = torch.zeros((off,), dtype=torch.int32, device=dev)
-        rf = self.result.view(torch.float32)
-        seg = lambda t, name: t[self.result_layout[name][0]: self.result_layout[name][0] + self.result_layout[name][1]]   # noqa: E731
-        self.prop = ops.ProposalWorkspace(A, h, w_, pre_n, post_n, dev, debug=keep_rpn_debug,
-                                          outputs=(seg(rf, "rois").view(post_n, 4), seg(rf, "scores"), seg(self.result, "count")[:1]))
-        C = self.acts[-1].hi.shape[2]
-        self.pool5 = act(1, post_n, 49 * C)
-        self.fc6 = act(1, post_n, 4096)
-        self.fc7 = act(1, post_n, 4096)
-        self.head_out = torch.empty((post_n, weights.head_ld), dtype=torch.float32, device=dev)
-        # split-K slabs of the swapped-operand head GEMMs (ops.linear); one buffer sized for the largest layer
-        nc5 = 5 * weights.num_classes
-        self.fc_work = ops.linear_workspace(post_n, 49 * C, 4096, dev)
-        for k_, c_ in ((4096, 4096), (4096, nc5)):
-            wk = ops.linear_workspace(post_n, k_, c_, dev)
-            if wk.numel() > self.fc_work.numel():
-                self.fc_work = wk
-        self.prob = seg(rf, "prob").view(post_n, NC)
-        self.boxes = seg(rf, "boxes").view(post_n, 4 * NC)
-        self.det = (seg(self.result, "keep_idx").view(NC - 1, post_n), seg(self.result, "keep_count"), seg(self.result, "conf_count"))
+        self.use_graph, self.keep_rpn_debug, self.fuse_pool = use_graph, keep_rpn_debug, fuse_pool
+        # hwc_input: the static input holds the bytes of dense (H,W,3) float32 images (what a forward.py-style caller's
+        # `img.transpose(2,0,1).astype(np.float32)` really is in memory); the first kernel reads them with HWC strides
+        self.hwc_input = bool(hwc_input)
+        self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(weights.device)
         self._host = None
         self.graph = None
-        self.use_graph = use_graph
         self.im_h, self.im_w = H, W
         self.n_launches = 0
 
+    def _act(self, *shape, zero=False):
+        """Activation planes of `shape` behind the plan's leading dimensions: bf16 hi, and lo in bf16x3."""
+        new, like = (torch.zeros, torch.zeros_like) if zero else (torch.empty, torch.empty_like)
+        hi = new(self._lead + shape, dtype=torch.bfloat16, device=self.w.device)
+        return ops.Act(hi, like(hi) if self.w.precision == "bf16x3" else None)
+
     def _alloc_trunk(self, H, W):
         """VGG16 activations; returns the feature-map size.  (resnet_engine.ResNetForwardPlan overrides both trunk hooks.)"""
-        act, fuse_pool = self._act, self.fuse_pool
-        n_c8 = ops._lib.load().frcnn_image_c8_elems(H, W)          # compact first-layer input: [H][W+2][8] (+ slack), flat planes
-        hi0 = torch.empty((n_c8,), dtype=torch.bfloat16, device=self.x_in.device)
-        self.acts = [ops.Act(hi0, torch.empty_like(hi0) if self.w.precision == "bf16x3" else None)]
-        h, w_ = H, W
-        self.trunk_steps = []          # (layer name, fuse the following 2x2 pool into the conv epilogue)
-        for i, item in enumerate(VGG16_LAYERS):
-            if item == "pool":
-                continue
-            fuse = fuse_pool and i + 1 < len(VGG16_LAYERS) and VGG16_LAYERS[i + 1] == "pool"
-            pooled = i + 1 < len(VGG16_LAYERS) and VGG16_LAYERS[i + 1] == "pool"
-            if fuse:
-                h, w_ = (h + 1) // 2, (w_ + 1) // 2
-                self.acts.append(act(h, w_, item[2]))
-                self.trunk_steps.append((item[0], True, False))
-            else:
-                self.acts.append(act(h, w_, item[2]))
-                self.trunk_steps.append((item[0], False, pooled))
-                if pooled:
-                    h, w_ = (h + 1) // 2, (w_ + 1) // 2
-                    self.acts.append(act(h, w_, item[2]))
-        return h, w_
+        self.acts = [self._act(ops._lib.load().frcnn_image_c8_elems(H, W))]     # compact first-layer input: [H][W+2][8] (+ slack)
+        self.trunk, feat_hw = vgg16_schedule(H, W, self.fuse_pool)
+        self.trunk_steps = [(s.name, s.fused_pool, s.pool_after) for s in self.trunk]
+        for s in self.trunk:
+            self.acts.append(self._act(s.out_h, s.out_w, s.cout))
+            if s.pool_after:
+                self.acts.append(self._act((s.out_h + 1) // 2, (s.out_w + 1) // 2, s.cout))
+        return feat_hw
 
-    def _run_trunk(self):
-        """Launches the trunk; returns (feature map Act, number of launches)."""
-        w = self.w
-        n = 0
-        x = self.acts[0]
-        ops.pack_image_c8(self.x_in, out=x, hwc_memory=self.hwc_input)
-        n += 1
-        i = 0
-        for name, fused, pool_after in self.trunk_steps:
-            hi, lo, b = w.convs[name]
-            if i == 0:                          # conv1_1: sliding-window reads of the compact image, K = 3 x 32
-                ops.conv3x3_c8(self.acts[0], self.H, self.W, hi, lo, b, True, out=self.acts[1])
-            else:
-                ops.conv2d(self.acts[i], hi, lo, b, 3, True, out=self.acts[i + 1], fuse_pool=fused)
-            n += 1
-            i += 1
-            if pool_after:
-                ops.maxpool2x2_ceil(self.acts[i], out=self.acts[i + 1])
-                n += 1
-                i += 1
-        return self.acts[-1], n
-
-    # -- the launch sequence (static; safe to capture)
-    def _run(self):
-        w = self.w
-        feat, n = self._run_trunk()
-        self.feat = feat
-        hi, lo, b = w.rpn3
-        ops.conv2d(feat, hi, lo, b, 3, True, out=self.rpn_mid)
-        hi, lo, b = w.rpn_heads
-        ops.conv2d(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out)
-        ops.proposals(self.rpn_out, None, self.anchors, w.n_anchors, self.fh, self.fw, self.feat_stride,
-                      self.im_h, self.im_w, self.min_size, self.pre_n, self.post_n, self.nms_thresh,
-                      layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=self.prop,
-                      debug=self.prop.dbg_dets is not None)
-        n += 2 + 5          # rpn 3x3, rpn heads; decode, select, rank/scatter, IoU mask, mask scan
-        ops.roi_pool(feat, self.prop.rois, self.prop.count, 7, 7, 1.0 / self.feat_stride, out=self.pool5)
-        hi, lo, b = w.fc6
-        ops.linear(self.pool5, hi, lo, b, True, m_valid=self.prop.count, out=self.fc6, work=self.fc_work)
-        hi, lo, b = w.fc7
-        ops.linear(self.fc6, hi, lo, b, True, m_valid=self.prop.count, out=self.fc7, work=self.fc_work)
-        hi, lo, b = w.head
-        ops.linear(self.fc7, hi, lo, b, False, m_valid=self.prop.count, out_f32=self.head_out, ld_f32=w.head_ld,
-                   work=self.fc_work, want_act=False)
-        n += 3          # each head layer = the split-K GEMM + its reduction
-        ops.head_decode(self.head_out, w.head_ld, self.prop.rois, self.prop.count, w.num_classes, self.im_h, self.im_w,
-                        out_prob=self.prob, out_boxes=self.boxes)
-        n += 5
-        if self.with_detect:
-            ops.detect(self.prob, self.boxes, self.prop.count, self.det_nms_thresh, self.det_conf, out=self.det)
-            n += 1
-        self.n_launches = n
+    def _alloc_result(self, n):
+        """n result blocks (_result_layout) in ONE int32 buffer, so a host caller gets everything with one D2H; prob, boxes
+        and det are [n, ...] views into them.  Returns the (rois, scores, count) views that ProposalLayer writes."""
+        post_n, NC = self.post_n, self.w.num_classes
+        L, bw = self.result_layout, self.block_words = _result_layout(post_n, NC)
+        self.result_words_nodetect = L["keep_count"][0]
+        self.result = torch.zeros((n * bw,), dtype=torch.int32, device=self.w.device)
+        blocks = self.result.view(n, bw)
+        bf = blocks.view(torch.float32)
+        seg = lambda t, name: t[:, L[name][0]: L[name][0] + L[name][1]]      # noqa: E731
+        self.prob = seg(bf, "prob").view(n, post_n, NC)
+        self.boxes = seg(bf, "boxes").view(n, post_n, 4 * NC)
+        self.det = (seg(blocks, "keep_idx").view(n, NC - 1, post_n), seg(blocks, "keep_count"), seg(blocks, "conf_count"))
+        return seg(bf, "rois").view(n, post_n, 4), seg(bf, "scores"), seg(blocks, "count")[:, 0]
 
     def clone(self):
-        """A second set of buffers (and its own graph) over the SAME packed weights: lets another image be in flight."""
-        p = type(self)(self.w, self.H, self.W, **self._ctor)
+        """A second set of buffers (and its own graph) over the SAME packed weights: lets another image or batch be in flight."""
+        p = type(self)(self.w, *(self._lead + (self.H, self.W)), **self._ctor)
         p.set_clip(self.im_h, self.im_w)
         return p
 
@@ -274,12 +214,14 @@ class ForwardPlan(object):
             self.im_h, self.im_w = int(im_h), int(im_w)
             self.graph = None
 
-    # -- host-array front end (the reference's model-input interface: a float32 (3,H,W) HOST array in, host results out)
+    # -- host-array front end (the reference's model-input interface: a float32 HOST array in, host results out)
     def result_words(self):
-        return int(self.result.numel()) if self.with_detect else int(self.result_words_nodetect)
+        """Words of the result buffer a host caller needs: every block, the last one without the NMS lists when they are off."""
+        n = int(self.result.numel())
+        return n if self.with_detect else n - self.block_words + self.result_words_nodetect
 
     def host_io(self):
-        """Pinned staging for one synchronous host call at a time: the input image and a mirror of the result block."""
+        """Pinned staging for one synchronous host call at a time: the input and a mirror of the result blocks."""
         if self._host is None:
             dev = self.x_in.device
             self._host = dict(x=ops.PinnedBlock(tuple(self.x_in.shape), np.float32),
@@ -288,9 +230,10 @@ class ForwardPlan(object):
         return self._host
 
     def forward_host(self, x_np):
-        """x_np: float32 (3,H,W) (or (1,3,H,W)) numpy array.  Copies it into pinned staging (multi-threaded host copy),
-        uploads, replays the graph and brings the whole result block back with ONE D2H; blocks until it is there.
-        Returns a dict of numpy VIEWS into the pinned mirror (valid until the next forward_host on this plan)."""
+        """x_np: a float32 numpy array of x_in's shape ((3,H,W), or (1,3,H,W), for a ForwardPlan; (N,3,H,W) for a BatchPlan).
+        Copies it into pinned staging (multi-threaded host copy), uploads, replays the graph and brings the result blocks
+        back with ONE D2H; blocks until they are there.  Returns unpack_result's numpy VIEWS into the pinned mirror (valid
+        until the next forward_host on this plan)."""
         io = self.host_io()
         prof = HOST_PROFILE
         t0 = time.perf_counter() if prof is not None else 0.0
@@ -308,6 +251,83 @@ class ForwardPlan(object):
             t4 = time.perf_counter()
             prof.append((1e3 * (t1 - t0), 1e3 * (t2 - t1), 1e3 * (t3 - t2), 1e3 * (t4 - t3)))
         return self.unpack_result(io["res"].np)
+
+
+class ForwardPlan(_PlanBase):
+    """Buffers + launch sequence for one image shape.  Takes _PlanBase's keyword options."""
+
+    def __init__(self, weights, H, W, **options):
+        super(ForwardPlan, self).__init__(weights, H, W, **options)
+        dev, post_n = weights.device, self.post_n
+        self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)      # static input (C,H,W)
+        h, w_ = self.fh, self.fw = self._alloc_trunk(H, W)
+        self.rpn_mid = self._act(h, w_, weights.rpn3[0].shape[1])
+        self.rpn_out = torch.empty((h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
+        rois, scores, count = self._alloc_result(1)
+        self.prob, self.boxes, self.det = self.prob[0], self.boxes[0], tuple(t[0] for t in self.det)
+        self.prop = ops.ProposalWorkspace(weights.n_anchors, h, w_, self.pre_n, post_n, dev, debug=self.keep_rpn_debug,
+                                          outputs=(rois[0], scores[0], count))
+        C = self.acts[-1].hi.shape[2]
+        self.pool5 = self._act(1, post_n, 49 * C)
+        self.fc6 = self._act(1, post_n, 4096)
+        self.fc7 = self._act(1, post_n, 4096)
+        self.head_out = torch.empty((post_n, weights.head_ld), dtype=torch.float32, device=dev)
+        # split-K slabs of the swapped-operand head GEMMs (ops.linear); one buffer sized for the largest layer
+        self.fc_work = max((ops.linear_workspace(post_n, k_, c_, dev) for k_, c_ in
+                            ((49 * C, 4096), (4096, 4096), (4096, 5 * weights.num_classes))), key=lambda t: t.numel())
+
+    def _run_trunk(self):
+        """Launches the trunk; returns (feature map Act, number of launches)."""
+        acts = iter(self.acts)
+        x = next(acts)
+        ops.pack_image_c8(self.x_in, out=x, hwc_memory=self.hwc_input)
+        n = 1
+        for s in self.trunk:
+            hi, lo, b = self.w.convs[s.name]
+            y = next(acts)
+            if s.cin <= 3:                      # conv1_1: sliding-window reads of the compact image, K = 3 x 32
+                ops.conv3x3_c8(x, self.H, self.W, hi, lo, b, True, out=y)
+            else:
+                ops.conv2d(x, hi, lo, b, 3, True, out=y, fuse_pool=s.fused_pool)
+            x = y
+            n += 1
+            if s.pool_after:
+                x = next(acts)
+                ops.maxpool2x2_ceil(y, out=x)
+                n += 1
+        return x, n
+
+    # -- the launch sequence (static; safe to capture)
+    def _run(self):
+        w = self.w
+        feat, n = self._run_trunk()
+        self.feat = feat
+        hi, lo, b = w.rpn3
+        ops.conv2d(feat, hi, lo, b, 3, True, out=self.rpn_mid)
+        hi, lo, b = w.rpn_heads
+        ops.conv2d(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=w.rpn_ld, out_f32=self.rpn_out)
+        ops.proposals(self.rpn_out, None, self.anchors, w.n_anchors, self.fh, self.fw, self.feat_stride,
+                      self.im_h, self.im_w, self.min_size, self.pre_n, self.post_n, self.nms_thresh,
+                      layout="nhwc", ld=w.rpn_ld, cls_is_logits=True, work=self.prop,
+                      debug=self.prop.dbg_dets is not None)
+        n += 2 + 5          # rpn 3x3, rpn heads; decode, select, rank/scatter, IoU mask, mask scan
+        ops.roi_pool(feat, self.prop.rois, self.prop.count, 7, 7, 1.0 / self.feat_stride, out=self.pool5)
+        n += 1
+        hi, lo, b = w.fc6
+        ops.linear(self.pool5, hi, lo, b, True, m_valid=self.prop.count, out=self.fc6, work=self.fc_work)
+        hi, lo, b = w.fc7
+        ops.linear(self.fc6, hi, lo, b, True, m_valid=self.prop.count, out=self.fc7, work=self.fc_work)
+        hi, lo, b = w.head
+        ops.linear(self.fc7, hi, lo, b, False, m_valid=self.prop.count, out_f32=self.head_out, ld_f32=w.head_ld,
+                   work=self.fc_work, want_act=False)
+        n += 3 * 2          # each head layer = the split-K GEMM + its reduction
+        ops.head_decode(self.head_out, w.head_ld, self.prop.rois, self.prop.count, w.num_classes, self.im_h, self.im_w,
+                        out_prob=self.prob, out_boxes=self.boxes)
+        n += 1
+        if self.with_detect:
+            ops.detect(self.prob, self.boxes, self.prop.count, self.det_nms_thresh, self.det_conf, out=self.det)
+            n += 1
+        self.n_launches = n
 
     def unpack_result(self, words):
         """numpy int32 words of a result block -> dict of views (count int, prob [R,NC], boxes [R,4NC], rois, scores, detect lists)."""
@@ -340,7 +360,7 @@ def _launch(plan):
     plan.graph.replay()
 
 
-class BatchPlan(object):
+class BatchPlan(_PlanBase):
     """Buffers + launch sequence for N images of one shape (VGG16 trunk), all in ONE CUDA graph.
 
     Every stage runs once over all N images: the trunk, the RPN convolutions and the fc6 / fc7 / head GEMMs
@@ -352,84 +372,39 @@ class BatchPlan(object):
     everything with one D2H; the batched post-processing reads and writes those blocks in place at a stride of one block.
     Takes ForwardPlan's keyword options."""
 
-    def __init__(self, weights, N, H, W, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
-                 anchors=None, with_detect=False, det_nms_thresh=0.3, det_conf=0.8, use_graph=True, keep_rpn_debug=False,
-                 fuse_pool=True, hwc_input=False):
+    def __init__(self, weights, N, H, W, **options):
         if int(N) != N or N < 1:
             raise FrcnnError("BatchPlan needs N >= 1 images (got %r)" % (N,))
-        if anchors is None:
-            raise FrcnnError("BatchPlan needs the [A,4] float64 anchor table")
+        super(BatchPlan, self).__init__(weights, H, W, **options)
         if "conv1_1" not in weights.convs:
             raise FrcnnError("BatchPlan runs the VGG16 trunk only")
-        N = int(N)
-        self.w, self.N, self.H, self.W = weights, N, H, W
-        self._ctor = dict(pre_n=pre_n, post_n=post_n, nms_thresh=nms_thresh, min_size=min_size, feat_stride=feat_stride,
-                          anchors=anchors, with_detect=with_detect, det_nms_thresh=det_nms_thresh, det_conf=det_conf,
-                          use_graph=use_graph, keep_rpn_debug=keep_rpn_debug, fuse_pool=fuse_pool, hwc_input=hwc_input)
-        self.hwc_input = bool(hwc_input)       # x_in holds the bytes of dense (N,H,W,3) images
-        self.pre_n, self.post_n, self.nms_thresh, self.min_size, self.feat_stride = pre_n, post_n, nms_thresh, min_size, feat_stride
-        self.with_detect, self.det_nms_thresh, self.det_conf = with_detect, det_nms_thresh, det_conf
-        dev = weights.device
-        x3 = weights.precision == "bf16x3"
-        A, NC = weights.n_anchors, weights.num_classes
-        self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
-
-        def act(*shape, zero=False):
-            hi = (torch.zeros if zero else torch.empty)(shape, dtype=torch.bfloat16, device=dev)
-            return ops.Act(hi, torch.zeros_like(hi) if (x3 and zero) else (torch.empty_like(hi) if x3 else None))
-
+        N = self.N = int(N)
+        self._lead = (N,)
+        dev, post_n = weights.device, self.post_n
         self._alloc_input(dev)
-        self.acts = [act(N, ops._lib.load().frcnn_image_c8_elems(H, W))]
-        h, w_ = H, W
-        self.trunk_steps = []          # as ForwardPlan._alloc_trunk
-        for i, item in enumerate(VGG16_LAYERS):
-            if item == "pool":
-                continue
-            pooled = i + 1 < len(VGG16_LAYERS) and VGG16_LAYERS[i + 1] == "pool"
-            fuse = fuse_pool and pooled
-            if fuse:
-                h, w_ = (h + 1) // 2, (w_ + 1) // 2
-            self.acts.append(act(N, h, w_, item[2]))
-            self.trunk_steps.append((item[0], fuse, pooled and not fuse))
-            if pooled and not fuse:
-                h, w_ = (h + 1) // 2, (w_ + 1) // 2
-                self.acts.append(act(N, h, w_, item[2]))
-        self.fh, self.fw = h, w_
-        self.rpn_mid = act(N, h, w_, weights.rpn3[0].shape[1])
+        h, w_ = self.fh, self.fw = self._alloc_trunk(H, W)
+        self.rpn_mid = self._act(h, w_, weights.rpn3[0].shape[1])
         self.rpn_out = torch.empty((N * h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
-        self.result_layout, self.block_words = _result_layout(post_n, NC)
-        self.result_words_nodetect = self.result_layout["keep_count"][0]
-        self.result = torch.zeros((N * self.block_words,), dtype=torch.int32, device=dev)
+        # every per-image result as ONE [N, ...] view of the N blocks (image stride = block_words): the batched entries
+        # write straight into the blocks
+        outputs = self._alloc_result(N)
+        self.prop = ops.ProposalBatchWorkspace(N, weights.n_anchors, h, w_, self.pre_n, post_n, dev, debug=self.keep_rpn_debug,
+                                               outputs=outputs)
+        self.images = [dict(prob=self.prob[n], boxes=self.boxes[n], det=tuple(t[n] for t in self.det)) for n in range(N)]
         # the RoI counts for frcnn_linear_batch: word `count` of every block, block_words apart
         self.counts = self.result[self.result_layout["count"][0]:]
         # head activations: one segment of ld1 rows per image; rows [post_n, ld1) of pool5 stay zero
         self.ld1 = ops.round_up(post_n, 32)
         C = self.acts[-1].hi.shape[-1]
-        self.pool5 = act(N, self.ld1, 49 * C, zero=True)
-        self.fc6 = act(N, self.ld1, 4096)
-        self.fc7 = act(N, self.ld1, 4096)
+        self.pool5 = self._act(self.ld1, 49 * C, zero=True)
+        self.fc6 = self._act(self.ld1, 4096)
+        self.fc7 = self._act(self.ld1, 4096)
         self.head_out = torch.empty((N, self.ld1, weights.head_ld), dtype=torch.float32, device=dev)
         self.fc_work = max((ops.linear_batch_workspace(N, post_n, k_, c_, dev) for k_, c_ in
-                            ((49 * C, 4096), (4096, 4096), (4096, 5 * NC))), key=lambda t: t.numel())
-        # every per-image result as ONE [N, ...] view of the N blocks (image stride = block_words): the batched entries
-        # write straight into the blocks
-        blocks = self.result.view(N, self.block_words)
-        seg = lambda t, name: t[:, self.result_layout[name][0]: self.result_layout[name][0] + self.result_layout[name][1]]   # noqa: E731
-        bf = blocks.view(torch.float32)
-        self.prop = ops.ProposalBatchWorkspace(N, A, h, w_, pre_n, post_n, dev, debug=keep_rpn_debug,
-                                               outputs=(seg(bf, "rois").view(N, post_n, 4), seg(bf, "scores"), seg(blocks, "count")[:, 0]))
-        self.prob = seg(bf, "prob").view(N, post_n, NC)
-        self.boxes = seg(bf, "boxes").view(N, post_n, 4 * NC)
-        self.det = (seg(blocks, "keep_idx").view(N, NC - 1, post_n), seg(blocks, "keep_count"), seg(blocks, "conf_count"))
-        self.images = [dict(prob=self.prob[n], boxes=self.boxes[n], det=tuple(t[n] for t in self.det)) for n in range(N)]
+                            ((49 * C, 4096), (4096, 4096), (4096, 5 * weights.num_classes))), key=lambda t: t.numel())
         # per-image device int32 [N, 2] extents (height, width) and clip bounds (im_h, im_w) of a canvas batch
         # (CanvasBatchPlan); None: every image fills the H x W slot and (im_h, im_w) clips all of them
         self.extents = self.im_info = None
-        self._host = None
-        self.graph = None
-        self.use_graph = use_graph
-        self.im_h, self.im_w = H, W
-        self.n_launches = 0
 
     def _alloc_input(self, dev):
         """The static input that the first launch reads: (N,3,H,W) float32 images."""
@@ -444,23 +419,23 @@ class BatchPlan(object):
         ext = self.extents
         self._pack_input()
         n = 1
-        i = 0
-        k = 0           # 2x2 pools before the current layer: its extents are ceil(extent / 2^k)
-        for name, fused, pool_after in self.trunk_steps:
-            hi, lo, b = w.convs[name]
-            if i == 0:
-                ops.conv3x3_c8_batch(self.acts[0], N, self.H, self.W, hi, lo, b, True, out=self.acts[1], extents=ext)
+        acts = iter(self.acts)
+        x = next(acts)
+        for s in self.trunk:            # a layer's extents are ceil(extent / 2^halvings)
+            hi, lo, b = w.convs[s.name]
+            y = next(acts)
+            if s.cin <= 3:
+                ops.conv3x3_c8_batch(x, N, self.H, self.W, hi, lo, b, True, out=y, extents=ext)
             else:
-                ops.conv2d_batch(self.acts[i], hi, lo, b, 3, True, out=self.acts[i + 1], fuse_pool=fused, extents=ext, halvings=k)
+                ops.conv2d_batch(x, hi, lo, b, 3, True, out=y, fuse_pool=s.fused_pool, extents=ext, halvings=s.halvings)
+            x = y
             n += 1
-            i += 1
-            k += 1 if fused else 0
-            if pool_after:
-                ops.maxpool2x2_ceil_batch(self.acts[i], out=self.acts[i + 1])
+            if s.pool_after:
+                x = next(acts)
+                ops.maxpool2x2_ceil_batch(y, out=x)
                 n += 1
-                i += 1
-                k += 1
-        feat = self.feat = self.acts[-1]
+        feat = self.feat = x
+        k = VGG16_LAYERS.count("pool")
         hi, lo, b = w.rpn3
         ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid, extents=ext, halvings=k)
         hi, lo, b = w.rpn_heads
@@ -491,21 +466,6 @@ class BatchPlan(object):
             ops.detect_batch(self.prob, self.boxes, self.prop.count, self.det_nms_thresh, self.det_conf, out=self.det)
             n += 1
         self.n_launches = n
-
-    def clone(self):
-        """A second set of buffers (and its own graph) over the SAME packed weights: lets another batch be in flight."""
-        p = type(self)(self.w, self.N, self.H, self.W, **self._ctor)
-        p.set_clip(self.im_h, self.im_w)
-        return p
-
-    set_clip = ForwardPlan.set_clip
-    host_io = ForwardPlan.host_io
-    forward_host = ForwardPlan.forward_host       # x_np: float32 (N,3,H,W); returns unpack_result's list
-
-    def result_words(self):
-        """Words of the result buffer a host caller needs: every block, the last one without the NMS lists when they are off."""
-        last = self.block_words if self.with_detect else self.result_words_nodetect
-        return (self.N - 1) * self.block_words + last
 
     def unpack_result(self, words):
         """numpy int32 words of the result buffer -> list of N dicts as ForwardPlan.unpack_result returns them."""
@@ -546,7 +506,6 @@ class CanvasBatchPlan(BatchPlan):
             raise FrcnnError("CanvasBatchPlan has no RPN debug outputs (keep_rpn_debug=True)")
         if kw.get("hwc_input"):
             raise FrcnnError("CanvasBatchPlan takes (3,H,W) images (hwc_input=True)")
-        from . import preprocess
         self.raw_input = bool(raw_input)
         self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
                                                               dtype=np.float64).reshape(-1)[:3])
@@ -567,7 +526,6 @@ class CanvasBatchPlan(BatchPlan):
     def _alloc_input(self, dev):
         if not self.raw_input:
             return super(CanvasBatchPlan, self)._alloc_input(dev)
-        from . import preprocess
         layout, self.header_bytes = preprocess.raw_header_layout(self.N)
         self.x_in = None
         self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=dev)
@@ -586,7 +544,6 @@ class CanvasBatchPlan(BatchPlan):
 
     def raw_batch_header(self, shapes, img_infos=None):
         """preprocess.raw_batch_header for this plan's slots, canvas and arena (raises FrcnnError when something does not fit)."""
-        from . import preprocess
         if not self.raw_input:
             raise FrcnnError("CanvasBatchPlan: raw photos need a plan built with raw_input=True")
         return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
@@ -598,7 +555,6 @@ class CanvasBatchPlan(BatchPlan):
         img_infos: optional per-image clip bounds, default the resized (H_n, W_n); forward.py passes (H_n, H_n) (SURVEY.md
         Q7).  Raises FrcnnError before anything is queued if a resized image does not fit the canvas or the photos do not
         fit the arena.  Returns BatchPlan.forward's (list of prob, list of boxes, counts) and the list of im_scale."""
-        from . import preprocess
         images = list(images)
         on_host = all(isinstance(x, np.ndarray) for x in images)
         if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
@@ -606,20 +562,18 @@ class CanvasBatchPlan(BatchPlan):
         for n, x in enumerate(images):
             if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
                 raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
-        hdr, scales, used = self.raw_batch_header([x.shape[:2] for x in images], img_infos)
-        offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
+        hdr, scales, _ = self.raw_batch_header([x.shape[:2] for x in images], img_infos)
         cur = torch.cuda.current_stream()
         if self._stage is None:
             self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
         pin, done = self._stage
         done.synchronize()                    # the previous upload has left the pinned mirror
-        pin.np[:hdr.size] = hdr
         if on_host:
-            for n, x in enumerate(images):
-                ops.host_copy(pin.ptr + self.header_bytes + int(offs[n]), np.ascontiguousarray(x))
-            pin.h2d(self.block, cur, nbytes=self.header_bytes + used)
+            pin.h2d(self.block, cur, nbytes=preprocess.fill_raw_block(pin.np, hdr, images, self.N))
         else:
+            pin.np[:hdr.size] = hdr
             pin.h2d(self.block, cur, nbytes=self.header_bytes)
+            offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
             for n, x in enumerate(images):
                 self.arena[int(offs[n]):int(offs[n]) + x.numel()].copy_(x.contiguous().view(-1), non_blocking=True)
         done.record(cur)
@@ -641,29 +595,25 @@ class CanvasBatchPlan(BatchPlan):
         top-left of slots 0, 1, ...; the remaining slots are empty (count 0).  img_infos: optional per-image clip bounds
         (im_h, im_w) (forward.py passes (H, H), SURVEY.md Q7); default (H_n, W_n).  None reuses the current slots, sizes and
         clip bounds.  Returns BatchPlan.forward's (list of prob, list of boxes, counts)."""
-        if images is not None and self.raw_input:
-            raise FrcnnError("CanvasBatchPlan(raw_input=True) takes raw photos through forward_raw")
         if images is not None:
-            images = list(images)
-            if len(images) > self.N:
-                raise FrcnnError("CanvasBatchPlan: %d images for %d slots" % (len(images), self.N))
-            if img_infos is not None and len(img_infos) != len(images):
-                raise FrcnnError("CanvasBatchPlan: %d img_infos for %d images" % (len(img_infos), len(images)))
-            sizes = np.zeros((2, self.N, 2), dtype=np.int32)
-            for n, x in enumerate(images):
-                if x.dim() != 3 or x.shape[0] != 3 or not (0 < x.shape[1] <= self.H and 0 < x.shape[2] <= self.W):
-                    raise FrcnnError("CanvasBatchPlan: image %d of shape %s does not fit a (3,%d,%d) canvas" %
-                                     (n, tuple(x.shape), self.H, self.W))
-                sizes[0, n] = x.shape[1:]
-                sizes[1, n] = x.shape[1:] if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
-            for n, x in enumerate(images):
-                self.x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
-            # a pageable source: the copy is staged before copy_ returns, so `sizes` may go out of scope at once
-            self._sizes.copy_(torch.from_numpy(sizes), non_blocking=True)
-            self.image_sizes = [tuple(int(v) for v in sizes[0, n]) for n in range(self.N)]
-        _launch(self)
-        counts = self.result.view(self.N, self.block_words)[:, self.result_layout["count"][0]]
-        return [im["prob"] for im in self.images], [im["boxes"] for im in self.images], counts
+            if self.raw_input:
+                raise FrcnnError("CanvasBatchPlan(raw_input=True) takes raw photos through forward_raw")
+            sizes = _fill_canvas(list(images), img_infos, self.x_in, self._sizes)
+            self.image_sizes = [tuple(int(v) for v in e) for e in sizes[0]]
+        return super(CanvasBatchPlan, self).forward(None)
+
+
+def _fill_canvas(images, img_infos, x_in, sizes_dev):
+    """Float (3,H_n,W_n) CUDA images into the top-left of the slots of the canvas x_in [N,3,Hc,Wc], and their extents and
+    clip bounds into sizes_dev [2,N,2] (preprocess.canvas_sizes, which raises first if they do not fit).  Returns the host
+    sizes array."""
+    N, _, Hc, Wc = x_in.shape
+    sizes = preprocess.canvas_sizes([tuple(x.shape) for x in images], N, Hc, Wc, img_infos)
+    for n, x in enumerate(images):
+        x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
+    # a pageable source: the copy is staged before copy_ returns, so `sizes` may go out of scope at once
+    sizes_dev.copy_(torch.from_numpy(sizes), non_blocking=True)
+    return sizes
 
 
 class LanePool(object):
@@ -823,7 +773,6 @@ class CanvasStreamRunner(object):
     def _deliver(self, b, batches, results, on_result):
         s, N = b % self.depth, self.plan.N
         self.step_done[s].synchronize()
-        from . import preprocess
         res = self.plan.unpack_result(self.res[s].np)
         for n, im_scale in enumerate(batches[b][1]):
             dets = preprocess.result_detections(res[n], im_scale)
@@ -837,33 +786,24 @@ class CanvasStreamRunner(object):
         im_scale) in image order and returns the list of detections; a last partial batch runs with its other slots empty."""
         plan, D, L, N = self.plan, self.depth, len(self.pool), self.plan.N
         raw_images = list(raw_images)
-        for i, x in enumerate(raw_images):
-            if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or x.ndim != 3 or x.shape[2] != 3:
-                raise FrcnnError("CanvasStreamRunner: image %d is not a uint8 (h, w, 3) numpy array" % i)
-        from . import preprocess
-        batches = []
-        for s0 in range(0, len(raw_images), N):
-            chunk = raw_images[s0:s0 + N]
-            batches.append(plan.raw_batch_header([x.shape[:2] for x in chunk], None if img_infos is None else img_infos[s0:s0 + N]))
+        shapes = preprocess.raw_photo_shapes(raw_images)
+        batches = [plan.raw_batch_header(shapes[s0:s0 + N], None if img_infos is None else img_infos[s0:s0 + N])
+                   for s0 in range(0, len(raw_images), N)]
         results = []
         self.pool.fork()
         self.copy_stream.wait_stream(torch.cuda.current_stream())
-        for b, (hdr, scales, used) in enumerate(batches):
+        for b, (hdr, _, _) in enumerate(batches):
             s, k = b % D, b % L
             lane, cur = self.pool.plans[k], self.pool.streams[k]
             if b >= D:
                 self._deliver(b - D, batches, results, on_result)         # slot reuse: batch b-D is finished and handed over
-            pin = self.stage[s]
-            pin.np[:hdr.size] = hdr
-            offs = preprocess.raw_header_views(hdr, N)["src_off"]
-            for n in range(len(scales)):
-                ops.host_copy(pin.ptr + plan.header_bytes + int(offs[n]), np.ascontiguousarray(raw_images[b * N + n]))
+            nbytes = preprocess.fill_raw_block(self.stage[s].np, hdr, raw_images[b * N:b * N + N], N)
             if b >= L:
                 self.copy_stream.wait_event(self.lane_done[k])            # the lane's previous replay no longer reads its block
-            pin.h2d(lane.block, self.copy_stream, nbytes=plan.header_bytes + used)
+            self.stage[s].h2d(lane.block, self.copy_stream, nbytes=nbytes)
             self.h2d_done[s].record(self.copy_stream)
             self.h2d_copies += 1
-            self.h2d_bytes += plan.header_bytes + used
+            self.h2d_bytes += nbytes
             with torch.cuda.stream(cur):
                 cur.wait_event(self.h2d_done[s])
                 lane.forward(None)
@@ -893,52 +833,54 @@ class _PlanLease(object):
 class Engine(object):
     """Weights + per-shape plans.  `engine(x)` -> (prob [R,21], boxes [R,84]) device tensors, R synced."""
     supports_hwc_input = True          # the VGG16 plan's first kernel takes source strides (ForwardPlan(hwc_input=True))
+    plan_class = ForwardPlan           # the one-image plan of plan() / thread_plan()
 
     def __init__(self, params, precision="bf16x3", device="cuda", anchors=None, num_classes=21, n_anchors=9,
                  feat_stride=16, **plan_kwargs):
-        self.weights = PackedWeights(params, precision, device, num_classes, n_anchors)
+        self.weights = self._pack_weights(params, precision, device, num_classes, n_anchors)
         self.anchors, self.feat_stride = anchors, feat_stride
         self.plan_kwargs = plan_kwargs
         self.plans = {}
-        import threading
         self._tls, self._lock = threading.local(), threading.Lock()
+        self._plan_pool = {}               # thread_plan: the plans handed back, per base plan
 
-    def plan(self, H, W, **overrides):
+    def _pack_weights(self, params, precision, device, num_classes, n_anchors):
+        return PackedWeights(params, precision, device, num_classes, n_anchors)
+
+    def _cached(self, kind, cls, shape, overrides):
+        """The cls plan of `shape` with the engine's plan options updated by `overrides`, built on first use; cached under
+        (kind, *shape, options), or (*shape, options) when kind is None."""
         kw = dict(self.plan_kwargs)
         kw.update(overrides)
-        key = (H, W, tuple(sorted(kw.items())))
+        key = (() if kind is None else (kind,)) + tuple(shape) + (tuple(sorted(kw.items())),)
         if key not in self.plans:
-            self.plans[key] = ForwardPlan(self.weights, H, W, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
+            self.plans[key] = cls(self.weights, *shape, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
         return self.plans[key]
 
+    def plan(self, H, W, **overrides):
+        return self._cached(None, self.plan_class, (H, W), overrides)
+
     def thread_plan(self, H, W, **overrides):
-        """A ForwardPlan private to the calling thread (buffers, graph, stream over the shared weights): several host
-        threads may call the model concurrently, one image each, and their graphs overlap on the GPU.  Plans live in a pool
-        per (shape, options): a thread checks one out on its first call and a finalizer on its thread-local state hands it
-        back when the thread ends, so the next thread reuses the captured graph and the pinned staging -- nothing is freed
-        at thread exit (cudaFree / cudaFreeHost there would stall every other caller)."""
-        kw = dict(self.plan_kwargs)
-        kw.update(overrides)
-        key = (H, W, tuple(sorted(kw.items())))
+        """A plan private to the calling thread (buffers, graph, stream over the shared weights): several host threads may
+        call the model concurrently, one image each, and their graphs overlap on the GPU.  Plans live in a pool per (shape,
+        options): a thread checks one out on its first call and a finalizer on its thread-local state hands it back when
+        the thread ends, so the next thread reuses the captured graph and the pinned staging -- nothing is freed at thread
+        exit (cudaFree / cudaFreeHost there would stall every other caller)."""
         held = self._tls.__dict__.setdefault("plans", {})
-        lease = held.get(key)
+        call = (H, W, tuple(sorted(overrides.items())))
+        lease = held.get(call)
         if lease is None:
             with self._lock:
-                pool = self.__dict__.setdefault("_plan_pool", {}).setdefault(key, [])
-                p = pool.pop() if pool else None
-                if p is None:
-                    base = self.plan(H, W, **overrides)
-                    if not getattr(base, "_leased", False):
-                        p = base
-                    else:
-                        p = base.clone()
+                base = self.plan(H, W, **overrides)
+                pool = self._plan_pool.setdefault(base, [])
+                p = pool.pop() if pool else (base.clone() if getattr(base, "_leased", False) else base)
                 p._leased = True
-            lease = held[key] = _PlanLease(self, key, p)
+            lease = held[call] = _PlanLease(self, base, p)
         return lease.plan
 
-    def _return_plan(self, key, plan):
+    def _return_plan(self, base, plan):
         with self._lock:
-            self.__dict__.setdefault("_plan_pool", {}).setdefault(key, []).append(plan)
+            self._plan_pool.setdefault(base, []).append(plan)
 
     def call_host(self, x_np, img_info=None, **overrides):
         """Host-array call: x_np float32 (3,H,W) numpy -> dict of numpy results (ForwardPlan.forward_host).  A C-contiguous
@@ -972,12 +914,7 @@ class Engine(object):
 
     def batch_plan(self, N, H, W, **overrides):
         """The BatchPlan for N images of H x W (cached per shape and options)."""
-        kw = dict(self.plan_kwargs)
-        kw.update(overrides)
-        key = ("batch", N, H, W, tuple(sorted(kw.items())))
-        if key not in self.plans:
-            self.plans[key] = BatchPlan(self.weights, N, H, W, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
-        return self.plans[key]
+        return self._cached("batch", BatchPlan, (N, H, W), overrides)
 
     def forward_batch(self, x_nchw, img_info=None, **overrides):
         """N same-size images (N,3,H,W) float32 CUDA -> list of per-image (prob [R_n,NC], boxes [R_n,4NC]) device tensors,
@@ -994,12 +931,7 @@ class Engine(object):
 
     def canvas_plan(self, N, Hc, Wc, **overrides):
         """The CanvasBatchPlan of N slots of Hc x Wc (cached per canvas and options)."""
-        kw = dict(self.plan_kwargs)
-        kw.update(overrides)
-        key = ("canvas", N, Hc, Wc, tuple(sorted(kw.items())))
-        if key not in self.plans:
-            self.plans[key] = CanvasBatchPlan(self.weights, N, Hc, Wc, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
-        return self.plans[key]
+        return self._cached("canvas", CanvasBatchPlan, (N, Hc, Wc), overrides)
 
     def forward_images(self, images, img_infos=None, N=None, canvas=None, **overrides):
         """Images of any sizes, a list of (3,H_n,W_n) float32 CUDA tensors -> list of per-image (prob [R_n,NC], boxes
@@ -1030,7 +962,6 @@ class Engine(object):
         """The CanvasBatchPlan(raw_input=True, with_detect=True) that serves `raw_images` N per replay: the canvas defaults
         to the largest resized H and W, each rounded up to a multiple of 64, and the arena to N times the largest photo,
         rounded up to 1 MiB."""
-        from . import preprocess
         shapes = [tuple(int(v) for v in x.shape[:2]) for x in raw_images]
         N = len(shapes) if N is None else int(N)
         if canvas is None:
@@ -1047,7 +978,6 @@ class Engine(object):
         preprocess.detections gives, (cls_id, x1, y1, x2, y2, score) in source-image coordinates.  N images per graph
         replay (default: all of them), one upload and one download per replay; the canvas as raw_canvas_plan picks it.
         img_infos: optional per-image clip bounds (forward.py passes the resized (H, H))."""
-        from . import preprocess
         raw_images = list(raw_images)
         if not raw_images:
             return []
@@ -1071,8 +1001,8 @@ def _c_structs(weights, H, W, anchors, pre_n, post_n, nms_thresh, min_size, feat
     p = lambda t: None if t is None else t.data_ptr()                     # noqa: E731
     layer = lambda hi, lo, b: _lib.PackedLayer(p(hi), p(lo), p(b))         # noqa: E731
     wt = _lib.Vgg16Weights()
-    for i, item in enumerate([it for it in VGG16_LAYERS if it != "pool"]):
-        wt.conv[i] = layer(*weights.convs[item[0]])
+    for i, s in enumerate(vgg16_schedule(H, W, True)[0]):
+        wt.conv[i] = layer(*weights.convs[s.name])
     wt.rpn3, wt.rpn_heads = layer(*weights.rpn3), layer(*weights.rpn_heads)
     wt.fc6, wt.fc7, wt.head = layer(*weights.fc6), layer(*weights.fc7), layer(*weights.head)
     wt.anchors = anchors.data_ptr()
@@ -1143,7 +1073,7 @@ class CCanvasForward(object):
     def __init__(self, weights, N, Hc, Wc, anchors, pre_n=6000, post_n=300, nms_thresh=0.7, min_size=16, feat_stride=16,
                  raw_input=False, pixel_means=None, arena_bytes=None, det_nms_thresh=0.3, det_conf=0.8):
         import ctypes
-        from . import _lib, preprocess
+        from . import _lib
         if int(N) != N or N < 1:
             raise FrcnnError("CCanvasForward needs N >= 1 images (got %r)" % (N,))
         self._lib, self._ct = _lib.load(), ctypes
@@ -1206,20 +1136,7 @@ class CCanvasForward(object):
         0, 1, ...; the other slots are empty.  img_infos: optional per-image clip bounds (im_h, im_w), default (H_n, W_n)."""
         if self.raw_input:
             raise FrcnnError("CCanvasForward(raw_input=True) takes raw photos (stage_raw / detect_raw)")
-        images = list(images)
-        if len(images) > self.N or (img_infos is not None and len(img_infos) != len(images)):
-            raise FrcnnError("CCanvasForward: %d images (%s img_infos) for %d slots" %
-                             (len(images), "no" if img_infos is None else len(img_infos), self.N))
-        sizes = np.zeros((2, self.N, 2), dtype=np.int32)
-        for n, x in enumerate(images):
-            if x.dim() != 3 or x.shape[0] != 3 or not (0 < x.shape[1] <= self.H and 0 < x.shape[2] <= self.W):
-                raise FrcnnError("CCanvasForward: image %d of shape %s does not fit a (3,%d,%d) canvas" %
-                                 (n, tuple(x.shape), self.H, self.W))
-            sizes[0, n] = x.shape[1:]
-            sizes[1, n] = x.shape[1:] if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
-        for n, x in enumerate(images):
-            self.x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
-        self._sizes.copy_(torch.from_numpy(sizes), non_blocking=True)        # pageable: staged before copy_ returns
+        _fill_canvas(list(images), img_infos, self.x_in, self._sizes)
 
     def forward(self, images, img_infos=None):
         """set_images + launch.  Returns (prob [N,post_n,NC], boxes [N,post_n,4NC], count [N]) device tensors; rows past an
@@ -1231,28 +1148,21 @@ class CCanvasForward(object):
     def stage_raw(self, photos, img_infos=None):
         """Raw input: at most N uint8 (h0,w0,3) BGR numpy photos and their header (preprocess.raw_batch_header) into the block
         with one host-to-device copy, and their im_scale into `im_scale`.  Returns the list of im_scale."""
-        from . import preprocess
         if not self.raw_input:
             raise FrcnnError("CCanvasForward: raw photos need raw_input=True")
         photos = list(photos)
-        for n, x in enumerate(photos):
-            if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or x.ndim != 3 or x.shape[2] != 3:
-                raise FrcnnError("CCanvasForward: photo %d is not a uint8 (h, w, 3) numpy array" % n)
-        hdr, scales, used = preprocess.raw_batch_header([x.shape[:2] for x in photos], self.N, self.H, self.W, self.arena_bytes,
-                                                        img_infos)
+        hdr, scales, _ = preprocess.raw_batch_header(preprocess.raw_photo_shapes(photos), self.N, self.H, self.W, self.arena_bytes,
+                                                     img_infos)
         cur = torch.cuda.current_stream()
         if self._stage is None:
             self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), ops.PinnedBlock((self.N,), np.float64),
                            torch.cuda.Event())
         pin, pin_scale, done = self._stage
         done.synchronize()                    # the previous upload has left the pinned mirrors
-        pin.np[:hdr.size] = hdr
-        offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
-        for n, x in enumerate(photos):
-            ops.host_copy(pin.ptr + self.header_bytes + int(offs[n]), np.ascontiguousarray(x))
+        nbytes = preprocess.fill_raw_block(pin.np, hdr, photos, self.N)
         pin_scale.np[:] = 0.0
         pin_scale.np[:len(scales)] = scales
-        pin.h2d(self.block, cur, nbytes=self.header_bytes + used)
+        pin.h2d(self.block, cur, nbytes=nbytes)
         pin_scale.h2d(self.im_scale, cur)
         done.record(cur)
         return scales

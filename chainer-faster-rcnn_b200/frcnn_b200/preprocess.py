@@ -88,6 +88,45 @@ def raw_header_views(buf, N):
     return {name: buf[off:off + 8 * N].view(dt).reshape((N, 2) if items == 2 else (N,)) for name, (off, dt, items) in layout.items()}
 
 
+def canvas_sizes(shapes, N, Hc, Wc, img_infos=None):
+    """The int32 [2, N, 2] extents (row 0) and clip bounds (row 1) of one canvas batch of float images: shapes = the
+    (3, H, W) of at most N images, each at the top-left of its Hc x Wc slot; the remaining slots are empty (0 x 0).
+    img_infos: per-image clip bounds, default (H, W).  Raises FrcnnError when there are too many images or an image does
+    not fit the canvas."""
+    if len(shapes) > N or (img_infos is not None and len(img_infos) != len(shapes)):
+        raise _lib.FrcnnError("canvas batch: %d images (%s img_infos) for %d slots" %
+                              (len(shapes), "no" if img_infos is None else len(img_infos), N))
+    sizes = np.zeros((2, N, 2), dtype=np.int32)
+    for n, shape in enumerate(shapes):
+        if len(shape) != 3 or shape[0] != 3 or not (0 < shape[1] <= Hc and 0 < shape[2] <= Wc):
+            raise _lib.FrcnnError("canvas batch: image %d of shape %s does not fit a (3,%d,%d) canvas" % (n, tuple(shape), Hc, Wc))
+        sizes[0, n] = shape[1:]
+        sizes[1, n] = shape[1:] if img_infos is None else (int(img_infos[n][0]), int(img_infos[n][1]))
+    return sizes
+
+
+def raw_photo_shapes(photos):
+    """The (h0, w0) of raw photos; raises FrcnnError unless every one is a uint8 (h, w, 3) numpy array."""
+    for n, x in enumerate(photos):
+        if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or x.ndim != 3 or x.shape[2] != 3:
+            raise _lib.FrcnnError("raw batch: photo %d is not a uint8 (h, w, 3) numpy array" % n)
+    return [x.shape[:2] for x in photos]
+
+
+def fill_raw_block(buf, hdr, photos, N):
+    """Writes one batch into `buf`, a uint8 numpy view of a host [header | pixels] block for N slots: the header that
+    raw_batch_header made for `photos` (raw_photo_shapes' photos), then each photo at its src_off.  Returns the bytes to
+    upload, header included."""
+    offs = raw_header_views(hdr, N)["src_off"]
+    nbytes = hdr.size + max([int(offs[n]) + x.nbytes for n, x in enumerate(photos)], default=0)
+    if nbytes > buf.size:
+        raise _lib.FrcnnError("raw batch: %d bytes for a block of %d" % (nbytes, buf.size))
+    buf[:hdr.size] = hdr
+    for n, x in enumerate(photos):
+        ops.host_copy(buf.ctypes.data + hdr.size + int(offs[n]), np.ascontiguousarray(x))
+    return nbytes
+
+
 def raw_batch_header(shapes, N, Hc, Wc, arena_bytes, img_infos=None, scale=600, max_size=1000):
     """The header of one batch of raw images: shapes = the (h0, w0) of at most N uint8 BGR images, laid out one after the
     other (RAW_ALIGN) in a pixel area of arena_bytes; the remaining slots are empty.  img_infos: per-image clip bounds,

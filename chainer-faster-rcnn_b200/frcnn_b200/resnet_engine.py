@@ -127,23 +127,15 @@ class ResNetForwardPlan(ForwardPlan):
 class ResNetEngine(Engine):
     """`Engine` for FasterRCNN(trunk_class=ResNet, rpn_in_ch=2048, feat_stride=32)."""
     supports_hwc_input = False         # the 7x7 first layer's im2col kernel reads dense (C,H,W) only
+    plan_class = ResNetForwardPlan
 
     def __init__(self, params, n_layers=101, precision="bf16x3", device="cuda", anchors=None, num_classes=21, n_anchors=9,
                  feat_stride=32, **plan_kwargs):
-        self.weights = ResNetPackedWeights(params, n_layers, precision, device, num_classes, n_anchors)
-        self.anchors, self.feat_stride = anchors, feat_stride
-        self.plan_kwargs = plan_kwargs
-        self.plans = {}
-        import threading
-        self._tls, self._lock = threading.local(), threading.Lock()
+        self.n_layers = n_layers
+        super(ResNetEngine, self).__init__(params, precision, device, anchors, num_classes, n_anchors, feat_stride, **plan_kwargs)
 
-    def plan(self, H, W, **overrides):
-        kw = dict(self.plan_kwargs)
-        kw.update(overrides)
-        key = (H, W, tuple(sorted(kw.items())))
-        if key not in self.plans:
-            self.plans[key] = ResNetForwardPlan(self.weights, H, W, anchors=self.anchors, feat_stride=self.feat_stride, **kw)
-        return self.plans[key]
+    def _pack_weights(self, params, precision, device, num_classes, n_anchors):
+        return ResNetPackedWeights(params, self.n_layers, precision, device, num_classes, n_anchors)
 
     def batch_plan(self, N, H, W, **overrides):
         raise FrcnnError("ResNetEngine runs one image at a time: batches (BatchPlan) need the VGG16 trunk")

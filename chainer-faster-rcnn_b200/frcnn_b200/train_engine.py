@@ -22,12 +22,13 @@ import torch
 
 from . import ops, shard, train_ops
 from ._lib import FrcnnError
-from .engine import VGG16_LAYERS
+from .engine import vgg16_schedule
 
 ROIS_PER_IMAGE, FG_FRACTION = 128, 0.25                          # models/proposal_target_layer.py:49-50
 FG_THRESH, BG_THRESH_HI, BG_THRESH_LO = 0.5, 0.5, 0.1            # :46-48
-TRUNK = [it for it in VGG16_LAYERS if it != "pool"]              # (name, cin, cout) x 13
-POOL_AFTER = {VGG16_LAYERS[i - 1][0] for i, it in enumerate(VGG16_LAYERS) if it == "pool"}
+_STEPS = vgg16_schedule(1, 1, fuse_pool=False)[0]                # the layer table; training never fuses a pool
+TRUNK = [s[:3] for s in _STEPS]                                  # (name, cin, cout) x 13
+POOL_AFTER = {s.name for s in _STEPS if s.pool_after}
 
 
 class _ConvTrainer(object):

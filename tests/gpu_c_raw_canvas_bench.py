@@ -80,16 +80,12 @@ class CRawStream(object):
             chunk, s = imgs[s0:s0 + cf.N], b % D
             if b >= D:
                 deliver(b - D)                        # slot reuse: batch b-D is finished
-            hdr, scales, used = preprocess.raw_batch_header([x.shape[:2] for x in chunk], cf.N, cf.H, cf.W, cf.arena_bytes)
+            hdr, scales, _ = preprocess.raw_batch_header(preprocess.raw_photo_shapes(chunk), cf.N, cf.H, cf.W, cf.arena_bytes)
             batches.append(len(chunk))
-            pin = self.stage[s]
-            pin.np[:hdr.size] = hdr
-            offs = preprocess.raw_header_views(hdr, cf.N)["src_off"]
-            for n, x in enumerate(chunk):
-                ops.host_copy(pin.ptr + cf.header_bytes + int(offs[n]), x)
+            nbytes = preprocess.fill_raw_block(self.stage[s].np, hdr, chunk, cf.N)
             self.scale[s].np[:] = 0.0
             self.scale[s].np[:len(scales)] = scales
-            pin.h2d(cf.block, cur, nbytes=cf.header_bytes + used)
+            self.stage[s].h2d(cf.block, cur, nbytes=nbytes)
             self.scale[s].h2d(cf.im_scale, cur)
             self.graph.replay()
             self.res[s].d2h(cf.lists, cur)
