@@ -121,9 +121,11 @@ __global__ void __launch_bounds__(1024) rcnn_loss_kernel(const float* __restrict
             if (dhead) dhead[(size_t)r * ld + num_classes + j] = (float)((ad < delta ? d : (d > 0 ? delta : -delta)) * grad_scale / n);
         }
         for (int o = 16; o > 0; o >>= 1) hub += __shfl_xor_sync(0xffffffffu, hub, o);
+        // softmax as exp(z - m) / se, not exp(z - lse): at |m| beyond ~2^29 lse = m + log(se) rounds log(se) away and
+        // classes tied at the maximum would each get probability 1
         if (dhead)
             for (int c = lane; c < num_classes; c += 32)
-                dhead[(size_t)r * ld + c] = (float)((exp((double)z[c] - lse) - (c == t ? 1.0 : 0.0)) * grad_scale / n);
+                dhead[(size_t)r * ld + c] = (float)((exp((double)z[c] - m) / se - (c == t ? 1.0 : 0.0)) * grad_scale / n);
         // a ground-truth class outside [0, num_classes) (a dataset with another class count, a NaN label) must not index the
         // score row: its loss becomes NaN -- loud in the reported loss, the caller's check -- instead of a silently wrong value
         const bool t_ok = t >= 0 && t < num_classes;
@@ -267,8 +269,8 @@ int frcnn_rcnn_loss(const float* head_out, int ld, int R_cap, const int* keep_in
                     const float* bbox_reg_targets, int num_classes, double delta, double grad_scale, float* losses, float* dhead,
                     void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(head_out && keep_inds && labels && bbox_reg_targets && losses && R_cap > 0 && ld >= 5 * num_classes,
-                  "rcnn_loss: bad arguments");
+    FRCNN_REQUIRE(head_out && keep_inds && labels && bbox_reg_targets && losses && R_cap > 0 && num_classes >= 1 &&
+                  ld / 5 >= num_classes, "rcnn_loss: bad arguments");                   // ld >= 5*num_classes, no overflow
     FRCNN_REQUIRE(n >= 1 && n <= 128, "rcnn_loss: 1 <= kept rows <= 128 (ROIS_PER_IMAGE), got %d", n);
     FRCNN_REQUIRE(delta > 0, "rcnn_loss: delta must be positive");
     rcnn_loss_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(head_out, ld, R_cap, keep_inds, n, labels, bbox_reg_targets, num_classes,

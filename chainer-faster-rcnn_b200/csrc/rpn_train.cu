@@ -403,6 +403,10 @@ int frcnn_anchor_targets(const double* anchors, int A, int feat_h, int feat_w, i
     FRCNN_REQUIRE(anchors && gt_boxes && labels_full && targets_full && inds_inside && counts && workspace, "anchor_targets: null pointer");
     FRCNN_REQUIRE(subsample_mode >= 0 && subsample_mode <= 2, "anchor_targets: subsample_mode %d not in {0,1,2}", subsample_mode);
     FRCNN_REQUIRE(subsample_mode != 2 || n_disable == 0 || disable_pos, "anchor_targets: mode 2 without an index list");
+    // the reference's np.random.choice raises when asked for more negatives than exist; here num_bg = batch - n_fg would
+    // go negative and the normaliser counts[1] + counts[2] with it
+    FRCNN_REQUIRE(subsample_mode != 1 || (num_fg >= 0 && num_fg <= batch),
+                  "anchor_targets: mode 1 needs 0 <= num_fg <= batch, got num_fg=%d batch=%d", num_fg, batch);
     FRCNN_REQUIRE(aligned(targets_full, 16), "anchor_targets: targets_full must be 16-byte aligned");
     const long n_all_l = (long)A * feat_h * feat_w;
     FRCNN_REQUIRE(n_all_l < (1l << 30), "anchor_targets: too many anchors");
@@ -445,7 +449,9 @@ int frcnn_rpn_loss(const float* score, long score_cs, long score_ps, const float
     FRCNN_REQUIRE(score && bbox && anchors && labels_full && targets_full && counts && losses && workspace, "rpn_loss: null pointer");
     FRCNN_REQUIRE(aligned(targets_full, 16), "rpn_loss: targets_full must be 16-byte aligned");
     FRCNN_REQUIRE(delta > 0, "rpn_loss: delta must be positive");
-    const int n_all = A * feat_h * feat_w;
+    const long n_all_l = (long)A * feat_h * feat_w;
+    FRCNN_REQUIRE(n_all_l < (1l << 30), "rpn_loss: too many anchors");
+    const int n_all = (int)n_all_l;
     if (workspace_bytes < frcnn_rpn_loss_workspace_bytes(n_all)) {
         set_error("rpn_loss: workspace %zu < %zu bytes", workspace_bytes, frcnn_rpn_loss_workspace_bytes(n_all));
         return FRCNN_ERR_WORKSPACE;

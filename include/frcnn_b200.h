@@ -532,14 +532,23 @@ int frcnn_bbox_overlaps(const double* boxes, int n, const double* query, int k, 
  *   subsample_mode 0: labels BEFORE subsampling (:131-146);
  *                  1: device subsampling (:148-168) by a counter hash of (seed, anchor index) -- the
  *                     reference draws from NumPy's global RNG on the host, which cannot be matched
- *                     bit-for-bit without that host state; no host sync;
+ *                     bit-for-bit without that host state; no host sync.  Requires 0 <= num_fg <= batch.
+ *                     Rule: with key(s, i) = (mix64(s ^ i*0xD6E8FEB86659FD93) & 0xFFFFFFFF00000000) | i
+ *                     in uint64 (mix64 = one splitmix64 step: add 0x9E3779B97F4A7C15, then its
+ *                     finaliser; i = anchor index in [0, n_all)), if n_fg > num_fg the
+ *                     n_fg - num_fg positives with the smallest key(seed, i) become -1; then, with
+ *                     num_bg = batch - (positives left), if n_bg > num_bg the n_bg - num_bg negatives with
+ *                     the smallest key(seed ^ 0xA5A5A5A5DEADBEEF, i) become -1 (the top 32 bits of the
+ *                     key decide, the lower index goes first on a tie);
  *                  2: disable_pos[n_disable] = positions in the inside-compact arrays to set to -1
  *                     (exactly what the reference's np.random.choice calls return).
  * Outputs (device): labels_full int32 [n_all] in {-1,0,1}, -1 for anchors outside the image
  *   (= bbox_labels_mapped of region_proposal_network.py:164-165); targets_full float32 [n_all,4]
  *   (16-byte aligned; zeros outside); inds_inside int32 [n_all capacity] (ascending);
  *   counts int32 [8] = {n_inside, n_fg, n_bg, n_fg before subsampling, n_bg before, n_all, 0, 0}.
- * The reference's compact outputs are labels_full[inds_inside], targets_full[inds_inside]. */
+ * The reference's compact outputs are labels_full[inds_inside], targets_full[inds_inside].
+ * No anchor inside the image (the reference raises on its empty arg-max): counts = {0, 0, 0, 0, 0, n_all, 0, 0},
+ * every label -1, every target 0, and frcnn_rpn_loss then returns four zero losses and zero gradients. */
 size_t frcnn_anchor_targets_workspace_bytes(int n_all, int n_gt);
 int frcnn_anchor_targets(const double* anchors, int A, int feat_h, int feat_w, int feat_stride, const float* gt_boxes,
                          int n_gt, int im_h, int im_w, double neg_thr, double pos_thr, int batch, int num_fg,
@@ -583,7 +592,9 @@ int frcnn_bbox_transform(const float* ex_rois, const float* gt_rois, int gt_stri
 int frcnn_keep_inside(const float* boxes, int n, int im_h, int im_w, unsigned char* flags, void* stream);
 /* faster_rcnn.py:151-165 on the merged head output head_out [R_cap][ld] (columns [0,num_classes) scores, then
  * 4*num_classes deltas): losses float32 [4] = {loss_cls, loss_bbox, cls_accuracy, loss_rcnn}; dhead (optional, same shape)
- * = grad_scale * d(loss_rcnn)/d(head_out), zero on rows not kept.  1 <= n <= 128. */
+ * = grad_scale * d(loss_rcnn)/d(head_out), zero on rows not kept and on columns >= 5*num_classes.  1 <= n <= 128,
+ * num_classes >= 1, ld >= 5*num_classes.  keep_inds must not repeat a row (the reference's sampling never does): a repeated
+ * row's gradient is written, not summed.  A label outside [0, num_classes) makes loss_cls NaN; loss_bbox stays finite. */
 int frcnn_rcnn_loss(const float* head_out, int ld, int R_cap, const int* keep_inds, int n, const int* labels,
                     const float* bbox_reg_targets, int num_classes, double delta, double grad_scale, float* losses, float* dhead,
                     void* stream);
