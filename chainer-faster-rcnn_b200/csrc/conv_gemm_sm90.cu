@@ -720,8 +720,8 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
                        const int* extents = nullptr, int ext_halvings = 0) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     for (int& v : g_last_plan) v = 0;          // a call that launches nothing leaves an empty record
-    FRCNN_REQUIRE(n_img >= 1 && (n_img == 1 || (!ge && !m_valid && !re)), "frcnn_conv2d: bad batch of %d images", n_img);
-    FRCNN_REQUIRE(!extents || (!ge && !m_valid && !re && ext_halvings >= 0 && ext_halvings <= 30),
+    FRCNN_REQUIRE(n_img >= 1 && (n_img == 1 || (!ge && !m_valid)), "frcnn_conv2d: bad batch of %d images", n_img);
+    FRCNN_REQUIRE(!extents || (!ge && !m_valid && ext_halvings >= 0 && ext_halvings <= 30),
                   "frcnn_conv2d: extents need a plain convolution and 0 <= halvings <= 30 (got %d)", ext_halvings);
     FRCNN_REQUIRE(x_hi && w_hi && (bias || ge), "frcnn_conv2d: x_hi, w_hi and bias are required");
     FRCNN_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "frcnn_conv2d: x_lo and w_lo must both be given (bf16x3) or both NULL");
@@ -955,6 +955,29 @@ extern "C" int frcnn_conv2d_batch_ext(const void* x_hi, const void* x_lo, int N,
     FRCNN_REQUIRE(N >= 1 && extents, "frcnn_conv2d_batch_ext: needs N >= 1 (got %d) and the device extents", N);
     return conv2d_impl(x_hi, x_lo, H, W, Cin, w_hi, w_lo, bias, Cout, ksize, relu, fuse_pool2x2, y_hi, y_lo, y_f32, ld_f32,
                        nullptr, stream_, nullptr, nullptr, nullptr, N, extents, halvings);
+}
+
+// the residual is [N][H][W][Cout] like the output: the epilogue reads it at the output pixel's own image offset, and a pixel
+// outside a canvas extent is zeroed after the add, whatever the residual holds there
+extern "C" int frcnn_conv2d_res_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi,
+                                      const void* w_lo, const float* bias, int Cout, int ksize, int relu, const void* res_hi,
+                                      const void* res_lo, void* y_hi, void* y_lo, void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1, "frcnn_conv2d_res_batch: N must be >= 1 (got %d)", N);
+    ResExtra re{res_hi, res_lo};
+    return conv2d_impl(x_hi, x_lo, H, W, Cin, w_hi, w_lo, bias, Cout, ksize, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_,
+                       nullptr, &re, nullptr, N);
+}
+
+extern "C" int frcnn_conv2d_res_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi,
+                                          const void* w_lo, const float* bias, int Cout, int ksize, int relu, const void* res_hi,
+                                          const void* res_lo, void* y_hi, void* y_lo, const int* extents, int halvings,
+                                          void* stream_) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && extents, "frcnn_conv2d_res_batch_ext: needs N >= 1 (got %d) and the device extents", N);
+    ResExtra re{res_hi, res_lo};
+    return conv2d_impl(x_hi, x_lo, H, W, Cin, w_hi, w_lo, bias, Cout, ksize, relu, 0, y_hi, y_lo, nullptr, 0, nullptr, stream_,
+                       nullptr, &re, nullptr, N, extents, halvings);
 }
 
 extern "C" int frcnn_conv3x3_c8_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi,

@@ -33,26 +33,51 @@ __device__ __forceinline__ void store8f(__nv_bfloat16* hi, __nv_bfloat16* lo, lo
     if (lo) *reinterpret_cast<uint4*>(lo + off) = *reinterpret_cast<const uint4*>(l);
 }
 
+// Output size of a ksize / stride / pad convolution over e input pixels (0 when not even one window fits).  C division
+// truncates towards zero, so a negative numerator is answered before it is divided.
+__host__ __device__ __forceinline__ int conv_out(int e, int ks, int stride, int pad) {
+    const int t = e + 2 * pad - ks;
+    return t < 0 ? 0 : t / stride + 1;
+}
+
+// Output size of the 3x3 / 2, pad 0, cover_all max-pool over c pixels: ceil((c - 3) / 2) + 1 = (c - 2) / 2 + 1, 0 for c <= 1.
+__host__ __device__ __forceinline__ int pool3s2_out(int c) { return c < 2 ? 0 : (c - 2) / 2 + 1; }
+
 // General first-layer im2col: (C,H,W) fp32 -> [Ho][Wo][Kp] bf16 hi/lo, K index (r*ks + s)*C + c, zero padded borders,
-// zeros for k >= ks*ks*C.  One thread per 8 consecutive k of one output pixel.
+// zeros for k >= ks*ks*C.  One thread per 8 consecutive k of one output pixel; blockIdx.y is the image of a batch
+// ((N,C,H,W) in, [N][Ho][Wo][Kp] out).  extents (a canvas batch; NULL: every image fills H x W): image n is extents[2n] x
+// extents[2n+1] input pixels, a tap outside it reads as the zero padding and every output pixel outside
+// conv_out(extent) is written as 0.
 __global__ void im2col_kernel(const float* __restrict__ x, int C, int H, int W, int ks, int stride, int pad, int Ho, int Wo,
-                              int Kp, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+                              int Kp, const int* __restrict__ extents, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
     const int k8n = Kp / 8;
     const long total = (long)Ho * Wo * k8n;
     const int kmax = ks * ks * C;
+    const int img = blockIdx.y;
+    x += (long)img * C * H * W;
+    hi += (long)img * Ho * Wo * Kp;
+    if (lo) lo += (long)img * Ho * Wo * Kp;
+    int eh = H, ew = W, oh = Ho, ow = Wo;
+    if (extents) {
+        eh = canvas_extent(extents, img, 0, 0, H);
+        ew = canvas_extent(extents, img, 1, 0, W);
+        oh = conv_out(eh, ks, stride, pad);
+        ow = conv_out(ew, ks, stride, pad);
+    }
     for (long t = blockIdx.x * (long)blockDim.x + threadIdx.x; t < total; t += (long)gridDim.x * blockDim.x) {
         const int k8 = (int)(t % k8n);
         const long p = t / k8n;
         const int wo = (int)(p % Wo), ho = (int)(p / Wo);
+        const bool live = ho < oh && wo < ow;
         float v[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int k = k8 * 8 + j;
             float val = 0.f;
-            if (k < kmax) {
+            if (live && k < kmax) {
                 const int tap = k / C, c = k - tap * C;
                 const int hh = ho * stride - pad + tap / ks, ww = wo * stride - pad + tap % ks;
-                if (hh >= 0 && hh < H && ww >= 0 && ww < W) val = x[((long)c * H + hh) * W + ww];
+                if (hh >= 0 && hh < eh && ww >= 0 && ww < ew) val = x[((long)c * H + hh) * W + ww];
             }
             v[j] = val;
         }
@@ -80,46 +105,89 @@ __global__ void pack_weights_im2col_general_kernel(const float* __restrict__ w, 
 }
 
 // F.max_pooling_2d(x, 3, stride=2) with Chainer's defaults pad=0, cover_all=True: Ho = ceil((H-3)/2) + 1, windows clipped
-// at the bottom / right border.
+// at the bottom / right border.  blockIdx.y is the image of a batch ([N][H][W][C] -> [N][Ho][Wo][C]).  extents (a canvas
+// batch of N images, each at the top-left of its H x W slot, at THIS map's resolution; NULL: H x W each): a window is
+// clipped at the image's own border exactly as at the slot's, so no pixel outside the image is ever read, and every output
+// pixel outside pool3s2_out(extent) is written as 0.
 __global__ void maxpool3x3s2_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl, int H, int W, int C,
-                                    int Ho, int Wo, __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl) {
+                                    int Ho, int Wo, const int* __restrict__ extents, __nv_bfloat16* __restrict__ yh,
+                                    __nv_bfloat16* __restrict__ yl) {
     const int C8 = C / 8;
     const long total = (long)Ho * Wo * C8;
+    const int img = blockIdx.y;
+    xh += (long)img * H * W * C;
+    if (xl) xl += (long)img * H * W * C;
+    yh += (long)img * Ho * Wo * C;
+    if (yl) yl += (long)img * Ho * Wo * C;
+    int eh = H, ew = W, oh = Ho, ow = Wo;
+    if (extents) {
+        eh = canvas_extent(extents, img, 0, 0, H);
+        ew = canvas_extent(extents, img, 1, 0, W);
+        oh = pool3s2_out(eh);
+        ow = pool3s2_out(ew);
+    }
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         const int c8 = (int)(i % C8);
         const long p = i / C8;
         const int wo = (int)(p % Wo), ho = (int)(p / Wo);
         float m[8];
-        bool first = true;
-        for (int dy = 0; dy < 3; ++dy) {
-            const int h = ho * 2 + dy;
-            if (h >= H) break;
-            for (int dx = 0; dx < 3; ++dx) {
-                const int w = wo * 2 + dx;
-                if (w >= W) break;
-                float v[8];
-                load8f(xh, xl, ((long)h * W + w) * C + c8 * 8, v);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) m[j] = first ? v[j] : fmaxf(m[j], v[j]);
-                first = false;
+        for (int j = 0; j < 8; ++j) m[j] = 0.f;
+        if (ho < oh && wo < ow) {           // the window's first pixel (2ho, 2wo) lies inside the image
+            bool first = true;
+            for (int dy = 0; dy < 3; ++dy) {
+                const int h = ho * 2 + dy;
+                if (h >= eh) break;
+                for (int dx = 0; dx < 3; ++dx) {
+                    const int w = wo * 2 + dx;
+                    if (w >= ew) break;
+                    float v[8];
+                    load8f(xh, xl, ((long)h * W + w) * C + c8 * 8, v);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) m[j] = first ? v[j] : fmaxf(m[j], v[j]);
+                    first = false;
+                }
             }
         }
         store8f(yh, yl, p * C + c8 * 8, m);
     }
 }
 
-// pixels (2h, 2w): the input of a stride-2, pad-0 1x1 convolution
+// pixels (2h, 2w): the input of a stride-2, pad-0 1x1 convolution; blockIdx.y is the image of a batch
 __global__ void subsample2x_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl, int H, int W, int C,
                                    int Ho, int Wo, __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl) {
     const int C8 = C / 8;
     const long total = (long)Ho * Wo * C8;
+    const long xo = (long)blockIdx.y * H * W * C, yo = (long)blockIdx.y * Ho * Wo * C;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         const int c8 = (int)(i % C8);
         const long p = i / C8;
         const int wo = (int)(p % Wo), ho = (int)(p / Wo);
-        const long src = ((long)(2 * ho) * W + 2 * wo) * C + c8 * 8, dst = p * C + c8 * 8;
+        const long src = xo + ((long)(2 * ho) * W + 2 * wo) * C + c8 * 8, dst = yo + p * C + c8 * 8;
         *reinterpret_cast<uint4*>(yh + dst) = *reinterpret_cast<const uint4*>(xh + src);
         if (xl) *reinterpret_cast<uint4*>(yl + dst) = *reinterpret_cast<const uint4*>(xl + src);
+    }
+}
+
+// The per-level extents of a ResNet canvas batch: out [5][N][2] = conv1, pool1, res3, res4, res5 (res2 keeps pool1's),
+// each clamped to that level's canvas size.  One thread per image.
+__global__ void resnet_level_extents_kernel(const int* __restrict__ extents, int N, int Hc, int Wc, int* __restrict__ out) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    for (int axis = 0; axis < 2; ++axis) {
+        int lim = axis ? Wc : Hc;
+        int e = canvas_extent(extents, n, axis, 0, lim);
+        lim = conv_out(lim, 7, 2, 3);
+        e = min(conv_out(e, 7, 2, 3), lim);
+        out[(0 * N + n) * 2 + axis] = e;
+        lim = pool3s2_out(lim);
+        e = min(pool3s2_out(e), lim);
+        out[(1 * N + n) * 2 + axis] = e;
+        for (int k = 2; k < 5; ++k) {
+            lim = (lim + 1) / 2;
+            e = min((e + 1) / 2, lim);
+            out[(k * N + n) * 2 + axis] = e;
+        }
     }
 }
 
@@ -133,20 +201,63 @@ static int grid_cover(long total, int block) {
 
 using namespace frcnn;
 
+// the launches behind the one-image, batch and canvas-batch entries
+static int im2col_launch(const float* x, int N, int C, int H, int W, int ksize, int stride, int pad, int K_pad, const int* extents,
+                         void* y_hi, void* y_lo, void* stream) {
+    FRCNN_REQUIRE(x && y_hi && C > 0 && H > 0 && W > 0 && ksize > 0 && stride > 0 && pad >= 0, "pack_image_im2col: bad arguments");
+    FRCNN_REQUIRE(K_pad % 8 == 0 && K_pad >= ksize * ksize * C, "pack_image_im2col: K_pad must be a multiple of 8 and >= ksize^2*C");
+    const int Ho = conv_out(H, ksize, stride, pad), Wo = conv_out(W, ksize, stride, pad);
+    FRCNN_REQUIRE(Ho > 0 && Wo > 0, "pack_image_im2col: image smaller than the filter");
+    const long total = (long)Ho * Wo * (K_pad / 8);
+    im2col_kernel<<<dim3(grid_cover(total, 256), N), 256, 0, (cudaStream_t)stream>>>(x, C, H, W, ksize, stride, pad, Ho, Wo, K_pad,
+                                                                                  extents, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+static int maxpool3x3s2_launch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, const int* extents, void* y_hi,
+                               void* y_lo, void* stream) {
+    FRCNN_REQUIRE(x_hi && y_hi && H >= 3 && W >= 3 && C > 0 && C % 8 == 0, "maxpool3x3s2_ceil: bad arguments (H=%d W=%d C=%d)", H, W, C);
+    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "maxpool3x3s2_ceil: lo planes must both be given or both NULL");
+    const int Ho = pool3s2_out(H), Wo = pool3s2_out(W);
+    const long total = (long)Ho * Wo * (C / 8);
+    maxpool3x3s2_kernel<<<dim3(grid_cover(total, 256), N), 256, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, H, W, C, Ho, Wo, extents, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+static int subsample2x_launch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_REQUIRE(x_hi && y_hi && H > 0 && W > 0 && C > 0 && C % 8 == 0, "subsample2x: bad arguments");
+    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "subsample2x: lo planes must both be given or both NULL");
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    const long total = (long)Ho * Wo * (C / 8);
+    subsample2x_kernel<<<dim3(grid_cover(total, 256), N), 256, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, H, W, C, Ho, Wo, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
 extern "C" {
 
 int frcnn_pack_image_im2col(const float* x_chw, int C, int H, int W, int ksize, int stride, int pad, int K_pad, void* y_hi,
                             void* y_lo, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(x_chw && y_hi && C > 0 && H > 0 && W > 0 && ksize > 0 && stride > 0 && pad >= 0, "pack_image_im2col: bad arguments");
-    FRCNN_REQUIRE(K_pad % 8 == 0 && K_pad >= ksize * ksize * C, "pack_image_im2col: K_pad must be a multiple of 8 and >= ksize^2*C");
-    const int Ho = (H + 2 * pad - ksize) / stride + 1, Wo = (W + 2 * pad - ksize) / stride + 1;
-    FRCNN_REQUIRE(Ho > 0 && Wo > 0, "pack_image_im2col: image smaller than the filter");
-    const long total = (long)Ho * Wo * (K_pad / 8);
-    im2col_kernel<<<grid_cover(total, 256), 256, 0, (cudaStream_t)stream>>>(x_chw, C, H, W, ksize, stride, pad, Ho, Wo, K_pad,
-                                                                         (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return im2col_launch(x_chw, 1, C, H, W, ksize, stride, pad, K_pad, nullptr, y_hi, y_lo, stream);
+}
+
+int frcnn_pack_image_im2col_batch(const float* x_nchw, int N, int C, int H, int W, int ksize, int stride, int pad, int K_pad,
+                                  void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "pack_image_im2col_batch: N must be in [1, 65535] (got %d)", N);
+    return im2col_launch(x_nchw, N, C, H, W, ksize, stride, pad, K_pad, nullptr, y_hi, y_lo, stream);
+}
+
+int frcnn_pack_image_im2col_batch_ext(const float* x_nchw, int N, int C, int H, int W, int ksize, int stride, int pad, int K_pad,
+                                      const int* extents, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && extents, "pack_image_im2col_batch_ext: needs N in [1, 65535] (got %d) and the device extents", N);
+    return im2col_launch(x_nchw, N, C, H, W, ksize, stride, pad, K_pad, extents, y_hi, y_lo, stream);
 }
 
 int frcnn_pack_conv_weights_im2col(const float* w_oihw, const float* scale, int Cout, int Cin, int ksize, int K_pad, void* w_hi,
@@ -162,24 +273,38 @@ int frcnn_pack_conv_weights_im2col(const float* w_oihw, const float* scale, int 
 
 int frcnn_maxpool3x3s2_ceil(const void* x_hi, const void* x_lo, int H, int W, int C, void* y_hi, void* y_lo, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(x_hi && y_hi && H >= 3 && W >= 3 && C > 0 && C % 8 == 0, "maxpool3x3s2_ceil: bad arguments (H=%d W=%d C=%d)", H, W, C);
-    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "maxpool3x3s2_ceil: lo planes must both be given or both NULL");
-    const int Ho = (H - 3 + 1) / 2 + 1, Wo = (W - 3 + 1) / 2 + 1;            // ceil((H-3)/2) + 1
-    const long total = (long)Ho * Wo * (C / 8);
-    maxpool3x3s2_kernel<<<grid_cover(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, H, W, C, Ho, Wo, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return maxpool3x3s2_launch(x_hi, x_lo, 1, H, W, C, nullptr, y_hi, y_lo, stream);
+}
+
+int frcnn_maxpool3x3s2_ceil_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "maxpool3x3s2_ceil_batch: N must be in [1, 65535] (got %d)", N);
+    return maxpool3x3s2_launch(x_hi, x_lo, N, H, W, C, nullptr, y_hi, y_lo, stream);
+}
+
+int frcnn_maxpool3x3s2_ceil_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int C, const int* extents, void* y_hi,
+                                      void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && extents, "maxpool3x3s2_ceil_batch_ext: needs N in [1, 65535] (got %d) and the device extents", N);
+    return maxpool3x3s2_launch(x_hi, x_lo, N, H, W, C, extents, y_hi, y_lo, stream);
 }
 
 int frcnn_subsample2x(const void* x_hi, const void* x_lo, int H, int W, int C, void* y_hi, void* y_lo, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(x_hi && y_hi && H > 0 && W > 0 && C > 0 && C % 8 == 0, "subsample2x: bad arguments");
-    FRCNN_REQUIRE((x_lo == nullptr) == (y_lo == nullptr), "subsample2x: lo planes must both be given or both NULL");
-    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
-    const long total = (long)Ho * Wo * (C / 8);
-    subsample2x_kernel<<<grid_cover(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x_hi, (const __nv_bfloat16*)x_lo, H, W, C, Ho, Wo, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
+    return subsample2x_launch(x_hi, x_lo, 1, H, W, C, y_hi, y_lo, stream);
+}
+
+int frcnn_subsample2x_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "subsample2x_batch: N must be in [1, 65535] (got %d)", N);
+    return subsample2x_launch(x_hi, x_lo, N, H, W, C, y_hi, y_lo, stream);
+}
+
+int frcnn_resnet_level_extents(const int* extents, int N, int Hc, int Wc, int* out, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(extents && out, "resnet_level_extents: NULL extents or output");
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && Hc > 0 && Wc > 0, "resnet_level_extents: bad shape N=%d Hc=%d Wc=%d", N, Hc, Wc);
+    resnet_level_extents_kernel<<<cdiv(N, 128), 128, 0, (cudaStream_t)stream>>>(extents, N, Hc, Wc, out);
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }

@@ -110,6 +110,19 @@ SIGNATURES = {
     "frcnn_pack_conv_weights_im2col": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_maxpool3x3s2_ceil": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_subsample2x": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "frcnn_pack_image_im2col_batch": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                              c_void_p]),
+    "frcnn_pack_image_im2col_batch_ext": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                                  c_void_p, c_void_p, c_void_p]),
+    "frcnn_maxpool3x3s2_ceil_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "frcnn_maxpool3x3s2_ceil_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p]),
+    "frcnn_subsample2x_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "frcnn_conv2d_res_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                       c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_conv2d_res_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                           c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "frcnn_resnet_level_extents": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "frcnn_roi_overlaps": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_roi_targets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "frcnn_bbox_transform": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -371,13 +371,14 @@ class BatchPlan(_PlanBase):
     ForwardPlan's on that image.  The result buffer holds N consecutive blocks in ForwardPlan's layout, so the host gets
     everything with one D2H; the batched post-processing reads and writes those blocks in place at a stride of one block.
     Takes ForwardPlan's keyword options."""
+    _trunk_name, _trunk_layer = "VGG16", "conv1_1"        # the trunk the launch sequence runs, and a layer only it has
 
     def __init__(self, weights, N, H, W, **options):
         if int(N) != N or N < 1:
             raise FrcnnError("BatchPlan needs N >= 1 images (got %r)" % (N,))
         super(BatchPlan, self).__init__(weights, H, W, **options)
-        if "conv1_1" not in weights.convs:
-            raise FrcnnError("BatchPlan runs the VGG16 trunk only")
+        if self._trunk_layer not in weights.convs:
+            raise FrcnnError("%s runs the %s trunk only" % (type(self).__name__, self._trunk_name))
         N = self.N = int(N)
         self._lead = (N,)
         dev, post_n = weights.device, self.post_n
@@ -414,9 +415,9 @@ class BatchPlan(_PlanBase):
         """The first launch: the static input -> the compact first-layer planes acts[0]."""
         ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input, extents=self.extents)
 
-    def _run(self):
-        w, N, post_n = self.w, self.N, self.post_n
-        ext = self.extents
+    def _run_trunk(self):
+        """Launches the input stage and the trunk; returns (feature map Act, number of launches)."""
+        w, N, ext = self.w, self.N, self.extents
         self._pack_input()
         n = 1
         acts = iter(self.acts)
@@ -434,8 +435,18 @@ class BatchPlan(_PlanBase):
                 x = next(acts)
                 ops.maxpool2x2_ceil_batch(y, out=x)
                 n += 1
-        feat = self.feat = x
-        k = VGG16_LAYERS.count("pool")
+        return x, n
+
+    def _feature_extents(self):
+        """(extents, halvings) of the feature map for the RPN, ProposalLayer and RoI pooling launches: the image extents
+        after the trunk's four ceil-mode pools (None: every image fills its slot)."""
+        return self.extents, VGG16_LAYERS.count("pool")
+
+    def _run(self):
+        w, N, post_n = self.w, self.N, self.post_n
+        feat, n = self._run_trunk()
+        self.feat = feat
+        ext, k = self._feature_extents()
         hi, lo, b = w.rpn3
         ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid, extents=ext, halvings=k)
         hi, lo, b = w.rpn_heads

@@ -431,6 +431,110 @@ def subsample2x(x, out=None):
     return out
 
 
+def _dense_planes(what, *acts):
+    for a in acts:
+        for t in (a.hi, a.lo):
+            if t is not None and not t.is_contiguous():
+                raise FrcnnError("%s: planes must be dense [N,H,W,C]" % what)
+
+
+def resnet_level_extents(extents, Hc, Wc, out=None):
+    """frcnn_resnet_level_extents: int32 [N, 2] device image sizes in Hc x Wc canvas slots -> int32 [5, N, 2] device extents of
+    the ResNet levels conv1, pool1, res3, res4, res5 (each clamped to that level's canvas)."""
+    N = int(extents.shape[0])
+    ext = _per_image_pairs(extents, N, "extents")
+    if out is None:
+        out = torch.empty((5, N, 2), dtype=torch.int32, device=extents.device)
+    if out.dtype != torch.int32 or tuple(out.shape) != (5, N, 2) or not out.is_contiguous():
+        raise FrcnnError("resnet_level_extents: out must be a dense int32 [5, %d, 2] CUDA tensor" % N)
+    check(_lib.load().frcnn_resnet_level_extents(ext, N, int(Hc), int(Wc), _p(out), _stream()), "frcnn_resnet_level_extents")
+    return out
+
+
+def pack_image_im2col_batch(x_nchw, ksize, stride, pad, k_pad, precision="bf16x3", out=None, extents=None):
+    """(N,C,H,W) float32 CUDA images -> Act [N,Ho,Wo,k_pad]: pack_image_im2col_general of every image.  extents: int32 [N, 2]
+    device image sizes in the H x W slots (frcnn_pack_image_im2col_batch_ext: taps outside an image read as the zero padding,
+    output pixels outside its own output size are written as 0)."""
+    _need_cuda(x_nchw)
+    x = x_nchw.contiguous().float()
+    N, C, H, W = x.shape
+    Ho, Wo = (H + 2 * pad - ksize) // stride + 1, (W + 2 * pad - ksize) // stride + 1
+    if out is None:
+        hi = torch.empty((N, Ho, Wo, k_pad), dtype=torch.bfloat16, device=x.device)
+        out = Act(hi, torch.empty_like(hi) if precision == "bf16x3" else None)
+    if tuple(out.hi.shape) != (N, Ho, Wo, k_pad):
+        raise FrcnnError("pack_image_im2col_batch: output %s, expected %s" % (tuple(out.hi.shape), (N, Ho, Wo, k_pad)))
+    _dense_planes("pack_image_im2col_batch", out)
+    lib = _lib.load()
+    if extents is not None:
+        check(lib.frcnn_pack_image_im2col_batch_ext(_p(x), N, C, H, W, ksize, stride, pad, k_pad, _per_image_pairs(extents, N, "extents"),
+                                                    _p(out.hi), _p(out.lo), _stream()), "frcnn_pack_image_im2col_batch_ext")
+        return out
+    check(lib.frcnn_pack_image_im2col_batch(_p(x), N, C, H, W, ksize, stride, pad, k_pad, _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_pack_image_im2col_batch")
+    return out
+
+
+def maxpool3x3s2_ceil_batch(x, out=None, extents=None):
+    """frcnn_maxpool3x3s2_ceil_batch: Act [N,H,W,C] -> Act [N,ceil((H-3)/2)+1,...,C], one launch.  extents: int32 [N, 2] device
+    image sizes at THIS map's resolution (frcnn_maxpool3x3s2_ceil_batch_ext: windows clipped at each image's border, output
+    pixels outside the image's pooled size written as 0)."""
+    N, H, W, C = x.hi.shape
+    if out is None:
+        yh = torch.empty((N, (H - 2) // 2 + 1, (W - 2) // 2 + 1, C), dtype=torch.bfloat16, device=x.hi.device)
+        out = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    _dense_planes("maxpool3x3s2_ceil_batch", x, out)
+    lib = _lib.load()
+    if extents is not None:
+        check(lib.frcnn_maxpool3x3s2_ceil_batch_ext(_p(x.hi), _p(x.lo), N, H, W, C, _per_image_pairs(extents, N, "extents"), _p(out.hi),
+                                                    _p(out.lo), _stream()), "frcnn_maxpool3x3s2_ceil_batch_ext")
+        return out
+    check(lib.frcnn_maxpool3x3s2_ceil_batch(_p(x.hi), _p(x.lo), N, H, W, C, _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_maxpool3x3s2_ceil_batch")
+    return out
+
+
+def subsample2x_batch(x, out=None):
+    """frcnn_subsample2x_batch: Act [N,H,W,C] -> Act [N,ceil(H/2),ceil(W/2),C], one launch.  On a canvas the input must be 0
+    outside every image; the output then is too."""
+    N, H, W, C = x.hi.shape
+    if out is None:
+        yh = torch.empty((N, (H + 1) // 2, (W + 1) // 2, C), dtype=torch.bfloat16, device=x.hi.device)
+        out = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    _dense_planes("subsample2x_batch", x, out)
+    check(_lib.load().frcnn_subsample2x_batch(_p(x.hi), _p(x.lo), N, H, W, C, _p(out.hi), _p(out.lo), _stream()),
+          "frcnn_subsample2x_batch")
+    return out
+
+
+def conv2d_res_batch(x, w_hi, w_lo, bias, ksize, relu, res, out=None, extents=None, halvings=0):
+    """frcnn_conv2d_res_batch: conv2d_res over x Act [N,H,W,Cin] with res an Act [N,H,W,Cout]; each image equals conv2d_res on
+    it, bit for bit.  extents: int32 [N, 2] device image sizes, ceil(extent / 2^halvings) at this layer
+    (frcnn_conv2d_res_batch_ext: every output pixel outside is written as 0)."""
+    N, H, W, Cin = x.hi.shape
+    taps, Cout, cin_w = w_hi.shape
+    if cin_w != Cin or taps != ksize * ksize or tuple(res.hi.shape) != (N, H, W, Cout) or \
+            (res.lo is not None and tuple(res.lo.shape) != (N, H, W, Cout)):
+        raise FrcnnError("conv2d_res_batch: shapes do not match (x %s, w %s, res %s)" % (tuple(x.hi.shape), tuple(w_hi.shape),
+                                                                                          tuple(res.hi.shape)))
+    if (x.lo is None) != (w_lo is None):
+        raise FrcnnError("conv2d_res_batch: activation and weight precision modes differ")
+    if out is None:
+        yh = torch.empty((N, H, W, Cout), dtype=torch.bfloat16, device=x.hi.device)
+        out = Act(yh, torch.empty_like(yh) if x.lo is not None else None)
+    _dense_planes("conv2d_res_batch", res, out)
+    lib = _lib.load()
+    if extents is not None:
+        check(lib.frcnn_conv2d_res_batch_ext(_p(x.hi), _p(x.lo), N, H, W, Cin, _p(w_hi), _p(w_lo), _p(bias), Cout, ksize,
+                                             1 if relu else 0, _p(res.hi), _p(res.lo), _p(out.hi), _p(out.lo),
+                                             _per_image_pairs(extents, N, "extents"), int(halvings), _stream()),
+              "frcnn_conv2d_res_batch_ext")
+        return out
+    check(lib.frcnn_conv2d_res_batch(_p(x.hi), _p(x.lo), N, H, W, Cin, _p(w_hi), _p(w_lo), _p(bias), Cout, ksize, 1 if relu else 0,
+                                     _p(res.hi), _p(res.lo), _p(out.hi), _p(out.lo), _stream()), "frcnn_conv2d_res_batch")
+    return out
+
+
 def set_conv_tile(block_n=0, tile_h=0, tile_w=0):
     _lib.load().frcnn_conv2d_set_tile(block_n, tile_h, tile_w)
 

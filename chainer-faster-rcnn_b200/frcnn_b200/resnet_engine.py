@@ -19,7 +19,7 @@ import torch
 
 from . import ops
 from ._lib import FrcnnError
-from .engine import Engine, ForwardPlan, PackedWeights, _t
+from .engine import BatchPlan, CanvasBatchPlan, Engine, ForwardPlan, PackedWeights, _t
 
 RESNET_BLOCKS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
 RESNET_STAGES = (("res2", 64, 64, 256, 1), ("res3", 256, 128, 512, 2), ("res4", 512, 256, 1024, 2), ("res5", 1024, 512, 2048, 2))
@@ -124,6 +124,73 @@ class ResNetForwardPlan(ForwardPlan):
         return self.blocks[-1]["out"], n
 
 
+class ResNetBatchPlan(BatchPlan):
+    """BatchPlan with the ResNet trunk: N images of one shape in ONE CUDA graph, every launch of ResNetForwardPlan's trunk
+    once over all N (frcnn_pack_image_im2col_batch, frcnn_maxpool3x3s2_ceil_batch, frcnn_subsample2x_batch,
+    frcnn_conv2d_batch, frcnn_conv2d_res_batch), then BatchPlan's RPN / ProposalLayer / RoI pool / head.  Every image's
+    results are bit-identical to a ResNetForwardPlan's on that image.  Takes ForwardPlan's keyword options except
+    hwc_input (the 7x7 first layer reads dense (C,H,W) images) and keep_rpn_debug."""
+    _trunk_name, _trunk_layer = "ResNet", "conv1"
+    _alloc_trunk = ResNetForwardPlan._alloc_trunk      # activations through self._act: [N, ...] planes in a batch
+
+    def __init__(self, weights, N, H, W, **options):
+        for opt, why in (("raw_input", "raw photos need the VGG16 trunk's first layer"),
+                         ("hwc_input", "the 7x7 first layer reads dense (3,H,W) images"),
+                         ("keep_rpn_debug", "no RPN debug outputs")):
+            if options.get(opt):
+                raise FrcnnError("%s: %s=True is not supported (%s)" % (type(self).__name__, opt, why))
+        super(ResNetBatchPlan, self).__init__(weights, N, H, W, **options)
+        # a canvas batch: the extents of conv1, pool1, res3, res4 and res5, derived on the device by the first launch
+        self.level_ext = None if self.extents is None else torch.zeros((5, self.N, 2), dtype=torch.int32, device=weights.device)
+
+    def _run_trunk(self):
+        cv, lv = self.w.convs, self.level_ext
+        ext = lambda k: None if lv is None else lv[k]          # noqa: E731  (level k's [N, 2] extents, halvings 0)
+        n = 0
+        if lv is not None:
+            ops.resnet_level_extents(self.extents, self.H, self.W, out=lv)
+            n += 1
+        ops.pack_image_im2col_batch(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col, extents=self.extents)
+        hi, lo, b = cv["conv1"]
+        ops.conv2d_batch(self.x_col, hi, lo, b, 1, True, out=self.c1, extents=ext(0))
+        ops.maxpool3x3s2_ceil_batch(self.c1, out=self.p1, extents=ext(0))
+        n += 3
+        level = 1
+        for B in self.blocks:
+            x = B["x"]
+            if B["stride"] == 2:
+                ops.subsample2x_batch(x, out=B["xs"])
+                x = B["xs"]
+                level += 1
+                n += 1
+            e = ext(level)
+            hi, lo, b = cv[B["name"] + "/conv1"]
+            ops.conv2d_batch(x, hi, lo, b, 1, True, out=B["y1"], extents=e)
+            hi, lo, b = cv[B["name"] + "/conv2"]
+            ops.conv2d_batch(B["y1"], hi, lo, b, 3, True, out=B["y2"], extents=e)
+            if B["proj"]:
+                hi, lo, b = cv[B["name"] + "/conv4"]
+                ops.conv2d_batch(x, hi, lo, b, 1, False, out=B["sc"], extents=e)
+                res = B["sc"]
+                n += 1
+            else:
+                res = B["x"]
+            hi, lo, b = cv[B["name"] + "/conv3"]
+            ops.conv2d_res_batch(B["y2"], hi, lo, b, 1, True, res, out=B["out"], extents=e)
+            n += 3
+        return self.blocks[-1]["out"], n
+
+    def _feature_extents(self):
+        return (None if self.level_ext is None else self.level_ext[4]), 0
+
+
+class ResNetCanvasBatchPlan(ResNetBatchPlan, CanvasBatchPlan):
+    """CanvasBatchPlan with the ResNet trunk: N images of different sizes, each at the top-left of its Hc x Wc slot, in ONE
+    captured graph.  The first launch derives every level's extents from the per-image sizes (frcnn_resnet_level_extents);
+    each later launch reads its level's and writes 0 outside every image, so each image's results are bit-identical to a
+    ResNetForwardPlan's on that image alone.  Preprocessed float images only (no raw_input)."""
+
+
 class ResNetEngine(Engine):
     """`Engine` for FasterRCNN(trunk_class=ResNet, rpn_in_ch=2048, feat_stride=32)."""
     supports_hwc_input = False         # the 7x7 first layer's im2col kernel reads dense (C,H,W) only
@@ -138,10 +205,26 @@ class ResNetEngine(Engine):
         return ResNetPackedWeights(params, self.n_layers, precision, device, num_classes, n_anchors)
 
     def batch_plan(self, N, H, W, **overrides):
-        raise FrcnnError("ResNetEngine runs one image at a time: batches (BatchPlan) need the VGG16 trunk")
+        raise FrcnnError("ResNetEngine runs one image at a time: batches (BatchPlan) need the VGG16 trunk or ResNetBatchEngine")
 
     def canvas_plan(self, N, Hc, Wc, **overrides):
-        raise FrcnnError("ResNetEngine runs one image at a time: canvas batches (CanvasBatchPlan) need the VGG16 trunk")
+        raise FrcnnError("ResNetEngine runs one image at a time: canvas batches (CanvasBatchPlan) need the VGG16 trunk or "
+                         "ResNetBatchEngine")
+
+
+class ResNetBatchEngine(ResNetEngine):
+    """ResNetEngine that also runs batches: batch_plan() is a ResNetBatchPlan and canvas_plan() a ResNetCanvasBatchPlan, so
+    Engine.forward_batch (N same-size images) and Engine.forward_images (images of different sizes on a canvas) run N images
+    per graph replay, each image bit-identical to ResNetForwardPlan on it.  Preprocessed float images only: detect_images
+    (raw photos) raises FrcnnError before anything is allocated.  ResNetEngine itself keeps running one image at a time."""
+
+    def batch_plan(self, N, H, W, **overrides):
+        """The ResNetBatchPlan for N images of H x W (cached per shape and options)."""
+        return self._cached("batch", ResNetBatchPlan, (N, H, W), overrides)
+
+    def canvas_plan(self, N, Hc, Wc, **overrides):
+        """The ResNetCanvasBatchPlan of N slots of Hc x Wc (cached per canvas and options)."""
+        return self._cached("canvas", ResNetCanvasBatchPlan, (N, Hc, Wc), overrides)
 
 
 class TrunkOnly(object):

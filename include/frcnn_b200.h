@@ -515,6 +515,52 @@ int frcnn_maxpool3x3s2_ceil(const void* x_hi, const void* x_lo, int H, int W, in
 /* Pixels (2h, 2w) of an NHWC map: the input of a stride-2 1x1 convolution.  [H][W][C] -> [ceil(H/2)][ceil(W/2)][C]. */
 int frcnn_subsample2x(const void* x_hi, const void* x_lo, int H, int W, int C, void* y_hi, void* y_lo, void* stream);
 
+/* The same kernels over a batch of N images of one shape in one launch (1 <= N <= 65535; image n's planes n image sizes
+ * into every buffer), each image bit-identical to the one-image entry on it:
+ *   frcnn_pack_image_im2col_batch    (N,C,H,W) fp32 -> [N][Ho][Wo][K_pad]
+ *   frcnn_maxpool3x3s2_ceil_batch    [N][H][W][C] -> [N][ceil((H-3)/2)+1][...][C]
+ *   frcnn_subsample2x_batch          [N][H][W][C] -> [N][ceil(H/2)][ceil(W/2)][C]
+ *   frcnn_conv2d_res_batch           frcnn_conv2d_res with x [N,H,W,Cin] and res, y [N,H,W,Cout] (frcnn_conv2d_batch's plan)
+ * The caller passes the residual planes of the output's shape; they are read at each output pixel's own image offset. */
+int frcnn_pack_image_im2col_batch(const float* x_nchw, int N, int C, int H, int W, int ksize, int stride, int pad, int K_pad,
+                                  void* y_hi, void* y_lo, void* stream);
+int frcnn_maxpool3x3s2_ceil_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo, void* stream);
+int frcnn_subsample2x_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int C, void* y_hi, void* y_lo, void* stream);
+int frcnn_conv2d_res_batch(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi, const void* w_lo,
+                           const float* bias, int Cout, int ksize, int relu, const void* res_hi, const void* res_lo, void* y_hi,
+                           void* y_lo, void* stream);
+/* A ResNet trunk over a CANVAS batch: image n sits at the top-left of its slot and its true size is extents[2n] x
+ * extents[2n+1] (device int32 [N][2], read at run time, clamped to the slot) at the resolution of the entry's INPUT.
+ *   frcnn_pack_image_im2col_batch_ext   extents in input pixels: a tap outside the image reads as the zero padding (whatever
+ *                                       the canvas holds there) and every output pixel outside the image's own output size
+ *                                       ((e + 2*pad - ksize) / stride + 1, 0 when negative) is written as 0.
+ *   frcnn_maxpool3x3s2_ceil_batch_ext   extents of the pooled map: each window is clipped at the image's border as the
+ *                                       one-image kernel clips it at the map's, so no pixel outside the image is read; every
+ *                                       output pixel outside (e - 2) / 2 + 1 (0 for e <= 1) is written as 0.
+ *   frcnn_conv2d_res_batch_ext          frcnn_conv2d_batch_ext with the residual add: every output pixel outside
+ *                                       ceil(extent / 2^halvings) is written as 0 after the add, whatever the residual holds
+ *                                       there.
+ * frcnn_subsample2x_batch needs no extents: an output pixel inside ceil(e / 2) reads an input pixel inside e, and one
+ * outside reads an input pixel outside e -- so its input must be 0 outside every image (what the entries above write),
+ * and the output then is too.  Each image's pixels equal the one-image entry on the image alone.  NULL extents or N outside
+ * [1, 65535] (frcnn_conv2d_res_batch_ext: N < 1, halvings outside [0,30]) -> FRCNN_ERR_ARG. */
+int frcnn_pack_image_im2col_batch_ext(const float* x_nchw, int N, int C, int H, int W, int ksize, int stride, int pad, int K_pad,
+                                      const int* extents, void* y_hi, void* y_lo, void* stream);
+int frcnn_maxpool3x3s2_ceil_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int C, const int* extents, void* y_hi,
+                                      void* y_lo, void* stream);
+int frcnn_conv2d_res_batch_ext(const void* x_hi, const void* x_lo, int N, int H, int W, int Cin, const void* w_hi, const void* w_lo,
+                               const float* bias, int Cout, int ksize, int relu, const void* res_hi, const void* res_lo, void* y_hi,
+                               void* y_lo, const int* extents, int halvings, void* stream);
+/* The per-level extents of a ResNet canvas batch of N Hc x Wc slots, in one launch (the first of the plan, so that every
+ * later launch reads its level's [N][2] slice with halvings 0): out (device int32 [5][N][2]) receives, per image and axis,
+ * from its extent e (extents [N][2], input pixels):
+ *   level 0  conv1 7x7/2 pad 3      c  = (e - 1) / 2 + 1               (0 for e = 0)
+ *   level 1  pool1 3x3/2 cover_all  p  = (c - 2) / 2 + 1               (0 for c <= 1)
+ *   level 2..4  res3, res4, res5    r' = (r + 1) / 2                   (res2 keeps level 1)
+ * each clamped to that level's canvas size (the same rules applied to Hc and Wc).  NULL pointers, N outside [1, 65535] or a
+ * non-positive canvas -> FRCNN_ERR_ARG. */
+int frcnn_resnet_level_extents(const int* extents, int N, int Hc, int Wc, int* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * RPN training targets and losses (SURVEY.md 8f rank 1, the train_rpn.py step).  Box arithmetic is
  * float64 in the reference's operation order: labels and indices are bit-identical to the reference.
