@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "nms_math.cuh"
+#include "raw_photo.cuh"
 
 namespace frcnn {
 
@@ -198,48 +199,14 @@ __global__ void pack_weights_c8_kernel(const float* w, int Cout, int Cin, __nv_b
 }
 
 // Caller-side preprocessing (forward.py:34-45, img_preprocessing): uint8 BGR HWC image -> float32(pixel - mean)
-// -> cv.resize(INTER_LINEAR) -> (3,H,W) float32.  One thread per output pixel, all three channels.  OpenCV's
-// float bilinear, restated: coordinate / floor / fraction in double, weight cast to float,
-// h = fma(S[x1] - S[x0], tx, S[x0]) on both source rows, out = fma(h1 - h0, ty, h0).
+// -> cv.resize(INTER_LINEAR) -> (3,H,W) float32.  One thread per output pixel, all three channels; the arithmetic is
+// bilinear_bgr8 (raw_photo.cuh).
 struct PreArgs {
     const unsigned char* src; int h0, w0;
     double m0, m1, m2, sx, sy;
     int H, W;
     float* out;
 };
-
-// One axis of the resize: output index o of a source axis of n pixels -> the two source indices and the weight of the
-// second.  Whatever inv_scale holds, i0 and i1 end up inside [0, n - 1] (the conversion to int saturates, NaN gives 0).
-struct BilinearTap { int i0, i1; float t; };
-__device__ __forceinline__ BilinearTap bilinear_tap(int o, double inv_scale, int n) {
-    const double f = ((double)o + 0.5) * inv_scale - 0.5;
-    BilinearTap r;
-    r.i0 = (int)floor(f);
-    r.t = (float)(f - (double)r.i0);
-    if (r.i0 < 0) { r.i0 = 0; r.t = 0.0f; }
-    if (r.i0 >= n - 1) { r.i0 = n - 1; r.t = 0.0f; }
-    r.i1 = min(r.i0 + 1, n - 1);
-    return r;
-}
-
-// The resized, mean-subtracted pixel at taps (y, x) of a dense uint8 (h0, w0, 3) image: out[c], c = B, G, R.  The one
-// statement of the arithmetic for preprocess_bgr8_kernel and preprocess_bgr8_canvas_kernel.
-__device__ __forceinline__ void bilinear_bgr8(const unsigned char* src, int w0, const BilinearTap& y, const BilinearTap& x,
-                                              double m0, double m1, double m2, float out[3]) {
-    const unsigned char* r0 = src + (long)y.i0 * w0 * 3;
-    const unsigned char* r1 = src + (long)y.i1 * w0 * 3;
-    const double mean[3] = {m0, m1, m2};
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const float p00 = (float)((double)r0[x.i0 * 3 + c] - mean[c]);
-        const float p01 = (float)((double)r0[x.i1 * 3 + c] - mean[c]);
-        const float p10 = (float)((double)r1[x.i0 * 3 + c] - mean[c]);
-        const float p11 = (float)((double)r1[x.i1 * 3 + c] - mean[c]);
-        const float ha = __fmaf_rn(__fsub_rn(p01, p00), x.t, p00);
-        const float hb = __fmaf_rn(__fsub_rn(p11, p10), x.t, p10);
-        out[c] = __fmaf_rn(__fsub_rn(hb, ha), y.t, ha);
-    }
-}
 
 __global__ void preprocess_bgr8_kernel(const PreArgs a) {
     const long total = (long)a.H * a.W;
@@ -257,7 +224,7 @@ __global__ void preprocess_bgr8_kernel(const PreArgs a) {
 // arena + src_off[n]; its resized extent, source size, offset and 1 / im_scale are device arrays read here, so a captured
 // launch serves any mix of sizes.  One block per stored row [Wc+2][8] of the slot (the last one also zeroes the 8 slack
 // pixels): the row's y taps are computed once per thread, and every stored pixel outside the extent is written as 0.  A
-// slot whose source does not lie inside [0, arena_bytes) or whose source size is not positive is an empty slot.
+// slot whose source does not lie inside [0, arena_bytes) or whose source size is not positive is an empty slot (raw_slot).
 struct PreCanvasArgs {
     const unsigned char* arena; long long arena_bytes;
     const long long* src_off; const int* src_hw; const double* inv_scale; const int* extents;
@@ -270,22 +237,16 @@ __global__ void preprocess_bgr8_canvas_kernel(const PreCanvasArgs a) {
     const int n = blockIdx.y, h = blockIdx.x, WP = a.Wc + 2;
     __nv_bfloat16* hi = a.hi + n * a.out_elems;
     __nv_bfloat16* lo = a.lo ? a.lo + n * a.out_elems : nullptr;
-    const int h0 = __ldg(a.src_hw + 2 * n), w0 = __ldg(a.src_hw + 2 * n + 1);
-    const long long off = __ldg(a.src_off + n);
-    const bool live = h0 > 0 && w0 > 0 && off >= 0 && off <= a.arena_bytes && (long long)h0 * w0 <= (a.arena_bytes - off) / 3;
-    const int eh = live ? canvas_extent(a.extents, n, 0, 0, a.Hc) : 0;
-    const int ew = live ? canvas_extent(a.extents, n, 1, 0, a.Wc) : 0;
+    const RawSlot s = raw_slot(a.arena, a.arena_bytes, a.src_off, a.src_hw, a.inv_scale, a.extents, n, a.Hc, a.Wc);
     F8 f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) f.v[j] = 0.0f;
     const long row = (long)h * WP;
-    if (h < eh) {
-        const unsigned char* src = a.arena + off;
-        const double inv = __ldg(a.inv_scale + n);
-        const BilinearTap ty = bilinear_tap(h, inv, h0);
+    if (h < s.eh) {
+        const BilinearTap ty = bilinear_tap(h, s.inv_scale, s.h0);
         for (int wp = threadIdx.x; wp < WP; wp += blockDim.x) {
             F8 g = f;
-            if (wp >= 1 && wp <= ew) bilinear_bgr8(src, w0, ty, bilinear_tap(wp - 1, inv, w0), a.m0, a.m1, a.m2, g.v);
+            if (wp >= 1 && wp <= s.ew) bilinear_bgr8(s.src, s.w0, ty, bilinear_tap(wp - 1, s.inv_scale, s.w0), a.m0, a.m1, a.m2, g.v);
             store8(hi, lo, (row + wp) * 8, g);
         }
     } else {

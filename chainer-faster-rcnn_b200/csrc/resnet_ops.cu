@@ -7,7 +7,9 @@
 //                                          -> frcnn_conv2d / frcnn_conv2d_res (residual add fused into the epilogue);
 //                                             a stride-2 1x1 convolution = frcnn_subsample2x + a stride-1 1x1 convolution
 // All three kernels are HBM-bound: 16-byte accesses along the channel axis of the NHWC bf16 hi/lo planes.
+// frcnn_preprocess_bgr8_canvas_im2col feeds conv1 of a canvas batch straight from raw uint8 photos.
 #include "common.cuh"
+#include "raw_photo.cuh"
 
 namespace frcnn {
 
@@ -82,6 +84,67 @@ __global__ void im2col_kernel(const float* __restrict__ x, int C, int H, int W, 
             v[j] = val;
         }
         store8f(hi, lo, p * Kp + k8 * 8, v);
+    }
+}
+
+// Raw photos straight into the first-layer im2col planes of a canvas batch: preprocess_bgr8_kernel, a copy into a zeroed
+// canvas and im2col_kernel(extents) for all N slots in one launch, bit for bit.  Slot blockIdx.y is raw_slot's; one CTA
+// per (band of `band` output rows, tile of `tile` output columns).  The CTA first stages the resized, mean-subtracted input
+// window its outputs read -- rows [ho0*stride - pad, +rows), columns [wo0*stride - pad, +cols), float32 [rows][cols][3] in
+// shared memory, 0 outside the image's extent -- so each input pixel's bilinear is computed once per CTA instead of once
+// per covering output pixel, then writes the tile's [Wo][Kp] rows as 16-byte hi/lo stores, reading every K index through
+// a table of its window offset.  Every output pixel outside conv_out(extent) and every k >= ks*ks*3 is written as 0.
+struct PreIm2colArgs {
+    const unsigned char* arena; long long arena_bytes;
+    const long long* src_off; const int* src_hw; const double* inv_scale; const int* extents;
+    int Hc, Wc, ks, stride, pad, Kp, Ho, Wo;
+    int band, tile, tiles, cols;        // output rows per band, output columns per tile, tiles per band, staged row pitch
+    double m0, m1, m2;
+    __nv_bfloat16 *hi, *lo;
+};
+__global__ void __launch_bounds__(256) preprocess_bgr8_canvas_im2col_kernel(const PreIm2colArgs a) {
+    extern __shared__ float smem[];
+    const int kmax = a.ks * a.ks * 3;
+    int* tab = reinterpret_cast<int*>(smem);           // [kmax]: window offset of K index k
+    float* win = smem + kmax;                          // [rows][a.cols][3]
+    const int n = blockIdx.y;
+    const int ho0 = (int)(blockIdx.x / a.tiles) * a.band, wo0 = (int)(blockIdx.x % a.tiles) * a.tile;
+    const int nb = min(a.band, a.Ho - ho0), nt = min(a.tile, a.Wo - wo0);
+    const RawSlot s = raw_slot(a.arena, a.arena_bytes, a.src_off, a.src_hw, a.inv_scale, a.extents, n, a.Hc, a.Wc);
+    const int oh = conv_out(s.eh, a.ks, a.stride, a.pad), ow = conv_out(s.ew, a.ks, a.stride, a.pad);
+    const bool any = ho0 < oh && wo0 < ow;             // CTA-uniform: a tile wholly outside the image only writes zeros
+    if (any) {
+        for (int k = threadIdx.x; k < kmax; k += blockDim.x) {
+            const int tap = k / 3, c = k - tap * 3;
+            tab[k] = ((tap / a.ks) * a.cols + tap % a.ks) * 3 + c;
+        }
+        const int y0 = ho0 * a.stride - a.pad, x0 = wo0 * a.stride - a.pad;
+        const int rows = a.stride * (nb - 1) + a.ks, cols = a.stride * (nt - 1) + a.ks;
+        for (int p = threadIdx.x; p < rows * cols; p += blockDim.x) {
+            const int i = p / cols, j = p - i * cols, y = y0 + i, x = x0 + j;
+            float v[3] = {0.0f, 0.0f, 0.0f};
+            if (y >= 0 && y < s.eh && x >= 0 && x < s.ew)
+                bilinear_bgr8(s.src, s.w0, bilinear_tap(y, s.inv_scale, s.h0), bilinear_tap(x, s.inv_scale, s.w0), a.m0, a.m1, a.m2, v);
+            float* w = win + (i * a.cols + j) * 3;
+            w[0] = v[0];
+            w[1] = v[1];
+            w[2] = v[2];
+        }
+    }
+    __syncthreads();
+    const int k8n = a.Kp / 8;
+    const long img = (long)n * a.Ho * a.Wo;
+    for (int t = threadIdx.x; t < nb * nt * k8n; t += blockDim.x) {
+        const int k8 = t % k8n, q = t / k8n, wl = q % nt, hl = q / nt;
+        const bool live = any && ho0 + hl < oh && wo0 + wl < ow;
+        const float* w = win + (hl * a.stride * a.cols + wl * a.stride) * 3;
+        float v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int k = k8 * 8 + j;
+            v[j] = live && k < kmax ? w[tab[k]] : 0.0f;
+        }
+        store8f(a.hi, a.lo, ((img + (long)(ho0 + hl) * a.Wo + wo0 + wl) * a.Kp) + k8 * 8, v);
     }
 }
 
@@ -191,6 +254,11 @@ __global__ void resnet_level_extents_kernel(const int* __restrict__ extents, int
     }
 }
 
+// frcnn_preprocess_bgr8_canvas_im2col: the shared memory of one CTA (the K table and the staged window), and the largest
+// filter whose one-output-pixel window (4 + 12 bytes per K index and window pixel) fits it
+static const size_t PRE_IM2COL_SMEM = 48 * 1024;
+static const int PRE_IM2COL_MAX_KSIZE = 45;
+
 static int grid_cover(long total, int block) {
     long g = (total + block - 1) / block;
     const long cap = 132l * 16;
@@ -258,6 +326,58 @@ int frcnn_pack_image_im2col_batch_ext(const float* x_nchw, int N, int C, int H, 
     FRCNN_ENTRY();
     FRCNN_REQUIRE(N >= 1 && N <= 65535 && extents, "pack_image_im2col_batch_ext: needs N in [1, 65535] (got %d) and the device extents", N);
     return im2col_launch(x_nchw, N, C, H, W, ksize, stride, pad, K_pad, extents, y_hi, y_lo, stream);
+}
+
+int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                        const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
+                                        double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
+                                        void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    const char* fn = "frcnn_preprocess_bgr8_canvas_im2col";
+    FRCNN_REQUIRE(arena, "%s: arena is NULL", fn);
+    FRCNN_REQUIRE(arena_bytes > 0, "%s: arena_bytes must be positive (got %lld)", fn, arena_bytes);
+    FRCNN_REQUIRE(src_off, "%s: src_off is NULL", fn);
+    FRCNN_REQUIRE(src_hw, "%s: src_hw is NULL", fn);
+    FRCNN_REQUIRE(inv_scale, "%s: inv_scale is NULL", fn);
+    FRCNN_REQUIRE(extents, "%s: extents is NULL", fn);
+    FRCNN_REQUIRE(y_hi, "%s: y_hi is NULL", fn);
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "%s: needs 1 <= N <= 65535 (got N=%d)", fn, N);
+    FRCNN_REQUIRE(Hc > 0 && Wc > 0, "%s: the canvas must be positive (got Hc=%d Wc=%d)", fn, Hc, Wc);
+    FRCNN_REQUIRE(ksize > 0 && ksize <= PRE_IM2COL_MAX_KSIZE, "%s: needs 1 <= ksize <= %d (got ksize=%d)", fn, PRE_IM2COL_MAX_KSIZE,
+                  ksize);
+    FRCNN_REQUIRE(stride > 0, "%s: stride must be positive (got stride=%d)", fn, stride);
+    FRCNN_REQUIRE(pad >= 0 && 2ll * pad + (Hc > Wc ? Hc : Wc) <= (1ll << 30),
+                  "%s: pad must be >= 0 with 2*pad + the canvas side <= 2^30 (got pad=%d)", fn, pad);
+    const int kmax = ksize * ksize * 3;
+    FRCNN_REQUIRE(K_pad % 8 == 0 && K_pad >= kmax && K_pad <= 65536,
+                  "%s: K_pad must be a multiple of 8 in [3*ksize^2 = %d, 65536] (got K_pad=%d)", fn, kmax, K_pad);
+    const int Ho = conv_out(Hc, ksize, stride, pad), Wo = conv_out(Wc, ksize, stride, pad);
+    FRCNN_REQUIRE(Ho > 0 && Wo > 0, "%s: canvas %dx%d smaller than the filter (ksize=%d pad=%d)", fn, Hc, Wc, ksize, pad);
+    PreIm2colArgs a;
+    a.arena = arena; a.arena_bytes = arena_bytes;
+    a.src_off = src_off; a.src_hw = src_hw; a.inv_scale = inv_scale; a.extents = extents;
+    a.Hc = Hc; a.Wc = Wc; a.ks = ksize; a.stride = stride; a.pad = pad; a.Kp = K_pad; a.Ho = Ho; a.Wo = Wo;
+    a.m0 = mean_b; a.m1 = mean_g; a.m2 = mean_r;
+    a.hi = (__nv_bfloat16*)y_hi; a.lo = (__nv_bfloat16*)y_lo;
+    // the tile: up to 8 output rows, then as many output columns as the window fits PRE_IM2COL_SMEM (the K table comes
+    // first); PRE_IM2COL_MAX_KSIZE guarantees one output pixel's window fits
+    const int px = (int)((PRE_IM2COL_SMEM - (size_t)kmax * 4) / 12);
+    a.band = Ho < 8 ? Ho : 8;
+    while (a.band > 1 && ((long)stride * (a.band - 1) + ksize) * ksize > px) --a.band;
+    const int rows = stride * (a.band - 1) + ksize;
+    const int k8n = K_pad / 8;
+    a.tile = (px / rows - ksize) / stride + 1;
+    a.tile = a.tile < Wo ? a.tile : Wo;
+    const int cap = (int)((0x7fffffffl / a.band) / k8n);         // band * tile * K_pad / 8 thread items stay an int
+    a.tile = a.tile < cap ? a.tile : (cap > 1 ? cap : 1);
+    a.cols = stride * (a.tile - 1) + ksize;
+    a.tiles = cdiv(Wo, a.tile);
+    const long blocks = (long)cdiv(Ho, a.band) * a.tiles;
+    FRCNN_REQUIRE(blocks <= 0x7fffffffl, "%s: canvas %dx%d needs too many tiles", fn, Hc, Wc);
+    const size_t smem = (size_t)kmax * 4 + (size_t)rows * a.cols * 12;
+    preprocess_bgr8_canvas_im2col_kernel<<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
 }
 
 int frcnn_pack_conv_weights_im2col(const float* w_oihw, const float* scale, int Cout, int Cin, int ksize, int K_pad, void* w_hi,

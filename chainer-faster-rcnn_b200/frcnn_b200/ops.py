@@ -256,13 +256,7 @@ def preprocess_pack_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc, p
     uint8 CUDA tensor holding image n's (h0,w0,3) pixels at byte src_off[n] (int64 [N]); src_hw: int32 [N, 2] (h0, w0), <= 0
     = empty slot; inv_scale: float64 [N] = 1 / im_scale; extents: int32 [N, 2] resized (H, W).  All of them device tensors
     read when the kernel runs."""
-    _need_cuda(arena, src_off, src_hw, inv_scale, extents)
-    N = int(extents.shape[0])
-    if arena.dtype != torch.uint8 or not arena.is_contiguous():
-        raise FrcnnError("preprocess_pack_canvas: arena must be a dense uint8 CUDA tensor")
-    for t, dt, what in ((src_off, torch.int64, "src_off"), (inv_scale, torch.float64, "inv_scale")):
-        if t.dtype != dt or tuple(t.shape) != (N,) or not t.is_contiguous():
-            raise FrcnnError("preprocess_pack_canvas: %s must be a dense %s [%d] CUDA tensor" % (what, dt, N))
+    N = _raw_descriptors("preprocess_pack_canvas", arena, src_off, src_hw, inv_scale, extents)
     lib = _lib.load()
     n = lib.frcnn_image_c8_elems(Hc, Wc)
     if out is None:
@@ -275,6 +269,40 @@ def preprocess_pack_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc, p
                                            _p(inv_scale), _per_image_pairs(extents, N, "extents"), N, int(Hc), int(Wc),
                                            float(m[0]), float(m[1]), float(m[2]), _p(out.hi), _p(out.lo), _stream()),
           "frcnn_preprocess_bgr8_canvas")
+    return out
+
+
+def _raw_descriptors(what, arena, src_off, src_hw, inv_scale, extents):
+    """The dtype / shape checks of a raw-photo canvas's arena and descriptors; returns the slot count N."""
+    _need_cuda(arena, src_off, src_hw, inv_scale, extents)
+    N = int(extents.shape[0])
+    if arena.dtype != torch.uint8 or not arena.is_contiguous():
+        raise FrcnnError("%s: arena must be a dense uint8 CUDA tensor" % what)
+    for t, dt, name in ((src_off, torch.int64, "src_off"), (inv_scale, torch.float64, "inv_scale")):
+        if t.dtype != dt or tuple(t.shape) != (N,) or not t.is_contiguous():
+            raise FrcnnError("%s: %s must be a dense %s [%d] CUDA tensor" % (what, name, dt, N))
+    return N
+
+
+def preprocess_im2col_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc, pixel_means, ksize, stride, pad, k_pad,
+                             precision="bf16x3", out=None):
+    """frcnn_preprocess_bgr8_canvas_im2col: raw uint8 BGR photos -> the first-layer im2col planes of an N-slot Hc x Wc canvas,
+    Act [N, Ho, Wo, k_pad] (pack_image_im2col_batch's layout), in one launch (resize + mean subtraction + im2col; 0 outside
+    every image's output extent).  The descriptors are preprocess_pack_canvas's, all device tensors read when the kernel
+    runs."""
+    N = _raw_descriptors("preprocess_im2col_canvas", arena, src_off, src_hw, inv_scale, extents)
+    Ho, Wo = (Hc + 2 * pad - ksize) // stride + 1, (Wc + 2 * pad - ksize) // stride + 1
+    if out is None:
+        hi = torch.empty((N, Ho, Wo, k_pad), dtype=torch.bfloat16, device=arena.device)
+        out = Act(hi, torch.empty_like(hi) if precision == "bf16x3" else None)
+    if tuple(out.hi.shape) != (N, Ho, Wo, k_pad) or (out.lo is not None and out.lo.shape != out.hi.shape):
+        raise FrcnnError("preprocess_im2col_canvas: output %s, expected %s" % (tuple(out.hi.shape), (N, Ho, Wo, k_pad)))
+    _dense_planes("preprocess_im2col_canvas", out)
+    m = np.asarray(pixel_means, dtype=np.float64).reshape(-1)
+    check(_lib.load().frcnn_preprocess_bgr8_canvas_im2col(
+        _p(arena), arena.numel(), _p(src_off), _per_image_pairs(src_hw, N, "src_hw"), _p(inv_scale),
+        _per_image_pairs(extents, N, "extents"), N, int(Hc), int(Wc), float(m[0]), float(m[1]), float(m[2]), int(ksize),
+        int(stride), int(pad), int(k_pad), _p(out.hi), _p(out.lo), _stream()), "frcnn_preprocess_bgr8_canvas_im2col")
     return out
 
 

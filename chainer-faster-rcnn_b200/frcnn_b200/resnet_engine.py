@@ -13,6 +13,11 @@ On the device every BatchNormalization (test mode) is folded into the preceding 
 convolution is the tcgen05 kernel of the VGG path (1x1 = plain GEMM tiles, 3x3 = shared-halo implicit GEMM), conv1 is an
 im2col GEMM (K = 147 -> 160), the residual add + ReLU is the epilogue of conv3 (frcnn_conv2d_res), and a stride-2 1x1
 convolution is frcnn_subsample2x (shared by conv1 and the projection shortcut) followed by a stride-1 GEMM.
+
+Engines: ResNetEngine runs one image at a time; ResNetBatchEngine adds same-size batches (ResNetBatchPlan) and canvases of
+images of different sizes (ResNetCanvasBatchPlan); ResNetPhotoEngine adds raw uint8 photos on a canvas
+(ResNetRawCanvasBatchPlan, whose first launch frcnn_preprocess_bgr8_canvas_im2col resizes the photos straight into conv1's
+im2col planes), so detect_images and engine.CanvasStreamRunner serve the ResNet detector as they serve VGG16.
 """
 import numpy as np
 import torch
@@ -132,12 +137,13 @@ class ResNetBatchPlan(BatchPlan):
     hwc_input (the 7x7 first layer reads dense (C,H,W) images) and keep_rpn_debug."""
     _trunk_name, _trunk_layer = "ResNet", "conv1"
     _alloc_trunk = ResNetForwardPlan._alloc_trunk      # activations through self._act: [N, ...] planes in a batch
+    _takes_raw_input = False                           # ResNetRawCanvasBatchPlan: raw photos on a canvas
 
     def __init__(self, weights, N, H, W, **options):
-        for opt, why in (("raw_input", "raw photos need the VGG16 trunk's first layer"),
+        for opt, why in (("raw_input", "raw photos need ResNetRawCanvasBatchPlan"),
                          ("hwc_input", "the 7x7 first layer reads dense (3,H,W) images"),
                          ("keep_rpn_debug", "no RPN debug outputs")):
-            if options.get(opt):
+            if options.get(opt) and not (opt == "raw_input" and self._takes_raw_input):
                 raise FrcnnError("%s: %s=True is not supported (%s)" % (type(self).__name__, opt, why))
         super(ResNetBatchPlan, self).__init__(weights, N, H, W, **options)
         # a canvas batch: the extents of conv1, pool1, res3, res4 and res5, derived on the device by the first launch
@@ -150,7 +156,7 @@ class ResNetBatchPlan(BatchPlan):
         if lv is not None:
             ops.resnet_level_extents(self.extents, self.H, self.W, out=lv)
             n += 1
-        ops.pack_image_im2col_batch(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col, extents=self.extents)
+        self._pack_input()
         hi, lo, b = cv["conv1"]
         ops.conv2d_batch(self.x_col, hi, lo, b, 1, True, out=self.c1, extents=ext(0))
         ops.maxpool3x3s2_ceil_batch(self.c1, out=self.p1, extents=ext(0))
@@ -180,6 +186,10 @@ class ResNetBatchPlan(BatchPlan):
             n += 3
         return self.blocks[-1]["out"], n
 
+    def _pack_input(self):
+        """The first launch after the level extents: the static float input -> conv1's im2col planes x_col."""
+        ops.pack_image_im2col_batch(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col, extents=self.extents)
+
     def _feature_extents(self):
         return (None if self.level_ext is None else self.level_ext[4]), 0
 
@@ -188,7 +198,27 @@ class ResNetCanvasBatchPlan(ResNetBatchPlan, CanvasBatchPlan):
     """CanvasBatchPlan with the ResNet trunk: N images of different sizes, each at the top-left of its Hc x Wc slot, in ONE
     captured graph.  The first launch derives every level's extents from the per-image sizes (frcnn_resnet_level_extents);
     each later launch reads its level's and writes 0 outside every image, so each image's results are bit-identical to a
-    ResNetForwardPlan's on that image alone.  Preprocessed float images only (no raw_input)."""
+    ResNetForwardPlan's on that image alone.  Preprocessed float images only: raw photos take ResNetRawCanvasBatchPlan."""
+
+
+class ResNetRawCanvasBatchPlan(ResNetCanvasBatchPlan):
+    """ResNetCanvasBatchPlan on RAW uint8 (h0,w0,3) BGR photos: CanvasBatchPlan(raw_input=True)'s static input (one device
+    block [descriptor header | pixels], forward_raw, raw_batch_header, fetch_result), with the ResNet trunk behind it.  After
+    the level extents, the first launch (frcnn_preprocess_bgr8_canvas_im2col) resizes every photo as forward.py does,
+    subtracts pixel_means and writes conv1's 7x7/2 im2col planes straight from the photos, so the plan holds no float32
+    images and one host-to-device copy of the block delivers a whole batch.  The launch count is the float canvas plan's.
+    Every image's results are bit-identical to a ResNetForwardPlan's on preprocess.img_preprocessing of that photo alone."""
+    _takes_raw_input = True
+
+    def __init__(self, weights, N, Hc, Wc, raw_input=True, **options):
+        if not raw_input:
+            raise FrcnnError("ResNetRawCanvasBatchPlan takes raw photos only (raw_input=False: use ResNetCanvasBatchPlan)")
+        super(ResNetRawCanvasBatchPlan, self).__init__(weights, N, Hc, Wc, raw_input=True, **options)
+
+    def _pack_input(self):
+        h = self._hdr
+        ops.preprocess_im2col_canvas(self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"], self.H, self.W,
+                                     self.pixel_means, 7, 2, 3, CONV1_KPAD, out=self.x_col)
 
 
 class ResNetEngine(Engine):
@@ -216,7 +246,8 @@ class ResNetBatchEngine(ResNetEngine):
     """ResNetEngine that also runs batches: batch_plan() is a ResNetBatchPlan and canvas_plan() a ResNetCanvasBatchPlan, so
     Engine.forward_batch (N same-size images) and Engine.forward_images (images of different sizes on a canvas) run N images
     per graph replay, each image bit-identical to ResNetForwardPlan on it.  Preprocessed float images only: detect_images
-    (raw photos) raises FrcnnError before anything is allocated.  ResNetEngine itself keeps running one image at a time."""
+    (raw photos) raises FrcnnError before anything is allocated; ResNetPhotoEngine takes raw photos.  ResNetEngine itself
+    keeps running one image at a time."""
 
     def batch_plan(self, N, H, W, **overrides):
         """The ResNetBatchPlan for N images of H x W (cached per shape and options)."""
@@ -225,6 +256,19 @@ class ResNetBatchEngine(ResNetEngine):
     def canvas_plan(self, N, Hc, Wc, **overrides):
         """The ResNetCanvasBatchPlan of N slots of Hc x Wc (cached per canvas and options)."""
         return self._cached("canvas", ResNetCanvasBatchPlan, (N, Hc, Wc), overrides)
+
+
+class ResNetPhotoEngine(ResNetBatchEngine):
+    """ResNetBatchEngine that also detects on raw photos: canvas_plan(..., raw_input=True) is a ResNetRawCanvasBatchPlan, so
+    Engine.raw_canvas_plan, Engine.detect_images (forward.py's detection lists from uint8 BGR photos of any sizes, N per
+    graph replay) and engine.CanvasStreamRunner work as they do for the VGG16 detector."""
+
+    def canvas_plan(self, N, Hc, Wc, **overrides):
+        """raw_input=True: the ResNetRawCanvasBatchPlan of N slots of Hc x Wc (cached under its own key); otherwise
+        ResNetBatchEngine.canvas_plan."""
+        if overrides.get("raw_input"):
+            return self._cached("raw_canvas", ResNetRawCanvasBatchPlan, (N, Hc, Wc), overrides)
+        return super(ResNetPhotoEngine, self).canvas_plan(N, Hc, Wc, **overrides)
 
 
 class TrunkOnly(object):

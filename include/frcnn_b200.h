@@ -560,6 +560,19 @@ int frcnn_conv2d_res_batch_ext(const void* x_hi, const void* x_lo, int N, int H,
  * each clamped to that level's canvas size (the same rules applied to Hc and Wc).  NULL pointers, N outside [1, 65535] or a
  * non-positive canvas -> FRCNN_ERR_ARG. */
 int frcnn_resnet_level_extents(const int* extents, int N, int Hc, int Wc, int* out, void* stream);
+/* Raw photos into the first-layer im2col planes of a ResNet canvas batch in ONE launch: frcnn_preprocess_bgr8, a copy into
+ * the top-left of a zeroed Hc x Wc slot and frcnn_pack_image_im2col_batch_ext for all N slots, without the float32 images
+ * in between.  The descriptors (arena, src_off, src_hw, inv_scale, extents) and the empty-slot rule are those of
+ * frcnn_preprocess_bgr8_canvas; ksize / stride / pad / K_pad those of frcnn_pack_image_im2col_batch_ext with C = 3.
+ * y_hi / y_lo (y_lo may be NULL) receive the whole [N][Ho][Wo][K_pad], Ho = (Hc + 2*pad - ksize) / stride + 1 (Wo alike):
+ * inside each image's conv_out(extent), bit for bit what those three steps write (a tap outside the resized image reads as
+ * the zero padding), and 0 at every other output pixel and at every k >= 3*ksize^2.  NULL pointers, N outside 1..65535, a
+ * non-positive canvas, ksize outside 1..45, stride < 1, pad < 0 or 2*pad + max(Hc, Wc) > 2^30, K_pad not a multiple of 8
+ * in [3*ksize^2, 65536] or a canvas smaller than the filter -> FRCNN_ERR_ARG. */
+int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                        const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
+                                        double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
+                                        void* y_hi, void* y_lo, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * RPN training targets and losses (SURVEY.md 8f rank 1, the train_rpn.py step).  Box arithmetic is
