@@ -382,7 +382,10 @@ class BatchPlan(_PlanBase):
         N = self.N = int(N)
         self._lead = (N,)
         dev, post_n = weights.device, self.post_n
-        self._alloc_input(dev)
+        # the static input that the first launch reads; extents / im_info: per-image device int32 [N, 2] sizes and clip
+        # bounds on a canvas, None when every image fills the H x W slot and (im_h, im_w) clips all of them
+        self.input = self._new_input(dev)
+        self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
         h, w_ = self.fh, self.fw = self._alloc_trunk(H, W)
         self.rpn_mid = self._act(h, w_, weights.rpn3[0].shape[1])
         self.rpn_out = torch.empty((N * h * w_, weights.rpn_ld), dtype=torch.float32, device=dev)
@@ -403,22 +406,14 @@ class BatchPlan(_PlanBase):
         self.head_out = torch.empty((N, self.ld1, weights.head_ld), dtype=torch.float32, device=dev)
         self.fc_work = max((ops.linear_batch_workspace(N, post_n, k_, c_, dev) for k_, c_ in
                             ((49 * C, 4096), (4096, 4096), (4096, 5 * weights.num_classes))), key=lambda t: t.numel())
-        # per-image device int32 [N, 2] extents (height, width) and clip bounds (im_h, im_w) of a canvas batch
-        # (CanvasBatchPlan); None: every image fills the H x W slot and (im_h, im_w) clips all of them
-        self.extents = self.im_info = None
 
-    def _alloc_input(self, dev):
-        """The static input that the first launch reads: (N,3,H,W) float32 images."""
-        self.x_in = torch.zeros((self.N, 3, self.H, self.W), dtype=torch.float32, device=dev)
-
-    def _pack_input(self):
-        """The first launch: the static input -> the compact first-layer planes acts[0]."""
-        ops.pack_image_c8_batch(self.x_in, out=self.acts[0], hwc_memory=self.hwc_input, extents=self.extents)
+    def _new_input(self, dev):
+        return ImageInput(self.N, self.H, self.W, dev, hwc_memory=self.hwc_input)
 
     def _run_trunk(self):
         """Launches the input stage and the trunk; returns (feature map Act, number of launches)."""
         w, N, ext = self.w, self.N, self.extents
-        self._pack_input()
+        self.input.pack_c8(self.acts[0])
         n = 1
         acts = iter(self.acts)
         x = next(acts)
@@ -505,12 +500,8 @@ class CanvasBatchPlan(BatchPlan):
     Every image's results are bit-identical to a ForwardPlan's on that image alone.  Takes ForwardPlan's keyword options
     except keep_rpn_debug (the debug rows would carry canvas anchor indices) and hwc_input.
 
-    raw_input=True: the plan takes RAW uint8 (h0,w0,3) BGR photos (forward_raw) instead of preprocessed float32 tensors.  Its
-    static input is one device block [descriptor header | pixels] (preprocess.raw_header_layout): the header holds every
-    slot's extents, clip bounds, source size, pixel offset and 1 / im_scale, the pixel area of arena_bytes (default: N
-    sources of up to Hc x Wc pixels) the photos themselves.  The first launch (frcnn_preprocess_bgr8_canvas) resizes,
-    subtracts pixel_means and packs all slots straight into the first-layer planes, so the plan holds no float32 images and
-    one host-to-device copy of that block delivers a whole batch."""
+    raw_input=True: the plan takes RAW uint8 (h0,w0,3) BGR photos (forward_raw) instead of preprocessed float32 tensors, in
+    a RawPhotoInput (pixel_means, arena_bytes): one host-to-device copy of its block delivers a whole batch."""
 
     def __init__(self, weights, N, Hc, Wc, raw_input=False, pixel_means=None, arena_bytes=None, **kw):
         if kw.get("keep_rpn_debug"):
@@ -518,46 +509,29 @@ class CanvasBatchPlan(BatchPlan):
         if kw.get("hwc_input"):
             raise FrcnnError("CanvasBatchPlan takes (3,H,W) images (hwc_input=True)")
         self.raw_input = bool(raw_input)
-        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
-                                                              dtype=np.float64).reshape(-1)[:3])
-        self.arena_bytes = int(N) * 3 * int(Hc) * int(Wc) if arena_bytes is None else int(arena_bytes)
-        if self.raw_input and self.arena_bytes < 1:
-            raise FrcnnError("CanvasBatchPlan: arena_bytes must be positive (got %d)" % self.arena_bytes)
+        self._raw_options = dict(pixel_means=pixel_means, arena_bytes=arena_bytes)
         super(CanvasBatchPlan, self).__init__(weights, N, Hc, Wc, **kw)
         if self.raw_input:
+            inp = self.input
+            self.block, self.arena, self.header_bytes = inp.block, inp.arena, inp.header_bytes
+            self.pixel_means, self.arena_bytes = inp.pixel_means, inp.arena_bytes
             self._ctor.update(raw_input=True, pixel_means=self.pixel_means, arena_bytes=self.arena_bytes)
-            self.extents, self.im_info = self._hdr["extents"], self._hdr["im_info"]
-        else:
-            # rows 0 / 1: extents and clip bounds, written with one upload per forward
-            self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=weights.device)
-            self.extents, self.im_info = self._sizes[0], self._sizes[1]
         self.image_sizes = [(0, 0)] * self.N
         self._res_host = None       # pinned mirror of the result blocks (fetch_result)
 
-    def _alloc_input(self, dev):
-        if not self.raw_input:
-            return super(CanvasBatchPlan, self)._alloc_input(dev)
-        layout, self.header_bytes = preprocess.raw_header_layout(self.N)
-        self.x_in = None
-        self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=dev)
-        self.arena = self.block[self.header_bytes:]
-        tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64}
-        self._hdr = {name: self.block[off:off + 8 * self.N].view(tdt[dt]).view((self.N, 2) if items == 2 else (self.N,))
-                     for name, (off, dt, items) in layout.items()}
-        self._stage = None          # pinned host mirror of the block + the event of its last upload (forward_raw)
+    def _new_input(self, dev):
+        if self.raw_input:
+            return RawPhotoInput(self.N, self.H, self.W, dev, **self._raw_options)
+        return ImageInput(self.N, self.H, self.W, dev, canvas=True)
 
-    def _pack_input(self):
-        if not self.raw_input:
-            return super(CanvasBatchPlan, self)._pack_input()
-        h = self._hdr
-        ops.preprocess_pack_canvas(self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"], self.H, self.W,
-                                   self.pixel_means, out=self.acts[0])
-
-    def raw_batch_header(self, shapes, img_infos=None):
-        """preprocess.raw_batch_header for this plan's slots, canvas and arena (raises FrcnnError when something does not fit)."""
+    def _raw(self):
         if not self.raw_input:
             raise FrcnnError("CanvasBatchPlan: raw photos need a plan built with raw_input=True")
-        return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
+        return self.input
+
+    def raw_batch_header(self, shapes, img_infos=None):
+        """RawPhotoInput.header of this plan's input."""
+        return self._raw().header(shapes, img_infos)
 
     def forward_raw(self, images, img_infos=None):
         """images: a list of at most N RAW uint8 (h0,w0,3) BGR photos of any sizes -- all numpy arrays (copied into a pinned
@@ -566,28 +540,7 @@ class CanvasBatchPlan(BatchPlan):
         img_infos: optional per-image clip bounds, default the resized (H_n, W_n); forward.py passes (H_n, H_n) (SURVEY.md
         Q7).  Raises FrcnnError before anything is queued if a resized image does not fit the canvas or the photos do not
         fit the arena.  Returns BatchPlan.forward's (list of prob, list of boxes, counts) and the list of im_scale."""
-        images = list(images)
-        on_host = all(isinstance(x, np.ndarray) for x in images)
-        if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
-            raise FrcnnError("forward_raw: the images must be all numpy arrays or all CUDA tensors")
-        for n, x in enumerate(images):
-            if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
-                raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
-        hdr, scales, _ = self.raw_batch_header([x.shape[:2] for x in images], img_infos)
-        cur = torch.cuda.current_stream()
-        if self._stage is None:
-            self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
-        pin, done = self._stage
-        done.synchronize()                    # the previous upload has left the pinned mirror
-        if on_host:
-            pin.h2d(self.block, cur, nbytes=preprocess.fill_raw_block(pin.np, hdr, images, self.N))
-        else:
-            pin.np[:hdr.size] = hdr
-            pin.h2d(self.block, cur, nbytes=self.header_bytes)
-            offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
-            for n, x in enumerate(images):
-                self.arena[int(offs[n]):int(offs[n]) + x.numel()].copy_(x.contiguous().view(-1), non_blocking=True)
-        done.record(cur)
+        hdr, scales = self._raw().upload(list(images), img_infos)
         self.image_sizes = [tuple(int(v) for v in e) for e in preprocess.raw_header_views(hdr, self.N)["extents"]]
         return self.forward(None) + (scales,)
 
@@ -609,22 +562,97 @@ class CanvasBatchPlan(BatchPlan):
         if images is not None:
             if self.raw_input:
                 raise FrcnnError("CanvasBatchPlan(raw_input=True) takes raw photos through forward_raw")
-            sizes = _fill_canvas(list(images), img_infos, self.x_in, self._sizes)
+            sizes = self.input.put(list(images), img_infos)
             self.image_sizes = [tuple(int(v) for v in e) for e in sizes[0]]
         return super(CanvasBatchPlan, self).forward(None)
 
 
-def _fill_canvas(images, img_infos, x_in, sizes_dev):
-    """Float (3,H_n,W_n) CUDA images into the top-left of the slots of the canvas x_in [N,3,Hc,Wc], and their extents and
-    clip bounds into sizes_dev [2,N,2] (preprocess.canvas_sizes, which raises first if they do not fit).  Returns the host
-    sizes array."""
-    N, _, Hc, Wc = x_in.shape
-    sizes = preprocess.canvas_sizes([tuple(x.shape) for x in images], N, Hc, Wc, img_infos)
-    for n, x in enumerate(images):
-        x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
-    # a pageable source: the copy is staged before copy_ returns, so `sizes` may go out of scope at once
-    sizes_dev.copy_(torch.from_numpy(sizes), non_blocking=True)
-    return sizes
+class ImageInput(object):
+    """Float32 images x_in [N,3,H,W] (hwc_memory: the bytes of (N,H,W,3) images), and on a canvas the int32 [2,N,2] `sizes`
+    whose rows `extents` and `im_info` are each slot's image size and clip bounds (None in a same-size batch).  pack_c8 /
+    pack_im2col: the first launch of the VGG16 / ResNet trunk, into the first layer's planes `out`."""
+
+    def __init__(self, N, H, W, device, canvas=False, hwc_memory=False):
+        self.x_in = torch.zeros((N, 3, H, W), dtype=torch.float32, device=device)
+        self.hwc_memory = bool(hwc_memory)
+        self.sizes = torch.zeros((2, N, 2), dtype=torch.int32, device=device) if canvas else None
+        self.extents, self.im_info = (None, None) if self.sizes is None else (self.sizes[0], self.sizes[1])
+
+    def put(self, images, img_infos=None):
+        """A list of float (3,H_n,W_n) CUDA images into the top-left of the canvas slots 0, 1, ..., and their extents and clip
+        bounds into `sizes` (preprocess.canvas_sizes, which raises first if they do not fit).  Returns the host sizes."""
+        N, _, Hc, Wc = self.x_in.shape
+        sizes = preprocess.canvas_sizes([tuple(x.shape) for x in images], N, Hc, Wc, img_infos)
+        for n, x in enumerate(images):
+            self.x_in[n, :, :x.shape[1], :x.shape[2]].copy_(x, non_blocking=True)
+        # a pageable source: the copy is staged before copy_ returns, so `sizes` may go out of scope at once
+        self.sizes.copy_(torch.from_numpy(sizes), non_blocking=True)
+        return sizes
+
+    def pack_c8(self, out):
+        ops.pack_image_c8_batch(self.x_in, out=out, hwc_memory=self.hwc_memory, extents=self.extents)
+
+    def pack_im2col(self, out, ksize, stride, pad, k_pad):
+        ops.pack_image_im2col_batch(self.x_in, ksize, stride, pad, k_pad, out=out, extents=self.extents)
+
+
+class RawPhotoInput(object):
+    """RAW uint8 (h0,w0,3) BGR photos on a canvas: one device block [header | pixels] (preprocess.raw_header_layout) whose
+    header holds each slot's extents, clip bounds, source size, pixel offset and 1 / im_scale, and whose `arena` of
+    arena_bytes (default: N sources of Hc x Wc) the photos.  pack_c8 / pack_im2col (frcnn_preprocess_bgr8_canvas[_im2col])
+    resize, subtract pixel_means and pack every slot straight into the first layer's planes: there is no x_in."""
+    x_in = None
+
+    def __init__(self, N, Hc, Wc, device, pixel_means=None, arena_bytes=None):
+        self.N, self.H, self.W = int(N), int(Hc), int(Wc)
+        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
+                                                              dtype=np.float64).reshape(-1)[:3])
+        self.arena_bytes = self.N * 3 * self.H * self.W if arena_bytes is None else int(arena_bytes)
+        if self.arena_bytes < 1:
+            raise FrcnnError("raw batch: arena_bytes must be positive (got %d)" % self.arena_bytes)
+        layout, self.header_bytes = preprocess.raw_header_layout(self.N)
+        self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=device)
+        self.arena = self.block[self.header_bytes:]
+        tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64}
+        h = {name: self.block[off:off + 8 * self.N].view(tdt[dt]).view((self.N, 2) if items == 2 else (self.N,))
+             for name, (off, dt, items) in layout.items()}
+        self.extents, self.im_info = h["extents"], h["im_info"]
+        # what both first-layer kernels read from the block
+        self.descriptors = (self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"])
+        self._stage = None          # pinned host mirror of the block + the event of its last upload
+
+    def header(self, shapes, img_infos=None):
+        """preprocess.raw_batch_header for these slots, canvas and arena (raises FrcnnError when something does not fit)."""
+        return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
+
+    def upload(self, images, img_infos=None):
+        """A list of photos into the block on the current stream, as CanvasBatchPlan.forward_raw describes.  Returns (host
+        header, [im_scale])."""
+        on_host = all(isinstance(x, np.ndarray) for x in images)
+        if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
+            raise FrcnnError("forward_raw: the images must be all numpy arrays or all CUDA tensors")
+        for n, x in enumerate(images):
+            if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
+                raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
+        hdr, scales, _ = self.header([x.shape[:2] for x in images], img_infos)
+        cur = torch.cuda.current_stream()
+        if self._stage is None:
+            self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
+        pin, done = self._stage
+        done.synchronize()                    # the previous upload has left the pinned mirror
+        pin.h2d(self.block, cur, nbytes=preprocess.fill_raw_block(pin.np, hdr, images if on_host else [], self.N))
+        if not on_host:
+            offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
+            for n, x in enumerate(images):
+                self.arena[int(offs[n]):int(offs[n]) + x.numel()].copy_(x.contiguous().view(-1), non_blocking=True)
+        done.record(cur)
+        return hdr, scales
+
+    def pack_c8(self, out):
+        ops.preprocess_pack_canvas(*self.descriptors, self.H, self.W, self.pixel_means, out=out)
+
+    def pack_im2col(self, out, ksize, stride, pad, k_pad):
+        ops.preprocess_im2col_canvas(*self.descriptors, self.H, self.W, self.pixel_means, ksize, stride, pad, k_pad, out=out)
 
 
 class LanePool(object):
@@ -1074,9 +1102,9 @@ class CCanvasForward(object):
     CanvasBatchPlan._run; this wrapper fills the C structs from a PackedWeights and owns the workspace, the static inputs and
     the outputs, so launch() can be captured into a CUDA graph and replayed for any mix of sizes.
 
-    raw_input=False: the input is (N,3,Hc,Wc) float32 images plus the int32 [N, 2] extents and clip bounds (forward).
-    raw_input=True: the input is the device block [header | pixels] of raw uint8 BGR photos (preprocess.raw_header_layout,
-    arena_bytes of pixels, default N sources of up to Hc x Wc) and the float64 [N] im_scale; the call also runs the per-class
+    raw_input=False: the input is an ImageInput canvas, (N,3,Hc,Wc) float32 images plus the int32 [N, 2] extents and clip
+    bounds (forward).  raw_input=True: the input is a RawPhotoInput, the device block [header | pixels] of raw uint8 BGR
+    photos (pixel_means, arena_bytes), and the float64 [N] im_scale; the call also runs the per-class
     NMS (det_nms_thresh, det_conf) and writes forward.py's detection lists into ONE int32 buffer `lists`
     [det_count (N, padded to 64 words) | dets [N][cap][5] | scores [N][cap] (float32)], cap = (NC-1) * post_n, so a host
     caller gets them with one device-to-host copy (detect_raw)."""
@@ -1091,8 +1119,6 @@ class CCanvasForward(object):
         self.w, self.N, self.H, self.W, self.post_n = weights, int(N), int(Hc), int(Wc), post_n
         self.raw_input = bool(raw_input)
         self.det_nms_thresh, self.det_conf = float(det_nms_thresh), float(det_conf)
-        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
-                                                              dtype=np.float64).reshape(-1)[:3])
         dev = weights.device
         self.anchors, self.cfg, self.wt = _c_structs(weights, self.H, self.W, anchors, pre_n, post_n, nms_thresh, min_size,
                                                      feat_stride)
@@ -1105,15 +1131,10 @@ class CCanvasForward(object):
         self.boxes = torch.zeros((self.N, post_n, 4 * NC), dtype=torch.float32, device=dev)
         self.count = torch.zeros((self.N,), dtype=torch.int32, device=dev)
         if not self.raw_input:
-            self.x_in = torch.zeros((self.N, 3, self.H, self.W), dtype=torch.float32, device=dev)
-            self._sizes = torch.zeros((2, self.N, 2), dtype=torch.int32, device=dev)     # rows: extents, clip bounds
-            self.extents, self.im_info = self._sizes[0], self._sizes[1]
+            self.input = ImageInput(self.N, self.H, self.W, dev, canvas=True)
             return
-        self.arena_bytes = self.N * 3 * self.H * self.W if arena_bytes is None else int(arena_bytes)
-        if self.arena_bytes < 1:
-            raise FrcnnError("CCanvasForward: arena_bytes must be positive (got %d)" % self.arena_bytes)
-        self.header_bytes = int(self._lib.frcnn_raw_header_bytes(self.N))
-        self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=dev)
+        inp = self.input = RawPhotoInput(self.N, self.H, self.W, dev, pixel_means, arena_bytes)
+        self.block, self.header_bytes, self.arena_bytes = inp.block, inp.header_bytes, inp.arena_bytes
         self.im_scale = torch.zeros((self.N,), dtype=torch.float64, device=dev)
         self.cap = (NC - 1) * post_n
         self.lists_layout = dict(det_count=0, dets=ops.round_up(self.N, 64), scores=ops.round_up(self.N, 64) + self.N * self.cap * 5)
@@ -1122,24 +1143,25 @@ class CCanvasForward(object):
         self.det_count = self.lists[:self.N]
         self.dets = self.lists[L["dets"]:L["scores"]].view(self.N, self.cap, 5)
         self.scores = self.lists[L["scores"]:].view(torch.float32).view(self.N, self.cap)
-        self._stage = None          # pinned mirrors of the block and of im_scale (stage_raw)
+        # pinned mirror of im_scale + the event of its last upload (stage_raw)
+        self._scale_stage = (ops.PinnedBlock((self.N,), np.float64), torch.cuda.Event())
         self._res_host = None       # pinned mirror of `lists` (fetch_detections)
 
     def launch(self):
         """Enqueue the C call on the current stream over the current contents of the static inputs (capturable)."""
         from . import _lib
-        ct, p = self._ct, lambda t: self._ct.c_void_p(t.data_ptr())          # noqa: E731
+        inp, ct, p = self.input, self._ct, lambda t: self._ct.c_void_p(t.data_ptr())          # noqa: E731
         st = ct.c_void_p(torch.cuda.current_stream().cuda_stream)
         if self.raw_input:
-            m = self.pixel_means
-            _lib.check(self._lib.frcnn_detect_vgg16_raw(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(self.block), self.arena_bytes,
+            m = inp.pixel_means
+            _lib.check(self._lib.frcnn_detect_vgg16_raw(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(inp.block), inp.arena_bytes,
                                                         m[0], m[1], m[2], p(self.im_scale), self.det_nms_thresh,
                                                         ct.c_float(self.det_conf), p(self.ws), self.ws.numel(), p(self.prob),
                                                         p(self.boxes), p(self.count), p(self.dets), p(self.scores),
                                                         p(self.det_count), st), "frcnn_detect_vgg16_raw")
         else:
-            _lib.check(self._lib.frcnn_forward_vgg16_canvas(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(self.x_in), p(self.extents),
-                                                            p(self.im_info), p(self.ws), self.ws.numel(), p(self.prob),
+            _lib.check(self._lib.frcnn_forward_vgg16_canvas(ct.byref(self.cfg), ct.byref(self.wt), self.N, p(inp.x_in), p(inp.extents),
+                                                            p(inp.im_info), p(self.ws), self.ws.numel(), p(self.prob),
                                                             p(self.boxes), p(self.count), st), "frcnn_forward_vgg16_canvas")
 
     def set_images(self, images, img_infos=None):
@@ -1147,7 +1169,7 @@ class CCanvasForward(object):
         0, 1, ...; the other slots are empty.  img_infos: optional per-image clip bounds (im_h, im_w), default (H_n, W_n)."""
         if self.raw_input:
             raise FrcnnError("CCanvasForward(raw_input=True) takes raw photos (stage_raw / detect_raw)")
-        _fill_canvas(list(images), img_infos, self.x_in, self._sizes)
+        self.input.put(list(images), img_infos)
 
     def forward(self, images, img_infos=None):
         """set_images + launch.  Returns (prob [N,post_n,NC], boxes [N,post_n,4NC], count [N]) device tensors; rows past an
@@ -1162,19 +1184,14 @@ class CCanvasForward(object):
         if not self.raw_input:
             raise FrcnnError("CCanvasForward: raw photos need raw_input=True")
         photos = list(photos)
-        hdr, scales, _ = preprocess.raw_batch_header(preprocess.raw_photo_shapes(photos), self.N, self.H, self.W, self.arena_bytes,
-                                                     img_infos)
+        preprocess.raw_photo_shapes(photos)             # numpy photos only
+        _, scales = self.input.upload(photos, img_infos)
         cur = torch.cuda.current_stream()
-        if self._stage is None:
-            self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), ops.PinnedBlock((self.N,), np.float64),
-                           torch.cuda.Event())
-        pin, pin_scale, done = self._stage
-        done.synchronize()                    # the previous upload has left the pinned mirrors
-        nbytes = preprocess.fill_raw_block(pin.np, hdr, photos, self.N)
-        pin_scale.np[:] = 0.0
-        pin_scale.np[:len(scales)] = scales
-        pin.h2d(self.block, cur, nbytes=nbytes)
-        pin_scale.h2d(self.im_scale, cur)
+        pin, done = self._scale_stage
+        done.synchronize()                    # the previous upload has left the pinned mirror
+        pin.np[:] = 0.0
+        pin.np[:len(scales)] = scales
+        pin.h2d(self.im_scale, cur)
         done.record(cur)
         return scales
 

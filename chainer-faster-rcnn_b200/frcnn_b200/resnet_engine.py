@@ -156,7 +156,7 @@ class ResNetBatchPlan(BatchPlan):
         if lv is not None:
             ops.resnet_level_extents(self.extents, self.H, self.W, out=lv)
             n += 1
-        self._pack_input()
+        self.input.pack_im2col(self.x_col, 7, 2, 3, CONV1_KPAD)
         hi, lo, b = cv["conv1"]
         ops.conv2d_batch(self.x_col, hi, lo, b, 1, True, out=self.c1, extents=ext(0))
         ops.maxpool3x3s2_ceil_batch(self.c1, out=self.p1, extents=ext(0))
@@ -186,10 +186,6 @@ class ResNetBatchPlan(BatchPlan):
             n += 3
         return self.blocks[-1]["out"], n
 
-    def _pack_input(self):
-        """The first launch after the level extents: the static float input -> conv1's im2col planes x_col."""
-        ops.pack_image_im2col_batch(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col, extents=self.extents)
-
     def _feature_extents(self):
         return (None if self.level_ext is None else self.level_ext[4]), 0
 
@@ -214,11 +210,6 @@ class ResNetRawCanvasBatchPlan(ResNetCanvasBatchPlan):
         if not raw_input:
             raise FrcnnError("ResNetRawCanvasBatchPlan takes raw photos only (raw_input=False: use ResNetCanvasBatchPlan)")
         super(ResNetRawCanvasBatchPlan, self).__init__(weights, N, Hc, Wc, raw_input=True, **options)
-
-    def _pack_input(self):
-        h = self._hdr
-        ops.preprocess_im2col_canvas(self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"], self.H, self.W,
-                                     self.pixel_means, 7, 2, 3, CONV1_KPAD, out=self.x_col)
 
 
 class ResNetEngine(Engine):

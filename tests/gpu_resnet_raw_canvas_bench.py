@@ -134,6 +134,9 @@ def main():
     fl = [torch.empty((3, H, W), device="cuda") for H, W in sizes]
     planes = ops.Act(torch.empty_like(plan.x_col.hi), torch.empty_like(plan.x_col.lo))
 
+    def fused():
+        plan.input.pack_im2col(plan.x_col, 7, 2, 3, CONV1_KPAD)
+
     def chain():
         for k in range(4):
             preprocess.img_preprocessing(dimg[k], out=fl[k])
@@ -144,13 +147,13 @@ def main():
         ops.pack_image_im2col_batch(x_in, 7, 2, 3, CONV1_KPAD, out=planes, extents=ext)
 
     reps, kern = 100, {"fused": [], "preprocess_copy_im2col": [], "im2col_only": []}
-    for fn in (plan._pack_input, chain):
+    for fn in (fused, chain):
         for _ in range(10):
             fn()
     assert torch.equal(planes.hi.view(torch.int16), plan.x_col.hi.view(torch.int16))
     assert torch.equal(planes.lo.view(torch.int16), plan.x_col.lo.view(torch.int16))
     for _ in range(args.rounds):
-        for name, fn in (("fused", plan._pack_input), ("preprocess_copy_im2col", chain), ("im2col_only", im2col)):
+        for name, fn in (("fused", fused), ("preprocess_copy_im2col", chain), ("im2col_only", im2col)):
             _, _, ms = timed(lambda: [fn() for _ in range(reps)])
             kern[name].append(1e3 * ms / reps)
     plane_bytes = plan.x_col.hi.numel() * 2 * 2                              # N slots, bf16, hi + lo

@@ -110,6 +110,36 @@ def test_raw_photo_shapes():
             preprocess.raw_photo_shapes([ok, bad])
 
 
+def test_input_buffers():
+    """The two static inputs on a CPU device: a float canvas's put() fills the slots and the [2, N, 2] sizes that extents /
+    im_info view; a raw input's header arrays are views into its block at raw_header_layout's offsets, with the default
+    arena and means, and a non-positive arena is refused."""
+    torch = pytest.importorskip("torch")
+    same = engine.ImageInput(2, 8, 12, "cpu", hwc_memory=True)
+    assert same.extents is None and same.im_info is None and same.hwc_memory and tuple(same.x_in.shape) == (2, 3, 8, 12)
+    canvas = engine.ImageInput(3, 8, 12, "cpu", canvas=True)
+    x = torch.arange(3 * 5 * 7, dtype=torch.float32).view(3, 5, 7)
+    assert canvas.put([x], img_infos=[(5, 5)]).tolist() == [[[5, 7], [0, 0], [0, 0]], [[5, 5], [0, 0], [0, 0]]]
+    assert canvas.extents.tolist() == [[5, 7], [0, 0], [0, 0]] and canvas.im_info.tolist() == [[5, 5], [0, 0], [0, 0]]
+    assert torch.equal(canvas.x_in[0, :, :5, :7], x) and canvas.x_in[0, :, 5:].abs().sum() == 0 and canvas.x_in[1:].abs().sum() == 0
+    raw = engine.RawPhotoInput(3, 600, 1000, "cpu")
+    layout, hb = preprocess.raw_header_layout(3)
+    assert raw.x_in is None and raw.header_bytes == hb and raw.arena_bytes == 3 * 3 * 600 * 1000
+    assert raw.block.numel() == hb + raw.arena_bytes and raw.arena.data_ptr() == raw.block.data_ptr() + hb
+    assert raw.pixel_means == tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS).reshape(-1))
+    hdr, _, _ = raw.header([(300, 500), (375, 500)], img_infos=[(600, 600), (600, 800)])
+    raw.block[:hb] = torch.from_numpy(hdr)
+    want = preprocess.raw_header_views(hdr, 3)
+    for name, t in zip(("arena", "src_off", "src_hw", "inv_scale", "extents"), raw.descriptors):
+        if name != "arena":
+            assert t.data_ptr() == raw.block.data_ptr() + layout[name][0] and np.array_equal(t.numpy(), want[name]), name
+    assert raw.extents.tolist() == [[600, 1000], [600, 800], [0, 0]] and raw.im_info.tolist() == [[600, 600], [600, 800], [0, 0]]
+    assert engine.RawPhotoInput(1, 8, 8, "cpu", pixel_means=np.array([[1, 2, 3]]), arena_bytes=64).pixel_means == (1.0, 2.0, 3.0)
+    for bad in (0, -5):
+        with pytest.raises(FrcnnError, match="arena_bytes"):
+            engine.RawPhotoInput(2, 8, 8, "cpu", arena_bytes=bad)
+
+
 class _StubPlan(object):
     """Records its constructor arguments; clone() makes another one."""
 
