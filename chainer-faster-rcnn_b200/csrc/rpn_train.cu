@@ -26,6 +26,27 @@ struct AnchorGeom {
     int A, H, W, stride, im_h, im_w;
 };
 
+// The anchors of N slots.  One image (extents == NULL): H x W is its feature map and (im_h, im_w) its clip bounds.  A canvas:
+// H x W is the canvas feature map, slot n's map is ceil(extents[n] / 2^halvings) (canvas_extent) and its clip bounds are
+// im_info[n].  Every per-slot anchor array is `cap` = A*H*W entries long, and anchor (y*fw_n + x)*A + a is numbered in the
+// slot's own frame, so a slot's arrays are those of its image alone.
+struct AnchorSlots {
+    AnchorGeom geo;
+    const int* extents; int halvings; const int* im_info;
+    long cap;
+};
+
+__device__ __forceinline__ AnchorGeom slot_geom(const AnchorSlots& s, int n) {
+    AnchorGeom g = s.geo;
+    if (s.extents != nullptr) {
+        g.H = canvas_extent(s.extents, n, 0, s.halvings, s.geo.H);
+        g.W = canvas_extent(s.extents, n, 1, s.halvings, s.geo.W);
+        g.im_h = __ldg(s.im_info + 2 * n);
+        g.im_w = __ldg(s.im_info + 2 * n + 1);
+    }
+    return g;
+}
+
 __device__ __forceinline__ bool anchor_box(const AnchorGeom& g, int i, double b[4]) {
     int a = i % g.A, k = i / g.A;
     double sx = (double)((k % g.W) * g.stride), sy = (double)((k / g.W) * g.stride);
@@ -51,12 +72,46 @@ __global__ void bbox_overlaps_kernel(const double* __restrict__ boxes, int N, co
 // ------------------------------------------------------------------------------------------ 1. overlaps: row max / arg-max, column max
 constexpr int GT_CHUNK = 256;
 
-__global__ void __launch_bounds__(256) anchor_overlap_kernel(AnchorGeom g, int n_all, const float* __restrict__ gt, int n_gt,
-                                                            double* __restrict__ max_ov, int* __restrict__ argmax,
-                                                            unsigned long long* __restrict__ gt_max_bits) {
+// Everything the three target kernels read and write, for N slots (blockIdx.y = slot).  Slot n's ground truth is
+// gt_counts[n] (clamped to max_gt; NULL: n_gt) rows at gt + n*max_gt*5; its arrays and workspace sit n*cap (n*max_gt for
+// gt_max, n*8 for counts) entries in.  A slot with no ground-truth row is empty, like one with a 0 x 0 extent.
+struct TargetArgs {
+    AnchorSlots s;
+    const float* gt; int max_gt; const int* gt_counts; int n_gt;
+    double* max_ov; int* argmax; unsigned long long* gt_max;
+    int* labels_full; float* targets_full; int* inds_inside; int* counts;
+};
+
+struct TargetSlot {
+    AnchorGeom g;
+    int n_all, n_gt;
+    const float* gt;
+    long base;                       // offset of the slot's anchor arrays
+};
+
+__device__ __forceinline__ TargetSlot target_slot(const TargetArgs& t, int n) {
+    TargetSlot r;
+    r.g = slot_geom(t.s, n);
+    r.n_gt = t.gt_counts != nullptr ? min(__ldg(t.gt_counts + n), t.max_gt) : t.n_gt;
+    if (r.n_gt < 1) r.g.H = r.g.W = 0;
+    r.n_all = r.g.A * r.g.H * r.g.W;
+    r.gt = t.gt + (size_t)n * t.max_gt * 5;
+    r.base = (long)n * t.s.cap;
+    return r;
+}
+
+__global__ void __launch_bounds__(256) anchor_overlap_kernel(TargetArgs ta) {
     __shared__ float s_gt[GT_CHUNK * 4];
     __shared__ double s_area[GT_CHUNK];
     __shared__ unsigned long long s_max[GT_CHUNK];
+    const TargetSlot sl = target_slot(ta, blockIdx.y);
+    if ((long)blockIdx.x * blockDim.x >= sl.n_all) return;             // whole block past the slot's anchors
+    const AnchorGeom g = sl.g;
+    const int n_all = sl.n_all, n_gt = sl.n_gt;
+    const float* __restrict__ gt = sl.gt;
+    double* __restrict__ max_ov = ta.max_ov + sl.base;
+    int* __restrict__ argmax = ta.argmax + sl.base;
+    unsigned long long* __restrict__ gt_max_bits = ta.gt_max + (size_t)blockIdx.y * ta.max_gt;
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     double b[4];
     bool inside = i < n_all && anchor_box(g, i, b);
@@ -92,13 +147,18 @@ __global__ void __launch_bounds__(256) anchor_overlap_kernel(AnchorGeom g, int n
 }
 
 // ------------------------------------------------------------------------------------------ 2. labels (before subsampling) + targets
-__global__ void __launch_bounds__(256) anchor_label_kernel(AnchorGeom g, int n_all, const float* __restrict__ gt, int n_gt,
-                                                          const double* __restrict__ max_ov, const int* __restrict__ argmax,
-                                                          const unsigned long long* __restrict__ gt_max_bits,
-                                                          double neg_thr, double pos_thr,
-                                                          int* __restrict__ labels_full, float* __restrict__ targets_full) {
+__global__ void __launch_bounds__(256) anchor_label_kernel(TargetArgs t, double neg_thr, double pos_thr) {
+    const TargetSlot sl = target_slot(t, blockIdx.y);
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_all) return;
+    if (i >= sl.n_all) return;
+    const AnchorGeom g = sl.g;
+    const int n_gt = sl.n_gt;
+    const float* __restrict__ gt = sl.gt;
+    const double* __restrict__ max_ov = t.max_ov + sl.base;
+    const int* __restrict__ argmax = t.argmax + sl.base;
+    const unsigned long long* __restrict__ gt_max_bits = t.gt_max + (size_t)blockIdx.y * t.max_gt;
+    int* __restrict__ labels_full = t.labels_full + sl.base;
+    float* __restrict__ targets_full = t.targets_full + 4 * sl.base;
     double b[4];
     bool inside = anchor_box(g, i, b);
     float4 tgt = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -216,12 +276,23 @@ __device__ void disable_smallest(int* labels, int n_all, int which, int n_dis, u
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(1024) anchor_subsample_kernel(AnchorGeom g, int n_all, int mode, unsigned long long seed,
-                                                               const int* __restrict__ disable_pos, int n_disable,
-                                                               int batch, int num_fg, int* __restrict__ labels_full,
-                                                               int* __restrict__ inds_inside, int* __restrict__ counts) {
+// Subsampling of one slot per CTA.  Mode 1 draws with seeds[n] (NULL: seed); mode 2 disables slot n's list
+// disable_pos[disable_offsets[n] .. disable_offsets[n+1]) (NULL offsets: the whole list), clamped to [0, n_disable).
+struct SubsampleArgs {
+    int mode; unsigned long long seed; const unsigned long long* seeds;
+    const int* disable_pos; int n_disable; const int* disable_offsets;
+    int batch, num_fg;
+};
+
+__global__ void __launch_bounds__(1024) anchor_subsample_kernel(TargetArgs t, SubsampleArgs sa) {
     __shared__ int s_warp[32];
     __shared__ int s_base;
+    const TargetSlot sl = target_slot(t, blockIdx.y);
+    const AnchorGeom g = sl.g;
+    const int n_all = sl.n_all, mode = sa.mode;
+    int* __restrict__ labels_full = t.labels_full + sl.base;
+    int* __restrict__ inds_inside = t.inds_inside + sl.base;
+    int* __restrict__ counts = t.counts + 8 * blockIdx.y;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_base = 0;
     __syncthreads();
@@ -255,6 +326,8 @@ __global__ void __launch_bounds__(1024) anchor_subsample_kernel(AnchorGeom g, in
     const int fg_before = block_sum(fg, s_warp), bg_before = block_sum(bg, s_warp);
     int fg_after = fg_before, bg_after = bg_before;
     if (mode == 1) {
+        const int batch = sa.batch, num_fg = sa.num_fg;
+        const unsigned long long seed = sa.seeds != nullptr ? sa.seeds[blockIdx.y] : sa.seed;
         // anchor_target_layer.py:148-168: at most num_fg positives, then at most batch - (#positives) negatives
         if (fg_before > num_fg) { disable_smallest(labels_full, n_all, 1, fg_before - num_fg, seed, s_warp); fg_after = num_fg; }
         int num_bg = batch - fg_after;
@@ -263,6 +336,14 @@ __global__ void __launch_bounds__(1024) anchor_subsample_kernel(AnchorGeom g, in
             bg_after = num_bg;
         }
     } else if (mode == 2) {
+        const int* disable_pos = sa.disable_pos;
+        int n_disable = sa.n_disable;
+        if (sa.disable_offsets != nullptr) {
+            const int lo = min(max(sa.disable_offsets[blockIdx.y], 0), sa.n_disable);
+            const int hi = min(max(sa.disable_offsets[blockIdx.y + 1], lo), sa.n_disable);
+            disable_pos += lo;
+            n_disable = hi - lo;
+        }
         __syncthreads();
         for (int t = threadIdx.x; t < n_disable; t += blockDim.x) {
             int p = disable_pos[t];
@@ -291,16 +372,42 @@ struct LossArgs {
     const int* labels_full; const float* targets_full; const int* counts;
     float* dscore; float* dbbox;
     double delta, lambda, grad_scale;
-    double* partials;        // [grid][4]: sum ce, sum huber, #correct, unused
+    double* partials;        // [N][gridDim.x][4]: sum ce, sum huber, #correct, unused
+    // canvas (s.extents != NULL): slot n's pixel (y, x) is row n*H*W + y*W + x of the score / bbox addressing, and when
+    // zero_ld > 0 the gradient is an NHWC matrix [N*H*W][zero_ld] whose every element outside the slots' anchor entries
+    // (other rows, columns >= 6A) is written as 0 by the same launch
+    int zero_ld;
 };
 
-__global__ void __launch_bounds__(256) rpn_loss_kernel(AnchorGeom g, int n_all, LossArgs p) {
+__device__ __forceinline__ AnchorGeom loss_slot(const AnchorSlots& s, const LossArgs& p, int n, int& n_all) {
+    AnchorGeom g = slot_geom(s, n);
+    if (s.extents != nullptr && p.counts[8 * n + 5] == 0) g.H = g.W = 0;      // a slot frcnn_anchor_targets_batch left empty
+    n_all = g.A * g.H * g.W;
+    return g;
+}
+
+__global__ void __launch_bounds__(256) rpn_loss_kernel(AnchorSlots s, LossArgs p) {
     __shared__ double s_red[8][3];
+    const int slot = blockIdx.y;
+    int n_all;
+    const AnchorGeom g = loss_slot(s, p, slot, n_all);
+    p.labels_full += (long)slot * s.cap;
+    p.targets_full += 4 * (long)slot * s.cap;
+    p.counts += 8 * slot;
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     double ce = 0.0, hub = 0.0, correct = 0.0;
+    if (p.zero_ld > 0) {
+        const long px = (long)s.geo.H * s.geo.W, total = px * p.zero_ld, c6 = 6l * g.A;
+        float* dst = p.dscore + slot * px * p.zero_ld;
+        for (long e = i; e < total; e += (long)gridDim.x * blockDim.x) {
+            const long r = e / p.zero_ld, c = e - r * p.zero_ld;
+            if (c >= c6 || r / s.geo.W >= g.H || r % s.geo.W >= g.W) dst[e] = 0.f;
+        }
+    }
     if (i < n_all) {
         const int a = i % g.A;
-        const long k = i / g.A;                                   // pixel index h*W + w
+        const int kk = i / g.A;                                   // pixel index h*W + w in the slot's own frame
+        const long k = (long)slot * s.geo.H * s.geo.W + (long)(kk / g.W) * s.geo.W + kk % g.W;
         double b[4];
         const bool inside = anchor_box(g, i, b);
         const int valid_n = max(p.counts[1] + p.counts[2], 1);     // softmax_cross_entropy normalize=True: 1/max(count,1)
@@ -349,13 +456,26 @@ __global__ void __launch_bounds__(256) rpn_loss_kernel(AnchorGeom g, int n_all, 
     if (threadIdx.x == 0) {
         double a0 = 0, a1 = 0, a2 = 0;
         for (int w = 0; w < 8; ++w) { a0 += s_red[w][0]; a1 += s_red[w][1]; a2 += s_red[w][2]; }
-        p.partials[blockIdx.x * 4 + 0] = a0; p.partials[blockIdx.x * 4 + 1] = a1; p.partials[blockIdx.x * 4 + 2] = a2;
+        double* part = p.partials + ((long)slot * gridDim.x + blockIdx.x) * 4;
+        part[0] = a0; part[1] = a1; part[2] = a2;
     }
 }
 
-__global__ void rpn_loss_finish_kernel(const double* __restrict__ partials, int n_blocks, const int* __restrict__ counts,
-                                       int n_all, double lambda, float* __restrict__ losses) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+// one CTA per slot: the slot's first cdiv(n_all, 256) block partials in order; an empty slot gets four zeros
+__global__ void rpn_loss_finish_kernel(AnchorSlots s, LossArgs p, int grid_x, float* __restrict__ losses) {
+    if (threadIdx.x != 0) return;
+    const int slot = blockIdx.x;
+    int n_all;
+    loss_slot(s, p, slot, n_all);
+    const double* partials = p.partials + (long)slot * grid_x * 4;
+    const int* counts = p.counts + 8 * slot;
+    const double lambda = p.lambda;
+    losses += 4 * slot;
+    if (n_all == 0) {
+        losses[0] = losses[1] = losses[2] = losses[3] = 0.f;
+        return;
+    }
+    const int n_blocks = (n_all + 255) / 256;
     double ce = 0, hub = 0, ok = 0;
     for (int b = 0; b < n_blocks; ++b) { ce += partials[b * 4]; hub += partials[b * 4 + 1]; ok += partials[b * 4 + 2]; }
     int valid = counts[1] + counts[2];
@@ -392,6 +512,34 @@ size_t frcnn_anchor_targets_workspace_bytes(int n_all, int n_gt) {
            align_up((size_t)(n_gt > 0 ? n_gt : 1) * sizeof(unsigned long long), 256);
 }
 
+size_t frcnn_anchor_targets_batch_workspace_bytes(int N, int n_cap, int max_gt) {
+    FRCNN_ENTRY();
+    if (N < 1 || n_cap < 0 || max_gt < 0) return 0;
+    const size_t n = (size_t)N * n_cap;
+    return align_up(n * sizeof(double), 256) + align_up(n * sizeof(int), 256) +
+           align_up((size_t)N * (max_gt > 0 ? max_gt : 1) * sizeof(unsigned long long), 256);
+}
+
+// overlaps, labels + targets, then one subsampling CTA per slot; the workspace holds max_ov [N*cap], argmax [N*cap] and
+// gt_max [N*max_gt]
+static int launch_targets(TargetArgs t, const SubsampleArgs& sa, int N, double neg_thr, double pos_thr, void* workspace,
+                          cudaStream_t st) {
+    const size_t n = (size_t)N * t.s.cap;
+    char* w = (char*)workspace;
+    t.max_ov = (double*)w;                      w += align_up(n * sizeof(double), 256);
+    t.argmax = (int*)w;                         w += align_up(n * sizeof(int), 256);
+    t.gt_max = (unsigned long long*)w;
+    FRCNN_CUDA_OK(cudaMemsetAsync(t.gt_max, 0, (size_t)N * t.max_gt * sizeof(unsigned long long), st));
+    const dim3 grid(cdiv((int)t.s.cap, 256), N);
+    anchor_overlap_kernel<<<grid, 256, 0, st>>>(t);
+    FRCNN_LAUNCH_OK();
+    anchor_label_kernel<<<grid, 256, 0, st>>>(t, neg_thr, pos_thr);
+    FRCNN_LAUNCH_OK();
+    anchor_subsample_kernel<<<dim3(1, N), 1024, 0, st>>>(t, sa);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
 int frcnn_anchor_targets(const double* anchors, int A, int feat_h, int feat_w, int feat_stride, const float* gt_boxes,
                          int n_gt, int im_h, int im_w, double neg_thr, double pos_thr, int batch, int num_fg,
                          int subsample_mode, unsigned long long seed, const int* disable_pos, int n_disable,
@@ -415,28 +563,75 @@ int frcnn_anchor_targets(const double* anchors, int A, int feat_h, int feat_w, i
         set_error("anchor_targets: workspace %zu < %zu bytes", workspace_bytes, frcnn_anchor_targets_workspace_bytes(n_all, n_gt));
         return FRCNN_ERR_WORKSPACE;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    char* w = (char*)workspace;
-    double* max_ov = (double*)w;                w += align_up((size_t)n_all * sizeof(double), 256);
-    int* argmax = (int*)w;                      w += align_up((size_t)n_all * sizeof(int), 256);
-    unsigned long long* gt_max = (unsigned long long*)w;
-    AnchorGeom g{anchors, A, feat_h, feat_w, feat_stride, im_h, im_w};
-    FRCNN_CUDA_OK(cudaMemsetAsync(gt_max, 0, (size_t)n_gt * sizeof(unsigned long long), st));
-    const int grid = cdiv(n_all, 256);
-    anchor_overlap_kernel<<<grid, 256, 0, st>>>(g, n_all, gt_boxes, n_gt, max_ov, argmax, gt_max);
-    FRCNN_LAUNCH_OK();
-    anchor_label_kernel<<<grid, 256, 0, st>>>(g, n_all, gt_boxes, n_gt, max_ov, argmax, gt_max, neg_thr, pos_thr, labels_full, targets_full);
-    FRCNN_LAUNCH_OK();
-    anchor_subsample_kernel<<<1, 1024, 0, st>>>(g, n_all, subsample_mode, seed, disable_pos, n_disable, batch, num_fg,
-                                                 labels_full, inds_inside, counts);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    TargetArgs t{};
+    t.s = AnchorSlots{AnchorGeom{anchors, A, feat_h, feat_w, feat_stride, im_h, im_w}, nullptr, 0, nullptr, n_all};
+    t.gt = gt_boxes; t.max_gt = n_gt; t.gt_counts = nullptr; t.n_gt = n_gt;
+    t.labels_full = labels_full; t.targets_full = targets_full; t.inds_inside = inds_inside; t.counts = counts;
+    const SubsampleArgs sa{subsample_mode, seed, nullptr, disable_pos, n_disable, nullptr, batch, num_fg};
+    return launch_targets(t, sa, 1, neg_thr, pos_thr, workspace, (cudaStream_t)stream);
+}
+
+int frcnn_anchor_targets_batch(const double* anchors, int A, int fhc, int fwc, int feat_stride, int N, const int* extents,
+                               int halvings, const int* im_info, const float* gt, int max_gt, const int* gt_counts, double neg_thr,
+                               double pos_thr, int batch, int num_fg, int subsample_mode, const unsigned long long* seeds,
+                               const int* disable_pos, int n_disable, const int* disable_offsets, int* labels_full,
+                               float* targets_full, int* inds_inside, int* counts, void* workspace, size_t workspace_bytes,
+                               void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "anchor_targets_batch: N = %d not in [1, 65535]", N);
+    FRCNN_REQUIRE(A > 0 && fhc > 0 && fwc > 0 && feat_stride > 0, "anchor_targets_batch: bad geometry A=%d H=%d W=%d", A, fhc, fwc);
+    FRCNN_REQUIRE(halvings >= 0 && halvings <= 30, "anchor_targets_batch: halvings must be in [0,30] (got %d)", halvings);
+    FRCNN_REQUIRE(max_gt >= 1, "anchor_targets_batch: max_gt must be at least 1 (got %d)", max_gt);
+    FRCNN_REQUIRE(extents && im_info && gt_counts, "anchor_targets_batch: null extents / im_info / gt_counts");
+    FRCNN_REQUIRE(anchors && gt && labels_full && targets_full && inds_inside && counts, "anchor_targets_batch: null pointer");
+    FRCNN_REQUIRE(subsample_mode >= 0 && subsample_mode <= 2, "anchor_targets_batch: subsample_mode %d not in {0,1,2}", subsample_mode);
+    FRCNN_REQUIRE(subsample_mode != 1 || seeds, "anchor_targets_batch: mode 1 without per-slot seeds");
+    FRCNN_REQUIRE(subsample_mode != 1 || (num_fg >= 0 && num_fg <= batch),
+                  "anchor_targets_batch: mode 1 needs 0 <= num_fg <= batch, got num_fg=%d batch=%d", num_fg, batch);
+    FRCNN_REQUIRE(subsample_mode != 2 || (disable_offsets && n_disable >= 0 && (n_disable == 0 || disable_pos)),
+                  "anchor_targets_batch: mode 2 needs the offsets [N+1] and an index list of n_disable >= 0 entries");
+    FRCNN_REQUIRE(aligned(targets_full, 16), "anchor_targets_batch: targets_full must be 16-byte aligned");
+    const long cap = (long)A * fhc * fwc;
+    FRCNN_REQUIRE(cap < (1l << 30) && (long)N * cap < (1l << 31) && (long)N * max_gt < (1l << 31),
+                  "anchor_targets_batch: too many anchors or ground-truth rows");
+    if (!workspace) {
+        set_error("anchor_targets_batch: no workspace");
+        return FRCNN_ERR_WORKSPACE;
+    }
+    const size_t need = frcnn_anchor_targets_batch_workspace_bytes(N, (int)cap, max_gt);
+    if (workspace_bytes < need) {
+        set_error("anchor_targets_batch: workspace %zu < %zu bytes", workspace_bytes, need);
+        return FRCNN_ERR_WORKSPACE;
+    }
+    TargetArgs t{};
+    t.s = AnchorSlots{AnchorGeom{anchors, A, fhc, fwc, feat_stride, 0, 0}, extents, halvings, im_info, cap};
+    t.gt = gt; t.max_gt = max_gt; t.gt_counts = gt_counts; t.n_gt = max_gt;
+    t.labels_full = labels_full; t.targets_full = targets_full; t.inds_inside = inds_inside; t.counts = counts;
+    const SubsampleArgs sa{subsample_mode, 0ull, subsample_mode == 1 ? seeds : nullptr, disable_pos, subsample_mode == 2 ? n_disable : 0,
+                           subsample_mode == 2 ? disable_offsets : nullptr, batch, num_fg};
+    return launch_targets(t, sa, N, neg_thr, pos_thr, workspace, (cudaStream_t)stream);
 }
 
 size_t frcnn_rpn_loss_workspace_bytes(int n_all) {
     FRCNN_ENTRY();
     if (n_all < 0) return 0;
     return (size_t)cdiv(n_all > 0 ? n_all : 1, 256) * 4 * sizeof(double);
+}
+
+size_t frcnn_rpn_loss_batch_workspace_bytes(int N, int n_cap) {
+    FRCNN_ENTRY();
+    if (N < 1 || n_cap < 0) return 0;
+    return (size_t)N * frcnn_rpn_loss_workspace_bytes(n_cap);
+}
+
+// the loss kernel over cdiv(cap, 256) x N blocks, then one finishing CTA per slot
+static int launch_loss(const AnchorSlots& s, const LossArgs& p, int N, float* losses, cudaStream_t st) {
+    const int grid_x = cdiv((int)(s.cap > 0 ? s.cap : 1), 256);
+    rpn_loss_kernel<<<dim3(grid_x, N), 256, 0, st>>>(s, p);
+    FRCNN_LAUNCH_OK();
+    rpn_loss_finish_kernel<<<N, 32, 0, st>>>(s, p, grid_x, losses);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
 }
 
 int frcnn_rpn_loss(const float* score, long score_cs, long score_ps, const float* bbox, long bbox_cs, long bbox_ps,
@@ -456,16 +651,39 @@ int frcnn_rpn_loss(const float* score, long score_cs, long score_ps, const float
         set_error("rpn_loss: workspace %zu < %zu bytes", workspace_bytes, frcnn_rpn_loss_workspace_bytes(n_all));
         return FRCNN_ERR_WORKSPACE;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    AnchorGeom g{anchors, A, feat_h, feat_w, feat_stride, im_h, im_w};
-    LossArgs p{score, score_cs, score_ps, bbox, bbox_cs, bbox_ps, labels_full, targets_full, counts, dscore, dbbox,
-               delta, loss_lambda, grad_scale, (double*)workspace};
-    const int grid = cdiv(n_all, 256);
-    rpn_loss_kernel<<<grid, 256, 0, st>>>(g, n_all, p);
-    FRCNN_LAUNCH_OK();
-    rpn_loss_finish_kernel<<<1, 32, 0, st>>>((const double*)workspace, grid, counts, n_all, loss_lambda, losses);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    const AnchorSlots s{AnchorGeom{anchors, A, feat_h, feat_w, feat_stride, im_h, im_w}, nullptr, 0, nullptr, n_all};
+    const LossArgs p{score, score_cs, score_ps, bbox, bbox_cs, bbox_ps, labels_full, targets_full, counts, dscore, dbbox,
+                     delta, loss_lambda, grad_scale, (double*)workspace, 0};
+    return launch_loss(s, p, 1, losses, (cudaStream_t)stream);
+}
+
+int frcnn_rpn_loss_batch(const float* head, int ld, const double* anchors, int A, int fhc, int fwc, int feat_stride, int N,
+                         const int* extents, int halvings, const int* im_info, const int* labels_full, const float* targets_full,
+                         const int* counts, double delta, double loss_lambda, double grad_scale, float* losses, float* dhead,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(N >= 1 && N <= 65535, "rpn_loss_batch: N = %d not in [1, 65535]", N);
+    FRCNN_REQUIRE(A > 0 && fhc > 0 && fwc > 0 && feat_stride > 0, "rpn_loss_batch: bad geometry A=%d H=%d W=%d", A, fhc, fwc);
+    FRCNN_REQUIRE(ld >= 6 * A, "rpn_loss_batch: ld = %d < 6A = %d", ld, 6 * A);
+    FRCNN_REQUIRE(halvings >= 0 && halvings <= 30, "rpn_loss_batch: halvings must be in [0,30] (got %d)", halvings);
+    FRCNN_REQUIRE(extents && im_info, "rpn_loss_batch: null extents / im_info");
+    FRCNN_REQUIRE(head && anchors && labels_full && targets_full && counts && losses, "rpn_loss_batch: null pointer");
+    FRCNN_REQUIRE(aligned(targets_full, 16), "rpn_loss_batch: targets_full must be 16-byte aligned");
+    FRCNN_REQUIRE(delta > 0, "rpn_loss_batch: delta must be positive");
+    const long cap = (long)A * fhc * fwc;
+    FRCNN_REQUIRE(cap < (1l << 30) && (long)N * fhc * fwc * ld < (1l << 40), "rpn_loss_batch: too many anchors");
+    if (!workspace) {
+        set_error("rpn_loss_batch: no workspace");
+        return FRCNN_ERR_WORKSPACE;
+    }
+    if (workspace_bytes < frcnn_rpn_loss_batch_workspace_bytes(N, (int)cap)) {
+        set_error("rpn_loss_batch: workspace %zu < %zu bytes", workspace_bytes, frcnn_rpn_loss_batch_workspace_bytes(N, (int)cap));
+        return FRCNN_ERR_WORKSPACE;
+    }
+    const AnchorSlots s{AnchorGeom{anchors, A, fhc, fwc, feat_stride, 0, 0}, extents, halvings, im_info, cap};
+    const LossArgs p{head, 1, ld, head + 2 * A, 1, ld, labels_full, targets_full, counts, dhead, dhead ? dhead + 2 * A : nullptr,
+                     delta, loss_lambda, grad_scale, (double*)workspace, dhead ? ld : 0};
+    return launch_loss(s, p, N, losses, (cudaStream_t)stream);
 }
 
 }  // extern "C"

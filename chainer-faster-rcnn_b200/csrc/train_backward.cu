@@ -29,7 +29,9 @@ struct PrepArgs {
     int H, W, C, Wp;
     long Kp;
     __nv_bfloat16 *o_hi, *o_lo;      // NHWC [H][W][C] out (optional)
-    __nv_bfloat16 *t_hi, *t_lo;      // transposed [planes][C][Kp] out (optional)
+    __nv_bfloat16 *t_hi, *t_lo;      // transposed [planes][C][t_ld] out (optional); image n's block at columns [n*Kp, (n+1)*Kp)
+    long t_ld;                       // N*Kp
+    int c_blocks;                    // blockIdx.z = image * c_blocks + 64-channel block
     int planes;                      // 1: plane at q; 3: planes shifted by -1/0/+1 pixel
     int times2;                      // multiply the result by 2 (the 1/(1-ratio) of a ratio-0.5 dropout), correctly rounded
 };
@@ -148,13 +150,33 @@ __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int 
 constexpr int PREP_PX = 256;
 constexpr int PREP_SMEM = (PREP_PX + 2) * 128 * 2;        // rows -1 .. 256, 128 B per plane
 
+// Image n of a batch: every NHWC pointer moves by one image, the transposed planes by one Kp block.
+__device__ __forceinline__ void prep_image(PrepArgs& a, int n) {
+    if (n == 0) return;
+    const long img = (long)a.H * a.W * a.C, pooled = (long)((a.H + 1) / 2) * ((a.W + 1) / 2) * a.C;
+    const long g_img = a.p_hi != nullptr ? pooled : img;
+    if (a.g_hi) a.g_hi += n * g_img;
+    if (a.g_lo) a.g_lo += n * g_img;
+    if (a.g_f32) a.g_f32 += n * (long)a.H * a.W * a.ld_f32;
+    if (a.y_hi) a.y_hi += n * img;
+    if (a.y_lo) a.y_lo += n * img;
+    if (a.p_hi) a.p_hi += n * pooled;
+    if (a.p_lo) a.p_lo += n * pooled;
+    if (a.o_hi) a.o_hi += n * img;
+    if (a.o_lo) a.o_lo += n * img;
+    if (a.t_hi) a.t_hi += n * a.Kp;
+    if (a.t_lo) a.t_lo += n * a.Kp;
+}
+
 template <int PLANES>
 __global__ void __launch_bounds__(256) grad_prepare_kernel(PrepArgs a) {
     extern __shared__ uint4 prep_smem[];
     uint4* s_hi = prep_smem;                                // [258][8] 16-byte units, unit column = c8 ^ ((row >> 3) & 7)
     uint4* s_lo = prep_smem + (PREP_PX + 2) * 8;
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    const int h = blockIdx.y, w0 = blockIdx.x * PREP_PX, c0 = blockIdx.z * 8;      // c0 in chunks
+    const int img = blockIdx.z / a.c_blocks;
+    prep_image(a, img);
+    const int h = blockIdx.y, w0 = blockIdx.x * PREP_PX, c0 = (blockIdx.z - img * a.c_blocks) * 8;      // c0 in chunks
     // ---- phase 1
     {
         const int c8l = t & 7, c8 = c0 + c8l;
@@ -213,7 +235,7 @@ __global__ void __launch_bounds__(256) grad_prepare_kernel(PrepArgs a) {
             vh.y = __byte_perm(hw[b0 + 2][m], hw[b0 + 3][m], sel);
             vh.z = __byte_perm(hw[b0 + 4][m], hw[b0 + 5][m], sel);
             vh.w = __byte_perm(hw[b0 + 6][m], hw[b0 + 7][m], sel);
-            const long row = ((long)pl * a.C + c8 * 8 + j) * a.Kp + k0;
+            const long row = ((long)pl * a.C + c8 * 8 + j) * a.t_ld + k0;
             *reinterpret_cast<uint4*>(a.t_hi + row) = vh;
             if (a.t_lo) {
                 vl.x = __byte_perm(lw[b0 + 0][m], lw[b0 + 1][m], sel);
@@ -335,6 +357,43 @@ static long padded_pixels(int H, int W, int* wp_out) {
     return (raw + 63) / 64 * 64;
 }
 
+static int grad_prepare(const char* fn, const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi,
+                        const void* y_lo, const void* p_hi, const void* p_lo, int N, int H, int W, int C, void* o_hi, void* o_lo,
+                        void* t_hi, void* t_lo, int planes, int times2, cudaStream_t stream) {
+    FRCNN_REQUIRE(N >= 1, "%s: N = %d < 1", fn, N);
+    FRCNN_REQUIRE(H > 0 && W > 0 && C > 0 && C % 8 == 0, "%s: bad shape H=%d W=%d C=%d (C %% 8 == 0)", fn, H, W, C);
+    FRCNN_REQUIRE((g_hi != nullptr) != (g_f32 != nullptr), "%s: give the source as bf16 planes OR fp32", fn);
+    FRCNN_REQUIRE(!g_f32 || (ld_f32 >= 1 && !p_hi), "%s: fp32 source needs ld_f32 and no pooling", fn);
+    FRCNN_REQUIRE(!p_hi || y_hi, "%s: pooled routing needs the un-pooled forward activation", fn);
+    FRCNN_REQUIRE(planes == 1 || planes == 3, "%s: planes must be 1 or 3", fn);
+    FRCNN_REQUIRE(o_hi || t_hi, "%s: no output requested", fn);
+    PrepArgs a;
+    a.g_hi = (const __nv_bfloat16*)g_hi; a.g_lo = (const __nv_bfloat16*)g_lo; a.g_f32 = g_f32; a.ld_f32 = ld_f32;
+    a.y_hi = (const __nv_bfloat16*)y_hi; a.y_lo = (const __nv_bfloat16*)y_lo;
+    a.p_hi = (const __nv_bfloat16*)p_hi; a.p_lo = (const __nv_bfloat16*)p_lo;
+    a.H = H; a.W = W; a.C = C;
+    a.Kp = padded_pixels(H, W, &a.Wp);
+    a.o_hi = (__nv_bfloat16*)o_hi; a.o_lo = (__nv_bfloat16*)o_lo; a.t_hi = (__nv_bfloat16*)t_hi; a.t_lo = (__nv_bfloat16*)t_lo;
+    a.t_ld = (long)N * a.Kp;
+    a.planes = planes;
+    a.times2 = times2 ? 1 : 0;
+    a.c_blocks = cdiv(C, 64);
+    FRCNN_REQUIRE(!times2 || !g_f32, "%s: times2 is not available for an fp32 source", fn);
+    const long gz = (long)N * a.c_blocks;
+    FRCNN_REQUIRE(H <= 65535 && gz <= 65535, "%s: image too tall / too many channels or images for one launch", fn);
+    dim3 grid(cdiv(W, 256), H, (unsigned)gz);
+    static bool attr_set = false;
+    if (!attr_set) {
+        FRCNN_CUDA_OK(cudaFuncSetAttribute(grad_prepare_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PREP_SMEM));
+        FRCNN_CUDA_OK(cudaFuncSetAttribute(grad_prepare_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, PREP_SMEM));
+        attr_set = true;
+    }
+    if (planes == 3) grad_prepare_kernel<3><<<grid, 256, PREP_SMEM, stream>>>(a);
+    else grad_prepare_kernel<1><<<grid, 256, PREP_SMEM, stream>>>(a);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
 extern "C" {
 
 long frcnn_padded_pixels(int H, int W, int* row_pitch) { return padded_pixels(H, W, row_pitch); }
@@ -343,34 +402,16 @@ int frcnn_grad_prepare(const void* g_hi, const void* g_lo, const float* g_f32, i
                        const void* p_hi, const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo,
                        int planes, int times2, void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(H > 0 && W > 0 && C > 0 && C % 8 == 0, "grad_prepare: bad shape H=%d W=%d C=%d (C %% 8 == 0)", H, W, C);
-    FRCNN_REQUIRE((g_hi != nullptr) != (g_f32 != nullptr), "grad_prepare: give the source as bf16 planes OR fp32");
-    FRCNN_REQUIRE(!g_f32 || (ld_f32 >= 1 && !p_hi), "grad_prepare: fp32 source needs ld_f32 and no pooling");
-    FRCNN_REQUIRE(!p_hi || y_hi, "grad_prepare: pooled routing needs the un-pooled forward activation");
-    FRCNN_REQUIRE(planes == 1 || planes == 3, "grad_prepare: planes must be 1 or 3");
-    FRCNN_REQUIRE(o_hi || t_hi, "grad_prepare: no output requested");
-    PrepArgs a;
-    a.g_hi = (const __nv_bfloat16*)g_hi; a.g_lo = (const __nv_bfloat16*)g_lo; a.g_f32 = g_f32; a.ld_f32 = ld_f32;
-    a.y_hi = (const __nv_bfloat16*)y_hi; a.y_lo = (const __nv_bfloat16*)y_lo;
-    a.p_hi = (const __nv_bfloat16*)p_hi; a.p_lo = (const __nv_bfloat16*)p_lo;
-    a.H = H; a.W = W; a.C = C;
-    a.Kp = padded_pixels(H, W, &a.Wp);
-    a.o_hi = (__nv_bfloat16*)o_hi; a.o_lo = (__nv_bfloat16*)o_lo; a.t_hi = (__nv_bfloat16*)t_hi; a.t_lo = (__nv_bfloat16*)t_lo;
-    a.planes = planes;
-    a.times2 = times2 ? 1 : 0;
-    FRCNN_REQUIRE(!times2 || !g_f32, "grad_prepare: times2 is not available for an fp32 source");
-    dim3 grid(cdiv(W, 256), H, cdiv(C, 64));
-    FRCNN_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "grad_prepare: image too tall / too many channels for one launch");
-    static bool attr_set = false;
-    if (!attr_set) {
-        FRCNN_CUDA_OK(cudaFuncSetAttribute(grad_prepare_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PREP_SMEM));
-        FRCNN_CUDA_OK(cudaFuncSetAttribute(grad_prepare_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, PREP_SMEM));
-        attr_set = true;
-    }
-    if (planes == 3) grad_prepare_kernel<3><<<grid, 256, PREP_SMEM, (cudaStream_t)stream>>>(a);
-    else grad_prepare_kernel<1><<<grid, 256, PREP_SMEM, (cudaStream_t)stream>>>(a);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return grad_prepare("grad_prepare", g_hi, g_lo, g_f32, ld_f32, y_hi, y_lo, p_hi, p_lo, 1, H, W, C, o_hi, o_lo, t_hi, t_lo,
+                        planes, times2, (cudaStream_t)stream);
+}
+
+int frcnn_grad_prepare_batch(const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi,
+                             const void* y_lo, const void* p_hi, const void* p_lo, int N, int H, int W, int C, void* o_hi,
+                             void* o_lo, void* t_hi, void* t_lo, int planes, int times2, void* stream) {
+    FRCNN_ENTRY();
+    return grad_prepare("grad_prepare_batch", g_hi, g_lo, g_f32, ld_f32, y_hi, y_lo, p_hi, p_lo, N, H, W, C, o_hi, o_lo, t_hi,
+                        t_lo, planes, times2, (cudaStream_t)stream);
 }
 
 int frcnn_wgrad_reduce(const float* parts, int groups, int splits, int M_parts, int M, int ld, int N, float scale, float* dw,

@@ -92,6 +92,16 @@ SIGNATURES = {
     "frcnn_rpn_loss": (c_int, [c_void_p, c_long, c_long, c_void_p, c_long, c_long, c_void_p, c_int, c_int, c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "frcnn_anchor_targets_batch_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "frcnn_anchor_targets_batch": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                           c_void_p, c_double, c_double, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "frcnn_rpn_loss_batch_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "frcnn_rpn_loss_batch": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_void_p, c_void_p, c_void_p,
+                                     c_size_t, c_void_p]),
+    "frcnn_grad_prepare_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                         c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "frcnn_gemm_nt_splitk_splits": (c_int, [c_int, c_int]),
     "frcnn_gemm_nt_splitk": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                      c_void_p, c_void_p, c_int, c_void_p]),

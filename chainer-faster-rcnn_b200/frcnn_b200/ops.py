@@ -64,16 +64,18 @@ def pack_image(x_chw, c_pad=16, precision="bf16x3"):
     return Act(hi, lo)
 
 
-def pack_conv_weights(w, cin_pad=None, precision="bf16x3", perm_chw=None):
-    """OIHW (or (Cout, K)) float32 weights -> ([taps, Cout, cin_pad] bf16 hi, lo or None)."""
+def pack_conv_weights(w, cin_pad=None, precision="bf16x3", perm_chw=None, out=None):
+    """OIHW (or (Cout, K)) float32 weights -> ([taps, Cout, cin_pad] bf16 hi, lo or None).  out: an earlier result of the
+    same shape to overwrite in place (a captured graph keeps reading it)."""
     _need_cuda(w)
     w = w.contiguous().float()
     if w.dim() == 2:
         w = w[:, :, None, None]
     Cout, Cin, kh, kw = w.shape
     cin_pad = cin_pad or round_up(Cin, 8)
-    hi = torch.empty((kh * kw, Cout, cin_pad), dtype=torch.bfloat16, device=w.device)
-    lo = torch.empty_like(hi) if precision == "bf16x3" else None
+    hi, lo = out if out is not None else (torch.empty((kh * kw, Cout, cin_pad), dtype=torch.bfloat16, device=w.device), None)
+    if out is None and precision == "bf16x3":
+        lo = torch.empty_like(hi)
     pc, ph, pw = perm_chw if perm_chw else (0, 0, 0)
     check(_lib.load().frcnn_pack_conv_weights(_p(w), Cout, Cin, kh, kw, cin_pad, _p(hi), _p(lo),
                                               1 if perm_chw else 0, pc, ph, pw, _stream()), "frcnn_pack_conv_weights")
@@ -139,22 +141,25 @@ def conv3x3_c8(x_c8, H, W, w_hi, w_lo, bias, relu=True, out=None):
     return out
 
 
-def pack_conv_weights_im2col(w, precision="bf16x3"):
-    """OIHW (Cout, Cin<=3, 3, 3) float32 -> ([1, Cout, 32] bf16 hi, lo or None), K order of pack_image_im2col."""
+def pack_conv_weights_im2col(w, precision="bf16x3", out=None):
+    """OIHW (Cout, Cin<=3, 3, 3) float32 -> ([1, Cout, 32] bf16 hi, lo or None), K order of pack_image_im2col.  out: an
+    earlier result to overwrite in place."""
     _need_cuda(w)
     w = w.contiguous().float()
     Cout, Cin, kh, kw = w.shape
     if (kh, kw) != (3, 3):
         raise FrcnnError("pack_conv_weights_im2col: 3x3 kernels only")
-    hi = torch.empty((1, Cout, 32), dtype=torch.bfloat16, device=w.device)
-    lo = torch.empty_like(hi) if precision == "bf16x3" else None
+    hi, lo = out if out is not None else (torch.empty((1, Cout, 32), dtype=torch.bfloat16, device=w.device), None)
+    if out is None and precision == "bf16x3":
+        lo = torch.empty_like(hi)
     check(_lib.load().frcnn_pack_conv_weights_im2col3x3(_p(w), Cout, Cin, _p(hi), _p(lo), _stream()),
           "frcnn_pack_conv_weights_im2col3x3")
     return hi, lo
 
 
-def pad_bias(b, n):
-    out = torch.zeros(round_up(max(n, b.numel()), 32), dtype=torch.float32, device=b.device)
+def pad_bias(b, n, out=None):
+    if out is None:
+        out = torch.zeros(round_up(max(n, b.numel()), 32), dtype=torch.float32, device=b.device)
     out[: b.numel()] = b.float()
     return out
 

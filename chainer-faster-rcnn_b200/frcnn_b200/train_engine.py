@@ -4,6 +4,7 @@ RpnTrainer -- one train_rpn.py step: forward (trunk + RPN) -> AnchorTargetLayer 
 heads, the RPN 3x3 conv and the 13 trunk convs -> [gradient all-reduce] -> WeightDecay + MomentumSGD.
 RcnnTrainer -- one train_rcnn.py step: trunk -> frozen test-mode RPN -> ProposalTargetLayer -> RoI pool -> fc6/fc7 with
 dropout -> head losses -> backward through the head, the RoI pooling and the trunk -> the same optimizer.
+CanvasRpnTrainer -- RpnTrainer's step on N images of different sizes per update (an N-slot canvas), one captured graph.
 
 Mirrors /root/reference train_rpn.py:144-179 with `model.rpn_train = True`: FasterRCNN.__call__ takes the RPN training
 branch (models/faster_rcnn.py:114-116 -> models/region_proposal_network.py:117-156), the optimizer is
@@ -22,7 +23,7 @@ import torch
 
 from . import ops, shard, train_ops
 from ._lib import FrcnnError
-from .engine import vgg16_schedule
+from .engine import ImageInput, vgg16_schedule
 
 ROIS_PER_IMAGE, FG_FRACTION = 128, 0.25                          # models/proposal_target_layer.py:49-50
 FG_THRESH, BG_THRESH_HI, BG_THRESH_LO = 0.5, 0.5, 0.1            # :46-48
@@ -36,7 +37,7 @@ class _ConvTrainer(object):
     their stored activations, weight (re)packing, the trunk forward, the generic conv-backward chain and the optimizer."""
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                     extra_layers, extra_params, load_transform=None):
+                     extra_layers, extra_params, load_transform=None, lead=()):
         if precision not in ops.PRECISIONS:
             raise FrcnnError("precision must be one of %s" % (ops.PRECISIONS,))
         self.x3 = precision == "bf16x3"
@@ -68,15 +69,16 @@ class _ConvTrainer(object):
             if load_transform is not None:
                 src = load_transform(n, src)
             self.w_flat[o:o + sz] = torch.from_numpy(np.ascontiguousarray(src).reshape(-1)).to(dev)
-        # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools)
+        # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools); `lead`: the
+        # leading [N] of a canvas trainer's activations
         x3 = self.x3
 
         def act(h, w, c):
-            hi = torch.empty((h, w, c), dtype=torch.bfloat16, device=dev)
+            hi = torch.empty(tuple(lead) + (h, w, c), dtype=torch.bfloat16, device=dev)
             return ops.Act(hi, torch.empty_like(hi) if x3 else None)
 
         self._act = act
-        self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)
+        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
         self.x_col = act(H, W, 32)
         h, w = H, W
         for L in self.layers[:13]:
@@ -254,7 +256,7 @@ class RpnTrainer(_ConvTrainer):
 
     def _wgrad(self, dyT, xT, M, N, groups, dw, m_out=None):
         """dw (flat view) = sum_pixels dY (x) X over the padded pixel axis; dyT: TBuf 1 plane [M_parts, Kp]; xT: TBuf."""
-        K = dyT.Kp
+        K = dyT.hi.shape[-1]                    # N*Kp: a canvas sums its N images in the one GEMM
         a_hi, a_lo = dyT.hi[0], (dyT.lo[0] if dyT.lo is not None else None)
         if groups == 9:
             b_hi, b_lo = xT.hi, xT.lo
@@ -603,3 +605,248 @@ class RcnnTrainer(RpnTrainer):
         self.update()
         return losses
 
+
+
+class CanvasRpnTrainer(RpnTrainer):
+    """The RPN-mode training step on N images of different sizes per update, with one set of weights and optimizer state.
+
+    Each image sits at the top-left of its slot of an N-slot Hc x Wc canvas (engine.ImageInput); its size and clip bounds
+    are device arrays that every launch reads at run time, so one trainer -- and one captured CUDA graph -- serves any mix
+    of sizes up to the canvas.  Forward and backward are RpnTrainer's chain over [N]-slabs: the *_batch_ext convolutions
+    (zero outside each image), frcnn_anchor_targets_batch / frcnn_rpn_loss_batch (slot n is normalised by its own counts
+    and anchor count, like the reference's per-device loss), frcnn_grad_prepare_batch and weight-gradient GEMMs over
+    K = N*Kp, so the gradient is the SUM of the N per-image gradients (ParallelUpdater's addgrads, train_rpn.py:169-174),
+    followed by one WeightDecay + MomentumSGD update.  Inside each image every activation, masked gradient and data
+    gradient equals RpnTrainer's on that image alone, bit for bit; with N = 1 and an image that fills the canvas the whole
+    step does.
+
+    subsample "device": slot n of step t draws with seed + t*N + n (a device counter advanced inside the step, so a replayed
+    graph draws fresh samples): the k-th image of a stream gets the labels RpnTrainer(seed=seed) gives its k-th image.
+    "list": put() takes per-image disable lists (positions in the inside-compact order, frcnn_anchor_targets mode 2).
+    "none": labels before subsampling."""
+
+    _MODES = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST, "none": train_ops.SUBSAMPLE_NONE}
+
+    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
+                 process_group=None):
+        if int(N) != N or N < 1:
+            raise FrcnnError("CanvasRpnTrainer needs N >= 1 slots (got %r)" % (N,))
+        if subsample not in self._MODES:
+            raise FrcnnError("CanvasRpnTrainer: subsample must be one of %s" % (sorted(self._MODES),))
+        if int(max_gt) < 1:
+            raise FrcnnError("CanvasRpnTrainer: max_gt must be at least 1")
+        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
+        A = len(anchors)
+        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
+        extra = [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], extra, lead=(N,))
+        dev = self.device
+        self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
+        self.n_heads = 6 * self.A
+        self.head_ld = ops.round_up(self.n_heads, 32)
+        self.input = ImageInput(N, Hc, Wc, dev, canvas=True)
+        self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
+        halvings = 0
+        for L in self.layers[:13]:                   # a layer's extents are ceil(extent / 2^halvings)
+            L["halvings"] = halvings
+            halvings += 1 if L["pool"] else 0
+        self.halvings = halvings
+        R = self.layers[13]
+        R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, halvings
+        R["y"] = self._act(self.fh, self.fw, 512)
+        rows = N * self.fh * self.fw
+        self.head_out = torch.empty((rows, self.head_ld), dtype=torch.float32, device=dev)
+        self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rpn_loss_batch
+        self.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, max_gt, dev)
+        self.gt = torch.zeros((N, max_gt, 5), dtype=torch.float32, device=dev)
+        self.gt_counts = torch.zeros((N,), dtype=torch.int32, device=dev)
+        self.seeds = torch.arange(N, dtype=torch.int64, device=dev) + int(seed)
+        self.disable_pos = torch.zeros((max(N * self.targets.cap, 1),), dtype=torch.int32, device=dev)
+        self.disable_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
+        self.image_sizes = [(0, 0)] * N
+        self.graph = None
+        self.repack()
+
+    # ---------------------------------------------------------------- buffers with the [N] lead
+    def _gact(self, h, w, c, tag=0):
+        key = (h, w, c, tag)
+        if key not in self._acts:
+            hi = torch.empty((self.N, h, w, c), dtype=torch.bfloat16, device=self.device)
+            self._acts[key] = ops.Act(hi, torch.empty_like(hi) if self.x3 else None)
+        return self._acts[key]
+
+    def _tbuf(self, planes, c, h, w, tag=0):
+        key = (planes, c, h, w, tag)
+        if key not in self._tbufs:
+            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3, N=self.N)
+        return self._tbufs[key]
+
+    def _chw(self, act):
+        """[N, C, H, W] float32 copy of an [N, H, W, C] Act (debug)."""
+        return torch.stack([ops.Act(act.hi[n], None if act.lo is None else act.lo[n]).to_chw_f32() for n in range(self.N)])
+
+    # ---------------------------------------------------------------- weights: repacked in place (a captured graph reads them)
+    def repack(self):
+        pr = self.precision
+        for i, L in enumerate(self.layers):
+            name = L["name"]
+            w, b = self.weights(name + "/W"), self.weights(name + "/b")
+            old = self.packed.get(name)
+            if i == 0:
+                fwd, dg = ops.pack_conv_weights_im2col(w, precision=pr, out=old and old[0]), None
+            else:
+                fwd = ops.pack_conv_weights(w, cin_pad=L["cin"], precision=pr, out=old and old[0])
+                dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=L["cout"], x3=self.x3, out=old and old[2])
+            self.packed[name] = (fwd, ops.pad_bias(b, L["cout"], out=old and old[1]), dg)
+        old = self.packed.get("heads")
+        wh, bh = self._heads_w(self.w_flat), self._heads_b(self.w_flat)
+        fwd = ops.pack_conv_weights(wh, precision=pr, out=old and old[0])
+        dg = train_ops.pack_conv_weights_dgrad(wh, cout_pad=self.head_ld, x3=self.x3, out=old and old[2])
+        self.packed["heads"] = (fwd, ops.pad_bias(bh, self.head_ld, out=old and old[1]), dg)
+
+    # ---------------------------------------------------------------- staging
+    def put(self, images, gt_boxes, img_infos=None, disable_pos=None):
+        """Stages up to N (3,H_n,W_n) float32 CUDA images, their [G_n,5] ground-truth boxes (1 <= G_n <= max_gt), optional
+        clip bounds (default (H_n, W_n)) and, in "list" mode, optional per-image disable lists into the static buffers
+        (the remaining slots are empty).  Raises FrcnnError before anything is queued when something does not fit."""
+        images, gt_boxes = list(images), list(gt_boxes)
+        if len(gt_boxes) != len(images):
+            raise FrcnnError("CanvasRpnTrainer.put: %d images and %d ground-truth lists" % (len(images), len(gt_boxes)))
+        for n, g in enumerate(gt_boxes):
+            if g.dim() != 2 or g.shape[1] != 5 or not 1 <= g.shape[0] <= self.max_gt:
+                raise FrcnnError("CanvasRpnTrainer.put: image %d has ground truth of shape %s, needs (G, 5) with 1 <= G <= %d"
+                                 % (n, tuple(g.shape), self.max_gt))
+        if disable_pos is not None:
+            disable_pos = list(disable_pos)
+            if self.subsample != "list":
+                raise FrcnnError("CanvasRpnTrainer.put: disable lists need subsample='list' (the trainer has %r)" % self.subsample)
+            if len(disable_pos) != len(images):
+                raise FrcnnError("CanvasRpnTrainer.put: %d images and %d disable lists" % (len(images), len(disable_pos)))
+            if any(int(d.numel()) > self.targets.cap for d in disable_pos):
+                raise FrcnnError("CanvasRpnTrainer.put: a disable list is longer than %d anchors" % self.targets.cap)
+        sizes = self.input.put(images, img_infos)          # raises before its first copy if an image does not fit
+        self.image_sizes = [tuple(int(v) for v in e) for e in sizes[0]]
+        counts = np.zeros((self.N,), dtype=np.int32)
+        for n, g in enumerate(gt_boxes):
+            counts[n] = g.shape[0]
+            self.gt[n, :g.shape[0]].copy_(g, non_blocking=True)
+        self.gt_counts.copy_(torch.from_numpy(counts), non_blocking=True)
+        if self.subsample == "list":
+            lens = np.zeros((self.N,), dtype=np.int64)
+            lens[:len(disable_pos or [])] = [int(d.numel()) for d in disable_pos or []]
+            offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+            for n, d in enumerate(disable_pos or []):
+                if lens[n]:
+                    self.disable_pos[offs[n]:offs[n + 1]].copy_(d.reshape(-1), non_blocking=True)
+            self.disable_offsets.copy_(torch.from_numpy(offs), non_blocking=True)
+
+    # ---------------------------------------------------------------- forward
+    def forward(self):
+        """Forward over the staged canvas, the anchor targets and the per-slot losses (float32 [N, 4] device buffer:
+        rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss; zeros for an empty slot)."""
+        ext = self.extents
+        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
+        x = self.x_col
+        for i, L in enumerate(self.layers[:13]):
+            (hi, lo), b, _ = self.packed[L["name"]]
+            ops.conv2d_batch(x, hi, lo, b, 1 if i == 0 else 3, True, out=L["y"], extents=ext, halvings=L["halvings"])
+            x = L["y"]
+            if L["pool"]:
+                ops.maxpool2x2_ceil_batch(L["y"], out=L["p"])
+                x = L["p"]
+        self.feat = x
+        R, k = self.layers[13], self.halvings
+        (hi, lo), b, _ = self.packed[R["name"]]
+        ops.conv2d_batch(x, hi, lo, b, 3, True, out=R["y"], extents=ext, halvings=k)
+        (hi, lo), b, _ = self.packed["heads"]
+        ops.conv2d_batch(R["y"], hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out, extents=ext,
+                         halvings=k)
+        mode = self._MODES[self.subsample]
+        train_ops.anchor_targets_batch(self.anchors, self.A, self.feat_stride, ext, self.im_info, self.gt, self.gt_counts,
+                                       self.targets, halvings=k, mode=mode, seeds=self.seeds, disable_pos=self.disable_pos,
+                                       disable_offsets=self.disable_offsets)
+        if mode == train_ops.SUBSAMPLE_DEVICE:
+            self.seeds.add_(self.N)
+        losses = train_ops.rpn_loss_batch(self.head_out, self.head_ld, self.anchors, self.A, self.feat_stride, ext, self.im_info,
+                                          self.targets, halvings=k, delta=self.delta, loss_lambda=self.loss_lambda,
+                                          dhead=self.head_grad)
+        self.last_losses = losses
+        return losses
+
+    # ---------------------------------------------------------------- backward
+    def backward(self, debug=None):
+        """Fills g_flat with the sum over the slots of d(rpn_loss_n)/d(parameter).  debug: as RpnTrainer.backward, every
+        tensor with a leading [N]."""
+        N, fh, fw, ld, ext = self.N, self.fh, self.fw, self.head_ld, self.extents
+        R = self.layers[13]
+        dyh = self._gact(fh, fw, ld)
+        dyhT = self._tbuf(1, ld, fh, fw)
+        train_ops.grad_prepare_batch(N, fh, fw, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
+        midT = self._tbuf(3, 512, fh, fw)
+        train_ops.grad_prepare_batch(N, fh, fw, 512, g=R["y"], tbuf=midT)
+        self._wgrad(dyhT, midT, ld, 512, 1, self._heads_w(self.g_flat), m_out=self.n_heads)
+        train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
+        _, _, (dhi, dlo) = self.packed["heads"]
+        g = self._gact(fh, fw, 512, tag=1)
+        ops.conv2d_batch(dyh, dhi, dlo, self.zero_bias, 1, False, out=g, extents=ext, halvings=self.halvings)
+        if debug is not None:
+            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
+        for L in [R] + self.layers[12::-1]:
+            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
+            first = L is self.layers[0]
+            dy = self._gact(h, w, co)
+            dyT = self._tbuf(1, co, h, w)
+            train_ops.grad_prepare_batch(N, h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
+            if debug is not None:
+                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
+            x = self._input_of(L)
+            if first:
+                xT = self._tbuf(1, 32, h, w)
+                train_ops.grad_prepare_batch(N, h, w, 32, g=x, tbuf=xT)
+                dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
+                self._wgrad(dyT, xT, co, 32, 1, dwc)
+                self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
+            else:
+                xT = self._tbuf(3, ci, h, w)
+                train_ops.grad_prepare_batch(N, h, w, ci, g=x, tbuf=xT)
+                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
+            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
+            self._early_exchange(L["name"])
+            if not first:
+                _, _, (dhi, dlo) = self.packed[L["name"]]
+                g = self._gact(h, w, ci, tag=1)
+                ops.conv2d_batch(dy, dhi, dlo, self.zero_bias, 3, False, out=g, extents=ext, halvings=L["halvings"])
+                if debug is not None:
+                    debug[L["name"]]["g_out"] = self._chw(g)
+
+    # ---------------------------------------------------------------- the step
+    def run(self):
+        """Enqueues forward + backward + update on the current stream, with no host synchronisation."""
+        self.forward()
+        self.backward()
+        self.update()
+
+    def step(self, images, gt_boxes, img_infos=None, disable_pos=None):
+        """put() + run().  In a single process the first call runs eagerly (which also sets up every kernel's lazy state)
+        and captures run() into a CUDA graph that every later call replays; with a process group of more than one rank
+        the step stays eager, so the gradient exchange is not captured.  Returns the per-slot losses, float32 [N, 4] on
+        the device."""
+        self.put(images, gt_boxes, img_infos, disable_pos)
+        if self._multi():
+            self.run()
+        elif self.graph is None:
+            self.run()
+            losses = self.targets.losses.clone()
+            torch.cuda.current_stream().synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                self.run()
+            self.n_updates -= 1                      # the capture ran nothing
+            self.graph = g
+            return losses
+        else:
+            self.graph.replay()
+            self.n_updates += 1
+        return self.targets.losses.clone()

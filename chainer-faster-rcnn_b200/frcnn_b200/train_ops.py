@@ -1,5 +1,5 @@
 """torch-tensor front end of the RPN-training entry points of the C ABI (include/frcnn_b200.h:
-frcnn_bbox_overlaps, frcnn_anchor_targets, frcnn_rpn_loss).  Like ops.py: device pointers + the current
+frcnn_bbox_overlaps, frcnn_anchor_targets, frcnn_rpn_loss and their canvas forms).  Like ops.py: device pointers + the current
 stream in, tensors out, no CPU path.
 
 Replaces models/bbox.pyx:16-56, models/anchor_target_layer.py:66-198 and the two loss functions of
@@ -112,6 +112,71 @@ def rpn_loss(score, bbox, anchors, A, H, W, feat_stride, im_h, im_w, work, delta
     return work.losses.clone(), ds, db          # a fresh tensor per call: the workspace buffer is overwritten by the next step
 
 
+class AnchorTargetsBatch(object):
+    """Device buffers of frcnn_anchor_targets_batch / frcnn_rpn_loss_batch for N slots of an H x W canvas feature map: slot
+    n's labels_full [n][cap] int32, targets_full [n][cap,4] float32, inds_inside [n][cap] int32, counts [n][8] int32 and
+    losses [n][4] float32, cap = A*H*W."""
+
+    def __init__(self, N, A, H, W, max_gt, device):
+        self.shape, self.N, self.max_gt = (A, H, W), int(N), int(max_gt)
+        self.cap = n = A * H * W
+        self.labels_full = torch.empty((N, n), dtype=torch.int32, device=device)
+        self.targets_full = torch.empty((N, n, 4), dtype=torch.float32, device=device)
+        self.inds_inside = torch.empty((N, n), dtype=torch.int32, device=device)
+        self.counts = torch.zeros((N, 8), dtype=torch.int32, device=device)
+        self.losses = torch.zeros((N, 4), dtype=torch.float32, device=device)
+        lib = _lib.load()
+        self.ws = torch.empty((lib.frcnn_anchor_targets_batch_workspace_bytes(N, n, max_gt),), dtype=torch.uint8, device=device)
+        self.loss_ws = torch.empty((lib.frcnn_rpn_loss_batch_workspace_bytes(N, n),), dtype=torch.uint8, device=device)
+
+
+def _slot_array(t, dtype, shape, what):
+    _need_cuda(t)
+    if t.dtype != dtype or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise FrcnnError("%s: expected a dense %s %s CUDA tensor, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape)))
+    return _p(t)
+
+
+def anchor_targets_batch(anchors, A, feat_stride, extents, im_info, gt, gt_counts, work, halvings=4, mode=SUBSAMPLE_DEVICE,
+                         seeds=None, disable_pos=None, disable_offsets=None, neg_thr=RPN_NEGATIVE_OVERLAP,
+                         pos_thr=RPN_POSITIVE_OVERLAP, batch=RPN_BATCHSIZE, num_fg=int(RPN_FG_FRACTION * RPN_BATCHSIZE)):
+    """frcnn_anchor_targets_batch into `work` (AnchorTargetsBatch).  extents / im_info int32 [N, 2]; gt float32
+    [N, max_gt, 5]; gt_counts int32 [N]; mode 1: seeds uint64 (torch.int64) [N]; mode 2: disable_pos int32 [n] and
+    disable_offsets int32 [N+1].  All device tensors, read when the kernels run."""
+    _need_cuda(anchors)
+    N, (_, H, W) = work.N, work.shape
+    args = [_slot_array(extents, torch.int32, (N, 2), "extents"), int(halvings), _slot_array(im_info, torch.int32, (N, 2), "im_info"),
+            _slot_array(gt, torch.float32, (N, work.max_gt, 5), "gt"), work.max_gt, _slot_array(gt_counts, torch.int32, (N,), "gt_counts")]
+    sp, dp, nd, do = None, None, 0, None
+    if mode == SUBSAMPLE_DEVICE:
+        sp = _slot_array(seeds, torch.int64, (N,), "seeds")
+    elif mode == SUBSAMPLE_LIST:
+        nd = int(disable_pos.numel())
+        dp = _slot_array(disable_pos, torch.int32, (nd,), "disable_pos") if nd else None
+        do = _slot_array(disable_offsets, torch.int32, (N + 1,), "disable_offsets")
+    check(_lib.load().frcnn_anchor_targets_batch(
+        _p(anchors), A, H, W, int(feat_stride), N, *args, float(neg_thr), float(pos_thr), int(batch), int(num_fg), int(mode), sp, dp,
+        nd, do, _p(work.labels_full), _p(work.targets_full), _p(work.inds_inside), _p(work.counts), _p(work.ws), work.ws.numel(),
+        _stream()), "frcnn_anchor_targets_batch")
+    return work
+
+
+def rpn_loss_batch(head, ld, anchors, A, feat_stride, extents, im_info, work, halvings=4, delta=3.0, loss_lambda=1.0,
+                   grad_scale=1.0, dhead=None):
+    """frcnn_rpn_loss_batch on the NHWC head matrix head [N*H*W, ld] float32; dhead (same shape, optional) receives the
+    gradient in every element.  Returns work.losses ([N, 4], overwritten by the next call)."""
+    N, (_, H, W) = work.N, work.shape
+    for t in (head, dhead):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != (N * H * W, ld)):
+            raise FrcnnError("rpn_loss_batch: head / dhead must be contiguous float32 [%d, %d]" % (N * H * W, ld))
+    check(_lib.load().frcnn_rpn_loss_batch(
+        _p(head), int(ld), _p(anchors), A, H, W, int(feat_stride), N, _slot_array(extents, torch.int32, (N, 2), "extents"),
+        int(halvings), _slot_array(im_info, torch.int32, (N, 2), "im_info"), _p(work.labels_full), _p(work.targets_full),
+        _p(work.counts), float(delta), float(loss_lambda), float(grad_scale), _p(work.losses), _p(dhead), _p(work.loss_ws),
+        work.loss_ws.numel(), _stream()), "frcnn_rpn_loss_batch")
+    return work.losses
+
+
 def split_bf16(x):
     """float32 CUDA tensor -> (hi, lo) bf16 planes with x ~= hi + lo (the kernels' "bf16x3" operand format)."""
     hi = x.to(torch.bfloat16)
@@ -161,12 +226,13 @@ def padded_pixels(H, W):
 
 
 class TBuf(object):
-    """Transposed padded planes [planes, C, Kp] bf16 hi (+ lo), zeroed once (the kernels write the interior only)."""
+    """Transposed padded planes [planes, C, N*Kp] bf16 hi (+ lo), zeroed once (the kernels write the interior only); image n
+    of a batch in columns [n*Kp, (n+1)*Kp)."""
 
-    def __init__(self, planes, C, H, W, device, x3=True):
+    def __init__(self, planes, C, H, W, device, x3=True, N=1):
         self.Kp, self.Wp = padded_pixels(H, W)
-        self.planes, self.C, self.H, self.W = planes, C, H, W
-        self.hi = torch.zeros((planes, C, self.Kp), dtype=torch.bfloat16, device=device)
+        self.planes, self.C, self.H, self.W, self.N = planes, C, H, W, N
+        self.hi = torch.zeros((planes, C, N * self.Kp), dtype=torch.bfloat16, device=device)
         self.lo = torch.zeros_like(self.hi) if x3 else None
 
 
@@ -184,6 +250,21 @@ def grad_prepare(H, W, C, g=None, g_f32=None, y=None, p=None, out=None, tbuf=Non
         tbuf.planes if tbuf is not None else 1, 1 if times2 else 0, _stream()), "frcnn_grad_prepare")
 
 
+def grad_prepare_batch(N, H, W, C, g=None, g_f32=None, y=None, p=None, out=None, tbuf=None, times2=False):
+    """frcnn_grad_prepare_batch: grad_prepare over N images; every Act is [N, ...], g_f32 [N*H*W, ld], tbuf a TBuf of N
+    blocks."""
+    if tbuf is not None and tbuf.N != N:
+        raise FrcnnError("grad_prepare_batch: the transposed buffer holds %d images, not %d" % (tbuf.N, N))
+    ld = int(g_f32.shape[1]) if g_f32 is not None else 0
+    check(_lib.load().frcnn_grad_prepare_batch(
+        _p(g.hi) if g is not None else None, _p(g.lo) if g is not None else None, _p(g_f32), ld,
+        _p(y.hi) if y is not None else None, _p(y.lo) if y is not None else None,
+        _p(p.hi) if p is not None else None, _p(p.lo) if p is not None else None, int(N), int(H), int(W), int(C),
+        _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
+        _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None,
+        tbuf.planes if tbuf is not None else 1, 1 if times2 else 0, _stream()), "frcnn_grad_prepare_batch")
+
+
 def wgrad_reduce(parts, M, N, dw, scale=1.0):
     """parts [groups, S, M_parts, ld] -> dw (flat fp32 view of M*N*groups elements, OIHW order)."""
     groups, S, Mp, ld = parts.shape
@@ -192,7 +273,9 @@ def wgrad_reduce(parts, M, N, dw, scale=1.0):
 
 
 def bias_grad(tbuf, C, db, scale=1.0):
-    check(_lib.load().frcnn_bias_grad(_p(tbuf.hi), _p(tbuf.lo), int(C), tbuf.Kp, float(scale), _p(db), _stream()), "frcnn_bias_grad")
+    """db = scale * the sum over all N*Kp columns of the transposed dY."""
+    check(_lib.load().frcnn_bias_grad(_p(tbuf.hi), _p(tbuf.lo), int(C), tbuf.N * tbuf.Kp, float(scale), _p(db), _stream()),
+          "frcnn_bias_grad")
 
 
 def sgd_momentum(w, v, g, lr, momentum, weight_decay):
@@ -210,15 +293,17 @@ def sgd_momentum_bf16g(w, v, g_bf16, lr, momentum, weight_decay):
                                                float(weight_decay), _stream()), "frcnn_sgd_momentum_bf16g")
 
 
-def pack_conv_weights_dgrad(w, cout_pad=None, x3=True):
-    """OIHW float32 CUDA weights -> ([taps, Cin, cout_pad] bf16 hi, lo or None): the filter of the data-gradient conv."""
+def pack_conv_weights_dgrad(w, cout_pad=None, x3=True, out=None):
+    """OIHW float32 CUDA weights -> ([taps, Cin, cout_pad] bf16 hi, lo or None): the filter of the data-gradient conv.
+    out: an earlier result to overwrite in place."""
     w = w.contiguous().float()
     if w.dim() == 2:
         w = w[:, :, None, None]
     Cout, Cin, kh, kw = w.shape
     cout_pad = cout_pad or (Cout + 7) // 8 * 8
-    hi = torch.empty((kh * kw, Cin, cout_pad), dtype=torch.bfloat16, device=w.device)
-    lo = torch.empty_like(hi) if x3 else None
+    hi, lo = out if out is not None else (torch.empty((kh * kw, Cin, cout_pad), dtype=torch.bfloat16, device=w.device), None)
+    if out is None and x3:
+        lo = torch.empty_like(hi)
     check(_lib.load().frcnn_pack_conv_weights_dgrad(_p(w), Cout, Cin, kh, kw, cout_pad, _p(hi), _p(lo), _stream()),
           "frcnn_pack_conv_weights_dgrad")
     return hi, lo

@@ -631,6 +631,40 @@ int frcnn_rpn_loss(const float* score, long score_cs, long score_ps, const float
                    double grad_scale, float* losses, float* dscore, float* dbbox, void* workspace, size_t workspace_bytes,
                    void* stream);
 
+/* frcnn_anchor_targets over the N slots of a canvas whose feature map is fhc x fwc (one launch per kernel, the slot is a
+ * grid dimension; frcnn_anchor_targets launches the same kernels with N = 1).
+ *   extents int32 [N][2]: each image's (height, width) in input pixels; its feature map is fh_n x fw_n =
+ *   ceil(extent / 2^halvings) (clamped to fhc x fwc; halvings = 4 for VGG16).  im_info int32 [N][2]: the clip bounds of
+ *   the inside test.  gt float32 [N][max_gt][5]: slot n's gt_counts[n] boxes (clamped to max_gt) in its first rows.
+ *   subsample_mode 0: none; 1: the rule of frcnn_anchor_targets with slot n's seed seeds[n] (uint64 device memory, read
+ *   when the kernel runs); 2: slot n disables the inside positions disable_pos[disable_offsets[n] .. disable_offsets[n+1])
+ *   (offsets int32 [N+1] device memory, clamped to [0, n_disable)).
+ * Outputs: slot n's labels_full / targets_full / inds_inside start at n*cap, cap = A*fhc*fwc, and its counts at 8n.
+ * Anchors are numbered in the image's own frame, (y*fw_n + x)*A + a, and the device-subsample key hashes that index, so
+ * slot n's first A*fh_n*fw_n entries (and its first counts[0] inside indices) equal what frcnn_anchor_targets returns for
+ * that image alone, bit for bit; entries past them are not written.  A slot with a 0 x 0 extent or gt_counts[n] < 1 is
+ * empty: its counts are all zero.  Workspace: frcnn_anchor_targets_batch_workspace_bytes(N, cap, max_gt). */
+size_t frcnn_anchor_targets_batch_workspace_bytes(int N, int n_cap, int max_gt);
+int frcnn_anchor_targets_batch(const double* anchors, int A, int fhc, int fwc, int feat_stride, int N, const int* extents,
+                               int halvings, const int* im_info, const float* gt, int max_gt, const int* gt_counts, double neg_thr,
+                               double pos_thr, int batch, int num_fg, int subsample_mode, const unsigned long long* seeds,
+                               const int* disable_pos, int n_disable, const int* disable_offsets, int* labels_full,
+                               float* targets_full, int* inds_inside, int* counts, void* workspace, size_t workspace_bytes,
+                               void* stream);
+
+/* frcnn_rpn_loss over the N slots of frcnn_anchor_targets_batch (same canvas, extents, halvings and im_info), on the NHWC
+ * head matrix head [N*fhc*fwc][ld] (slot n's pixel (y, x) in row n*fhc*fwc + y*fwc + x; scores in columns [0, 2A), deltas
+ * in [2A, 6A), ld >= 6A).  losses float32 [N][4] as frcnn_rpn_loss's.  dhead (optional) [N*fhc*fwc][ld]: EVERY element is
+ * written -- slot n's anchors get grad_scale * d(rpn_loss_n)/d(.), every other row and the columns >= 6A get 0 -- so it
+ * needs no zeroing.  Each slot is normalised by its own counts and its own A*fh_n*fw_n, like the reference's per-device
+ * loss: slot n's losses and gradient rows equal frcnn_rpn_loss on that image alone, bit for bit.  An empty slot (counts[5]
+ * == 0) gets zero losses and a zero gradient.  Workspace: frcnn_rpn_loss_batch_workspace_bytes(N, A*fhc*fwc). */
+size_t frcnn_rpn_loss_batch_workspace_bytes(int N, int n_cap);
+int frcnn_rpn_loss_batch(const float* head, int ld, const double* anchors, int A, int fhc, int fwc, int feat_stride, int N,
+                         const int* extents, int halvings, const int* im_info, const int* labels_full, const float* targets_full,
+                         const int* counts, double delta, double loss_lambda, double grad_scale, float* losses, float* dhead,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- RCNN-head training (rcnn_train.cu; train_rcnn.py, models/faster_rcnn.py:136-173) ---- */
 
 /* ProposalTargetLayer, part 1 (proposal_target_layer.py:91-96): best ground-truth overlap of every proposal, float64 in
@@ -710,6 +744,21 @@ long frcnn_padded_pixels(int H, int W, int* row_pitch);
 int frcnn_grad_prepare(const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi, const void* y_lo,
                        const void* p_hi, const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo,
                        int planes, int times2, void* stream);
+
+/* frcnn_grad_prepare over N images in one launch (frcnn_grad_prepare is this with N = 1): every NHWC source, mask and
+ * output is [N][H][W][C] (the pooled ones [N][ceil(H/2)][ceil(W/2)][C], the fp32 source [N*H*W][ld_f32]), and the
+ * transposed planes are [planes][C][N*Kp] with image n's padded block in columns [n*Kp, (n+1)*Kp).  Image n's results
+ * equal frcnn_grad_prepare on it, bit for bit.
+ * Each Kp block keeps its own zero halo (rows 0 and H+1, the 8 left columns, the columns past W, the tail past
+ * (H+2)*Wp), so frcnn_gemm_nt_splitk with K = N*Kp, unchanged, sums the weight gradient over the N images, the 9-tap
+ * groups included: an A column k is nonzero only at a pixel row 1..H of its block, and the B read at k +- Wp (and the
+ * +-1 pixel plane shift) then stays inside that block's halo.  This needs the buffer zeroed once, as for one image.
+ * On a canvas no extents are needed: every forward launch is an _ext entry, so each stored post-ReLU activation is exactly
+ * 0 outside its image and the ReLU mask zeroes every incoming gradient there -- including what the ceil-mode pool routes
+ * to a window element past an odd edge -- and the data-gradient convolutions are _ext launches too. */
+int frcnn_grad_prepare_batch(const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi,
+                             const void* y_lo, const void* p_hi, const void* p_lo, int N, int H, int W, int C, void* o_hi,
+                             void* o_lo, void* t_hi, void* t_lo, int planes, int times2, void* stream);
 
 /* dw[m][n][g] (the reference's OIHW float32, g = r*3+s or 1) = scale * sum over splits of parts[g][s][m][n], m < M;
  * parts slabs have M_parts >= M rows of ld floats. */
