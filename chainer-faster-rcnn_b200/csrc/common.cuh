@@ -156,4 +156,20 @@ __device__ __forceinline__ int canvas_extent(const int* extents, int img, int ax
     return (int)min(e, (long long)limit);
 }
 
+// The counter hash of device-side sampling (include/frcnn_b200.h, frcnn_anchor_targets mode 1): the anchor-target and
+// proposal-target subsampling and the dropout masks all draw through this one key, so their rules cannot drift apart.
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {       // splitmix64 finaliser
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+
+// key(seed, i): the top 32 bits hash (seed, i), the low 32 bits are i, so keys are distinct and a hash tie goes to the
+// lower index
+__device__ __forceinline__ unsigned long long sample_key(unsigned long long seed, int i) {
+    return (mix64(seed ^ ((unsigned long long)(unsigned)i * 0xD6E8FEB86659FD93ull)) & 0xFFFFFFFF00000000ull) | (unsigned)i;
+}
+constexpr unsigned long long BG_SEED_XOR = 0xA5A5A5A5DEADBEEFull;     // the negatives / background draw with seed ^ this
+
 }  // namespace frcnn

@@ -195,17 +195,7 @@ __global__ void __launch_bounds__(256) anchor_label_kernel(TargetArgs t, double 
 }
 
 // ------------------------------------------------------------------------------------------ 3. compaction + subsampling (one CTA)
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {       // splitmix64 finaliser
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
-
-__device__ __forceinline__ unsigned long long sample_key(unsigned long long seed, int i) {
-    return (mix64(seed ^ ((unsigned long long)(unsigned)i * 0xD6E8FEB86659FD93ull)) & 0xFFFFFFFF00000000ull) | (unsigned)i;
-}
-
+// (mix64 / sample_key: common.cuh)
 __device__ int block_sum(int v, int* s_warp) {           // all threads get the total; blockDim.x == 1024
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     __syncthreads();
@@ -332,7 +322,7 @@ __global__ void __launch_bounds__(1024) anchor_subsample_kernel(TargetArgs t, Su
         if (fg_before > num_fg) { disable_smallest(labels_full, n_all, 1, fg_before - num_fg, seed, s_warp); fg_after = num_fg; }
         int num_bg = batch - fg_after;
         if (bg_before > num_bg) {
-            disable_smallest(labels_full, n_all, 0, bg_before - num_bg, seed ^ 0xA5A5A5A5DEADBEEFull, s_warp);
+            disable_smallest(labels_full, n_all, 0, bg_before - num_bg, seed ^ BG_SEED_XOR, s_warp);
             bg_after = num_bg;
         }
     } else if (mode == 2) {

@@ -146,6 +146,16 @@ SIGNATURES = {
     "frcnn_roi_pool_backward_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "frcnn_roi_pool_backward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "frcnn_proposal_targets_batch": (c_int, [c_int, c_void_p, c_long, c_void_p, c_long, c_int, c_void_p, c_int, c_void_p, c_int,
+                                             c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_rcnn_loss_batch": (c_int, [c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double,
+                                      c_double, c_void_p, c_void_p, c_void_p]),
+    "frcnn_roi_pool_backward_batch_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "frcnn_roi_pool_backward_batch_ext": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_long,
+                                                  c_int, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p, c_size_t, c_void_p]),
+    "frcnn_dropout_masks_batch": (c_int, [c_int, c_int, c_int, c_void_p, ctypes.c_ulonglong, c_void_p, c_void_p]),
     "frcnn_forward_workspace_bytes": (c_size_t, [c_void_p]),
     "frcnn_forward_vgg16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),

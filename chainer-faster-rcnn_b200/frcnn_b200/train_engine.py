@@ -5,6 +5,7 @@ heads, the RPN 3x3 conv and the 13 trunk convs -> [gradient all-reduce] -> Weigh
 RcnnTrainer -- one train_rcnn.py step: trunk -> frozen test-mode RPN -> ProposalTargetLayer -> RoI pool -> fc6/fc7 with
 dropout -> head losses -> backward through the head, the RoI pooling and the trunk -> the same optimizer.
 CanvasRpnTrainer -- RpnTrainer's step on N images of different sizes per update (an N-slot canvas), one captured graph.
+CanvasRcnnTrainer -- RcnnTrainer's step on such a canvas, with device-side RoI sampling and dropout masks.
 
 Mirrors /root/reference train_rpn.py:144-179 with `model.rpn_train = True`: FasterRCNN.__call__ takes the RPN training
 branch (models/faster_rcnn.py:114-116 -> models/region_proposal_network.py:117-156), the optimizer is
@@ -403,6 +404,17 @@ class RpnTrainer(_ConvTrainer):
         return losses
 
 
+def _rcnn_params(nc):
+    """The head parameters of the RCNN step in flat-buffer order (cls_score | bbox_pred adjacent: one [5*nc, 4096] matrix)."""
+    heads = [("cls_score", nc), ("bbox_pred", 4 * nc)]
+    extra = [("fc6/W", (4096, 512 * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
+    return extra + [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
+
+
+def _fc6_to_hwc(name, a):                           # fc6 columns (c, h, w) -> (h, w, c), the order the RoI pooling emits
+    return a.reshape(4096, 512, 49).transpose(0, 2, 1) if name == "fc6/W" else a
+
+
 class RcnnTrainer(RpnTrainer):
     """One train_rcnn.py step (`model.rcnn_train = True`, /root/reference models/faster_rcnn.py:114-173): trunk -> RPN in TEST
     mode (its weights are frozen here: proposals are plain arrays, faster_rcnn.py:117-120) -> ProposalTargetLayer ->
@@ -419,14 +431,8 @@ class RcnnTrainer(RpnTrainer):
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
                  sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
         nc = self.num_classes = num_classes
-        heads = [("cls_score", nc), ("bbox_pred", 4 * nc)]
-        extra = [("fc6/W", (4096, 512 * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
-        extra += [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
-
-        def to_hwc(name, a):                         # fc6 columns (c, h, w) -> (h, w, c)
-            return a.reshape(4096, 512, 49).transpose(0, 2, 1) if name == "fc6/W" else a
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [], extra, load_transform=to_hwc)
+                          [], _rcnn_params(nc), load_transform=_fc6_to_hwc)
         self.delta, self.sample, self.dropout = delta, sample, dropout
         self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
         self.n_heads = 5 * nc
@@ -434,15 +440,7 @@ class RcnnTrainer(RpnTrainer):
         dev = self.device
         self.gen = torch.Generator(device=dev)
         self.gen.manual_seed(seed)
-        # frozen RPN (forward only)
-        T = lambda k: torch.from_numpy(np.ascontiguousarray(params[k], dtype=np.float32)).to(dev)
-        hi, lo = ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=512, precision=precision)
-        self.rpn3 = (hi, lo, ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
-        wh = torch.cat([T("RPN/rpn_cls_score/W"), T("RPN/rpn_bbox_pred/W")], dim=0)
-        bh = torch.cat([T("RPN/rpn_cls_score/b"), T("RPN/rpn_bbox_pred/b")], dim=0)
-        self.rpn_ld = ops.round_up(6 * self.A, 32)
-        hi, lo = ops.pack_conv_weights(wh, precision=precision)
-        self.rpn_heads = (hi, lo, ops.pad_bias(bh, self.rpn_ld))
+        self._frozen_rpn(params)
         fh, fw = self.fh, self.fw
         self.rpn_mid = self._act(fh, fw, 512)
         self.rpn_out = torch.empty((fh * fw, self.rpn_ld), dtype=torch.float32, device=dev)
@@ -455,6 +453,17 @@ class RcnnTrainer(RpnTrainer):
         self.dfeat = torch.empty((fh * fw, 512), dtype=torch.float32, device=dev)
         self.roi_ws = None
         self.repack()
+
+    def _frozen_rpn(self, params):
+        """The RPN's 3x3 and twin-head weights, packed once (forward only: the RCNN step gives them no gradient)."""
+        T = lambda k: torch.from_numpy(np.ascontiguousarray(params[k], dtype=np.float32)).to(self.device)     # noqa: E731
+        hi, lo = ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=512, precision=self.precision)
+        self.rpn3 = (hi, lo, ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
+        wh = torch.cat([T("RPN/rpn_cls_score/W"), T("RPN/rpn_bbox_pred/W")], dim=0)
+        bh = torch.cat([T("RPN/rpn_cls_score/b"), T("RPN/rpn_bbox_pred/b")], dim=0)
+        self.rpn_ld = ops.round_up(6 * self.A, 32)
+        hi, lo = ops.pack_conv_weights(wh, precision=self.precision)
+        self.rpn_heads = (hi, lo, ops.pad_bias(bh, self.rpn_ld))
 
     # ---------------------------------------------------------------- parameters
     def _heads_w(self, flat):
@@ -606,8 +615,168 @@ class RcnnTrainer(RpnTrainer):
         return losses
 
 
+class _CanvasSteps(object):
+    """The canvas machinery shared by CanvasRpnTrainer and CanvasRcnnTrainer: the N-slot image input with its device extents,
+    the staged ground truth, the [N]-lead gradient buffers, the in-place repack of the convolutions (a captured graph reads
+    the packed weights), the canvas trunk forward and backward, and the capture-then-replay step."""
 
-class CanvasRpnTrainer(RpnTrainer):
+    def _canvas_init(self, N, Hc, Wc, max_gt, seed):
+        dev = self.device
+        self.input = ImageInput(N, Hc, Wc, dev, canvas=True)
+        self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
+        halvings = 0
+        for L in self.layers[:13]:                   # a layer's extents are ceil(extent / 2^halvings)
+            L["halvings"] = halvings
+            halvings += 1 if L["pool"] else 0
+        self.halvings = halvings
+        self.gt = torch.zeros((N, max_gt, 5), dtype=torch.float32, device=dev)
+        self.gt_counts = torch.zeros((N,), dtype=torch.int32, device=dev)
+        self.seeds = torch.arange(N, dtype=torch.int64, device=dev) + int(seed)
+        self.image_sizes = [(0, 0)] * N
+        self.graph = None
+
+    # ---------------------------------------------------------------- buffers with the [N] lead
+    def _gact(self, h, w, c, tag=0):
+        key = (h, w, c, tag)
+        if key not in self._acts:
+            hi = torch.empty((self.N, h, w, c), dtype=torch.bfloat16, device=self.device)
+            self._acts[key] = ops.Act(hi, torch.empty_like(hi) if self.x3 else None)
+        return self._acts[key]
+
+    def _tbuf(self, planes, c, h, w, tag=0):
+        key = (planes, c, h, w, tag)
+        if key not in self._tbufs:
+            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3, N=self.N)
+        return self._tbufs[key]
+
+    def _chw(self, act):
+        """[N, C, H, W] float32 copy of an [N, H, W, C] Act (debug)."""
+        return torch.stack([ops.Act(act.hi[n], None if act.lo is None else act.lo[n]).to_chw_f32() for n in range(self.N)])
+
+    # ---------------------------------------------------------------- weights: repacked in place
+    def _repack(self, name, w, b, cout_pad, first=False, cin_pad=None):
+        pr, old = self.precision, self.packed.get(name)
+        if first:
+            fwd, dg = ops.pack_conv_weights_im2col(w, precision=pr, out=old and old[0]), None
+        else:
+            fwd = ops.pack_conv_weights(w, cin_pad=cin_pad, precision=pr, out=old and old[0])
+            dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=cout_pad, x3=self.x3, out=old and old[2])
+        self.packed[name] = (fwd, ops.pad_bias(b, cout_pad, out=old and old[1]), dg)
+
+    def _repack_convs(self):
+        for i, L in enumerate(self.layers):
+            name = L["name"]
+            self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
+
+    # ---------------------------------------------------------------- staging
+    def _check_gt(self, images, gt_boxes):
+        who = type(self).__name__
+        if len(gt_boxes) != len(images):
+            raise FrcnnError("%s.put: %d images and %d ground-truth lists" % (who, len(images), len(gt_boxes)))
+        for n, g in enumerate(gt_boxes):
+            if g.dim() != 2 or g.shape[1] != 5 or not 1 <= g.shape[0] <= self.max_gt:
+                raise FrcnnError("%s.put: image %d has ground truth of shape %s, needs (G, 5) with 1 <= G <= %d"
+                                 % (who, n, tuple(g.shape), self.max_gt))
+
+    def _stage(self, images, gt_boxes, img_infos):
+        """Images (ImageInput.put raises before its first copy if one does not fit) and ground truth into the static buffers."""
+        sizes = self.input.put(images, img_infos)
+        self.image_sizes = [tuple(int(v) for v in e) for e in sizes[0]]
+        counts = np.zeros((self.N,), dtype=np.int32)
+        for n, g in enumerate(gt_boxes):
+            counts[n] = g.shape[0]
+            self.gt[n, :g.shape[0]].copy_(g, non_blocking=True)
+        self.gt_counts.copy_(torch.from_numpy(counts), non_blocking=True)
+
+    @staticmethod
+    def _stage_lists(lists, N, buf, offsets):
+        """Per-image int32 lists into one flat device buffer + offsets [N+1] (slots without a list get an empty range)."""
+        lens = np.zeros((N,), dtype=np.int64)
+        lens[:len(lists or [])] = [int(d.numel()) for d in lists or []]
+        offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+        for n, d in enumerate(lists or []):
+            if lens[n]:
+                buf[offs[n]:offs[n + 1]].copy_(d.reshape(-1), non_blocking=True)
+        offsets.copy_(torch.from_numpy(offs), non_blocking=True)
+
+    # ---------------------------------------------------------------- trunk forward / backward over the canvas
+    def _canvas_trunk(self):
+        ext = self.extents
+        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
+        x = self.x_col
+        for i, L in enumerate(self.layers[:13]):
+            (hi, lo), b, _ = self.packed[L["name"]]
+            ops.conv2d_batch(x, hi, lo, b, 1 if i == 0 else 3, True, out=L["y"], extents=ext, halvings=L["halvings"])
+            x = L["y"]
+            if L["pool"]:
+                ops.maxpool2x2_ceil_batch(L["y"], out=L["p"])
+                x = L["p"]
+        self.feat = x
+        return x
+
+    def _canvas_chain(self, chain, g, debug=None):
+        """RpnTrainer._backward_chain over the canvas: grad_prepare_batch re-layouts, weight gradients over K = N*Kp (the sum
+        over the slots), data gradients through the _ext convolutions."""
+        N, ext = self.N, self.extents
+        for L in chain:
+            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
+            first = L is self.layers[0]
+            dy = self._gact(h, w, co)
+            dyT = self._tbuf(1, co, h, w)
+            train_ops.grad_prepare_batch(N, h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
+            if debug is not None:
+                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
+            x = self._input_of(L)
+            if first:
+                xT = self._tbuf(1, 32, h, w)
+                train_ops.grad_prepare_batch(N, h, w, 32, g=x, tbuf=xT)
+                dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
+                self._wgrad(dyT, xT, co, 32, 1, dwc)
+                self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
+            else:
+                xT = self._tbuf(3, ci, h, w)
+                train_ops.grad_prepare_batch(N, h, w, ci, g=x, tbuf=xT)
+                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
+            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
+            self._early_exchange(L["name"])
+            if not first:
+                _, _, (dhi, dlo) = self.packed[L["name"]]
+                g = self._gact(h, w, ci, tag=1)
+                ops.conv2d_batch(dy, dhi, dlo, self.zero_bias, 3, False, out=g, extents=ext, halvings=L["halvings"])
+                if debug is not None:
+                    debug[L["name"]]["g_out"] = self._chw(g)
+
+    # ---------------------------------------------------------------- the step
+    def run(self):
+        """Enqueues forward + backward + update on the current stream, with no host synchronisation."""
+        self.forward()
+        self.backward()
+        self.update()
+
+    def _step(self):
+        """run() on what put() staged.  In a single process the first call runs eagerly (which also sets up every kernel's
+        lazy state) and captures run() into a CUDA graph that every later call replays; with a process group of more than
+        one rank the step stays eager, so the gradient exchange is not captured.  Returns the per-slot losses, float32
+        [N, 4] on the device."""
+        if self._multi():
+            self.run()
+        elif self.graph is None:
+            self.run()
+            losses = self.step_losses.clone()
+            torch.cuda.current_stream().synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                self.run()
+            self.n_updates -= 1                      # the capture ran nothing
+            self.graph = g
+            return losses
+        else:
+            self.graph.replay()
+            self.n_updates += 1
+        return self.step_losses.clone()
+
+
+class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
     """The RPN-mode training step on N images of different sizes per update, with one set of weights and optimizer state.
 
     Each image sits at the top-left of its slot of an N-slot Hc x Wc canvas (engine.ImageInput); its size and clip bounds
@@ -646,65 +815,22 @@ class CanvasRpnTrainer(RpnTrainer):
         self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
         self.n_heads = 6 * self.A
         self.head_ld = ops.round_up(self.n_heads, 32)
-        self.input = ImageInput(N, Hc, Wc, dev, canvas=True)
-        self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
-        halvings = 0
-        for L in self.layers[:13]:                   # a layer's extents are ceil(extent / 2^halvings)
-            L["halvings"] = halvings
-            halvings += 1 if L["pool"] else 0
-        self.halvings = halvings
+        self._canvas_init(N, Hc, Wc, max_gt, seed)
         R = self.layers[13]
-        R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, halvings
+        R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, self.halvings
         R["y"] = self._act(self.fh, self.fw, 512)
         rows = N * self.fh * self.fw
         self.head_out = torch.empty((rows, self.head_ld), dtype=torch.float32, device=dev)
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rpn_loss_batch
         self.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, max_gt, dev)
-        self.gt = torch.zeros((N, max_gt, 5), dtype=torch.float32, device=dev)
-        self.gt_counts = torch.zeros((N,), dtype=torch.int32, device=dev)
-        self.seeds = torch.arange(N, dtype=torch.int64, device=dev) + int(seed)
+        self.step_losses = self.targets.losses
         self.disable_pos = torch.zeros((max(N * self.targets.cap, 1),), dtype=torch.int32, device=dev)
         self.disable_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
-        self.image_sizes = [(0, 0)] * N
-        self.graph = None
         self.repack()
 
-    # ---------------------------------------------------------------- buffers with the [N] lead
-    def _gact(self, h, w, c, tag=0):
-        key = (h, w, c, tag)
-        if key not in self._acts:
-            hi = torch.empty((self.N, h, w, c), dtype=torch.bfloat16, device=self.device)
-            self._acts[key] = ops.Act(hi, torch.empty_like(hi) if self.x3 else None)
-        return self._acts[key]
-
-    def _tbuf(self, planes, c, h, w, tag=0):
-        key = (planes, c, h, w, tag)
-        if key not in self._tbufs:
-            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3, N=self.N)
-        return self._tbufs[key]
-
-    def _chw(self, act):
-        """[N, C, H, W] float32 copy of an [N, H, W, C] Act (debug)."""
-        return torch.stack([ops.Act(act.hi[n], None if act.lo is None else act.lo[n]).to_chw_f32() for n in range(self.N)])
-
-    # ---------------------------------------------------------------- weights: repacked in place (a captured graph reads them)
     def repack(self):
-        pr = self.precision
-        for i, L in enumerate(self.layers):
-            name = L["name"]
-            w, b = self.weights(name + "/W"), self.weights(name + "/b")
-            old = self.packed.get(name)
-            if i == 0:
-                fwd, dg = ops.pack_conv_weights_im2col(w, precision=pr, out=old and old[0]), None
-            else:
-                fwd = ops.pack_conv_weights(w, cin_pad=L["cin"], precision=pr, out=old and old[0])
-                dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=L["cout"], x3=self.x3, out=old and old[2])
-            self.packed[name] = (fwd, ops.pad_bias(b, L["cout"], out=old and old[1]), dg)
-        old = self.packed.get("heads")
-        wh, bh = self._heads_w(self.w_flat), self._heads_b(self.w_flat)
-        fwd = ops.pack_conv_weights(wh, precision=pr, out=old and old[0])
-        dg = train_ops.pack_conv_weights_dgrad(wh, cout_pad=self.head_ld, x3=self.x3, out=old and old[2])
-        self.packed["heads"] = (fwd, ops.pad_bias(bh, self.head_ld, out=old and old[1]), dg)
+        self._repack_convs()
+        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- staging
     def put(self, images, gt_boxes, img_infos=None, disable_pos=None):
@@ -712,12 +838,7 @@ class CanvasRpnTrainer(RpnTrainer):
         clip bounds (default (H_n, W_n)) and, in "list" mode, optional per-image disable lists into the static buffers
         (the remaining slots are empty).  Raises FrcnnError before anything is queued when something does not fit."""
         images, gt_boxes = list(images), list(gt_boxes)
-        if len(gt_boxes) != len(images):
-            raise FrcnnError("CanvasRpnTrainer.put: %d images and %d ground-truth lists" % (len(images), len(gt_boxes)))
-        for n, g in enumerate(gt_boxes):
-            if g.dim() != 2 or g.shape[1] != 5 or not 1 <= g.shape[0] <= self.max_gt:
-                raise FrcnnError("CanvasRpnTrainer.put: image %d has ground truth of shape %s, needs (G, 5) with 1 <= G <= %d"
-                                 % (n, tuple(g.shape), self.max_gt))
+        self._check_gt(images, gt_boxes)
         if disable_pos is not None:
             disable_pos = list(disable_pos)
             if self.subsample != "list":
@@ -726,37 +847,16 @@ class CanvasRpnTrainer(RpnTrainer):
                 raise FrcnnError("CanvasRpnTrainer.put: %d images and %d disable lists" % (len(images), len(disable_pos)))
             if any(int(d.numel()) > self.targets.cap for d in disable_pos):
                 raise FrcnnError("CanvasRpnTrainer.put: a disable list is longer than %d anchors" % self.targets.cap)
-        sizes = self.input.put(images, img_infos)          # raises before its first copy if an image does not fit
-        self.image_sizes = [tuple(int(v) for v in e) for e in sizes[0]]
-        counts = np.zeros((self.N,), dtype=np.int32)
-        for n, g in enumerate(gt_boxes):
-            counts[n] = g.shape[0]
-            self.gt[n, :g.shape[0]].copy_(g, non_blocking=True)
-        self.gt_counts.copy_(torch.from_numpy(counts), non_blocking=True)
+        self._stage(images, gt_boxes, img_infos)
         if self.subsample == "list":
-            lens = np.zeros((self.N,), dtype=np.int64)
-            lens[:len(disable_pos or [])] = [int(d.numel()) for d in disable_pos or []]
-            offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-            for n, d in enumerate(disable_pos or []):
-                if lens[n]:
-                    self.disable_pos[offs[n]:offs[n + 1]].copy_(d.reshape(-1), non_blocking=True)
-            self.disable_offsets.copy_(torch.from_numpy(offs), non_blocking=True)
+            self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
 
     # ---------------------------------------------------------------- forward
     def forward(self):
         """Forward over the staged canvas, the anchor targets and the per-slot losses (float32 [N, 4] device buffer:
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss; zeros for an empty slot)."""
         ext = self.extents
-        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
-        x = self.x_col
-        for i, L in enumerate(self.layers[:13]):
-            (hi, lo), b, _ = self.packed[L["name"]]
-            ops.conv2d_batch(x, hi, lo, b, 1 if i == 0 else 3, True, out=L["y"], extents=ext, halvings=L["halvings"])
-            x = L["y"]
-            if L["pool"]:
-                ops.maxpool2x2_ceil_batch(L["y"], out=L["p"])
-                x = L["p"]
-        self.feat = x
+        x = self._canvas_trunk()
         R, k = self.layers[13], self.halvings
         (hi, lo), b, _ = self.packed[R["name"]]
         ops.conv2d_batch(x, hi, lo, b, 3, True, out=R["y"], extents=ext, halvings=k)
@@ -793,60 +893,224 @@ class CanvasRpnTrainer(RpnTrainer):
         ops.conv2d_batch(dyh, dhi, dlo, self.zero_bias, 1, False, out=g, extents=ext, halvings=self.halvings)
         if debug is not None:
             debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
-        for L in [R] + self.layers[12::-1]:
-            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
-            first = L is self.layers[0]
-            dy = self._gact(h, w, co)
-            dyT = self._tbuf(1, co, h, w)
-            train_ops.grad_prepare_batch(N, h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
-            if debug is not None:
-                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
-            x = self._input_of(L)
-            if first:
-                xT = self._tbuf(1, 32, h, w)
-                train_ops.grad_prepare_batch(N, h, w, 32, g=x, tbuf=xT)
-                dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
-                self._wgrad(dyT, xT, co, 32, 1, dwc)
-                self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
-            else:
-                xT = self._tbuf(3, ci, h, w)
-                train_ops.grad_prepare_batch(N, h, w, ci, g=x, tbuf=xT)
-                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
-            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
-            self._early_exchange(L["name"])
-            if not first:
-                _, _, (dhi, dlo) = self.packed[L["name"]]
-                g = self._gact(h, w, ci, tag=1)
-                ops.conv2d_batch(dy, dhi, dlo, self.zero_bias, 3, False, out=g, extents=ext, halvings=L["halvings"])
-                if debug is not None:
-                    debug[L["name"]]["g_out"] = self._chw(g)
-
-    # ---------------------------------------------------------------- the step
-    def run(self):
-        """Enqueues forward + backward + update on the current stream, with no host synchronisation."""
-        self.forward()
-        self.backward()
-        self.update()
+        self._canvas_chain([R] + self.layers[12::-1], g, debug)
 
     def step(self, images, gt_boxes, img_infos=None, disable_pos=None):
-        """put() + run().  In a single process the first call runs eagerly (which also sets up every kernel's lazy state)
-        and captures run() into a CUDA graph that every later call replays; with a process group of more than one rank
-        the step stays eager, so the gradient exchange is not captured.  Returns the per-slot losses, float32 [N, 4] on
-        the device."""
+        """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
+        losses, float32 [N, 4] on the device."""
         self.put(images, gt_boxes, img_infos, disable_pos)
-        if self._multi():
-            self.run()
-        elif self.graph is None:
-            self.run()
-            losses = self.targets.losses.clone()
-            torch.cuda.current_stream().synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                self.run()
-            self.n_updates -= 1                      # the capture ran nothing
-            self.graph = g
-            return losses
-        else:
-            self.graph.replay()
-            self.n_updates += 1
-        return self.targets.losses.clone()
+        return self._step()
+
+
+class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
+    """The RCNN-mode training step (RcnnTrainer's, train_rcnn.py) on N images of different sizes per update, with one set of
+    weights and optimizer state and one captured CUDA graph.
+
+    Forward: the canvas trunk, the frozen RPN (_ext convolutions + frcnn_proposals_batch_ext, whose per-slot proposal count
+    is written straight into column 1 of the [N][2] extents (1, R_n) of the head), frcnn_proposal_targets_batch,
+    frcnn_roi_pool_batch_ext, fc6 / fc7 / cls_score | bbox_pred as _ext convolutions over N x 1 x R_cap (rows >= R_n are 0,
+    as RcnnTrainer's m_valid leaves them), dropout, frcnn_rcnn_loss_batch (slot n normalised by its own kept count).
+    Backward: the head and fc layers through frcnn_grad_prepare_batch with weight GEMMs over K = N*Kp,
+    frcnn_roi_pool_backward_batch_ext, then the trunk; one WeightDecay + MomentumSGD update on the summed gradient.
+    Inside each image every activation and data gradient equals RcnnTrainer's on that image with the same kept rows and
+    masks, bit for bit.
+
+    sample "device": slot n of step t samples with seed + t*N + n (frcnn_proposal_targets_batch mode 1, a device counter
+    advanced inside the step); "list": put() takes per-image kept lists (RcnnTrainer's keep_inds, at most 128 distinct rows).
+    dropout "device": masks drawn by frcnn_dropout_masks_batch from the same per-slot seeds (salt 1: fc6, 2: fc7); "explicit":
+    put() takes per-image (fc6, fc7) uint8 [post_n, 4096] masks; None: no dropout.  `masks` [2, N, post_n, 4096] holds the
+    masks the last step used."""
+
+    _SAMPLE = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST}
+    _DROPOUT = ("device", "explicit", None)
+
+    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
+                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None):
+        if int(N) != N or N < 1:
+            raise FrcnnError("CanvasRcnnTrainer needs N >= 1 slots (got %r)" % (N,))
+        if sample not in self._SAMPLE:
+            raise FrcnnError("CanvasRcnnTrainer: sample must be one of %s" % (sorted(self._SAMPLE),))
+        if dropout not in self._DROPOUT:
+            raise FrcnnError("CanvasRcnnTrainer: dropout must be one of %s" % (self._DROPOUT,))
+        if int(max_gt) < 1:
+            raise FrcnnError("CanvasRcnnTrainer: max_gt must be at least 1")
+        if not 1 <= int(post_n) <= 4096:
+            raise FrcnnError("CanvasRcnnTrainer: post_n must be in [1, 4096] (got %r)" % (post_n,))
+        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
+        nc = self.num_classes = num_classes
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          [], _rcnn_params(nc), load_transform=_fc6_to_hwc, lead=(N,))
+        self._canvas_init(N, Hc, Wc, max_gt, seed)
+        self.delta, self.sample, self.dropout = delta, sample, dropout
+        self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
+        self.n_heads = 5 * nc
+        self.head_ld = ops.round_up(self.n_heads, 32)
+        dev, fh, fw = self.device, self.fh, self.fw
+        self._frozen_rpn(params)
+        self.rpn_mid = self._act(fh, fw, 512)
+        self.rpn_out = torch.empty((N * fh * fw, self.rpn_ld), dtype=torch.float32, device=dev)
+        # the head's extents (1, R_n): column 1 is the proposal count frcnn_proposals_batch_ext writes
+        self.head_ext = torch.ones((N, 2), dtype=torch.int32, device=dev)
+        self.prop = ops.ProposalBatchWorkspace(N, self.A, fh, fw, pre_n, post_n, dev, outputs=(
+            torch.zeros((N, post_n, 4), dtype=torch.float32, device=dev), torch.zeros((N, post_n), dtype=torch.float32, device=dev),
+            self.head_ext[:, 1]))
+        self.ptargets = train_ops.ProposalTargetsBatch(N, post_n, nc, dev)
+        self.step_losses = self.ptargets.losses
+        self.keep_list = torch.zeros((N * train_ops.ROIS_PER_IMAGE,), dtype=torch.int32, device=dev)
+        self.keep_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
+        self.pool5 = self._act(1, post_n, 49 * 512)
+        self.fc6 = self._act(1, post_n, 4096)
+        self.fc7 = self._act(1, post_n, 4096)
+        self.masks = torch.zeros((2, N, post_n, 4096), dtype=torch.uint8, device=dev) if dropout is not None else None
+        self.head_out = torch.empty((N * post_n, self.head_ld), dtype=torch.float32, device=dev)
+        self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rcnn_loss_batch
+        self.dfeat = torch.empty((N * fh * fw, 512), dtype=torch.float32, device=dev)
+        self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_batch_workspace_bytes(N, fh, fw, 512),),
+                                  dtype=torch.uint8, device=dev)
+        self.repack()
+
+    def repack(self):
+        self._repack_convs()
+        for n in ("fc6", "fc7"):
+            self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), 4096)
+        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
+
+    # ---------------------------------------------------------------- staging
+    def put(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
+        """Stages up to N (3,H_n,W_n) float32 CUDA images with their [G_n,5] ground truth (1 <= G_n <= max_gt) and optional
+        clip bounds; in "list" mode optional per-image kept lists (int, at most 128 distinct rows each; a slot without one
+        keeps nothing), with dropout "explicit" per-image (fc6, fc7) uint8 [post_n, 4096] masks (a slot without masks keeps
+        nothing).  Raises FrcnnError before anything is queued when something does not fit."""
+        images, gt_boxes = list(images), list(gt_boxes)
+        self._check_gt(images, gt_boxes)
+        if keep_inds is not None:
+            keep_inds = [torch.as_tensor(k).reshape(-1) for k in keep_inds]
+            if self.sample != "list":
+                raise FrcnnError("CanvasRcnnTrainer.put: kept lists need sample='list' (the trainer has %r)" % self.sample)
+            if len(keep_inds) != len(images):
+                raise FrcnnError("CanvasRcnnTrainer.put: %d images and %d kept lists" % (len(images), len(keep_inds)))
+            for n, k in enumerate(keep_inds):
+                if k.numel() > train_ops.ROIS_PER_IMAGE:
+                    raise FrcnnError("CanvasRcnnTrainer.put: image %d keeps %d rows, at most %d"
+                                     % (n, k.numel(), train_ops.ROIS_PER_IMAGE))
+                if torch.unique(k).numel() != k.numel():
+                    raise FrcnnError("CanvasRcnnTrainer.put: image %d's kept list repeats a row" % n)
+            keep_inds = [k.to(device=self.device, dtype=torch.int32) for k in keep_inds]
+        if masks is not None:
+            masks = list(masks)
+            if self.dropout != "explicit":
+                raise FrcnnError("CanvasRcnnTrainer.put: masks need dropout='explicit' (the trainer has %r)" % (self.dropout,))
+            if len(masks) != len(images):
+                raise FrcnnError("CanvasRcnnTrainer.put: %d images and %d mask pairs" % (len(images), len(masks)))
+            want = (self.post_n, 4096)
+            for n, pair in enumerate(masks):
+                if len(pair) != 2 or any(tuple(m.shape) not in (want, (want[0] * want[1],)) or m.dtype != torch.uint8 for m in pair):
+                    raise FrcnnError("CanvasRcnnTrainer.put: image %d needs two uint8 %s masks" % (n, want))
+        self._stage(images, gt_boxes, img_infos)
+        if self.sample == "list":
+            self._stage_lists(keep_inds, self.N, self.keep_list, self.keep_offsets)
+        if self.dropout == "explicit":
+            self.masks.zero_()
+            for n, pair in enumerate(masks or []):
+                for j in range(2):
+                    self.masks[j, n].copy_(pair[j].reshape(self.post_n, 4096), non_blocking=True)
+
+    # ---------------------------------------------------------------- forward
+    def forward(self):
+        """Forward over the staged canvas, the proposal targets and the per-slot losses (float32 [N, 4] device buffer:
+        loss_cls, loss_bbox, cls_accuracy, loss_rcnn; zeros for a slot that kept nothing)."""
+        N, ext, k, R_cap = self.N, self.extents, self.halvings, self.post_n
+        feat = self._canvas_trunk()
+        hi, lo, b = self.rpn3
+        ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid, extents=ext, halvings=k)
+        hi, lo, b = self.rpn_heads
+        ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=self.rpn_ld, out_f32=self.rpn_out, extents=ext,
+                         halvings=k)
+        ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, self.rpn_ld), None, self.anchors, self.A, self.fh, self.fw,
+                            self.feat_stride, 0, 0, self.min_size, self.pre_n, R_cap, self.nms_thresh, layout="nhwc",
+                            ld=self.rpn_ld, cls_is_logits=True, work=self.prop, extents=ext, halvings=k, im_info=self.im_info)
+        rois, count = self.prop.rois, self.head_ext[:, 1]
+        train_ops.proposal_targets_batch(rois, count, self.gt, self.gt_counts, self.ptargets, mode=self._SAMPLE[self.sample],
+                                         seeds=self.seeds, keep_list=self.keep_list, list_offsets=self.keep_offsets)
+        p5 = ops.Act(self.pool5.hi.view(N, R_cap, -1), None if self.pool5.lo is None else self.pool5.lo.view(N, R_cap, -1))
+        ops.roi_pool_batch(feat, rois, count, 7, 7, 1.0 / self.feat_stride, out=p5, extents=ext, halvings=k)
+        if self.dropout == "device":
+            for j in range(2):
+                train_ops.dropout_masks_batch(self.seeds, j + 1, self.masks[j])
+        if self.sample == "device" or self.dropout == "device":
+            self.seeds.add_(N)
+        hx = self.head_ext
+        (hi, lo), b, _ = self.packed["fc6"]
+        ops.conv2d_batch(self.pool5, hi, lo, b, 1, True, out=self.fc6, extents=hx, halvings=0)
+        if self.masks is not None:
+            train_ops.dropout_(self.fc6, self.masks[0])                                      # F.dropout, faster_rcnn.py:127
+        (hi, lo), b, _ = self.packed["fc7"]
+        ops.conv2d_batch(self.fc6, hi, lo, b, 1, True, out=self.fc7, extents=hx, halvings=0)
+        if self.masks is not None:
+            train_ops.dropout_(self.fc7, self.masks[1])                                      # :128
+        (hi, lo), b, _ = self.packed["heads"]
+        ops.conv2d_batch(self.fc7, hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out, extents=hx,
+                         halvings=0)
+        losses = train_ops.rcnn_loss_batch(self.head_out, self.ptargets, delta=self.delta, dhead=self.head_grad)
+        self.last_losses = losses
+        return losses
+
+    # ---------------------------------------------------------------- backward
+    def backward(self, debug=None):
+        """Fills g_flat with the sum over the slots of d(loss_rcnn_n)/d(parameter).  debug: as RcnnTrainer.backward, every
+        tensor with a leading [N] (dfeat [N*fh*fw, 512])."""
+        N, R_cap, ld, hx = self.N, self.post_n, self.head_ld, self.head_ext
+        twice = self.masks is not None               # ratio-0.5 dropout: dz = 2 * g * (y > 0), y = the post-dropout activation
+        # ---- cls_score | bbox_pred
+        dyh = self._gact(1, R_cap, ld)
+        dyhT = self._tbuf(1, ld, 1, R_cap)
+        train_ops.grad_prepare_batch(N, 1, R_cap, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
+        fc7T = self._tbuf(1, 4096, 1, R_cap)
+        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=self.fc7, tbuf=fc7T)
+        self._fc_wgrad(dyhT, fc7T, ld, 4096, self._heads_w(self.g_flat), m_out=self.n_heads)
+        train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
+        _, _, (dhi, dlo) = self.packed["heads"]
+        g = self._gact(1, R_cap, 4096, tag=1)
+        ops.conv2d_batch(dyh, dhi, dlo, self.zero_bias, 1, False, out=g, extents=hx, halvings=0)
+        if debug is not None:
+            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
+        # ---- fc7
+        dy7 = self._gact(1, R_cap, 4096)
+        dy7T = self._tbuf(1, 4096, 1, R_cap, tag=1)
+        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=g, y=self.fc7, out=dy7, tbuf=dy7T, times2=twice)
+        if debug is not None:
+            debug["fc7"] = dict(g_in=self._chw(g), dy=self._chw(dy7))
+        fc6T = self._tbuf(1, 4096, 1, R_cap)          # the buffer of fc7T: the heads' weight gradient has consumed it
+        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=self.fc6, tbuf=fc6T)
+        self._fc_wgrad(dy7T, fc6T, 4096, 4096, self.grads("fc7/W"))
+        train_ops.bias_grad(dy7T, 4096, self.grads("fc7/b"))
+        _, _, (dhi, dlo) = self.packed["fc7"]
+        g6 = self._gact(1, R_cap, 4096, tag=2)
+        ops.conv2d_batch(dy7, dhi, dlo, self.zero_bias, 1, False, out=g6, extents=hx, halvings=0)
+        # ---- fc6
+        dy6 = self._gact(1, R_cap, 4096)
+        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=g6, y=self.fc6, out=dy6, tbuf=dy7T, times2=twice)
+        if debug is not None:
+            debug["fc6"] = dict(g_in=self._chw(g6), dy=self._chw(dy6))
+        p5T = self._tbuf(1, 49 * 512, 1, R_cap)
+        train_ops.grad_prepare_batch(N, 1, R_cap, 49 * 512, g=self.pool5, tbuf=p5T)
+        self._fc_wgrad(dy7T, p5T, 4096, 49 * 512, self.grads("fc6/W"))
+        train_ops.bias_grad(dy7T, 4096, self.grads("fc6/b"))
+        _, _, (dhi, dlo) = self.packed["fc6"]
+        gp = self._gact(1, R_cap, 49 * 512, tag=1)
+        ops.conv2d_batch(dy6, dhi, dlo, self.zero_bias, 1, False, out=gp, extents=hx, halvings=0)
+        # ---- RoI pooling backward -> gradient of conv5_3's output, then the trunk
+        train_ops.roi_pool_backward_batch(self.feat, self.prop.rois, hx[:, 1], gp, self.extents, self.halvings, 7, 7,
+                                          1.0 / self.feat_stride, out=self.dfeat, ws=self.roi_ws)
+        gfeat = self._gact(self.fh, self.fw, 512, tag=3)
+        train_ops.grad_prepare_batch(N, self.fh, self.fw, 512, g_f32=self.dfeat, out=gfeat)
+        if debug is not None:
+            debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
+        self._canvas_chain(self.layers[12::-1], gfeat, debug)
+
+    def step(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
+        """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
+        losses, float32 [N, 4] on the device."""
+        self.put(images, gt_boxes, img_infos, keep_inds, masks)
+        return self._step()

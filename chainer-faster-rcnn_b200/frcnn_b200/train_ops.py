@@ -1,5 +1,7 @@
 """torch-tensor front end of the RPN-training entry points of the C ABI (include/frcnn_b200.h:
-frcnn_bbox_overlaps, frcnn_anchor_targets, frcnn_rpn_loss and their canvas forms).  Like ops.py: device pointers + the current
+frcnn_bbox_overlaps, frcnn_anchor_targets, frcnn_rpn_loss and their canvas forms), of the RCNN-head training entries and
+their canvas forms (frcnn_proposal_targets_batch, frcnn_rcnn_loss_batch, frcnn_roi_pool_backward_batch_ext,
+frcnn_dropout_masks_batch).  Like ops.py: device pointers + the current
 stream in, tensors out, no CPU path.
 
 Replaces models/bbox.pyx:16-56, models/anchor_target_layer.py:66-198 and the two loss functions of
@@ -18,6 +20,7 @@ from .ops import _need_cuda, _p, _stream
 RPN_NEGATIVE_OVERLAP, RPN_POSITIVE_OVERLAP = 0.3, 0.7       # models/anchor_target_layer.py:44-45
 RPN_FG_FRACTION, RPN_BATCHSIZE = 0.5, 256                   # :46-47
 SUBSAMPLE_NONE, SUBSAMPLE_DEVICE, SUBSAMPLE_LIST = 0, 1, 2
+ROIS_PER_IMAGE = 128                                        # models/proposal_target_layer.py:49
 
 
 def bbox_overlaps(boxes, query):
@@ -385,3 +388,95 @@ def keep_inside_flags(boxes, im_h, im_w):
     flags = torch.empty((b.shape[0],), dtype=torch.uint8, device=b.device)
     check(_lib.load().frcnn_keep_inside(_p(b), b.shape[0], int(im_h), int(im_w), _p(flags), _stream()), "frcnn_keep_inside")
     return flags
+
+
+# ---------------------------------------------------------------------------------------------- RCNN-head training on a canvas
+class ProposalTargetsBatch(object):
+    """Device buffers of frcnn_proposal_targets_batch / frcnn_rcnn_loss_batch for N slots of R_cap proposals: keep, labels
+    int32 [N][128], use_gt [N][128][5], bbox_reg_targets [N][128][4*num_classes] fp32, max_overlaps float64 [N][R_cap],
+    argmax int32 [N][R_cap], counts int32 [N][8] and losses fp32 [N][4]."""
+
+    def __init__(self, N, R_cap, num_classes, device):
+        self.N, self.R_cap, self.num_classes = N, R_cap, num_classes = int(N), int(R_cap), int(num_classes)
+        K = ROIS_PER_IMAGE
+        self.keep = torch.empty((N, K), dtype=torch.int32, device=device)
+        self.labels = torch.empty((N, K), dtype=torch.int32, device=device)
+        self.use_gt = torch.empty((N, K, 5), dtype=torch.float32, device=device)
+        self.bbox_reg_targets = torch.empty((N, K, 4 * num_classes), dtype=torch.float32, device=device)
+        self.max_overlaps = torch.empty((N, R_cap), dtype=torch.float64, device=device)
+        self.argmax = torch.empty((N, R_cap), dtype=torch.int32, device=device)
+        self.counts = torch.zeros((N, 8), dtype=torch.int32, device=device)
+        self.losses = torch.zeros((N, 4), dtype=torch.float32, device=device)
+
+
+def proposal_targets_batch(rois, counts, gt, gt_counts, work, mode=SUBSAMPLE_DEVICE, seeds=None, keep_list=None,
+                           list_offsets=None):
+    """frcnn_proposal_targets_batch into `work` (ProposalTargetsBatch).  rois [N, R_cap, 4] fp32 (each slot's block dense);
+    counts: int32 with one entry per slot (e.g. a column of an [N, 2] array) or None; gt fp32 [N, max_gt, 5]; gt_counts
+    int32 [N]; mode 1: seeds uint64 (torch.int64) [N]; mode 2: keep_list int32 [n] and list_offsets int32 [N+1]."""
+    from .ops import _counts_stride, _image_stride
+    N, R_cap = work.N, work.R_cap
+    rs = _image_stride(rois, (R_cap, 4), "proposal_targets_batch rois")
+    cs = _counts_stride(counts, N, "proposal_targets_batch")
+    _need_cuda(gt)
+    if gt.dim() != 3 or gt.shape[0] != N or gt.shape[2] != 5 or gt.dtype != torch.float32 or not gt.is_contiguous():
+        raise FrcnnError("proposal_targets_batch: gt must be a dense float32 [%d, max_gt, 5] CUDA tensor" % N)
+    sp, kp, nl, lo = None, None, 0, None
+    if mode == SUBSAMPLE_DEVICE:
+        sp = _slot_array(seeds, torch.int64, (N,), "seeds")
+    elif mode == SUBSAMPLE_LIST:
+        nl = int(keep_list.numel())
+        kp = _slot_array(keep_list, torch.int32, (nl,), "keep_list") if nl else None
+        lo = _slot_array(list_offsets, torch.int32, (N + 1,), "list_offsets")
+    check(_lib.load().frcnn_proposal_targets_batch(
+        N, _p(rois), rs, _p(counts), cs, R_cap, _p(gt), int(gt.shape[1]), _slot_array(gt_counts, torch.int32, (N,), "gt_counts"),
+        work.num_classes, int(mode), sp, kp, nl, lo, _p(work.keep), _p(work.labels), _p(work.use_gt), _p(work.bbox_reg_targets),
+        _p(work.max_overlaps), _p(work.argmax), _p(work.counts), _stream()), "frcnn_proposal_targets_batch")
+    return work
+
+
+def rcnn_loss_batch(head, work, delta=1.0, grad_scale=1.0, dhead=None):
+    """frcnn_rcnn_loss_batch on head [N*R_cap, ld] fp32 with the kept rows of `work`; dhead (same shape, optional) receives
+    the gradient in every element.  Returns work.losses ([N, 4], overwritten by the next call)."""
+    N, R_cap = work.N, work.R_cap
+    ld = int(head.shape[1])
+    for t in (head, dhead):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != (N * R_cap, ld)):
+            raise FrcnnError("rcnn_loss_batch: head / dhead must be contiguous float32 [%d, %d]" % (N * R_cap, ld))
+    check(_lib.load().frcnn_rcnn_loss_batch(N, _p(head), ld, R_cap, _p(work.keep), _p(work.labels), _p(work.bbox_reg_targets),
+                                            _p(work.counts), work.num_classes, float(delta), float(grad_scale), _p(work.losses),
+                                            _p(dhead), _stream()), "frcnn_rcnn_loss_batch")
+    return work.losses
+
+
+def roi_pool_backward_batch(feat, rois, counts, g, extents, halvings, outh=7, outw=7, scale=1.0 / 16, out=None, ws=None):
+    """frcnn_roi_pool_backward_batch_ext: feat Act [N,H,W,C], rois [N,R_cap,4], counts int32 per slot (or None), g Act
+    [N,...,R_cap*outh*outw*C], extents int32 [N, 2] -> dfeat fp32 [N*H*W, C] (0 outside each image)."""
+    from .ops import _counts_stride, _image_stride, _per_image_pairs
+    N, H, W, C = feat.hi.shape
+    R_cap = rois.shape[1]
+    rs = _image_stride(rois, (R_cap, 4), "roi_pool_backward_batch rois")
+    cs = _counts_stride(counts, N, "roi_pool_backward_batch")
+    if g.hi.numel() != N * R_cap * outh * outw * C or not g.hi.is_contiguous():
+        raise FrcnnError("roi_pool_backward_batch: g must be a dense [N, R_cap, %d] gradient" % (outh * outw * C))
+    lib = _lib.load()
+    if ws is None:
+        ws = torch.empty((lib.frcnn_roi_pool_backward_batch_workspace_bytes(N, H, W, C),), dtype=torch.uint8, device=feat.hi.device)
+    if out is None:
+        out = torch.empty((N * H * W, C), dtype=torch.float32, device=feat.hi.device)
+    check(lib.frcnn_roi_pool_backward_batch_ext(_p(feat.hi), _p(feat.lo), N, H, W, C, _p(rois), rs, _p(counts), cs, R_cap, outh, outw,
+                                                float(scale), _per_image_pairs(extents, N, "extents"), int(halvings), _p(g.hi),
+                                                _p(g.lo), _p(out), _p(ws), ws.numel(), _stream()), "frcnn_roi_pool_backward_batch_ext")
+    return out
+
+
+def dropout_masks_batch(seeds, salt, out):
+    """frcnn_dropout_masks_batch: seeds uint64 (torch.int64) [N] device -> out uint8 [N, rows, cols] (written in place)."""
+    _need_cuda(out)
+    N, rows, cols = out.shape
+    if out.dtype != torch.uint8 or not out.is_contiguous():
+        raise FrcnnError("dropout_masks_batch: out must be a dense uint8 [N, rows, cols] CUDA tensor")
+    check(_lib.load().frcnn_dropout_masks_batch(N, rows, cols, _slot_array(seeds, torch.int64, (N,), "seeds"),
+                                                ctypes.c_ulonglong(int(salt) & (2 ** 64 - 1)), _p(out), _stream()),
+          "frcnn_dropout_masks_batch")
+    return out

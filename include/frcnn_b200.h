@@ -675,7 +675,7 @@ int frcnn_roi_overlaps(const float* rois, const int* count, int R_cap, const flo
                        int* argmax, void* stream);
 /* part 2 (:138-147): use_gt_boxes [n,5] = gt[argmax[keep]], labels int32 [n] = use_gt_boxes[:,4] (faster_rcnn.py:154),
  * bbox_reg_targets [n, 4*num_classes] = float32 bbox_transform of the kept proposal scattered to its class's 4 columns
- * (rows whose class is 0 stay zero). */
+ * (rows whose class is 0 stay zero).  A kept row with argmax -1 (no overlap above -1) takes gt row 0. */
 int frcnn_roi_targets(const float* rois, const float* gt_boxes, const int* argmax, const int* keep_inds, int n, int num_classes,
                       float* use_gt_boxes, float* bbox_reg_targets, int* labels, void* stream);
 /* Array-level helpers of models/bbox_transform.py used by the training code: bbox_transform (:18-38) on float32 rows
@@ -699,6 +699,66 @@ size_t frcnn_roi_pool_backward_workspace_bytes(int H, int W, int C);
 int frcnn_roi_pool_backward(const void* feat_hi, const void* feat_lo, int H, int W, int C, const float* rois, const int* count,
                             int R_cap, int outh, int outw, float scale, const void* g_hi, const void* g_lo, float* dfeat,
                             void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- the RCNN step over the N slots of a canvas (rcnn_train.cu).  The slot is a grid dimension and every per-slot count,
+ * extent and seed is device memory read when the kernel runs, so one launch sequence (and one captured graph) serves any
+ * mix of sizes.  frcnn_rcnn_loss and frcnn_roi_pool_backward launch the kernels of their _batch forms with N = 1; the
+ * one-image overlaps / targets and the batched proposal targets share their per-row device code. */
+
+/* ProposalTargetLayer (proposal_target_layer.py:76-150) over N slots, one CTA per slot.
+ *   rois: slot n's proposals [R_cap][4] fp32 at rois + n*rois_stride (16-byte aligned), the first counts[n*count_stride] of
+ *   them valid (counts NULL: R_cap) -- the rois / count outputs of frcnn_proposals_batch_ext as they are.  1 <= R_cap <= 4096.
+ *   gt [N][max_gt][5] fp32 with gt_counts[n] (clamped to max_gt) rows in slot n.
+ *   Part 1: max_overlaps double [N][R_cap] and argmax int32 [N][R_cap] as frcnn_roi_overlaps computes them.
+ *   Part 2, the kept set (at most 128 rows):
+ *     mode 1 (device): fg = {r < R_n : max_ov >= 0.5}, bg = {r < R_n : 0.1 <= max_ov < 0.5} (a row without an overlap,
+ *       max_ov = -1, is in neither); the min(32, |fg|) fg rows with the smallest key(seeds[n], r), then the
+ *       min(128 - n_fg, |bg|) bg rows with the smallest key(seeds[n] ^ 0xA5A5A5A5DEADBEEF, r), key as in
+ *       frcnn_anchor_targets mode 1 (seeds uint64 [N] device memory).  The kept list is the kept fg rows in ascending r,
+ *       then the kept bg rows in ascending r.
+ *     mode 2 (list): slot n keeps keep_list[list_offsets[n] .. list_offsets[n+1]) in that order (offsets int32 [N+1],
+ *       clamped to [0, n_list)); entries outside [0, R_n), and entries past the 128th kept one, are skipped and counted.
+ *       The list must not repeat a row (see frcnn_rcnn_loss).
+ *   Part 3: keep int32 [N][128], labels int32 [N][128] (= use_gt_boxes[:, 4], background rows included, faster_rcnn.py:154),
+ *   use_gt_boxes [N][128][5], bbox_reg_targets [N][128][4*num_classes] as frcnn_roi_targets computes them; rows past
+ *   n_keep hold keep -1 and zeros.
+ *   out_counts int32 [N][8] = {n_keep, kept rows with max_ov >= 0.5, |fg|, |bg|, list entries skipped, R_n, 0, 0}.
+ * A slot with no ground truth or no RoIs has all-zero counts.  In list mode each slot's outputs equal frcnn_roi_overlaps +
+ * frcnn_roi_targets on that slot, bit for bit (both give a kept row with argmax -1 gt row 0). */
+int frcnn_proposal_targets_batch(int N, const float* rois, long rois_stride, const int* counts, long count_stride, int R_cap,
+                                 const float* gt, int max_gt, const int* gt_counts, int num_classes, int mode,
+                                 const unsigned long long* seeds, const int* keep_list, int n_list, const int* list_offsets,
+                                 int* keep, int* labels, float* use_gt_boxes, float* bbox_reg_targets, double* max_overlaps,
+                                 int* argmax, int* out_counts, void* stream);
+
+/* frcnn_rcnn_loss over the N slots of frcnn_proposal_targets_batch: head [N*R_cap][ld] with slot n's row r at n*R_cap + r;
+ * keep / labels / bbox_reg_targets [N][128][...] and counts [N][8] as that entry writes them (slot n reads its n_keep =
+ * counts[8n] on the device).  losses float32 [N][4].  dhead (optional, [N*R_cap][ld]) is written in EVERY element: kept rows
+ * get grad_scale * d(loss_rcnn_n)/d(.), everything else 0, so it needs no zeroing.  Each slot is normalised by its own
+ * n_keep, like the reference's per-device loss (ParallelUpdater sums the gradients); its losses and gradient rows equal
+ * frcnn_rcnn_loss on it, bit for bit.  A slot with n_keep = 0 gets zero losses and a zero gradient (counts shows which). */
+int frcnn_rcnn_loss_batch(int N, const float* head, int ld, int R_cap, const int* keep, const int* labels,
+                          const float* bbox_reg_targets, const int* counts, int num_classes, double delta, double grad_scale,
+                          float* losses, float* dhead, void* stream);
+
+/* frcnn_roi_pool_backward on an N-slot canvas feature map feat [N][H][W][C] (bf16 hi/lo): slot n's RoIs at
+ * rois + n*rois_stride, its count at counts[n*count_stride] (NULL: R_cap), its gradient rows g [N][R_cap][outh*outw][C].
+ * Bins are clamped to the slot's own ceil(extents[n] / 2^halvings) map, exactly as frcnn_roi_pool_batch_ext clamps them,
+ * and each slot has its own fixed-point accumulator, so dfeat [N*H*W][C] fp32 is 0 outside each image and slot n's map
+ * equals frcnn_roi_pool_backward on that image's own map, bit for bit.
+ * Workspace: frcnn_roi_pool_backward_batch_workspace_bytes(N, H, W, C). */
+size_t frcnn_roi_pool_backward_batch_workspace_bytes(int N, int H, int W, int C);
+int frcnn_roi_pool_backward_batch_ext(const void* feat_hi, const void* feat_lo, int N, int H, int W, int C, const float* rois,
+                                      long rois_stride, const int* counts, long count_stride, int R_cap, int outh, int outw,
+                                      float scale, const int* extents, int halvings, const void* g_hi, const void* g_lo,
+                                      float* dfeat, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Ratio-0.5 F.dropout keep masks for N slots: masks uint8 [N][rows][cols], element (r, c) of slot n =
+ *     key(seeds[n] ^ mix64(salt), r*cols + c) >> 63
+ * with key and mix64 as in frcnn_anchor_targets mode 1 (seeds uint64 [N] device memory; salt tells the layers apart).
+ * frcnn_dropout applies them to the flat [N*rows][cols] activations. */
+int frcnn_dropout_masks_batch(int N, int rows, int cols, const unsigned long long* seeds, unsigned long long salt,
+                              unsigned char* masks, void* stream);
 
 /* ---- the backward pass of the reference's training steps.  In the reference it is `loss.backward()` inside Chainer's
  * updater (train_rpn.py:169-174 / train_rcnn.py with StandardUpdater or ParallelUpdater; the graph is the one
