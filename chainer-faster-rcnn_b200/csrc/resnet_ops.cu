@@ -13,6 +13,7 @@
 
 namespace frcnn {
 
+// The values of 8 split pairs (pool_pair_value: an infinite hi stands alone, its lo is the NaN of inf - inf).
 __device__ __forceinline__ void load8f(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long off, float v[8]) {
     const uint4 h = *reinterpret_cast<const uint4*>(hi + off);
     const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h);
@@ -22,7 +23,7 @@ __device__ __forceinline__ void load8f(const __nv_bfloat16* hi, const __nv_bfloa
         const uint4 l = *reinterpret_cast<const uint4*>(lo + off);
         const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] += __bfloat162float(lb[j]);
+        for (int j = 0; j < 8; ++j) v[j] = pool_pair_value(v[j], __bfloat162float(lb[j]));
     }
 }
 

@@ -100,14 +100,20 @@ def test_bn_folding_matches_unfolded_oracle():
     assert np.array_equal(Wf, Wo) and np.array_equal(bf, bo)
 
 
-@pytest.mark.parametrize("n_layers,shape", [(50, (160, 224)), (101, (150, 201))])
+@pytest.mark.parametrize("n_layers,shape", [(50, (160, 224)), (101, (150, 201)), (152, (600, 1000))])
 def test_resnet_faster_rcnn_forward_stagewise(n_layers, shape):
+    """Each stage on the device's own upstream tensors.  Boxes: bbox_transform_inv makes x1 = cx + dx*w - exp(dw)*w/2 (and
+    alike), so a delta error e moves a coordinate by up to e*w*(1 + exp(dw)/2); the decode amplifies the head's error by
+    the exponential of the size deltas.  Each coordinate is held to 1e-4 of the image scale, or, where it is larger, to the
+    deltas' own 1e-4 max-norm bound carried through that sensitivity: the synthetic head's deltas reach 7.6 on ResNet-152 at
+    600x1000 (exp(7.6)/2 ~ 1000), where a 1e-5 delta error alone moves a box by 2.5e-4 of the image scale."""
     from frcnn_b200.resnet_engine import ResNetEngine
     H, W = shape
+    post_n = 300 if H * W >= 600 * 1000 else 100          # the reference's test-time count where the map has the anchors
     params = orc.make_resnet_params(n_layers, seed=11)
     x = orc.make_image(H, W, seed=4)
     info = np.array([[H, W]], np.int32)
-    eng = ResNetEngine(params, n_layers, precision="bf16x3", anchors=ANCHORS, keep_rpn_debug=True, use_graph=False, post_n=100)
+    eng = ResNetEngine(params, n_layers, precision="bf16x3", anchors=ANCHORS, keep_rpn_debug=True, use_graph=False, post_n=post_n)
     prob, boxes, plan = eng(torch.from_numpy(x[0]).cuda())
     torch.cuda.synchronize()
     R = prob.shape[0]
@@ -125,7 +131,7 @@ def test_resnet_faster_rcnn_forward_stagewise(n_layers, shape):
     deltas_dev = rpn[:, 18:54].T.reshape(1, 36, fh, fw)
     h_ref = orc.relu(orc.conv2d(feat_dev, params["RPN/rpn_conv_3x3/W"], params["RPN/rpn_conv_3x3/b"], 1))
     assert _rel(plan.rpn_mid.to_chw_f32().cpu().numpy()[None], h_ref) < 1e-4
-    want_rois, want_fg = orc.proposal_layer(orc.softmax_axis1(logits_dev), deltas_dev, info, feat_stride=32, post_nms_top_n=100)
+    want_rois, want_fg = orc.proposal_layer(orc.softmax_axis1(logits_dev), deltas_dev, info, feat_stride=32, post_nms_top_n=post_n)
     rois_dev = plan.prop.rois.cpu().numpy()
     assert R == len(want_rois) and R > 0
     assert np.array_equal(rois_dev[:R], want_rois)
@@ -141,11 +147,22 @@ def test_resnet_faster_rcnn_forward_stagewise(n_layers, shape):
     print("fc6 (K=100352): device vs float64 %.2e, fp32 oracle vs float64 %.2e" % (_rel(fc6_dev, fc6_64), _rel(aux["fc6"], fc6_64)))
     assert _rel(fc6_dev, fc6_64) < 5e-5
     assert np.abs(prob.cpu().numpy() - cls_ref).max() < 1e-4 * cls_ref.max()
-    e_box = _rel(boxes.cpu().numpy(), box_ref)
-    print("boxes: max err %.2e of scale (max |delta| %.2f)" % (e_box, np.abs(aux["bbox_pred"]).max()))
-    assert e_box < 1e-4
+    ho = plan.head_out.cpu().numpy()[:R]
+    d_dev, d_ref = ho[:, 21:105].astype(np.float64), aux["bbox_pred"].astype(np.float64)
+    e_delta = _rel(d_dev, d_ref)
+    assert e_delta < 1e-4
+    r = rois_dev[:R].astype(np.float64)
+    size = np.stack([r[:, 2] - r[:, 0] + 1, r[:, 3] - r[:, 1] + 1], 1)                          # RoI w, h
+    d_size = np.maximum(np.abs(d_dev), np.abs(d_ref)).reshape(R, -1, 4)[:, :, 2:]                # dw, dh
+    sens = size[:, None, :] * (1 + 0.5 * np.exp(d_size))                                        # [R, classes, (x, y)]
+    sens = np.concatenate([sens, sens], axis=2).reshape(R, -1)                                  # x1, y1, x2, y2
+    err = np.abs(boxes.cpu().numpy().astype(np.float64) - box_ref)
+    tol = np.maximum(1e-4 * np.abs(box_ref).max(), 1e-4 * np.abs(d_ref).max() * sens)
+    print("boxes: max err %.2e of scale, worst err / tol %.2f (max |delta| %.2f, deltas %.2e)" %
+          (_rel(boxes.cpu().numpy(), box_ref), (err / tol).max(), np.abs(d_ref).max(), e_delta))
+    assert (err <= tol).all()
     # graph replay == eager, and lanes work with the subclassed plan
-    eng_g = ResNetEngine(params, n_layers, precision="bf16x3", anchors=ANCHORS, use_graph=True, post_n=100)
+    eng_g = ResNetEngine(params, n_layers, precision="bf16x3", anchors=ANCHORS, use_graph=True, post_n=post_n)
     pg, bg, plan_g = eng_g(torch.from_numpy(x[0]).cuda())
     assert torch.equal(pg, prob) and torch.equal(bg, boxes)
     assert type(plan_g.clone()) is type(plan_g)
