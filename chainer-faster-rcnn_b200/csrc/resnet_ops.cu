@@ -88,8 +88,9 @@ __global__ void im2col_kernel(const float* __restrict__ x, int C, int H, int W, 
     }
 }
 
-// Raw photos straight into the first-layer im2col planes of a canvas batch: preprocess_bgr8_kernel, a copy into a zeroed
-// canvas and im2col_kernel(extents) for all N slots in one launch, bit for bit.  Slot blockIdx.y is raw_slot's; one CTA
+// Raw photos straight into the first-layer im2col planes of a canvas batch: preprocess_bgr8_kernel (kCubic: the VOC
+// dataset's bicubic, cubic_bgr8), a copy into a zeroed canvas and im2col_kernel(extents) for all N slots in one launch, bit
+// for bit.  Slot blockIdx.y is raw_slot's; one CTA
 // per (band of `band` output rows, tile of `tile` output columns).  The CTA first stages the resized, mean-subtracted input
 // window its outputs read -- rows [ho0*stride - pad, +rows), columns [wo0*stride - pad, +cols), float32 [rows][cols][3] in
 // shared memory, 0 outside the image's extent -- so each input pixel's bilinear is computed once per CTA instead of once
@@ -103,7 +104,8 @@ struct PreIm2colArgs {
     double m0, m1, m2;
     __nv_bfloat16 *hi, *lo;
 };
-__global__ void __launch_bounds__(256) preprocess_bgr8_canvas_im2col_kernel(const PreIm2colArgs a) {
+template <bool kCubic>
+__global__ void __launch_bounds__(256) preprocess_canvas_im2col_kernel(const PreIm2colArgs a) {
     extern __shared__ float smem[];
     const int kmax = a.ks * a.ks * 3;
     int* tab = reinterpret_cast<int*>(smem);           // [kmax]: window offset of K index k
@@ -124,8 +126,14 @@ __global__ void __launch_bounds__(256) preprocess_bgr8_canvas_im2col_kernel(cons
         for (int p = threadIdx.x; p < rows * cols; p += blockDim.x) {
             const int i = p / cols, j = p - i * cols, y = y0 + i, x = x0 + j;
             float v[3] = {0.0f, 0.0f, 0.0f};
-            if (y >= 0 && y < s.eh && x >= 0 && x < s.ew)
-                bilinear_bgr8(s.src, s.w0, bilinear_tap(y, s.inv_scale, s.h0), bilinear_tap(x, s.inv_scale, s.w0), a.m0, a.m1, a.m2, v);
+            if (y >= 0 && y < s.eh && x >= 0 && x < s.ew) {
+                if (kCubic)
+                    cubic_bgr8(s.src, s.w0, cubic_tap(y, s.inv_scale, s.h0), cubic_tap(x, s.inv_scale, s.w0), x, s.ew, a.m0, a.m1,
+                               a.m2, v);
+                else
+                    bilinear_bgr8(s.src, s.w0, bilinear_tap(y, s.inv_scale, s.h0), bilinear_tap(x, s.inv_scale, s.w0), a.m0, a.m1,
+                                  a.m2, v);
+            }
             float* w = win + (i * a.cols + j) * 3;
             w[0] = v[0];
             w[1] = v[1];
@@ -147,6 +155,19 @@ __global__ void __launch_bounds__(256) preprocess_bgr8_canvas_im2col_kernel(cons
         }
         store8f(a.hi, a.lo, ((img + (long)(ho0 + hl) * a.Wo + wo0 + wl) * a.Kp) + k8 * 8, v);
     }
+}
+
+// The VOC dataset's box scaling on the device: gt[n][g] = (f32(box) * f32(im_scale) for the four coordinates, the label
+// unchanged) for g < count[n] (clamped to [0, max_gt]), 0 for the rows after it; gt_counts[n] = that count.  One thread per
+// (slot, row, column).
+__global__ void voc_scale_gt_kernel(const float* __restrict__ scale, const int* __restrict__ count, const float* __restrict__ raw,
+                                    int N, int max_gt, float* __restrict__ gt, int* __restrict__ gt_counts) {
+    const long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
+    if (i >= (long)N * max_gt * 5) return;
+    const int n = (int)(i / ((long)max_gt * 5)), g = (int)(i / 5 % max_gt), j = (int)(i % 5);
+    const int cnt = min(max(__ldg(count + n), 0), max_gt);
+    gt[i] = g < cnt ? (j < 4 ? __fmul_rn(raw[i], __ldg(scale + n)) : raw[i]) : 0.0f;
+    if (g == 0 && j == 0) gt_counts[n] = cnt;
 }
 
 // OIHW (Cout, C, ks, ks) fp32 -> [1][Cout][Kp] bf16 hi/lo in the K order of im2col_kernel; scale[o] (optional) multiplies
@@ -329,12 +350,13 @@ int frcnn_pack_image_im2col_batch_ext(const float* x_nchw, int N, int C, int H, 
     return im2col_launch(x_nchw, N, C, H, W, ksize, stride, pad, K_pad, extents, y_hi, y_lo, stream);
 }
 
-int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
-                                        const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
-                                        double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
-                                        void* y_hi, void* y_lo, void* stream) {
-    FRCNN_ENTRY();
-    const char* fn = "frcnn_preprocess_bgr8_canvas_im2col";
+}  // extern "C"
+
+// the launch behind frcnn_preprocess_bgr8_canvas_im2col (bilinear) and frcnn_preprocess_voc_canvas_im2col (cubic)
+static int preprocess_canvas_im2col_launch(const char* fn, bool cubic, const unsigned char* arena, long long arena_bytes,
+                                           const long long* src_off, const int* src_hw, const double* inv_scale, const int* extents,
+                                           int N, int Hc, int Wc, double mean_b, double mean_g, double mean_r, int ksize, int stride,
+                                           int pad, int K_pad, void* y_hi, void* y_lo, void* stream) {
     FRCNN_REQUIRE(arena, "%s: arena is NULL", fn);
     FRCNN_REQUIRE(arena_bytes > 0, "%s: arena_bytes must be positive (got %lld)", fn, arena_bytes);
     FRCNN_REQUIRE(src_off, "%s: src_off is NULL", fn);
@@ -376,7 +398,45 @@ int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long ar
     const long blocks = (long)cdiv(Ho, a.band) * a.tiles;
     FRCNN_REQUIRE(blocks <= 0x7fffffffl, "%s: canvas %dx%d needs too many tiles", fn, Hc, Wc);
     const size_t smem = (size_t)kmax * 4 + (size_t)rows * a.cols * 12;
-    preprocess_bgr8_canvas_im2col_kernel<<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
+    if (cubic)
+        preprocess_canvas_im2col_kernel<true><<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
+    else
+        preprocess_canvas_im2col_kernel<false><<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+extern "C" {
+
+int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                        const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
+                                        double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
+                                        void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    return preprocess_canvas_im2col_launch("frcnn_preprocess_bgr8_canvas_im2col", false, arena, arena_bytes, src_off, src_hw,
+                                           inv_scale, extents, N, Hc, Wc, mean_b, mean_g, mean_r, ksize, stride, pad, K_pad, y_hi,
+                                           y_lo, stream);
+}
+
+int frcnn_preprocess_voc_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                       const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
+                                       double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
+                                       void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    return preprocess_canvas_im2col_launch("frcnn_preprocess_voc_canvas_im2col", true, arena, arena_bytes, src_off, src_hw,
+                                           inv_scale, extents, N, Hc, Wc, mean_b, mean_g, mean_r, ksize, stride, pad, K_pad, y_hi,
+                                           y_lo, stream);
+}
+
+int frcnn_voc_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, int N, int max_gt, float* gt, int* gt_counts,
+                             void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(scale && count && raw_gt && gt && gt_counts, "frcnn_voc_scale_gt_batch: NULL argument");
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && max_gt >= 1 && max_gt <= (1 << 20),
+                  "frcnn_voc_scale_gt_batch: needs 1 <= N <= 65535 and 1 <= max_gt <= 2^20 (got N=%d max_gt=%d)", N, max_gt);
+    const long total = (long)N * max_gt * 5;
+    voc_scale_gt_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(scale, count, raw_gt, N, max_gt, gt,
+                                                                                          gt_counts);
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }

@@ -65,6 +65,13 @@ class VOC(object):
         label = rng.randint(1, len(self.LABELS), size=n).astype(np.int32)
         return img, bbox, label
 
+    def get_raw_example(self, i):
+        """Example i before the transform: (uint8 (h, w, 3) BGR photo, float32 (n, 4) boxes in photo coordinates, int32 (n,)
+        labels) -- what CanvasRpnTrainer / CanvasRcnnTrainer(raw_input=True).put_raw take.  Their device transform follows
+        the reference (float32 mean subtraction, then the bicubic resize); get_example below subtracts the means in float64."""
+        img, bbox, label = self._raw_example(i)
+        return np.ascontiguousarray(img.transpose(1, 2, 0).astype(np.uint8)), bbox, label
+
     def get_example(self, i):
         img, bbox, label = self._raw_example(i)
         img = img.transpose(1, 2, 0)

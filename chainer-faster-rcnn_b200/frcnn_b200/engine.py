@@ -600,34 +600,48 @@ class RawPhotoInput(object):
     """RAW uint8 (h0,w0,3) BGR photos on a canvas: one device block [header | pixels] (preprocess.raw_header_layout) whose
     header holds each slot's extents, clip bounds, source size, pixel offset and 1 / im_scale, and whose `arena` of
     arena_bytes (default: N sources of Hc x Wc) the photos.  pack_c8 / pack_im2col (frcnn_preprocess_bgr8_canvas[_im2col])
-    resize, subtract pixel_means and pack every slot straight into the first layer's planes: there is no x_in."""
+    resize, subtract pixel_means and pack every slot straight into the first layer's planes: there is no x_in.
+
+    max_gt (a training canvas): the photos are the VOC training dataset's, so the block also carries a ground-truth section
+    (preprocess.voc_gt_layout) between the header and the pixels, pixel_means default to preprocess.VOC_MEANS, pack_im2col
+    resizes bicubically as the dataset does (frcnn_preprocess_voc_canvas_im2col) and scale_gt writes the scaled boxes."""
     x_in = None
 
-    def __init__(self, N, Hc, Wc, device, pixel_means=None, arena_bytes=None):
+    def __init__(self, N, Hc, Wc, device, pixel_means=None, arena_bytes=None, max_gt=None):
         self.N, self.H, self.W = int(N), int(Hc), int(Wc)
-        self.pixel_means = tuple(float(v) for v in np.asarray(preprocess.PIXEL_MEANS if pixel_means is None else pixel_means,
-                                                              dtype=np.float64).reshape(-1)[:3])
+        self.max_gt = None if max_gt is None else int(max_gt)
+        if pixel_means is None:
+            pixel_means = preprocess.PIXEL_MEANS if self.max_gt is None else preprocess.VOC_MEANS
+        self.pixel_means = tuple(float(v) for v in np.asarray(pixel_means, dtype=np.float64).reshape(-1)[:3])
         self.arena_bytes = self.N * 3 * self.H * self.W if arena_bytes is None else int(arena_bytes)
         if self.arena_bytes < 1:
             raise FrcnnError("raw batch: arena_bytes must be positive (got %d)" % self.arena_bytes)
         layout, self.header_bytes = preprocess.raw_header_layout(self.N)
+        gt_at = self.header_bytes
+        if self.max_gt is not None:
+            gt_layout, gt_bytes = preprocess.voc_gt_layout(self.N, self.max_gt)
+            self.header_bytes += gt_bytes
         self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=device)
         self.arena = self.block[self.header_bytes:]
-        tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64}
+        tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64, np.float32: torch.float32}
         h = {name: self.block[off:off + 8 * self.N].view(tdt[dt]).view((self.N, 2) if items == 2 else (self.N,))
              for name, (off, dt, items) in layout.items()}
         self.extents, self.im_info = h["extents"], h["im_info"]
         # what both first-layer kernels read from the block
         self.descriptors = (self.arena, h["src_off"], h["src_hw"], h["inv_scale"], h["extents"])
+        if self.max_gt is not None:
+            self.gt_fields = tuple(self.block[gt_at + off:gt_at + off + int(np.prod(shape)) * 4].view(tdt[dt]).view(shape)
+                                   for off, dt, shape in (gt_layout[k] for k in ("scale", "count", "raw_gt")))
         self._stage = None          # pinned host mirror of the block + the event of its last upload
 
     def header(self, shapes, img_infos=None):
         """preprocess.raw_batch_header for these slots, canvas and arena (raises FrcnnError when something does not fit)."""
         return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
 
-    def upload(self, images, img_infos=None):
-        """A list of photos into the block on the current stream, as CanvasBatchPlan.forward_raw describes.  Returns (host
-        header, [im_scale])."""
+    def upload(self, images, img_infos=None, boxes=None, labels=None):
+        """A list of photos into the block on the current stream, as CanvasBatchPlan.forward_raw describes; on a training
+        canvas also their boxes (source-photo coordinates) and labels (preprocess.voc_gt_section).  Raises FrcnnError before
+        anything is queued when something does not fit.  Returns (host header, [im_scale])."""
         on_host = all(isinstance(x, np.ndarray) for x in images)
         if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
             raise FrcnnError("forward_raw: the images must be all numpy arrays or all CUDA tensors")
@@ -635,12 +649,17 @@ class RawPhotoInput(object):
             if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
                 raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
         hdr, scales, _ = self.header([x.shape[:2] for x in images], img_infos)
+        block_hdr = hdr
+        if self.max_gt is not None:
+            if boxes is None or labels is None:
+                raise FrcnnError("raw training batch: the photos need their boxes and labels")
+            block_hdr = np.concatenate([hdr, preprocess.voc_gt_section(list(boxes), list(labels), scales, self.N, self.max_gt)])
         cur = torch.cuda.current_stream()
         if self._stage is None:
             self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
         pin, done = self._stage
         done.synchronize()                    # the previous upload has left the pinned mirror
-        pin.h2d(self.block, cur, nbytes=preprocess.fill_raw_block(pin.np, hdr, images if on_host else [], self.N))
+        pin.h2d(self.block, cur, nbytes=preprocess.fill_raw_block(pin.np, block_hdr, images if on_host else [], self.N))
         if not on_host:
             offs = preprocess.raw_header_views(hdr, self.N)["src_off"]
             for n, x in enumerate(images):
@@ -649,10 +668,17 @@ class RawPhotoInput(object):
         return hdr, scales
 
     def pack_c8(self, out):
+        if self.max_gt is not None:
+            raise FrcnnError("raw batch: a training canvas packs im2col planes only")
         ops.preprocess_pack_canvas(*self.descriptors, self.H, self.W, self.pixel_means, out=out)
 
     def pack_im2col(self, out, ksize, stride, pad, k_pad):
-        ops.preprocess_im2col_canvas(*self.descriptors, self.H, self.W, self.pixel_means, ksize, stride, pad, k_pad, out=out)
+        pack = ops.preprocess_im2col_canvas if self.max_gt is None else ops.preprocess_voc_im2col_canvas
+        pack(*self.descriptors, self.H, self.W, self.pixel_means, ksize, stride, pad, k_pad, out=out)
+
+    def scale_gt(self, gt, gt_counts):
+        """A training canvas's boxes times each slot's im_scale, labels and counts into gt [N, max_gt, 5] / gt_counts [N]."""
+        ops.voc_scale_gt(*self.gt_fields, gt, gt_counts)
 
 
 class LanePool(object):

@@ -295,20 +295,48 @@ def preprocess_im2col_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc,
     Act [N, Ho, Wo, k_pad] (pack_image_im2col_batch's layout), in one launch (resize + mean subtraction + im2col; 0 outside
     every image's output extent).  The descriptors are preprocess_pack_canvas's, all device tensors read when the kernel
     runs."""
-    N = _raw_descriptors("preprocess_im2col_canvas", arena, src_off, src_hw, inv_scale, extents)
+    return _preprocess_im2col(_lib.load().frcnn_preprocess_bgr8_canvas_im2col, "frcnn_preprocess_bgr8_canvas_im2col", arena, src_off, src_hw, inv_scale, extents, Hc, Wc,
+                              pixel_means, ksize, stride, pad, k_pad, precision, out)
+
+
+def preprocess_voc_im2col_canvas(arena, src_off, src_hw, inv_scale, extents, Hc, Wc, pixel_means, ksize, stride, pad, k_pad,
+                                 precision="bf16x3", out=None):
+    """frcnn_preprocess_voc_canvas_im2col: preprocess_im2col_canvas with the VOC training dataset's bicubic resize (OpenCV's
+    float INTER_CUBIC) in place of forward.py's bilinear."""
+    return _preprocess_im2col(_lib.load().frcnn_preprocess_voc_canvas_im2col, "frcnn_preprocess_voc_canvas_im2col", arena, src_off, src_hw, inv_scale, extents, Hc, Wc,
+                              pixel_means, ksize, stride, pad, k_pad, precision, out)
+
+
+def _preprocess_im2col(fn, entry, arena, src_off, src_hw, inv_scale, extents, Hc, Wc, pixel_means, ksize, stride, pad, k_pad, precision,
+                       out):
+    N = _raw_descriptors(entry, arena, src_off, src_hw, inv_scale, extents)
     Ho, Wo = (Hc + 2 * pad - ksize) // stride + 1, (Wc + 2 * pad - ksize) // stride + 1
     if out is None:
         hi = torch.empty((N, Ho, Wo, k_pad), dtype=torch.bfloat16, device=arena.device)
         out = Act(hi, torch.empty_like(hi) if precision == "bf16x3" else None)
     if tuple(out.hi.shape) != (N, Ho, Wo, k_pad) or (out.lo is not None and out.lo.shape != out.hi.shape):
-        raise FrcnnError("preprocess_im2col_canvas: output %s, expected %s" % (tuple(out.hi.shape), (N, Ho, Wo, k_pad)))
-    _dense_planes("preprocess_im2col_canvas", out)
+        raise FrcnnError("%s: output %s, expected %s" % (entry, tuple(out.hi.shape), (N, Ho, Wo, k_pad)))
+    _dense_planes(entry, out)
     m = np.asarray(pixel_means, dtype=np.float64).reshape(-1)
-    check(_lib.load().frcnn_preprocess_bgr8_canvas_im2col(
+    check(fn(
         _p(arena), arena.numel(), _p(src_off), _per_image_pairs(src_hw, N, "src_hw"), _p(inv_scale),
         _per_image_pairs(extents, N, "extents"), N, int(Hc), int(Wc), float(m[0]), float(m[1]), float(m[2]), int(ksize),
-        int(stride), int(pad), int(k_pad), _p(out.hi), _p(out.lo), _stream()), "frcnn_preprocess_bgr8_canvas_im2col")
+        int(stride), int(pad), int(k_pad), _p(out.hi), _p(out.lo), _stream()), entry)
     return out
+
+
+def voc_scale_gt(scale, count, raw_gt, gt, gt_counts):
+    """frcnn_voc_scale_gt_batch: gt [N, max_gt, 5] float32 <- the raw boxes of raw_gt [N, max_gt, 5] times scale[n] (float32
+    [N]), labels copied, 0 after count[n] (int32 [N]) rows; gt_counts [N] int32 <- the clamped counts.  Device tensors."""
+    _need_cuda(scale, count, raw_gt, gt, gt_counts)
+    N, max_gt = int(gt.shape[0]), int(gt.shape[1])
+    for t, dt, shape, name in ((scale, torch.float32, (N,), "scale"), (count, torch.int32, (N,), "count"),
+                               (raw_gt, torch.float32, (N, max_gt, 5), "raw_gt"), (gt, torch.float32, (N, max_gt, 5), "gt"),
+                               (gt_counts, torch.int32, (N,), "gt_counts")):
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise FrcnnError("voc_scale_gt: %s must be a dense %s %s CUDA tensor" % (name, dt, shape))
+    check(_lib.load().frcnn_voc_scale_gt_batch(_p(scale), _p(count), _p(raw_gt), N, max_gt, _p(gt), _p(gt_counts), _stream()),
+          "frcnn_voc_scale_gt_batch")
 
 
 def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None, extents=None):

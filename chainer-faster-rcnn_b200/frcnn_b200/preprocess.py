@@ -158,3 +158,44 @@ def raw_batch_header(shapes, N, Hc, Wc, arena_bytes, img_infos=None, scale=600, 
         v["inv_scale"][n] = 1.0 / im_scale
         scales.append(im_scale)
     return hdr, scales, used
+
+
+# ---- raw photos into a training canvas (CanvasRpnTrainer / CanvasRcnnTrainer(raw_input=True)): one block
+# [raw header | ground-truth section | pixels].  The raw header is raw_header_layout's, unchanged; the ground-truth section
+# carries each slot's float32 im_scale, box count and raw boxes + labels, so photos and boxes travel in one H2D copy.
+VOC_MEANS = (103.939, 116.779, 123.68)    # datasets/pascal_voc_dataset.py VOC.mean (BGR)
+
+
+def voc_gt_layout(N, max_gt):
+    """({name: (byte offset inside the section, dtype, shape)}, section bytes, a multiple of 256): "scale" float32 [N],
+    "count" int32 [N], "raw_gt" float32 [N, max_gt, 5] (x1, y1, x2, y2 in source-photo coordinates, label)."""
+    off_count = ops.round_up(4 * N, 16)
+    off_gt = off_count + ops.round_up(4 * N, 16)
+    return ({"scale": (0, np.float32, (N,)), "count": (off_count, np.int32, (N,)),
+             "raw_gt": (off_gt, np.float32, (N, max_gt, 5))}, ops.round_up(off_gt + 20 * N * max_gt, 256))
+
+
+def voc_gt_section(boxes, labels, scales, N, max_gt):
+    """The uint8 ground-truth section for the photos whose im_scale are `scales`: boxes[n] (G_n, 4) and labels[n] (G_n,)
+    with 1 <= G_n <= max_gt.  Raises FrcnnError when a list does not fit."""
+    if len(boxes) != len(scales) or len(labels) != len(scales):
+        raise _lib.FrcnnError("raw training batch: %d photos, %d box lists and %d label lists" % (len(scales), len(boxes), len(labels)))
+    layout, nbytes = voc_gt_layout(N, max_gt)
+    sec = np.zeros((nbytes,), dtype=np.uint8)
+    v = {name: sec[off:off + int(np.prod(shape)) * 4].view(dt).reshape(shape) for name, (off, dt, shape) in layout.items()}
+    for n, (b, l) in enumerate(zip(boxes, labels)):
+        b, l = np.asarray(b), np.asarray(l)
+        G = b.shape[0] if b.ndim == 2 else -1
+        if b.ndim != 2 or b.shape[1] != 4 or l.shape != (G,) or not 1 <= G <= max_gt:
+            raise _lib.FrcnnError("raw training batch: photo %d has boxes of shape %s and labels of shape %s, needs (G, 4) and "
+                                  "(G,) with 1 <= G <= %d" % (n, b.shape, l.shape, max_gt))
+        v["raw_gt"][n, :G, :4] = b
+        v["raw_gt"][n, :G, 4] = l
+        v["count"][n] = G
+        v["scale"][n] = scales[n]
+    return sec
+
+
+def voc_scale_boxes(boxes, im_scale):
+    """The reference's `bbox *= im_scale` on float32 boxes, as NumPy >= 2 computes it: f32(box) * f32(im_scale), float32."""
+    return np.asarray(boxes, dtype=np.float32) * np.float32(im_scale)

@@ -22,9 +22,9 @@ frcnn_grad_prepare.  Gradients / master weights / momentum are float32 in three 
 import numpy as np
 import torch
 
-from . import ops, shard, train_ops
+from . import ops, preprocess, shard, train_ops
 from ._lib import FrcnnError
-from .engine import ImageInput, vgg16_schedule
+from .engine import ImageInput, RawPhotoInput, vgg16_schedule
 
 ROIS_PER_IMAGE, FG_FRACTION = 128, 0.25                          # models/proposal_target_layer.py:49-50
 FG_THRESH, BG_THRESH_HI, BG_THRESH_LO = 0.5, 0.5, 0.1            # :46-48
@@ -619,10 +619,12 @@ class _CanvasSteps(object):
     """The canvas machinery shared by CanvasRpnTrainer and CanvasRcnnTrainer: the N-slot image input with its device extents,
     the staged ground truth, the [N]-lead gradient buffers, the in-place repack of the convolutions (a captured graph reads
     the packed weights), the canvas trunk forward and backward, and the capture-then-replay step."""
+    raw_input = False           # True: the input is RawPhotoInput's training block (put_raw / step_raw)
 
-    def _canvas_init(self, N, Hc, Wc, max_gt, seed):
+    def _canvas_init(self, N, Hc, Wc, max_gt, seed, raw_input):
         dev = self.device
-        self.input = ImageInput(N, Hc, Wc, dev, canvas=True)
+        self.raw_input = bool(raw_input)
+        self.input = RawPhotoInput(N, Hc, Wc, dev, max_gt=max_gt) if self.raw_input else ImageInput(N, Hc, Wc, dev, canvas=True)
         self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
         halvings = 0
         for L in self.layers[:13]:                   # a layer's extents are ceil(extent / 2^halvings)
@@ -669,6 +671,13 @@ class _CanvasSteps(object):
             self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
 
     # ---------------------------------------------------------------- staging
+    def _need_input(self, call):
+        """Raises FrcnnError when `call` ("put" or "put_raw") does not match the input the trainer was built with."""
+        if self.raw_input != (call == "put_raw"):
+            raise FrcnnError("%s.%s: the trainer was built with raw_input=%s, so it takes %s" % (
+                type(self).__name__, call, self.raw_input, "raw photos through put_raw / step_raw" if self.raw_input
+                else "float images through put / step"))
+
     def _check_gt(self, images, gt_boxes):
         who = type(self).__name__
         if len(gt_boxes) != len(images):
@@ -688,6 +697,14 @@ class _CanvasSteps(object):
             self.gt[n, :g.shape[0]].copy_(g, non_blocking=True)
         self.gt_counts.copy_(torch.from_numpy(counts), non_blocking=True)
 
+    def _stage_raw(self, photos, boxes, labels):
+        """Photos, boxes and labels into the raw block in one host-to-device copy (RawPhotoInput.upload raises before it if
+        something does not fit); the first launch of the step resizes them and scales the boxes.  Returns [im_scale]."""
+        preprocess.raw_photo_shapes(photos)
+        hdr, scales = self.input.upload(photos, boxes=list(boxes), labels=list(labels))
+        self.image_sizes = [tuple(int(v) for v in e) for e in preprocess.raw_header_views(hdr, self.N)["extents"]]
+        return scales
+
     @staticmethod
     def _stage_lists(lists, N, buf, offsets):
         """Per-image int32 lists into one flat device buffer + offsets [N+1] (slots without a list get an empty range)."""
@@ -703,6 +720,8 @@ class _CanvasSteps(object):
     def _canvas_trunk(self):
         ext = self.extents
         self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
+        if self.raw_input:
+            self.input.scale_gt(self.gt, self.gt_counts)
         x = self.x_col
         for i, L in enumerate(self.layers[:13]):
             (hi, lo), b, _ = self.packed[L["name"]]
@@ -798,7 +817,7 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
-                 process_group=None):
+                 process_group=None, raw_input=False):
         if int(N) != N or N < 1:
             raise FrcnnError("CanvasRpnTrainer needs N >= 1 slots (got %r)" % (N,))
         if subsample not in self._MODES:
@@ -815,7 +834,7 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
         self.n_heads = 6 * self.A
         self.head_ld = ops.round_up(self.n_heads, 32)
-        self._canvas_init(N, Hc, Wc, max_gt, seed)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         R = self.layers[13]
         R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, self.halvings
         R["y"] = self._act(self.fh, self.fw, 512)
@@ -837,19 +856,38 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         """Stages up to N (3,H_n,W_n) float32 CUDA images, their [G_n,5] ground-truth boxes (1 <= G_n <= max_gt), optional
         clip bounds (default (H_n, W_n)) and, in "list" mode, optional per-image disable lists into the static buffers
         (the remaining slots are empty).  Raises FrcnnError before anything is queued when something does not fit."""
+        self._need_input("put")
         images, gt_boxes = list(images), list(gt_boxes)
         self._check_gt(images, gt_boxes)
-        if disable_pos is not None:
-            disable_pos = list(disable_pos)
-            if self.subsample != "list":
-                raise FrcnnError("CanvasRpnTrainer.put: disable lists need subsample='list' (the trainer has %r)" % self.subsample)
-            if len(disable_pos) != len(images):
-                raise FrcnnError("CanvasRpnTrainer.put: %d images and %d disable lists" % (len(images), len(disable_pos)))
-            if any(int(d.numel()) > self.targets.cap for d in disable_pos):
-                raise FrcnnError("CanvasRpnTrainer.put: a disable list is longer than %d anchors" % self.targets.cap)
+        disable_pos = self._check_disable("put", len(images), disable_pos)
         self._stage(images, gt_boxes, img_infos)
         if self.subsample == "list":
             self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
+
+    def put_raw(self, photos, boxes, labels, disable_pos=None):
+        """put() for a trainer built with raw_input=True: up to N raw uint8 (h, w, 3) BGR photos (numpy), their boxes (G_n, 4)
+        in source-photo coordinates and labels (G_n,), 1 <= G_n <= max_gt, uploaded in one host-to-device copy.  The step
+        applies the VOC training dataset's transform on the device: mean subtraction, the bicubic resize of
+        preprocess.plan_size (short side 600, long side at most 1000), boxes times float32 im_scale; the clip bounds are the
+        resized (H_n, W_n).  Raises FrcnnError before anything is queued when something does not fit.  Returns [im_scale]."""
+        self._need_input("put_raw")
+        photos = list(photos)
+        disable_pos = self._check_disable("put_raw", len(photos), disable_pos)
+        scales = self._stage_raw(photos, boxes, labels)
+        if self.subsample == "list":
+            self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
+        return scales
+
+    def _check_disable(self, call, n_images, disable_pos):
+        if disable_pos is not None:
+            disable_pos = list(disable_pos)
+            if self.subsample != "list":
+                raise FrcnnError("CanvasRpnTrainer.%s: disable lists need subsample='list' (the trainer has %r)" % (call, self.subsample))
+            if len(disable_pos) != n_images:
+                raise FrcnnError("CanvasRpnTrainer.%s: %d images and %d disable lists" % (call, n_images, len(disable_pos)))
+            if any(int(d.numel()) > self.targets.cap for d in disable_pos):
+                raise FrcnnError("CanvasRpnTrainer.%s: a disable list is longer than %d anchors" % (call, self.targets.cap))
+        return disable_pos
 
     # ---------------------------------------------------------------- forward
     def forward(self):
@@ -901,6 +939,11 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         self.put(images, gt_boxes, img_infos, disable_pos)
         return self._step()
 
+    def step_raw(self, photos, boxes, labels, disable_pos=None):
+        """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
+        self.put_raw(photos, boxes, labels, disable_pos)
+        return self._step()
+
 
 class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
     """The RCNN-mode training step (RcnnTrainer's, train_rcnn.py) on N images of different sizes per update, with one set of
@@ -926,7 +969,7 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None):
+                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False):
         if int(N) != N or N < 1:
             raise FrcnnError("CanvasRcnnTrainer needs N >= 1 slots (got %r)" % (N,))
         if sample not in self._SAMPLE:
@@ -941,7 +984,7 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         nc = self.num_classes = num_classes
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [], _rcnn_params(nc), load_transform=_fc6_to_hwc, lead=(N,))
-        self._canvas_init(N, Hc, Wc, max_gt, seed)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         self.delta, self.sample, self.dropout = delta, sample, dropout
         self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
         self.n_heads = 5 * nc
@@ -982,32 +1025,50 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         clip bounds; in "list" mode optional per-image kept lists (int, at most 128 distinct rows each; a slot without one
         keeps nothing), with dropout "explicit" per-image (fc6, fc7) uint8 [post_n, 4096] masks (a slot without masks keeps
         nothing).  Raises FrcnnError before anything is queued when something does not fit."""
+        self._need_input("put")
         images, gt_boxes = list(images), list(gt_boxes)
         self._check_gt(images, gt_boxes)
+        keep_inds, masks = self._check_extras("put", len(images), keep_inds, masks)
+        self._stage(images, gt_boxes, img_infos)
+        self._stage_extras(keep_inds, masks)
+
+    def put_raw(self, photos, boxes, labels, keep_inds=None, masks=None):
+        """put() for a trainer built with raw_input=True: raw photos, boxes and labels as CanvasRpnTrainer.put_raw takes
+        them, with put()'s kept lists and masks.  Returns [im_scale]."""
+        self._need_input("put_raw")
+        photos = list(photos)
+        keep_inds, masks = self._check_extras("put_raw", len(photos), keep_inds, masks)
+        scales = self._stage_raw(photos, boxes, labels)
+        self._stage_extras(keep_inds, masks)
+        return scales
+
+    def _check_extras(self, call, n_images, keep_inds, masks):
         if keep_inds is not None:
             keep_inds = [torch.as_tensor(k).reshape(-1) for k in keep_inds]
             if self.sample != "list":
-                raise FrcnnError("CanvasRcnnTrainer.put: kept lists need sample='list' (the trainer has %r)" % self.sample)
-            if len(keep_inds) != len(images):
-                raise FrcnnError("CanvasRcnnTrainer.put: %d images and %d kept lists" % (len(images), len(keep_inds)))
+                raise FrcnnError("CanvasRcnnTrainer.%s: kept lists need sample='list' (the trainer has %r)" % (call, self.sample))
+            if len(keep_inds) != n_images:
+                raise FrcnnError("CanvasRcnnTrainer.%s: %d images and %d kept lists" % (call, n_images, len(keep_inds)))
             for n, k in enumerate(keep_inds):
                 if k.numel() > train_ops.ROIS_PER_IMAGE:
-                    raise FrcnnError("CanvasRcnnTrainer.put: image %d keeps %d rows, at most %d"
-                                     % (n, k.numel(), train_ops.ROIS_PER_IMAGE))
+                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d keeps %d rows, at most %d"
+                                     % (call, n, k.numel(), train_ops.ROIS_PER_IMAGE))
                 if torch.unique(k).numel() != k.numel():
-                    raise FrcnnError("CanvasRcnnTrainer.put: image %d's kept list repeats a row" % n)
+                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d's kept list repeats a row" % (call, n))
             keep_inds = [k.to(device=self.device, dtype=torch.int32) for k in keep_inds]
         if masks is not None:
             masks = list(masks)
             if self.dropout != "explicit":
-                raise FrcnnError("CanvasRcnnTrainer.put: masks need dropout='explicit' (the trainer has %r)" % (self.dropout,))
-            if len(masks) != len(images):
-                raise FrcnnError("CanvasRcnnTrainer.put: %d images and %d mask pairs" % (len(images), len(masks)))
+                raise FrcnnError("CanvasRcnnTrainer.%s: masks need dropout='explicit' (the trainer has %r)" % (call, self.dropout))
+            if len(masks) != n_images:
+                raise FrcnnError("CanvasRcnnTrainer.%s: %d images and %d mask pairs" % (call, n_images, len(masks)))
             want = (self.post_n, 4096)
             for n, pair in enumerate(masks):
                 if len(pair) != 2 or any(tuple(m.shape) not in (want, (want[0] * want[1],)) or m.dtype != torch.uint8 for m in pair):
-                    raise FrcnnError("CanvasRcnnTrainer.put: image %d needs two uint8 %s masks" % (n, want))
-        self._stage(images, gt_boxes, img_infos)
+                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d needs two uint8 %s masks" % (call, n, want))
+        return keep_inds, masks
+
+    def _stage_extras(self, keep_inds, masks):
         if self.sample == "list":
             self._stage_lists(keep_inds, self.N, self.keep_list, self.keep_offsets)
         if self.dropout == "explicit":
@@ -1113,4 +1174,9 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
         losses, float32 [N, 4] on the device."""
         self.put(images, gt_boxes, img_infos, keep_inds, masks)
+        return self._step()
+
+    def step_raw(self, photos, boxes, labels, keep_inds=None, masks=None):
+        """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
+        self.put_raw(photos, boxes, labels, keep_inds, masks)
         return self._step()

@@ -573,6 +573,24 @@ int frcnn_preprocess_bgr8_canvas_im2col(const unsigned char* arena, long long ar
                                         const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
                                         double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
                                         void* y_hi, void* y_lo, void* stream);
+/* The VOC training dataset's transform (datasets/pascal_voc_dataset.py get_example: float32 mean subtraction, then
+ * cv.resize(..., INTER_CUBIC)) on raw photos, straight into the first-layer im2col planes of a canvas batch in ONE launch.
+ * Arguments, descriptors, output layout, empty-slot rule and errors are those of frcnn_preprocess_bgr8_canvas_im2col; only the
+ * resize differs: OpenCV's generic float bicubic (A = -0.75, float coordinate, replicate borders, no clamping of the
+ * result), restated bit for bit -- what cv2.resize computes on a float32 image with IPP off.  Each tap's pixel is
+ * float(double(u8) - mean_c).  A descriptor whose inv_scale is 0, negative, infinite or NaN moves no access outside the
+ * arena or the slot and gives finite values.  The training canvas uses ksize 3, stride 1, pad 1, K_pad 32. */
+int frcnn_preprocess_voc_canvas_im2col(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                       const int* src_hw, const double* inv_scale, const int* extents, int N, int Hc, int Wc,
+                                       double mean_b, double mean_g, double mean_r, int ksize, int stride, int pad, int K_pad,
+                                       void* y_hi, void* y_lo, void* stream);
+/* The VOC dataset's box scaling (`bbox *= im_scale` on float32 boxes) for N canvas slots, into a trainer's ground truth:
+ * gt [N][max_gt][5] (device float32) row g of slot n = (f32(box) * f32(im_scale) for x1, y1, x2, y2, the label copied) for
+ * g < c = clamp(count[n], 0, max_gt), and 0 for g >= c; gt_counts[n] (device int32 [N]) = c.  scale (device float32 [N]):
+ * im_scale rounded to float32; count (device int32 [N]); raw_gt (device float32 [N][max_gt][5]): the boxes in source-photo
+ * coordinates and the labels.  NULL pointers, N outside [1, 65535] or max_gt outside [1, 2^20] -> FRCNN_ERR_ARG. */
+int frcnn_voc_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, int N, int max_gt, float* gt, int* gt_counts,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * RPN training targets and losses (SURVEY.md 8f rank 1, the train_rpn.py step).  Box arithmetic is
