@@ -34,7 +34,13 @@ struct PrepArgs {
     int c_blocks;                    // blockIdx.z = image * c_blocks + 64-channel block
     int planes;                      // 1: plane at q; 3: planes shifted by -1/0/+1 pixel
     int times2;                      // multiply the result by 2 (the 1/(1-ratio) of a ratio-0.5 dropout), correctly rounded
+    int route;                       // ROUTE_*: how the source reaches pixel (h, w)
 };
+
+// ROUTE_PLAIN: the source at (h, w), or routed through the 2x2 ceil-mode pool when p is given (frcnn_grad_prepare);
+// ROUTE_POOL3: the 3x3/2 cover_all max-pool backward, p [pool3s2_out(H)][pool3s2_out(W)][C] (frcnn_maxpool3x3s2_backward);
+// ROUTE_STRIDE2: the source [ceil(H/2)][ceil(W/2)][C] at the even pixels (2i, 2j), 0 elsewhere (frcnn_grad_prepare_stride2).
+enum { ROUTE_PLAIN = 0, ROUTE_POOL3 = 1, ROUTE_STRIDE2 = 2 };
 
 constexpr int PAD_LEFT = 8;          // zero columns left of pixel 0 in the transposed layout: every 8-pixel group starts 16-B aligned
 
@@ -78,6 +84,66 @@ __device__ __forceinline__ uint32_t times2_bf16x2(uint32_t x) {
     return *reinterpret_cast<const uint32_t*>(&v);
 }
 
+// The values of 8 split pairs, read as pool_pair_value reads them (an infinite hi stands alone).
+__device__ __forceinline__ void pair_values(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long off, float v[8]) {
+    uint32_t hw[4], lw[4] = {0u, 0u, 0u, 0u};
+    ld4(hi, off, hw);
+    if (lo) ld4(lo, off, lw);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int m = j >> 1, sh = (j & 1) * 16;
+        v[j] = pool_pair_value(__uint_as_float(((hw[m] >> sh) & 0xFFFFu) << 16), __uint_as_float(((lw[m] >> sh) & 0xFFFFu) << 16));
+    }
+}
+
+// F.max_pooling_2d(3, stride=2, pad=0, cover_all=True) backward at pixel (r, c) of the H x W pool input, as a gather: window
+// (i, j) covers rows [2i, min(2i+3, H)) and columns [2j, min(2j+3, W)) and sends g[i][j] to the FIRST element in scan order
+// whose value equals p[i][j] (values compared as floats: +0 == -0, NaN equals nothing).  Up to four windows cover a pixel;
+// their contributions are summed in fp32 in ascending (i, j) order starting from +0, then masked by y > 0 and re-split.
+__device__ __forceinline__ void pool3_words(const PrepArgs& a, int r, int c, int c8, uint32_t hw[4], uint32_t lw[4]) {
+    const int ph = (a.H - 2) / 2 + 1, pw = (a.W - 2) / 2 + 1;
+    const long self = ((long)r * a.W + c) * a.C + c8 * 8;
+    float yv[8], acc[8];
+    pair_values(a.y_hi, a.y_lo, self, yv);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+    const int i0 = r < 2 ? 0 : (r - 1) / 2, i1 = min(r / 2, ph - 1);
+    const int j0 = c < 2 ? 0 : (c - 1) / 2, j1 = min(c / 2, pw - 1);
+    for (int i = i0; i <= i1; ++i) {
+        for (int j = j0; j <= j1; ++j) {
+            const long q = ((long)i * pw + j) * a.C + c8 * 8;
+            float pv[8], gv[8];
+            pair_values(a.p_hi, a.p_lo, q, pv);
+            pair_values(a.g_hi, a.g_lo, q, gv);
+            bool hit[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) hit[k] = yv[k] == pv[k];
+            const int w_end = min(2 * j + 3, a.W);
+            for (int e = 0; e < 9; ++e) {                   // the window elements before (r, c) in scan order
+                const int rr = 2 * i + e / 3, cc = 2 * j + e % 3;
+                if (rr == r && cc == c) break;
+                if (cc >= w_end) continue;
+                float ev[8];
+                pair_values(a.y_hi, a.y_lo, ((long)rr * a.W + cc) * a.C + c8 * 8, ev);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) hit[k] = hit[k] && !(ev[k] == pv[k]);
+            }
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+                if (hit[k]) acc[k] = __fadd_rn(acc[k], gv[k]);
+        }
+    }
+    pack8(acc, hw, lw);
+    uint32_t yh[4];
+    ld4(a.y_hi, self, yh);
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+        const uint32_t keep = positive_mask(yh[m]);          // y > 0
+        hw[m] &= keep;
+        lw[m] &= keep;
+    }
+}
+
 // The (masked / routed) gradient of 8 channels (chunk c8) at pixel (h, w) as packed bf16 words -- integer SIMD only:
 //   * a value is the pair (hi, lo) with hi = bf16(v), lo = bf16(v - hi): v > 0 iff hi > 0 (read as int16, NaN excluded);
 //     equality of two values is tested on the exact float sums (eq_values);
@@ -86,6 +152,10 @@ __device__ __forceinline__ uint32_t times2_bf16x2(uint32_t x) {
 // Masked elements become +0 in both planes; kept elements keep the source's (hi, lo) words untouched (an fp32 source is
 // split into (hi, lo) first).
 __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int c8, uint32_t hw[4], uint32_t lw[4]) {
+    if (a.route == ROUTE_POOL3) {
+        pool3_words(a, h, w, c8, hw, lw);
+        return;
+    }
     const long off = ((long)h * a.W + w) * a.C + c8 * 8;
     uint32_t keep[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
     uint32_t yh[4], yl[4] = {0u, 0u, 0u, 0u};
@@ -106,6 +176,14 @@ __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int 
     }
     if (a.y_hi != nullptr && a.y_lo) ld4(a.y_lo, off, yl);
     long goff = off;
+    if (a.route == ROUTE_STRIDE2) {                         // odd rows and columns receive nothing
+        if ((h | w) & 1) {
+#pragma unroll
+            for (int m = 0; m < 4; ++m) hw[m] = lw[m] = 0u;
+            return;
+        }
+        goff = ((long)(h >> 1) * ((a.W + 1) / 2) + (w >> 1)) * a.C + c8 * 8;
+    }
     if (a.p_hi != nullptr) {
         const int Wq = (a.W + 1) / 2;
         const int ph = h >> 1, pw = w >> 1;
@@ -359,7 +437,7 @@ static long padded_pixels(int H, int W, int* wp_out) {
 
 static int grad_prepare(const char* fn, const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi,
                         const void* y_lo, const void* p_hi, const void* p_lo, int N, int H, int W, int C, void* o_hi, void* o_lo,
-                        void* t_hi, void* t_lo, int planes, int times2, cudaStream_t stream) {
+                        void* t_hi, void* t_lo, int planes, int times2, cudaStream_t stream, int route = ROUTE_PLAIN) {
     FRCNN_REQUIRE(N >= 1, "%s: N = %d < 1", fn, N);
     FRCNN_REQUIRE(H > 0 && W > 0 && C > 0 && C % 8 == 0, "%s: bad shape H=%d W=%d C=%d (C %% 8 == 0)", fn, H, W, C);
     FRCNN_REQUIRE((g_hi != nullptr) != (g_f32 != nullptr), "%s: give the source as bf16 planes OR fp32", fn);
@@ -367,6 +445,9 @@ static int grad_prepare(const char* fn, const void* g_hi, const void* g_lo, cons
     FRCNN_REQUIRE(!p_hi || y_hi, "%s: pooled routing needs the un-pooled forward activation", fn);
     FRCNN_REQUIRE(planes == 1 || planes == 3, "%s: planes must be 1 or 3", fn);
     FRCNN_REQUIRE(o_hi || t_hi, "%s: no output requested", fn);
+    FRCNN_REQUIRE(route != ROUTE_POOL3 || (g_hi && y_hi && p_hi && H >= 2 && W >= 2 && !times2),
+                  "%s: needs the pooled gradient, y and p, and a pool input of at least 2 x 2 (got H=%d W=%d)", fn, H, W);
+    FRCNN_REQUIRE(route != ROUTE_STRIDE2 || (g_hi && !p_hi && !times2), "%s: needs a bf16 source and no pooled map", fn);
     PrepArgs a;
     a.g_hi = (const __nv_bfloat16*)g_hi; a.g_lo = (const __nv_bfloat16*)g_lo; a.g_f32 = g_f32; a.ld_f32 = ld_f32;
     a.y_hi = (const __nv_bfloat16*)y_hi; a.y_lo = (const __nv_bfloat16*)y_lo;
@@ -377,6 +458,7 @@ static int grad_prepare(const char* fn, const void* g_hi, const void* g_lo, cons
     a.t_ld = (long)N * a.Kp;
     a.planes = planes;
     a.times2 = times2 ? 1 : 0;
+    a.route = route;
     a.c_blocks = cdiv(C, 64);
     FRCNN_REQUIRE(!times2 || !g_f32, "%s: times2 is not available for an fp32 source", fn);
     const long gz = (long)N * a.c_blocks;
@@ -412,6 +494,20 @@ int frcnn_grad_prepare_batch(const void* g_hi, const void* g_lo, const float* g_
     FRCNN_ENTRY();
     return grad_prepare("grad_prepare_batch", g_hi, g_lo, g_f32, ld_f32, y_hi, y_lo, p_hi, p_lo, N, H, W, C, o_hi, o_lo, t_hi,
                         t_lo, planes, times2, (cudaStream_t)stream);
+}
+
+int frcnn_maxpool3x3s2_backward(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, const void* p_hi,
+                                const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo, void* stream) {
+    FRCNN_ENTRY();
+    return grad_prepare("maxpool3x3s2_backward", g_hi, g_lo, nullptr, 0, y_hi, y_lo, p_hi, p_lo, 1, H, W, C, o_hi, o_lo, t_hi,
+                        t_lo, 1, 0, (cudaStream_t)stream, ROUTE_POOL3);
+}
+
+int frcnn_grad_prepare_stride2(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, int H, int W, int C,
+                               void* o_hi, void* o_lo, void* t_hi, void* t_lo, int planes, void* stream) {
+    FRCNN_ENTRY();
+    return grad_prepare("grad_prepare_stride2", g_hi, g_lo, nullptr, 0, y_hi, y_lo, nullptr, nullptr, 1, H, W, C, o_hi, o_lo,
+                        t_hi, t_lo, planes, 0, (cudaStream_t)stream, ROUTE_STRIDE2);
 }
 
 int frcnn_wgrad_reduce(const float* parts, int groups, int splits, int M_parts, int M, int ld, int N, float scale, float* dw,

@@ -108,6 +108,12 @@ SIGNATURES = {
     "frcnn_padded_pixels": (c_long, [c_int, c_int, c_void_p]),
     "frcnn_grad_prepare": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "frcnn_maxpool3x3s2_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_grad_prepare_stride2": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_void_p]),
+    "frcnn_fold_batchnorm": (c_int, [c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_wgrad_reduce_scaled": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_wgrad_reduce": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "frcnn_bias_grad": (c_int, [c_void_p, c_void_p, c_int, c_long, c_float, c_void_p, c_void_p]),
     "frcnn_sgd_momentum": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_float, c_float, c_float, c_void_p]),

@@ -1,0 +1,315 @@
+"""The train_rpn.py step with the ResNet-50/101/152 trunk: `FasterRCNN(trunk_class=ResNet, rpn_in_ch=2048, feat_stride=32)`
+with `rpn_train = True` (the reference's utils/prepare_train.py offers --trunk_model ResNet50/101/152).
+
+ResNetRpnTrainer -- forward (conv1 7x7/2 + pool 3x3/2 + bottleneck blocks + RPN) -> AnchorTargetLayer -> rpn_loss -> backward
+through the RPN heads, the RPN 3x3 conv and every trunk convolution -> [gradient all-reduce] -> WeightDecay + MomentumSGD.
+
+BatchNorm is FROZEN: every BN layer applies its stored statistics and affine (gamma, beta, avg_mean, avg_var are constants,
+not in the flat parameter buffer and not weight-decayed).  The reasons: the reference never ran a batch-statistics ResNet
+detector (FasterRCNN calls trunk_class() without n_layers), per-image batch statistics with one image per update would be a
+different model from the test-mode BN the forward engines define, and frozen BN is how ResNet Faster R-CNN is trained in
+practice (py-faster-rcnn's use_global_stats with the scale layers at lr_mult 0).  Trainable: every trunk convolution's W,
+trunk/conv1/b, and the RPN's parameters.
+
+A convolution and its frozen BN are then the folded convolution Wf = W*s, bf = beta + (b - mean)*s, s = gamma/sqrt(var+eps):
+    forward          the folded weights, rebuilt from the fp32 masters at every repack (frcnn_fold_batchnorm, the float64
+                     arithmetic of resnet_engine.fold_batchnorm) and packed by the forward engines' packers, so the planes
+                     equal ResNetPackedWeights' of the exported parameters; the launches are ResNetForwardPlan._run_trunk's
+    data gradient    frcnn_conv2d on the folded weights' dgrad planes; the residual sums are the epilogue of
+                     frcnn_conv2d_res with relu = 0 (identity block: dgrad_conv1(dy1) + dy3; projection block:
+                     dgrad_conv1(dy1) + dgrad_conv4(dy3))
+    weight gradient  dW = s[co] * sum dz (x) x, d(conv1/b) = s * sum dz: the split-K GEMM of the folded convolution, reduced
+                     in fixed order and scaled per output channel (frcnn_wgrad_reduce_scaled)
+    re-layouts       the 3x3/2 cover_all max-pool backward fused with conv1's ReLU mask (frcnn_maxpool3x3s2_backward), and the
+                     backward of the stride-2 subsample fused with the ReLU mask of the block output it reads
+                     (frcnn_grad_prepare_stride2)
+Everything else -- the flat buffers, the RPN heads' backward, the loss, the optimizer and the gradient exchange (one bucket,
+after backward) -- is RpnTrainer's.
+"""
+import numpy as np
+import torch
+
+from . import ops, train_ops
+from ._lib import FrcnnError
+from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
+from .train_engine import RpnTrainer
+
+SUBSAMPLE_MODES = ("device", "numpy", "none")
+
+
+def bn_scale(params, bn):
+    """s = gamma / sqrt(var + eps) in float64, as resnet_engine.fold_batchnorm computes it."""
+    return np.asarray(params[bn + "/gamma"], np.float64) / np.sqrt(np.asarray(params[bn + "/avg_var"], np.float64) + BN_EPS)
+
+
+def trunk_convs(n_layers):
+    """[(conv name, bn name, cin, cout, k)] of the trunk in flat-buffer order: conv1, then per block conv1..conv3 (+ conv4)."""
+    out = [("trunk/conv1", "trunk/bn1", 3, 64, 7)]
+    for stage, blk, cin, mid, cout, stride, proj in block_list(n_layers):
+        base = "trunk/%s/%s" % (stage, blk)
+        out += [(base + "/conv1", base + "/bn1", cin, mid, 1), (base + "/conv2", base + "/bn2", mid, mid, 3),
+                (base + "/conv3", base + "/bn3", mid, cout, 1)]
+        if proj:
+            out.append((base + "/conv4", base + "/bn4", cin, cout, 1))
+    return out
+
+
+class ResNetRpnTrainer(RpnTrainer):
+    """Weights, optimizer state and buffers of the RPN-mode training step with the ResNet trunk for one image shape.  The
+    surface is RpnTrainer's: forward / backward(debug) / update / step / weights / grads / export_params, subsample modes
+    "device", "numpy" and "none", disable_pos.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming;
+    its BN entries are read once and stay constant."""
+
+    def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+        if n_layers not in RESNET_BLOCKS:
+            raise FrcnnError("ResNetRpnTrainer: n_layers must be one of %s (got %r)" % (sorted(RESNET_BLOCKS), n_layers))
+        if subsample not in SUBSAMPLE_MODES:
+            raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
+        if feat_stride != 32:
+            raise FrcnnError("ResNetRpnTrainer: the ResNet trunk's feature stride is 32 (got feat_stride=%r)" % (feat_stride,))
+        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1           # conv1 7x7/2 pad 3
+        if min(Ho, Wo) < 3:
+            raise FrcnnError("ResNetRpnTrainer: the image must be at least 5 x 5 (got %d x %d)" % (H, W))
+        self.n_layers = n_layers
+        A = len(anchors)
+        convs = trunk_convs(n_layers)
+        need = {n + "/W": (co, ci, k, k) for n, _, ci, co, k in convs}
+        need["trunk/conv1/b"] = (64,)
+        for _, bn, _, co, _ in convs:
+            for f in ("gamma", "beta", "avg_mean", "avg_var"):
+                need["%s/%s" % (bn, f)] = (co,)
+        need.update({"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,), "RPN/rpn_cls_score/W": (2 * A, 512, 1, 1),
+                     "RPN/rpn_cls_score/b": (2 * A,), "RPN/rpn_bbox_pred/W": (4 * A, 512, 1, 1), "RPN/rpn_bbox_pred/b": (4 * A,)})
+        for k, sh in need.items():
+            if k not in params or tuple(np.shape(params[k])) != sh:
+                raise FrcnnError("ResNetRpnTrainer: parameter %s must have shape %s (got %s)"
+                                 % (k, sh, None if k not in params else tuple(np.shape(params[k]))))
+        layers = [dict(name=n, bn=bn, cin=ci, cout=co, k=k, bias=n == "trunk/conv1") for n, bn, ci, co, k in convs]
+        layers.append(dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3))
+        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
+        extra = [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
+        self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          layers, extra)
+        self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
+        self.n_heads = 6 * self.A
+        self.head_ld = ops.round_up(self.n_heads, 32)
+        dev = self.device
+        # ---- frozen BN: s (float64) per conv, the constant folded bias of every conv but conv1, the folded-weight buffers
+        T = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)     # noqa: E731
+        self.conv = {}
+        for L in layers[:-1]:
+            n, bn = L["name"], L["bn"]
+            L["s"] = T(bn_scale(params, bn), torch.float64)
+            L["wf"] = torch.empty((L["cout"], L["cin"], L["k"], L["k"]), dtype=torch.float32, device=dev)
+            if L["bias"]:
+                L["beta"], L["mean"] = T(params[bn + "/beta"]), T(params[bn + "/avg_mean"])
+                L["bf"] = torch.empty((L["cout"],), dtype=torch.float32, device=dev)
+            else:
+                L["bf"] = T(fold_batchnorm(params[n + "/W"], params[bn + "/gamma"], params[bn + "/beta"], params[bn + "/avg_mean"],
+                                           params[bn + "/avg_var"])[1])
+            self.conv[n] = L
+        self.bn_params = {k: np.asarray(params[k]).copy() for k in need if "/bn" in k}
+        # ---- activations (ResNetForwardPlan._alloc_trunk's, every one kept for backward)
+        act = self._act
+        self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)
+        self.x_col = act(Ho, Wo, CONV1_KPAD)
+        self.c1 = act(Ho, Wo, 64)
+        h, w = (Ho - 2) // 2 + 1, (Wo - 2) // 2 + 1
+        self.p1 = act(h, w, 64)
+        self.c1_hw = (Ho, Wo)
+        self.blocks = []
+        x = self.p1
+        for stage, blk, cin, mid, cout, stride, proj in block_list(n_layers):
+            B = dict(name="trunk/%s/%s" % (stage, blk), x=x, stride=stride, proj=proj, cin=cin, mid=mid, cout=cout)
+            if stride == 2:
+                h, w = (h + 1) // 2, (w + 1) // 2
+                B["xs"] = act(h, w, cin)
+            B["H"], B["W"] = h, w
+            B["y1"], B["y2"] = act(h, w, mid), act(h, w, mid)
+            if proj:
+                B["sc"] = act(h, w, cout)
+            B["out"] = act(h, w, cout)
+            self.blocks.append(B)
+            x = B["out"]
+        self.fh, self.fw = h, w
+        R = self.rpn_layer = layers[-1]
+        R["H"], R["W"], R["pool"] = h, w, False
+        R["y"] = act(h, w, 512)
+        self.head_out = torch.empty((h * w, self.head_ld), dtype=torch.float32, device=dev)
+        self.targets = train_ops.AnchorTargets(self.A, h, w, dev)
+        self.db_raw = torch.empty((64,), dtype=torch.float32, device=dev)
+        self.repack()
+
+    # ---------------------------------------------------------------- weights: fold, then the forward engines' packers
+    def _repack_convs(self):
+        pr, x3 = self.precision, self.x3
+        for n, L in self.conv.items():
+            first = n == "trunk/conv1"
+            train_ops.fold_batchnorm(self.weights(n + "/W"), L["s"], L["wf"], b=self.weights(n + "/b") if first else None,
+                                     beta=L.get("beta"), mean=L.get("mean"), bf=L["bf"] if first else None)
+            if first:
+                fwd, dg = ops.pack_conv_weights_im2col_general(L["wf"], CONV1_KPAD, precision=pr), None
+            else:
+                fwd = ops.pack_conv_weights(L["wf"], cin_pad=L["cin"], precision=pr)
+                dg = train_ops.pack_conv_weights_dgrad(L["wf"], cout_pad=L["cout"], x3=x3)
+            self.packed[n] = (fwd, ops.pad_bias(L["bf"], L["cout"]), dg)
+        R = self.rpn_layer
+        w, b = self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b")
+        self.packed[R["name"]] = (ops.pack_conv_weights(w, cin_pad=R["cin"], precision=pr), ops.pad_bias(b, R["cout"]),
+                                  train_ops.pack_conv_weights_dgrad(w, cout_pad=R["cout"], x3=x3))
+
+    def folded_params(self):
+        """{conv name: (Wf, bf)} float32 numpy: the folded weights the device packed at the last repack."""
+        return {n: (L["wf"].cpu().numpy().copy(), L["bf"].cpu().numpy().copy()) for n, L in self.conv.items()}
+
+    # ---------------------------------------------------------------- forward
+    def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
+        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
+        if not (torch.is_tensor(x_chw) and x_chw.is_cuda and tuple(x_chw.shape) == (3, self.H, self.W)):
+            raise FrcnnError("ResNetRpnTrainer.forward: x_chw must be a (3, %d, %d) CUDA tensor" % (self.H, self.W))
+        if not (torch.is_tensor(gt_boxes) and gt_boxes.is_cuda and gt_boxes.dim() == 2 and gt_boxes.shape[1] == 5
+                and gt_boxes.shape[0] >= 1):
+            raise FrcnnError("ResNetRpnTrainer.forward: gt_boxes must be a (G >= 1, 5) CUDA tensor")
+        return super(ResNetRpnTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos)
+
+    def _forward_trunk(self, x_chw):
+        """ResNetForwardPlan._run_trunk's launches on the folded weights, with every activation kept."""
+        pk = self.packed
+        self.x_in.copy_(x_chw, non_blocking=True)
+        ops.pack_image_im2col_general(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col)
+        (hi, lo), b, _ = pk["trunk/conv1"]
+        ops.conv2d(self.x_col, hi, lo, b, 1, True, out=self.c1)
+        ops.maxpool3x3s2_ceil(self.c1, out=self.p1)
+        for B in self.blocks:
+            x = B["x"]
+            if B["stride"] == 2:
+                ops.subsample2x(x, out=B["xs"])
+                x = B["xs"]
+            (hi, lo), b, _ = pk[B["name"] + "/conv1"]
+            ops.conv2d(x, hi, lo, b, 1, True, out=B["y1"])
+            (hi, lo), b, _ = pk[B["name"] + "/conv2"]
+            ops.conv2d(B["y1"], hi, lo, b, 3, True, out=B["y2"])
+            if B["proj"]:
+                (hi, lo), b, _ = pk[B["name"] + "/conv4"]
+                ops.conv2d(x, hi, lo, b, 1, False, out=B["sc"])
+                res = B["sc"]
+            else:
+                res = B["x"]
+            (hi, lo), b, _ = pk[B["name"] + "/conv3"]
+            ops.conv2d_res(B["y2"], hi, lo, b, 1, True, res, out=B["out"])
+        self.feat = self.blocks[-1]["out"]
+        return self.feat
+
+    def input_of(self, B):
+        """The activation block B's conv1 and conv4 read: the subsampled input of a stride-2 block, else its input."""
+        return B["xs"] if B["stride"] == 2 else B["x"]
+
+    # ---------------------------------------------------------------- backward
+    def _dgrad(self, name, dy, ksize, cin, tag, res=None):
+        """The data gradient of `name` (its folded weights), plus `res` (frcnn_conv2d_res, relu = 0) when given."""
+        _, _, (dhi, dlo) = self.packed[name]
+        h, w, _ = dy.hi.shape
+        g = self._gact(h, w, cin, tag=tag)
+        if res is None:
+            ops.conv2d(dy, dhi, dlo, self.zero_bias, ksize, False, out=g)
+        else:
+            ops.conv2d_res(dy, dhi, dlo, self.zero_bias, ksize, False, res, out=g)
+        return g
+
+    def backward(self, debug=None):
+        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per conv
+        name, float32 (C,H,W) copies of the incoming gradient ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the
+        block output for conv3 / conv4, at the subsampled resolution when the next block reads it through the stride-2
+        subsample), the masked / routed gradient w.r.t. the (folded) conv output ("dy") and the data gradient the conv
+        passes on ("g_out"; for a block's conv1 the summed gradient of the block input, residual included)."""
+        dbg = (lambda a: a.to_chw_f32().clone()) if debug is not None else None      # noqa: E731
+        g = self._backward_heads(debug)
+        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
+        R = self.rpn_layer
+        fh, fw = self.fh, self.fw
+        dy = self._gact(fh, fw, 512)
+        dyT = self._tbuf(1, 512, fh, fw)
+        train_ops.grad_prepare(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
+        xT = self._tbuf(3, 2048, fh, fw)
+        train_ops.grad_prepare(fh, fw, 2048, g=self.feat, tbuf=xT)
+        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
+        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
+        g_in = g
+        g = self._dgrad(R["name"], dy, 3, 2048, tag=3)
+        if debug is not None:
+            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
+        # ---- the bottleneck blocks, last first; `half`: g is w.r.t. the stride-2 subsample of this block's output
+        half = False
+        for B in reversed(self.blocks):
+            g = self._backward_block(B, g, half, debug)
+            half = B["stride"] == 2
+        # ---- pool1 + conv1: g is w.r.t. p1
+        Ho, Wo = self.c1_hw
+        dz = self._gact(Ho, Wo, 64)
+        dzT = self._tbuf(1, 64, Ho, Wo)
+        train_ops.maxpool3x3s2_backward(g, self.c1, self.p1, out=dz, tbuf=dzT)
+        xT = self._tbuf(1, CONV1_KPAD, Ho, Wo)
+        train_ops.grad_prepare(Ho, Wo, CONV1_KPAD, g=self.x_col, tbuf=xT)
+        L = self.conv["trunk/conv1"]
+        dwc = torch.empty((64, CONV1_KPAD), dtype=torch.float32, device=self.device)
+        self._wgrad(dzT, xT, 64, CONV1_KPAD, 1, dwc, scale=L["s"])
+        # im2col column k = tap*3 + c  ->  OIHW [co][c][tap]
+        self.grads("trunk/conv1/W").copy_(dwc[:, :147].reshape(64, 49, 3).permute(0, 2, 1).reshape(64, 3, 7, 7))
+        train_ops.bias_grad(dzT, 64, self.db_raw)
+        train_ops.wgrad_reduce_scaled(self.db_raw.view(1, 1, 64, 1), 64, 1, L["s"], self.grads("trunk/conv1/b"))
+        if debug is not None:
+            debug["trunk/conv1"] = dict(g_in=dbg(g), dy=dbg(dz))
+
+    def _backward_block(self, B, g, half, debug):
+        """One bottleneck block's backward; g: gradient w.r.t. B["out"] (or its stride-2 subsample when `half`).  Returns
+        the gradient w.r.t. the block's conv input (B["xs"] for a stride-2 block, else B["x"])."""
+        dbg = lambda a: a.to_chw_f32().clone()        # noqa: E731
+        h, w, cin, mid, cout = B["H"], B["W"], B["cin"], B["mid"], B["cout"]
+        base = B["name"]
+        s = lambda i: self.conv["%s/conv%d" % (base, i)]["s"]       # noqa: E731
+        # dz: w.r.t. conv3's (folded) output and the shortcut, = g * (out > 0)
+        dz = self._gact(h, w, cout)
+        dzT = self._tbuf(1, cout, h, w, tag=1)
+        if half:
+            train_ops.grad_prepare_stride2(h, w, cout, g, y=B["out"], out=dz, tbuf=dzT)
+        else:
+            train_ops.grad_prepare(h, w, cout, g=g, y=B["out"], out=dz, tbuf=dzT)
+        # conv3 (1x1, mid -> cout)
+        y2T = self._tbuf(1, mid, h, w, tag=2)
+        train_ops.grad_prepare(h, w, mid, g=B["y2"], tbuf=y2T)
+        self._wgrad(dzT, y2T, cout, mid, 1, self.grads(base + "/conv3/W"), scale=s(3))
+        g2 = self._dgrad(base + "/conv3", dz, 1, mid, tag=1)
+        if debug is not None:
+            debug[base + "/conv3"] = dict(g_in=dbg(g), dy=dbg(dz), g_out=dbg(g2))
+        # conv2 (3x3, mid -> mid)
+        dy2 = self._gact(h, w, mid)
+        dyT = self._tbuf(1, mid, h, w)
+        train_ops.grad_prepare(h, w, mid, g=g2, y=B["y2"], out=dy2, tbuf=dyT)
+        if debug is not None:                              # g2's buffer receives g1 below
+            debug[base + "/conv2"] = dict(g_in=dbg(g2), dy=dbg(dy2))
+        y1T = self._tbuf(3, mid, h, w)
+        train_ops.grad_prepare(h, w, mid, g=B["y1"], tbuf=y1T)
+        self._wgrad(dyT, y1T, mid, mid, 9, self.grads(base + "/conv2/W"), scale=s(2))
+        g1 = self._dgrad(base + "/conv2", dy2, 3, mid, tag=1)
+        if debug is not None:
+            debug[base + "/conv2"]["g_out"] = dbg(g1)
+        # conv1 (1x1, cin -> mid) and conv4 (1x1, cin -> cout) on the same input
+        dy1 = self._gact(h, w, mid)
+        train_ops.grad_prepare(h, w, mid, g=g1, y=B["y1"], out=dy1, tbuf=dyT)
+        if debug is not None:
+            debug[base + "/conv1"] = dict(g_in=dbg(g1), dy=dbg(dy1))
+        xT = self._tbuf(1, cin, h, w, tag=3)
+        train_ops.grad_prepare(h, w, cin, g=self.input_of(B), tbuf=xT)
+        self._wgrad(dyT, xT, mid, cin, 1, self.grads(base + "/conv1/W"), scale=s(1))
+        if B["proj"]:
+            self._wgrad(dzT, xT, cout, cin, 1, self.grads(base + "/conv4/W"), scale=s(4))
+            res = self._dgrad(base + "/conv4", dz, 1, cin, tag=2)
+            if debug is not None:
+                debug[base + "/conv4"] = dict(g_in=dbg(g), dy=dbg(dz), g_out=dbg(res))
+        else:
+            res = dz
+        gx = self._dgrad(base + "/conv1", dy1, 1, cin, tag=3, res=res)
+        if debug is not None:
+            debug[base + "/conv1"]["g_out"] = dbg(gx)
+        return gx

@@ -39,6 +39,29 @@ class _ConvTrainer(object):
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                      extra_layers, extra_params, load_transform=None, lead=()):
+        layers = [dict(name="trunk/" + n, cin=ci, cout=co, k=3) for n, ci, co in TRUNK] + list(extra_layers)
+        self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          layers, extra_params, load_transform, lead)
+        # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools); `lead`: the
+        # leading [N] of a canvas trainer's activations
+        act, dev = self._act, self.device
+        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
+        self.x_col = act(H, W, 32)
+        h, w = H, W
+        for L in self.layers[:13]:
+            L["H"], L["W"] = h, w
+            L["y"] = act(h, w, L["cout"])
+            short = L["name"].split("/")[1]
+            L["pool"] = short in POOL_AFTER
+            if L["pool"]:
+                h, w = (h + 1) // 2, (w + 1) // 2
+                L["p"] = act(h, w, L["cout"])
+        self.fh, self.fw = h, w
+
+    def _init_params(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                     layers, extra_params, load_transform=None, lead=()):
+        """What every trainer shares: hyper-parameters, the flat float32 master / momentum / gradient buffers over `layers`
+        (W, then b unless the layer has bias=False) and `extra_params`, the activation allocator and the exchange state."""
         if precision not in ops.PRECISIONS:
             raise FrcnnError("precision must be one of %s" % (ops.PRECISIONS,))
         self.x3 = precision == "bf16x3"
@@ -49,11 +72,14 @@ class _ConvTrainer(object):
         self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
         self.A = int(self.anchors.shape[0])
         # ---- trainable parameters in the reference's naming; one flat fp32 master / momentum / gradient buffer
-        self.layers = [dict(name="trunk/" + n, cin=ci, cout=co, k=3) for n, ci, co in TRUNK] + list(extra_layers)
+        self.layers = layers
         names, shapes = [], []
         for L in self.layers:
-            names += [L["name"] + "/W", L["name"] + "/b"]
-            shapes += [(L["cout"], L["cin"], L["k"], L["k"]), (L["cout"],)]
+            names.append(L["name"] + "/W")
+            shapes.append((L["cout"], L["cin"], L["k"], L["k"]))
+            if L.get("bias", True):
+                names.append(L["name"] + "/b")
+                shapes.append((L["cout"],))
         for n, sh in extra_params:              # stored in the given order with NO padding (adjacent twin heads stay one matrix)
             names.append(n)
             shapes.append(tuple(sh))
@@ -70,8 +96,6 @@ class _ConvTrainer(object):
             if load_transform is not None:
                 src = load_transform(n, src)
             self.w_flat[o:o + sz] = torch.from_numpy(np.ascontiguousarray(src).reshape(-1)).to(dev)
-        # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools); `lead`: the
-        # leading [N] of a canvas trainer's activations
         x3 = self.x3
 
         def act(h, w, c):
@@ -79,18 +103,6 @@ class _ConvTrainer(object):
             return ops.Act(hi, torch.empty_like(hi) if x3 else None)
 
         self._act = act
-        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
-        self.x_col = act(H, W, 32)
-        h, w = H, W
-        for L in self.layers[:13]:
-            L["H"], L["W"] = h, w
-            L["y"] = act(h, w, L["cout"])
-            short = L["name"].split("/")[1]
-            L["pool"] = short in POOL_AFTER
-            if L["pool"]:
-                h, w = (h + 1) // 2, (w + 1) // 2
-                L["p"] = act(h, w, L["cout"])
-        self.fh, self.fw = h, w
         self.zero_bias = torch.zeros((32768,), dtype=torch.float32, device=dev)
         # gradient activations (NHWC) and transposed buffers, shared between layers of identical shape
         self._acts, self._tbufs = {}, {}
@@ -124,7 +136,7 @@ class RpnTrainer(_ConvTrainer):
         self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
         self.n_heads = 6 * self.A
         self.head_ld = ops.round_up(self.n_heads, 32)
-        R = self.layers[13]
+        R = self.rpn_layer = self.layers[13]
         R["H"], R["W"], R["pool"] = self.fh, self.fw, False
         R["y"] = self._act(self.fh, self.fw, 512)
         self.head_out = torch.empty((self.fh * self.fw, self.head_ld), dtype=torch.float32, device=self.device)
@@ -189,7 +201,7 @@ class RpnTrainer(_ConvTrainer):
         region_proposal_network.py:122-124; its output does not enter the RPN loss and is skipped.)"""
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
         x = self._forward_trunk(x_chw)
-        R = self.layers[13]
+        R = self.rpn_layer
         (hi, lo), b, _ = self.packed[R["name"]]
         ops.conv2d(x, hi, lo, b, 3, True, out=R["y"])
         (hi, lo), b, _ = self.packed["heads"]
@@ -255,8 +267,9 @@ class RpnTrainer(_ConvTrainer):
         s = max(1, (target + tiles - 1) // tiles)
         return int(min(s, max(1, kb_total // 8)))
 
-    def _wgrad(self, dyT, xT, M, N, groups, dw, m_out=None):
-        """dw (flat view) = sum_pixels dY (x) X over the padded pixel axis; dyT: TBuf 1 plane [M_parts, Kp]; xT: TBuf."""
+    def _wgrad(self, dyT, xT, M, N, groups, dw, m_out=None, scale=None):
+        """dw (flat view) = sum_pixels dY (x) X over the padded pixel axis; dyT: TBuf 1 plane [M_parts, Kp]; xT: TBuf.
+        scale: float64 [M] per-output-channel factor (a frozen BatchNorm's s), applied in the fixed-order reduction."""
         K = dyT.hi.shape[-1]                    # N*Kp: a canvas sums its N images in the one GEMM
         a_hi, a_lo = dyT.hi[0], (dyT.lo[0] if dyT.lo is not None else None)
         if groups == 9:
@@ -266,14 +279,23 @@ class RpnTrainer(_ConvTrainer):
             b_hi, b_lo = xT.hi[pl], (xT.lo[pl] if xT.lo is not None else None)
         parts = train_ops.gemm_nt_splitk(a_hi, a_lo, b_hi, b_lo, groups=groups, row_stride=dyT.Wp,
                                          splits=self._splits(groups, M, N, K // 64))
-        train_ops.wgrad_reduce(parts, m_out or M, N, dw)
+        if scale is None:
+            train_ops.wgrad_reduce(parts, m_out or M, N, dw)
+        else:
+            train_ops.wgrad_reduce_scaled(parts, m_out or M, N, scale, dw)
 
     def backward(self, debug=None):
         """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per
         layer name, float32 (C,H,W) copies of the incoming gradient ("g_in"), the masked / routed gradient ("dy") and the
         data gradient the layer passes on ("g_out") -- the buffers themselves are reused from layer to layer."""
+        g = self._backward_heads(debug)
+        # ---- RPN 3x3 conv, then the trunk, last layer first
+        self._backward_chain([self.layers[13]] + self.layers[12::-1], g, debug)
+
+    def _backward_heads(self, debug=None):
+        """The twin 1x1 heads' weight / bias gradients; returns the gradient w.r.t. the RPN 3x3 conv's post-ReLU output."""
         fh, fw, ld = self.fh, self.fw, self.head_ld
-        R = self.layers[13]
+        R = self.rpn_layer
         # ---- twin 1x1 heads: dY = head_grad [fh*fw, ld] fp32 (columns >= 6A are zero)
         dyh = self._gact(fh, fw, ld)
         dyhT = self._tbuf(1, ld, fh, fw)
@@ -287,8 +309,7 @@ class RpnTrainer(_ConvTrainer):
         ops.conv2d(dyh, dhi, dlo, self.zero_bias, 1, False, out=g)
         if debug is not None:
             debug["heads"] = dict(dy=dyh.to_chw_f32().clone(), g_out=g.to_chw_f32().clone())
-        # ---- RPN 3x3 conv, then the trunk, last layer first
-        self._backward_chain([R] + self.layers[12::-1], g, debug)
+        return g
 
     def _backward_chain(self, chain, g, debug=None):
         """g: gradient (ops.Act) w.r.t. the post-ReLU output of chain[0] -- at pooled resolution if that layer is followed

@@ -7,7 +7,8 @@ stream in, tensors out, no CPU path.
 Replaces models/bbox.pyx:16-56, models/anchor_target_layer.py:66-198 and the two loss functions of
 models/region_proposal_network.py:160-204 (all under /root/reference); the second half wraps the conv-backward entry
 points (frcnn_gemm_nt_splitk, frcnn_grad_prepare, frcnn_wgrad_reduce, frcnn_bias_grad, frcnn_sgd_momentum,
-frcnn_pack_conv_weights_dgrad) used by train_engine.py.
+frcnn_pack_conv_weights_dgrad) used by train_engine.py, and those the ResNet trunk adds (frcnn_maxpool3x3s2_backward,
+frcnn_grad_prepare_stride2, frcnn_fold_batchnorm, frcnn_wgrad_reduce_scaled) used by resnet_train.py.
 """
 import ctypes
 
@@ -266,6 +267,55 @@ def grad_prepare_batch(N, H, W, C, g=None, g_f32=None, y=None, p=None, out=None,
         _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
         _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None,
         tbuf.planes if tbuf is not None else 1, 1 if times2 else 0, _stream()), "frcnn_grad_prepare_batch")
+
+
+def maxpool3x3s2_backward(g, y, p, out=None, tbuf=None):
+    """frcnn_maxpool3x3s2_backward: the pooled gradient g and pooled map p (Acts [h, w, C]) routed back to the 3x3/2
+    cover_all windows of y (Act [H, W, C], the post-ReLU pool input) and masked by y > 0; out: Act [H, W, C] (optional),
+    tbuf: TBuf with planes = 1 (optional)."""
+    H, W, C = y.hi.shape
+    ph, pw = (H - 2) // 2 + 1, (W - 2) // 2 + 1
+    for name, a in (("g", g), ("p", p)):
+        if tuple(a.hi.shape) != (ph, pw, C):
+            raise FrcnnError("maxpool3x3s2_backward: %s must be [%d, %d, %d], got %s" % (name, ph, pw, C, tuple(a.hi.shape)))
+    if tbuf is not None and tbuf.planes != 1:
+        raise FrcnnError("maxpool3x3s2_backward: the transposed buffer must have 1 plane")
+    check(_lib.load().frcnn_maxpool3x3s2_backward(
+        _p(g.hi), _p(g.lo), _p(y.hi), _p(y.lo), _p(p.hi), _p(p.lo), int(H), int(W), int(C),
+        _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
+        _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None, _stream()),
+        "frcnn_maxpool3x3s2_backward")
+
+
+def grad_prepare_stride2(H, W, C, g, y=None, out=None, tbuf=None):
+    """frcnn_grad_prepare_stride2: g (Act [ceil(H/2), ceil(W/2), C]) placed at the even pixels of an H x W map, zero
+    elsewhere, masked by y > 0 when y (Act [H, W, C]) is given; out / tbuf as in grad_prepare."""
+    if tuple(g.hi.shape) != ((H + 1) // 2, (W + 1) // 2, C):
+        raise FrcnnError("grad_prepare_stride2: g must be [%d, %d, %d], got %s" % ((H + 1) // 2, (W + 1) // 2, C, tuple(g.hi.shape)))
+    check(_lib.load().frcnn_grad_prepare_stride2(
+        _p(g.hi), _p(g.lo), _p(y.hi) if y is not None else None, _p(y.lo) if y is not None else None, int(H), int(W), int(C),
+        _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
+        _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None,
+        tbuf.planes if tbuf is not None else 1, _stream()), "frcnn_grad_prepare_stride2")
+
+
+def fold_batchnorm(w, s, wf, b=None, beta=None, mean=None, bf=None):
+    """frcnn_fold_batchnorm: wf = f32(f64(w) * s[co]) (w, wf float32 [Cout, ...], s float64 [Cout]); bf (optional, float32
+    [Cout]) = f32(f64(beta) + (f64(b) - f64(mean)) * s), b = 0 when None."""
+    Cout = int(w.shape[0])
+    per_out = w.numel() // Cout
+    if wf.shape != w.shape or wf.dtype != torch.float32 or s.dtype != torch.float64 or s.numel() != Cout:
+        raise FrcnnError("fold_batchnorm: w / wf float32 of one shape and s float64 [Cout] needed")
+    check(_lib.load().frcnn_fold_batchnorm(_p(w), _p(s), Cout, per_out, _p(b), _p(beta), _p(mean), _p(wf), _p(bf), _stream()),
+          "frcnn_fold_batchnorm")
+    return wf
+
+
+def wgrad_reduce_scaled(parts, M, N, s, dw):
+    """parts [groups, S, M_parts, ld] -> dw (flat fp32 view, OIHW order) = f32(s[m] * fixed-order split sum), s float64 [>= M]."""
+    groups, S, Mp, ld = parts.shape
+    check(_lib.load().frcnn_wgrad_reduce_scaled(_p(parts), groups, S, Mp, int(M), ld, int(N), _p(s), _p(dw), _stream()),
+          "frcnn_wgrad_reduce_scaled")
 
 
 def wgrad_reduce(parts, M, N, dw, scale=1.0):

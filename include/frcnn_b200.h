@@ -838,6 +838,36 @@ int frcnn_grad_prepare_batch(const void* g_hi, const void* g_lo, const float* g_
                              const void* y_lo, const void* p_hi, const void* p_lo, int N, int H, int W, int C, void* o_hi,
                              void* o_lo, void* t_hi, void* t_lo, int planes, int times2, void* stream);
 
+/* The two re-layouts the ResNet trunk's backward adds (frcnn_grad_prepare's outputs, N = 1, bit-exact rules restated by
+ * tests/resnet_train_ref.py):
+ *   frcnn_maxpool3x3s2_backward  F.max_pooling_2d(3, stride=2, pad=0, cover_all=True) backward fused with the ReLU mask of
+ *       its input: g and p [pool3s2_out(H)][pool3s2_out(W)][C] (the pooled gradient and the pooled map), y [H][W][C] the
+ *       post-ReLU pool input, H, W >= 2.  Window (i, j) covers rows [2i, min(2i+3, H)) x columns [2j, min(2j+3, W)) and sends
+ *       g[i][j] to the FIRST element in scan order whose value equals p[i][j]; pairs are read as DESIGN §2 reads them (an
+ *       infinite hi stands alone) and compared as floats (+0 == -0, NaN equals nothing).  A pixel sums what its (up to four)
+ *       windows send, in fp32 in ascending (i, j) order from +0; the sum is kept where y > 0 (hi read as int16 in
+ *       (0, +inf]), +0 elsewhere, and re-split into hi/lo.  Transposed output: planes = 1.
+ *   frcnn_grad_prepare_stride2   the backward of frcnn_subsample2x: the source g [ceil(H/2)][ceil(W/2)][C] at pixels (2i, 2j)
+ *       of the H x W map and 0 everywhere else, then the optional y > 0 mask as in frcnn_grad_prepare (kept pairs keep their
+ *       words); transposed output with planes = 1 or 3. */
+int frcnn_maxpool3x3s2_backward(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, const void* p_hi,
+                                const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo, void* stream);
+int frcnn_grad_prepare_stride2(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, int H, int W, int C,
+                               void* o_hi, void* o_lo, void* t_hi, void* t_lo, int planes, void* stream);
+
+/* ---- frozen BatchNorm in training (resnet_train.cu).  A convolution and its frozen BN are the folded convolution
+ * Wf = W*s, bf = beta + (b - mean)*s, s = gamma/sqrt(var + eps) (float64, per output channel).
+ *   frcnn_fold_batchnorm       wf[i] = f32(f64(w[i]) * s[i / per_out]) for Cout*per_out weights; bf (optional) [Cout] =
+ *                              f32(f64(beta) + (f64(b) - f64(mean)) * s), b = 0 when NULL -- resnet_engine.fold_batchnorm's
+ *                              arithmetic, bit for bit.
+ *   frcnn_wgrad_reduce_scaled  frcnn_wgrad_reduce with a per-output-channel float64 scale instead of the scalar one:
+ *                              dw[m][n][g] = f32(f64(s[m]) * f64(fp32 sum over splits s = 0, 1, ... of parts[g][s][m][n])).
+ *                              With groups = splits = N = ld = 1 and parts = a bias sum [M] it scales a bias gradient. */
+int frcnn_fold_batchnorm(const float* w, const double* s, int Cout, long per_out, const float* b, const float* beta,
+                         const float* mean, float* wf, float* bf, void* stream);
+int frcnn_wgrad_reduce_scaled(const float* parts, int groups, int splits, int M_parts, int M, int ld, int N, const double* s,
+                              float* dw, void* stream);
+
 /* dw[m][n][g] (the reference's OIHW float32, g = r*3+s or 1) = scale * sum over splits of parts[g][s][m][n], m < M;
  * parts slabs have M_parts >= M rows of ld floats. */
 int frcnn_wgrad_reduce(const float* parts, int groups, int splits, int M_parts, int M, int ld, int N, float scale, float* dw,
