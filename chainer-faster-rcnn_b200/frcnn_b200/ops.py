@@ -462,12 +462,14 @@ def pack_image_im2col_general(x_chw, ksize, stride, pad, k_pad, precision="bf16x
     return out
 
 
-def pack_conv_weights_im2col_general(w, k_pad, precision="bf16x3"):
-    """OIHW float32 -> ([1, Cout, k_pad] bf16 hi, lo or None) in the K order of pack_image_im2col_general."""
+def pack_conv_weights_im2col_general(w, k_pad, precision="bf16x3", out=None):
+    """OIHW float32 -> ([1, Cout, k_pad] bf16 hi, lo or None) in the K order of pack_image_im2col_general.  out: an earlier
+    result to overwrite in place."""
     w = w.contiguous().float()
     Cout, Cin, kh, kw = w.shape
-    hi = torch.empty((1, Cout, k_pad), dtype=torch.bfloat16, device=w.device)
-    lo = torch.empty_like(hi) if precision == "bf16x3" else None
+    hi, lo = out if out is not None else (torch.empty((1, Cout, k_pad), dtype=torch.bfloat16, device=w.device), None)
+    if out is None and precision == "bf16x3":
+        lo = torch.empty_like(hi)
     check(_lib.load().frcnn_pack_conv_weights_im2col(_p(w), None, Cout, Cin, kh, k_pad, _p(hi), _p(lo), _stream()),
           "frcnn_pack_conv_weights_im2col")
     return hi, lo

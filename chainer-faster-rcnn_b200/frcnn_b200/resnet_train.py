@@ -32,7 +32,7 @@ import torch
 from . import ops, train_ops
 from ._lib import FrcnnError
 from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
-from .train_engine import RpnTrainer
+from .train_engine import RpnTrainer, _rpn_params
 
 SUBSAMPLE_MODES = ("device", "numpy", "none")
 
@@ -79,21 +79,16 @@ class ResNetRpnTrainer(RpnTrainer):
         for _, bn, _, co, _ in convs:
             for f in ("gamma", "beta", "avg_mean", "avg_var"):
                 need["%s/%s" % (bn, f)] = (co,)
-        need.update({"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,), "RPN/rpn_cls_score/W": (2 * A, 512, 1, 1),
-                     "RPN/rpn_cls_score/b": (2 * A,), "RPN/rpn_bbox_pred/W": (4 * A, 512, 1, 1), "RPN/rpn_bbox_pred/b": (4 * A,)})
+        need.update({"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)})
+        need.update(_rpn_params(A))
         for k, sh in need.items():
             if k not in params or tuple(np.shape(params[k])) != sh:
                 raise FrcnnError("ResNetRpnTrainer: parameter %s must have shape %s (got %s)"
                                  % (k, sh, None if k not in params else tuple(np.shape(params[k]))))
         layers = [dict(name=n, bn=bn, cin=ci, cout=co, k=k, bias=n == "trunk/conv1") for n, bn, ci, co, k in convs]
         layers.append(dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3))
-        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
-        extra = [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
         self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          layers, extra)
-        self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
-        self.n_heads = 6 * self.A
-        self.head_ld = ops.round_up(self.n_heads, 32)
+                          layers, _rpn_params(A))
         dev = self.device
         # ---- frozen BN: s (float64) per conv, the constant folded bias of every conv but conv1, the folded-weight buffers
         T = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)     # noqa: E731
@@ -133,31 +128,23 @@ class ResNetRpnTrainer(RpnTrainer):
             self.blocks.append(B)
             x = B["out"]
         self.fh, self.fw = h, w
-        R = self.rpn_layer = layers[-1]
-        R["H"], R["W"], R["pool"] = h, w, False
-        R["y"] = act(h, w, 512)
-        self.head_out = torch.empty((h * w, self.head_ld), dtype=torch.float32, device=dev)
+        self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self.targets = train_ops.AnchorTargets(self.A, h, w, dev)
         self.db_raw = torch.empty((64,), dtype=torch.float32, device=dev)
         self.repack()
 
     # ---------------------------------------------------------------- weights: fold, then the forward engines' packers
+    def _pack_image_layer(self, w, out=None):
+        return ops.pack_conv_weights_im2col_general(w, CONV1_KPAD, precision=self.precision, out=out)
+
     def _repack_convs(self):
-        pr, x3 = self.precision, self.x3
         for n, L in self.conv.items():
             first = n == "trunk/conv1"
             train_ops.fold_batchnorm(self.weights(n + "/W"), L["s"], L["wf"], b=self.weights(n + "/b") if first else None,
                                      beta=L.get("beta"), mean=L.get("mean"), bf=L["bf"] if first else None)
-            if first:
-                fwd, dg = ops.pack_conv_weights_im2col_general(L["wf"], CONV1_KPAD, precision=pr), None
-            else:
-                fwd = ops.pack_conv_weights(L["wf"], cin_pad=L["cin"], precision=pr)
-                dg = train_ops.pack_conv_weights_dgrad(L["wf"], cout_pad=L["cout"], x3=x3)
-            self.packed[n] = (fwd, ops.pad_bias(L["bf"], L["cout"]), dg)
+            self._repack(n, L["wf"], L["bf"], L["cout"], first=first, cin_pad=L["cin"])
         R = self.rpn_layer
-        w, b = self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b")
-        self.packed[R["name"]] = (ops.pack_conv_weights(w, cin_pad=R["cin"], precision=pr), ops.pad_bias(b, R["cout"]),
-                                  train_ops.pack_conv_weights_dgrad(w, cout_pad=R["cout"], x3=x3))
+        self._repack(R["name"], self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b"), R["cout"], cin_pad=R["cin"])
 
     def folded_params(self):
         """{conv name: (Wf, bf)} float32 numpy: the folded weights the device packed at the last repack."""

@@ -34,8 +34,10 @@ POOL_AFTER = {s.name for s in _STEPS if s.pool_after}
 
 
 class _ConvTrainer(object):
-    """Shared by RpnTrainer / RcnnTrainer: flat float32 master / momentum / gradient buffers, the 13 trunk layers with
-    their stored activations, weight (re)packing, the trunk forward, the generic conv-backward chain and the optimizer."""
+    """Shared by every trainer: flat float32 master / momentum / gradient buffers, the 13 trunk layers with their stored
+    activations, and the launch layer over one image -- _conv, _prep, _pool, _chw, the cached gradient buffers and the
+    in-place repack.  _CanvasSteps overrides the launches for a canvas, so every step is written once."""
+    halvings = None             # the feature map's canvas level (the VGG16 trunk's: set by _init_common)
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                      extra_layers, extra_params, load_transform=None, lead=()):
@@ -43,20 +45,20 @@ class _ConvTrainer(object):
         self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           layers, extra_params, load_transform, lead)
         # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools); `lead`: the
-        # leading [N] of a canvas trainer's activations
+        # leading [N] of a canvas trainer's activations; on a canvas a layer's extents are ceil(extent / 2^halvings)
         act, dev = self._act, self.device
         self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
         self.x_col = act(H, W, 32)
-        h, w = H, W
+        h, w, halvings = H, W, 0
         for L in self.layers[:13]:
-            L["H"], L["W"] = h, w
+            L["H"], L["W"], L["halvings"] = h, w, halvings
             L["y"] = act(h, w, L["cout"])
             short = L["name"].split("/")[1]
             L["pool"] = short in POOL_AFTER
             if L["pool"]:
-                h, w = (h + 1) // 2, (w + 1) // 2
+                h, w, halvings = (h + 1) // 2, (w + 1) // 2, halvings + 1
                 L["p"] = act(h, w, L["cout"])
-        self.fh, self.fw = h, w
+        self.fh, self.fw, self.halvings = h, w, halvings
 
     def _init_params(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                      layers, extra_params, load_transform=None, lead=()):
@@ -103,6 +105,7 @@ class _ConvTrainer(object):
             return ops.Act(hi, torch.empty_like(hi) if x3 else None)
 
         self._act = act
+        self._slots = int(lead[0]) if lead else 1           # images per step
         self.zero_bias = torch.zeros((32768,), dtype=torch.float32, device=dev)
         # gradient activations (NHWC) and transposed buffers, shared between layers of identical shape
         self._acts, self._tbufs = {}, {}
@@ -121,27 +124,74 @@ class _ConvTrainer(object):
         self.n_updates = 0                  # optimizer steps taken (the drop-in model syncs its Link params when this moves)
         self._ev_bwd = self._ev_comm = None
 
+    # ---------------------------------------------------------------- launches over one image (_CanvasSteps: a canvas)
+    def _conv(self, x, planes, bias, ksize, relu, at, **kw):
+        """frcnn_conv2d.  at: where the rows live -- a trunk level given by its halvings (nothing to pass for one image),
+        "rois": the head's forward, which computes the first prop.count rows, or "roi_grads": the head's data gradients."""
+        if at == "rois":
+            kw["m_valid"] = self.prop.count
+        return ops.conv2d(x, planes[0], planes[1], bias, ksize, relu, **kw)
+
+    def _prep(self, h, w, c, **kw):
+        train_ops.grad_prepare(h, w, c, **kw)
+
+    def _pool(self, y, out):
+        ops.maxpool2x2_ceil(y, out=out)
+
+    def _chw(self, act):
+        """float32 (C,H,W) copy of an Act (debug)."""
+        return act.to_chw_f32()
+
+    def _gact(self, h, w, c, tag=0):
+        """A gradient activation, shared between layers of identical shape and tag."""
+        key = (h, w, c, tag)
+        if key not in self._acts:
+            self._acts[key] = self._act(h, w, c)
+        return self._acts[key]
+
+    def _tbuf(self, planes, c, h, w, tag=0):
+        key = (planes, c, h, w, tag)
+        if key not in self._tbufs:
+            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3, N=self._slots)
+        return self._tbufs[key]
+
+    # ---------------------------------------------------------------- weights: repacked in place from the fp32 masters
+    def _pack_image_layer(self, w, out=None):
+        """The first convolution's planes, in the K order of the trunk's im2col input."""
+        return ops.pack_conv_weights_im2col(w, precision=self.precision, out=out)
+
+    def _repack(self, name, w, b, cout_pad, first=False, cin_pad=None):
+        """packed[name] = (forward planes, padded bias, data-gradient planes or None for the first layer), overwriting the
+        earlier tensors: a captured graph, and whoever else holds them, reads the new weights."""
+        old = self.packed.get(name)
+        if first:
+            fwd, dg = self._pack_image_layer(w, out=old and old[0]), None
+        else:
+            fwd = ops.pack_conv_weights(w, cin_pad=cin_pad, precision=self.precision, out=old and old[0])
+            dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=cout_pad, x3=self.x3, out=old and old[2])
+        self.packed[name] = (fwd, ops.pad_bias(b, cout_pad, out=old and old[1]), dg)
+
 
 class RpnTrainer(_ConvTrainer):
     """Weights, optimizer state and buffers of the RPN-mode training step for one image shape."""
 
     def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
-        A = len(anchors)
-        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
-        # the twin heads are stored adjacently so that (W_cls | W_bbox) is ONE [6A, 512] matrix: cls W, bbox W, cls b, bbox b
-        extra = [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], extra)
+                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], _rpn_params(len(anchors)))
+        self._init_rpn_head(loss_lambda, delta, subsample, seed)
+        self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
+        self.repack()
+
+    def _init_rpn_head(self, loss_lambda, delta, subsample, seed):
+        """The RPN step's loss settings, its 3x3 conv (the last layer) at the feature map and the twin heads' output."""
         self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
         self.n_heads = 6 * self.A
         self.head_ld = ops.round_up(self.n_heads, 32)
-        R = self.rpn_layer = self.layers[13]
-        R["H"], R["W"], R["pool"] = self.fh, self.fw, False
+        R = self.rpn_layer = self.layers[-1]
+        R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, self.halvings
         R["y"] = self._act(self.fh, self.fw, 512)
-        self.head_out = torch.empty((self.fh * self.fw, self.head_ld), dtype=torch.float32, device=self.device)
-        self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
-        self.repack()
+        self.head_out = torch.empty((self._slots * self.fh * self.fw, self.head_ld), dtype=torch.float32, device=self.device)
 
     # ---------------------------------------------------------------- views
     def view(self, flat, name):
@@ -162,37 +212,15 @@ class RpnTrainer(_ConvTrainer):
         o, _, _ = self.index["RPN/rpn_cls_score/b"]
         return flat[o:o + self.n_heads]
 
-    def _gact(self, h, w, c, tag=0):
-        key = (h, w, c, tag)
-        if key not in self._acts:
-            hi = torch.empty((h, w, c), dtype=torch.bfloat16, device=self.device)
-            self._acts[key] = ops.Act(hi, torch.empty_like(hi) if self.x3 else None)
-        return self._acts[key]
-
-    def _tbuf(self, planes, c, h, w, tag=0):
-        key = (planes, c, h, w, tag)
-        if key not in self._tbufs:
-            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3)
-        return self._tbufs[key]
-
     # ---------------------------------------------------------------- weight (re)packing from the fp32 masters
     def _repack_convs(self):
         for i, L in enumerate(self.layers):
-            w, b = self.weights(L["name"] + "/W"), self.weights(L["name"] + "/b")
-            if i == 0:
-                fwd = ops.pack_conv_weights_im2col(w, precision=self.precision)
-                dg = None                                                   # the image needs no gradient
-            else:
-                fwd = ops.pack_conv_weights(w, cin_pad=L["cin"], precision=self.precision)
-                dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=L["cout"], x3=self.x3)
-            self.packed[L["name"]] = (fwd, ops.pad_bias(b, L["cout"]), dg)
+            name = L["name"]
+            self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
 
     def repack(self):
         self._repack_convs()
-        wh, bh = self._heads_w(self.w_flat), self._heads_b(self.w_flat)
-        fwd = ops.pack_conv_weights(wh, precision=self.precision)
-        dg = train_ops.pack_conv_weights_dgrad(wh, cout_pad=self.head_ld, x3=self.x3)     # [1, 512, head_ld]
-        self.packed["heads"] = (fwd, ops.pad_bias(bh, self.head_ld), dg)
+        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- forward
     def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
@@ -200,12 +228,9 @@ class RpnTrainer(_ConvTrainer):
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss.  (The reference also runs the ProposalLayer here,
         region_proposal_network.py:122-124; its output does not enter the RPN loss and is skipped.)"""
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
-        x = self._forward_trunk(x_chw)
         R = self.rpn_layer
-        (hi, lo), b, _ = self.packed[R["name"]]
-        ops.conv2d(x, hi, lo, b, 3, True, out=R["y"])
-        (hi, lo), b, _ = self.packed["heads"]
-        ops.conv2d(R["y"], hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out)
+        self._rpn_forward(self._forward_trunk(x_chw), self.packed[R["name"]], self.packed["heads"], R["y"], self.head_ld,
+                          self.head_out)
         if disable_pos is None and self.subsample == "numpy":
             disable_pos = self._numpy_subsample(gt_boxes, im_h, im_w)
         if disable_pos is not None:
@@ -244,20 +269,30 @@ class RpnTrainer(_ConvTrainer):
             disable.append(np.random.choice(bg_inds, size=int(len(bg_inds) - num_bg), replace=False))
         return torch.from_numpy(np.concatenate(disable).astype(np.int32)).to(self.device)
 
-    def _forward_trunk(self, x_chw):
-        """The 13 VGG16 convolutions with every output kept (pools un-fused: backward needs the un-pooled maps)."""
+    def _pack_input(self, x_chw):
+        """The trunk's first launch: the image into the first layer's im2col planes x_col."""
         self.x_in.copy_(x_chw, non_blocking=True)
         ops.pack_image_im2col(self.x_in, out=self.x_col)
+
+    def _forward_trunk(self, x_chw=None):
+        """The 13 VGG16 convolutions with every output kept (pools un-fused: backward needs the un-pooled maps)."""
+        self._pack_input(x_chw)
         x = self.x_col
         for i, L in enumerate(self.layers[:13]):
-            (hi, lo), b, _ = self.packed[L["name"]]
-            ops.conv2d(x, hi, lo, b, 1 if i == 0 else 3, True, out=L["y"])
+            fwd, b, _ = self.packed[L["name"]]
+            self._conv(x, fwd, b, 1 if i == 0 else 3, True, L["halvings"], out=L["y"])
             x = L["y"]
             if L["pool"]:
-                ops.maxpool2x2_ceil(L["y"], out=L["p"])
+                self._pool(L["y"], out=L["p"])
                 x = L["p"]
         self.feat = x
         return x
+
+    def _rpn_forward(self, x, conv, heads, mid, ld, out):
+        """An RPN on the feature map x: its 3x3 conv + ReLU into `mid`, its twin 1x1 heads into the fp32 [rows, ld] `out`.
+        conv / heads: (planes, bias, ...) -- the trained layers' `packed` entries or the RCNN step's frozen ones."""
+        self._conv(x, conv[0], conv[1], 3, True, self.halvings, out=mid)
+        self._conv(mid, heads[0], heads[1], 1, False, self.halvings, out_act=False, ld_f32=ld, out_f32=out)
 
     # ---------------------------------------------------------------- backward
     def _splits(self, groups, M, N, kb_total):
@@ -285,9 +320,10 @@ class RpnTrainer(_ConvTrainer):
             train_ops.wgrad_reduce_scaled(parts, m_out or M, N, scale, dw)
 
     def backward(self, debug=None):
-        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per
-        layer name, float32 (C,H,W) copies of the incoming gradient ("g_in"), the masked / routed gradient ("dy") and the
-        data gradient the layer passes on ("g_out") -- the buffers themselves are reused from layer to layer."""
+        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter (on a canvas: the sum over the slots).
+        debug: a dict that receives, per layer name, float32 (C,H,W) copies ([N,C,H,W] on a canvas) of the incoming
+        gradient ("g_in"), the masked / routed gradient ("dy") and the data gradient the layer passes on ("g_out") -- the
+        buffers themselves are reused from layer to layer."""
         g = self._backward_heads(debug)
         # ---- RPN 3x3 conv, then the trunk, last layer first
         self._backward_chain([self.layers[13]] + self.layers[12::-1], g, debug)
@@ -299,49 +335,48 @@ class RpnTrainer(_ConvTrainer):
         # ---- twin 1x1 heads: dY = head_grad [fh*fw, ld] fp32 (columns >= 6A are zero)
         dyh = self._gact(fh, fw, ld)
         dyhT = self._tbuf(1, ld, fh, fw)
-        train_ops.grad_prepare(fh, fw, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
+        self._prep(fh, fw, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
         midT = self._tbuf(3, 512, fh, fw)
-        train_ops.grad_prepare(fh, fw, 512, g=R["y"], tbuf=midT)
+        self._prep(fh, fw, 512, g=R["y"], tbuf=midT)
         self._wgrad(dyhT, midT, ld, 512, 1, self._heads_w(self.g_flat), m_out=self.n_heads)
         train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
-        _, _, (dhi, dlo) = self.packed["heads"]
         g = self._gact(fh, fw, 512, tag=1)
-        ops.conv2d(dyh, dhi, dlo, self.zero_bias, 1, False, out=g)
+        self._conv(dyh, self.packed["heads"][2], self.zero_bias, 1, False, self.halvings, out=g)
         if debug is not None:
-            debug["heads"] = dict(dy=dyh.to_chw_f32().clone(), g_out=g.to_chw_f32().clone())
+            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
         return g
 
     def _backward_chain(self, chain, g, debug=None):
         """g: gradient (ops.Act) w.r.t. the post-ReLU output of chain[0] -- at pooled resolution if that layer is followed
-        by a pool.  Per layer: ReLU / pool backward + re-layout, weight + bias gradient, data gradient for the next one."""
+        by a pool.  Per layer: ReLU / pool backward + re-layout, weight + bias gradient, data gradient for the next one.
+        On a canvas the weight gradients run over K = N*Kp, the sum over the slots."""
         for L in chain:
             h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
             first = L is self.layers[0]
             dy = self._gact(h, w, co)
             dyT = self._tbuf(1, co, h, w)
-            train_ops.grad_prepare(h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
+            self._prep(h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
             if debug is not None:
-                debug[L["name"]] = dict(g_in=g.to_chw_f32().clone(), dy=dy.to_chw_f32().clone())
+                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
             x = self._input_of(L)
             if first:
                 xT = self._tbuf(1, 32, h, w)
-                train_ops.grad_prepare(h, w, 32, g=x, tbuf=xT)
+                self._prep(h, w, 32, g=x, tbuf=xT)
                 dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
                 self._wgrad(dyT, xT, co, 32, 1, dwc)
                 # im2col column k = tap*3 + c  ->  OIHW [co][c][tap]
                 self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
             else:
                 xT = self._tbuf(3, ci, h, w)
-                train_ops.grad_prepare(h, w, ci, g=x, tbuf=xT)
+                self._prep(h, w, ci, g=x, tbuf=xT)
                 self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
             train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
             self._early_exchange(L["name"])
             if not first:
-                _, _, (dhi, dlo) = self.packed[L["name"]]
                 g = self._gact(h, w, ci, tag=1)
-                ops.conv2d(dy, dhi, dlo, self.zero_bias, 3, False, out=g)
+                self._conv(dy, self.packed[L["name"]][2], self.zero_bias, 3, False, L["halvings"], out=g)
                 if debug is not None:
-                    debug[L["name"]]["g_out"] = g.to_chw_f32().clone()
+                    debug[L["name"]]["g_out"] = self._chw(g)
 
     def _input_of(self, L):
         i = self.layers.index(L)
@@ -425,6 +460,13 @@ class RpnTrainer(_ConvTrainer):
         return losses
 
 
+def _rpn_params(A):
+    """The RPN heads' parameters in flat-buffer order, stored adjacently so that (W_cls | W_bbox) is ONE [6A, 512] matrix:
+    cls W, bbox W, cls b, bbox b."""
+    heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
+    return [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
+
+
 def _rcnn_params(nc):
     """The head parameters of the RCNN step in flat-buffer order (cls_score | bbox_pred adjacent: one [5*nc, 4096] matrix)."""
     heads = [("cls_score", nc), ("bbox_pred", 4 * nc)]
@@ -454,37 +496,40 @@ class RcnnTrainer(RpnTrainer):
         nc = self.num_classes = num_classes
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [], _rcnn_params(nc), load_transform=_fc6_to_hwc)
-        self.delta, self.sample, self.dropout = delta, sample, dropout
-        self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
-        self.n_heads = 5 * nc
-        self.head_ld = ops.round_up(self.n_heads, 32)
-        dev = self.device
-        self.gen = torch.Generator(device=dev)
+        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+        self.sample, self.dropout = sample, dropout
+        self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
-        self._frozen_rpn(params)
-        fh, fw = self.fh, self.fw
-        self.rpn_mid = self._act(fh, fw, 512)
-        self.rpn_out = torch.empty((fh * fw, self.rpn_ld), dtype=torch.float32, device=dev)
-        self.prop = ops.ProposalWorkspace(self.A, fh, fw, pre_n, post_n, dev)
-        # head activations
-        self.pool5 = self._act(1, post_n, 49 * 512)
-        self.fc6 = self._act(1, post_n, 4096)
-        self.fc7 = self._act(1, post_n, 4096)
-        self.head_out = torch.empty((post_n, self.head_ld), dtype=torch.float32, device=dev)
-        self.dfeat = torch.empty((fh * fw, 512), dtype=torch.float32, device=dev)
+        self.prop = ops.ProposalWorkspace(self.A, self.fh, self.fw, pre_n, post_n, self.device)
         self.roi_ws = None
         self.repack()
 
+    def _init_rcnn_head(self, params, delta, post_n, pre_n, nms_thresh, min_size):
+        """The RCNN step's frozen RPN with its outputs, and the head's settings and activations."""
+        self.delta = delta
+        self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
+        self.n_heads = 5 * self.num_classes
+        self.head_ld = ops.round_up(self.n_heads, 32)
+        dev, rows = self.device, self._slots * self.fh * self.fw
+        self._frozen_rpn(params)
+        self.rpn_mid = self._act(self.fh, self.fw, 512)
+        self.rpn_out = torch.empty((rows, self.rpn_ld), dtype=torch.float32, device=dev)
+        self.pool5 = self._act(1, post_n, 49 * 512)
+        self.fc6 = self._act(1, post_n, 4096)
+        self.fc7 = self._act(1, post_n, 4096)
+        self.head_out = torch.empty((self._slots * post_n, self.head_ld), dtype=torch.float32, device=dev)
+        self.dfeat = torch.empty((rows, 512), dtype=torch.float32, device=dev)
+
     def _frozen_rpn(self, params):
-        """The RPN's 3x3 and twin-head weights, packed once (forward only: the RCNN step gives them no gradient)."""
+        """The RPN's 3x3 and twin-head weights as (planes, bias), packed once (forward only: the RCNN step gives them no
+        gradient)."""
         T = lambda k: torch.from_numpy(np.ascontiguousarray(params[k], dtype=np.float32)).to(self.device)     # noqa: E731
-        hi, lo = ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=512, precision=self.precision)
-        self.rpn3 = (hi, lo, ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
+        self.rpn3 = (ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=512, precision=self.precision),
+                     ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
         wh = torch.cat([T("RPN/rpn_cls_score/W"), T("RPN/rpn_bbox_pred/W")], dim=0)
         bh = torch.cat([T("RPN/rpn_cls_score/b"), T("RPN/rpn_bbox_pred/b")], dim=0)
         self.rpn_ld = ops.round_up(6 * self.A, 32)
-        hi, lo = ops.pack_conv_weights(wh, precision=self.precision)
-        self.rpn_heads = (hi, lo, ops.pad_bias(bh, self.rpn_ld))
+        self.rpn_heads = (ops.pack_conv_weights(wh, precision=self.precision), ops.pad_bias(bh, self.rpn_ld))
 
     # ---------------------------------------------------------------- parameters
     def _heads_w(self, flat):
@@ -506,14 +551,8 @@ class RcnnTrainer(RpnTrainer):
     def repack(self):
         self._repack_convs()
         for n in ("fc6", "fc7"):
-            w, b = self.weights(n + "/W"), self.weights(n + "/b")
-            fwd = ops.pack_conv_weights(w, precision=self.precision)
-            dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=4096, x3=self.x3)
-            self.packed[n] = (fwd, ops.pad_bias(b, 4096), dg)
-        wh, bh = self._heads_w(self.w_flat), self._heads_b(self.w_flat)
-        fwd = ops.pack_conv_weights(wh, precision=self.precision)
-        dg = train_ops.pack_conv_weights_dgrad(wh, cout_pad=self.head_ld, x3=self.x3)        # [1, 4096, head_ld]
-        self.packed["heads"] = (fwd, ops.pad_bias(bh, self.head_ld), dg)
+            self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), 4096)
+        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- ProposalTargetLayer sampling (host, like the reference)
     def _sample(self, max_ov, R):
@@ -534,10 +573,7 @@ class RcnnTrainer(RpnTrainer):
         """Returns losses float32[4] (device): loss_cls, loss_bbox, cls_accuracy, loss_rcnn."""
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
         feat = self._forward_trunk(x_chw)
-        hi, lo, b = self.rpn3
-        ops.conv2d(feat, hi, lo, b, 3, True, out=self.rpn_mid)
-        hi, lo, b = self.rpn_heads
-        ops.conv2d(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=self.rpn_ld, out_f32=self.rpn_out)
+        self._rpn_forward(feat, self.rpn3, self.rpn_heads, self.rpn_mid, self.rpn_ld, self.rpn_out)
         ops.proposals(self.rpn_out, None, self.anchors, self.A, self.fh, self.fw, self.feat_stride, im_h, im_w, self.min_size,
                       self.pre_n, self.post_n, self.nms_thresh, layout="nhwc", ld=self.rpn_ld, cls_is_logits=True, work=self.prop)
         rois, count = self.prop.rois, self.prop.count
@@ -553,19 +589,23 @@ class RcnnTrainer(RpnTrainer):
         if masks is None and self.dropout:
             masks = [(torch.rand((self.post_n, 4096), device=self.device, generator=self.gen) >= 0.5).to(torch.uint8) for _ in range(2)]
         self.masks = masks
-        (hi, lo), b, _ = self.packed["fc6"]
-        ops.conv2d(self.pool5, hi, lo, b, 1, True, out=self.fc6, m_valid=count)
-        if masks is not None:
-            train_ops.dropout_(self.fc6, masks[0])                                           # F.dropout(train=rcnn_train), :127
-        (hi, lo), b, _ = self.packed["fc7"]
-        ops.conv2d(self.fc6, hi, lo, b, 1, True, out=self.fc7, m_valid=count)
-        if masks is not None:
-            train_ops.dropout_(self.fc7, masks[1])                                           # :128
-        (hi, lo), b, _ = self.packed["heads"]
-        ops.conv2d(self.fc7, hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out, m_valid=count)
+        self._head_forward()
         losses, self.head_grad = train_ops.rcnn_loss(self.head_out, self.keep, self.labels, self.ext, self.num_classes, self.delta)
         self.last_losses = losses
         return losses
+
+    def _head_forward(self):
+        """fc6 -> fc7 -> cls_score | bbox_pred over the pooled RoIs into head_out, with `masks` dropout after fc6 and fc7."""
+        fwd, b, _ = self.packed["fc6"]
+        self._conv(self.pool5, fwd, b, 1, True, "rois", out=self.fc6)
+        if self.masks is not None:
+            train_ops.dropout_(self.fc6, self.masks[0])                                      # F.dropout(train=rcnn_train), :127
+        fwd, b, _ = self.packed["fc7"]
+        self._conv(self.fc6, fwd, b, 1, True, "rois", out=self.fc7)
+        if self.masks is not None:
+            train_ops.dropout_(self.fc7, self.masks[1])                                      # :128
+        fwd, b, _ = self.packed["heads"]
+        self._conv(self.fc7, fwd, b, 1, False, "rois", out_act=False, ld_f32=self.head_ld, out_f32=self.head_out)
 
     # ---------------------------------------------------------------- backward
     def _fc_wgrad(self, dyT, xT, M, N, dw, m_out=None):
@@ -579,55 +619,60 @@ class RcnnTrainer(RpnTrainer):
             train_ops.wgrad_reduce(parts, m_out or M, N, dw)
 
     def backward(self, debug=None):
+        """Fills g_flat with d(loss_rcnn)/d(parameter) for every trainable parameter.  debug: as RpnTrainer.backward, plus
+        "roi": the gradient of the pooled RoIs ("dpool5") and of conv5_3's output (fp32 [fh*fw, 512], "dfeat")."""
         R_cap, ld = self.post_n, self.head_ld
         twice = self.masks is not None               # ratio-0.5 dropout: dz = 2 * g * (y > 0), y = the post-dropout activation
         # ---- cls_score | bbox_pred: dY = head_grad [R_cap, ld] fp32 (zero rows for RoIs that were not kept)
         dyh = self._gact(1, R_cap, ld)
         dyhT = self._tbuf(1, ld, 1, R_cap)
-        train_ops.grad_prepare(1, R_cap, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
+        self._prep(1, R_cap, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
         fc7T = self._tbuf(1, 4096, 1, R_cap)
-        train_ops.grad_prepare(1, R_cap, 4096, g=self.fc7, tbuf=fc7T)
+        self._prep(1, R_cap, 4096, g=self.fc7, tbuf=fc7T)
         self._fc_wgrad(dyhT, fc7T, ld, 4096, self._heads_w(self.g_flat), m_out=self.n_heads)
         train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
-        _, _, (dhi, dlo) = self.packed["heads"]
         g = self._gact(1, R_cap, 4096, tag=1)
-        ops.conv2d(dyh, dhi, dlo, self.zero_bias, 1, False, out=g)
+        self._conv(dyh, self.packed["heads"][2], self.zero_bias, 1, False, "roi_grads", out=g)
+        if debug is not None:
+            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
         # ---- fc7
         dy7 = self._gact(1, R_cap, 4096)
         dy7T = self._tbuf(1, 4096, 1, R_cap, tag=1)
-        train_ops.grad_prepare(1, R_cap, 4096, g=g, y=self.fc7, out=dy7, tbuf=dy7T, times2=twice)
+        self._prep(1, R_cap, 4096, g=g, y=self.fc7, out=dy7, tbuf=dy7T, times2=twice)
         if debug is not None:
-            debug["fc7"] = dict(g_in=g.to_chw_f32().clone(), dy=dy7.to_chw_f32().clone())
+            debug["fc7"] = dict(g_in=self._chw(g), dy=self._chw(dy7))
         fc6T = self._tbuf(1, 4096, 1, R_cap)          # the buffer of fc7T: the heads' weight gradient has consumed it
-        train_ops.grad_prepare(1, R_cap, 4096, g=self.fc6, tbuf=fc6T)
+        self._prep(1, R_cap, 4096, g=self.fc6, tbuf=fc6T)
         self._fc_wgrad(dy7T, fc6T, 4096, 4096, self.grads("fc7/W"))
         train_ops.bias_grad(dy7T, 4096, self.grads("fc7/b"))
-        _, _, (dhi, dlo) = self.packed["fc7"]
         g6 = self._gact(1, R_cap, 4096, tag=2)
-        ops.conv2d(dy7, dhi, dlo, self.zero_bias, 1, False, out=g6)
+        self._conv(dy7, self.packed["fc7"][2], self.zero_bias, 1, False, "roi_grads", out=g6)
         # ---- fc6
         dy6 = self._gact(1, R_cap, 4096)
-        train_ops.grad_prepare(1, R_cap, 4096, g=g6, y=self.fc6, out=dy6, tbuf=dy7T, times2=twice)      # dy7T's buffer now holds dy6^T
+        self._prep(1, R_cap, 4096, g=g6, y=self.fc6, out=dy6, tbuf=dy7T, times2=twice)       # dy7T's buffer now holds dy6^T
         if debug is not None:
-            debug["fc6"] = dict(g_in=g6.to_chw_f32().clone(), dy=dy6.to_chw_f32().clone())
+            debug["fc6"] = dict(g_in=self._chw(g6), dy=self._chw(dy6))
         p5T = self._tbuf(1, 49 * 512, 1, R_cap)
-        train_ops.grad_prepare(1, R_cap, 49 * 512, g=self.pool5, tbuf=p5T)
+        self._prep(1, R_cap, 49 * 512, g=self.pool5, tbuf=p5T)
         self._fc_wgrad(dy7T, p5T, 4096, 49 * 512, self.grads("fc6/W"))
         train_ops.bias_grad(dy7T, 4096, self.grads("fc6/b"))
-        _, _, (dhi, dlo) = self.packed["fc6"]
         gp = self._gact(1, R_cap, 49 * 512, tag=1)
-        ops.conv2d(dy6, dhi, dlo, self.zero_bias, 1, False, out=gp)
+        self._conv(dy6, self.packed["fc6"][2], self.zero_bias, 1, False, "roi_grads", out=gp)
         # ---- RoI pooling backward -> gradient of conv5_3's output, then the trunk
+        self._roi_pool_backward(gp)
+        gfeat = self._gact(self.fh, self.fw, 512, tag=3)
+        self._prep(self.fh, self.fw, 512, g_f32=self.dfeat, out=gfeat)
+        if debug is not None:
+            debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
+        self._backward_chain(self.layers[12::-1], gfeat, debug)
+
+    def _roi_pool_backward(self, g):
+        """dfeat = the RoI pooling's backward of g (the gradient of pool5)."""
         if self.roi_ws is None:
             self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_workspace_bytes(self.fh, self.fw, 512),),
                                       dtype=torch.uint8, device=self.device)
-        train_ops.roi_pool_backward(self.feat, self.prop.rois, self.prop.count, gp, 7, 7, 1.0 / self.feat_stride, out=self.dfeat,
+        train_ops.roi_pool_backward(self.feat, self.prop.rois, self.prop.count, g, 7, 7, 1.0 / self.feat_stride, out=self.dfeat,
                                     ws=self.roi_ws)
-        gfeat = self._gact(self.fh, self.fw, 512, tag=3)
-        train_ops.grad_prepare(self.fh, self.fw, 512, g_f32=self.dfeat, out=gfeat)
-        if debug is not None:
-            debug["roi"] = dict(dpool5=gp.to_chw_f32().clone(), dfeat=self.dfeat.clone())
-        self._backward_chain(self.layers[12::-1], gfeat, debug)
 
     def step(self, x_chw, gt_boxes, im_info=None, keep_inds=None, masks=None):
         losses = self.forward(x_chw, gt_boxes, im_info, keep_inds, masks)
@@ -638,8 +683,8 @@ class RcnnTrainer(RpnTrainer):
 
 class _CanvasSteps(object):
     """The canvas machinery shared by CanvasRpnTrainer and CanvasRcnnTrainer: the N-slot image input with its device extents,
-    the staged ground truth, the [N]-lead gradient buffers, the in-place repack of the convolutions (a captured graph reads
-    the packed weights), the canvas trunk forward and backward, and the capture-then-replay step."""
+    the staged ground truth, the launches over the canvas (the _ext convolutions, zero outside each image, and the _batch
+    re-layouts) that override _ConvTrainer's, and the capture-then-replay step."""
     raw_input = False           # True: the input is RawPhotoInput's training block (put_raw / step_raw)
 
     def _canvas_init(self, N, Hc, Wc, max_gt, seed, raw_input):
@@ -647,49 +692,33 @@ class _CanvasSteps(object):
         self.raw_input = bool(raw_input)
         self.input = RawPhotoInput(N, Hc, Wc, dev, max_gt=max_gt) if self.raw_input else ImageInput(N, Hc, Wc, dev, canvas=True)
         self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
-        halvings = 0
-        for L in self.layers[:13]:                   # a layer's extents are ceil(extent / 2^halvings)
-            L["halvings"] = halvings
-            halvings += 1 if L["pool"] else 0
-        self.halvings = halvings
         self.gt = torch.zeros((N, max_gt, 5), dtype=torch.float32, device=dev)
         self.gt_counts = torch.zeros((N,), dtype=torch.int32, device=dev)
         self.seeds = torch.arange(N, dtype=torch.int64, device=dev) + int(seed)
         self.image_sizes = [(0, 0)] * N
         self.graph = None
 
-    # ---------------------------------------------------------------- buffers with the [N] lead
-    def _gact(self, h, w, c, tag=0):
-        key = (h, w, c, tag)
-        if key not in self._acts:
-            hi = torch.empty((self.N, h, w, c), dtype=torch.bfloat16, device=self.device)
-            self._acts[key] = ops.Act(hi, torch.empty_like(hi) if self.x3 else None)
-        return self._acts[key]
+    # ---------------------------------------------------------------- launches over the canvas
+    def _conv(self, x, planes, bias, ksize, relu, at, **kw):
+        """frcnn_conv2d_batch_ext over the trunk level's extents, or over the head's (1, R_n) for "rois" / "roi_grads"."""
+        ext, k = (self.head_ext, 0) if at in ("rois", "roi_grads") else (self.extents, at)
+        return ops.conv2d_batch(x, planes[0], planes[1], bias, ksize, relu, extents=ext, halvings=k, **kw)
 
-    def _tbuf(self, planes, c, h, w, tag=0):
-        key = (planes, c, h, w, tag)
-        if key not in self._tbufs:
-            self._tbufs[key] = train_ops.TBuf(planes, c, h, w, self.device, self.x3, N=self.N)
-        return self._tbufs[key]
+    def _prep(self, h, w, c, **kw):
+        train_ops.grad_prepare_batch(self.N, h, w, c, **kw)
+
+    def _pool(self, y, out):
+        ops.maxpool2x2_ceil_batch(y, out=out)
 
     def _chw(self, act):
         """[N, C, H, W] float32 copy of an [N, H, W, C] Act (debug)."""
         return torch.stack([ops.Act(act.hi[n], None if act.lo is None else act.lo[n]).to_chw_f32() for n in range(self.N)])
 
-    # ---------------------------------------------------------------- weights: repacked in place
-    def _repack(self, name, w, b, cout_pad, first=False, cin_pad=None):
-        pr, old = self.precision, self.packed.get(name)
-        if first:
-            fwd, dg = ops.pack_conv_weights_im2col(w, precision=pr, out=old and old[0]), None
-        else:
-            fwd = ops.pack_conv_weights(w, cin_pad=cin_pad, precision=pr, out=old and old[0])
-            dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=cout_pad, x3=self.x3, out=old and old[2])
-        self.packed[name] = (fwd, ops.pad_bias(b, cout_pad, out=old and old[1]), dg)
-
-    def _repack_convs(self):
-        for i, L in enumerate(self.layers):
-            name = L["name"]
-            self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
+    def _pack_input(self, x_chw=None):
+        """The staged slots into x_col; raw photos are resized on the way, and their boxes scaled into gt."""
+        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
+        if self.raw_input:
+            self.input.scale_gt(self.gt, self.gt_counts)
 
     # ---------------------------------------------------------------- staging
     def _need_input(self, call):
@@ -736,55 +765,6 @@ class _CanvasSteps(object):
             if lens[n]:
                 buf[offs[n]:offs[n + 1]].copy_(d.reshape(-1), non_blocking=True)
         offsets.copy_(torch.from_numpy(offs), non_blocking=True)
-
-    # ---------------------------------------------------------------- trunk forward / backward over the canvas
-    def _canvas_trunk(self):
-        ext = self.extents
-        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
-        if self.raw_input:
-            self.input.scale_gt(self.gt, self.gt_counts)
-        x = self.x_col
-        for i, L in enumerate(self.layers[:13]):
-            (hi, lo), b, _ = self.packed[L["name"]]
-            ops.conv2d_batch(x, hi, lo, b, 1 if i == 0 else 3, True, out=L["y"], extents=ext, halvings=L["halvings"])
-            x = L["y"]
-            if L["pool"]:
-                ops.maxpool2x2_ceil_batch(L["y"], out=L["p"])
-                x = L["p"]
-        self.feat = x
-        return x
-
-    def _canvas_chain(self, chain, g, debug=None):
-        """RpnTrainer._backward_chain over the canvas: grad_prepare_batch re-layouts, weight gradients over K = N*Kp (the sum
-        over the slots), data gradients through the _ext convolutions."""
-        N, ext = self.N, self.extents
-        for L in chain:
-            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
-            first = L is self.layers[0]
-            dy = self._gact(h, w, co)
-            dyT = self._tbuf(1, co, h, w)
-            train_ops.grad_prepare_batch(N, h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
-            if debug is not None:
-                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
-            x = self._input_of(L)
-            if first:
-                xT = self._tbuf(1, 32, h, w)
-                train_ops.grad_prepare_batch(N, h, w, 32, g=x, tbuf=xT)
-                dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
-                self._wgrad(dyT, xT, co, 32, 1, dwc)
-                self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
-            else:
-                xT = self._tbuf(3, ci, h, w)
-                train_ops.grad_prepare_batch(N, h, w, ci, g=x, tbuf=xT)
-                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
-            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
-            self._early_exchange(L["name"])
-            if not first:
-                _, _, (dhi, dlo) = self.packed[L["name"]]
-                g = self._gact(h, w, ci, tag=1)
-                ops.conv2d_batch(dy, dhi, dlo, self.zero_bias, 3, False, out=g, extents=ext, halvings=L["halvings"])
-                if debug is not None:
-                    debug[L["name"]]["g_out"] = self._chw(g)
 
     # ---------------------------------------------------------------- the step
     def run(self):
@@ -846,31 +826,17 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         if int(max_gt) < 1:
             raise FrcnnError("CanvasRpnTrainer: max_gt must be at least 1")
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
-        A = len(anchors)
-        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
-        extra = [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], extra, lead=(N,))
-        dev = self.device
-        self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
-        self.n_heads = 6 * self.A
-        self.head_ld = ops.round_up(self.n_heads, 32)
+                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], _rpn_params(len(anchors)), lead=(N,))
+        self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
-        R = self.layers[13]
-        R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, self.halvings
-        R["y"] = self._act(self.fh, self.fw, 512)
-        rows = N * self.fh * self.fw
-        self.head_out = torch.empty((rows, self.head_ld), dtype=torch.float32, device=dev)
+        dev = self.device
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rpn_loss_batch
         self.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, max_gt, dev)
         self.step_losses = self.targets.losses
         self.disable_pos = torch.zeros((max(N * self.targets.cap, 1),), dtype=torch.int32, device=dev)
         self.disable_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
         self.repack()
-
-    def repack(self):
-        self._repack_convs()
-        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- staging
     def put(self, images, gt_boxes, img_infos=None, disable_pos=None):
@@ -914,14 +880,8 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
     def forward(self):
         """Forward over the staged canvas, the anchor targets and the per-slot losses (float32 [N, 4] device buffer:
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss; zeros for an empty slot)."""
-        ext = self.extents
-        x = self._canvas_trunk()
-        R, k = self.layers[13], self.halvings
-        (hi, lo), b, _ = self.packed[R["name"]]
-        ops.conv2d_batch(x, hi, lo, b, 3, True, out=R["y"], extents=ext, halvings=k)
-        (hi, lo), b, _ = self.packed["heads"]
-        ops.conv2d_batch(R["y"], hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out, extents=ext,
-                         halvings=k)
+        ext, k, R = self.extents, self.halvings, self.rpn_layer
+        self._rpn_forward(self._forward_trunk(), self.packed[R["name"]], self.packed["heads"], R["y"], self.head_ld, self.head_out)
         mode = self._MODES[self.subsample]
         train_ops.anchor_targets_batch(self.anchors, self.A, self.feat_stride, ext, self.im_info, self.gt, self.gt_counts,
                                        self.targets, halvings=k, mode=mode, seeds=self.seeds, disable_pos=self.disable_pos,
@@ -933,26 +893,6 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
                                           dhead=self.head_grad)
         self.last_losses = losses
         return losses
-
-    # ---------------------------------------------------------------- backward
-    def backward(self, debug=None):
-        """Fills g_flat with the sum over the slots of d(rpn_loss_n)/d(parameter).  debug: as RpnTrainer.backward, every
-        tensor with a leading [N]."""
-        N, fh, fw, ld, ext = self.N, self.fh, self.fw, self.head_ld, self.extents
-        R = self.layers[13]
-        dyh = self._gact(fh, fw, ld)
-        dyhT = self._tbuf(1, ld, fh, fw)
-        train_ops.grad_prepare_batch(N, fh, fw, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
-        midT = self._tbuf(3, 512, fh, fw)
-        train_ops.grad_prepare_batch(N, fh, fw, 512, g=R["y"], tbuf=midT)
-        self._wgrad(dyhT, midT, ld, 512, 1, self._heads_w(self.g_flat), m_out=self.n_heads)
-        train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
-        _, _, (dhi, dlo) = self.packed["heads"]
-        g = self._gact(fh, fw, 512, tag=1)
-        ops.conv2d_batch(dyh, dhi, dlo, self.zero_bias, 1, False, out=g, extents=ext, halvings=self.halvings)
-        if debug is not None:
-            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
-        self._canvas_chain([R] + self.layers[12::-1], g, debug)
 
     def step(self, images, gt_boxes, img_infos=None, disable_pos=None):
         """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
@@ -1006,14 +946,9 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [], _rcnn_params(nc), load_transform=_fc6_to_hwc, lead=(N,))
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
-        self.delta, self.sample, self.dropout = delta, sample, dropout
-        self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
-        self.n_heads = 5 * nc
-        self.head_ld = ops.round_up(self.n_heads, 32)
+        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+        self.sample, self.dropout = sample, dropout
         dev, fh, fw = self.device, self.fh, self.fw
-        self._frozen_rpn(params)
-        self.rpn_mid = self._act(fh, fw, 512)
-        self.rpn_out = torch.empty((N * fh * fw, self.rpn_ld), dtype=torch.float32, device=dev)
         # the head's extents (1, R_n): column 1 is the proposal count frcnn_proposals_batch_ext writes
         self.head_ext = torch.ones((N, 2), dtype=torch.int32, device=dev)
         self.prop = ops.ProposalBatchWorkspace(N, self.A, fh, fw, pre_n, post_n, dev, outputs=(
@@ -1023,22 +958,11 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         self.step_losses = self.ptargets.losses
         self.keep_list = torch.zeros((N * train_ops.ROIS_PER_IMAGE,), dtype=torch.int32, device=dev)
         self.keep_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
-        self.pool5 = self._act(1, post_n, 49 * 512)
-        self.fc6 = self._act(1, post_n, 4096)
-        self.fc7 = self._act(1, post_n, 4096)
         self.masks = torch.zeros((2, N, post_n, 4096), dtype=torch.uint8, device=dev) if dropout is not None else None
-        self.head_out = torch.empty((N * post_n, self.head_ld), dtype=torch.float32, device=dev)
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rcnn_loss_batch
-        self.dfeat = torch.empty((N * fh * fw, 512), dtype=torch.float32, device=dev)
         self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_batch_workspace_bytes(N, fh, fw, 512),),
                                   dtype=torch.uint8, device=dev)
         self.repack()
-
-    def repack(self):
-        self._repack_convs()
-        for n in ("fc6", "fc7"):
-            self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), 4096)
-        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- staging
     def put(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
@@ -1103,12 +1027,8 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         """Forward over the staged canvas, the proposal targets and the per-slot losses (float32 [N, 4] device buffer:
         loss_cls, loss_bbox, cls_accuracy, loss_rcnn; zeros for a slot that kept nothing)."""
         N, ext, k, R_cap = self.N, self.extents, self.halvings, self.post_n
-        feat = self._canvas_trunk()
-        hi, lo, b = self.rpn3
-        ops.conv2d_batch(feat, hi, lo, b, 3, True, out=self.rpn_mid, extents=ext, halvings=k)
-        hi, lo, b = self.rpn_heads
-        ops.conv2d_batch(self.rpn_mid, hi, lo, b, 1, False, out_act=False, ld_f32=self.rpn_ld, out_f32=self.rpn_out, extents=ext,
-                         halvings=k)
+        feat = self._forward_trunk()
+        self._rpn_forward(feat, self.rpn3, self.rpn_heads, self.rpn_mid, self.rpn_ld, self.rpn_out)
         ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, self.rpn_ld), None, self.anchors, self.A, self.fh, self.fw,
                             self.feat_stride, 0, 0, self.min_size, self.pre_n, R_cap, self.nms_thresh, layout="nhwc",
                             ld=self.rpn_ld, cls_is_logits=True, work=self.prop, extents=ext, halvings=k, im_info=self.im_info)
@@ -1122,74 +1042,14 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
                 train_ops.dropout_masks_batch(self.seeds, j + 1, self.masks[j])
         if self.sample == "device" or self.dropout == "device":
             self.seeds.add_(N)
-        hx = self.head_ext
-        (hi, lo), b, _ = self.packed["fc6"]
-        ops.conv2d_batch(self.pool5, hi, lo, b, 1, True, out=self.fc6, extents=hx, halvings=0)
-        if self.masks is not None:
-            train_ops.dropout_(self.fc6, self.masks[0])                                      # F.dropout, faster_rcnn.py:127
-        (hi, lo), b, _ = self.packed["fc7"]
-        ops.conv2d_batch(self.fc6, hi, lo, b, 1, True, out=self.fc7, extents=hx, halvings=0)
-        if self.masks is not None:
-            train_ops.dropout_(self.fc7, self.masks[1])                                      # :128
-        (hi, lo), b, _ = self.packed["heads"]
-        ops.conv2d_batch(self.fc7, hi, lo, b, 1, False, out_act=False, ld_f32=self.head_ld, out_f32=self.head_out, extents=hx,
-                         halvings=0)
+        self._head_forward()
         losses = train_ops.rcnn_loss_batch(self.head_out, self.ptargets, delta=self.delta, dhead=self.head_grad)
         self.last_losses = losses
         return losses
 
-    # ---------------------------------------------------------------- backward
-    def backward(self, debug=None):
-        """Fills g_flat with the sum over the slots of d(loss_rcnn_n)/d(parameter).  debug: as RcnnTrainer.backward, every
-        tensor with a leading [N] (dfeat [N*fh*fw, 512])."""
-        N, R_cap, ld, hx = self.N, self.post_n, self.head_ld, self.head_ext
-        twice = self.masks is not None               # ratio-0.5 dropout: dz = 2 * g * (y > 0), y = the post-dropout activation
-        # ---- cls_score | bbox_pred
-        dyh = self._gact(1, R_cap, ld)
-        dyhT = self._tbuf(1, ld, 1, R_cap)
-        train_ops.grad_prepare_batch(N, 1, R_cap, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
-        fc7T = self._tbuf(1, 4096, 1, R_cap)
-        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=self.fc7, tbuf=fc7T)
-        self._fc_wgrad(dyhT, fc7T, ld, 4096, self._heads_w(self.g_flat), m_out=self.n_heads)
-        train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
-        _, _, (dhi, dlo) = self.packed["heads"]
-        g = self._gact(1, R_cap, 4096, tag=1)
-        ops.conv2d_batch(dyh, dhi, dlo, self.zero_bias, 1, False, out=g, extents=hx, halvings=0)
-        if debug is not None:
-            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
-        # ---- fc7
-        dy7 = self._gact(1, R_cap, 4096)
-        dy7T = self._tbuf(1, 4096, 1, R_cap, tag=1)
-        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=g, y=self.fc7, out=dy7, tbuf=dy7T, times2=twice)
-        if debug is not None:
-            debug["fc7"] = dict(g_in=self._chw(g), dy=self._chw(dy7))
-        fc6T = self._tbuf(1, 4096, 1, R_cap)          # the buffer of fc7T: the heads' weight gradient has consumed it
-        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=self.fc6, tbuf=fc6T)
-        self._fc_wgrad(dy7T, fc6T, 4096, 4096, self.grads("fc7/W"))
-        train_ops.bias_grad(dy7T, 4096, self.grads("fc7/b"))
-        _, _, (dhi, dlo) = self.packed["fc7"]
-        g6 = self._gact(1, R_cap, 4096, tag=2)
-        ops.conv2d_batch(dy7, dhi, dlo, self.zero_bias, 1, False, out=g6, extents=hx, halvings=0)
-        # ---- fc6
-        dy6 = self._gact(1, R_cap, 4096)
-        train_ops.grad_prepare_batch(N, 1, R_cap, 4096, g=g6, y=self.fc6, out=dy6, tbuf=dy7T, times2=twice)
-        if debug is not None:
-            debug["fc6"] = dict(g_in=self._chw(g6), dy=self._chw(dy6))
-        p5T = self._tbuf(1, 49 * 512, 1, R_cap)
-        train_ops.grad_prepare_batch(N, 1, R_cap, 49 * 512, g=self.pool5, tbuf=p5T)
-        self._fc_wgrad(dy7T, p5T, 4096, 49 * 512, self.grads("fc6/W"))
-        train_ops.bias_grad(dy7T, 4096, self.grads("fc6/b"))
-        _, _, (dhi, dlo) = self.packed["fc6"]
-        gp = self._gact(1, R_cap, 49 * 512, tag=1)
-        ops.conv2d_batch(dy6, dhi, dlo, self.zero_bias, 1, False, out=gp, extents=hx, halvings=0)
-        # ---- RoI pooling backward -> gradient of conv5_3's output, then the trunk
-        train_ops.roi_pool_backward_batch(self.feat, self.prop.rois, hx[:, 1], gp, self.extents, self.halvings, 7, 7,
+    def _roi_pool_backward(self, g):
+        train_ops.roi_pool_backward_batch(self.feat, self.prop.rois, self.head_ext[:, 1], g, self.extents, self.halvings, 7, 7,
                                           1.0 / self.feat_stride, out=self.dfeat, ws=self.roi_ws)
-        gfeat = self._gact(self.fh, self.fw, 512, tag=3)
-        train_ops.grad_prepare_batch(N, self.fh, self.fw, 512, g_f32=self.dfeat, out=gfeat)
-        if debug is not None:
-            debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
-        self._canvas_chain(self.layers[12::-1], gfeat, debug)
 
     def step(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
         """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
