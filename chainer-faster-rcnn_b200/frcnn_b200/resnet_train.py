@@ -1,5 +1,6 @@
-"""The train_rpn.py step with the ResNet-50/101/152 trunk: `FasterRCNN(trunk_class=ResNet, rpn_in_ch=2048, feat_stride=32)`
-with `rpn_train = True` (the reference's utils/prepare_train.py offers --trunk_model ResNet50/101/152).
+"""The train_rpn.py and train_rcnn.py steps with the ResNet-50/101/152 trunk: `FasterRCNN(trunk_class=ResNet,
+rpn_in_ch=2048, feat_stride=32)` with `rpn_train = True` or `rcnn_train = True` (the reference's utils/prepare_train.py
+offers --trunk_model ResNet50/101/152).
 
 ResNetRpnTrainer -- forward (conv1 7x7/2 + pool 3x3/2 + bottleneck blocks + RPN) -> AnchorTargetLayer -> rpn_loss -> backward
 through the RPN heads, the RPN 3x3 conv and every trunk convolution -> [gradient all-reduce] -> WeightDecay + MomentumSGD.
@@ -25,6 +26,13 @@ A convolution and its frozen BN are then the folded convolution Wf = W*s, bf = b
                      (frcnn_grad_prepare_stride2)
 Everything else -- the flat buffers, the RPN heads' backward, the loss, the optimizer and the gradient exchange (one bucket,
 after backward) -- is RpnTrainer's.
+
+ResNetRcnnTrainer -- RcnnTrainer's step on the same trunk: trunk -> frozen test-mode RPN (2048 -> 512 3x3, twin heads) ->
+ProposalLayer -> ProposalTargetLayer -> RoI pool 7x7 at 1/32 over 2048 channels -> fc6 (K = 2048*49) / fc7 with dropout ->
+cls_score | bbox_pred -> losses -> backward through the head, the RoI pooling and every bottleneck -> WeightDecay +
+MomentumSGD.  The head, its losses and backward are RcnnTrainer's with feat_ch = 2048; the trunk part (_ResNetTrunk) is
+ResNetRpnTrainer's, launch for launch.  Trainable: every trunk convolution's W, trunk/conv1/b, fc6, fc7, cls_score and
+bbox_pred; the RPN is packed once and gets no gradient, the BN entries stay constant.
 """
 import numpy as np
 import torch
@@ -32,7 +40,7 @@ import torch
 from . import ops, train_ops
 from ._lib import FrcnnError
 from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
-from .train_engine import RpnTrainer, _rpn_params
+from .train_engine import RcnnTrainer, RpnTrainer, _fc6_to_hwc, _rcnn_params, _rpn_params
 
 SUBSAMPLE_MODES = ("device", "numpy", "none")
 
@@ -54,46 +62,45 @@ def trunk_convs(n_layers):
     return out
 
 
-class ResNetRpnTrainer(RpnTrainer):
-    """Weights, optimizer state and buffers of the RPN-mode training step with the ResNet trunk for one image shape.  The
-    surface is RpnTrainer's: forward / backward(debug) / update / step / weights / grads / export_params, subsample modes
-    "device", "numpy" and "none", disable_pos.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming;
-    its BN entries are read once and stay constant."""
+class _ResNetTrunk(object):
+    """The ResNet trunk with frozen BatchNorm, shared by ResNetRpnTrainer and ResNetRcnnTrainer (ahead of RpnTrainer /
+    RcnnTrainer in their MRO): the layer table and BN constants, the activations, the forward launches, the fold + repack,
+    and the bottleneck backward (_backward_trunk, from the gradient of the feature map)."""
+    feat_ch = 2048
 
-    def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+    def _init_trunk(self, params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
+                    process_group, extra_layers, extra_params, need, load_transform=None):
+        """Checks the options and parameters (FrcnnError before anything is allocated), then lays out the flat buffers over
+        the trunk convolutions + extra_layers and extra_params, the frozen-BN constants and the trunk activations.
+        need: {name: shape} of the non-trunk parameters the step reads."""
+        who = type(self).__name__
         if n_layers not in RESNET_BLOCKS:
-            raise FrcnnError("ResNetRpnTrainer: n_layers must be one of %s (got %r)" % (sorted(RESNET_BLOCKS), n_layers))
-        if subsample not in SUBSAMPLE_MODES:
-            raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
+            raise FrcnnError("%s: n_layers must be one of %s (got %r)" % (who, sorted(RESNET_BLOCKS), n_layers))
         if feat_stride != 32:
-            raise FrcnnError("ResNetRpnTrainer: the ResNet trunk's feature stride is 32 (got feat_stride=%r)" % (feat_stride,))
+            raise FrcnnError("%s: the ResNet trunk's feature stride is 32 (got feat_stride=%r)" % (who, feat_stride))
         Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1           # conv1 7x7/2 pad 3
         if min(Ho, Wo) < 3:
-            raise FrcnnError("ResNetRpnTrainer: the image must be at least 5 x 5 (got %d x %d)" % (H, W))
+            raise FrcnnError("%s: the image must be at least 5 x 5 (got %d x %d)" % (who, H, W))
         self.n_layers = n_layers
-        A = len(anchors)
         convs = trunk_convs(n_layers)
-        need = {n + "/W": (co, ci, k, k) for n, _, ci, co, k in convs}
-        need["trunk/conv1/b"] = (64,)
+        want = {n + "/W": (co, ci, k, k) for n, _, ci, co, k in convs}
+        want["trunk/conv1/b"] = (64,)
         for _, bn, _, co, _ in convs:
             for f in ("gamma", "beta", "avg_mean", "avg_var"):
-                need["%s/%s" % (bn, f)] = (co,)
-        need.update({"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)})
-        need.update(_rpn_params(A))
-        for k, sh in need.items():
+                want["%s/%s" % (bn, f)] = (co,)
+        want.update(need)
+        for k, sh in want.items():
             if k not in params or tuple(np.shape(params[k])) != sh:
-                raise FrcnnError("ResNetRpnTrainer: parameter %s must have shape %s (got %s)"
-                                 % (k, sh, None if k not in params else tuple(np.shape(params[k]))))
+                raise FrcnnError("%s: parameter %s must have shape %s (got %s)"
+                                 % (who, k, sh, None if k not in params else tuple(np.shape(params[k]))))
         layers = [dict(name=n, bn=bn, cin=ci, cout=co, k=k, bias=n == "trunk/conv1") for n, bn, ci, co, k in convs]
-        layers.append(dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3))
         self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          layers, _rpn_params(A))
+                          layers + list(extra_layers), extra_params, load_transform)
         dev = self.device
         # ---- frozen BN: s (float64) per conv, the constant folded bias of every conv but conv1, the folded-weight buffers
         T = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)     # noqa: E731
         self.conv = {}
-        for L in layers[:-1]:
+        for L in layers:
             n, bn = L["name"], L["bn"]
             L["s"] = T(bn_scale(params, bn), torch.float64)
             L["wf"] = torch.empty((L["cout"], L["cin"], L["k"], L["k"]), dtype=torch.float32, device=dev)
@@ -104,7 +111,7 @@ class ResNetRpnTrainer(RpnTrainer):
                 L["bf"] = T(fold_batchnorm(params[n + "/W"], params[bn + "/gamma"], params[bn + "/beta"], params[bn + "/avg_mean"],
                                            params[bn + "/avg_var"])[1])
             self.conv[n] = L
-        self.bn_params = {k: np.asarray(params[k]).copy() for k in need if "/bn" in k}
+        self.bn_params = {k: np.asarray(params[k]).copy() for k in want if "/bn" in k}
         # ---- activations (ResNetForwardPlan._alloc_trunk's, every one kept for backward)
         act = self._act
         self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)
@@ -128,38 +135,36 @@ class ResNetRpnTrainer(RpnTrainer):
             self.blocks.append(B)
             x = B["out"]
         self.fh, self.fw = h, w
-        self._init_rpn_head(loss_lambda, delta, subsample, seed)
-        self.targets = train_ops.AnchorTargets(self.A, h, w, dev)
         self.db_raw = torch.empty((64,), dtype=torch.float32, device=dev)
-        self.repack()
+
+    def _check_input(self, x_chw, gt_boxes):
+        who = type(self).__name__
+        if not (torch.is_tensor(x_chw) and x_chw.is_cuda and tuple(x_chw.shape) == (3, self.H, self.W)):
+            raise FrcnnError("%s.forward: x_chw must be a (3, %d, %d) CUDA tensor" % (who, self.H, self.W))
+        if not (torch.is_tensor(gt_boxes) and gt_boxes.is_cuda and gt_boxes.dim() == 2 and gt_boxes.shape[1] == 5
+                and gt_boxes.shape[0] >= 1):
+            raise FrcnnError("%s.forward: gt_boxes must be a (G >= 1, 5) CUDA tensor" % who)
 
     # ---------------------------------------------------------------- weights: fold, then the forward engines' packers
     def _pack_image_layer(self, w, out=None):
         return ops.pack_conv_weights_im2col_general(w, CONV1_KPAD, precision=self.precision, out=out)
 
     def _repack_convs(self):
+        """Folds and repacks every trunk convolution, then repacks the step's other convolutions (the RPN 3x3, if trained)."""
         for n, L in self.conv.items():
             first = n == "trunk/conv1"
             train_ops.fold_batchnorm(self.weights(n + "/W"), L["s"], L["wf"], b=self.weights(n + "/b") if first else None,
                                      beta=L.get("beta"), mean=L.get("mean"), bf=L["bf"] if first else None)
             self._repack(n, L["wf"], L["bf"], L["cout"], first=first, cin_pad=L["cin"])
-        R = self.rpn_layer
-        self._repack(R["name"], self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b"), R["cout"], cin_pad=R["cin"])
+        for L in self.layers[len(self.conv):]:
+            n = L["name"]
+            self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), L["cout"], cin_pad=L["cin"])
 
     def folded_params(self):
         """{conv name: (Wf, bf)} float32 numpy: the folded weights the device packed at the last repack."""
         return {n: (L["wf"].cpu().numpy().copy(), L["bf"].cpu().numpy().copy()) for n, L in self.conv.items()}
 
     # ---------------------------------------------------------------- forward
-    def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
-        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
-        if not (torch.is_tensor(x_chw) and x_chw.is_cuda and tuple(x_chw.shape) == (3, self.H, self.W)):
-            raise FrcnnError("ResNetRpnTrainer.forward: x_chw must be a (3, %d, %d) CUDA tensor" % (self.H, self.W))
-        if not (torch.is_tensor(gt_boxes) and gt_boxes.is_cuda and gt_boxes.dim() == 2 and gt_boxes.shape[1] == 5
-                and gt_boxes.shape[0] >= 1):
-            raise FrcnnError("ResNetRpnTrainer.forward: gt_boxes must be a (G >= 1, 5) CUDA tensor")
-        return super(ResNetRpnTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos)
-
     def _forward_trunk(self, x_chw):
         """ResNetForwardPlan._run_trunk's launches on the folded weights, with every activation kept."""
         pk = self.packed
@@ -204,28 +209,10 @@ class ResNetRpnTrainer(RpnTrainer):
             ops.conv2d_res(dy, dhi, dlo, self.zero_bias, ksize, False, res, out=g)
         return g
 
-    def backward(self, debug=None):
-        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per conv
-        name, float32 (C,H,W) copies of the incoming gradient ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the
-        block output for conv3 / conv4, at the subsampled resolution when the next block reads it through the stride-2
-        subsample), the masked / routed gradient w.r.t. the (folded) conv output ("dy") and the data gradient the conv
-        passes on ("g_out"; for a block's conv1 the summed gradient of the block input, residual included)."""
+    def _backward_trunk(self, g, debug=None):
+        """Backward through the bottleneck blocks (last first), pool1 and conv1 from g, the gradient of the feature map
+        (ops.Act [fh, fw, 2048]).  debug: receives the per-convolution entries described in ResNetRpnTrainer.backward."""
         dbg = (lambda a: a.to_chw_f32().clone()) if debug is not None else None      # noqa: E731
-        g = self._backward_heads(debug)
-        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
-        R = self.rpn_layer
-        fh, fw = self.fh, self.fw
-        dy = self._gact(fh, fw, 512)
-        dyT = self._tbuf(1, 512, fh, fw)
-        train_ops.grad_prepare(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
-        xT = self._tbuf(3, 2048, fh, fw)
-        train_ops.grad_prepare(fh, fw, 2048, g=self.feat, tbuf=xT)
-        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
-        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
-        g_in = g
-        g = self._dgrad(R["name"], dy, 3, 2048, tag=3)
-        if debug is not None:
-            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
         # ---- the bottleneck blocks, last first; `half`: g is w.r.t. the stride-2 subsample of this block's output
         half = False
         for B in reversed(self.blocks):
@@ -300,3 +287,83 @@ class ResNetRpnTrainer(RpnTrainer):
         if debug is not None:
             debug[base + "/conv1"]["g_out"] = dbg(gx)
         return gx
+
+
+class ResNetRpnTrainer(_ResNetTrunk, RpnTrainer):
+    """Weights, optimizer state and buffers of the RPN-mode training step with the ResNet trunk for one image shape.  The
+    surface is RpnTrainer's: forward / backward(debug) / update / step / weights / grads / export_params, subsample modes
+    "device", "numpy" and "none", disable_pos.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming;
+    its BN entries are read once and stay constant."""
+
+    def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+        if subsample not in SUBSAMPLE_MODES:
+            raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
+        A = len(anchors)
+        need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
+        need.update(_rpn_params(A))
+        self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
+                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), need)
+        self._init_rpn_head(loss_lambda, delta, subsample, seed)
+        self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
+        self.repack()
+
+    # ---------------------------------------------------------------- forward
+    def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
+        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
+        self._check_input(x_chw, gt_boxes)
+        return super(ResNetRpnTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos)
+
+    # ---------------------------------------------------------------- backward
+    def backward(self, debug=None):
+        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per conv
+        name, float32 (C,H,W) copies of the incoming gradient ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the
+        block output for conv3 / conv4, at the subsampled resolution when the next block reads it through the stride-2
+        subsample), the masked / routed gradient w.r.t. the (folded) conv output ("dy") and the data gradient the conv
+        passes on ("g_out"; for a block's conv1 the summed gradient of the block input, residual included)."""
+        dbg = (lambda a: a.to_chw_f32().clone()) if debug is not None else None      # noqa: E731
+        g = self._backward_heads(debug)
+        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
+        R = self.rpn_layer
+        fh, fw = self.fh, self.fw
+        dy = self._gact(fh, fw, 512)
+        dyT = self._tbuf(1, 512, fh, fw)
+        train_ops.grad_prepare(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
+        xT = self._tbuf(3, 2048, fh, fw)
+        train_ops.grad_prepare(fh, fw, 2048, g=self.feat, tbuf=xT)
+        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
+        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
+        g_in = g
+        g = self._dgrad(R["name"], dy, 3, 2048, tag=3)
+        if debug is not None:
+            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
+        self._backward_trunk(g, debug)
+
+
+class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
+    """Weights, optimizer state and buffers of the RCNN-mode training step (train_rcnn.py) with the ResNet trunk for one
+    image shape.  The surface is RcnnTrainer's: forward(x, gt, im_info, keep_inds, masks) / backward(debug) / update / step
+    / weights / grads / export_params, sample="numpy" (a seeded run draws the reference's kept set), keep_inds= and masks=
+    pins.  backward(debug=...) fills RcnnTrainer's head entries ("heads", "fc7", "fc6", "roi") and ResNetRpnTrainer's
+    per-convolution entries.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming; the BN entries and
+    the RPN are read once and stay constant.  fc6/W is held in the (h, w, c) column order the RoI pool emits, c = 2048;
+    export_params returns the reference's (c, h, w)."""
+
+    def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
+                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
+        nc = self.num_classes = num_classes
+        head = _rcnn_params(nc, self.feat_ch)
+        need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
+        need.update(_rpn_params(len(anchors)))
+        need.update(head)
+        self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
+                         process_group, [], head, need, load_transform=_fc6_to_hwc)
+        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_one_image_rcnn(sample, seed, dropout)
+        self.repack()
+
+    def forward(self, x_chw, gt_boxes, im_info=None, keep_inds=None, masks=None):
+        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RcnnTrainer."""
+        self._check_input(x_chw, gt_boxes)
+        return super(ResNetRcnnTrainer, self).forward(x_chw, gt_boxes, im_info, keep_inds, masks)

@@ -38,6 +38,7 @@ class _ConvTrainer(object):
     activations, and the launch layer over one image -- _conv, _prep, _pool, _chw, the cached gradient buffers and the
     in-place repack.  _CanvasSteps overrides the launches for a canvas, so every step is written once."""
     halvings = None             # the feature map's canvas level (the VGG16 trunk's: set by _init_common)
+    feat_ch = 512               # channels of the feature map the RPN and the RoI pooling read (VGG16's conv5_3)
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                      extra_layers, extra_params, load_transform=None, lead=()):
@@ -106,7 +107,8 @@ class _ConvTrainer(object):
 
         self._act = act
         self._slots = int(lead[0]) if lead else 1           # images per step
-        self.zero_bias = torch.zeros((32768,), dtype=torch.float32, device=dev)
+        # the data gradients' bias: as wide as the widest one, fc6's into the 7x7 RoI pool (feat_ch * 49 outputs)
+        self.zero_bias = torch.zeros((max(32768, 49 * self.feat_ch),), dtype=torch.float32, device=dev)
         # gradient activations (NHWC) and transposed buffers, shared between layers of identical shape
         self._acts, self._tbufs = {}, {}
         self.packed = {}
@@ -467,15 +469,16 @@ def _rpn_params(A):
     return [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
 
 
-def _rcnn_params(nc):
-    """The head parameters of the RCNN step in flat-buffer order (cls_score | bbox_pred adjacent: one [5*nc, 4096] matrix)."""
+def _rcnn_params(nc, feat_ch=512):
+    """The head parameters of the RCNN step in flat-buffer order (cls_score | bbox_pred adjacent: one [5*nc, 4096] matrix);
+    fc6 reads the 7x7 RoI pool of a feat_ch-channel feature map."""
     heads = [("cls_score", nc), ("bbox_pred", 4 * nc)]
-    extra = [("fc6/W", (4096, 512 * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
+    extra = [("fc6/W", (4096, feat_ch * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
     return extra + [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
 
 
 def _fc6_to_hwc(name, a):                           # fc6 columns (c, h, w) -> (h, w, c), the order the RoI pooling emits
-    return a.reshape(4096, 512, 49).transpose(0, 2, 1) if name == "fc6/W" else a
+    return a.reshape(4096, -1, 49).transpose(0, 2, 1) if name == "fc6/W" else a
 
 
 class RcnnTrainer(RpnTrainer):
@@ -497,12 +500,16 @@ class RcnnTrainer(RpnTrainer):
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [], _rcnn_params(nc), load_transform=_fc6_to_hwc)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_one_image_rcnn(sample, seed, dropout)
+        self.repack()
+
+    def _init_one_image_rcnn(self, sample, seed, dropout):
+        """The one-image step's sampling and dropout settings and its proposal workspace."""
         self.sample, self.dropout = sample, dropout
         self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
-        self.prop = ops.ProposalWorkspace(self.A, self.fh, self.fw, pre_n, post_n, self.device)
+        self.prop = ops.ProposalWorkspace(self.A, self.fh, self.fw, self.pre_n, self.post_n, self.device)
         self.roi_ws = None
-        self.repack()
 
     def _init_rcnn_head(self, params, delta, post_n, pre_n, nms_thresh, min_size):
         """The RCNN step's frozen RPN with its outputs, and the head's settings and activations."""
@@ -510,21 +517,21 @@ class RcnnTrainer(RpnTrainer):
         self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
         self.n_heads = 5 * self.num_classes
         self.head_ld = ops.round_up(self.n_heads, 32)
-        dev, rows = self.device, self._slots * self.fh * self.fw
+        dev, rows, C = self.device, self._slots * self.fh * self.fw, self.feat_ch
         self._frozen_rpn(params)
         self.rpn_mid = self._act(self.fh, self.fw, 512)
         self.rpn_out = torch.empty((rows, self.rpn_ld), dtype=torch.float32, device=dev)
-        self.pool5 = self._act(1, post_n, 49 * 512)
+        self.pool5 = self._act(1, post_n, 49 * C)
         self.fc6 = self._act(1, post_n, 4096)
         self.fc7 = self._act(1, post_n, 4096)
         self.head_out = torch.empty((self._slots * post_n, self.head_ld), dtype=torch.float32, device=dev)
-        self.dfeat = torch.empty((rows, 512), dtype=torch.float32, device=dev)
+        self.dfeat = torch.empty((rows, C), dtype=torch.float32, device=dev)
 
     def _frozen_rpn(self, params):
         """The RPN's 3x3 and twin-head weights as (planes, bias), packed once (forward only: the RCNN step gives them no
         gradient)."""
         T = lambda k: torch.from_numpy(np.ascontiguousarray(params[k], dtype=np.float32)).to(self.device)     # noqa: E731
-        self.rpn3 = (ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=512, precision=self.precision),
+        self.rpn3 = (ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=self.feat_ch, precision=self.precision),
                      ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
         wh = torch.cat([T("RPN/rpn_cls_score/W"), T("RPN/rpn_bbox_pred/W")], dim=0)
         bh = torch.cat([T("RPN/rpn_cls_score/b"), T("RPN/rpn_bbox_pred/b")], dim=0)
@@ -542,10 +549,10 @@ class RcnnTrainer(RpnTrainer):
 
     def export_params(self):
         """Trainable parameters as numpy arrays in the reference's layouts (fc6/W back to (c, h, w) columns)."""
-        out = {}
+        out, C = {}, self.feat_ch
         for n in self.index:
             a = self.weights(n).detach().cpu().numpy().copy()
-            out[n] = a.reshape(4096, 49, 512).transpose(0, 2, 1).reshape(4096, 512 * 49) if n == "fc6/W" else a
+            out[n] = a.reshape(4096, 49, C).transpose(0, 2, 1).reshape(4096, C * 49) if n == "fc6/W" else a
         return out
 
     def repack(self):
@@ -620,8 +627,8 @@ class RcnnTrainer(RpnTrainer):
 
     def backward(self, debug=None):
         """Fills g_flat with d(loss_rcnn)/d(parameter) for every trainable parameter.  debug: as RpnTrainer.backward, plus
-        "roi": the gradient of the pooled RoIs ("dpool5") and of conv5_3's output (fp32 [fh*fw, 512], "dfeat")."""
-        R_cap, ld = self.post_n, self.head_ld
+        "roi": the gradient of the pooled RoIs ("dpool5") and of the feature map (fp32 [fh*fw, feat_ch], "dfeat")."""
+        R_cap, ld, C = self.post_n, self.head_ld, self.feat_ch
         twice = self.masks is not None               # ratio-0.5 dropout: dz = 2 * g * (y > 0), y = the post-dropout activation
         # ---- cls_score | bbox_pred: dY = head_grad [R_cap, ld] fp32 (zero rows for RoIs that were not kept)
         dyh = self._gact(1, R_cap, ld)
@@ -652,24 +659,28 @@ class RcnnTrainer(RpnTrainer):
         self._prep(1, R_cap, 4096, g=g6, y=self.fc6, out=dy6, tbuf=dy7T, times2=twice)       # dy7T's buffer now holds dy6^T
         if debug is not None:
             debug["fc6"] = dict(g_in=self._chw(g6), dy=self._chw(dy6))
-        p5T = self._tbuf(1, 49 * 512, 1, R_cap)
-        self._prep(1, R_cap, 49 * 512, g=self.pool5, tbuf=p5T)
-        self._fc_wgrad(dy7T, p5T, 4096, 49 * 512, self.grads("fc6/W"))
+        p5T = self._tbuf(1, 49 * C, 1, R_cap)
+        self._prep(1, R_cap, 49 * C, g=self.pool5, tbuf=p5T)
+        self._fc_wgrad(dy7T, p5T, 4096, 49 * C, self.grads("fc6/W"))
         train_ops.bias_grad(dy7T, 4096, self.grads("fc6/b"))
-        gp = self._gact(1, R_cap, 49 * 512, tag=1)
+        gp = self._gact(1, R_cap, 49 * C, tag=1)
         self._conv(dy6, self.packed["fc6"][2], self.zero_bias, 1, False, "roi_grads", out=gp)
-        # ---- RoI pooling backward -> gradient of conv5_3's output, then the trunk
+        # ---- RoI pooling backward -> gradient of the feature map, then the trunk
         self._roi_pool_backward(gp)
-        gfeat = self._gact(self.fh, self.fw, 512, tag=3)
-        self._prep(self.fh, self.fw, 512, g_f32=self.dfeat, out=gfeat)
+        gfeat = self._gact(self.fh, self.fw, C, tag=3)
+        self._prep(self.fh, self.fw, C, g_f32=self.dfeat, out=gfeat)
         if debug is not None:
             debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
-        self._backward_chain(self.layers[12::-1], gfeat, debug)
+        self._backward_trunk(gfeat, debug)
+
+    def _backward_trunk(self, g, debug=None):
+        """Backward through the trunk from g, the gradient of the feature map (ops.Act): the 13 VGG16 convolutions."""
+        self._backward_chain(self.layers[12::-1], g, debug)
 
     def _roi_pool_backward(self, g):
         """dfeat = the RoI pooling's backward of g (the gradient of pool5)."""
         if self.roi_ws is None:
-            self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_workspace_bytes(self.fh, self.fw, 512),),
+            self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_workspace_bytes(self.fh, self.fw, self.feat_ch),),
                                       dtype=torch.uint8, device=self.device)
         train_ops.roi_pool_backward(self.feat, self.prop.rois, self.prop.count, g, 7, 7, 1.0 / self.feat_stride, out=self.dfeat,
                                     ws=self.roi_ws)
@@ -960,7 +971,7 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         self.keep_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
         self.masks = torch.zeros((2, N, post_n, 4096), dtype=torch.uint8, device=dev) if dropout is not None else None
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rcnn_loss_batch
-        self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_batch_workspace_bytes(N, fh, fw, 512),),
+        self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_batch_workspace_bytes(N, fh, fw, self.feat_ch),),
                                   dtype=torch.uint8, device=dev)
         self.repack()
 

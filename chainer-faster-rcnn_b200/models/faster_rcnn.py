@@ -8,7 +8,8 @@ clip) is frcnn_b200.engine: hand-written sm_100a kernels behind the C ABI, repla
 per image shape.  Link names / parameter paths are the reference's, so `serializers.load_npz` of a
 reference checkpoint (forward.py:29) fills this model.  RPN training mode (:114-116) returns rpn_loss computed on the
 device (targets + losses + head gradient, models/region_proposal_network.py); RCNN training mode (:117-173) returns
-loss_rcnn from frcnn_b200.train_engine.RcnnTrainer (kept in `self.rcnn_trainer` for backward / update).
+loss_rcnn from frcnn_b200.train_engine.RcnnTrainer, or resnet_train.ResNetRcnnTrainer for a models.resnet.ResNet trunk
+(kept in `self.rcnn_trainer` for backward / update).
 """
 import os
 
@@ -134,6 +135,7 @@ class FasterRCNN(links.Link):
             # reference) -> RoI pool -> fc6/fc7 with dropout -> losses on the kept rows, all in frcnn_b200.train_engine.
             # The trainer (weights, stored activations) is kept in self.rcnn_trainer: .backward() / .update() complete the
             # train_rcnn.py step; loss_cls / cls_accuracy / loss_bbox are attributes like the reference's reports.
+            from frcnn_b200.resnet_train import ResNetRcnnTrainer
             from frcnn_b200.train_engine import RcnnTrainer
             fam = arrays.family(x)
             t = arrays.to_device(x)
@@ -146,10 +148,15 @@ class FasterRCNN(links.Link):
                 # a new image shape (VOC images vary in size) or externally changed parameters: the new trainer starts from
                 # the CURRENT parameters (synced above) and inherits the momentum of the one it replaces
                 old = tr
-                tr = RcnnTrainer(self.param_dict(), int(t.shape[2]), int(t.shape[3]), pl._anchors, precision=self.precision,
-                                 feat_stride=self._feat_stride, num_classes=self._num_classes, delta=float(self._rcnn_delta),
-                                 post_n=pl._post_nms_top_n, pre_n=pl._pre_nms_top_n, nms_thresh=pl._nms_thresh,
-                                 min_size=pl._min_size, device=t.device)
+                kw = dict(precision=self.precision, feat_stride=self._feat_stride, num_classes=self._num_classes,
+                          delta=float(self._rcnn_delta), post_n=pl._post_nms_top_n, pre_n=pl._pre_nms_top_n,
+                          nms_thresh=pl._nms_thresh, min_size=pl._min_size, device=t.device)
+                n_layers = getattr(self.trunk, "n_layers", None)
+                if n_layers is not None:                # models.resnet.ResNet trunk: frozen BatchNorm, as engine() runs it
+                    tr = ResNetRcnnTrainer(self.param_dict(), int(t.shape[2]), int(t.shape[3]), pl._anchors, n_layers=n_layers,
+                                           **kw)
+                else:
+                    tr = RcnnTrainer(self.param_dict(), int(t.shape[2]), int(t.shape[3]), pl._anchors, **kw)
                 if old is not None and old.index == tr.index:
                     tr.v_flat.copy_(old.v_flat)
                 self.__dict__["rcnn_trainer"], self.__dict__["_rcnn_trainer_key"] = tr, key
