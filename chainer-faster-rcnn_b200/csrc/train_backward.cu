@@ -228,11 +228,16 @@ __device__ __forceinline__ void prep_words(const PrepArgs& a, int h, int w, int 
 constexpr int PREP_PX = 256;
 constexpr int PREP_SMEM = (PREP_PX + 2) * 128 * 2;        // rows -1 .. 256, 128 B per plane
 
-// Image n of a batch: every NHWC pointer moves by one image, the transposed planes by one Kp block.
+// Image n of a batch: every NHWC pointer moves by one image, the transposed planes by one Kp block.  The source g and the
+// pooled map p are smaller than the H x W map, by a size that depends on the route: the 2x2 ceil pool's
+// [ceil(H/2)][ceil(W/2)], the 3x3/2 cover_all pool's [(H-2)/2+1][(W-2)/2+1] (pool3_words), the stride-2 subsample's
+// [ceil(H/2)][ceil(W/2)] with no p.
 __device__ __forceinline__ void prep_image(PrepArgs& a, int n) {
     if (n == 0) return;
-    const long img = (long)a.H * a.W * a.C, pooled = (long)((a.H + 1) / 2) * ((a.W + 1) / 2) * a.C;
-    const long g_img = a.p_hi != nullptr ? pooled : img;
+    const long img = (long)a.H * a.W * a.C;
+    const long pooled = a.route == ROUTE_POOL3 ? (long)((a.H - 2) / 2 + 1) * ((a.W - 2) / 2 + 1) * a.C
+                                               : (long)((a.H + 1) / 2) * ((a.W + 1) / 2) * a.C;
+    const long g_img = (a.p_hi != nullptr || a.route == ROUTE_STRIDE2) ? pooled : img;
     if (a.g_hi) a.g_hi += n * g_img;
     if (a.g_lo) a.g_lo += n * g_img;
     if (a.g_f32) a.g_f32 += n * (long)a.H * a.W * a.ld_f32;
@@ -508,6 +513,21 @@ int frcnn_grad_prepare_stride2(const void* g_hi, const void* g_lo, const void* y
     FRCNN_ENTRY();
     return grad_prepare("grad_prepare_stride2", g_hi, g_lo, nullptr, 0, y_hi, y_lo, nullptr, nullptr, 1, H, W, C, o_hi, o_lo,
                         t_hi, t_lo, planes, 0, (cudaStream_t)stream, ROUTE_STRIDE2);
+}
+
+int frcnn_maxpool3x3s2_backward_batch(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, const void* p_hi,
+                                      const void* p_lo, int N, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo,
+                                      void* stream) {
+    FRCNN_ENTRY();
+    return grad_prepare("maxpool3x3s2_backward_batch", g_hi, g_lo, nullptr, 0, y_hi, y_lo, p_hi, p_lo, N, H, W, C, o_hi, o_lo,
+                        t_hi, t_lo, 1, 0, (cudaStream_t)stream, ROUTE_POOL3);
+}
+
+int frcnn_grad_prepare_stride2_batch(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, int N, int H, int W,
+                                     int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo, int planes, void* stream) {
+    FRCNN_ENTRY();
+    return grad_prepare("grad_prepare_stride2_batch", g_hi, g_lo, nullptr, 0, y_hi, y_lo, nullptr, nullptr, N, H, W, C, o_hi,
+                        o_lo, t_hi, t_lo, planes, 0, (cudaStream_t)stream, ROUTE_STRIDE2);
 }
 
 int frcnn_wgrad_reduce(const float* parts, int groups, int splits, int M_parts, int M, int ld, int N, float scale, float* dw,

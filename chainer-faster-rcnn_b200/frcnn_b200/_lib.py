@@ -112,6 +112,10 @@ SIGNATURES = {
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "frcnn_grad_prepare_stride2": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_int, c_void_p]),
+    "frcnn_maxpool3x3s2_backward_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                                  c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_grad_prepare_stride2_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                 c_void_p, c_void_p, c_int, c_void_p]),
     "frcnn_fold_batchnorm": (c_int, [c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "frcnn_wgrad_reduce_scaled": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_wgrad_reduce": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),

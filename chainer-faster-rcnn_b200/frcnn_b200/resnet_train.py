@@ -40,7 +40,8 @@ import torch
 from . import ops, train_ops
 from ._lib import FrcnnError
 from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
-from .train_engine import RcnnTrainer, RpnTrainer, _fc6_to_hwc, _rcnn_params, _rpn_params
+from .train_engine import (CanvasRcnnTrainer, CanvasRpnTrainer, RcnnTrainer, RpnTrainer, _fc6_to_hwc, _rcnn_params,
+                           _rpn_params)
 
 SUBSAMPLE_MODES = ("device", "numpy", "none")
 
@@ -65,14 +66,20 @@ def trunk_convs(n_layers):
 class _ResNetTrunk(object):
     """The ResNet trunk with frozen BatchNorm, shared by ResNetRpnTrainer and ResNetRcnnTrainer (ahead of RpnTrainer /
     RcnnTrainer in their MRO): the layer table and BN constants, the activations, the forward launches, the fold + repack,
-    and the bottleneck backward (_backward_trunk, from the gradient of the feature map)."""
+    and the bottleneck backward (_backward_trunk, from the gradient of the feature map).  Every launch goes through the
+    trainer's launch layer (_conv, _res_conv, _pool3, _subsample, _prep, _pool3_backward, _prep_stride2, _pack_input), so
+    the same code runs one image and, with _CanvasSteps' launches, a canvas.  A trunk level is an index into
+    frcnn_resnet_level_extents' five: 0 conv1, 1 pool1 / res2, 2 res3, 3 res4, 4 res5."""
     feat_ch = 2048
+    halvings = 4                        # the feature map's level (res5)
+    first_layer = (7, 2, 3, CONV1_KPAD)
 
     def _init_trunk(self, params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                    process_group, extra_layers, extra_params, need, load_transform=None):
+                    process_group, extra_layers, extra_params, need, load_transform=None, lead=()):
         """Checks the options and parameters (FrcnnError before anything is allocated), then lays out the flat buffers over
         the trunk convolutions + extra_layers and extra_params, the frozen-BN constants and the trunk activations.
-        need: {name: shape} of the non-trunk parameters the step reads."""
+        need: {name: shape} of the non-trunk parameters the step reads; lead: the leading [N] of a canvas trainer's
+        activations."""
         who = type(self).__name__
         if n_layers not in RESNET_BLOCKS:
             raise FrcnnError("%s: n_layers must be one of %s (got %r)" % (who, sorted(RESNET_BLOCKS), n_layers))
@@ -95,7 +102,7 @@ class _ResNetTrunk(object):
                                  % (who, k, sh, None if k not in params else tuple(np.shape(params[k]))))
         layers = [dict(name=n, bn=bn, cin=ci, cout=co, k=k, bias=n == "trunk/conv1") for n, bn, ci, co, k in convs]
         self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          layers + list(extra_layers), extra_params, load_transform)
+                          layers + list(extra_layers), extra_params, load_transform, lead)
         dev = self.device
         # ---- frozen BN: s (float64) per conv, the constant folded bias of every conv but conv1, the folded-weight buffers
         T = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)     # noqa: E731
@@ -114,20 +121,20 @@ class _ResNetTrunk(object):
         self.bn_params = {k: np.asarray(params[k]).copy() for k in want if "/bn" in k}
         # ---- activations (ResNetForwardPlan._alloc_trunk's, every one kept for backward)
         act = self._act
-        self.x_in = torch.zeros((3, H, W), dtype=torch.float32, device=dev)
+        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
         self.x_col = act(Ho, Wo, CONV1_KPAD)
         self.c1 = act(Ho, Wo, 64)
         h, w = (Ho - 2) // 2 + 1, (Wo - 2) // 2 + 1
         self.p1 = act(h, w, 64)
         self.c1_hw = (Ho, Wo)
         self.blocks = []
-        x = self.p1
+        x, level = self.p1, 1
         for stage, blk, cin, mid, cout, stride, proj in block_list(n_layers):
             B = dict(name="trunk/%s/%s" % (stage, blk), x=x, stride=stride, proj=proj, cin=cin, mid=mid, cout=cout)
             if stride == 2:
-                h, w = (h + 1) // 2, (w + 1) // 2
+                h, w, level = (h + 1) // 2, (w + 1) // 2, level + 1
                 B["xs"] = act(h, w, cin)
-            B["H"], B["W"] = h, w
+            B["H"], B["W"], B["level"] = h, w, level
             B["y1"], B["y2"] = act(h, w, mid), act(h, w, mid)
             if proj:
                 B["sc"] = act(h, w, cout)
@@ -149,6 +156,9 @@ class _ResNetTrunk(object):
     def _pack_image_layer(self, w, out=None):
         return ops.pack_conv_weights_im2col_general(w, CONV1_KPAD, precision=self.precision, out=out)
 
+    def _pack_image(self, x, out):
+        ops.pack_image_im2col_general(x, *self.first_layer, out=out)
+
     def _repack_convs(self):
         """Folds and repacks every trunk convolution, then repacks the step's other convolutions (the RPN 3x3, if trained)."""
         for n, L in self.conv.items():
@@ -165,31 +175,31 @@ class _ResNetTrunk(object):
         return {n: (L["wf"].cpu().numpy().copy(), L["bf"].cpu().numpy().copy()) for n, L in self.conv.items()}
 
     # ---------------------------------------------------------------- forward
-    def _forward_trunk(self, x_chw):
-        """ResNetForwardPlan._run_trunk's launches on the folded weights, with every activation kept."""
+    def _forward_trunk(self, x_chw=None):
+        """ResNetForwardPlan._run_trunk's launches (ResNetBatchPlan's on a canvas) on the folded weights, with every
+        activation kept."""
         pk = self.packed
-        self.x_in.copy_(x_chw, non_blocking=True)
-        ops.pack_image_im2col_general(self.x_in, 7, 2, 3, CONV1_KPAD, out=self.x_col)
-        (hi, lo), b, _ = pk["trunk/conv1"]
-        ops.conv2d(self.x_col, hi, lo, b, 1, True, out=self.c1)
-        ops.maxpool3x3s2_ceil(self.c1, out=self.p1)
+        self._pack_input(x_chw)
+        fwd, b, _ = pk["trunk/conv1"]
+        self._conv(self.x_col, fwd, b, 1, True, 0, out=self.c1)
+        self._pool3(self.c1, self.p1, 0)
         for B in self.blocks:
-            x = B["x"]
+            x, lv = B["x"], B["level"]
             if B["stride"] == 2:
-                ops.subsample2x(x, out=B["xs"])
+                self._subsample(x, B["xs"])
                 x = B["xs"]
-            (hi, lo), b, _ = pk[B["name"] + "/conv1"]
-            ops.conv2d(x, hi, lo, b, 1, True, out=B["y1"])
-            (hi, lo), b, _ = pk[B["name"] + "/conv2"]
-            ops.conv2d(B["y1"], hi, lo, b, 3, True, out=B["y2"])
+            fwd, b, _ = pk[B["name"] + "/conv1"]
+            self._conv(x, fwd, b, 1, True, lv, out=B["y1"])
+            fwd, b, _ = pk[B["name"] + "/conv2"]
+            self._conv(B["y1"], fwd, b, 3, True, lv, out=B["y2"])
             if B["proj"]:
-                (hi, lo), b, _ = pk[B["name"] + "/conv4"]
-                ops.conv2d(x, hi, lo, b, 1, False, out=B["sc"])
+                fwd, b, _ = pk[B["name"] + "/conv4"]
+                self._conv(x, fwd, b, 1, False, lv, out=B["sc"])
                 res = B["sc"]
             else:
                 res = B["x"]
-            (hi, lo), b, _ = pk[B["name"] + "/conv3"]
-            ops.conv2d_res(B["y2"], hi, lo, b, 1, True, res, out=B["out"])
+            fwd, b, _ = pk[B["name"] + "/conv3"]
+            self._res_conv(B["y2"], fwd, b, 1, True, res, lv, B["out"])
         self.feat = self.blocks[-1]["out"]
         return self.feat
 
@@ -198,21 +208,22 @@ class _ResNetTrunk(object):
         return B["xs"] if B["stride"] == 2 else B["x"]
 
     # ---------------------------------------------------------------- backward
-    def _dgrad(self, name, dy, ksize, cin, tag, res=None):
-        """The data gradient of `name` (its folded weights), plus `res` (frcnn_conv2d_res, relu = 0) when given."""
-        _, _, (dhi, dlo) = self.packed[name]
-        h, w, _ = dy.hi.shape
+    def _dgrad(self, name, dy, ksize, cin, tag, level, res=None):
+        """The data gradient of `name` (its folded weights) at trunk level `level`, plus `res` (frcnn_conv2d_res,
+        relu = 0) when given."""
+        dg = self.packed[name][2]
+        h, w, _ = dy.hi.shape[-3:]
         g = self._gact(h, w, cin, tag=tag)
         if res is None:
-            ops.conv2d(dy, dhi, dlo, self.zero_bias, ksize, False, out=g)
+            self._conv(dy, dg, self.zero_bias, ksize, False, level, out=g)
         else:
-            ops.conv2d_res(dy, dhi, dlo, self.zero_bias, ksize, False, res, out=g)
+            self._res_conv(dy, dg, self.zero_bias, ksize, False, res, level, g)
         return g
 
     def _backward_trunk(self, g, debug=None):
         """Backward through the bottleneck blocks (last first), pool1 and conv1 from g, the gradient of the feature map
         (ops.Act [fh, fw, 2048]).  debug: receives the per-convolution entries described in ResNetRpnTrainer.backward."""
-        dbg = (lambda a: a.to_chw_f32().clone()) if debug is not None else None      # noqa: E731
+        dbg = (lambda a: self._chw(a).clone()) if debug is not None else None        # noqa: E731
         # ---- the bottleneck blocks, last first; `half`: g is w.r.t. the stride-2 subsample of this block's output
         half = False
         for B in reversed(self.blocks):
@@ -222,9 +233,9 @@ class _ResNetTrunk(object):
         Ho, Wo = self.c1_hw
         dz = self._gact(Ho, Wo, 64)
         dzT = self._tbuf(1, 64, Ho, Wo)
-        train_ops.maxpool3x3s2_backward(g, self.c1, self.p1, out=dz, tbuf=dzT)
+        self._pool3_backward(g, self.c1, self.p1, dz, dzT)
         xT = self._tbuf(1, CONV1_KPAD, Ho, Wo)
-        train_ops.grad_prepare(Ho, Wo, CONV1_KPAD, g=self.x_col, tbuf=xT)
+        self._prep(Ho, Wo, CONV1_KPAD, g=self.x_col, tbuf=xT)
         L = self.conv["trunk/conv1"]
         dwc = torch.empty((64, CONV1_KPAD), dtype=torch.float32, device=self.device)
         self._wgrad(dzT, xT, 64, CONV1_KPAD, 1, dwc, scale=L["s"])
@@ -238,58 +249,101 @@ class _ResNetTrunk(object):
     def _backward_block(self, B, g, half, debug):
         """One bottleneck block's backward; g: gradient w.r.t. B["out"] (or its stride-2 subsample when `half`).  Returns
         the gradient w.r.t. the block's conv input (B["xs"] for a stride-2 block, else B["x"])."""
-        dbg = lambda a: a.to_chw_f32().clone()        # noqa: E731
-        h, w, cin, mid, cout = B["H"], B["W"], B["cin"], B["mid"], B["cout"]
+        dbg = lambda a: self._chw(a).clone()          # noqa: E731
+        h, w, cin, mid, cout, lv = B["H"], B["W"], B["cin"], B["mid"], B["cout"], B["level"]
         base = B["name"]
         s = lambda i: self.conv["%s/conv%d" % (base, i)]["s"]       # noqa: E731
         # dz: w.r.t. conv3's (folded) output and the shortcut, = g * (out > 0)
         dz = self._gact(h, w, cout)
         dzT = self._tbuf(1, cout, h, w, tag=1)
         if half:
-            train_ops.grad_prepare_stride2(h, w, cout, g, y=B["out"], out=dz, tbuf=dzT)
+            self._prep_stride2(h, w, cout, g, B["out"], dz, dzT)
         else:
-            train_ops.grad_prepare(h, w, cout, g=g, y=B["out"], out=dz, tbuf=dzT)
+            self._prep(h, w, cout, g=g, y=B["out"], out=dz, tbuf=dzT)
         # conv3 (1x1, mid -> cout)
         y2T = self._tbuf(1, mid, h, w, tag=2)
-        train_ops.grad_prepare(h, w, mid, g=B["y2"], tbuf=y2T)
+        self._prep(h, w, mid, g=B["y2"], tbuf=y2T)
         self._wgrad(dzT, y2T, cout, mid, 1, self.grads(base + "/conv3/W"), scale=s(3))
-        g2 = self._dgrad(base + "/conv3", dz, 1, mid, tag=1)
+        g2 = self._dgrad(base + "/conv3", dz, 1, mid, 1, lv)
         if debug is not None:
             debug[base + "/conv3"] = dict(g_in=dbg(g), dy=dbg(dz), g_out=dbg(g2))
         # conv2 (3x3, mid -> mid)
         dy2 = self._gact(h, w, mid)
         dyT = self._tbuf(1, mid, h, w)
-        train_ops.grad_prepare(h, w, mid, g=g2, y=B["y2"], out=dy2, tbuf=dyT)
+        self._prep(h, w, mid, g=g2, y=B["y2"], out=dy2, tbuf=dyT)
         if debug is not None:                              # g2's buffer receives g1 below
             debug[base + "/conv2"] = dict(g_in=dbg(g2), dy=dbg(dy2))
         y1T = self._tbuf(3, mid, h, w)
-        train_ops.grad_prepare(h, w, mid, g=B["y1"], tbuf=y1T)
+        self._prep(h, w, mid, g=B["y1"], tbuf=y1T)
         self._wgrad(dyT, y1T, mid, mid, 9, self.grads(base + "/conv2/W"), scale=s(2))
-        g1 = self._dgrad(base + "/conv2", dy2, 3, mid, tag=1)
+        g1 = self._dgrad(base + "/conv2", dy2, 3, mid, 1, lv)
         if debug is not None:
             debug[base + "/conv2"]["g_out"] = dbg(g1)
         # conv1 (1x1, cin -> mid) and conv4 (1x1, cin -> cout) on the same input
         dy1 = self._gact(h, w, mid)
-        train_ops.grad_prepare(h, w, mid, g=g1, y=B["y1"], out=dy1, tbuf=dyT)
+        self._prep(h, w, mid, g=g1, y=B["y1"], out=dy1, tbuf=dyT)
         if debug is not None:
             debug[base + "/conv1"] = dict(g_in=dbg(g1), dy=dbg(dy1))
         xT = self._tbuf(1, cin, h, w, tag=3)
-        train_ops.grad_prepare(h, w, cin, g=self.input_of(B), tbuf=xT)
+        self._prep(h, w, cin, g=self.input_of(B), tbuf=xT)
         self._wgrad(dyT, xT, mid, cin, 1, self.grads(base + "/conv1/W"), scale=s(1))
         if B["proj"]:
             self._wgrad(dzT, xT, cout, cin, 1, self.grads(base + "/conv4/W"), scale=s(4))
-            res = self._dgrad(base + "/conv4", dz, 1, cin, tag=2)
+            res = self._dgrad(base + "/conv4", dz, 1, cin, 2, lv)
             if debug is not None:
                 debug[base + "/conv4"] = dict(g_in=dbg(g), dy=dbg(dz), g_out=dbg(res))
         else:
             res = dz
-        gx = self._dgrad(base + "/conv1", dy1, 1, cin, tag=3, res=res)
+        gx = self._dgrad(base + "/conv1", dy1, 1, cin, 3, lv, res=res)
         if debug is not None:
             debug[base + "/conv1"]["g_out"] = dbg(gx)
         return gx
 
 
-class ResNetRpnTrainer(_ResNetTrunk, RpnTrainer):
+def _rpn_need(A):
+    """The non-trunk parameters of the RPN step: the RPN 3x3 conv (2048 -> 512) and its twin heads."""
+    need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
+    need.update(_rpn_params(A))
+    return need
+
+
+def _rcnn_need(A, head):
+    """The parameters the RCNN step reads besides the trunk: the frozen RPN and the head."""
+    need = _rpn_need(A)
+    need.update(head)
+    return need
+
+
+class _ResNetRpnStep(_ResNetTrunk):
+    """The RPN step's backward on the ResNet trunk, shared by ResNetRpnTrainer and CanvasResNetRpnTrainer."""
+
+    def backward(self, debug=None):
+        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter (on a canvas: the sum over the slots).
+        debug: a dict that receives, per conv name, float32 (C,H,W) copies ([N,C,H,W] on a canvas) of the incoming gradient
+        ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the block output for conv3 / conv4, at the subsampled
+        resolution when the next block reads it through the stride-2 subsample), the masked / routed gradient w.r.t. the
+        (folded) conv output ("dy") and the data gradient the conv passes on ("g_out"; for a block's conv1 the summed
+        gradient of the block input, residual included)."""
+        dbg = (lambda a: self._chw(a).clone()) if debug is not None else None        # noqa: E731
+        g = self._backward_heads(debug)
+        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
+        R = self.rpn_layer
+        fh, fw = self.fh, self.fw
+        dy = self._gact(fh, fw, 512)
+        dyT = self._tbuf(1, 512, fh, fw)
+        self._prep(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
+        xT = self._tbuf(3, 2048, fh, fw)
+        self._prep(fh, fw, 2048, g=self.feat, tbuf=xT)
+        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
+        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
+        g_in = g
+        g = self._dgrad(R["name"], dy, 3, 2048, 3, self.halvings)
+        if debug is not None:
+            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
+        self._backward_trunk(g, debug)
+
+
+class ResNetRpnTrainer(_ResNetRpnStep, RpnTrainer):
     """Weights, optimizer state and buffers of the RPN-mode training step with the ResNet trunk for one image shape.  The
     surface is RpnTrainer's: forward / backward(debug) / update / step / weights / grads / export_params, subsample modes
     "device", "numpy" and "none", disable_pos.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming;
@@ -300,10 +354,8 @@ class ResNetRpnTrainer(_ResNetTrunk, RpnTrainer):
         if subsample not in SUBSAMPLE_MODES:
             raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
         A = len(anchors)
-        need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
-        need.update(_rpn_params(A))
         self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), need)
+                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), _rpn_need(A))
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
         self.repack()
@@ -313,31 +365,6 @@ class ResNetRpnTrainer(_ResNetTrunk, RpnTrainer):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
         self._check_input(x_chw, gt_boxes)
         return super(ResNetRpnTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos)
-
-    # ---------------------------------------------------------------- backward
-    def backward(self, debug=None):
-        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter.  debug: a dict that receives, per conv
-        name, float32 (C,H,W) copies of the incoming gradient ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the
-        block output for conv3 / conv4, at the subsampled resolution when the next block reads it through the stride-2
-        subsample), the masked / routed gradient w.r.t. the (folded) conv output ("dy") and the data gradient the conv
-        passes on ("g_out"; for a block's conv1 the summed gradient of the block input, residual included)."""
-        dbg = (lambda a: a.to_chw_f32().clone()) if debug is not None else None      # noqa: E731
-        g = self._backward_heads(debug)
-        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
-        R = self.rpn_layer
-        fh, fw = self.fh, self.fw
-        dy = self._gact(fh, fw, 512)
-        dyT = self._tbuf(1, 512, fh, fw)
-        train_ops.grad_prepare(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
-        xT = self._tbuf(3, 2048, fh, fw)
-        train_ops.grad_prepare(fh, fw, 2048, g=self.feat, tbuf=xT)
-        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
-        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
-        g_in = g
-        g = self._dgrad(R["name"], dy, 3, 2048, tag=3)
-        if debug is not None:
-            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
-        self._backward_trunk(g, debug)
 
 
 class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
@@ -354,11 +381,8 @@ class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
                  sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
         nc = self.num_classes = num_classes
         head = _rcnn_params(nc, self.feat_ch)
-        need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
-        need.update(_rpn_params(len(anchors)))
-        need.update(head)
         self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [], head, need, load_transform=_fc6_to_hwc)
+                         process_group, [], head, _rcnn_need(len(anchors), head), load_transform=_fc6_to_hwc)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self._init_one_image_rcnn(sample, seed, dropout)
         self.repack()
@@ -367,3 +391,58 @@ class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RcnnTrainer."""
         self._check_input(x_chw, gt_boxes)
         return super(ResNetRcnnTrainer, self).forward(x_chw, gt_boxes, im_info, keep_inds, masks)
+
+
+class CanvasResNetRpnTrainer(_ResNetRpnStep, CanvasRpnTrainer):
+    """CanvasRpnTrainer's step with the ResNet trunk: N images of different sizes per update (put / put_raw / forward /
+    backward(debug) / update / run / step / step_raw, per-slot losses [N, 4]), one set of weights with ResNetRpnTrainer's
+    parameters, frozen BatchNorm and folded_params().
+
+    The trunk is _ResNetTrunk's, launch for launch, through _CanvasSteps' launches: the first launch of the step derives
+    the extents of the five levels from the staged sizes (frcnn_resnet_level_extents, as ResNetCanvasBatchPlan does),
+    every convolution, pool and RPN / target / loss launch reads its level's [N][2] extents with halvings 0, and the
+    backward runs the _batch re-layouts (frcnn_maxpool3x3s2_backward_batch, frcnn_grad_prepare_stride2_batch,
+    frcnn_grad_prepare_batch) and weight-gradient GEMMs over K = N*Kp.  So the gradient is the SUM of the N per-image
+    gradients, followed by one WeightDecay + MomentumSGD update; inside each image every activation, masked gradient and
+    data gradient equals ResNetRpnTrainer's on that image alone, bit for bit.
+
+    subsample "device": slot n of step t draws with seed + t*N + n; "list": put() takes per-image disable lists; "none":
+    labels before subsampling.  raw_input=True: put_raw takes raw photos and the VOC transform runs on the device,
+    straight into conv1's 7x7/2 im2col planes.  The step is captured after the first call in a single process and runs
+    eagerly with a process group of more than one rank; the gradient exchange is then one bucket after backward (the
+    early deep-layer bucket is keyed to the VGG16 trunk's conv4_1)."""
+
+    def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
+                 weight_decay=0.0005, feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256,
+                 device="cuda", process_group=None, raw_input=False):
+        self._rpn_options(N, subsample, max_gt)
+        self.N, self.max_gt = int(N), int(max_gt)
+        A = len(anchors)
+        self._init_trunk(params, Hc, Wc, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
+                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), _rpn_need(A),
+                         lead=(self.N,))
+        self.level_ext = torch.zeros((5, self.N, 2), dtype=torch.int32, device=self.device)
+        self._init_canvas_rpn(Hc, Wc, loss_lambda, delta, subsample, seed, raw_input)
+
+
+class CanvasResNetRcnnTrainer(_ResNetTrunk, CanvasRcnnTrainer):
+    """CanvasRcnnTrainer's step with the ResNet trunk: N images of different sizes per update, with ResNetRcnnTrainer's
+    parameters (the head on res5's 2048-channel RoIs, fc6 with K = 2048*49; the RPN frozen and packed once; frozen
+    BatchNorm) and CanvasRcnnTrainer's surface, sample ("device" | "list") and dropout ("device" | "explicit" | None)
+    modes.  The trunk runs as in CanvasResNetRpnTrainer; RoI pooling and its backward read res5's level extents.  Inside
+    each image every activation and data gradient equals ResNetRcnnTrainer's on that image with the same kept rows and
+    masks, bit for bit; the gradient is the sum over the slots, then one WeightDecay + MomentumSGD update.  The gradient
+    exchange of a multi-rank run is one bucket after backward, as in CanvasResNetRpnTrainer."""
+
+    def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
+                 weight_decay=0.0005, feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7,
+                 min_size=16, sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None,
+                 raw_input=False):
+        self._rcnn_options(N, sample, dropout, max_gt, post_n)
+        self.N, self.max_gt = int(N), int(max_gt)
+        nc = self.num_classes = num_classes
+        head = _rcnn_params(nc, self.feat_ch)
+        self._init_trunk(params, Hc, Wc, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
+                         process_group, [], head, _rcnn_need(len(anchors), head), load_transform=_fc6_to_hwc, lead=(self.N,))
+        self.level_ext = torch.zeros((5, self.N, 2), dtype=torch.int32, device=self.device)
+        self._init_canvas_rcnn(params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input)

@@ -39,6 +39,7 @@ class _ConvTrainer(object):
     in-place repack.  _CanvasSteps overrides the launches for a canvas, so every step is written once."""
     halvings = None             # the feature map's canvas level (the VGG16 trunk's: set by _init_common)
     feat_ch = 512               # channels of the feature map the RPN and the RoI pooling read (VGG16's conv5_3)
+    first_layer = (3, 1, 1, 32)     # ksize, stride, pad, K_pad of the first layer's im2col input
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                      extra_layers, extra_params, load_transform=None, lead=()):
@@ -128,8 +129,9 @@ class _ConvTrainer(object):
 
     # ---------------------------------------------------------------- launches over one image (_CanvasSteps: a canvas)
     def _conv(self, x, planes, bias, ksize, relu, at, **kw):
-        """frcnn_conv2d.  at: where the rows live -- a trunk level given by its halvings (nothing to pass for one image),
-        "rois": the head's forward, which computes the first prop.count rows, or "roi_grads": the head's data gradients."""
+        """frcnn_conv2d.  at: where the rows live -- a trunk level (nothing to pass for one image; on a canvas
+        _CanvasSteps._level resolves it), "rois": the head's forward, which computes the first prop.count rows, or
+        "roi_grads": the head's data gradients."""
         if at == "rois":
             kw["m_valid"] = self.prop.count
         return ops.conv2d(x, planes[0], planes[1], bias, ksize, relu, **kw)
@@ -139,6 +141,28 @@ class _ConvTrainer(object):
 
     def _pool(self, y, out):
         ops.maxpool2x2_ceil(y, out=out)
+
+    def _pack_image(self, x, out):
+        """The first layer's im2col planes of one image."""
+        ops.pack_image_im2col(x, out=out)
+
+    # the ResNet trunk's launches (resnet_train._ResNetTrunk); `at` as in _conv
+    def _res_conv(self, x, planes, bias, ksize, relu, res, at, out):
+        """frcnn_conv2d_res: y = act(conv(x) + bias + res)."""
+        ops.conv2d_res(x, planes[0], planes[1], bias, ksize, relu, res, out=out)
+
+    def _pool3(self, y, out, at):
+        """The 3x3/2 cover_all max-pool of y (at: y's level)."""
+        ops.maxpool3x3s2_ceil(y, out=out)
+
+    def _subsample(self, x, out):
+        ops.subsample2x(x, out=out)
+
+    def _pool3_backward(self, g, y, p, out, tbuf):
+        train_ops.maxpool3x3s2_backward(g, y, p, out=out, tbuf=tbuf)
+
+    def _prep_stride2(self, h, w, c, g, y, out, tbuf):
+        train_ops.grad_prepare_stride2(h, w, c, g, y=y, out=out, tbuf=tbuf)
 
     def _chw(self, act):
         """float32 (C,H,W) copy of an Act (debug)."""
@@ -274,7 +298,7 @@ class RpnTrainer(_ConvTrainer):
     def _pack_input(self, x_chw):
         """The trunk's first launch: the image into the first layer's im2col planes x_col."""
         self.x_in.copy_(x_chw, non_blocking=True)
-        ops.pack_image_im2col(self.x_in, out=self.x_col)
+        self._pack_image(self.x_in, self.x_col)
 
     def _forward_trunk(self, x_chw=None):
         """The 13 VGG16 convolutions with every output kept (pools un-fused: backward needs the un-pooled maps)."""
@@ -697,6 +721,15 @@ class _CanvasSteps(object):
     the staged ground truth, the launches over the canvas (the _ext convolutions, zero outside each image, and the _batch
     re-layouts) that override _ConvTrainer's, and the capture-then-replay step."""
     raw_input = False           # True: the input is RawPhotoInput's training block (put_raw / step_raw)
+    level_ext = None            # the ResNet trunk's per-level extents int32 [5, N, 2] (None: the VGG16 trunk's halvings)
+
+    def _canvas_options(self, N, max_gt):
+        """Raises FrcnnError for a bad slot count or max_gt (before anything is allocated)."""
+        who = type(self).__name__
+        if int(N) != N or N < 1:
+            raise FrcnnError("%s needs N >= 1 slots (got %r)" % (who, N))
+        if int(max_gt) < 1:
+            raise FrcnnError("%s: max_gt must be at least 1" % who)
 
     def _canvas_init(self, N, Hc, Wc, max_gt, seed, raw_input):
         dev = self.device
@@ -710,9 +743,16 @@ class _CanvasSteps(object):
         self.graph = None
 
     # ---------------------------------------------------------------- launches over the canvas
+    def _level(self, at):
+        """(extents, halvings) of the trunk level `at`: the image extents and `at` halvings on the VGG16 trunk; on the ResNet
+        trunk, whose levels are not ceil(e / 2^k) (pool1 is (c - 2) / 2 + 1), level `at` of level_ext with halvings 0."""
+        if self.level_ext is None:
+            return self.extents, at
+        return self.level_ext[at], 0
+
     def _conv(self, x, planes, bias, ksize, relu, at, **kw):
         """frcnn_conv2d_batch_ext over the trunk level's extents, or over the head's (1, R_n) for "rois" / "roi_grads"."""
-        ext, k = (self.head_ext, 0) if at in ("rois", "roi_grads") else (self.extents, at)
+        ext, k = (self.head_ext, 0) if at in ("rois", "roi_grads") else self._level(at)
         return ops.conv2d_batch(x, planes[0], planes[1], bias, ksize, relu, extents=ext, halvings=k, **kw)
 
     def _prep(self, h, w, c, **kw):
@@ -721,13 +761,32 @@ class _CanvasSteps(object):
     def _pool(self, y, out):
         ops.maxpool2x2_ceil_batch(y, out=out)
 
+    def _res_conv(self, x, planes, bias, ksize, relu, res, at, out):
+        ext, k = self._level(at)
+        ops.conv2d_res_batch(x, planes[0], planes[1], bias, ksize, relu, res, out=out, extents=ext, halvings=k)
+
+    def _pool3(self, y, out, at):
+        ops.maxpool3x3s2_ceil_batch(y, out=out, extents=self._level(at)[0])
+
+    def _subsample(self, x, out):
+        ops.subsample2x_batch(x, out=out)          # 0 outside each image, as its input is
+
+    def _pool3_backward(self, g, y, p, out, tbuf):
+        train_ops.maxpool3x3s2_backward_batch(self.N, g, y, p, out=out, tbuf=tbuf)
+
+    def _prep_stride2(self, h, w, c, g, y, out, tbuf):
+        train_ops.grad_prepare_stride2_batch(self.N, h, w, c, g, y=y, out=out, tbuf=tbuf)
+
     def _chw(self, act):
         """[N, C, H, W] float32 copy of an [N, H, W, C] Act (debug)."""
         return torch.stack([ops.Act(act.hi[n], None if act.lo is None else act.lo[n]).to_chw_f32() for n in range(self.N)])
 
     def _pack_input(self, x_chw=None):
-        """The staged slots into x_col; raw photos are resized on the way, and their boxes scaled into gt."""
-        self.input.pack_im2col(self.x_col, 3, 1, 1, 32)
+        """The staged slots into x_col; raw photos are resized on the way, and their boxes scaled into gt.  On the ResNet
+        trunk the first launch derives every level's extents from the staged sizes, so a captured step re-derives them."""
+        if self.level_ext is not None:
+            ops.resnet_level_extents(self.extents, self.H, self.W, out=self.level_ext)
+        self.input.pack_im2col(self.x_col, *self.first_layer)
         if self.raw_input:
             self.input.scale_gt(self.gt, self.gt_counts)
 
@@ -830,15 +889,21 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
                  process_group=None, raw_input=False):
-        if int(N) != N or N < 1:
-            raise FrcnnError("CanvasRpnTrainer needs N >= 1 slots (got %r)" % (N,))
-        if subsample not in self._MODES:
-            raise FrcnnError("CanvasRpnTrainer: subsample must be one of %s" % (sorted(self._MODES),))
-        if int(max_gt) < 1:
-            raise FrcnnError("CanvasRpnTrainer: max_gt must be at least 1")
+        self._rpn_options(N, subsample, max_gt)
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], _rpn_params(len(anchors)), lead=(N,))
+        self._init_canvas_rpn(Hc, Wc, loss_lambda, delta, subsample, seed, raw_input)
+
+    def _rpn_options(self, N, subsample, max_gt):
+        self._canvas_options(N, max_gt)
+        if subsample not in self._MODES:
+            raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
+
+    def _init_canvas_rpn(self, Hc, Wc, loss_lambda, delta, subsample, seed, raw_input):
+        """After the trunk: the RPN head, the canvas input, the batched anchor targets and the subsampling lists; then the
+        first repack."""
+        N, max_gt = self.N, self.max_gt
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         dev = self.device
@@ -877,21 +942,22 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         return scales
 
     def _check_disable(self, call, n_images, disable_pos):
+        who = type(self).__name__
         if disable_pos is not None:
             disable_pos = list(disable_pos)
             if self.subsample != "list":
-                raise FrcnnError("CanvasRpnTrainer.%s: disable lists need subsample='list' (the trainer has %r)" % (call, self.subsample))
+                raise FrcnnError("%s.%s: disable lists need subsample='list' (the trainer has %r)" % (who, call, self.subsample))
             if len(disable_pos) != n_images:
-                raise FrcnnError("CanvasRpnTrainer.%s: %d images and %d disable lists" % (call, n_images, len(disable_pos)))
+                raise FrcnnError("%s.%s: %d images and %d disable lists" % (who, call, n_images, len(disable_pos)))
             if any(int(d.numel()) > self.targets.cap for d in disable_pos):
-                raise FrcnnError("CanvasRpnTrainer.%s: a disable list is longer than %d anchors" % (call, self.targets.cap))
+                raise FrcnnError("%s.%s: a disable list is longer than %d anchors" % (who, call, self.targets.cap))
         return disable_pos
 
     # ---------------------------------------------------------------- forward
     def forward(self):
         """Forward over the staged canvas, the anchor targets and the per-slot losses (float32 [N, 4] device buffer:
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss; zeros for an empty slot)."""
-        ext, k, R = self.extents, self.halvings, self.rpn_layer
+        (ext, k), R = self._level(self.halvings), self.rpn_layer
         self._rpn_forward(self._forward_trunk(), self.packed[R["name"]], self.packed["heads"], R["y"], self.head_ld, self.head_out)
         mode = self._MODES[self.subsample]
         train_ops.anchor_targets_batch(self.anchors, self.A, self.feat_stride, ext, self.im_info, self.gt, self.gt_counts,
@@ -942,20 +1008,27 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
                  sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False):
-        if int(N) != N or N < 1:
-            raise FrcnnError("CanvasRcnnTrainer needs N >= 1 slots (got %r)" % (N,))
-        if sample not in self._SAMPLE:
-            raise FrcnnError("CanvasRcnnTrainer: sample must be one of %s" % (sorted(self._SAMPLE),))
-        if dropout not in self._DROPOUT:
-            raise FrcnnError("CanvasRcnnTrainer: dropout must be one of %s" % (self._DROPOUT,))
-        if int(max_gt) < 1:
-            raise FrcnnError("CanvasRcnnTrainer: max_gt must be at least 1")
-        if not 1 <= int(post_n) <= 4096:
-            raise FrcnnError("CanvasRcnnTrainer: post_n must be in [1, 4096] (got %r)" % (post_n,))
+        self._rcnn_options(N, sample, dropout, max_gt, post_n)
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
         nc = self.num_classes = num_classes
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           [], _rcnn_params(nc), load_transform=_fc6_to_hwc, lead=(N,))
+        self._init_canvas_rcnn(params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input)
+
+    def _rcnn_options(self, N, sample, dropout, max_gt, post_n):
+        who = type(self).__name__
+        self._canvas_options(N, max_gt)
+        if sample not in self._SAMPLE:
+            raise FrcnnError("%s: sample must be one of %s" % (who, sorted(self._SAMPLE)))
+        if dropout not in self._DROPOUT:
+            raise FrcnnError("%s: dropout must be one of %s" % (who, self._DROPOUT))
+        if not 1 <= int(post_n) <= 4096:
+            raise FrcnnError("%s: post_n must be in [1, 4096] (got %r)" % (who, post_n))
+
+    def _init_canvas_rcnn(self, params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input):
+        """After the trunk: the canvas input, the frozen RPN and the head, the batched proposals, targets, kept lists and
+        masks; then the first repack."""
+        N, max_gt, nc = self.N, self.max_gt, self.num_classes
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self.sample, self.dropout = sample, dropout
@@ -999,29 +1072,30 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         return scales
 
     def _check_extras(self, call, n_images, keep_inds, masks):
+        who = type(self).__name__
         if keep_inds is not None:
             keep_inds = [torch.as_tensor(k).reshape(-1) for k in keep_inds]
             if self.sample != "list":
-                raise FrcnnError("CanvasRcnnTrainer.%s: kept lists need sample='list' (the trainer has %r)" % (call, self.sample))
+                raise FrcnnError("%s.%s: kept lists need sample='list' (the trainer has %r)" % (who, call, self.sample))
             if len(keep_inds) != n_images:
-                raise FrcnnError("CanvasRcnnTrainer.%s: %d images and %d kept lists" % (call, n_images, len(keep_inds)))
+                raise FrcnnError("%s.%s: %d images and %d kept lists" % (who, call, n_images, len(keep_inds)))
             for n, k in enumerate(keep_inds):
                 if k.numel() > train_ops.ROIS_PER_IMAGE:
-                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d keeps %d rows, at most %d"
-                                     % (call, n, k.numel(), train_ops.ROIS_PER_IMAGE))
+                    raise FrcnnError("%s.%s: image %d keeps %d rows, at most %d"
+                                     % (who, call, n, k.numel(), train_ops.ROIS_PER_IMAGE))
                 if torch.unique(k).numel() != k.numel():
-                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d's kept list repeats a row" % (call, n))
+                    raise FrcnnError("%s.%s: image %d's kept list repeats a row" % (who, call, n))
             keep_inds = [k.to(device=self.device, dtype=torch.int32) for k in keep_inds]
         if masks is not None:
             masks = list(masks)
             if self.dropout != "explicit":
-                raise FrcnnError("CanvasRcnnTrainer.%s: masks need dropout='explicit' (the trainer has %r)" % (call, self.dropout))
+                raise FrcnnError("%s.%s: masks need dropout='explicit' (the trainer has %r)" % (who, call, self.dropout))
             if len(masks) != n_images:
-                raise FrcnnError("CanvasRcnnTrainer.%s: %d images and %d mask pairs" % (call, n_images, len(masks)))
+                raise FrcnnError("%s.%s: %d images and %d mask pairs" % (who, call, n_images, len(masks)))
             want = (self.post_n, 4096)
             for n, pair in enumerate(masks):
                 if len(pair) != 2 or any(tuple(m.shape) not in (want, (want[0] * want[1],)) or m.dtype != torch.uint8 for m in pair):
-                    raise FrcnnError("CanvasRcnnTrainer.%s: image %d needs two uint8 %s masks" % (call, n, want))
+                    raise FrcnnError("%s.%s: image %d needs two uint8 %s masks" % (who, call, n, want))
         return keep_inds, masks
 
     def _stage_extras(self, keep_inds, masks):
@@ -1037,7 +1111,7 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
     def forward(self):
         """Forward over the staged canvas, the proposal targets and the per-slot losses (float32 [N, 4] device buffer:
         loss_cls, loss_bbox, cls_accuracy, loss_rcnn; zeros for a slot that kept nothing)."""
-        N, ext, k, R_cap = self.N, self.extents, self.halvings, self.post_n
+        N, (ext, k), R_cap = self.N, self._level(self.halvings), self.post_n
         feat = self._forward_trunk()
         self._rpn_forward(feat, self.rpn3, self.rpn_heads, self.rpn_mid, self.rpn_ld, self.rpn_out)
         ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, self.rpn_ld), None, self.anchors, self.A, self.fh, self.fw,
@@ -1059,8 +1133,9 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         return losses
 
     def _roi_pool_backward(self, g):
-        train_ops.roi_pool_backward_batch(self.feat, self.prop.rois, self.head_ext[:, 1], g, self.extents, self.halvings, 7, 7,
-                                          1.0 / self.feat_stride, out=self.dfeat, ws=self.roi_ws)
+        ext, k = self._level(self.halvings)
+        train_ops.roi_pool_backward_batch(self.feat, self.prop.rois, self.head_ext[:, 1], g, ext, k, 7, 7, 1.0 / self.feat_stride,
+                                          out=self.dfeat, ws=self.roi_ws)
 
     def step(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
         """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot

@@ -8,7 +8,7 @@ Replaces models/bbox.pyx:16-56, models/anchor_target_layer.py:66-198 and the two
 models/region_proposal_network.py:160-204 (all under /root/reference); the second half wraps the conv-backward entry
 points (frcnn_gemm_nt_splitk, frcnn_grad_prepare, frcnn_wgrad_reduce, frcnn_bias_grad, frcnn_sgd_momentum,
 frcnn_pack_conv_weights_dgrad) used by train_engine.py, and those the ResNet trunk adds (frcnn_maxpool3x3s2_backward,
-frcnn_grad_prepare_stride2, frcnn_fold_batchnorm, frcnn_wgrad_reduce_scaled) used by resnet_train.py.
+frcnn_grad_prepare_stride2 and their _batch forms, frcnn_fold_batchnorm, frcnn_wgrad_reduce_scaled) used by resnet_train.py.
 """
 import ctypes
 
@@ -297,6 +297,44 @@ def grad_prepare_stride2(H, W, C, g, y=None, out=None, tbuf=None):
         _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
         _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None,
         tbuf.planes if tbuf is not None else 1, _stream()), "frcnn_grad_prepare_stride2")
+
+
+def _check_batch_tbuf(what, tbuf, N, planes=None):
+    if tbuf is not None and tbuf.N != N:
+        raise FrcnnError("%s: the transposed buffer holds %d images, not %d" % (what, tbuf.N, N))
+    if tbuf is not None and planes is not None and tbuf.planes != planes:
+        raise FrcnnError("%s: the transposed buffer must have %d plane" % (what, planes))
+
+
+def maxpool3x3s2_backward_batch(N, g, y, p, out=None, tbuf=None):
+    """frcnn_maxpool3x3s2_backward_batch: maxpool3x3s2_backward over N images; g, p Acts [N, h, w, C], y Act [N, H, W, C],
+    out Act [N, H, W, C] (optional), tbuf a TBuf of N blocks with planes = 1 (optional)."""
+    _, H, W, C = y.hi.shape
+    ph, pw = (H - 2) // 2 + 1, (W - 2) // 2 + 1
+    for name, a in (("y", y), ("g", g), ("p", p)):
+        want = (N, H, W, C) if name == "y" else (N, ph, pw, C)
+        if tuple(a.hi.shape) != want:
+            raise FrcnnError("maxpool3x3s2_backward_batch: %s must be %s, got %s" % (name, list(want), tuple(a.hi.shape)))
+    _check_batch_tbuf("maxpool3x3s2_backward_batch", tbuf, N, planes=1)
+    check(_lib.load().frcnn_maxpool3x3s2_backward_batch(
+        _p(g.hi), _p(g.lo), _p(y.hi), _p(y.lo), _p(p.hi), _p(p.lo), int(N), int(H), int(W), int(C),
+        _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
+        _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None, _stream()),
+        "frcnn_maxpool3x3s2_backward_batch")
+
+
+def grad_prepare_stride2_batch(N, H, W, C, g, y=None, out=None, tbuf=None):
+    """frcnn_grad_prepare_stride2_batch: grad_prepare_stride2 over N images; g Act [N, ceil(H/2), ceil(W/2), C], y / out Acts
+    [N, H, W, C] (optional), tbuf a TBuf of N blocks (optional)."""
+    want = (N, (H + 1) // 2, (W + 1) // 2, C)
+    if tuple(g.hi.shape) != want:
+        raise FrcnnError("grad_prepare_stride2_batch: g must be %s, got %s" % (list(want), tuple(g.hi.shape)))
+    _check_batch_tbuf("grad_prepare_stride2_batch", tbuf, N)
+    check(_lib.load().frcnn_grad_prepare_stride2_batch(
+        _p(g.hi), _p(g.lo), _p(y.hi) if y is not None else None, _p(y.lo) if y is not None else None, int(N), int(H), int(W),
+        int(C), _p(out.hi) if out is not None else None, _p(out.lo) if out is not None else None,
+        _p(tbuf.hi) if tbuf is not None else None, _p(tbuf.lo) if tbuf is not None else None,
+        tbuf.planes if tbuf is not None else 1, _stream()), "frcnn_grad_prepare_stride2_batch")
 
 
 def fold_batchnorm(w, s, wf, b=None, beta=None, mean=None, bf=None):

@@ -849,11 +849,30 @@ int frcnn_grad_prepare_batch(const void* g_hi, const void* g_lo, const float* g_
  *       (0, +inf]), +0 elsewhere, and re-split into hi/lo.  Transposed output: planes = 1.
  *   frcnn_grad_prepare_stride2   the backward of frcnn_subsample2x: the source g [ceil(H/2)][ceil(W/2)][C] at pixels (2i, 2j)
  *       of the H x W map and 0 everywhere else, then the optional y > 0 mask as in frcnn_grad_prepare (kept pairs keep their
- *       words); transposed output with planes = 1 or 3. */
+ *       words); transposed output with planes = 1 or 3.
+ * Their _batch forms run N images in one launch (the one-image entries are these with N = 1): every NHWC plane is [N][...]
+ * of the one-image shape (g and p of frcnn_maxpool3x3s2_backward_batch [N][pool3s2_out(H)][pool3s2_out(W)][C], g of
+ * frcnn_grad_prepare_stride2_batch [N][ceil(H/2)][ceil(W/2)][C]), and the transposed planes are [planes][C][N*Kp] with image
+ * n's padded block in columns [n*Kp, (n+1)*Kp), as frcnn_grad_prepare_batch writes them.  Image n's results equal the
+ * one-image entry on it, bit for bit.  N < 1, N * ceil(C/64) > 65535 and the one-image entry's errors -> FRCNN_ERR_ARG.
+ * On a canvas no extents are needed, for the reason frcnn_grad_prepare_batch gives, and:
+ *   - pool backward: y (conv1's output) is 0 outside each image, and so are p and g, which frcnn_maxpool3x3s2_ceil_batch_ext
+ *     and the _ext data-gradient convolutions write as 0 outside the image's pooled extent.  A window that runs past the
+ *     image's border, which the one-image entry on the cropped image clips, only adds elements of value 0.  Where p > 0
+ *     they never match; where p == 0 the element chosen may differ, but the pixel it leaves or takes has y == 0 in both
+ *     cases, so the y > 0 mask zeroes it.  A window that exists on the canvas and not on the cropped image has g == 0, and
+ *     the fp32 sums start from +0, so one more +0 term changes no sum (a sum from +0 is never -0).
+ *   - stride-2 scatter: inside the image, pixel (2i, 2j) reads g[i][j] inside the subsampled extent, as on the cropped
+ *     image; outside it, y == 0 (and g == 0) give 0. */
 int frcnn_maxpool3x3s2_backward(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, const void* p_hi,
                                 const void* p_lo, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo, void* stream);
 int frcnn_grad_prepare_stride2(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, int H, int W, int C,
                                void* o_hi, void* o_lo, void* t_hi, void* t_lo, int planes, void* stream);
+int frcnn_maxpool3x3s2_backward_batch(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, const void* p_hi,
+                                      const void* p_lo, int N, int H, int W, int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo,
+                                      void* stream);
+int frcnn_grad_prepare_stride2_batch(const void* g_hi, const void* g_lo, const void* y_hi, const void* y_lo, int N, int H, int W,
+                                     int C, void* o_hi, void* o_lo, void* t_hi, void* t_lo, int planes, void* stream);
 
 /* ---- frozen BatchNorm in training (resnet_train.cu).  A convolution and its frozen BN are the folded convolution
  * Wf = W*s, bf = beta + (b - mean)*s, s = gamma/sqrt(var + eps) (float64, per output channel).
