@@ -24,15 +24,15 @@ A convolution and its frozen BN are then the folded convolution Wf = W*s, bf = b
     re-layouts       the 3x3/2 cover_all max-pool backward fused with conv1's ReLU mask (frcnn_maxpool3x3s2_backward), and the
                      backward of the stride-2 subsample fused with the ReLU mask of the block output it reads
                      (frcnn_grad_prepare_stride2)
-Everything else -- the flat buffers, the RPN heads' backward, the loss, the optimizer and the gradient exchange (one bucket,
-after backward) -- is RpnTrainer's.
+Everything else -- the flat buffers, the RPN step, the loss, the optimizer and the gradient exchange (one bucket, after
+backward) -- is shared with the VGG16 trainers (train_engine's _ConvTrainer and _RpnStep).
 
 ResNetRcnnTrainer -- RcnnTrainer's step on the same trunk: trunk -> frozen test-mode RPN (2048 -> 512 3x3, twin heads) ->
 ProposalLayer -> ProposalTargetLayer -> RoI pool 7x7 at 1/32 over 2048 channels -> fc6 (K = 2048*49) / fc7 with dropout ->
 cls_score | bbox_pred -> losses -> backward through the head, the RoI pooling and every bottleneck -> WeightDecay +
-MomentumSGD.  The head, its losses and backward are RcnnTrainer's with feat_ch = 2048; the trunk part (_ResNetTrunk) is
-ResNetRpnTrainer's, launch for launch.  Trainable: every trunk convolution's W, trunk/conv1/b, fc6, fc7, cls_score and
-bbox_pred; the RPN is packed once and gets no gradient, the BN entries stay constant.
+MomentumSGD.  The head, its losses and backward are RcnnTrainer's step (_RcnnStep) with feat_ch = 2048; the trunk
+(_ResNetTrunk) is ResNetRpnTrainer's, launch for launch.  Trainable: every trunk convolution's W, trunk/conv1/b, fc6, fc7,
+cls_score and bbox_pred; the RPN is packed once and gets no gradient, the BN entries stay constant.
 """
 import numpy as np
 import torch
@@ -40,10 +40,10 @@ import torch
 from . import ops, train_ops
 from ._lib import FrcnnError
 from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
-from .train_engine import (CanvasRcnnTrainer, CanvasRpnTrainer, RcnnTrainer, RpnTrainer, _fc6_to_hwc, _rcnn_params,
-                           _rpn_params)
+from .train_engine import _CanvasRcnnStep, _CanvasRpnStep, _RcnnStep, _RpnStep
 
 SUBSAMPLE_MODES = ("device", "numpy", "none")
+BN_FIELDS = ("gamma", "beta", "avg_mean", "avg_var")
 
 
 def bn_scale(params, bn):
@@ -64,51 +64,40 @@ def trunk_convs(n_layers):
 
 
 class _ResNetTrunk(object):
-    """The ResNet trunk with frozen BatchNorm, shared by ResNetRpnTrainer and ResNetRcnnTrainer (ahead of RpnTrainer /
-    RcnnTrainer in their MRO): the layer table and BN constants, the activations, the forward launches, the fold + repack,
-    and the bottleneck backward (_backward_trunk, from the gradient of the feature map).  Every launch goes through the
-    trainer's launch layer (_conv, _res_conv, _pool3, _subsample, _prep, _pool3_backward, _prep_stride2, _pack_input), so
-    the same code runs one image and, with _CanvasSteps' launches, a canvas.  A trunk level is an index into
-    frcnn_resnet_level_extents' five: 0 conv1, 1 pool1 / res2, 2 res3, 3 res4, 4 res5."""
+    """The ResNet trunk with frozen BatchNorm, the trunk of the four ResNet trainers: the layer table and BN constants, the
+    activations, the forward launches, the fold + repack, and the bottleneck backward (_backward_trunk, from the gradient
+    of the feature map).  Every launch goes through the trainer's launch layer (_conv, _res_conv, _pool3, _subsample,
+    _prep, _pool3_backward, _prep_stride2, _pack_input), so the same code runs one image and, with _CanvasSteps' launches,
+    a canvas.  A trunk level is an index into frcnn_resnet_level_extents' five: 0 conv1, 1 pool1 / res2, 2 res3, 3 res4,
+    4 res5.  The trainer sets n_layers before it is built."""
     feat_ch = 2048
     halvings = 4                        # the feature map's level (res5)
     first_layer = (7, 2, 3, CONV1_KPAD)
+    early_exchange = None               # no early bucket: a multi-rank exchange is one bucket after backward
+    feat_grad_tag = 3                   # the _gact tag of res5's input gradients, which the RPN conv's data gradient shares
 
-    def _init_trunk(self, params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                    process_group, extra_layers, extra_params, need, load_transform=None, lead=()):
-        """Checks the options and parameters (FrcnnError before anything is allocated), then lays out the flat buffers over
-        the trunk convolutions + extra_layers and extra_params, the frozen-BN constants and the trunk activations.
-        need: {name: shape} of the non-trunk parameters the step reads; lead: the leading [N] of a canvas trainer's
-        activations."""
-        who = type(self).__name__
+    def _trunk_table(self, H, W, feat_stride):
+        """Checks the trunk's options (FrcnnError); returns the trunk convolutions in flat-buffer order and the frozen-BN
+        constants [(name, shape)] they read."""
+        who, n_layers = type(self).__name__, self.n_layers
         if n_layers not in RESNET_BLOCKS:
             raise FrcnnError("%s: n_layers must be one of %s (got %r)" % (who, sorted(RESNET_BLOCKS), n_layers))
         if feat_stride != 32:
             raise FrcnnError("%s: the ResNet trunk's feature stride is 32 (got feat_stride=%r)" % (who, feat_stride))
-        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1           # conv1 7x7/2 pad 3
-        if min(Ho, Wo) < 3:
+        if min((H - 1) // 2 + 1, (W - 1) // 2 + 1) < 3:          # conv1 7x7/2 pad 3
             raise FrcnnError("%s: the image must be at least 5 x 5 (got %d x %d)" % (who, H, W))
-        self.n_layers = n_layers
         convs = trunk_convs(n_layers)
-        want = {n + "/W": (co, ci, k, k) for n, _, ci, co, k in convs}
-        want["trunk/conv1/b"] = (64,)
-        for _, bn, _, co, _ in convs:
-            for f in ("gamma", "beta", "avg_mean", "avg_var"):
-                want["%s/%s" % (bn, f)] = (co,)
-        want.update(need)
-        for k, sh in want.items():
-            if k not in params or tuple(np.shape(params[k])) != sh:
-                raise FrcnnError("%s: parameter %s must have shape %s (got %s)"
-                                 % (who, k, sh, None if k not in params else tuple(np.shape(params[k]))))
         layers = [dict(name=n, bn=bn, cin=ci, cout=co, k=k, bias=n == "trunk/conv1") for n, bn, ci, co, k in convs]
-        self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          layers + list(extra_layers), extra_params, load_transform, lead)
+        return layers, [("%s/%s" % (bn, f), (co,)) for _, bn, _, co, _ in convs for f in BN_FIELDS]
+
+    def _init_trunk(self, params, H, W, lead):
+        """The frozen-BN constants and the trunk activations; on a canvas (lead (N,)) also the per-level extents."""
         dev = self.device
         # ---- frozen BN: s (float64) per conv, the constant folded bias of every conv but conv1, the folded-weight buffers
         T = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)     # noqa: E731
-        self.conv = {}
-        for L in layers:
-            n, bn = L["name"], L["bn"]
+        self.conv = {L["name"]: L for L in self.layers if "bn" in L}
+        for n, L in self.conv.items():
+            bn = L["bn"]
             L["s"] = T(bn_scale(params, bn), torch.float64)
             L["wf"] = torch.empty((L["cout"], L["cin"], L["k"], L["k"]), dtype=torch.float32, device=dev)
             if L["bias"]:
@@ -117,11 +106,11 @@ class _ResNetTrunk(object):
             else:
                 L["bf"] = T(fold_batchnorm(params[n + "/W"], params[bn + "/gamma"], params[bn + "/beta"], params[bn + "/avg_mean"],
                                            params[bn + "/avg_var"])[1])
-            self.conv[n] = L
-        self.bn_params = {k: np.asarray(params[k]).copy() for k in want if "/bn" in k}
+        self.bn_params = {k: np.asarray(params[k]).copy() for k in ("%s/%s" % (L["bn"], f) for L in self.conv.values()
+                                                                    for f in BN_FIELDS)}
         # ---- activations (ResNetForwardPlan._alloc_trunk's, every one kept for backward)
         act = self._act
-        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
+        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
         self.x_col = act(Ho, Wo, CONV1_KPAD)
         self.c1 = act(Ho, Wo, 64)
         h, w = (Ho - 2) // 2 + 1, (Wo - 2) // 2 + 1
@@ -129,7 +118,7 @@ class _ResNetTrunk(object):
         self.c1_hw = (Ho, Wo)
         self.blocks = []
         x, level = self.p1, 1
-        for stage, blk, cin, mid, cout, stride, proj in block_list(n_layers):
+        for stage, blk, cin, mid, cout, stride, proj in block_list(self.n_layers):
             B = dict(name="trunk/%s/%s" % (stage, blk), x=x, stride=stride, proj=proj, cin=cin, mid=mid, cout=cout)
             if stride == 2:
                 h, w, level = (h + 1) // 2, (w + 1) // 2, level + 1
@@ -143,6 +132,8 @@ class _ResNetTrunk(object):
             x = B["out"]
         self.fh, self.fw = h, w
         self.db_raw = torch.empty((64,), dtype=torch.float32, device=dev)
+        if lead:
+            self.level_ext = torch.zeros((5, lead[0], 2), dtype=torch.int32, device=dev)
 
     def _check_input(self, x_chw, gt_boxes):
         who = type(self).__name__
@@ -159,16 +150,13 @@ class _ResNetTrunk(object):
     def _pack_image(self, x, out):
         ops.pack_image_im2col_general(x, *self.first_layer, out=out)
 
-    def _repack_convs(self):
-        """Folds and repacks every trunk convolution, then repacks the step's other convolutions (the RPN 3x3, if trained)."""
+    def _repack_trunk(self):
+        """Folds and repacks every trunk convolution."""
         for n, L in self.conv.items():
             first = n == "trunk/conv1"
             train_ops.fold_batchnorm(self.weights(n + "/W"), L["s"], L["wf"], b=self.weights(n + "/b") if first else None,
                                      beta=L.get("beta"), mean=L.get("mean"), bf=L["bf"] if first else None)
             self._repack(n, L["wf"], L["bf"], L["cout"], first=first, cin_pad=L["cin"])
-        for L in self.layers[len(self.conv):]:
-            n = L["name"]
-            self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), L["cout"], cin_pad=L["cin"])
 
     def folded_params(self):
         """{conv name: (Wf, bf)} float32 numpy: the folded weights the device packed at the last repack."""
@@ -222,7 +210,11 @@ class _ResNetTrunk(object):
 
     def _backward_trunk(self, g, debug=None):
         """Backward through the bottleneck blocks (last first), pool1 and conv1 from g, the gradient of the feature map
-        (ops.Act [fh, fw, 2048]).  debug: receives the per-convolution entries described in ResNetRpnTrainer.backward."""
+        (ops.Act [fh, fw, 2048]).  debug: receives, per conv name, the incoming gradient ("g_in": w.r.t. the conv's
+        post-ReLU output, or w.r.t. the block output for conv3 / conv4, at the subsampled resolution when the next block
+        reads it through the stride-2 subsample), the masked / routed gradient w.r.t. the (folded) conv output ("dy") and
+        the data gradient the conv passes on ("g_out"; for a block's conv1 the summed gradient of the block input, residual
+        included; none for trunk/conv1)."""
         dbg = (lambda a: self._chw(a).clone()) if debug is not None else None        # noqa: E731
         # ---- the bottleneck blocks, last first; `half`: g is w.r.t. the stride-2 subsample of this block's output
         half = False
@@ -234,13 +226,8 @@ class _ResNetTrunk(object):
         dz = self._gact(Ho, Wo, 64)
         dzT = self._tbuf(1, 64, Ho, Wo)
         self._pool3_backward(g, self.c1, self.p1, dz, dzT)
-        xT = self._tbuf(1, CONV1_KPAD, Ho, Wo)
-        self._prep(Ho, Wo, CONV1_KPAD, g=self.x_col, tbuf=xT)
         L = self.conv["trunk/conv1"]
-        dwc = torch.empty((64, CONV1_KPAD), dtype=torch.float32, device=self.device)
-        self._wgrad(dzT, xT, 64, CONV1_KPAD, 1, dwc, scale=L["s"])
-        # im2col column k = tap*3 + c  ->  OIHW [co][c][tap]
-        self.grads("trunk/conv1/W").copy_(dwc[:, :147].reshape(64, 49, 3).permute(0, 2, 1).reshape(64, 3, 7, 7))
+        self._first_layer_wgrad(dzT, Ho, Wo, 64, self.grads("trunk/conv1/W"), scale=L["s"])
         train_ops.bias_grad(dzT, 64, self.db_raw)
         train_ops.wgrad_reduce_scaled(self.db_raw.view(1, 1, 64, 1), 64, 1, L["s"], self.grads("trunk/conv1/b"))
         if debug is not None:
@@ -300,50 +287,7 @@ class _ResNetTrunk(object):
         return gx
 
 
-def _rpn_need(A):
-    """The non-trunk parameters of the RPN step: the RPN 3x3 conv (2048 -> 512) and its twin heads."""
-    need = {"RPN/rpn_conv_3x3/W": (512, 2048, 3, 3), "RPN/rpn_conv_3x3/b": (512,)}
-    need.update(_rpn_params(A))
-    return need
-
-
-def _rcnn_need(A, head):
-    """The parameters the RCNN step reads besides the trunk: the frozen RPN and the head."""
-    need = _rpn_need(A)
-    need.update(head)
-    return need
-
-
-class _ResNetRpnStep(_ResNetTrunk):
-    """The RPN step's backward on the ResNet trunk, shared by ResNetRpnTrainer and CanvasResNetRpnTrainer."""
-
-    def backward(self, debug=None):
-        """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter (on a canvas: the sum over the slots).
-        debug: a dict that receives, per conv name, float32 (C,H,W) copies ([N,C,H,W] on a canvas) of the incoming gradient
-        ("g_in": w.r.t. the conv's post-ReLU output, or w.r.t. the block output for conv3 / conv4, at the subsampled
-        resolution when the next block reads it through the stride-2 subsample), the masked / routed gradient w.r.t. the
-        (folded) conv output ("dy") and the data gradient the conv passes on ("g_out"; for a block's conv1 the summed
-        gradient of the block input, residual included)."""
-        dbg = (lambda a: self._chw(a).clone()) if debug is not None else None        # noqa: E731
-        g = self._backward_heads(debug)
-        # ---- RPN 3x3 conv (2048 -> 512, its own bias, no BN)
-        R = self.rpn_layer
-        fh, fw = self.fh, self.fw
-        dy = self._gact(fh, fw, 512)
-        dyT = self._tbuf(1, 512, fh, fw)
-        self._prep(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
-        xT = self._tbuf(3, 2048, fh, fw)
-        self._prep(fh, fw, 2048, g=self.feat, tbuf=xT)
-        self._wgrad(dyT, xT, 512, 2048, 9, self.grads(R["name"] + "/W"))
-        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
-        g_in = g
-        g = self._dgrad(R["name"], dy, 3, 2048, 3, self.halvings)
-        if debug is not None:
-            debug[R["name"]] = dict(g_in=dbg(g_in), dy=dbg(dy), g_out=dbg(g))
-        self._backward_trunk(g, debug)
-
-
-class ResNetRpnTrainer(_ResNetRpnStep, RpnTrainer):
+class ResNetRpnTrainer(_ResNetTrunk, _RpnStep):
     """Weights, optimizer state and buffers of the RPN-mode training step with the ResNet trunk for one image shape.  The
     surface is RpnTrainer's: forward / backward(debug) / update / step / weights / grads / export_params, subsample modes
     "device", "numpy" and "none", disable_pos.  `params` follows oracle.make_resnet_params / models.resnet.ResNet naming;
@@ -353,21 +297,17 @@ class ResNetRpnTrainer(_ResNetRpnStep, RpnTrainer):
                  feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
         if subsample not in SUBSAMPLE_MODES:
             raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
-        A = len(anchors)
-        self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), _rpn_need(A))
-        self._init_rpn_head(loss_lambda, delta, subsample, seed)
-        self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
-        self.repack()
+        self.n_layers = n_layers
+        self._init_rpn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                       loss_lambda, delta, subsample, seed)
 
-    # ---------------------------------------------------------------- forward
     def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
         self._check_input(x_chw, gt_boxes)
         return super(ResNetRpnTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos)
 
 
-class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
+class ResNetRcnnTrainer(_ResNetTrunk, _RcnnStep):
     """Weights, optimizer state and buffers of the RCNN-mode training step (train_rcnn.py) with the ResNet trunk for one
     image shape.  The surface is RcnnTrainer's: forward(x, gt, im_info, keep_inds, masks) / backward(debug) / update / step
     / weights / grads / export_params, sample="numpy" (a seeded run draws the reference's kept set), keep_inds= and masks=
@@ -379,13 +319,9 @@ class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
     def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
                  sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
-        nc = self.num_classes = num_classes
-        head = _rcnn_params(nc, self.feat_ch)
-        self._init_trunk(params, H, W, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [], head, _rcnn_need(len(anchors), head), load_transform=_fc6_to_hwc)
-        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
-        self._init_one_image_rcnn(sample, seed, dropout)
-        self.repack()
+        self.n_layers = n_layers
+        self._init_rcnn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout)
 
     def forward(self, x_chw, gt_boxes, im_info=None, keep_inds=None, masks=None):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RcnnTrainer."""
@@ -393,7 +329,7 @@ class ResNetRcnnTrainer(_ResNetTrunk, RcnnTrainer):
         return super(ResNetRcnnTrainer, self).forward(x_chw, gt_boxes, im_info, keep_inds, masks)
 
 
-class CanvasResNetRpnTrainer(_ResNetRpnStep, CanvasRpnTrainer):
+class CanvasResNetRpnTrainer(_ResNetTrunk, _CanvasRpnStep):
     """CanvasRpnTrainer's step with the ResNet trunk: N images of different sizes per update (put / put_raw / forward /
     backward(debug) / update / run / step / step_raw, per-slot losses [N, 4]), one set of weights with ResNetRpnTrainer's
     parameters, frozen BatchNorm and folded_params().
@@ -410,22 +346,17 @@ class CanvasResNetRpnTrainer(_ResNetRpnStep, CanvasRpnTrainer):
     labels before subsampling.  raw_input=True: put_raw takes raw photos and the VOC transform runs on the device,
     straight into conv1's 7x7/2 im2col planes.  The step is captured after the first call in a single process and runs
     eagerly with a process group of more than one rank; the gradient exchange is then one bucket after backward (the
-    early deep-layer bucket is keyed to the VGG16 trunk's conv4_1)."""
+    ResNet trunk names no early-exchange layer)."""
 
     def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
                  weight_decay=0.0005, feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256,
                  device="cuda", process_group=None, raw_input=False):
-        self._rpn_options(N, subsample, max_gt)
-        self.N, self.max_gt = int(N), int(max_gt)
-        A = len(anchors)
-        self._init_trunk(params, Hc, Wc, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [dict(name="RPN/rpn_conv_3x3", cin=2048, cout=512, k=3)], _rpn_params(A), _rpn_need(A),
-                         lead=(self.N,))
-        self.level_ext = torch.zeros((5, self.N, 2), dtype=torch.int32, device=self.device)
-        self._init_canvas_rpn(Hc, Wc, loss_lambda, delta, subsample, seed, raw_input)
+        self.n_layers = n_layers
+        self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                              delta, subsample, seed, max_gt, device, process_group, raw_input)
 
 
-class CanvasResNetRcnnTrainer(_ResNetTrunk, CanvasRcnnTrainer):
+class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
     """CanvasRcnnTrainer's step with the ResNet trunk: N images of different sizes per update, with ResNetRcnnTrainer's
     parameters (the head on res5's 2048-channel RoIs, fc6 with K = 2048*49; the RPN frozen and packed once; frozen
     BatchNorm) and CanvasRcnnTrainer's surface, sample ("device" | "list") and dropout ("device" | "explicit" | None)
@@ -438,11 +369,7 @@ class CanvasResNetRcnnTrainer(_ResNetTrunk, CanvasRcnnTrainer):
                  weight_decay=0.0005, feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7,
                  min_size=16, sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None,
                  raw_input=False):
-        self._rcnn_options(N, sample, dropout, max_gt, post_n)
-        self.N, self.max_gt = int(N), int(max_gt)
-        nc = self.num_classes = num_classes
-        head = _rcnn_params(nc, self.feat_ch)
-        self._init_trunk(params, Hc, Wc, anchors, n_layers, precision, lr, momentum, weight_decay, feat_stride, device,
-                         process_group, [], head, _rcnn_need(len(anchors), head), load_transform=_fc6_to_hwc, lead=(self.N,))
-        self.level_ext = torch.zeros((5, self.N, 2), dtype=torch.int32, device=self.device)
-        self._init_canvas_rcnn(params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input)
+        self.n_layers = n_layers
+        self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
+                               delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
+                               process_group, raw_input)

@@ -7,6 +7,10 @@ dropout -> head losses -> backward through the head, the RoI pooling and the tru
 CanvasRpnTrainer -- RpnTrainer's step on N images of different sizes per update (an N-slot canvas), one captured graph.
 CanvasRcnnTrainer -- RcnnTrainer's step on such a canvas, with device-side RoI sampling and dropout masks.
 
+Every trainer, here and in resnet_train, is one trunk (_Vgg16Trunk, _ResNetTrunk: layers, forward, backward from the
+feature map's gradient, repacking) and one step (_RpnStep, _RcnnStep, or on a canvas _CanvasRpnStep, _CanvasRcnnStep), both
+launching through _ConvTrainer's launch layer over one image, which _CanvasSteps overrides for a canvas.
+
 Mirrors /root/reference train_rpn.py:144-179 with `model.rpn_train = True`: FasterRCNN.__call__ takes the RPN training
 branch (models/faster_rcnn.py:114-116 -> models/region_proposal_network.py:117-156), the optimizer is
 MomentumSGD(lr=0.001) (momentum 0.9 default) + WeightDecay(0.0005) (train_rpn.py:165-167).  Only parameters that receive a
@@ -33,39 +37,51 @@ TRUNK = [s[:3] for s in _STEPS]                                  # (name, cin, c
 POOL_AFTER = {s.name for s in _STEPS if s.pool_after}
 
 
+def _entries(layers, params):
+    """[(name, shape)] in flat-buffer order: W, then b unless the layer has bias=False, of every layer in `layers`, then
+    `params` in the given order."""
+    out = []
+    for L in layers:
+        out.append((L["name"] + "/W", (L["cout"], L["cin"], L["k"], L["k"])))
+        if L.get("bias", True):
+            out.append((L["name"] + "/b", (L["cout"],)))
+    return out + [(n, tuple(sh)) for n, sh in params]
+
+
+def _fc6_to_hwc(name, a):                           # fc6 columns (c, h, w) -> (h, w, c), the order the RoI pooling emits
+    return a.reshape(4096, -1, 49).transpose(0, 2, 1) if name == "fc6/W" else a
+
+
 class _ConvTrainer(object):
-    """Shared by every trainer: flat float32 master / momentum / gradient buffers, the 13 trunk layers with their stored
-    activations, and the launch layer over one image -- _conv, _prep, _pool, _chw, the cached gradient buffers and the
-    in-place repack.  _CanvasSteps overrides the launches for a canvas, so every step is written once."""
-    halvings = None             # the feature map's canvas level (the VGG16 trunk's: set by _init_common)
-    feat_ch = 512               # channels of the feature map the RPN and the RoI pooling read (VGG16's conv5_3)
-    first_layer = (3, 1, 1, 32)     # ksize, stride, pad, K_pad of the first layer's im2col input
+    """Shared by every trainer: the construction with its parameter check, the flat float32 master / momentum / gradient
+    buffers and their views, the launch layer over one image -- _conv, _prep, _pool, _chw, the cached gradient buffers and
+    the in-place repack -- the weight gradients, the RPN forward, the gradient exchange and the optimizer.  _CanvasSteps
+    overrides the launches for a canvas, so every step is written once.  The trunk supplies feat_ch, halvings,
+    first_layer, early_exchange, feat_grad_tag and the _trunk / _pack_image hooks; the step _step_table and repack."""
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                     extra_layers, extra_params, load_transform=None, lead=()):
-        layers = [dict(name="trunk/" + n, cin=ci, cout=co, k=3) for n, ci, co in TRUNK] + list(extra_layers)
+                     lead=()):
+        """Checks the trunk's options and every parameter the trainer reads (FrcnnError before anything is allocated), then
+        lays out the flat buffers over the trunk's convolutions and the step's convolutions and parameters, and the
+        trunk's constants and activations.  lead: the leading [N] of a canvas trainer's activations."""
+        layers, consts = self._trunk_table(H, W, feat_stride)
+        step_layers, step_params, frozen = self._step_table(len(anchors))
+        layers += step_layers
+        entries = _entries(layers, step_params)
+        for name, shape in entries + consts + frozen:
+            got = tuple(np.shape(params[name])) if name in params else None
+            if got != shape:
+                raise FrcnnError("%s: parameter %s must have shape %s (got %s)" % (type(self).__name__, name, shape, got))
         self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          layers, extra_params, load_transform, lead)
-        # ---- geometry + activations (forward keeps every conv output; pooled maps where the graph pools); `lead`: the
-        # leading [N] of a canvas trainer's activations; on a canvas a layer's extents are ceil(extent / 2^halvings)
-        act, dev = self._act, self.device
-        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=dev)
-        self.x_col = act(H, W, 32)
-        h, w, halvings = H, W, 0
-        for L in self.layers[:13]:
-            L["H"], L["W"], L["halvings"] = h, w, halvings
-            L["y"] = act(h, w, L["cout"])
-            short = L["name"].split("/")[1]
-            L["pool"] = short in POOL_AFTER
-            if L["pool"]:
-                h, w, halvings = (h + 1) // 2, (w + 1) // 2, halvings + 1
-                L["p"] = act(h, w, L["cout"])
-        self.fh, self.fw, self.halvings = h, w, halvings
+                          layers, entries, lead)
+        self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=self.device)
+        self._init_trunk(params, H, W, lead)
 
     def _init_params(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                     layers, extra_params, load_transform=None, lead=()):
-        """What every trainer shares: hyper-parameters, the flat float32 master / momentum / gradient buffers over `layers`
-        (W, then b unless the layer has bias=False) and `extra_params`, the activation allocator and the exchange state."""
+                     layers, entries, lead=()):
+        """Hyper-parameters, the flat float32 master / momentum / gradient buffers over `entries` ([(name, shape)], stored
+        in the given order with NO padding: adjacent twin heads stay one matrix; fc6/W in the RoI pooling's (h, w, c)
+        column order), the activation allocator and the exchange state."""
         if precision not in ops.PRECISIONS:
             raise FrcnnError("precision must be one of %s" % (ops.PRECISIONS,))
         self.x3 = precision == "bf16x3"
@@ -77,28 +93,16 @@ class _ConvTrainer(object):
         self.A = int(self.anchors.shape[0])
         # ---- trainable parameters in the reference's naming; one flat fp32 master / momentum / gradient buffer
         self.layers = layers
-        names, shapes = [], []
-        for L in self.layers:
-            names.append(L["name"] + "/W")
-            shapes.append((L["cout"], L["cin"], L["k"], L["k"]))
-            if L.get("bias", True):
-                names.append(L["name"] + "/b")
-                shapes.append((L["cout"],))
-        for n, sh in extra_params:              # stored in the given order with NO padding (adjacent twin heads stay one matrix)
-            names.append(n)
-            shapes.append(tuple(sh))
-        sizes = [int(np.prod(s)) for s in shapes]
+        sizes = [int(np.prod(s)) for _, s in entries]
         offs = [0] + [int(v) for v in np.cumsum(sizes)[:-1]]
         total = int(sum(sizes))
         self.w_flat = torch.zeros((total,), dtype=torch.float32, device=dev)
         self.v_flat = torch.zeros_like(self.w_flat)
         self.g_flat = torch.zeros_like(self.w_flat)
         self.index = {}
-        for n, s, o, sz in zip(names, shapes, offs, sizes):
+        for (n, s), o, sz in zip(entries, offs, sizes):
             self.index[n] = (o, sz, s)
-            src = np.ascontiguousarray(params[n], dtype=np.float32)
-            if load_transform is not None:
-                src = load_transform(n, src)
+            src = _fc6_to_hwc(n, np.ascontiguousarray(params[n], dtype=np.float32))
             self.w_flat[o:o + sz] = torch.from_numpy(np.ascontiguousarray(src).reshape(-1)).to(dev)
         x3 = self.x3
 
@@ -117,8 +121,8 @@ class _ConvTrainer(object):
         # ---- multi-GPU gradient exchange (train_rpn.py:169-174): "fp32" = one exact SUM of the fp32 bucket (the parity
         # mode: bucket == sum of the per-image gradients bit for bit); "bf16" = BASELINE config #5: the bucket is rounded
         # to bf16 for the all-reduce (half the bytes), masters / momentum stay fp32.  The exchange runs on its own stream
-        # in two buckets: the deep layers (conv4_1 ... heads, 90 % of the parameters) are reduced while conv3_3 ... conv1_1
-        # still back-propagate; only the small shallow bucket is exposed.
+        # in two buckets when the trunk names an early_exchange layer: the layers from it on (VGG16: conv4_1 ... heads, 90 %
+        # of the parameters) are reduced while the shallower ones still back-propagate; else in one after backward.
         self.grad_dtype = "fp32"
         self.g_bf16 = None
         self.comm_stream = None
@@ -126,6 +130,17 @@ class _ConvTrainer(object):
         self._bucket_lo = None              # flat offset where the early (deep-layer) bucket starts
         self.n_updates = 0                  # optimizer steps taken (the drop-in model syncs its Link params when this moves)
         self._ev_bwd = self._ev_comm = None
+
+    # ---------------------------------------------------------------- views
+    def view(self, flat, name):
+        o, sz, shape = self.index[name]
+        return flat[o:o + sz].view(shape)
+
+    def weights(self, name):
+        return self.view(self.w_flat, name)
+
+    def grads(self, name):
+        return self.view(self.g_flat, name)
 
     # ---------------------------------------------------------------- launches over one image (_CanvasSteps: a canvas)
     def _conv(self, x, planes, bias, ksize, relu, at, **kw):
@@ -142,9 +157,10 @@ class _ConvTrainer(object):
     def _pool(self, y, out):
         ops.maxpool2x2_ceil(y, out=out)
 
-    def _pack_image(self, x, out):
-        """The first layer's im2col planes of one image."""
-        ops.pack_image_im2col(x, out=out)
+    def _pack_input(self, x_chw):
+        """The trunk's first launch: the image into the first layer's im2col planes x_col."""
+        self.x_in.copy_(x_chw, non_blocking=True)
+        self._pack_image(self.x_in, self.x_col)
 
     # the ResNet trunk's launches (resnet_train._ResNetTrunk); `at` as in _conv
     def _res_conv(self, x, planes, bias, ksize, relu, res, at, out):
@@ -182,10 +198,6 @@ class _ConvTrainer(object):
         return self._tbufs[key]
 
     # ---------------------------------------------------------------- weights: repacked in place from the fp32 masters
-    def _pack_image_layer(self, w, out=None):
-        """The first convolution's planes, in the K order of the trunk's im2col input."""
-        return ops.pack_conv_weights_im2col(w, precision=self.precision, out=out)
-
     def _repack(self, name, w, b, cout_pad, first=False, cin_pad=None):
         """packed[name] = (forward planes, padded bias, data-gradient planes or None for the first layer), overwriting the
         earlier tensors: a captured graph, and whoever else holds them, reads the new weights."""
@@ -197,17 +209,226 @@ class _ConvTrainer(object):
             dg = train_ops.pack_conv_weights_dgrad(w, cout_pad=cout_pad, x3=self.x3, out=old and old[2])
         self.packed[name] = (fwd, ops.pad_bias(b, cout_pad, out=old and old[1]), dg)
 
+    # ---------------------------------------------------------------- forward
+    def _rpn_forward(self, x, conv, heads, mid, ld, out):
+        """An RPN on the feature map x: its 3x3 conv + ReLU into `mid`, its twin 1x1 heads into the fp32 [rows, ld] `out`.
+        conv / heads: (planes, bias, ...) -- the trained layers' `packed` entries or the RCNN step's frozen ones."""
+        self._conv(x, conv[0], conv[1], 3, True, self.halvings, out=mid)
+        self._conv(mid, heads[0], heads[1], 1, False, self.halvings, out_act=False, ld_f32=ld, out_f32=out)
 
-class RpnTrainer(_ConvTrainer):
-    """Weights, optimizer state and buffers of the RPN-mode training step for one image shape."""
+    # ---------------------------------------------------------------- weight gradients
+    def _splits(self, groups, M, N, kb_total):
+        # measured (tests/gpu_wgrad_tune.py): ~2 waves of 148 tiles, 4 when the M tile is half empty (64 output channels)
+        tiles = groups * ((M + 127) // 128) * ((N + 127) // 128)
+        target = (4 if M <= 64 else 2) * 148
+        s = max(1, (target + tiles - 1) // tiles)
+        return int(min(s, max(1, kb_total // 8)))
 
-    def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
-        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], _rpn_params(len(anchors)))
+    def _wgrad(self, dyT, xT, M, N, groups, dw, m_out=None, scale=None):
+        """dw (flat view) = sum_pixels dY (x) X over the padded pixel axis; dyT: TBuf 1 plane [M_parts, Kp]; xT: TBuf.
+        scale: float64 [M] per-output-channel factor (a frozen BatchNorm's s), applied in the fixed-order reduction."""
+        K = dyT.hi.shape[-1]                    # N*Kp: a canvas sums its N images in the one GEMM
+        a_hi, a_lo = dyT.hi[0], (dyT.lo[0] if dyT.lo is not None else None)
+        if groups == 9:
+            b_hi, b_lo = xT.hi, xT.lo
+        else:
+            pl = 1 if xT.planes == 3 else 0
+            b_hi, b_lo = xT.hi[pl], (xT.lo[pl] if xT.lo is not None else None)
+        parts = train_ops.gemm_nt_splitk(a_hi, a_lo, b_hi, b_lo, groups=groups, row_stride=dyT.Wp,
+                                         splits=self._splits(groups, M, N, K // 64))
+        if scale is None:
+            train_ops.wgrad_reduce(parts, m_out or M, N, dw)
+        else:
+            train_ops.wgrad_reduce_scaled(parts, m_out or M, N, scale, dw)
+
+    def _first_layer_wgrad(self, dyT, h, w, co, dw, scale=None):
+        """The first convolution's weight gradient into dw (OIHW [co][3][k][k]) from dyT and its im2col input x_col: the
+        GEMM over the K_pad columns (scaled as _wgrad scales), then im2col column tap*3 + c -> OIHW [co][c][tap]."""
+        k, _, _, K_pad = self.first_layer
+        xT = self._tbuf(1, K_pad, h, w)
+        self._prep(h, w, K_pad, g=self.x_col, tbuf=xT)
+        dwc = torch.empty((co, K_pad), dtype=torch.float32, device=self.device)
+        self._wgrad(dyT, xT, co, K_pad, 1, dwc, scale=scale)
+        dw.copy_(dwc[:, :3 * k * k].reshape(co, k * k, 3).permute(0, 2, 1).reshape(co, 3, k, k))
+
+    # ---------------------------------------------------------------- gradient exchange + optimizer
+    def set_grad_exchange(self, grad_dtype="fp32", overlap=True):
+        """grad_dtype "fp32" (exact) or "bf16" (config #5); overlap: reduce the deep-layer bucket during the rest of backward."""
+        if grad_dtype not in ("fp32", "bf16"):
+            raise FrcnnError("grad_dtype must be fp32 or bf16")
+        self.grad_dtype = grad_dtype
+        if grad_dtype == "bf16" and self.g_bf16 is None:
+            self.g_bf16 = torch.zeros(self.g_flat.shape, dtype=torch.bfloat16, device=self.device)
+        self._overlap = bool(overlap)
+
+    def _multi(self):
+        return shard.dist.is_available() and shard.dist.is_initialized() and shard.dist.get_world_size(self.pg) > 1
+
+    def _exchange(self, lo, hi):
+        """All-reduce(SUM) of g_flat[lo:hi] on the communication stream, after everything queued so far on the compute stream."""
+        if self.comm_stream is None:
+            self.comm_stream = torch.cuda.Stream(device=self.device)
+        ev = torch.cuda.Event()
+        ev.record()
+        self.comm_stream.wait_event(ev)
+        with torch.cuda.stream(self.comm_stream):
+            if self.grad_dtype == "bf16":
+                train_ops.cast_f32_bf16(self.g_flat[lo:hi], self.g_bf16[lo:hi])
+                shard.allreduce_sum_(self.g_bf16[lo:hi], self.pg)
+            else:
+                shard.allreduce_sum_(self.g_flat[lo:hi], self.pg)
+
+    def _early_exchange(self, layer_name):
+        """Called from the trunk's backward right after `layer_name`'s gradients are enqueued: at the trunk's
+        early_exchange layer, starts the exchange of the deep-layer bucket."""
+        if not getattr(self, "_overlap", True) or not self._multi() or layer_name != self.early_exchange:
+            return
+        lo = self.index[layer_name + "/W"][0]
+        if lo % 4 != 0:
+            return
+        self._bucket_lo = lo
+        self._exchange(lo, self.g_flat.numel())
+
+    def update(self):
+        """[all-reduce SUM over ranks, like ParallelUpdater's addgrads] + WeightDecay + MomentumSGD, then repack."""
+        if self._multi():
+            hi = self._bucket_lo if self._bucket_lo is not None else self.g_flat.numel()
+            self._ev_bwd = torch.cuda.Event(enable_timing=True)
+            self._ev_bwd.record()                                  # backward fully enqueued on the compute stream
+            self._exchange(0, hi)
+            self._ev_comm = torch.cuda.Event(enable_timing=True)
+            self._ev_comm.record(self.comm_stream)
+            torch.cuda.current_stream().wait_event(self._ev_comm)
+            self._bucket_lo = None
+        if self.grad_dtype == "bf16" and self._multi():
+            train_ops.sgd_momentum_bf16g(self.w_flat, self.v_flat, self.g_bf16, self.lr, self.momentum, self.weight_decay)
+        else:
+            train_ops.sgd_momentum(self.w_flat, self.v_flat, self.g_flat, self.lr, self.momentum, self.weight_decay)
+        self.repack()
+        self.n_updates += 1
+
+    def last_exposed_exchange_ms(self):
+        """Time between "backward done" on the compute stream and "exchange done" on the communication stream for the last
+        step (what the optimizer had to wait for); call after a synchronize.  0 if the exchange finished first."""
+        if self._ev_bwd is None or self._ev_comm is None:
+            return 0.0
+        return max(0.0, self._ev_bwd.elapsed_time(self._ev_comm))
+
+    def export_params(self):
+        """Trainable parameters as numpy arrays under the reference's names (checkpoint / write-back into the Links)."""
+        return {n: self.weights(n).detach().cpu().numpy().copy() for n in self.index}
+
+
+class _Vgg16Trunk(object):
+    """The VGG16 trunk: 13 3x3 convolutions, the first on the image's 3x3 im2col planes, with every output kept (pools
+    un-fused: backward needs the un-pooled maps); the feature map is conv5_3's output at 1/16."""
+    feat_ch = 512                   # channels of the feature map the RPN and the RoI pooling read (conv5_3)
+    halvings = 4                    # the feature map's canvas level: after four 2x2 pools
+    first_layer = (3, 1, 1, 32)     # ksize, stride, pad, K_pad of the first layer's im2col input
+    early_exchange = "trunk/conv4_1"    # the deep bucket of the gradient exchange: conv4_1 on, 90 % of the parameters
+    feat_grad_tag = 1               # the _gact tag of the trunk's data gradients, which the RPN conv's data gradient shares
+
+    def _trunk_table(self, H, W, feat_stride):
+        """The trunk's convolutions in flat-buffer order and the constants it reads besides them (none)."""
+        return [dict(name="trunk/" + n, cin=ci, cout=co, k=3) for n, ci, co in TRUNK], []
+
+    def _init_trunk(self, params, H, W, lead):
+        """Geometry + activations: every conv output, and the pooled maps where the graph pools; `lead`: the leading [N]
+        of a canvas trainer's activations, whose extents at a layer are ceil(extent / 2^halvings)."""
+        act = self._act
+        self.x_col = act(H, W, 32)
+        h, w, halvings = H, W, 0
+        for L in self.layers[:13]:
+            L["H"], L["W"], L["halvings"] = h, w, halvings
+            L["y"] = act(h, w, L["cout"])
+            short = L["name"].split("/")[1]
+            L["pool"] = short in POOL_AFTER
+            if L["pool"]:
+                h, w, halvings = (h + 1) // 2, (w + 1) // 2, halvings + 1
+                L["p"] = act(h, w, L["cout"])
+        self.fh, self.fw = h, w
+
+    def _pack_image(self, x, out):
+        """The first layer's im2col planes of one image."""
+        ops.pack_image_im2col(x, out=out)
+
+    def _pack_image_layer(self, w, out=None):
+        """The first convolution's planes, in the K order of the trunk's im2col input."""
+        return ops.pack_conv_weights_im2col(w, precision=self.precision, out=out)
+
+    def _repack_trunk(self):
+        for i, L in enumerate(self.layers[:13]):
+            name = L["name"]
+            self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
+
+    def _forward_trunk(self, x_chw=None):
+        """The 13 VGG16 convolutions with every output kept (pools un-fused: backward needs the un-pooled maps)."""
+        self._pack_input(x_chw)
+        x = self.x_col
+        for i, L in enumerate(self.layers[:13]):
+            fwd, b, _ = self.packed[L["name"]]
+            self._conv(x, fwd, b, 1 if i == 0 else 3, True, L["halvings"], out=L["y"])
+            x = L["y"]
+            if L["pool"]:
+                self._pool(L["y"], out=L["p"])
+                x = L["p"]
+        self.feat = x
+        return x
+
+    def _backward_trunk(self, g, debug=None):
+        """Backward through the 13 convolutions, last first, from g: the gradient (ops.Act) w.r.t. the feature map.  Per
+        layer: ReLU / pool backward + re-layout, weight + bias gradient, data gradient for the next one.  On a canvas the
+        weight gradients run over K = N*Kp, the sum over the slots.  debug: per layer name, "g_in", "dy" and (but for
+        conv1_1) "g_out", as the step's backward describes them."""
+        for L in self.layers[12::-1]:
+            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
+            first = L is self.layers[0]
+            dy = self._gact(h, w, co)
+            dyT = self._tbuf(1, co, h, w)
+            self._prep(h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
+            if debug is not None:
+                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
+            if first:
+                self._first_layer_wgrad(dyT, h, w, co, self.grads(L["name"] + "/W"))
+            else:
+                xT = self._tbuf(3, ci, h, w)
+                self._prep(h, w, ci, g=self._input_of(L), tbuf=xT)
+                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
+            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
+            self._early_exchange(L["name"])
+            if not first:
+                g = self._gact(h, w, ci, tag=self.feat_grad_tag)
+                self._conv(dy, self.packed[L["name"]][2], self.zero_bias, 3, False, L["halvings"], out=g)
+                if debug is not None:
+                    debug[L["name"]]["g_out"] = self._chw(g)
+
+    def _input_of(self, L):
+        i = self.layers.index(L)
+        if i == 0:
+            return self.x_col
+        if i == 13:
+            return self.feat
+        prev = self.layers[i - 1]
+        return prev["p"] if prev["pool"] else prev["y"]
+
+
+class _RpnStep(_ConvTrainer):
+    """The RPN step over any trunk: the RPN 3x3 conv and its twin heads, AnchorTargetLayer, rpn_loss and the backward
+    through the heads and the RPN conv into the trunk's."""
+
+    def _init_rpn(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                  loss_lambda, delta, subsample, seed):
+        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
         self.repack()
+
+    def _step_table(self, A):
+        """The step's convolutions and parameters in flat-buffer order, and the parameters it reads but does not train.
+        The twin heads are stored adjacently so that (W_cls | W_bbox) is ONE [6A, 512] matrix: cls W, bbox W, cls b, bbox b."""
+        heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
+        return ([dict(name="RPN/rpn_conv_3x3", cin=self.feat_ch, cout=512, k=3)],
+                [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads], [])
 
     def _init_rpn_head(self, loss_lambda, delta, subsample, seed):
         """The RPN step's loss settings, its 3x3 conv (the last layer) at the feature map and the twin heads' output."""
@@ -219,17 +440,6 @@ class RpnTrainer(_ConvTrainer):
         R["y"] = self._act(self.fh, self.fw, 512)
         self.head_out = torch.empty((self._slots * self.fh * self.fw, self.head_ld), dtype=torch.float32, device=self.device)
 
-    # ---------------------------------------------------------------- views
-    def view(self, flat, name):
-        o, sz, shape = self.index[name]
-        return flat[o:o + sz].view(shape)
-
-    def weights(self, name):
-        return self.view(self.w_flat, name)
-
-    def grads(self, name):
-        return self.view(self.g_flat, name)
-
     def _heads_w(self, flat):
         o, _, _ = self.index["RPN/rpn_cls_score/W"]
         return flat[o:o + self.n_heads * 512].view(self.n_heads, 512)
@@ -238,14 +448,10 @@ class RpnTrainer(_ConvTrainer):
         o, _, _ = self.index["RPN/rpn_cls_score/b"]
         return flat[o:o + self.n_heads]
 
-    # ---------------------------------------------------------------- weight (re)packing from the fp32 masters
-    def _repack_convs(self):
-        for i, L in enumerate(self.layers):
-            name = L["name"]
-            self._repack(name, self.weights(name + "/W"), self.weights(name + "/b"), L["cout"], first=i == 0, cin_pad=L["cin"])
-
     def repack(self):
-        self._repack_convs()
+        self._repack_trunk()
+        R = self.rpn_layer
+        self._repack(R["name"], self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b"), 512, cin_pad=R["cin"])
         self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
 
     # ---------------------------------------------------------------- forward
@@ -295,64 +501,29 @@ class RpnTrainer(_ConvTrainer):
             disable.append(np.random.choice(bg_inds, size=int(len(bg_inds) - num_bg), replace=False))
         return torch.from_numpy(np.concatenate(disable).astype(np.int32)).to(self.device)
 
-    def _pack_input(self, x_chw):
-        """The trunk's first launch: the image into the first layer's im2col planes x_col."""
-        self.x_in.copy_(x_chw, non_blocking=True)
-        self._pack_image(self.x_in, self.x_col)
-
-    def _forward_trunk(self, x_chw=None):
-        """The 13 VGG16 convolutions with every output kept (pools un-fused: backward needs the un-pooled maps)."""
-        self._pack_input(x_chw)
-        x = self.x_col
-        for i, L in enumerate(self.layers[:13]):
-            fwd, b, _ = self.packed[L["name"]]
-            self._conv(x, fwd, b, 1 if i == 0 else 3, True, L["halvings"], out=L["y"])
-            x = L["y"]
-            if L["pool"]:
-                self._pool(L["y"], out=L["p"])
-                x = L["p"]
-        self.feat = x
-        return x
-
-    def _rpn_forward(self, x, conv, heads, mid, ld, out):
-        """An RPN on the feature map x: its 3x3 conv + ReLU into `mid`, its twin 1x1 heads into the fp32 [rows, ld] `out`.
-        conv / heads: (planes, bias, ...) -- the trained layers' `packed` entries or the RCNN step's frozen ones."""
-        self._conv(x, conv[0], conv[1], 3, True, self.halvings, out=mid)
-        self._conv(mid, heads[0], heads[1], 1, False, self.halvings, out_act=False, ld_f32=ld, out_f32=out)
-
     # ---------------------------------------------------------------- backward
-    def _splits(self, groups, M, N, kb_total):
-        # measured (tests/gpu_wgrad_tune.py): ~2 waves of 148 tiles, 4 when the M tile is half empty (64 output channels)
-        tiles = groups * ((M + 127) // 128) * ((N + 127) // 128)
-        target = (4 if M <= 64 else 2) * 148
-        s = max(1, (target + tiles - 1) // tiles)
-        return int(min(s, max(1, kb_total // 8)))
-
-    def _wgrad(self, dyT, xT, M, N, groups, dw, m_out=None, scale=None):
-        """dw (flat view) = sum_pixels dY (x) X over the padded pixel axis; dyT: TBuf 1 plane [M_parts, Kp]; xT: TBuf.
-        scale: float64 [M] per-output-channel factor (a frozen BatchNorm's s), applied in the fixed-order reduction."""
-        K = dyT.hi.shape[-1]                    # N*Kp: a canvas sums its N images in the one GEMM
-        a_hi, a_lo = dyT.hi[0], (dyT.lo[0] if dyT.lo is not None else None)
-        if groups == 9:
-            b_hi, b_lo = xT.hi, xT.lo
-        else:
-            pl = 1 if xT.planes == 3 else 0
-            b_hi, b_lo = xT.hi[pl], (xT.lo[pl] if xT.lo is not None else None)
-        parts = train_ops.gemm_nt_splitk(a_hi, a_lo, b_hi, b_lo, groups=groups, row_stride=dyT.Wp,
-                                         splits=self._splits(groups, M, N, K // 64))
-        if scale is None:
-            train_ops.wgrad_reduce(parts, m_out or M, N, dw)
-        else:
-            train_ops.wgrad_reduce_scaled(parts, m_out or M, N, scale, dw)
-
     def backward(self, debug=None):
         """Fills g_flat with d(rpn_loss)/d(parameter) for every trainable parameter (on a canvas: the sum over the slots).
         debug: a dict that receives, per layer name, float32 (C,H,W) copies ([N,C,H,W] on a canvas) of the incoming
         gradient ("g_in"), the masked / routed gradient ("dy") and the data gradient the layer passes on ("g_out") -- the
-        buffers themselves are reused from layer to layer."""
+        buffers themselves are reused from layer to layer.  The trunk's entries are those of its _backward_trunk."""
         g = self._backward_heads(debug)
-        # ---- RPN 3x3 conv, then the trunk, last layer first
-        self._backward_chain([self.layers[13]] + self.layers[12::-1], g, debug)
+        # ---- the RPN 3x3 conv (feat_ch -> 512, its own bias), then the trunk from the gradient of the feature map
+        R, fh, fw, C = self.rpn_layer, self.fh, self.fw, self.feat_ch
+        dy = self._gact(fh, fw, 512)
+        dyT = self._tbuf(1, 512, fh, fw)
+        self._prep(fh, fw, 512, g=g, y=R["y"], out=dy, tbuf=dyT)
+        if debug is not None:
+            debug[R["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
+        xT = self._tbuf(3, C, fh, fw)
+        self._prep(fh, fw, C, g=self.feat, tbuf=xT)
+        self._wgrad(dyT, xT, 512, C, 9, self.grads(R["name"] + "/W"))
+        train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
+        g = self._gact(fh, fw, C, tag=self.feat_grad_tag)
+        self._conv(dy, self.packed[R["name"]][2], self.zero_bias, 3, False, self.halvings, out=g)
+        if debug is not None:
+            debug[R["name"]]["g_out"] = self._chw(g)
+        self._backward_trunk(g, debug)
 
     def _backward_heads(self, debug=None):
         """The twin 1x1 heads' weight / bias gradients; returns the gradient w.r.t. the RPN 3x3 conv's post-ReLU output."""
@@ -372,113 +543,6 @@ class RpnTrainer(_ConvTrainer):
             debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
         return g
 
-    def _backward_chain(self, chain, g, debug=None):
-        """g: gradient (ops.Act) w.r.t. the post-ReLU output of chain[0] -- at pooled resolution if that layer is followed
-        by a pool.  Per layer: ReLU / pool backward + re-layout, weight + bias gradient, data gradient for the next one.
-        On a canvas the weight gradients run over K = N*Kp, the sum over the slots."""
-        for L in chain:
-            h, w, co, ci = L["H"], L["W"], L["cout"], L["cin"]
-            first = L is self.layers[0]
-            dy = self._gact(h, w, co)
-            dyT = self._tbuf(1, co, h, w)
-            self._prep(h, w, co, g=g, y=L["y"], p=L.get("p") if L["pool"] else None, out=dy, tbuf=dyT)
-            if debug is not None:
-                debug[L["name"]] = dict(g_in=self._chw(g), dy=self._chw(dy))
-            x = self._input_of(L)
-            if first:
-                xT = self._tbuf(1, 32, h, w)
-                self._prep(h, w, 32, g=x, tbuf=xT)
-                dwc = torch.empty((co, 32), dtype=torch.float32, device=self.device)
-                self._wgrad(dyT, xT, co, 32, 1, dwc)
-                # im2col column k = tap*3 + c  ->  OIHW [co][c][tap]
-                self.grads(L["name"] + "/W").copy_(dwc[:, :27].reshape(co, 9, 3).permute(0, 2, 1).reshape(co, 3, 3, 3))
-            else:
-                xT = self._tbuf(3, ci, h, w)
-                self._prep(h, w, ci, g=x, tbuf=xT)
-                self._wgrad(dyT, xT, co, ci, 9, self.grads(L["name"] + "/W"))
-            train_ops.bias_grad(dyT, co, self.grads(L["name"] + "/b"))
-            self._early_exchange(L["name"])
-            if not first:
-                g = self._gact(h, w, ci, tag=1)
-                self._conv(dy, self.packed[L["name"]][2], self.zero_bias, 3, False, L["halvings"], out=g)
-                if debug is not None:
-                    debug[L["name"]]["g_out"] = self._chw(g)
-
-    def _input_of(self, L):
-        i = self.layers.index(L)
-        if i == 0:
-            return self.x_col
-        if i == 13:
-            return self.feat
-        prev = self.layers[i - 1]
-        return prev["p"] if prev["pool"] else prev["y"]
-
-    # ---------------------------------------------------------------- gradient exchange + optimizer
-    def set_grad_exchange(self, grad_dtype="fp32", overlap=True):
-        """grad_dtype "fp32" (exact) or "bf16" (config #5); overlap: reduce the deep-layer bucket during the rest of backward."""
-        if grad_dtype not in ("fp32", "bf16"):
-            raise FrcnnError("grad_dtype must be fp32 or bf16")
-        self.grad_dtype = grad_dtype
-        if grad_dtype == "bf16" and self.g_bf16 is None:
-            self.g_bf16 = torch.zeros(self.g_flat.shape, dtype=torch.bfloat16, device=self.device)
-        self._overlap = bool(overlap)
-
-    def _multi(self):
-        return shard.dist.is_available() and shard.dist.is_initialized() and shard.dist.get_world_size(self.pg) > 1
-
-    def _exchange(self, lo, hi):
-        """All-reduce(SUM) of g_flat[lo:hi] on the communication stream, after everything queued so far on the compute stream."""
-        if self.comm_stream is None:
-            self.comm_stream = torch.cuda.Stream(device=self.device)
-        ev = torch.cuda.Event()
-        ev.record()
-        self.comm_stream.wait_event(ev)
-        with torch.cuda.stream(self.comm_stream):
-            if self.grad_dtype == "bf16":
-                train_ops.cast_f32_bf16(self.g_flat[lo:hi], self.g_bf16[lo:hi])
-                shard.allreduce_sum_(self.g_bf16[lo:hi], self.pg)
-            else:
-                shard.allreduce_sum_(self.g_flat[lo:hi], self.pg)
-
-    def _early_exchange(self, layer_name):
-        """Called from the backward chain right after `layer_name`'s gradients are enqueued."""
-        if not getattr(self, "_overlap", True) or not self._multi() or layer_name != "trunk/conv4_1":
-            return
-        lo = self.index["trunk/conv4_1/W"][0]
-        if lo % 4 != 0:
-            return
-        self._bucket_lo = lo
-        self._exchange(lo, self.g_flat.numel())
-
-    def update(self):
-        """[all-reduce SUM over ranks, like ParallelUpdater's addgrads] + WeightDecay + MomentumSGD, then repack."""
-        if self._multi():
-            hi = self._bucket_lo if self._bucket_lo is not None else self.g_flat.numel()
-            self._ev_bwd = torch.cuda.Event(enable_timing=True)
-            self._ev_bwd.record()                                  # backward fully enqueued on the compute stream
-            self._exchange(0, hi)
-            self._ev_comm = torch.cuda.Event(enable_timing=True)
-            self._ev_comm.record(self.comm_stream)
-            torch.cuda.current_stream().wait_event(self._ev_comm)
-            self._bucket_lo = None
-        if self.grad_dtype == "bf16" and self._multi():
-            train_ops.sgd_momentum_bf16g(self.w_flat, self.v_flat, self.g_bf16, self.lr, self.momentum, self.weight_decay)
-        else:
-            train_ops.sgd_momentum(self.w_flat, self.v_flat, self.g_flat, self.lr, self.momentum, self.weight_decay)
-        self.repack()
-        self.n_updates += 1
-
-    def last_exposed_exchange_ms(self):
-        """Time between "backward done" on the compute stream and "exchange done" on the communication stream for the last
-        step (what the optimizer had to wait for); call after a synchronize.  0 if the exchange finished first."""
-        if self._ev_bwd is None or self._ev_comm is None:
-            return 0.0
-        return max(0.0, self._ev_bwd.elapsed_time(self._ev_comm))
-
-    def export_params(self):
-        """Trainable parameters as numpy arrays under the reference's names (checkpoint / write-back into the Links)."""
-        return {n: self.weights(n).detach().cpu().numpy().copy() for n in self.index}
-
     def step(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
         losses = self.forward(x_chw, gt_boxes, im_info, disable_pos)
         self.backward()
@@ -486,54 +550,30 @@ class RpnTrainer(_ConvTrainer):
         return losses
 
 
-def _rpn_params(A):
-    """The RPN heads' parameters in flat-buffer order, stored adjacently so that (W_cls | W_bbox) is ONE [6A, 512] matrix:
-    cls W, bbox W, cls b, bbox b."""
-    heads = [("RPN/rpn_cls_score", 2 * A), ("RPN/rpn_bbox_pred", 4 * A)]
-    return [(n + "/W", (co, 512, 1, 1)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
+class _RcnnStep(_ConvTrainer):
+    """The RCNN step over any trunk: the frozen test-mode RPN, ProposalLayer, ProposalTargetLayer, RoI pooling, fc6 / fc7
+    with dropout, cls_score | bbox_pred, the losses and the backward through the head and the RoI pooling into the trunk's.
+    fc6/W is kept in the (h, w, c) input order the RoI-pool kernel emits (`export_params` converts back)."""
 
-
-def _rcnn_params(nc, feat_ch=512):
-    """The head parameters of the RCNN step in flat-buffer order (cls_score | bbox_pred adjacent: one [5*nc, 4096] matrix);
-    fc6 reads the 7x7 RoI pool of a feat_ch-channel feature map."""
-    heads = [("cls_score", nc), ("bbox_pred", 4 * nc)]
-    extra = [("fc6/W", (4096, feat_ch * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
-    return extra + [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads]
-
-
-def _fc6_to_hwc(name, a):                           # fc6 columns (c, h, w) -> (h, w, c), the order the RoI pooling emits
-    return a.reshape(4096, -1, 49).transpose(0, 2, 1) if name == "fc6/W" else a
-
-
-class RcnnTrainer(RpnTrainer):
-    """One train_rcnn.py step (`model.rcnn_train = True`, /root/reference models/faster_rcnn.py:114-173): trunk -> RPN in TEST
-    mode (its weights are frozen here: proposals are plain arrays, faster_rcnn.py:117-120) -> ProposalTargetLayer ->
-    RoI pooling of ALL proposals -> fc6 / fc7 with dropout -> cls_score | bbox_pred -> losses on the kept rows ->
-    backward through the head, the RoI pooling and the 13 trunk convolutions -> WeightDecay + MomentumSGD.
-    Trainable: trunk/*, fc6, fc7, cls_score, bbox_pred (the RPN links receive no gradient: cleargrads semantics).
-
-    fc6/W is kept internally in the (h, w, c) input order the RoI-pool kernel emits (`export_params` converts back).
-    Sampling (`sample="numpy"`): the proposals' best overlaps come back to the host and np.random.choice draws exactly as
-    proposal_target_layer.py:99-129 does, so a seeded run reproduces the reference's kept set; `keep_inds=` pins it.
-    Dropout masks are explicit inputs (uint8 [post_n, 4096] x 2) or drawn from a torch generator."""
-
-    def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
-        nc = self.num_classes = num_classes
-        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [], _rcnn_params(nc), load_transform=_fc6_to_hwc)
+    def _init_rcnn(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                   num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout):
+        self.num_classes = num_classes
+        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
-        self._init_one_image_rcnn(sample, seed, dropout)
-        self.repack()
-
-    def _init_one_image_rcnn(self, sample, seed, dropout):
-        """The one-image step's sampling and dropout settings and its proposal workspace."""
         self.sample, self.dropout = sample, dropout
         self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
         self.prop = ops.ProposalWorkspace(self.A, self.fh, self.fw, self.pre_n, self.post_n, self.device)
         self.roi_ws = None
+        self.repack()
+
+    def _step_table(self, A):
+        """The step's convolutions (none) and parameters in flat-buffer order (cls_score | bbox_pred adjacent: one
+        [5*nc, 4096] matrix; fc6 reads the 7x7 RoI pool of the feature map), and the frozen RPN: the RPN step's parameters."""
+        heads = [("cls_score", self.num_classes), ("bbox_pred", 4 * self.num_classes)]
+        fc = [("fc6/W", (4096, self.feat_ch * 49)), ("fc6/b", (4096,)), ("fc7/W", (4096, 4096)), ("fc7/b", (4096,))]
+        frozen_rpn = _entries(*_RpnStep._step_table(self, A)[:2])
+        return [], fc + [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads], frozen_rpn
 
     def _init_rcnn_head(self, params, delta, post_n, pre_n, nms_thresh, min_size):
         """The RCNN step's frozen RPN with its outputs, and the head's settings and activations."""
@@ -580,7 +620,7 @@ class RcnnTrainer(RpnTrainer):
         return out
 
     def repack(self):
-        self._repack_convs()
+        self._repack_trunk()
         for n in ("fc6", "fc7"):
             self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), 4096)
         self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
@@ -697,10 +737,6 @@ class RcnnTrainer(RpnTrainer):
             debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
         self._backward_trunk(gfeat, debug)
 
-    def _backward_trunk(self, g, debug=None):
-        """Backward through the trunk from g, the gradient of the feature map (ops.Act): the 13 VGG16 convolutions."""
-        self._backward_chain(self.layers[12::-1], g, debug)
-
     def _roi_pool_backward(self, g):
         """dfeat = the RoI pooling's backward of g (the gradient of pool5)."""
         if self.roi_ws is None:
@@ -717,7 +753,7 @@ class RcnnTrainer(RpnTrainer):
 
 
 class _CanvasSteps(object):
-    """The canvas machinery shared by CanvasRpnTrainer and CanvasRcnnTrainer: the N-slot image input with its device extents,
+    """The canvas machinery shared by _CanvasRpnStep and _CanvasRcnnStep: the N-slot image input with its device extents,
     the staged ground truth, the launches over the canvas (the _ext convolutions, zero outside each image, and the _batch
     re-layouts) that override _ConvTrainer's, and the capture-then-replay step."""
     raw_input = False           # True: the input is RawPhotoInput's training block (put_raw / step_raw)
@@ -866,44 +902,21 @@ class _CanvasSteps(object):
         return self.step_losses.clone()
 
 
-class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
-    """The RPN-mode training step on N images of different sizes per update, with one set of weights and optimizer state.
-
-    Each image sits at the top-left of its slot of an N-slot Hc x Wc canvas (engine.ImageInput); its size and clip bounds
-    are device arrays that every launch reads at run time, so one trainer -- and one captured CUDA graph -- serves any mix
-    of sizes up to the canvas.  Forward and backward are RpnTrainer's chain over [N]-slabs: the *_batch_ext convolutions
-    (zero outside each image), frcnn_anchor_targets_batch / frcnn_rpn_loss_batch (slot n is normalised by its own counts
-    and anchor count, like the reference's per-device loss), frcnn_grad_prepare_batch and weight-gradient GEMMs over
-    K = N*Kp, so the gradient is the SUM of the N per-image gradients (ParallelUpdater's addgrads, train_rpn.py:169-174),
-    followed by one WeightDecay + MomentumSGD update.  Inside each image every activation, masked gradient and data
-    gradient equals RpnTrainer's on that image alone, bit for bit; with N = 1 and an image that fills the canvas the whole
-    step does.
-
-    subsample "device": slot n of step t draws with seed + t*N + n (a device counter advanced inside the step, so a replayed
-    graph draws fresh samples): the k-th image of a stream gets the labels RpnTrainer(seed=seed) gives its k-th image.
-    "list": put() takes per-image disable lists (positions in the inside-compact order, frcnn_anchor_targets mode 2).
-    "none": labels before subsampling."""
+class _CanvasRpnStep(_CanvasSteps, _RpnStep):
+    """_RpnStep on a canvas (CanvasRpnTrainer describes it): staging, the batched anchor targets and loss."""
 
     _MODES = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST, "none": train_ops.SUBSAMPLE_NONE}
 
-    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
-                 process_group=None, raw_input=False):
-        self._rpn_options(N, subsample, max_gt)
-        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
-        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [dict(name="RPN/rpn_conv_3x3", cin=512, cout=512, k=3)], _rpn_params(len(anchors)), lead=(N,))
-        self._init_canvas_rpn(Hc, Wc, loss_lambda, delta, subsample, seed, raw_input)
-
-    def _rpn_options(self, N, subsample, max_gt):
+    def _init_canvas_rpn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                         delta, subsample, seed, max_gt, device, process_group, raw_input):
+        """Checks the options, then builds the trunk, the RPN head, the canvas input, the batched anchor targets and the
+        subsampling lists; then the first repack."""
         self._canvas_options(N, max_gt)
         if subsample not in self._MODES:
             raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
-
-    def _init_canvas_rpn(self, Hc, Wc, loss_lambda, delta, subsample, seed, raw_input):
-        """After the trunk: the RPN head, the canvas input, the batched anchor targets and the subsampling lists; then the
-        first repack."""
-        N, max_gt = self.N, self.max_gt
+        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          lead=(N,))
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         dev = self.device
@@ -983,39 +996,18 @@ class CanvasRpnTrainer(_CanvasSteps, RpnTrainer):
         return self._step()
 
 
-class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
-    """The RCNN-mode training step (RcnnTrainer's, train_rcnn.py) on N images of different sizes per update, with one set of
-    weights and optimizer state and one captured CUDA graph.
-
-    Forward: the canvas trunk, the frozen RPN (_ext convolutions + frcnn_proposals_batch_ext, whose per-slot proposal count
-    is written straight into column 1 of the [N][2] extents (1, R_n) of the head), frcnn_proposal_targets_batch,
-    frcnn_roi_pool_batch_ext, fc6 / fc7 / cls_score | bbox_pred as _ext convolutions over N x 1 x R_cap (rows >= R_n are 0,
-    as RcnnTrainer's m_valid leaves them), dropout, frcnn_rcnn_loss_batch (slot n normalised by its own kept count).
-    Backward: the head and fc layers through frcnn_grad_prepare_batch with weight GEMMs over K = N*Kp,
-    frcnn_roi_pool_backward_batch_ext, then the trunk; one WeightDecay + MomentumSGD update on the summed gradient.
-    Inside each image every activation and data gradient equals RcnnTrainer's on that image with the same kept rows and
-    masks, bit for bit.
-
-    sample "device": slot n of step t samples with seed + t*N + n (frcnn_proposal_targets_batch mode 1, a device counter
-    advanced inside the step); "list": put() takes per-image kept lists (RcnnTrainer's keep_inds, at most 128 distinct rows).
-    dropout "device": masks drawn by frcnn_dropout_masks_batch from the same per-slot seeds (salt 1: fc6, 2: fc7); "explicit":
-    put() takes per-image (fc6, fc7) uint8 [post_n, 4096] masks; None: no dropout.  `masks` [2, N, post_n, 4096] holds the
-    masks the last step used."""
+class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
+    """_RcnnStep on a canvas (CanvasRcnnTrainer describes it): staging, device-side sampling and dropout, the batched
+    proposals, targets, RoI pooling and loss."""
 
     _SAMPLE = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST}
     _DROPOUT = ("device", "explicit", None)
 
-    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False):
-        self._rcnn_options(N, sample, dropout, max_gt, post_n)
-        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
-        nc = self.num_classes = num_classes
-        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          [], _rcnn_params(nc), load_transform=_fc6_to_hwc, lead=(N,))
-        self._init_canvas_rcnn(params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input)
-
-    def _rcnn_options(self, N, sample, dropout, max_gt, post_n):
+    def _init_canvas_rcnn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
+                          delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device, process_group,
+                          raw_input):
+        """Checks the options, then builds the trunk, the canvas input, the frozen RPN and the head, the batched proposals,
+        targets, kept lists and masks; then the first repack."""
         who = type(self).__name__
         self._canvas_options(N, max_gt)
         if sample not in self._SAMPLE:
@@ -1024,11 +1016,9 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
             raise FrcnnError("%s: dropout must be one of %s" % (who, self._DROPOUT))
         if not 1 <= int(post_n) <= 4096:
             raise FrcnnError("%s: post_n must be in [1, 4096] (got %r)" % (who, post_n))
-
-    def _init_canvas_rcnn(self, params, Hc, Wc, delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, raw_input):
-        """After the trunk: the canvas input, the frozen RPN and the head, the batched proposals, targets, kept lists and
-        masks; then the first repack."""
-        N, max_gt, nc = self.N, self.max_gt, self.num_classes
+        self.N, self.max_gt, self.num_classes = N, max_gt, nc = int(N), int(max_gt), num_classes
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          lead=(N,))
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self.sample, self.dropout = sample, dropout
@@ -1147,3 +1137,83 @@ class CanvasRcnnTrainer(_CanvasSteps, RcnnTrainer):
         """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
         self.put_raw(photos, boxes, labels, keep_inds, masks)
         return self._step()
+
+
+class RpnTrainer(_Vgg16Trunk, _RpnStep):
+    """Weights, optimizer state and buffers of the RPN-mode training step for one image shape."""
+
+    def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+        self._init_rpn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                       loss_lambda, delta, subsample, seed)
+
+
+class RcnnTrainer(_Vgg16Trunk, _RcnnStep):
+    """One train_rcnn.py step (`model.rcnn_train = True`, /root/reference models/faster_rcnn.py:114-173): trunk -> RPN in TEST
+    mode (its weights are frozen here: proposals are plain arrays, faster_rcnn.py:117-120) -> ProposalTargetLayer ->
+    RoI pooling of ALL proposals -> fc6 / fc7 with dropout -> cls_score | bbox_pred -> losses on the kept rows ->
+    backward through the head, the RoI pooling and the 13 trunk convolutions -> WeightDecay + MomentumSGD.
+    Trainable: trunk/*, fc6, fc7, cls_score, bbox_pred (the RPN links receive no gradient: cleargrads semantics).
+
+    fc6/W is kept internally in the (h, w, c) input order the RoI-pool kernel emits (`export_params` converts back).
+    Sampling (`sample="numpy"`): the proposals' best overlaps come back to the host and np.random.choice draws exactly as
+    proposal_target_layer.py:99-129 does, so a seeded run reproduces the reference's kept set; `keep_inds=` pins it.
+    Dropout masks are explicit inputs (uint8 [post_n, 4096] x 2) or drawn from a torch generator."""
+
+    def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
+                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
+        self._init_rcnn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout)
+
+
+class CanvasRpnTrainer(_Vgg16Trunk, _CanvasRpnStep):
+    """The RPN-mode training step on N images of different sizes per update, with one set of weights and optimizer state.
+
+    Each image sits at the top-left of its slot of an N-slot Hc x Wc canvas (engine.ImageInput); its size and clip bounds
+    are device arrays that every launch reads at run time, so one trainer -- and one captured CUDA graph -- serves any mix
+    of sizes up to the canvas.  Forward and backward are RpnTrainer's chain over [N]-slabs: the *_batch_ext convolutions
+    (zero outside each image), frcnn_anchor_targets_batch / frcnn_rpn_loss_batch (slot n is normalised by its own counts
+    and anchor count, like the reference's per-device loss), frcnn_grad_prepare_batch and weight-gradient GEMMs over
+    K = N*Kp, so the gradient is the SUM of the N per-image gradients (ParallelUpdater's addgrads, train_rpn.py:169-174),
+    followed by one WeightDecay + MomentumSGD update.  Inside each image every activation, masked gradient and data
+    gradient equals RpnTrainer's on that image alone, bit for bit; with N = 1 and an image that fills the canvas the whole
+    step does.
+
+    subsample "device": slot n of step t draws with seed + t*N + n (a device counter advanced inside the step, so a replayed
+    graph draws fresh samples): the k-th image of a stream gets the labels RpnTrainer(seed=seed) gives its k-th image.
+    "list": put() takes per-image disable lists (positions in the inside-compact order, frcnn_anchor_targets mode 2).
+    "none": labels before subsampling."""
+
+    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
+                 process_group=None, raw_input=False):
+        self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                              delta, subsample, seed, max_gt, device, process_group, raw_input)
+
+
+class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
+    """The RCNN-mode training step (RcnnTrainer's, train_rcnn.py) on N images of different sizes per update, with one set of
+    weights and optimizer state and one captured CUDA graph.
+
+    Forward: the canvas trunk, the frozen RPN (_ext convolutions + frcnn_proposals_batch_ext, whose per-slot proposal count
+    is written straight into column 1 of the [N][2] extents (1, R_n) of the head), frcnn_proposal_targets_batch,
+    frcnn_roi_pool_batch_ext, fc6 / fc7 / cls_score | bbox_pred as _ext convolutions over N x 1 x R_cap (rows >= R_n are 0,
+    as RcnnTrainer's m_valid leaves them), dropout, frcnn_rcnn_loss_batch (slot n normalised by its own kept count).
+    Backward: the head and fc layers through frcnn_grad_prepare_batch with weight GEMMs over K = N*Kp,
+    frcnn_roi_pool_backward_batch_ext, then the trunk; one WeightDecay + MomentumSGD update on the summed gradient.
+    Inside each image every activation and data gradient equals RcnnTrainer's on that image with the same kept rows and
+    masks, bit for bit.
+
+    sample "device": slot n of step t samples with seed + t*N + n (frcnn_proposal_targets_batch mode 1, a device counter
+    advanced inside the step); "list": put() takes per-image kept lists (RcnnTrainer's keep_inds, at most 128 distinct rows).
+    dropout "device": masks drawn by frcnn_dropout_masks_batch from the same per-slot seeds (salt 1: fc6, 2: fc7); "explicit":
+    put() takes per-image (fc6, fc7) uint8 [post_n, 4096] masks; None: no dropout.  `masks` [2, N, post_n, 4096] holds the
+    masks the last step used."""
+
+    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
+                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False):
+        self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
+                               delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
+                               process_group, raw_input)

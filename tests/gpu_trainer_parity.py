@@ -1,10 +1,13 @@
 """Three training steps of every trainer kind with fixed seeds, saved to npz, to compare two builds of the trainers bit for
-bit: losses, g_flat, w_flat and v_flat after the last step.
+bit: losses, g_flat, w_flat and v_flat after the last step.  The kinds are the eight trainers (VGG16 and ResNet-50, one
+image and canvas, RPN and RCNN) and the one-image VGG16 RPN step with NumPy subsampling.  The flat buffers are saved as
+SHA-256 digests of their bytes: the ResNet RCNN trainers' are 1.6 GB each.
 
     python tests/gpu_trainer_parity.py --out a.npz [--pkg DIR]     # DIR: the chainer-faster-rcnn_b200 tree to import
     python tests/gpu_trainer_parity.py --compare a.npz b.npz
 """
 import argparse
+import hashlib
 import os
 import sys
 
@@ -25,19 +28,27 @@ def _inputs(torch, n, seed):
 def run(out):
     import torch
     import frcnn_oracle as orc
-    from frcnn_b200.resnet_train import ResNetRpnTrainer
+    from frcnn_b200.resnet_train import CanvasResNetRcnnTrainer, CanvasResNetRpnTrainer, ResNetRcnnTrainer, ResNetRpnTrainer
     from frcnn_b200.train_engine import CanvasRcnnTrainer, CanvasRpnTrainer, RcnnTrainer, RpnTrainer
     anchors = orc.generate_anchors(ratios=(0.5, 1, 2), scales=(8, 16, 32))
     vgg = orc.make_params(seed=77)
     rng = np.random.default_rng(78)
     for k in ("cls_score/W", "bbox_pred/W"):
         vgg[k] = (rng.standard_normal(vgg[k].shape) * 0.02).astype(np.float32)
+    r50 = orc.make_resnet_params(50, seed=3)
+    for k, s in (("RPN/rpn_cls_score/W", 0.05), ("RPN/rpn_bbox_pred/W", 0.05), ("fc6/W", 0.001), ("fc7/W", 0.01),
+                 ("cls_score/W", 0.01), ("bbox_pred/W", 0.01)):     # proposals that overlap the boxes, a live head
+        r50[k] = (rng.standard_normal(r50[k].shape) * s).astype(np.float32)
     res = {}
     kinds = [("rpn", lambda: RpnTrainer(vgg, H, W, anchors)),
+             ("rpn_numpy", lambda: RpnTrainer(vgg, H, W, anchors, subsample="numpy")),
              ("rcnn", lambda: RcnnTrainer(vgg, H, W, anchors, post_n=120)),
              ("canvas_rpn", lambda: CanvasRpnTrainer(vgg, 2, H, W, anchors)),
              ("canvas_rcnn", lambda: CanvasRcnnTrainer(vgg, 2, H, W, anchors, post_n=120)),
-             ("resnet50", lambda: ResNetRpnTrainer(orc.make_resnet_params(50, seed=3), H, W, anchors, n_layers=50))]
+             ("resnet50", lambda: ResNetRpnTrainer(orc.make_resnet_params(50, seed=3), H, W, anchors, n_layers=50)),
+             ("resnet50_rcnn", lambda: ResNetRcnnTrainer(r50, H, W, anchors, n_layers=50, post_n=120)),
+             ("canvas_resnet50_rpn", lambda: CanvasResNetRpnTrainer(r50, 2, H, W, anchors, n_layers=50)),
+             ("canvas_resnet50_rcnn", lambda: CanvasResNetRcnnTrainer(r50, 2, H, W, anchors, n_layers=50, post_n=120))]
     for name, make in kinds:
         torch.manual_seed(0)
         np.random.seed(0)
@@ -51,7 +62,7 @@ def run(out):
         torch.cuda.synchronize()
         res[name + "/losses"] = torch.stack(losses).cpu().numpy()
         for f in ("g_flat", "w_flat", "v_flat"):
-            res[name + "/" + f] = getattr(tr, f).cpu().numpy()
+            res[name + "/" + f] = np.array(hashlib.sha256(getattr(tr, f).cpu().numpy().tobytes()).hexdigest())
         print(name, res[name + "/losses"][-1].ravel().tolist(), flush=True)
         del tr
         torch.cuda.empty_cache()

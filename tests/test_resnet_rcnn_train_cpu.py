@@ -3,8 +3,9 @@
 - the float64 reference (resnet_rcnn_train_oracle.resnet_rcnn_train_step): its unfolded frozen-BN trunk gradients equal s times
   its folded ones;
 - the constructor's checks on device="cpu", every one raised before anything is allocated;
-- launch traces against the recording stand-in of test_trainer_launches_cpu: the trunk part of ResNetRcnnTrainer.backward
-  is, entry for entry, ResNetRpnTrainer's bottleneck backward, and update() repacks in place.
+- launch traces against the recording stand-in of test_trainer_launches_cpu: on either trunk, the trunk part of the RCNN
+  step's backward is, entry for entry, the RPN step's (ResNetRcnnTrainer's is ResNetRpnTrainer's bottleneck backward,
+  RcnnTrainer's is RpnTrainer's 13 convolutions), and update() repacks in place.
 
 fc6 alone is 4096 x 100,352 float32 (1.6 GB), so the trainer is built once, under the recorder, for the whole module."""
 import numpy as np
@@ -13,7 +14,7 @@ import torch
 
 import frcnn_oracle as orc
 import resnet_rcnn_train_oracle as rto
-from test_trainer_launches_cpu import ANCHORS, POST_N, H, W, Recorder, _image_and_gt, _install, _keep_and_masks, _normalised, _planes
+from test_trainer_launches_cpu import ANCHORS, POST_N, H, W, Recorder, _forward, _install, _normalised, _planes, _vgg_params
 
 f32 = np.float32
 
@@ -24,41 +25,49 @@ def params():
 
 
 @pytest.fixture(scope="module")
-def recorded(params):
-    """(recorder, ResNetRcnnTrainer, ResNetRpnTrainer) at 64 x 96, ResNet-50, built and warmed up under the recorder."""
+def recorder():
     from frcnn_b200 import _lib
-    from frcnn_b200.resnet_train import ResNetRcnnTrainer, ResNetRpnTrainer
     r = Recorder(_lib.load())
     with pytest.MonkeyPatch.context() as mp:
         _install(mp.setattr, r)
-        rcnn = ResNetRcnnTrainer(params, H, W, ANCHORS, n_layers=50, post_n=POST_N, device="cpu")
-        rpn = ResNetRpnTrainer(params, H, W, ANCHORS, n_layers=50, device="cpu")
-        for tr in (rcnn, rpn):
-            _forward(tr)
-            tr.backward()
-        yield r, rcnn, rpn
+        yield r
 
 
-def _forward(tr):
-    """One forward on the fixed inputs of test_trainer_launches_cpu (the ResNet trainers' own forward rejects CPU images)."""
+def _warmed(rcnn, rpn):
+    for tr in (rcnn, rpn):
+        _forward(tr)
+        tr.backward()
+    return rcnn, rpn
+
+
+@pytest.fixture(scope="module")
+def recorded(recorder, params):
+    """(recorder, ResNetRcnnTrainer, ResNetRpnTrainer) at 64 x 96, ResNet-50, built and warmed up under the recorder."""
+    from frcnn_b200.resnet_train import ResNetRcnnTrainer, ResNetRpnTrainer
+    return (recorder,) + _warmed(ResNetRcnnTrainer(params, H, W, ANCHORS, n_layers=50, post_n=POST_N, device="cpu"),
+                                 ResNetRpnTrainer(params, H, W, ANCHORS, n_layers=50, device="cpu"))
+
+
+@pytest.fixture(scope="module")
+def recorded_vgg16(recorder):
+    """(recorder, RcnnTrainer, RpnTrainer) at 64 x 96, built and warmed up under the recorder."""
     from frcnn_b200.train_engine import RcnnTrainer, RpnTrainer
-    x, gt = _image_and_gt()
-    keep, masks = _keep_and_masks()
-    if isinstance(tr, RcnnTrainer):
-        RcnnTrainer.forward(tr, x, gt, keep_inds=keep, masks=masks)
-    else:
-        RpnTrainer.forward(tr, x, gt)
+    vgg = _vgg_params()
+    return (recorder,) + _warmed(RcnnTrainer(vgg, H, W, ANCHORS, post_n=POST_N, device="cpu"),
+                                 RpnTrainer(vgg, H, W, ANCHORS, device="cpu"))
 
 
 def _trunk_trace(rec, tr):
-    """The normalised launches of tr.backward() from its _backward_trunk call on, and the launches before it."""
+    """The normalised launches of tr.backward() from its _backward_trunk call on, and the launches before it.  The
+    gradient _backward_trunk receives and the trunk's own data-gradient buffer at the feature map (tag feat_grad_tag) are
+    both named g: the RPN step hands the trunk its gradient in that buffer, VGG16's RCNN step in one of its own."""
     _forward(tr)
     rec.reset()
     start = []
     inner = tr._backward_trunk
 
     def hook(g, debug=None):
-        start.append(len(rec.calls))
+        start.append((len(rec.calls), g))
         return inner(g, debug)
     tr._backward_trunk = hook
     try:
@@ -66,20 +75,29 @@ def _trunk_trace(rec, tr):
     finally:
         del tr._backward_trunk
     assert len(start) == 1
-    return rec.calls[:start[0]], _normalised(rec.calls[start[0]:])
+    at, g = start[0]
+    names = {}
+    for act in (g, tr._gact(tr.fh, tr.fw, tr.feat_ch, tag=tr.feat_grad_tag)):
+        for part, t in (("g.hi", act.hi), ("g.lo", act.lo)):
+            if t is not None and t.data_ptr() in rec._ptrs:
+                names["p%d" % rec._ptrs[t.data_ptr()]] = part
+    return rec.calls[:at], _normalised(rec.calls[at:], names)
 
 
-def test_rcnn_trunk_backward_is_the_rpn_trunk_backward(recorded):
-    rec, rcnn, rpn = recorded
+@pytest.mark.parametrize("trunk,C,stride,least", [("recorded", 2048, 32, 150), ("recorded_vgg16", 512, 16, 50)],
+                         ids=["resnet50", "vgg16"])
+def test_rcnn_trunk_backward_is_the_rpn_trunk_backward(request, trunk, C, stride, least):
+    rec, rcnn, rpn = request.getfixturevalue(trunk)
     head_rcnn, trunk_rcnn = _trunk_trace(rec, rcnn)
     head_rpn, trunk_rpn = _trunk_trace(rec, rpn)
-    assert len(trunk_rcnn) > 150
+    assert len(trunk_rcnn) > least
     assert trunk_rcnn == trunk_rpn
-    # what comes before it: the head and fc layers, the RoI pooling backward over 2048 channels and its re-layout
+    # what comes before it: the head and fc layers, the RoI pooling backward over the feature map's C channels and its
+    # re-layout
     names = [c[0] for c in head_rcnn]
     assert names.count("frcnn_roi_pool_backward") == 1
     roi = head_rcnn[names.index("frcnn_roi_pool_backward")]
-    assert roi[3:6] == [rcnn.fh, rcnn.fw, 2048] and roi[11] == pytest.approx(1.0 / 32)
+    assert roi[3:6] == [rcnn.fh, rcnn.fw, C] and roi[11] == pytest.approx(1.0 / stride)
     assert [c[0] for c in head_rpn][-1] == "frcnn_conv2d"               # the RPN 3x3 conv's data gradient
 
 

@@ -10,7 +10,9 @@ Checked here:
 - the one-image and the N = 1 canvas trainers launch the same backward, entry for entry, once the batch entries are
   mapped to their one-image twins and the N, extents / halvings and m_valid arguments are dropped;
 - every trainer repacks its weights in place: `packed` keeps its tensors across update(), which a captured graph and
-  any caller holding the planes rely on.
+  any caller holding the planes rely on;
+- every public trainer is one trunk and one step, and a VGG16 trainer rejects a missing or misshapen parameter before
+  it allocates anything, as a ResNet trainer does.
 
 `python tests/test_trainer_launches_cpu.py out.json` dumps the forward, backward and update traces of every trainer and
 mode to JSON, for comparing two builds of the trainers."""
@@ -97,22 +99,24 @@ def rec(monkeypatch):
 
 
 def _install(setattr_, r):
-    from frcnn_b200 import _lib, ops, train_ops
+    from frcnn_b200 import _lib, ops, resnet_train, train_ops
     setattr_(_lib, "_lib", r)
     for m in (ops, train_ops):
         setattr_(m, "_p", r.pointer)
         setattr_(m, "_stream", lambda: None)
         setattr_(m, "_need_cuda", lambda *ts: None)
+    setattr_(resnet_train._ResNetTrunk, "_check_input", lambda self, x, g: None)      # the ResNet trainers take CPU images
 
 
-def _normalised(calls):
-    """Batch entries as their one-image twins, without N, extents / halvings and m_valid, pointers renumbered."""
-    out, ptrs = [], {}
+def _normalised(calls, names=None):
+    """Batch entries as their one-image twins, without N, extents / halvings and m_valid, pointers renumbered (those in
+    `names`, {recorded pointer: name}, named as given)."""
+    out, ptrs, names = [], {}, names or {}
     for c in calls:
         name, args = c[0], c[1:]
         name, drop = TWINS.get(name, (name, ONE_IMAGE_DROP.get(name, ())))
         args = [a for i, a in enumerate(args) if i not in drop]
-        out.append([name] + [ptrs.setdefault(a, "p%d" % len(ptrs)) if isinstance(a, str) else a for a in args])
+        out.append([name] + [names.get(a) or ptrs.setdefault(a, "p%d" % len(ptrs)) if isinstance(a, str) else a for a in args])
     return out
 
 
@@ -156,7 +160,7 @@ def _canvas_rcnn(params, N=1, **kw):
 
 def _forward(tr):
     """One forward of any trainer on the fixed inputs (staged first for a canvas trainer)."""
-    from frcnn_b200.train_engine import RcnnTrainer, RpnTrainer, _CanvasSteps
+    from frcnn_b200.train_engine import _CanvasSteps
     x, gt = _image_and_gt()
     keep, masks = _keep_and_masks()
     if isinstance(tr, _CanvasSteps):
@@ -171,10 +175,10 @@ def _forward(tr):
                 kw["masks"] = [masks] * n
             tr.put([x] * n, [gt] * n, **kw)
         tr.forward()
-    elif isinstance(tr, RcnnTrainer):
+    elif hasattr(tr, "num_classes"):
         tr.forward(x, gt, keep_inds=keep, masks=masks)
     else:
-        RpnTrainer.forward(tr, x, gt)                      # ResNetRpnTrainer.forward rejects a CPU image
+        tr.forward(x, gt)
 
 
 # ------------------------------------------------------------------------------------------------ tests
@@ -232,23 +236,73 @@ def test_update_repacks_in_place(rec, kind):
     assert _planes(tr) == before
 
 
+def test_each_trainer_has_one_trunk():
+    from frcnn_b200 import resnet_train, train_engine
+    trunks = (train_engine._Vgg16Trunk, resnet_train._ResNetTrunk)
+    for trunk, module, names in ((trunks[0], train_engine, ("RpnTrainer", "RcnnTrainer", "CanvasRpnTrainer", "CanvasRcnnTrainer")),
+                                 (trunks[1], resnet_train, ("ResNetRpnTrainer", "ResNetRcnnTrainer", "CanvasResNetRpnTrainer",
+                                                            "CanvasResNetRcnnTrainer"))):
+        for name in names:
+            mro = getattr(module, name).__mro__
+            assert [t for t in trunks if t in mro] == [trunk], name
+
+
+@pytest.mark.parametrize("kind,name,shape", [
+    ("rpn", "trunk/conv1_1/W", (64, 27)),                      # the right size: it used to be taken as it came
+    ("rpn", "trunk/conv5_3/b", (256,)),
+    ("rpn", "RPN/rpn_cls_score/W", None),
+    ("canvas_rpn", "RPN/rpn_conv_3x3/b", None),
+    ("rcnn", "fc6/W", (4096, 2048 * 49)),
+    ("rcnn", "cls_score/b", None),
+    ("rcnn", "RPN/rpn_conv_3x3/W", (512, 2048, 3, 3)),        # the frozen RPN the step reads
+    ("canvas_rcnn", "fc7/W", (4096 * 4096,)),
+])
+def test_vgg16_parameters_are_checked_first(monkeypatch, kind, name, shape):
+    from frcnn_b200 import train_engine
+    from frcnn_b200._lib import FrcnnError
+
+    def alloc(*a, **k):
+        raise AssertionError("the trainer allocated its buffers before it rejected the parameters")
+    monkeypatch.setattr(train_engine._ConvTrainer, "_init_params", alloc)
+    params = _vgg_params()
+    if shape is None:
+        del params[name]
+    else:
+        params[name] = np.zeros(shape, np.float32)
+    make = dict(rpn=_rpn, rcnn=_rcnn, canvas_rpn=_canvas_rpn, canvas_rcnn=_canvas_rcnn)[kind]
+    with pytest.raises(FrcnnError) as e:
+        make(params)
+    who = dict(rpn="RpnTrainer", rcnn="RcnnTrainer", canvas_rpn="CanvasRpnTrainer", canvas_rcnn="CanvasRcnnTrainer")[kind]
+    assert "%s: parameter %s must have shape" % (who, name) in str(e.value), str(e.value)
+
+
 # ------------------------------------------------------------------------------------------------ the dump
 def _cases():
-    from frcnn_b200.resnet_train import ResNetRpnTrainer
-    vgg = _vgg_params()
+    from frcnn_b200.resnet_train import CanvasResNetRcnnTrainer, CanvasResNetRpnTrainer, ResNetRcnnTrainer, ResNetRpnTrainer
+    vgg, r50 = _vgg_params(), orc.make_resnet_params(50, seed=3)
+    canvas = dict(rpn=_canvas_rpn, rcnn=_canvas_rcnn,
+                  resnet50_rpn=lambda params, n, **kw: CanvasResNetRpnTrainer(params, n, H, W, ANCHORS, n_layers=50, device="cpu",
+                                                                              **kw),
+                  resnet50_rcnn=lambda params, n, **kw: CanvasResNetRcnnTrainer(params, n, H, W, ANCHORS, n_layers=50,
+                                                                                post_n=POST_N, device="cpu", **kw))
     yield "rpn/device", lambda: _rpn(vgg, subsample="device")
     yield "rpn/none", lambda: _rpn(vgg, subsample="none")
     yield "rcnn", lambda: _rcnn(vgg)
-    for n in (1, 3):
-        for mode in ("device", "list", "none"):
-            yield "canvas_rpn/N%d/%s" % (n, mode), lambda n=n, mode=mode: _canvas_rpn(vgg, n, subsample=mode)
-        yield "canvas_rpn/N%d/raw" % n, lambda n=n: _canvas_rpn(vgg, n, raw_input=True)
-        for sample in ("device", "list"):
-            for dropout in ("device", "explicit", None):
-                yield ("canvas_rcnn/N%d/%s/%s" % (n, sample, dropout),
-                       lambda n=n, s=sample, d=dropout: _canvas_rcnn(vgg, n, sample=s, dropout=d))
-        yield "canvas_rcnn/N%d/raw" % n, lambda n=n: _canvas_rcnn(vgg, n, raw_input=True)
-    yield "resnet50", lambda: ResNetRpnTrainer(orc.make_resnet_params(50, seed=3), H, W, ANCHORS, n_layers=50, device="cpu")
+    for trunk, params in (("", vgg), ("resnet50_", r50)):
+        rpn, rcnn = canvas[trunk + "rpn"], canvas[trunk + "rcnn"]
+        for n in (1, 3):
+            for mode in ("device", "list", "none"):
+                yield ("%scanvas_rpn/N%d/%s" % (trunk, n, mode),
+                       lambda rpn=rpn, p=params, n=n, mode=mode: rpn(p, n, subsample=mode))
+            yield "%scanvas_rpn/N%d/raw" % (trunk, n), lambda rpn=rpn, p=params, n=n: rpn(p, n, raw_input=True)
+            for sample in ("device", "list"):
+                for dropout in ("device", "explicit", None):
+                    yield ("%scanvas_rcnn/N%d/%s/%s" % (trunk, n, sample, dropout),
+                           lambda rcnn=rcnn, p=params, n=n, s=sample, d=dropout: rcnn(p, n, sample=s, dropout=d))
+            yield "%scanvas_rcnn/N%d/raw" % (trunk, n), lambda rcnn=rcnn, p=params, n=n: rcnn(p, n, raw_input=True)
+    yield "resnet50", lambda: ResNetRpnTrainer(r50, H, W, ANCHORS, n_layers=50, device="cpu")
+    yield "resnet50/none", lambda: ResNetRpnTrainer(r50, H, W, ANCHORS, n_layers=50, subsample="none", device="cpu")
+    yield "resnet50_rcnn", lambda: ResNetRcnnTrainer(r50, H, W, ANCHORS, n_layers=50, post_n=POST_N, device="cpu")
 
 
 def dump(path):
