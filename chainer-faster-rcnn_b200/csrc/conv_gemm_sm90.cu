@@ -1,6 +1,7 @@
 // conv_gemm_sm90.cu -- implicit-GEMM 3x3 / 1x1 convolution (and plain GEMM) on Hopper tensor cores:
 // TMA -> swizzled shared memory -> wgmma (bf16 operands, fp32 accumulators in registers) -> epilogue with fused
-// bias + ReLU (+ residual, + bf16 hi/lo split, + optional fused 2x2 ceil-mode max-pool) -> global stores.
+// bias + ReLU (+ residual, + bf16 hi/lo split, + optional fused 2x2 ceil-mode max-pool) -> TMA tensor stores (bf16) or
+// global stores (fp32, pooled bf16).
 //
 // Replaces, for the forward path: L.Convolution2D at the reference's models/vgg16.py:39-67 and
 // models/region_proposal_network.py:53-57, L.Linear at models/faster_rcnn.py:33-36, and (fused)
@@ -28,7 +29,10 @@
 // adds and restarted, so the truncation bias of the tensor-core sum grows with acc_chunk, not with K.
 //
 // Epilogue: per 32-channel chunk a warpgroup transposes its 64 x 32 fp32 fragment through shared memory so that a
-// thread owns 16 consecutive channels of one pixel; it then stores 32-byte runs of bf16 hi / lo (or fp32).
+// thread owns 16 consecutive channels of one pixel.  fp32 and fused-pool results are stored from registers; unpooled
+// bf16 hi / lo results are staged in the same shared tile and leave as one TMA tensor store per plane (the map clips what
+// lies outside the output).  The issuing thread only waits for a store to have read the tile before the next chunk
+// reuses it, so the global writes drain behind the next tile's main loop; they are waited for once, before the CTA exits.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -85,8 +89,9 @@ struct ConvParams {
     int n_parts, tiles_per_part, splits, kb_per_split, kb_total, g_row_stride;
     long part_stride;
     // batch: n_img images of one H x W shape, [n_img][H][W][C] (A through a 4-D tensor map {C, W, H, image} when n_img > 1).
-    // Pixel tile mt is tile mt % img_tiles of image mt / img_tiles; each image keeps the one-image plan, and every output
-    // (bf16, pooled bf16, fp32, residual) is addressed in its own image at img_pix (img_opix pooled) pixels per image.
+    // Pixel tile mt is tile mt % img_tiles of image mt / img_tiles; each image keeps the one-image plan, and the fp32 output,
+    // the residual and the pooled bf16 output are addressed in the tile's own image at img_pix (img_opix pooled) pixels per
+    // image; the unpooled bf16 outputs are stored through a 4-D map.
     int n_img, img_tiles;
     FastDiv fd_img_tiles;
     long img_pix, img_opix;
@@ -151,10 +156,20 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b, float& ra, flo
     return u;
 }
 
-// One 16-channel run of one pixel: bias, residual, ReLU, validity, fp32 and bf16 (hi / lo, optionally 2x2-pooled) stores.
+// Position of 16-byte unit j (0..3: channels 8j .. 8j+7 of a 32-channel chunk) of staged pixel `spix` in a warpgroup's
+// bf16 staging plane: 64 B per pixel, in the 64-byte swizzle the output tensor maps use (16-byte unit index XOR bits 7-8
+// of the offset); every plane starts on a 512-byte boundary.  A quarter-warp's eight consecutive pixels hit eight
+// distinct bank groups.
+__device__ __forceinline__ uint32_t stage_off(int spix, int j) {
+    return (uint32_t)(spix * 64 + ((j ^ ((spix >> 1) & 3)) << 4));
+}
+
+// One 16-channel run of one pixel: bias, residual, ReLU, validity, the fp32 store and the bf16 hi / lo split.  Unpooled,
+// the packed hi / lo values are returned in hv / lv for the TMA store (whose tensor map clips pixels outside the image)
+// and the function returns true; with the fused 2x2 pool, one lane per window stores them here.
 // (ext_h, ext_w): the image's extent (H, W without a canvas); pixels outside it are stored as 0.
-__device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16], int part, int img, int h, int w, int n,
-                                             int lane, int m_valid, int ext_h, int ext_w) {
+__device__ __forceinline__ bool epilogue_run(const ConvParams& p, float (&v)[16], int part, int img, int h, int w, int n,
+                                             int lane, int m_valid, int ext_h, int ext_w, uint4 (&hv)[2], uint4 (&lv)[2]) {
     const bool in_img = (h < p.H) && (w < p.W);
     const long ipix = (long)h * p.W + w;
     const long pix = img * p.img_pix + ipix;
@@ -200,52 +215,57 @@ __device__ __forceinline__ void epilogue_run(const ConvParams& p, float (&v)[16]
 #pragma unroll
         for (int j = 0; j < 4; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
     }
-    if (p.y_hi != nullptr && n < p.Cout) {       // CTA-uniform condition
-        bool writer = in_img;
-        long opix = pix;
-        if (p.pool) {
-            // F.MaxPooling2D(2,2) ceil mode fused: the tile is 8 x 16 pixels and a warp holds two consecutive tile rows, so the
-            // 2x2 window is lanes {l, l^1, l^16, l^17}.  Out-of-image pixels were zeroed above and every valid value is >= 0
-            // (ReLU), so the max over the valid part of a partial window is unchanged (Chainer cover_all=True).
-            const int tw_mask = p.TW;
+    if (p.y_hi == nullptr || n >= p.Cout) return false;      // CTA-uniform condition
+    bool writer = true;
+    long opix = 0;
+    if (p.pool) {
+        // F.MaxPooling2D(2,2) ceil mode fused: the tile is 8 x 16 pixels and a warp holds two consecutive tile rows, so the
+        // 2x2 window is lanes {l, l^1, l^16, l^17}.  Out-of-image pixels were zeroed above and every valid value is >= 0
+        // (ReLU), so the max over the valid part of a partial window is unchanged (Chainer cover_all=True).
+        const int tw_mask = p.TW;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                float m = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
-                v[j] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, tw_mask));
-            }
-            writer = in_img && (lane & (1 | tw_mask)) == 0;
-            opix = img * p.img_opix + (long)(h >> 1) * ((p.W + 1) >> 1) + (w >> 1);
+        for (int j = 0; j < 16; ++j) {
+            float m = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
+            v[j] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, tw_mask));
         }
-        if (writer) {
-            uint4 hv[2], lv[2];
+        writer = in_img && (lane & (1 | tw_mask)) == 0;
+        opix = img * p.img_opix + (long)(h >> 1) * ((p.W + 1) >> 1) + (w >> 1);
+    }
+    if (writer) {
 #pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                float ra[8], d0, d1;
-                hv[q].x = pack_bf16x2(v[8 * q + 0], v[8 * q + 1], ra[0], ra[1]);
-                hv[q].y = pack_bf16x2(v[8 * q + 2], v[8 * q + 3], ra[2], ra[3]);
-                hv[q].z = pack_bf16x2(v[8 * q + 4], v[8 * q + 5], ra[4], ra[5]);
-                hv[q].w = pack_bf16x2(v[8 * q + 6], v[8 * q + 7], ra[6], ra[7]);
-                lv[q].x = pack_bf16x2(ra[0], ra[1], d0, d1);
-                lv[q].y = pack_bf16x2(ra[2], ra[3], d0, d1);
-                lv[q].z = pack_bf16x2(ra[4], ra[5], d0, d1);
-                lv[q].w = pack_bf16x2(ra[6], ra[7], d0, d1);
-            }
-            uint4* dh = reinterpret_cast<uint4*>(p.y_hi + opix * p.Cout + n);
-            dh[0] = hv[0];
-            dh[1] = hv[1];
-            if (p.y_lo != nullptr) {
-                uint4* dl = reinterpret_cast<uint4*>(p.y_lo + opix * p.Cout + n);
-                dl[0] = lv[0];
-                dl[1] = lv[1];
-            }
+        for (int q = 0; q < 2; ++q) {
+            float ra[8], d0, d1;
+            hv[q].x = pack_bf16x2(v[8 * q + 0], v[8 * q + 1], ra[0], ra[1]);
+            hv[q].y = pack_bf16x2(v[8 * q + 2], v[8 * q + 3], ra[2], ra[3]);
+            hv[q].z = pack_bf16x2(v[8 * q + 4], v[8 * q + 5], ra[4], ra[5]);
+            hv[q].w = pack_bf16x2(v[8 * q + 6], v[8 * q + 7], ra[6], ra[7]);
+            lv[q].x = pack_bf16x2(ra[0], ra[1], d0, d1);
+            lv[q].y = pack_bf16x2(ra[2], ra[3], d0, d1);
+            lv[q].z = pack_bf16x2(ra[4], ra[5], d0, d1);
+            lv[q].w = pack_bf16x2(ra[6], ra[7], d0, d1);
         }
     }
+    if (!p.pool) return true;
+    // a pooled chunk is 16 pixels per warpgroup, written by a quarter of the threads: direct stores cost less here than
+    // staging them for a TMA store (two more warpgroup barriers per chunk)
+    if (writer) {
+        uint4* dh = reinterpret_cast<uint4*>(p.y_hi + opix * p.Cout + n);
+        dh[0] = hv[0];
+        dh[1] = hv[1];
+        if (p.y_lo != nullptr) {
+            uint4* dl = reinterpret_cast<uint4*>(p.y_lo + opix * p.Cout + n);
+            dl[0] = lv[0];
+            dl[1] = lv[1];
+        }
+    }
+    return false;
 }
 
 template <int BN, int BK, bool X3, bool PROMOTE, int CG>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                 const __grid_constant__ CUtensorMap tm_y_hi, const __grid_constant__ CUtensorMap tm_y_lo,
                  const ConvParams p) {
     using C = Cfg<BN, BK>;
     constexpr int NACC = BN / 2;           // fp32 accumulator registers per thread of an m64nBN fragment
@@ -284,6 +304,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             ptx::prefetch_tensormap(&tm_a_lo);
             ptx::prefetch_tensormap(&tm_b_lo);
         }
+        if (p.y_hi != nullptr && !p.pool) ptx::prefetch_tensormap(&tm_y_hi);
+        if (p.y_lo != nullptr && !p.pool) ptx::prefetch_tensormap(&tm_y_lo);
         for (int i = 0; i < S; ++i) {
             ptx::mbar_init(&full_bar[i], 1);
             ptx::mbar_init(&empty_bar[i], 8 * CG);     // one arrive per MMA warp of every CTA that reads the stage
@@ -369,6 +391,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
         const int er = t & 63, eh = t >> 6;
         const int row = c * kWgRows + er;
         const int row_h = row / p.TW, row_w = row - row_h * p.TW;
+        // unpooled bf16 outputs leave through TMA tensor stores of the warpgroup's 64 pixels, a box of its 64 / TW whole tile
+        // rows (TW = 128: half a row); the 32-channel hi and lo planes of a chunk are staged in the transpose tile (2 x 4 KB)
+        uint8_t* stg = reinterpret_cast<uint8_t*>(scr);
+        const int box_dw = (kWgRows * c) % p.TW, box_dh = (kWgRows * c) / p.TW;
         const int m_valid = p.m_valid ? *p.m_valid : 0x7fffffff;
         const uint32_t a_off = (uint32_t)(c * kWgRows * C::ROW_BYTES);     // this warpgroup's 64 rows of the A tile
         float acc[NACC];
@@ -452,7 +478,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
     #pragma unroll
             for (int ch = 0; ch < BN / 32; ++ch) {
                 if (n0 + ch * 32 >= p.n_cover) break;   // CTA-uniform: nothing is stored past the covered columns
-                ptx::named_bar_sync(1 + c, 128);       // the previous chunk's transpose tile has been read
+                // the previous chunk's TMA stores have read the staging tile (their global writes may still be in flight)
+                if (t == 0) ptx::bulk_wait_group_read0();
+                ptx::named_bar_sync(1 + c, 128);       // ... and every thread has read the previous chunk's transpose tile
     #pragma unroll
                 for (int i = 4 * ch; i < 4 * ch + 4; ++i) {
     #pragma unroll
@@ -484,9 +512,37 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                     v[4 * q + 2] = f.z;
                     v[4 * q + 3] = f.w;
                 }
-                epilogue_run(p, v, part, img, h0 + row_h, w0 + row_w, n0 + ch * 32 + 16 * eh, lane, m_valid, ext_h, ext_w);
+                const int nc = n0 + ch * 32;
+                uint4 hv[2], lv[2];
+                if (epilogue_run(p, v, part, img, h0 + row_h, w0 + row_w, nc + 16 * eh, lane, m_valid, ext_h, ext_w, hv, lv)) {
+                    // CTA-uniform: an unpooled bf16 chunk
+                    ptx::named_bar_sync(1 + c, 128);       // every thread has read its transposed values: the tile is free
+                    const uint32_t sh = ptx::smem_u32(stg);
+                    ptx::st_shared_v4(sh + stage_off(er, 2 * eh), hv[0]);
+                    ptx::st_shared_v4(sh + stage_off(er, 2 * eh + 1), hv[1]);
+                    if (p.y_lo != nullptr) {
+                        ptx::st_shared_v4(sh + 4096 + stage_off(er, 2 * eh), lv[0]);
+                        ptx::st_shared_v4(sh + 4096 + stage_off(er, 2 * eh + 1), lv[1]);
+                    }
+                    ptx::fence_proxy_async_smem();
+                    ptx::named_bar_sync(1 + c, 128);
+                    if (t == 0) {
+                        const int bw = w0 + box_dw, bh = h0 + box_dh;
+                        if (p.n_img > 1) {
+                            ptx::tma_store_4d(&tm_y_hi, stg, nc, bw, bh, img);
+                            if (p.y_lo != nullptr) ptx::tma_store_4d(&tm_y_lo, stg + 4096, nc, bw, bh, img);
+                        } else {
+                            ptx::tma_store_3d(&tm_y_hi, stg, nc, bw, bh);
+                            if (p.y_lo != nullptr) ptx::tma_store_3d(&tm_y_lo, stg + 4096, nc, bw, bh);
+                        }
+                        ptx::bulk_commit_group();
+                    }
+                }
             }
         }
+        // no tile reads another tile's output, so the stores drain behind the following tiles' main loops; they must be
+        // complete before the CTA exits (the staging tile stays valid until they have read it)
+        if (t == 0) ptx::bulk_wait_group0();
     }
     if constexpr (CG == 2) ptx::cluster_sync();      // the peer may still multicast into our stages / arrive on our barriers
 }
@@ -669,7 +725,7 @@ static int launch_conv(const CUtensorMap* tm, ConvParams p, cudaStream_t stream)
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    FRCNN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], p));
+    FRCNN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p));
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }
@@ -855,7 +911,7 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     p.ext_halvings = ext_halvings;
     FRCNN_REQUIRE(!re || (re->hi && !fuse_pool2x2 && Cout % 32 == 0), "frcnn_conv2d_res: residual needs res_hi, Cout %% 32 == 0 and no fused pool");
 
-    CUtensorMap tm[4];
+    CUtensorMap tm[6];      // A hi / lo, B hi / lo, bf16 output hi / lo
     int rc;
     const uint64_t as1 = we ? 16 : 0, as2 = we ? (uint64_t)we->row_pixels * 16 : 0;     // sliding window: one pixel (8 ch) per step
     const uint64_t an = n_img > 1 ? n_img : 0, as3 = (n_img > 1 && we) ? (uint64_t)we->image_elems * 2 : 0;
@@ -868,6 +924,15 @@ static int conv2d_impl(const void* x_hi, const void* x_lo, int H, int W, int Cin
     } else {
         tm[1] = tm[0];
         tm[3] = tm[2];
+    }
+    // unpooled bf16 outputs: one TMA store box per MMA warpgroup and 32-channel chunk (its 64 pixels); the map clips the
+    // rows, columns and channels outside the output.  A batch stores through a 4-D map {C, W, H, image}.
+    tm[4] = tm[0];
+    tm[5] = tm[0];
+    if (y_hi != nullptr && !fuse_pool2x2) {
+        const uint32_t bw = TW < kWgRows ? TW : kWgRows, bh = TW < kWgRows ? kWgRows / TW : 1;
+        if ((rc = make_tmap_3d(&tm[4], y_hi, Cout, W, H, 32, bw, bh, 0, 0, an)) != FRCNN_OK) return rc;
+        if (y_lo != nullptr && (rc = make_tmap_3d(&tm[5], y_lo, Cout, W, H, 32, bw, bh, 0, 0, an)) != FRCNN_OK) return rc;
     }
 
 #define FRCNN_DISPATCH(BN_, BK_, X3_, PROMOTE_, CG_) \

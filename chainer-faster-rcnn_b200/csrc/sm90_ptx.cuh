@@ -111,6 +111,23 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const void* desc, uint64
         "r"(c2), "r"(c3)
         : "memory");
 }
+// TMA tensor stores (shared -> global, bulk async-group completion): the tensor map clips every element outside the
+// tensor.  The writing threads make the staging tile visible to the async proxy (fence_proxy_async_smem) first.
+__device__ __forceinline__ void tma_store_3d(const void* desc, const void* smem, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const void* desc, const void* smem, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the calling thread's committed bulk stores have finished READING shared memory (their global writes may be in flight)
+__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the calling thread's committed bulk stores are complete
+__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- clusters (CTA pairs)
 __device__ __forceinline__ uint32_t cluster_ctarank() {
