@@ -208,6 +208,11 @@ SIGNATURES = {
                              c_void_p, c_void_p]),
     "frcnn_detection_lists_batch": (c_int, [c_int, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p,
                                             c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_voc_eval_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "frcnn_voc_eval_append_batch": (c_int, [c_int, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p, c_long, c_void_p,
+                                            c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "frcnn_voc_eval": (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p,
+                               c_void_p, c_size_t, c_void_p]),
     "frcnn_forward_vgg16_canvas_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "frcnn_forward_vgg16_canvas": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
                                            c_void_p, c_void_p, c_void_p]),

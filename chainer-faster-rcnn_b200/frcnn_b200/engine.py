@@ -1055,6 +1055,32 @@ class Engine(object):
             out += [preprocess.result_detections(res[n], scales[n]) for n in range(len(chunk))]
         return out
 
+    def evaluate_images(self, raw_images, gt_boxes, gt_labels, gt_difficult=None, N=None, canvas=None, nms_thresh=0.3, conf=0.05,
+                        img_infos=None, iou_thresh=0.5, **overrides):
+        """PASCAL VOC average precision of the model on RAW photos (evaluate.VocEvaluator): detect_images' plan and batching,
+        but the detections stay on the device -- per replay one upload of the photos and the evaluator's append, no download;
+        the im_scale of every photo goes up in one copy first, and the result comes back in one download at the end.
+        gt_boxes / gt_labels / gt_difficult: per-photo ground truth in source-photo coordinates (VocEvaluator.evaluate).
+        conf: the detection threshold (0.05, the usual evaluation setting).  Returns the VocEvalResult."""
+        from .evaluate import VocEvaluator
+        raw_images = list(raw_images)
+        if not raw_images:
+            raise FrcnnError("evaluate_images: no images")
+        p = self.raw_canvas_plan(raw_images, N, canvas, nms_thresh, conf, **overrides)
+        M, NC = len(raw_images), self.weights.num_classes
+        ev = VocEvaluator(NC, max_images=M, capacity=M * (NC - 1) * p.post_n,
+                          max_gt=max(1, sum(len(b) for b in gt_boxes)), device=self.weights.device)
+        infos = lambda s: None if img_infos is None else img_infos[s:s + p.N]      # noqa: E731
+        shapes = preprocess.raw_photo_shapes(raw_images)
+        ev.put_scales([v for s in range(0, M, p.N) for v in p.raw_batch_header(shapes[s:s + p.N], infos(s))[1]])
+        for s in range(0, M, p.N):
+            chunk = raw_images[s:s + p.N]
+            p.forward_raw(chunk, infos(s))
+            keep_idx, _, conf_count = p.det
+            n = len(chunk)
+            ev._append(p.prob[:n], p.boxes[:n], keep_idx[:n], conf_count[:n])
+        return ev.evaluate(gt_boxes, gt_labels, gt_difficult, iou_thresh)
+
 
 def _c_structs(weights, H, W, anchors, pre_n, post_n, nms_thresh, min_size, feat_stride):
     """(device anchor table, frcnn_forward_config, frcnn_vgg16_weights) of the whole-graph C entries, filled from a

@@ -968,6 +968,62 @@ def detection_lists_batch(prob, boxes, keep_idx, conf_count, im_scale, out=None)
     return dets, scores, det_count
 
 
+def voc_eval_workspace_bytes(num_classes, capacity, max_images, max_gt):
+    """frcnn_voc_eval_workspace_bytes; raises on bad sizes."""
+    n = _lib.load().frcnn_voc_eval_workspace_bytes(int(num_classes), int(capacity), int(max_images), int(max_gt))
+    if n == 0:
+        raise FrcnnError("voc_eval_workspace_bytes: %s" % _lib.last_error())
+    return int(n)
+
+
+def voc_eval_append_batch(prob, boxes, keep_idx, conf_count, im_scale, image_base, capacity, max_images, ws):
+    """frcnn_voc_eval_append_batch: appends images image_base .. image_base+N-1 of a dataset to the evaluation workspace `ws`
+    (a uint8 CUDA tensor of voc_eval_workspace_bytes, zeroed before the dataset's first append).  prob / boxes / keep_idx /
+    conf_count as detection_lists_batch takes them; im_scale float64 [N] device, this batch's scales."""
+    N, R_cap, NC = prob.shape
+    _need_cuda(im_scale, ws)
+    for t, dt, what in ((prob, torch.float32, "prob"), (boxes, torch.float32, "boxes"), (keep_idx, torch.int32, "keep_idx"),
+                        (conf_count, torch.int32, "conf_count"), (ws, torch.uint8, "ws")):
+        if t.dtype != dt:
+            raise FrcnnError("voc_eval_append_batch: %s must be %s (got %s)" % (what, dt, t.dtype))
+    if im_scale.dtype != torch.float64 or tuple(im_scale.shape) != (N,) or not im_scale.is_contiguous():
+        raise FrcnnError("voc_eval_append_batch: im_scale must be a dense float64 [%d] CUDA tensor" % N)
+    ps = _image_stride(prob, (R_cap, NC), "voc_eval_append_batch prob")
+    bs = _image_stride(boxes, (R_cap, 4 * NC), "voc_eval_append_batch boxes")
+    ks = _image_stride(keep_idx, (NC - 1, R_cap), "voc_eval_append_batch keep_idx")
+    cc = _image_stride(conf_count, (NC - 1,), "voc_eval_append_batch conf_count")
+    check(_lib.load().frcnn_voc_eval_append_batch(N, _p(prob), ps, _p(boxes), bs, _p(keep_idx), ks, _p(conf_count), cc, _p(im_scale),
+                                                  R_cap, NC, int(image_base), int(capacity), int(max_images), _p(ws), ws.numel(),
+                                                  _stream()),
+          "frcnn_voc_eval_append_batch")
+
+
+def voc_eval(num_classes, capacity, max_images, max_gt, gt_offsets, gt_boxes, gt_labels, gt_difficult, iou_thresh, ws, out=None,
+             n_gt=None):
+    """frcnn_voc_eval over the detections appended to `ws`: the GT as a device CSR (gt_offsets int32 [n_images+1], gt_boxes
+    float32 [G,4], gt_labels int32 [G], gt_difficult uint8 [G]; n_gt: the boxes in use, default G -- a caller without GT
+    passes one-row arrays and n_gt = 0, since an empty tensor has no device pointer).  Returns `out`, the float64
+    [3 + 6*(num_classes-1)] device result (status, mAP07, mAP, then per class npos, n_det, tp, fp, ap07, ap)."""
+    _need_cuda(gt_offsets, gt_boxes, gt_labels, gt_difficult, ws)
+    G = int(gt_labels.shape[0])
+    n_gt = G if n_gt is None else int(n_gt)
+    if not 0 <= n_gt <= G:
+        raise FrcnnError("voc_eval: n_gt = %d outside [0, %d]" % (n_gt, G))
+    for t, dt, shape, what in ((gt_boxes, torch.float32, (G, 4), "gt_boxes"), (gt_labels, torch.int32, (G,), "gt_labels"),
+                               (gt_difficult, torch.uint8, (G,), "gt_difficult")):
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise FrcnnError("voc_eval: %s must be a dense %s %s CUDA tensor" % (what, dt, list(shape)))
+    if gt_offsets.dtype != torch.int32 or gt_offsets.dim() != 1 or not gt_offsets.is_contiguous():
+        raise FrcnnError("voc_eval: gt_offsets must be a dense int32 [n_images+1] CUDA tensor")
+    if out is None:
+        out = torch.empty((3 + 6 * (num_classes - 1),), dtype=torch.float64, device=ws.device)
+    check(_lib.load().frcnn_voc_eval(int(num_classes), int(capacity), int(max_images), int(max_gt), int(gt_offsets.shape[0]) - 1,
+                                     _p(gt_offsets), _p(gt_boxes), _p(gt_labels), _p(gt_difficult), n_gt, float(iou_thresh), _p(out),
+                                     _p(ws), ws.numel(), _stream()),
+          "frcnn_voc_eval")
+    return out
+
+
 class ProposalBatchWorkspace(object):
     """Scratch + outputs of frcnn_proposals_batch for N images of one (A,H,W,pre,post) shape: N workspace slices in one
     buffer, rois [N,post_n,4], scores [N,post_n], count [N] int32 and, with debug, dbg_dets [N,k,5], dbg_idx [N,k],

@@ -402,6 +402,45 @@ int frcnn_detection_lists_batch(int N, const float* prob, long prob_stride, cons
                                 const double* im_scale, int R_cap, int num_classes, int* out_dets, float* out_scores,
                                 int* out_det_count, void* stream);
 
+/* PASCAL VOC detection metric on the device (voc_eval.cu): per-class average precision over a dataset of images, from
+ * frcnn_detect_batch's keep lists, appended batch by batch into a workspace and evaluated against the ground truth in one
+ * static launch sequence.  Neither entry synchronises or allocates.
+ *
+ * The workspace (frcnn_voc_eval_workspace_bytes; 0 on bad sizes) holds the dataset's detections, at most `capacity` of them
+ * over all classes, and the evaluation's scratch; it must be zeroed (cudaMemsetAsync) before the first append of a dataset,
+ * and each image index appended once.  Its first bytes are the curves of the last frcnn_voc_eval: int32 tp_cum[capacity] at
+ * byte 0 and fp_cum[capacity] at byte align256(4 * capacity), class c's n_det[c] points in rank order starting at the sum of
+ * n_det over the classes before it.  capacity in [1, 2^30]; num_classes in [2, 65536]. */
+size_t frcnn_voc_eval_workspace_bytes(int num_classes, int capacity, int max_images, int max_gt);
+/* Appends images image_base .. image_base+N-1 of the dataset: for class c = 1 .. num_classes-1 the first conf_count[c-1] entries
+ * r of its keep_idx row, score prob[r][c] and box boxes[r][4c..4c+3] / (float)im_scale[n] as a float32 quotient (the division
+ * of frcnn_detection_lists_batch without its truncation).  Inputs and strides as frcnn_detection_lists_batch; im_scale: device
+ * double [N], this batch's scales.  conf_count is clamped to [0, R_cap]; a keep_idx entry outside [0, R_cap) appends a zero box
+ * of score 0.  A detection counter keeps counting past `capacity`, but nothing is written past it (frcnn_voc_eval then reports
+ * the overflow).  NULL pointers, N outside [1,65535], R_cap < 1, bad sizes, a negative stride or image_base + N > max_images
+ * -> FRCNN_ERR_ARG; a workspace below frcnn_voc_eval_workspace_bytes(num_classes, capacity, max_images, 0) ->
+ * FRCNN_ERR_WORKSPACE. */
+int frcnn_voc_eval_append_batch(int N, const float* prob, long prob_stride, const float* boxes, long boxes_stride,
+                                const int* keep_idx, long keep_idx_stride, const int* conf_count, long conf_count_stride,
+                                const double* im_scale, int R_cap, int num_classes, int image_base, int capacity, int max_images,
+                                void* ws, size_t ws_bytes, void* stream);
+/* The VOC devkit's metric over the appended detections.  Ground truth as a device CSR over n_images images: gt_offsets int32
+ * [n_images+1], image n's boxes rows [gt_offsets[n], gt_offsets[n+1]) of gt_boxes float32 [n_gt][4] (x1, y1, x2, y2 in
+ * source-photo coordinates), gt_labels int32 [n_gt] (1 .. num_classes-1), gt_difficult uint8 [n_gt].  Per class, the
+ * detections in rank order (score descending in the score order of DESIGN §2, then image, then keep-list position) are
+ * matched greedily per image: float64 +1 IoU with every GT box of the class (difficult included), the first maximum; above
+ * iou_thresh (strictly) a difficult GT ignores the detection, an unclaimed GT makes it a TP and is claimed, a claimed GT makes
+ * it an FP; otherwise (a NaN overlap included) it is an FP.  AP: the VOC07 11-point and the area (VOC2010+) variants.
+ * out: device double [3 + 6*(num_classes-1)]: out[0] the status (0, or 1: more than `capacity` detections were appended, and
+ * nothing else is meaningful), out[1] mAP07, out[2] mAP (means over the classes with npos > 0, NaN if none), then per class
+ * c = 1 .. num_classes-1 at out[3 + 6*(c-1)]: npos (non-difficult GT), n_det, tp, fp, ap07, ap (NaN when npos == 0).  Counts
+ * are exact in a double.  The evaluation leaves the appended detections as they are (it may be repeated).  NULL pointers,
+ * bad sizes, n_images outside [0, max_images], n_gt outside [0, max_gt] or a non-finite iou_thresh -> FRCNN_ERR_ARG; a short
+ * workspace -> FRCNN_ERR_WORKSPACE. */
+int frcnn_voc_eval(int num_classes, int capacity, int max_images, int max_gt, int n_images, const int* gt_offsets,
+                   const float* gt_boxes, const int* gt_labels, const unsigned char* gt_difficult, int n_gt, double iou_thresh,
+                   double* out, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * The whole forward path behind one call (forward_graph.cu): FasterRCNN.__call__, inference branch
  * (models/faster_rcnn.py:92-134,175-178) with the VGG16 trunk -- host orchestration only: it carves the caller's
