@@ -11,7 +11,9 @@
 //   frcnn_act_transpose3    forward activation -> three column-shifted transposed planes (the GEMM's B operand)
 //   frcnn_wgrad_reduce      split-K partials -> dW in the reference's OIHW float32 layout (fixed order: deterministic)
 //   frcnn_bias_grad         db[c] = sum over pixels of dY
-//   frcnn_sgd_momentum      MomentumSGD(lr, momentum) + WeightDecay(rate) hook (train_rpn.py:165-167), float32 masters
+//   frcnn_optimizer_update  WeightDecay(rate) hook + MomentumSGD / Adam / AdaGrad / RMSprop on the float32 masters, the
+//                           hyper-parameters read from device memory; frcnn_sgd_momentum(_bf16g) are its MomentumSGD rule
+//                           with them passed by value (train_rpn.py:165-167)
 #include "common.cuh"
 
 namespace frcnn {
@@ -372,16 +374,52 @@ __global__ void __launch_bounds__(256) bias_grad_kernel(const __nv_bfloat16* __r
     }
 }
 
-// ------------------------------------------------------------------------------------------ optimizer
-__global__ void sgd_momentum_kernel(float* __restrict__ w, float* __restrict__ v, const float* __restrict__ g, long n,
-                                    float lr, float momentum, float weight_decay) {
+// ------------------------------------------------------------------------------------------ optimizers
+// Chainer v1's update_one_cpu of each rule after the WeightDecay hook, in float32 with every operation rounded on its own
+// in the order NumPy evaluates it (explicit _rn intrinsics: nothing may be contracted).  h: the rule's hyper layout
+// (include/frcnn_b200.h), h[0] the decay rate.  s0 / s1: the rule's state (s1 only for Adam).
+struct OptHyper { float h[FRCNN_OPT_HYPER_LEN]; };
+
+template <int RULE>
+__device__ __forceinline__ void optimizer_one(float& w, float& s0, float& s1, const float g, const OptHyper& p) {
+    const float* h = p.h;
+    const float gi = __fmaf_rn(h[0], w, g);                  // WeightDecay: g += rate * w
+    if (RULE == FRCNN_OPT_MOMENTUM_SGD) {                    // v = momentum*v - lr*g; w += v
+        s0 = __fsub_rn(__fmul_rn(h[2], s0), __fmul_rn(h[1], gi));
+        w = __fadd_rn(w, s0);
+    } else if (RULE == FRCNN_OPT_ADAM) {                     // m += (1-beta1)*(g-m); v += (1-beta2)*(g*g-v); w -= lr_t*m / (sqrt(v)+eps)
+        s0 = __fadd_rn(s0, __fmul_rn(h[2], __fsub_rn(gi, s0)));
+        s1 = __fadd_rn(s1, __fmul_rn(h[3], __fsub_rn(__fmul_rn(gi, gi), s1)));
+        w = __fsub_rn(w, __fdiv_rn(__fmul_rn(h[1], s0), __fadd_rn(__fsqrt_rn(s1), h[4])));
+    } else if (RULE == FRCNN_OPT_ADAGRAD) {                  // h += g*g; w -= lr*g / (sqrt(h)+eps)
+        s0 = __fadd_rn(s0, __fmul_rn(gi, gi));
+        w = __fsub_rn(w, __fdiv_rn(__fmul_rn(h[1], gi), __fadd_rn(__fsqrt_rn(s0), h[2])));
+    } else {                                                 // ms *= alpha; ms += (1-alpha)*g*g; w -= lr*g / (sqrt(ms)+eps)
+        s0 = __fadd_rn(__fmul_rn(s0, h[2]), __fmul_rn(__fmul_rn(h[3], gi), gi));
+        w = __fsub_rn(w, __fdiv_rn(__fmul_rn(h[1], gi), __fadd_rn(__fsqrt_rn(s0), h[4])));
+    }
+}
+
+__device__ __forceinline__ float grad_value(const float g) { return g; }
+__device__ __forceinline__ float grad_value(const __nv_bfloat16 g) { return __bfloat162float(g); }
+
+// One element per thread.  hyper: the device array frcnn_optimizer_update reads at run time (a captured launch follows
+// whatever was written there before the replay); NULL: the by-value `by_value` of frcnn_sgd_momentum(_bf16g).
+template <int RULE, typename G>
+__global__ void optimizer_kernel(float* __restrict__ w, float* __restrict__ s0, float* __restrict__ s1, const G* __restrict__ g,
+                                 long n, const float* __restrict__ hyper, OptHyper by_value) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    // chainer.optimizer.WeightDecay hook: g += rate * w;  MomentumSGD.update_one: v = momentum*v - lr*g; w += v
-    const float gi = __fmaf_rn(weight_decay, w[i], g[i]);
-    const float vi = __fsub_rn(__fmul_rn(momentum, v[i]), __fmul_rn(lr, gi));
-    v[i] = vi;
-    w[i] = __fadd_rn(w[i], vi);
+    OptHyper p = by_value;
+    if (hyper) {
+#pragma unroll
+        for (int k = 0; k < FRCNN_OPT_HYPER_LEN; ++k) p.h[k] = hyper[k];
+    }
+    float wi = w[i], a = s0[i], b = RULE == FRCNN_OPT_ADAM ? s1[i] : 0.f;
+    optimizer_one<RULE>(wi, a, b, grad_value(g[i]), p);
+    s0[i] = a;
+    if (RULE == FRCNN_OPT_ADAM) s1[i] = b;
+    w[i] = wi;
 }
 
 // bf16 gradient bucket (BASELINE config #5: "bf16, NCCL grad allreduce"): the fp32 gradients of a bucket are rounded to bf16
@@ -398,16 +436,6 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
     } else {
         for (long k = i; k < n; ++k) dst[k] = __float2bfloat16_rn(src[k]);
     }
-}
-
-__global__ void sgd_momentum_bf16g_kernel(float* __restrict__ w, float* __restrict__ v, const __nv_bfloat16* __restrict__ g, long n,
-                                          float lr, float momentum, float weight_decay) {
-    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float gi = __fmaf_rn(weight_decay, w[i], __bfloat162float(g[i]));
-    const float vi = __fsub_rn(__fmul_rn(momentum, v[i]), __fmul_rn(lr, gi));
-    v[i] = vi;
-    w[i] = __fadd_rn(w[i], vi);
 }
 
 // ------------------------------------------------------------------------------------------ dgrad weight packing
@@ -438,6 +466,28 @@ static long padded_pixels(int H, int W, int* wp_out) {
     if (wp_out) *wp_out = Wp;
     const long raw = (long)(H + 2) * Wp;
     return (raw + 63) / 64 * 64;
+}
+
+template <typename G>
+static int optimizer_launch(int rule, float* w, float* s0, float* s1, const G* g, long n, const float* hyper, OptHyper by_value,
+                            cudaStream_t stream) {
+    if (n == 0) return FRCNN_OK;
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    switch (rule) {
+    case FRCNN_OPT_MOMENTUM_SGD:
+        optimizer_kernel<FRCNN_OPT_MOMENTUM_SGD, G><<<blocks, 256, 0, stream>>>(w, s0, s1, g, n, hyper, by_value); break;
+    case FRCNN_OPT_ADAM: optimizer_kernel<FRCNN_OPT_ADAM, G><<<blocks, 256, 0, stream>>>(w, s0, s1, g, n, hyper, by_value); break;
+    case FRCNN_OPT_ADAGRAD: optimizer_kernel<FRCNN_OPT_ADAGRAD, G><<<blocks, 256, 0, stream>>>(w, s0, s1, g, n, hyper, by_value); break;
+    default: optimizer_kernel<FRCNN_OPT_RMSPROP, G><<<blocks, 256, 0, stream>>>(w, s0, s1, g, n, hyper, by_value); break;
+    }
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+static OptHyper sgd_hyper(float lr, float momentum, float weight_decay) {
+    OptHyper p = {};
+    p.h[0] = weight_decay; p.h[1] = lr; p.h[2] = momentum;
+    return p;
 }
 
 static int grad_prepare(const char* fn, const void* g_hi, const void* g_lo, const float* g_f32, int ld_f32, const void* y_hi,
@@ -551,10 +601,8 @@ int frcnn_bias_grad(const void* t_hi, const void* t_lo, int C, long Kp, float sc
 int frcnn_sgd_momentum(float* w, float* v, const float* g, long n, float lr, float momentum, float weight_decay, void* stream) {
     FRCNN_ENTRY();
     FRCNN_REQUIRE(w && v && g && n >= 0, "sgd_momentum: bad arguments");
-    if (n == 0) return FRCNN_OK;
-    sgd_momentum_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, v, g, n, lr, momentum, weight_decay);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return optimizer_launch(FRCNN_OPT_MOMENTUM_SGD, w, v, nullptr, g, n, nullptr, sgd_hyper(lr, momentum, weight_decay),
+                            (cudaStream_t)stream);
 }
 
 int frcnn_cast_f32_bf16(const float* src, void* dst_bf16, long n, void* stream) {
@@ -573,11 +621,23 @@ int frcnn_sgd_momentum_bf16g(float* w, float* v, const void* g_bf16, long n, flo
                              void* stream) {
     FRCNN_ENTRY();
     FRCNN_REQUIRE(w && v && g_bf16 && n >= 0, "sgd_momentum_bf16g: bad arguments");
-    if (n == 0) return FRCNN_OK;
-    sgd_momentum_bf16g_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, v, (const __nv_bfloat16*)g_bf16, n, lr,
-                                                                                              momentum, weight_decay);
-    FRCNN_LAUNCH_OK();
-    return FRCNN_OK;
+    return optimizer_launch(FRCNN_OPT_MOMENTUM_SGD, w, v, nullptr, (const __nv_bfloat16*)g_bf16, n, nullptr,
+                            sgd_hyper(lr, momentum, weight_decay), (cudaStream_t)stream);
+}
+
+int frcnn_optimizer_update(int rule, float* w, float* s0, float* s1, const void* g, int g_bf16, long n, const float* hyper,
+                           void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(rule >= FRCNN_OPT_MOMENTUM_SGD && rule <= FRCNN_OPT_RMSPROP, "optimizer_update: unknown rule %d", rule);
+    FRCNN_REQUIRE(w && s0 && g && hyper, "optimizer_update: null pointer");
+    FRCNN_REQUIRE((s1 != nullptr) == (rule == FRCNN_OPT_ADAM), "optimizer_update: s1 must be %s for rule %d",
+                  rule == FRCNN_OPT_ADAM ? "given" : "NULL", rule);
+    FRCNN_REQUIRE(g_bf16 == 0 || g_bf16 == 1, "optimizer_update: g_bf16 must be 0 or 1 (got %d)", g_bf16);
+    FRCNN_REQUIRE(n >= 0, "optimizer_update: n = %ld < 0", n);
+    const OptHyper unused = {};
+    if (g_bf16)
+        return optimizer_launch(rule, w, s0, s1, (const __nv_bfloat16*)g, n, hyper, unused, (cudaStream_t)stream);
+    return optimizer_launch(rule, w, s0, s1, (const float*)g, n, hyper, unused, (cudaStream_t)stream);
 }
 
 int frcnn_pack_conv_weights_dgrad(const float* w_oihw, int Cout, int Cin, int kh, int kw, int Cout_pad, void* w_hi, void* w_lo,

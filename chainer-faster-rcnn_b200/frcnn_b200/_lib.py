@@ -123,6 +123,7 @@ SIGNATURES = {
     "frcnn_sgd_momentum": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_float, c_float, c_float, c_void_p]),
     "frcnn_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_long, c_void_p]),
     "frcnn_sgd_momentum_bf16g": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_float, c_float, c_float, c_void_p]),
+    "frcnn_optimizer_update": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p]),
     "frcnn_pack_conv_weights_dgrad": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_conv2d_res": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -294,12 +294,13 @@ class ResNetRpnTrainer(_ResNetTrunk, _RpnStep):
     its BN entries are read once and stay constant."""
 
     def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+                 feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None,
+                 optimizer=None):
         if subsample not in SUBSAMPLE_MODES:
             raise FrcnnError("ResNetRpnTrainer: subsample must be one of %s (got %r)" % (SUBSAMPLE_MODES, subsample))
         self.n_layers = n_layers
         self._init_rpn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                       loss_lambda, delta, subsample, seed)
+                       loss_lambda, delta, subsample, seed, optimizer=optimizer)
 
     def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RpnTrainer."""
@@ -318,10 +319,10 @@ class ResNetRcnnTrainer(_ResNetTrunk, _RcnnStep):
 
     def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
+                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None, optimizer=None):
         self.n_layers = n_layers
         self._init_rcnn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout)
+                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout, optimizer=optimizer)
 
     def forward(self, x_chw, gt_boxes, im_info=None, keep_inds=None, masks=None):
         """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[4] (device), as RcnnTrainer."""
@@ -350,10 +351,10 @@ class CanvasResNetRpnTrainer(_ResNetTrunk, _CanvasRpnStep):
 
     def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
                  weight_decay=0.0005, feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256,
-                 device="cuda", process_group=None, raw_input=False):
+                 device="cuda", process_group=None, raw_input=False, optimizer=None):
         self.n_layers = n_layers
         self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                              delta, subsample, seed, max_gt, device, process_group, raw_input)
+                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer)
 
 
 class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
@@ -368,8 +369,8 @@ class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
     def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
                  weight_decay=0.0005, feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7,
                  min_size=16, sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None,
-                 raw_input=False):
+                 raw_input=False, optimizer=None):
         self.n_layers = n_layers
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
-                               process_group, raw_input)
+                               process_group, raw_input, optimizer=optimizer)

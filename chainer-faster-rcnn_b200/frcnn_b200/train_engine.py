@@ -1,7 +1,8 @@
 """The reference's two training steps on the device.
 
 RpnTrainer -- one train_rpn.py step: forward (trunk + RPN) -> AnchorTargetLayer -> rpn_loss -> backward through the RPN
-heads, the RPN 3x3 conv and the 13 trunk convs -> [gradient all-reduce] -> WeightDecay + MomentumSGD.
+heads, the RPN 3x3 conv and the 13 trunk convs -> [gradient all-reduce] -> WeightDecay + the optimizer's rule
+(MomentumSGD by default; Adam, AdaGrad or RMSprop through `optimizer=`, frcnn_b200.optimizers).
 RcnnTrainer -- one train_rcnn.py step: trunk -> frozen test-mode RPN -> ProposalTargetLayer -> RoI pool -> fc6/fc7 with
 dropout -> head losses -> backward through the head, the RoI pooling and the trunk -> the same optimizer.
 CanvasRpnTrainer -- RpnTrainer's step on N images of different sizes per update (an N-slot canvas), one captured graph.
@@ -26,7 +27,7 @@ frcnn_grad_prepare.  Gradients / master weights / momentum are float32 in three 
 import numpy as np
 import torch
 
-from . import ops, preprocess, shard, train_ops
+from . import ops, optimizers, preprocess, shard, train_ops
 from ._lib import FrcnnError
 from .engine import ImageInput, RawPhotoInput, vgg16_schedule
 
@@ -60,10 +61,12 @@ class _ConvTrainer(object):
     first_layer, early_exchange, feat_grad_tag and the _trunk / _pack_image hooks; the step _step_table and repack."""
 
     def _init_common(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                     lead=()):
+                     lead=(), optimizer=None):
         """Checks the trunk's options and every parameter the trainer reads (FrcnnError before anything is allocated), then
         lays out the flat buffers over the trunk's convolutions and the step's convolutions and parameters, and the
-        trunk's constants and activations.  lead: the leading [N] of a canvas trainer's activations."""
+        trunk's constants and activations.  lead: the leading [N] of a canvas trainer's activations.  optimizer: the rule
+        (optimizers.MomentumSGD / Adam / AdaGrad / RMSprop), None for MomentumSGD(lr, momentum)."""
+        optimizer = optimizers.resolve(optimizer, lr, momentum)
         layers, consts = self._trunk_table(H, W, feat_stride)
         step_layers, step_params, frozen = self._step_table(len(anchors))
         layers += step_layers
@@ -72,21 +75,21 @@ class _ConvTrainer(object):
             got = tuple(np.shape(params[name])) if name in params else None
             if got != shape:
                 raise FrcnnError("%s: parameter %s must have shape %s (got %s)" % (type(self).__name__, name, shape, got))
-        self._init_params(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+        self._init_params(params, H, W, anchors, precision, optimizer, weight_decay, feat_stride, device, process_group,
                           layers, entries, lead)
         self.x_in = torch.zeros(tuple(lead) + (3, H, W), dtype=torch.float32, device=self.device)
         self._init_trunk(params, H, W, lead)
 
-    def _init_params(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+    def _init_params(self, params, H, W, anchors, precision, optimizer, weight_decay, feat_stride, device, process_group,
                      layers, entries, lead=()):
-        """Hyper-parameters, the flat float32 master / momentum / gradient buffers over `entries` ([(name, shape)], stored
+        """Hyper-parameters, the flat float32 master / optimizer-state / gradient buffers over `entries` ([(name, shape)], stored
         in the given order with NO padding: adjacent twin heads stay one matrix; fc6/W in the RoI pooling's (h, w, c)
         column order), the activation allocator and the exchange state."""
         if precision not in ops.PRECISIONS:
             raise FrcnnError("precision must be one of %s" % (ops.PRECISIONS,))
         self.x3 = precision == "bf16x3"
         self.precision, self.H, self.W = precision, H, W
-        self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
+        self.optimizer, self.weight_decay = optimizer, weight_decay
         self.feat_stride, self.pg = feat_stride, process_group
         dev = self.device = torch.device(device)
         self.anchors = torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.float64)).to(dev)
@@ -97,7 +100,13 @@ class _ConvTrainer(object):
         offs = [0] + [int(v) for v in np.cumsum(sizes)[:-1]]
         total = int(sum(sizes))
         self.w_flat = torch.zeros((total,), dtype=torch.float32, device=dev)
-        self.v_flat = torch.zeros_like(self.w_flat)
+        # the rule's state ({"v"}, Adam {"m", "v"}, AdaGrad {"h"}, RMSprop {"ms"}) in w_flat's layout; v_flat is
+        # MomentumSGD's velocity (None under another rule); opt_t counts the rule's updates (Adam's t)
+        self.opt_state = {k: torch.zeros_like(self.w_flat) for k in optimizer.states}
+        self.v_flat = self.opt_state["v"] if optimizer.rule == optimizers.MOMENTUM_SGD else None
+        self.opt_t = 0
+        self.hyper = torch.zeros((optimizers.HYPER_LEN,), dtype=torch.float32, device=dev)   # what the update reads
+        self._capturing = False
         self.g_flat = torch.zeros_like(self.w_flat)
         self.index = {}
         for (n, s), o, sz in zip(entries, offs, sizes):
@@ -289,8 +298,74 @@ class _ConvTrainer(object):
         self._bucket_lo = lo
         self._exchange(lo, self.g_flat.numel())
 
+    # ---------------------------------------------------------------- the rule's hyper-parameters and state
+    @property
+    def lr(self):
+        """The rule's learning rate: `optimizer.lr`, Adam's `optimizer.alpha`."""
+        return getattr(self.optimizer, self.optimizer.lr_name)
+
+    @lr.setter
+    def lr(self, value):
+        setattr(self.optimizer, self.optimizer.lr_name, value)
+
+    @property
+    def momentum(self):
+        """MomentumSGD's momentum (AttributeError under another rule)."""
+        if self.optimizer.rule != optimizers.MOMENTUM_SGD:
+            raise AttributeError("%s has no momentum" % type(self.optimizer).__name__)
+        return self.optimizer.momentum
+
+    @momentum.setter
+    def momentum(self, value):
+        if self.optimizer.rule != optimizers.MOMENTUM_SGD:
+            raise AttributeError("%s has no momentum" % type(self.optimizer).__name__)
+        self.optimizer.momentum = value
+
+    def _write_hyper(self):
+        """The next update's hyper-parameters (the current optimizer values, weight_decay and t + 1) into the device array
+        the update reads: one stream-ordered host-to-device copy from pinned memory, which the caching host allocator keeps
+        until the copy has run, so nothing waits.  Raises FrcnnError for a bad value before anything is queued."""
+        self.optimizer.check()
+        vals = torch.from_numpy(self.optimizer.hyper(self.weight_decay, self.opt_t + 1))
+        self.hyper.copy_(vals.pin_memory() if self.hyper.is_cuda else vals, non_blocking=True)
+        self.opt_t += 1
+
+    def _optimizer_update(self, g):
+        s = [self.opt_state[k] for k in self.optimizer.states]
+        train_ops.optimizer_update(self.optimizer.rule, self.w_flat, s[0], s[1] if len(s) > 1 else None, g, self.hyper)
+
+    def optimizer_state(self, to_host=True):
+        """The rule's state under the reference's parameter names: {"rule": name, "t": updates taken, state name: {param:
+        array}} with fp32 arrays in the reference's layouts (fc6/W in (c, h, w) column order, as export_params);
+        to_host=False: device tensors (copies) instead of NumPy arrays."""
+        out = {"rule": type(self.optimizer).__name__, "t": self.opt_t}
+        for k, buf in self.opt_state.items():
+            out[k] = self._host_arrays(buf) if to_host else {n: self._ref_layout(n, self.view(buf, n)).clone() for n in self.index}
+        return out
+
+    def load_optimizer_state(self, state):
+        """Loads what optimizer_state returned (NumPy arrays or tensors) for the same rule and parameters."""
+        who = type(self).__name__
+        if state.get("rule") != type(self.optimizer).__name__:
+            raise FrcnnError("%s.load_optimizer_state: the state is %r's, the trainer runs %s"
+                             % (who, state.get("rule"), type(self.optimizer).__name__))
+        for k in self.opt_state:
+            if k not in state or set(state[k]) != set(self.index):
+                raise FrcnnError("%s.load_optimizer_state: state %r must hold every trained parameter" % (who, k))
+            for n, a in state[k].items():
+                if tuple(a.shape) != self.index[n][2]:
+                    raise FrcnnError("%s.load_optimizer_state: %s/%s has shape %s, needs %s"
+                                     % (who, k, n, tuple(a.shape), self.index[n][2]))
+        for k, buf in self.opt_state.items():
+            for n, a in state[k].items():
+                t = torch.as_tensor(a, dtype=torch.float32)
+                self.view(buf, n).copy_(t.reshape(4096, -1, 49).transpose(1, 2).reshape(4096, -1) if n == "fc6/W" else t)
+        self.opt_t = int(state["t"])
+
     def update(self):
-        """[all-reduce SUM over ranks, like ParallelUpdater's addgrads] + WeightDecay + MomentumSGD, then repack."""
+        """[all-reduce SUM over ranks, like ParallelUpdater's addgrads] + WeightDecay + the optimizer's rule, then repack.
+        The hyper-parameters are written before the update is queued, except inside a capture (_CanvasSteps._step writes
+        them before each replay)."""
         if self._multi():
             hi = self._bucket_lo if self._bucket_lo is not None else self.g_flat.numel()
             self._ev_bwd = torch.cuda.Event(enable_timing=True)
@@ -300,10 +375,9 @@ class _ConvTrainer(object):
             self._ev_comm.record(self.comm_stream)
             torch.cuda.current_stream().wait_event(self._ev_comm)
             self._bucket_lo = None
-        if self.grad_dtype == "bf16" and self._multi():
-            train_ops.sgd_momentum_bf16g(self.w_flat, self.v_flat, self.g_bf16, self.lr, self.momentum, self.weight_decay)
-        else:
-            train_ops.sgd_momentum(self.w_flat, self.v_flat, self.g_flat, self.lr, self.momentum, self.weight_decay)
+        if not self._capturing:
+            self._write_hyper()
+        self._optimizer_update(self.g_bf16 if self.grad_dtype == "bf16" and self._multi() else self.g_flat)
         self.repack()
         self.n_updates += 1
 
@@ -314,9 +388,17 @@ class _ConvTrainer(object):
             return 0.0
         return max(0.0, self._ev_bwd.elapsed_time(self._ev_comm))
 
+    def _ref_layout(self, name, a):
+        """A parameter-shaped view of a flat buffer in the reference's layout: fc6/W's (h, w, c) columns back to (c, h, w)."""
+        return a.reshape(4096, 49, -1).transpose(1, 2).reshape(4096, -1) if name == "fc6/W" else a
+
+    def _host_arrays(self, flat):
+        return {n: self._ref_layout(n, self.view(flat, n)).detach().cpu().numpy().copy() for n in self.index}
+
     def export_params(self):
-        """Trainable parameters as numpy arrays under the reference's names (checkpoint / write-back into the Links)."""
-        return {n: self.weights(n).detach().cpu().numpy().copy() for n in self.index}
+        """Trainable parameters as numpy arrays under the reference's names and layouts (fc6/W in (c, h, w) column order):
+        checkpoint / write-back into the Links."""
+        return self._host_arrays(self.w_flat)
 
 
 class _Vgg16Trunk(object):
@@ -417,8 +499,9 @@ class _RpnStep(_ConvTrainer):
     through the heads and the RPN conv into the trunk's."""
 
     def _init_rpn(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                  loss_lambda, delta, subsample, seed):
-        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group)
+                  loss_lambda, delta, subsample, seed, optimizer=None):
+        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          optimizer=optimizer)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
         self.repack()
@@ -556,9 +639,10 @@ class _RcnnStep(_ConvTrainer):
     fc6/W is kept in the (h, w, c) input order the RoI-pool kernel emits (`export_params` converts back)."""
 
     def _init_rcnn(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                   num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout):
+                   num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout, optimizer=None):
         self.num_classes = num_classes
-        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group)
+        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          optimizer=optimizer)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self.sample, self.dropout = sample, dropout
         self.gen = torch.Generator(device=self.device)
@@ -610,14 +694,6 @@ class _RcnnStep(_ConvTrainer):
     def _heads_b(self, flat):
         o, _, _ = self.index["cls_score/b"]
         return flat[o:o + self.n_heads]
-
-    def export_params(self):
-        """Trainable parameters as numpy arrays in the reference's layouts (fc6/W back to (c, h, w) columns)."""
-        out, C = {}, self.feat_ch
-        for n in self.index:
-            a = self.weights(n).detach().cpu().numpy().copy()
-            out[n] = a.reshape(4096, 49, C).transpose(0, 2, 1).reshape(4096, C * 49) if n == "fc6/W" else a
-        return out
 
     def repack(self):
         self._repack_trunk()
@@ -891,12 +967,17 @@ class _CanvasSteps(object):
             losses = self.step_losses.clone()
             torch.cuda.current_stream().synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                self.run()
+            self._capturing = True                   # the hyper-parameters are written before each replay, not captured
+            try:
+                with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                    self.run()
+            finally:
+                self._capturing = False
             self.n_updates -= 1                      # the capture ran nothing
             self.graph = g
             return losses
         else:
+            self._write_hyper()
             self.graph.replay()
             self.n_updates += 1
         return self.step_losses.clone()
@@ -908,7 +989,7 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
     _MODES = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST, "none": train_ops.SUBSAMPLE_NONE}
 
     def _init_canvas_rpn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                         delta, subsample, seed, max_gt, device, process_group, raw_input):
+                         delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=None):
         """Checks the options, then builds the trunk, the RPN head, the canvas input, the batched anchor targets and the
         subsampling lists; then the first repack."""
         self._canvas_options(N, max_gt)
@@ -916,7 +997,7 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
             raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          lead=(N,))
+                          lead=(N,), optimizer=optimizer)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         dev = self.device
@@ -1005,7 +1086,7 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
 
     def _init_canvas_rcnn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                           delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device, process_group,
-                          raw_input):
+                          raw_input, optimizer=None):
         """Checks the options, then builds the trunk, the canvas input, the frozen RPN and the head, the batched proposals,
         targets, kept lists and masks; then the first repack."""
         who = type(self).__name__
@@ -1018,7 +1099,7 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
             raise FrcnnError("%s: post_n must be in [1, 4096] (got %r)" % (who, post_n))
         self.N, self.max_gt, self.num_classes = N, max_gt, nc = int(N), int(max_gt), num_classes
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          lead=(N,))
+                          lead=(N,), optimizer=optimizer)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self.sample, self.dropout = sample, dropout
@@ -1143,9 +1224,10 @@ class RpnTrainer(_Vgg16Trunk, _RpnStep):
     """Weights, optimizer state and buffers of the RPN-mode training step for one image shape."""
 
     def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
-                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None):
+                 feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, device="cuda", process_group=None,
+                 optimizer=None):
         self._init_rpn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                       loss_lambda, delta, subsample, seed)
+                       loss_lambda, delta, subsample, seed, optimizer=optimizer)
 
 
 class RcnnTrainer(_Vgg16Trunk, _RcnnStep):
@@ -1162,9 +1244,9 @@ class RcnnTrainer(_Vgg16Trunk, _RcnnStep):
 
     def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None):
+                 sample="numpy", seed=0, dropout=True, device="cuda", process_group=None, optimizer=None):
         self._init_rcnn(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout)
+                        num_classes, delta, post_n, pre_n, nms_thresh, min_size, sample, seed, dropout, optimizer=optimizer)
 
 
 class CanvasRpnTrainer(_Vgg16Trunk, _CanvasRpnStep):
@@ -1187,9 +1269,9 @@ class CanvasRpnTrainer(_Vgg16Trunk, _CanvasRpnStep):
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
-                 process_group=None, raw_input=False):
+                 process_group=None, raw_input=False, optimizer=None):
         self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                              delta, subsample, seed, max_gt, device, process_group, raw_input)
+                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer)
 
 
 class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
@@ -1213,7 +1295,8 @@ class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
-                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False):
+                 sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False,
+                 optimizer=None):
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
-                               process_group, raw_input)
+                               process_group, raw_input, optimizer=optimizer)

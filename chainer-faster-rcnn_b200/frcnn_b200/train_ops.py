@@ -6,9 +6,10 @@ stream in, tensors out, no CPU path.
 
 Replaces models/bbox.pyx:16-56, models/anchor_target_layer.py:66-198 and the two loss functions of
 models/region_proposal_network.py:160-204 (all under /root/reference); the second half wraps the conv-backward entry
-points (frcnn_gemm_nt_splitk, frcnn_grad_prepare, frcnn_wgrad_reduce, frcnn_bias_grad, frcnn_sgd_momentum,
-frcnn_pack_conv_weights_dgrad) used by train_engine.py, and those the ResNet trunk adds (frcnn_maxpool3x3s2_backward,
-frcnn_grad_prepare_stride2 and their _batch forms, frcnn_fold_batchnorm, frcnn_wgrad_reduce_scaled) used by resnet_train.py.
+points (frcnn_gemm_nt_splitk, frcnn_grad_prepare, frcnn_wgrad_reduce, frcnn_bias_grad, frcnn_optimizer_update,
+frcnn_sgd_momentum, frcnn_pack_conv_weights_dgrad) used by train_engine.py, and those the ResNet trunk adds
+(frcnn_maxpool3x3s2_backward, frcnn_grad_prepare_stride2 and their _batch forms, frcnn_fold_batchnorm,
+frcnn_wgrad_reduce_scaled) used by resnet_train.py.
 """
 import ctypes
 
@@ -382,6 +383,13 @@ def cast_f32_bf16(src, dst):
 def sgd_momentum_bf16g(w, v, g_bf16, lr, momentum, weight_decay):
     check(_lib.load().frcnn_sgd_momentum_bf16g(_p(w), _p(v), _p(g_bf16), w.numel(), float(lr), float(momentum),
                                                float(weight_decay), _stream()), "frcnn_sgd_momentum_bf16g")
+
+
+def optimizer_update(rule, w, s0, s1, g, hyper):
+    """frcnn_optimizer_update: WeightDecay + the rule (optimizers.RULES) on the flat fp32 masters w with state s0 (s1: Adam's
+    second state, else None), from the fp32 or bf16 gradient g, with the hyper-parameters in the device array `hyper`."""
+    check(_lib.load().frcnn_optimizer_update(int(rule), _p(w), _p(s0), _p(s1), _p(g), int(g.dtype == torch.bfloat16), w.numel(),
+                                             _p(hyper), _stream()), "frcnn_optimizer_update")
 
 
 def pack_conv_weights_dgrad(w, cout_pad=None, x3=True, out=None):

@@ -146,11 +146,14 @@ class FasterRCNN(links.Link):
             key = (tuple(t.shape[2:]), self.version_key())
             if tr is None or self.__dict__.get("_rcnn_trainer_key") != key:
                 # a new image shape (VOC images vary in size) or externally changed parameters: the new trainer starts from
-                # the CURRENT parameters (synced above) and inherits the momentum of the one it replaces
+                # the CURRENT parameters (synced above) and inherits the optimizer, weight decay and optimizer state of the
+                # one it replaces
                 old = tr
                 kw = dict(precision=self.precision, feat_stride=self._feat_stride, num_classes=self._num_classes,
                           delta=float(self._rcnn_delta), post_n=pl._post_nms_top_n, pre_n=pl._pre_nms_top_n,
                           nms_thresh=pl._nms_thresh, min_size=pl._min_size, device=t.device)
+                if old is not None:
+                    kw.update(optimizer=old.optimizer, weight_decay=old.weight_decay)
                 n_layers = getattr(self.trunk, "n_layers", None)
                 if n_layers is not None:                # models.resnet.ResNet trunk: frozen BatchNorm, as engine() runs it
                     tr = ResNetRcnnTrainer(self.param_dict(), int(t.shape[2]), int(t.shape[3]), pl._anchors, n_layers=n_layers,
@@ -158,7 +161,7 @@ class FasterRCNN(links.Link):
                 else:
                     tr = RcnnTrainer(self.param_dict(), int(t.shape[2]), int(t.shape[3]), pl._anchors, **kw)
                 if old is not None and old.index == tr.index:
-                    tr.v_flat.copy_(old.v_flat)
+                    tr.load_optimizer_state(old.optimizer_state(to_host=False))
                 self.__dict__["rcnn_trainer"], self.__dict__["_rcnn_trainer_key"] = tr, key
                 self.__dict__["_rcnn_synced_updates"] = tr.n_updates
             losses = tr.forward(t[0], arrays.to_device(gt_boxes)[0], im_info=(int(hw[0]), int(hw[1])))

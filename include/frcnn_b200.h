@@ -823,7 +823,7 @@ int frcnn_dropout_masks_batch(int N, int rows, int cols, const unsigned long lon
  * MomentumSGD + WeightDecay (train_rpn.py:165-167).  Chainer's per-function backward code is un-vendored; these entry
  * points are its replacement: L.Convolution2D / L.Linear backward-data = frcnn_conv2d on frcnn_pack_conv_weights_dgrad,
  * backward-filter = frcnn_gemm_nt_splitk (+ frcnn_wgrad_reduce, frcnn_bias_grad), F.relu / F.max_pooling_2d / F.dropout
- * backward = frcnn_grad_prepare, F.roi_pooling_2d backward = frcnn_roi_pool_backward, the optimizer = frcnn_sgd_momentum. */
+ * backward = frcnn_grad_prepare, F.roi_pooling_2d backward = frcnn_roi_pool_backward, the optimizer = frcnn_optimizer_update. */
 
 /* Split-K "NT" GEMM on the tensor-core kernel of frcnn_conv2d (same bf16 hi/lo operand planes), the engine of the
  * weight-gradient pass (conv backward-filter as a GEMM over the pixel axis):
@@ -935,7 +935,8 @@ int frcnn_wgrad_reduce(const float* parts, int groups, int splits, int M_parts, 
 int frcnn_bias_grad(const void* t_hi, const void* t_lo, int C, long Kp, float scale, float* db, void* stream);
 
 /* chainer.optimizer.WeightDecay(rate) hook + optimizers.MomentumSGD(lr, momentum) (train_rpn.py:165-167) on float32
- * master weights: g' = g + rate*w; v = momentum*v - lr*g'; w += v. */
+ * master weights: g' = fma(rate, w, g); v = momentum*v - lr*g'; w += v.  frcnn_optimizer_update's MomentumSGD rule with
+ * the hyper-parameters passed by value (the same kernel). */
 int frcnn_sgd_momentum(float* w, float* v, const float* g, long n, float lr, float momentum, float weight_decay, void* stream);
 
 /* bf16 gradient bucket for the multi-GPU step (train_rpn.py:169-174 ParallelUpdater; BASELINE config #5 "bf16, NCCL grad
@@ -944,6 +945,34 @@ int frcnn_sgd_momentum(float* w, float* v, const float* g, long n, float lr, flo
 int frcnn_cast_f32_bf16(const float* src, void* dst_bf16, long n, void* stream);
 int frcnn_sgd_momentum_bf16g(float* w, float* v, const void* g_bf16, long n, float lr, float momentum, float weight_decay,
                              void* stream);
+
+/* The optimizer step of every trainer: chainer.optimizer.WeightDecay(rate) hook + one of Chainer v1's rules, on n float32
+ * master weights w with the rule's float32 state s0 (and s1), each element on its own.  g: n float32 gradients, or
+ * (g_bf16 = 1) the bf16 bucket of the multi-GPU exchange, widened exactly.  hyper: FRCNN_OPT_HYPER_LEN float32 values in
+ * DEVICE memory, read when the kernel runs -- so a launch captured into a CUDA graph uses whatever was written there
+ * before each replay.  The arithmetic is update_one_cpu of Chainer 1.22 in float32, every operation correctly rounded on
+ * its own in the order written (no contraction), after g' = fma(rate, w, g):
+ *   FRCNN_OPT_MOMENTUM_SGD  s0 = v              hyper {rate, lr, momentum}
+ *       v = momentum*v - lr*g';  w = w + v                         (frcnn_sgd_momentum, bit for bit)
+ *   FRCNN_OPT_ADAM          s0 = m, s1 = v      hyper {rate, lr_t, 1-beta1, 1-beta2, eps}
+ *       m = m + (1-beta1)*(g' - m);  v = v + (1-beta2)*(g'*g' - v);  w = w - (lr_t*m) / (sqrt(v) + eps)
+ *       lr_t = alpha * sqrt(1 - beta2^t) / (1 - beta1^t) for update t = 1, 2, ... (Chainer's Adam.lr), in float64 on the
+ *       host and rounded once to float32
+ *   FRCNN_OPT_ADAGRAD       s0 = h              hyper {rate, lr, eps}
+ *       h = h + g'*g';  w = w - (lr*g') / (sqrt(h) + eps)
+ *   FRCNN_OPT_RMSPROP       s0 = ms             hyper {rate, lr, alpha, 1-alpha, eps}
+ *       ms = ms*alpha;  ms = ms + ((1-alpha)*g')*g';  w = w - (lr*g') / (sqrt(ms) + eps)
+ * Constants such as 1-beta1 are computed in float64 and rounded to float32 by the caller, as NumPy rounds a Python float
+ * that meets a float32 array; entries past the rule's list are not read.  s1 must be NULL for the one-state rules.
+ * Memory traffic: 20 bytes per element (Adam 28; 2 fewer with a bf16 gradient).  An unknown rule, a NULL pointer, s1
+ * given or missing against the rule, g_bf16 outside {0, 1} or n < 0 -> FRCNN_ERR_ARG; n = 0 launches nothing. */
+#define FRCNN_OPT_MOMENTUM_SGD 0
+#define FRCNN_OPT_ADAM 1
+#define FRCNN_OPT_ADAGRAD 2
+#define FRCNN_OPT_RMSPROP 3
+#define FRCNN_OPT_HYPER_LEN 5
+int frcnn_optimizer_update(int rule, float* w, float* s0, float* s1, const void* g, int g_bf16, long n, const float* hyper,
+                           void* stream);
 
 /* Weights of the data-gradient convolution: out[t][ci][co] = W[co][ci][kh-1-r][kw-1-s] (t = r*kw+s), bf16 hi/lo, co
  * zero-padded to Cout_pad -- feed to frcnn_conv2d with Cin := Cout_pad, Cout := Cin. */
