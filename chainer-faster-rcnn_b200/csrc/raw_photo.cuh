@@ -69,6 +69,14 @@ __device__ __forceinline__ CubicTap cubic_tap(int o, double inv_scale, int n) {
     return r;
 }
 
+// The taps of the horizontally mirrored source (p[:, ::-1]): the flipped image's column i is the source's column n - 1 - i.
+// The weights and the border flag stay those computed on the flipped image's own columns, so cubic_bgr8 with the mirrored
+// taps equals the resize of the flipped image bit for bit.
+__device__ __forceinline__ void mirror_taps(CubicTap& t, int n) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) t.i[k] = n - 1 - t.i[k];
+}
+
 // The resized, mean-subtracted pixel (y, x) of a dense uint8 (h0, w0, 3) image resized to W columns: out[c], c = B, G, R.
 // Each tap's pixel is float(double(u8) - mean_c), the reference's in-place float32 mean subtraction before its resize.
 // Horizontal pass: ((p0 + p1) + p2) + p3 per source row (0.0f + p0 first on a border column).  Vertical pass: OpenCV sums
@@ -114,6 +122,17 @@ __device__ __forceinline__ RawSlot raw_slot(const unsigned char* arena, long lon
     s.ew = live ? canvas_extent(extents, n, 1, 0, Wc) : 0;
     s.inv_scale = __ldg(inv_scale + n);
     return s;
+}
+
+// The augmentation draw of a training slot whose step seed is `seed` (frcnn_voc_augment_batch): the flip is the top bit of
+// sample_key(seed ^ mix64(3), 0), the index among S scale candidates ((sample_key(seed ^ mix64(3), 1) >> 32) * S) >> 32.
+// Salt 3 sets it apart from the other draws of the same seed: the subsampling's keys (seed, seed ^ BG_SEED_XOR) and the
+// dropout masks (seed ^ mix64(1), seed ^ mix64(2)).
+constexpr unsigned long long AUG_SALT = 3;
+__device__ __forceinline__ void aug_draw(unsigned long long seed, int S, int& flip, int& scale_index) {
+    const unsigned long long s = seed ^ mix64(AUG_SALT);
+    flip = (int)(sample_key(s, 0) >> 63);
+    scale_index = (int)(((sample_key(s, 1) >> 32) * (unsigned long long)S) >> 32);
 }
 
 }  // namespace frcnn

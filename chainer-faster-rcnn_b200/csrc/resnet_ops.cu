@@ -96,6 +96,7 @@ __global__ void im2col_kernel(const float* __restrict__ x, int C, int H, int W, 
 // shared memory, 0 outside the image's extent -- so each input pixel's bilinear is computed once per CTA instead of once
 // per covering output pixel, then writes the tile's [Wo][Kp] rows as 16-byte hi/lo stores, reading every K index through
 // a table of its window offset.  Every output pixel outside conv_out(extent) and every k >= ks*ks*3 is written as 0.
+// kFlip (cubic only): a slot whose flip[n] is nonzero is resized from its mirrored source (mirror_taps).
 struct PreIm2colArgs {
     const unsigned char* arena; long long arena_bytes;
     const long long* src_off; const int* src_hw; const double* inv_scale; const int* extents;
@@ -103,8 +104,9 @@ struct PreIm2colArgs {
     int band, tile, tiles, cols;        // output rows per band, output columns per tile, tiles per band, staged row pitch
     double m0, m1, m2;
     __nv_bfloat16 *hi, *lo;
+    const int* flip;                    // kFlip: device int32 [N]
 };
-template <bool kCubic>
+template <bool kCubic, bool kFlip = false>
 __global__ void __launch_bounds__(256) preprocess_canvas_im2col_kernel(const PreIm2colArgs a) {
     extern __shared__ float smem[];
     const int kmax = a.ks * a.ks * 3;
@@ -116,6 +118,7 @@ __global__ void __launch_bounds__(256) preprocess_canvas_im2col_kernel(const Pre
     const RawSlot s = raw_slot(a.arena, a.arena_bytes, a.src_off, a.src_hw, a.inv_scale, a.extents, n, a.Hc, a.Wc);
     const int oh = conv_out(s.eh, a.ks, a.stride, a.pad), ow = conv_out(s.ew, a.ks, a.stride, a.pad);
     const bool any = ho0 < oh && wo0 < ow;             // CTA-uniform: a tile wholly outside the image only writes zeros
+    const bool mirror = kFlip && __ldg(a.flip + n) != 0;
     if (any) {
         for (int k = threadIdx.x; k < kmax; k += blockDim.x) {
             const int tap = k / 3, c = k - tap * 3;
@@ -127,7 +130,11 @@ __global__ void __launch_bounds__(256) preprocess_canvas_im2col_kernel(const Pre
             const int i = p / cols, j = p - i * cols, y = y0 + i, x = x0 + j;
             float v[3] = {0.0f, 0.0f, 0.0f};
             if (y >= 0 && y < s.eh && x >= 0 && x < s.ew) {
-                if (kCubic)
+                if (kCubic && kFlip) {
+                    CubicTap tx = cubic_tap(x, s.inv_scale, s.w0);
+                    if (mirror) mirror_taps(tx, s.w0);
+                    cubic_bgr8(s.src, s.w0, cubic_tap(y, s.inv_scale, s.h0), tx, x, s.ew, a.m0, a.m1, a.m2, v);
+                } else if (kCubic)
                     cubic_bgr8(s.src, s.w0, cubic_tap(y, s.inv_scale, s.h0), cubic_tap(x, s.inv_scale, s.w0), x, s.ew, a.m0, a.m1,
                                a.m2, v);
                 else
@@ -159,15 +166,47 @@ __global__ void __launch_bounds__(256) preprocess_canvas_im2col_kernel(const Pre
 
 // The VOC dataset's box scaling on the device: gt[n][g] = (f32(box) * f32(im_scale) for the four coordinates, the label
 // unchanged) for g < count[n] (clamped to [0, max_gt]), 0 for the rows after it; gt_counts[n] = that count.  One thread per
-// (slot, row, column).
+// (slot, row, column).  kFlip: a slot whose flip[n] is nonzero first mirrors its boxes in the photo's w0 = src_hw[2n+1]
+// columns, py-faster-rcnn's inclusive flip in float32: x1' = (f32(w0) - x2) - 1, x2' = (f32(w0) - x1) - 1.
+template <bool kFlip>
 __global__ void voc_scale_gt_kernel(const float* __restrict__ scale, const int* __restrict__ count, const float* __restrict__ raw,
-                                    int N, int max_gt, float* __restrict__ gt, int* __restrict__ gt_counts) {
+                                    const int* __restrict__ src_hw, const int* __restrict__ flip, int N, int max_gt,
+                                    float* __restrict__ gt, int* __restrict__ gt_counts) {
     const long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
     if (i >= (long)N * max_gt * 5) return;
     const int n = (int)(i / ((long)max_gt * 5)), g = (int)(i / 5 % max_gt), j = (int)(i % 5);
     const int cnt = min(max(__ldg(count + n), 0), max_gt);
-    gt[i] = g < cnt ? (j < 4 ? __fmul_rn(raw[i], __ldg(scale + n)) : raw[i]) : 0.0f;
+    float v = raw[i];
+    if (kFlip && (j == 0 || j == 2) && __ldg(flip + n) != 0)
+        v = __fsub_rn(__fsub_rn((float)__ldg(src_hw + 2 * n + 1), raw[j == 0 ? i + 2 : i - 2]), 1.0f);
+    gt[i] = g < cnt ? (j < 4 ? __fmul_rn(v, __ldg(scale + n)) : v) : 0.0f;
     if (g == 0 && j == 0) gt_counts[n] = cnt;
+}
+
+// frcnn_voc_augment_batch: one thread per slot.  draw 1 / 2 first writes the slot's aug_draw into choice (2: the flip as 0);
+// then the chosen candidate (index clamped to [0, S-1]) becomes the slot's descriptors.  A slot without a source stays
+// empty: extent and clip bounds 0 x 0, inv_scale, scale and flip 0.
+__global__ void voc_augment_kernel(const unsigned long long* __restrict__ seeds, int N, int S, const int* __restrict__ cand_hw,
+                                   const double* __restrict__ cand_inv, const float* __restrict__ cand_scale,
+                                   const int* __restrict__ src_hw, int draw, int* __restrict__ choice, int* __restrict__ flip,
+                                   int* __restrict__ extents, int* __restrict__ im_info, double* __restrict__ inv_scale,
+                                   float* __restrict__ scale) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    if (draw) {
+        int f, k;
+        aug_draw(__ldg(seeds + n), S, f, k);
+        choice[2 * n] = draw == 1 ? f : 0;
+        choice[2 * n + 1] = k;
+    }
+    const int k = min(max(choice[2 * n + 1], 0), S - 1), c = n * S + k;
+    const bool live = __ldg(src_hw + 2 * n) > 0 && __ldg(src_hw + 2 * n + 1) > 0;
+    const int h = live ? __ldg(cand_hw + 2 * c) : 0, w = live ? __ldg(cand_hw + 2 * c + 1) : 0;
+    extents[2 * n] = im_info[2 * n] = h;
+    extents[2 * n + 1] = im_info[2 * n + 1] = w;
+    inv_scale[n] = live ? __ldg(cand_inv + c) : 0.0;
+    scale[n] = live ? __ldg(cand_scale + c) : 0.0f;
+    flip[n] = live && choice[2 * n] != 0 ? 1 : 0;
 }
 
 // OIHW (Cout, C, ks, ks) fp32 -> [1][Cout][Kp] bf16 hi/lo in the K order of im2col_kernel; scale[o] (optional) multiplies
@@ -352,11 +391,12 @@ int frcnn_pack_image_im2col_batch_ext(const float* x_nchw, int N, int C, int H, 
 
 }  // extern "C"
 
-// the launch behind frcnn_preprocess_bgr8_canvas_im2col (bilinear) and frcnn_preprocess_voc_canvas_im2col (cubic)
+// the launch behind frcnn_preprocess_bgr8_canvas_im2col (bilinear), frcnn_preprocess_voc_canvas_im2col (cubic) and
+// frcnn_preprocess_voc_canvas_im2col_flip (cubic, mirrored where flip[n] is nonzero; flip NULL for the other two)
 static int preprocess_canvas_im2col_launch(const char* fn, bool cubic, const unsigned char* arena, long long arena_bytes,
                                            const long long* src_off, const int* src_hw, const double* inv_scale, const int* extents,
                                            int N, int Hc, int Wc, double mean_b, double mean_g, double mean_r, int ksize, int stride,
-                                           int pad, int K_pad, void* y_hi, void* y_lo, void* stream) {
+                                           int pad, int K_pad, void* y_hi, void* y_lo, void* stream, const int* flip = nullptr) {
     FRCNN_REQUIRE(arena, "%s: arena is NULL", fn);
     FRCNN_REQUIRE(arena_bytes > 0, "%s: arena_bytes must be positive (got %lld)", fn, arena_bytes);
     FRCNN_REQUIRE(src_off, "%s: src_off is NULL", fn);
@@ -382,6 +422,7 @@ static int preprocess_canvas_im2col_launch(const char* fn, bool cubic, const uns
     a.Hc = Hc; a.Wc = Wc; a.ks = ksize; a.stride = stride; a.pad = pad; a.Kp = K_pad; a.Ho = Ho; a.Wo = Wo;
     a.m0 = mean_b; a.m1 = mean_g; a.m2 = mean_r;
     a.hi = (__nv_bfloat16*)y_hi; a.lo = (__nv_bfloat16*)y_lo;
+    a.flip = flip;
     // the tile: up to 8 output rows, then as many output columns as the window fits PRE_IM2COL_SMEM (the K table comes
     // first); PRE_IM2COL_MAX_KSIZE guarantees one output pixel's window fits
     const int px = (int)((PRE_IM2COL_SMEM - (size_t)kmax * 4) / 12);
@@ -398,7 +439,9 @@ static int preprocess_canvas_im2col_launch(const char* fn, bool cubic, const uns
     const long blocks = (long)cdiv(Ho, a.band) * a.tiles;
     FRCNN_REQUIRE(blocks <= 0x7fffffffl, "%s: canvas %dx%d needs too many tiles", fn, Hc, Wc);
     const size_t smem = (size_t)kmax * 4 + (size_t)rows * a.cols * 12;
-    if (cubic)
+    if (flip)
+        preprocess_canvas_im2col_kernel<true, true><<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
+    else if (cubic)
         preprocess_canvas_im2col_kernel<true><<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
     else
         preprocess_canvas_im2col_kernel<false><<<dim3((unsigned)blocks, N), 256, smem, (cudaStream_t)stream>>>(a);
@@ -428,15 +471,62 @@ int frcnn_preprocess_voc_canvas_im2col(const unsigned char* arena, long long are
                                            y_lo, stream);
 }
 
+int frcnn_preprocess_voc_canvas_im2col_flip(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                            const int* src_hw, const double* inv_scale, const int* extents, const int* flip, int N,
+                                            int Hc, int Wc, double mean_b, double mean_g, double mean_r, int ksize, int stride,
+                                            int pad, int K_pad, void* y_hi, void* y_lo, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(flip, "frcnn_preprocess_voc_canvas_im2col_flip: flip is NULL");
+    return preprocess_canvas_im2col_launch("frcnn_preprocess_voc_canvas_im2col_flip", true, arena, arena_bytes, src_off, src_hw,
+                                           inv_scale, extents, N, Hc, Wc, mean_b, mean_g, mean_r, ksize, stride, pad, K_pad, y_hi,
+                                           y_lo, stream, flip);
+}
+
+}  // extern "C"
+
+// the launch behind frcnn_voc_scale_gt_batch (src_hw and flip NULL) and frcnn_voc_flip_scale_gt_batch
+static int voc_scale_gt_launch(const char* fn, const float* scale, const int* count, const float* raw_gt, const int* src_hw,
+                               const int* flip, int N, int max_gt, float* gt, int* gt_counts, void* stream) {
+    FRCNN_REQUIRE(scale && count && raw_gt && gt && gt_counts, "%s: NULL argument", fn);
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && max_gt >= 1 && max_gt <= (1 << 20),
+                  "%s: needs 1 <= N <= 65535 and 1 <= max_gt <= 2^20 (got N=%d max_gt=%d)", fn, N, max_gt);
+    const long total = (long)N * max_gt * 5;
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (flip)
+        voc_scale_gt_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(scale, count, raw_gt, src_hw, flip, N, max_gt, gt, gt_counts);
+    else
+        voc_scale_gt_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(scale, count, raw_gt, src_hw, flip, N, max_gt, gt, gt_counts);
+    FRCNN_LAUNCH_OK();
+    return FRCNN_OK;
+}
+
+extern "C" {
+
 int frcnn_voc_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, int N, int max_gt, float* gt, int* gt_counts,
                              void* stream) {
     FRCNN_ENTRY();
-    FRCNN_REQUIRE(scale && count && raw_gt && gt && gt_counts, "frcnn_voc_scale_gt_batch: NULL argument");
-    FRCNN_REQUIRE(N >= 1 && N <= 65535 && max_gt >= 1 && max_gt <= (1 << 20),
-                  "frcnn_voc_scale_gt_batch: needs 1 <= N <= 65535 and 1 <= max_gt <= 2^20 (got N=%d max_gt=%d)", N, max_gt);
-    const long total = (long)N * max_gt * 5;
-    voc_scale_gt_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(scale, count, raw_gt, N, max_gt, gt,
-                                                                                          gt_counts);
+    return voc_scale_gt_launch("frcnn_voc_scale_gt_batch", scale, count, raw_gt, nullptr, nullptr, N, max_gt, gt, gt_counts, stream);
+}
+
+int frcnn_voc_flip_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, const int* src_hw, const int* flip,
+                                  int N, int max_gt, float* gt, int* gt_counts, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(src_hw && flip, "frcnn_voc_flip_scale_gt_batch: NULL argument");
+    return voc_scale_gt_launch("frcnn_voc_flip_scale_gt_batch", scale, count, raw_gt, src_hw, flip, N, max_gt, gt, gt_counts, stream);
+}
+
+int frcnn_voc_augment_batch(const unsigned long long* seeds, int N, int S, const int* cand_hw, const double* cand_inv,
+                            const float* cand_scale, const int* src_hw, int draw, int* choice, int* flip, int* extents, int* im_info,
+                            double* inv_scale, float* scale, void* stream) {
+    FRCNN_ENTRY();
+    FRCNN_REQUIRE(cand_hw && cand_inv && cand_scale && src_hw && choice && flip && extents && im_info && inv_scale && scale,
+                  "frcnn_voc_augment_batch: NULL argument");
+    FRCNN_REQUIRE(draw >= 0 && draw <= 2, "frcnn_voc_augment_batch: draw must be 0, 1 or 2 (got %d)", draw);
+    FRCNN_REQUIRE(seeds || !draw, "frcnn_voc_augment_batch: a draw needs the seeds");
+    FRCNN_REQUIRE(N >= 1 && N <= 65535 && S >= 1 && S <= 8,
+                  "frcnn_voc_augment_batch: needs 1 <= N <= 65535 and 1 <= S <= 8 (got N=%d S=%d)", N, S);
+    voc_augment_kernel<<<cdiv(N, 128), 128, 0, (cudaStream_t)stream>>>(seeds, N, S, cand_hw, cand_inv, cand_scale, src_hw, draw,
+                                                                       choice, flip, extents, im_info, inv_scale, scale);
     FRCNN_LAUNCH_OK();
     return FRCNN_OK;
 }

@@ -151,6 +151,13 @@ SIGNATURES = {
                                                    c_int, c_double, c_double, c_double, c_int, c_int, c_int, c_int, c_void_p,
                                                    c_void_p, c_void_p]),
     "frcnn_voc_scale_gt_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "frcnn_voc_augment_batch": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frcnn_preprocess_voc_canvas_im2col_flip": (c_int, [c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                        c_int, c_int, c_int, c_double, c_double, c_double, c_int, c_int, c_int, c_int,
+                                                        c_void_p, c_void_p, c_void_p]),
+    "frcnn_voc_flip_scale_gt_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                              c_void_p]),
     "frcnn_roi_overlaps": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "frcnn_roi_targets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "frcnn_bbox_transform": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -604,12 +604,21 @@ class RawPhotoInput(object):
 
     max_gt (a training canvas): the photos are the VOC training dataset's, so the block also carries a ground-truth section
     (preprocess.voc_gt_layout) between the header and the pixels, pixel_means default to preprocess.VOC_MEANS, pack_im2col
-    resizes bicubically as the dataset does (frcnn_preprocess_voc_canvas_im2col) and scale_gt writes the scaled boxes."""
+    resizes bicubically as the dataset does (frcnn_preprocess_voc_canvas_im2col) and scale_gt writes the scaled boxes.
+
+    scales (a training canvas that augments): the training short-side targets.  An augmentation section
+    (preprocess.voc_aug_layout) follows the ground-truth section; augment() selects each slot's flip and scale on the device
+    (frcnn_voc_augment_batch) and pack_im2col / scale_gt apply the flip (the _flip entries)."""
     x_in = None
 
-    def __init__(self, N, Hc, Wc, device, pixel_means=None, arena_bytes=None, max_gt=None):
+    def __init__(self, N, Hc, Wc, device, pixel_means=None, arena_bytes=None, max_gt=None, scales=None):
         self.N, self.H, self.W = int(N), int(Hc), int(Wc)
         self.max_gt = None if max_gt is None else int(max_gt)
+        self.scales = None if scales is None else tuple(int(s) for s in scales)
+        if self.scales is not None and (self.max_gt is None or not 1 <= len(self.scales) <= preprocess.AUG_MAX_SCALES
+                                        or min(self.scales) < 1):
+            raise FrcnnError("raw batch: augmentation needs a training canvas and 1 to %d positive scales (got %r)"
+                             % (preprocess.AUG_MAX_SCALES, scales))
         if pixel_means is None:
             pixel_means = preprocess.PIXEL_MEANS if self.max_gt is None else preprocess.VOC_MEANS
         self.pixel_means = tuple(float(v) for v in np.asarray(pixel_means, dtype=np.float64).reshape(-1)[:3])
@@ -621,6 +630,10 @@ class RawPhotoInput(object):
         if self.max_gt is not None:
             gt_layout, gt_bytes = preprocess.voc_gt_layout(self.N, self.max_gt)
             self.header_bytes += gt_bytes
+        aug_at = self.header_bytes
+        if self.scales is not None:
+            aug_layout, aug_bytes = preprocess.voc_aug_layout(self.N, len(self.scales))
+            self.header_bytes += aug_bytes
         self.block = torch.zeros((self.header_bytes + self.arena_bytes,), dtype=torch.uint8, device=device)
         self.arena = self.block[self.header_bytes:]
         tdt = {np.int32: torch.int32, np.int64: torch.int64, np.float64: torch.float64, np.float32: torch.float32}
@@ -632,28 +645,56 @@ class RawPhotoInput(object):
         if self.max_gt is not None:
             self.gt_fields = tuple(self.block[gt_at + off:gt_at + off + int(np.prod(shape)) * 4].view(tdt[dt]).view(shape)
                                    for off, dt, shape in (gt_layout[k] for k in ("scale", "count", "raw_gt")))
+        self.aug = None
+        if self.scales is not None:
+            self.aug = {k: self.block[aug_at + off:aug_at + off + int(np.prod(shape)) * np.dtype(dt).itemsize].view(tdt[dt]).view(shape)
+                        for k, (off, dt, shape) in aug_layout.items()}
         self._stage = None          # pinned host mirror of the block + the event of its last upload
 
     def header(self, shapes, img_infos=None):
         """preprocess.raw_batch_header for these slots, canvas and arena (raises FrcnnError when something does not fit)."""
         return preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos)
 
-    def upload(self, images, img_infos=None, boxes=None, labels=None):
+    def upload(self, images, img_infos=None, boxes=None, labels=None, flips=None, scale_index=None):
         """A list of photos into the block on the current stream, as CanvasBatchPlan.forward_raw describes; on a training
-        canvas also their boxes (source-photo coordinates) and labels (preprocess.voc_gt_section).  Raises FrcnnError before
-        anything is queued when something does not fit.  Returns (host header, [im_scale])."""
+        canvas also their boxes (source-photo coordinates) and labels (preprocess.voc_gt_section).  On an augmenting canvas
+        also every photo's candidate sizes (preprocess.voc_aug_section) and, when given, the choice: flips [bool] and
+        scale_index [int] per photo (omitted: no flip, index 0; augment(draw != 0) overwrites them).  Raises FrcnnError before
+        anything is queued when something does not fit.  Returns (host header, [im_scale]); on an augmenting canvas
+        [im_scale] holds each photo's tuple of candidate im_scale, and the header's sizes are those of the smallest scale
+        until augment() selects."""
         on_host = all(isinstance(x, np.ndarray) for x in images)
         if not on_host and not all(isinstance(x, torch.Tensor) and x.is_cuda for x in images):
             raise FrcnnError("forward_raw: the images must be all numpy arrays or all CUDA tensors")
         for n, x in enumerate(images):
             if x.dtype != (np.uint8 if on_host else torch.uint8) or len(x.shape) != 3 or x.shape[2] != 3:
                 raise FrcnnError("forward_raw: image %d is not a uint8 (h, w, 3) array" % n)
-        hdr, scales, _ = self.header([x.shape[:2] for x in images], img_infos)
+        shapes = [x.shape[:2] for x in images]
+        aug = None
+        if self.scales is not None:
+            aug, cands = preprocess.voc_aug_section(shapes, self.N, self.H, self.W, self.scales)
+            choice = preprocess.voc_aug_views(aug, self.N, len(self.scales))["choice"]
+            for col, vals, name, top in ((0, flips, "flips", 2), (1, scale_index, "scale_index", len(self.scales))):
+                if vals is None:
+                    continue
+                vals = [int(v) for v in vals]
+                if len(vals) != len(images) or any(not 0 <= v < top for v in vals):
+                    raise FrcnnError("raw training batch: %s needs one value in [0, %d) per photo (got %r for %d photos)"
+                                     % (name, top, vals, len(images)))
+                choice[:len(vals), col] = vals
+        elif flips is not None or scale_index is not None:
+            raise FrcnnError("raw batch: flips and scale_index need an augmenting input (scales=...)")
+        if aug is None:
+            hdr, scales, _ = self.header(shapes, img_infos)
+        else:
+            hdr, scales, _ = preprocess.raw_batch_header(shapes, self.N, self.H, self.W, self.arena_bytes, img_infos,
+                                                         scale=min(self.scales))
         block_hdr = hdr
         if self.max_gt is not None:
             if boxes is None or labels is None:
                 raise FrcnnError("raw training batch: the photos need their boxes and labels")
-            block_hdr = np.concatenate([hdr, preprocess.voc_gt_section(list(boxes), list(labels), scales, self.N, self.max_gt)])
+            block_hdr = np.concatenate([hdr, preprocess.voc_gt_section(list(boxes), list(labels), scales, self.N, self.max_gt)]
+                                       + ([] if aug is None else [aug]))
         cur = torch.cuda.current_stream()
         if self._stage is None:
             self._stage = (ops.PinnedBlock((self.block.numel(),), np.uint8), torch.cuda.Event())
@@ -665,7 +706,14 @@ class RawPhotoInput(object):
             for n, x in enumerate(images):
                 self.arena[int(offs[n]):int(offs[n]) + x.numel()].copy_(x.contiguous().view(-1), non_blocking=True)
         done.record(cur)
-        return hdr, scales
+        return hdr, (scales if aug is None else cands)
+
+    def augment(self, seeds, draw):
+        """frcnn_voc_augment_batch on the block: draw 1 (flip and scale) or 2 (scale only) from seeds (int64 [N]), 0 (the
+        uploaded choice); the chosen candidates become the slots' extents, clip bounds, inv_scale and box scale."""
+        h = self.descriptors
+        ops.voc_augment(seeds if draw else None, self.aug["cand_hw"], self.aug["cand_inv"], self.aug["cand_scale"], h[2],
+                        self.aug["choice"], self.aug["flip"], self.extents, self.im_info, h[3], self.gt_fields[0], draw)
 
     def pack_c8(self, out):
         if self.max_gt is not None:
@@ -673,11 +721,19 @@ class RawPhotoInput(object):
         ops.preprocess_pack_canvas(*self.descriptors, self.H, self.W, self.pixel_means, out=out)
 
     def pack_im2col(self, out, ksize, stride, pad, k_pad):
+        if self.aug is not None:
+            ops.preprocess_voc_im2col_canvas_flip(*self.descriptors, self.aug["flip"], self.H, self.W, self.pixel_means, ksize,
+                                                  stride, pad, k_pad, out=out)
+            return
         pack = ops.preprocess_im2col_canvas if self.max_gt is None else ops.preprocess_voc_im2col_canvas
         pack(*self.descriptors, self.H, self.W, self.pixel_means, ksize, stride, pad, k_pad, out=out)
 
     def scale_gt(self, gt, gt_counts):
-        """A training canvas's boxes times each slot's im_scale, labels and counts into gt [N, max_gt, 5] / gt_counts [N]."""
+        """A training canvas's boxes (mirrored first where the slot flips) times each slot's im_scale, labels and counts into
+        gt [N, max_gt, 5] / gt_counts [N]."""
+        if self.aug is not None:
+            ops.voc_flip_scale_gt(*self.gt_fields, self.descriptors[2], self.aug["flip"], gt, gt_counts)
+            return
         ops.voc_scale_gt(*self.gt_fields, gt, gt_counts)
 
 

@@ -307,6 +307,20 @@ def preprocess_voc_im2col_canvas(arena, src_off, src_hw, inv_scale, extents, Hc,
                               pixel_means, ksize, stride, pad, k_pad, precision, out)
 
 
+def preprocess_voc_im2col_canvas_flip(arena, src_off, src_hw, inv_scale, extents, flip, Hc, Wc, pixel_means, ksize, stride, pad,
+                                      k_pad, precision="bf16x3", out=None):
+    """frcnn_preprocess_voc_canvas_im2col_flip: preprocess_voc_im2col_canvas where a slot whose flip[n] (dense int32 [N] CUDA
+    tensor, read when the kernel runs) is nonzero is resized from its mirrored photo p[:, ::-1]."""
+    N = int(extents.shape[0])
+    _need_cuda(flip)
+    if flip.dtype != torch.int32 or tuple(flip.shape) != (N,) or not flip.is_contiguous():
+        raise FrcnnError("frcnn_preprocess_voc_canvas_im2col_flip: flip must be a dense int32 [%d] CUDA tensor" % N)
+    lib = _lib.load()
+    return _preprocess_im2col(lambda *a: lib.frcnn_preprocess_voc_canvas_im2col_flip(*a[:6], _p(flip), *a[6:]),
+                              "frcnn_preprocess_voc_canvas_im2col_flip", arena, src_off, src_hw, inv_scale, extents, Hc, Wc,
+                              pixel_means, ksize, stride, pad, k_pad, precision, out)
+
+
 def _preprocess_im2col(fn, entry, arena, src_off, src_hw, inv_scale, extents, Hc, Wc, pixel_means, ksize, stride, pad, k_pad, precision,
                        out):
     N = _raw_descriptors(entry, arena, src_off, src_hw, inv_scale, extents)
@@ -337,6 +351,43 @@ def voc_scale_gt(scale, count, raw_gt, gt, gt_counts):
             raise FrcnnError("voc_scale_gt: %s must be a dense %s %s CUDA tensor" % (name, dt, shape))
     check(_lib.load().frcnn_voc_scale_gt_batch(_p(scale), _p(count), _p(raw_gt), N, max_gt, _p(gt), _p(gt_counts), _stream()),
           "frcnn_voc_scale_gt_batch")
+
+
+def voc_flip_scale_gt(scale, count, raw_gt, src_hw, flip, gt, gt_counts):
+    """frcnn_voc_flip_scale_gt_batch: voc_scale_gt where a slot whose flip[n] (int32 [N]) is nonzero first mirrors its boxes
+    in its photo's src_hw[n, 1] columns (x1' = (w0 - x2) - 1, x2' = (w0 - x1) - 1, float32).  Device tensors."""
+    _need_cuda(scale, count, raw_gt, src_hw, flip, gt, gt_counts)
+    N, max_gt = int(gt.shape[0]), int(gt.shape[1])
+    for t, dt, shape, name in ((scale, torch.float32, (N,), "scale"), (count, torch.int32, (N,), "count"),
+                               (raw_gt, torch.float32, (N, max_gt, 5), "raw_gt"), (src_hw, torch.int32, (N, 2), "src_hw"),
+                               (flip, torch.int32, (N,), "flip"), (gt, torch.float32, (N, max_gt, 5), "gt"),
+                               (gt_counts, torch.int32, (N,), "gt_counts")):
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise FrcnnError("voc_flip_scale_gt: %s must be a dense %s %s CUDA tensor" % (name, dt, shape))
+    check(_lib.load().frcnn_voc_flip_scale_gt_batch(_p(scale), _p(count), _p(raw_gt), _p(src_hw), _p(flip), N, max_gt, _p(gt),
+                                                    _p(gt_counts), _stream()), "frcnn_voc_flip_scale_gt_batch")
+
+
+def voc_augment(seeds, cand_hw, cand_inv, cand_scale, src_hw, choice, flip, extents, im_info, inv_scale, scale, draw):
+    """frcnn_voc_augment_batch: draw 1 (flip and scale) or 2 (scale only) writes each slot's draw from seeds (int64 [N], read
+    as uint64) into choice [N, 2]; draw 0 reads choice as staged.  Then each slot's chosen candidate (cand_hw [N, S, 2],
+    cand_inv [N, S], cand_scale [N, S]) becomes its extents / im_info [N, 2], inv_scale [N] and scale [N], and flip [N]
+    its flip bit.  Device tensors; seeds may be None when draw is 0."""
+    _need_cuda(seeds, cand_hw, cand_inv, cand_scale, src_hw, choice, flip, extents, im_info, inv_scale, scale)
+    N, S = int(cand_hw.shape[0]), int(cand_hw.shape[1])
+    for t, dt, shape, name in ((seeds, torch.int64, (N,), "seeds"), (cand_hw, torch.int32, (N, S, 2), "cand_hw"),
+                               (cand_inv, torch.float64, (N, S), "cand_inv"), (cand_scale, torch.float32, (N, S), "cand_scale"),
+                               (src_hw, torch.int32, (N, 2), "src_hw"), (choice, torch.int32, (N, 2), "choice"),
+                               (flip, torch.int32, (N,), "flip"), (extents, torch.int32, (N, 2), "extents"),
+                               (im_info, torch.int32, (N, 2), "im_info"), (inv_scale, torch.float64, (N,), "inv_scale"),
+                               (scale, torch.float32, (N,), "scale")):
+        if t is None and name == "seeds" and not draw:
+            continue
+        if t is None or t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise FrcnnError("voc_augment: %s must be a dense %s %s CUDA tensor" % (name, dt, shape))
+    check(_lib.load().frcnn_voc_augment_batch(_p(seeds), N, S, _p(cand_hw), _p(cand_inv), _p(cand_scale), _p(src_hw), int(draw),
+                                              _p(choice), _p(flip), _p(extents), _p(im_info), _p(inv_scale), _p(scale), _stream()),
+          "frcnn_voc_augment_batch")
 
 
 def conv3x3_c8_batch(x_c8, N, H, W, w_hi, w_lo, bias, relu=True, out=None, extents=None):

@@ -196,6 +196,55 @@ def voc_gt_section(boxes, labels, scales, N, max_gt):
     return sec
 
 
+# ---- augmentation (CanvasRpnTrainer / CanvasRcnnTrainer(augment=...)): a section after the ground-truth section holds
+# each slot's S candidate sizes, from plan_size at every training scale, and its choice (flip, scale index); the first
+# launch of the step (frcnn_voc_augment_batch) draws or reads the choice and writes the chosen candidate into the header.
+AUG_MAX_SCALES = 8
+
+
+def voc_aug_layout(N, S):
+    """({name: (byte offset inside the section, dtype, shape)}, section bytes, a multiple of 256): "cand_inv" float64 [N, S]
+    (1 / im_scale), "cand_hw" int32 [N, S, 2] (the resized H, W), "cand_scale" float32 [N, S] (im_scale), "choice" int32
+    [N, 2] (flip, scale index) and "flip" int32 [N] (the flip the step applies)."""
+    fields = (("cand_inv", np.float64, (N, S)), ("cand_hw", np.int32, (N, S, 2)), ("cand_scale", np.float32, (N, S)),
+              ("choice", np.int32, (N, 2)), ("flip", np.int32, (N,)))
+    layout, off = {}, 0
+    for name, dt, shape in fields:
+        layout[name] = (off, dt, shape)
+        off = ops.round_up(off + int(np.prod(shape)) * np.dtype(dt).itemsize, 16)
+    return layout, ops.round_up(off, 256)
+
+
+def voc_aug_views(sec, N, S):
+    """numpy views of the augmentation arrays inside `sec`, a uint8 array that starts with the section."""
+    layout, _ = voc_aug_layout(N, S)
+    return {k: sec[o:o + int(np.prod(sh)) * np.dtype(dt).itemsize].view(dt).reshape(sh) for k, (o, dt, sh) in layout.items()}
+
+
+def voc_aug_section(shapes, N, Hc, Wc, scales, max_size=1000):
+    """The uint8 augmentation section for photos of source sizes `shapes` ((h0, w0) each, at most N) at the training
+    `scales` (short-side targets): candidate k of photo n is plan_size(h0, w0, scales[k], max_size); the remaining slots
+    and the choice are 0.  Returns (section, [tuple of im_scale per photo]).  Raises FrcnnError when a candidate of a photo
+    does not fit the Hc x Wc canvas."""
+    S = len(scales)
+    sec = np.zeros((voc_aug_layout(N, S)[1],), dtype=np.uint8)
+    v = voc_aug_views(sec, N, S)
+    out = []
+    for n, (h0, w0) in enumerate(shapes):
+        cands = []
+        for k, s in enumerate(scales):
+            im_scale, H, W = plan_size(h0, w0, s, max_size)
+            if not (0 < H <= Hc and 0 < W <= Wc):
+                raise _lib.FrcnnError("raw batch: image %d (%d x %d) at scale %d resizes to %d x %d, which does not fit a %d x %d "
+                                      "canvas" % (n, h0, w0, s, H, W, Hc, Wc))
+            v["cand_hw"][n, k] = (H, W)
+            v["cand_inv"][n, k] = 1.0 / im_scale
+            v["cand_scale"][n, k] = im_scale
+            cands.append(im_scale)
+        out.append(tuple(cands))
+    return sec, out
+
+
 def voc_scale_boxes(boxes, im_scale):
     """The reference's `bbox *= im_scale` on float32 boxes, as NumPy >= 2 computes it: f32(box) * f32(im_scale), float32."""
     return np.asarray(boxes, dtype=np.float32) * np.float32(im_scale)

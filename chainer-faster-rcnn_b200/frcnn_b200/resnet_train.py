@@ -345,16 +345,17 @@ class CanvasResNetRpnTrainer(_ResNetTrunk, _CanvasRpnStep):
 
     subsample "device": slot n of step t draws with seed + t*N + n; "list": put() takes per-image disable lists; "none":
     labels before subsampling.  raw_input=True: put_raw takes raw photos and the VOC transform runs on the device,
-    straight into conv1's 7x7/2 im2col planes.  The step is captured after the first call in a single process and runs
+    straight into conv1's 7x7/2 im2col planes, augmented as CanvasRpnTrainer's augment / scales / flip describe.  The step is captured after the first call in a single process and runs
     eagerly with a process group of more than one rank; the gradient exchange is then one bucket after backward (the
     ResNet trunk names no early-exchange layer)."""
 
     def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
                  weight_decay=0.0005, feat_stride=32, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256,
-                 device="cuda", process_group=None, raw_input=False, optimizer=None):
+                 device="cuda", process_group=None, raw_input=False, optimizer=None, augment=None, scales=(600,), flip=True):
         self.n_layers = n_layers
         self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer)
+                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer,
+                              augment=augment, scales=scales, flip=flip)
 
 
 class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
@@ -369,8 +370,8 @@ class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
     def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
                  weight_decay=0.0005, feat_stride=32, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7,
                  min_size=16, sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None,
-                 raw_input=False, optimizer=None):
+                 raw_input=False, optimizer=None, augment=None, scales=(600,), flip=True):
         self.n_layers = n_layers
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
-                               process_group, raw_input, optimizer=optimizer)
+                               process_group, raw_input, optimizer=optimizer, augment=augment, scales=scales, flip=flip)

@@ -833,6 +833,7 @@ class _CanvasSteps(object):
     the staged ground truth, the launches over the canvas (the _ext convolutions, zero outside each image, and the _batch
     re-layouts) that override _ConvTrainer's, and the capture-then-replay step."""
     raw_input = False           # True: the input is RawPhotoInput's training block (put_raw / step_raw)
+    augment = None              # "device" | "list": the step draws or reads each slot's flip and scale (raw input only)
     level_ext = None            # the ResNet trunk's per-level extents int32 [5, N, 2] (None: the VGG16 trunk's halvings)
 
     def _canvas_options(self, N, max_gt):
@@ -843,10 +844,29 @@ class _CanvasSteps(object):
         if int(max_gt) < 1:
             raise FrcnnError("%s: max_gt must be at least 1" % who)
 
-    def _canvas_init(self, N, Hc, Wc, max_gt, seed, raw_input):
+    def _augment_options(self, raw_input, augment, scales, flip):
+        """Raises FrcnnError for a bad augmentation (before anything is allocated)."""
+        who = type(self).__name__
+        if augment not in (None, "device", "list"):
+            raise FrcnnError("%s: augment must be None, 'device' or 'list' (got %r)" % (who, augment))
+        if augment is None:
+            if tuple(scales) != (600,) or not flip:
+                raise FrcnnError("%s: scales and flip need augment='device' or 'list'" % who)
+            return
+        if not raw_input:
+            raise FrcnnError("%s: augment=%r needs raw_input=True (the float input is augmented by the caller)" % (who, augment))
+        scales = tuple(scales)
+        if not 1 <= len(scales) <= preprocess.AUG_MAX_SCALES or any(int(v) != v or v < 1 for v in scales):
+            raise FrcnnError("%s: scales must be 1 to %d positive integers (got %r)" % (who, preprocess.AUG_MAX_SCALES, scales))
+
+    def _canvas_init(self, N, Hc, Wc, max_gt, seed, raw_input, augment=None, scales=(600,), flip=True):
         dev = self.device
         self.raw_input = bool(raw_input)
-        self.input = RawPhotoInput(N, Hc, Wc, dev, max_gt=max_gt) if self.raw_input else ImageInput(N, Hc, Wc, dev, canvas=True)
+        self.augment, self.flip = augment, bool(flip)
+        self.scales = tuple(int(v) for v in scales)
+        self._candidates = []                   # the staged photos' candidate im_scale (augment)
+        self.input = (RawPhotoInput(N, Hc, Wc, dev, max_gt=max_gt, scales=self.scales if augment else None) if self.raw_input
+                      else ImageInput(N, Hc, Wc, dev, canvas=True))
         self.x_in, self.extents, self.im_info = self.input.x_in, self.input.extents, self.input.im_info
         self.gt = torch.zeros((N, max_gt, 5), dtype=torch.float32, device=dev)
         self.gt_counts = torch.zeros((N,), dtype=torch.int32, device=dev)
@@ -895,7 +915,11 @@ class _CanvasSteps(object):
 
     def _pack_input(self, x_chw=None):
         """The staged slots into x_col; raw photos are resized on the way, and their boxes scaled into gt.  On the ResNet
-        trunk the first launch derives every level's extents from the staged sizes, so a captured step re-derives them."""
+        trunk the first launch derives every level's extents from the staged sizes, so a captured step re-derives them.  An
+        augmenting step first selects each slot's flip and scale (frcnn_voc_augment_batch: drawn from the step's seeds in
+        "device" mode, as put_raw staged them in "list" mode), so every later launch reads the augmented sizes."""
+        if self.augment is not None:
+            self.input.augment(self.seeds, 0 if self.augment == "list" else (1 if self.flip else 2))
         if self.level_ext is not None:
             ops.resnet_level_extents(self.extents, self.H, self.W, out=self.level_ext)
         self.input.pack_im2col(self.x_col, *self.first_layer)
@@ -929,13 +953,49 @@ class _CanvasSteps(object):
             self.gt[n, :g.shape[0]].copy_(g, non_blocking=True)
         self.gt_counts.copy_(torch.from_numpy(counts), non_blocking=True)
 
-    def _stage_raw(self, photos, boxes, labels):
+    def _stage_raw(self, photos, boxes, labels, flips=None, scale_index=None):
         """Photos, boxes and labels into the raw block in one host-to-device copy (RawPhotoInput.upload raises before it if
-        something does not fit); the first launch of the step resizes them and scales the boxes.  Returns [im_scale]."""
+        something does not fit); the first launch of the step resizes them and scales the boxes.  Returns [im_scale] (with
+        augment: each photo's tuple of candidate im_scale).  flips / scale_index: the choice of an augment="list" trainer."""
+        who = type(self).__name__
+        if (flips is not None or scale_index is not None) and self.augment != "list":
+            raise FrcnnError("%s.put_raw: flips and scale_index need augment='list' (the trainer has %r)" % (who, self.augment))
+        if flips is not None and not self.flip and any(flips):
+            raise FrcnnError("%s.put_raw: the trainer was built with flip=False" % who)
         preprocess.raw_photo_shapes(photos)
-        hdr, scales = self.input.upload(photos, boxes=list(boxes), labels=list(labels))
-        self.image_sizes = [tuple(int(v) for v in e) for e in preprocess.raw_header_views(hdr, self.N)["extents"]]
+        hdr, scales = self.input.upload(photos, boxes=list(boxes), labels=list(labels), flips=flips, scale_index=scale_index)
+        if self.augment is None:
+            self.image_sizes = [tuple(int(v) for v in e) for e in preprocess.raw_header_views(hdr, self.N)["extents"]]
+        else:
+            self._candidates = scales
+            self.image_sizes = None
+            if self.augment == "list":
+                k = [0] * len(photos) if scale_index is None else [int(v) for v in scale_index]
+                sizes = [preprocess.plan_size(x.shape[0], x.shape[1], self.scales[k[n]])[1:] for n, x in enumerate(photos)]
+                self.image_sizes = sizes + [(0, 0)] * (self.N - len(photos))
         return scales
+
+    def augmentation(self):
+        """Each slot's (flip, im_scale, (H, W)) in the last step that ran on the photos put_raw staged last, in one download
+        ((False, 0.0, (0, 0)) for an empty slot); it also sets image_sizes, which an augment="device" trainer leaves None
+        after put_raw.  Raises FrcnnError on a trainer built without augment."""
+        if self.augment is None:
+            raise FrcnnError("%s.augmentation: the trainer was built without augment" % type(self).__name__)
+        inp = self.input
+        host = inp.block[:inp.header_bytes].cpu().numpy()
+        views = preprocess.raw_header_views(host, self.N)
+        aug_at = inp.header_bytes - preprocess.voc_aug_layout(self.N, len(self.scales))[1]
+        aug = preprocess.voc_aug_views(host[aug_at:], self.N, len(self.scales))
+        out = []
+        for n in range(self.N):
+            H, W = (int(v) for v in views["extents"][n])
+            if n >= len(self._candidates) or H == 0:
+                out.append((False, 0.0, (0, 0)))
+                continue
+            k = min(max(int(aug["choice"][n, 1]), 0), len(self.scales) - 1)
+            out.append((bool(aug["flip"][n]), self._candidates[n][k], (H, W)))
+        self.image_sizes = [o[2] for o in out]
+        return out
 
     @staticmethod
     def _stage_lists(lists, N, buf, offsets):
@@ -989,17 +1049,19 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
     _MODES = {"device": train_ops.SUBSAMPLE_DEVICE, "list": train_ops.SUBSAMPLE_LIST, "none": train_ops.SUBSAMPLE_NONE}
 
     def _init_canvas_rpn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                         delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=None):
+                         delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=None, augment=None,
+                         scales=(600,), flip=True):
         """Checks the options, then builds the trunk, the RPN head, the canvas input, the batched anchor targets and the
         subsampling lists; then the first repack."""
         self._canvas_options(N, max_gt)
+        self._augment_options(raw_input, augment, scales, flip)
         if subsample not in self._MODES:
             raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           lead=(N,), optimizer=optimizer)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
-        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
         dev = self.device
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rpn_loss_batch
         self.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, max_gt, dev)
@@ -1021,16 +1083,21 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
         if self.subsample == "list":
             self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
 
-    def put_raw(self, photos, boxes, labels, disable_pos=None):
+    def put_raw(self, photos, boxes, labels, disable_pos=None, flips=None, scale_index=None):
         """put() for a trainer built with raw_input=True: up to N raw uint8 (h, w, 3) BGR photos (numpy), their boxes (G_n, 4)
         in source-photo coordinates and labels (G_n,), 1 <= G_n <= max_gt, uploaded in one host-to-device copy.  The step
         applies the VOC training dataset's transform on the device: mean subtraction, the bicubic resize of
         preprocess.plan_size (short side 600, long side at most 1000), boxes times float32 im_scale; the clip bounds are the
-        resized (H_n, W_n).  Raises FrcnnError before anything is queued when something does not fit.  Returns [im_scale]."""
+        resized (H_n, W_n).  Raises FrcnnError before anything is queued when something does not fit.  Returns [im_scale].
+
+        With augment, each photo is first mirrored (p[:, ::-1], boxes flipped in its w0 columns) when its flip is set, and
+        resized at its chosen short side among `scales`; every candidate must fit the canvas.  "device": the step draws both
+        from its seeds; "list": flips [bool] and scale_index [int] per photo (default no flip, index 0).  Returns each
+        photo's tuple of candidate im_scale."""
         self._need_input("put_raw")
         photos = list(photos)
         disable_pos = self._check_disable("put_raw", len(photos), disable_pos)
-        scales = self._stage_raw(photos, boxes, labels)
+        scales = self._stage_raw(photos, boxes, labels, flips, scale_index)
         if self.subsample == "list":
             self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
         return scales
@@ -1057,7 +1124,7 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
         train_ops.anchor_targets_batch(self.anchors, self.A, self.feat_stride, ext, self.im_info, self.gt, self.gt_counts,
                                        self.targets, halvings=k, mode=mode, seeds=self.seeds, disable_pos=self.disable_pos,
                                        disable_offsets=self.disable_offsets)
-        if mode == train_ops.SUBSAMPLE_DEVICE:
+        if mode == train_ops.SUBSAMPLE_DEVICE or self.augment == "device":
             self.seeds.add_(self.N)
         losses = train_ops.rpn_loss_batch(self.head_out, self.head_ld, self.anchors, self.A, self.feat_stride, ext, self.im_info,
                                           self.targets, halvings=k, delta=self.delta, loss_lambda=self.loss_lambda,
@@ -1071,9 +1138,9 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
         self.put(images, gt_boxes, img_infos, disable_pos)
         return self._step()
 
-    def step_raw(self, photos, boxes, labels, disable_pos=None):
+    def step_raw(self, photos, boxes, labels, disable_pos=None, flips=None, scale_index=None):
         """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
-        self.put_raw(photos, boxes, labels, disable_pos)
+        self.put_raw(photos, boxes, labels, disable_pos, flips, scale_index)
         return self._step()
 
 
@@ -1086,11 +1153,12 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
 
     def _init_canvas_rcnn(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                           delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device, process_group,
-                          raw_input, optimizer=None):
+                          raw_input, optimizer=None, augment=None, scales=(600,), flip=True):
         """Checks the options, then builds the trunk, the canvas input, the frozen RPN and the head, the batched proposals,
         targets, kept lists and masks; then the first repack."""
         who = type(self).__name__
         self._canvas_options(N, max_gt)
+        self._augment_options(raw_input, augment, scales, flip)
         if sample not in self._SAMPLE:
             raise FrcnnError("%s: sample must be one of %s" % (who, sorted(self._SAMPLE)))
         if dropout not in self._DROPOUT:
@@ -1100,7 +1168,7 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
         self.N, self.max_gt, self.num_classes = N, max_gt, nc = int(N), int(max_gt), num_classes
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           lead=(N,), optimizer=optimizer)
-        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
         self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
         self.sample, self.dropout = sample, dropout
         dev, fh, fw = self.device, self.fh, self.fw
@@ -1132,13 +1200,14 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
         self._stage(images, gt_boxes, img_infos)
         self._stage_extras(keep_inds, masks)
 
-    def put_raw(self, photos, boxes, labels, keep_inds=None, masks=None):
-        """put() for a trainer built with raw_input=True: raw photos, boxes and labels as CanvasRpnTrainer.put_raw takes
-        them, with put()'s kept lists and masks.  Returns [im_scale]."""
+    def put_raw(self, photos, boxes, labels, keep_inds=None, masks=None, flips=None, scale_index=None):
+        """put() for a trainer built with raw_input=True: raw photos, boxes and labels (and with augment="list" the flips and
+        scale indices) as CanvasRpnTrainer.put_raw takes them, with put()'s kept lists and masks.  Returns [im_scale] (with
+        augment: each photo's candidate im_scale tuple)."""
         self._need_input("put_raw")
         photos = list(photos)
         keep_inds, masks = self._check_extras("put_raw", len(photos), keep_inds, masks)
-        scales = self._stage_raw(photos, boxes, labels)
+        scales = self._stage_raw(photos, boxes, labels, flips, scale_index)
         self._stage_extras(keep_inds, masks)
         return scales
 
@@ -1196,7 +1265,7 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
         if self.dropout == "device":
             for j in range(2):
                 train_ops.dropout_masks_batch(self.seeds, j + 1, self.masks[j])
-        if self.sample == "device" or self.dropout == "device":
+        if self.sample == "device" or self.dropout == "device" or self.augment == "device":
             self.seeds.add_(N)
         self._head_forward()
         losses = train_ops.rcnn_loss_batch(self.head_out, self.ptargets, delta=self.delta, dhead=self.head_grad)
@@ -1214,9 +1283,9 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
         self.put(images, gt_boxes, img_infos, keep_inds, masks)
         return self._step()
 
-    def step_raw(self, photos, boxes, labels, keep_inds=None, masks=None):
+    def step_raw(self, photos, boxes, labels, keep_inds=None, masks=None, flips=None, scale_index=None):
         """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
-        self.put_raw(photos, boxes, labels, keep_inds, masks)
+        self.put_raw(photos, boxes, labels, keep_inds, masks, flips, scale_index)
         return self._step()
 
 
@@ -1265,13 +1334,19 @@ class CanvasRpnTrainer(_Vgg16Trunk, _CanvasRpnStep):
     subsample "device": slot n of step t draws with seed + t*N + n (a device counter advanced inside the step, so a replayed
     graph draws fresh samples): the k-th image of a stream gets the labels RpnTrainer(seed=seed) gives its k-th image.
     "list": put() takes per-image disable lists (positions in the inside-compact order, frcnn_anchor_targets mode 2).
-    "none": labels before subsampling."""
+    "none": labels before subsampling.
+
+    augment (raw_input=True only; None keeps the plain VOC transform): "device" draws each slot's horizontal flip and
+    short side among `scales` on the device from the step's seed (seed + t*N + n, salt 3), so a replayed graph augments
+    afresh; "list" takes them from put_raw(flips=, scale_index=).  flip=False jitters the scale only.  augmentation()
+    downloads what the last step chose."""
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, loss_lambda=1.0, delta=3.0, subsample="device", seed=0, max_gt=256, device="cuda",
-                 process_group=None, raw_input=False, optimizer=None):
+                 process_group=None, raw_input=False, optimizer=None, augment=None, scales=(600,), flip=True):
         self._init_canvas_rpn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
-                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer)
+                              delta, subsample, seed, max_gt, device, process_group, raw_input, optimizer=optimizer,
+                              augment=augment, scales=scales, flip=flip)
 
 
 class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
@@ -1291,12 +1366,13 @@ class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
     advanced inside the step); "list": put() takes per-image kept lists (RcnnTrainer's keep_inds, at most 128 distinct rows).
     dropout "device": masks drawn by frcnn_dropout_masks_batch from the same per-slot seeds (salt 1: fc6, 2: fc7); "explicit":
     put() takes per-image (fc6, fc7) uint8 [post_n, 4096] masks; None: no dropout.  `masks` [2, N, post_n, 4096] holds the
-    masks the last step used."""
+    masks the last step used.  augment / scales / flip: as CanvasRpnTrainer's; the draw shares the step's seed advance with
+    the sampling and the dropout."""
 
     def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
                  feat_stride=16, num_classes=21, delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16,
                  sample="device", dropout="device", seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False,
-                 optimizer=None):
+                 optimizer=None, augment=None, scales=(600,), flip=True):
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
-                               process_group, raw_input, optimizer=optimizer)
+                               process_group, raw_input, optimizer=optimizer, augment=augment, scales=scales, flip=flip)

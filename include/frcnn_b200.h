@@ -630,6 +630,45 @@ int frcnn_preprocess_voc_canvas_im2col(const unsigned char* arena, long long are
  * coordinates and the labels.  NULL pointers, N outside [1, 65535] or max_gt outside [1, 2^20] -> FRCNN_ERR_ARG. */
 int frcnn_voc_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, int N, int max_gt, float* gt, int* gt_counts,
                              void* stream);
+/* Training-time augmentation on raw photos (py-faster-rcnn's TRAIN.USE_FLIPPED and TRAIN.SCALES), drawn per slot on the
+ * device so that a captured step augments afresh on every replay.  The host computes S candidates per slot (1 <= S <= 8,
+ * frcnn_b200.preprocess.voc_aug_candidates, from plan_size at every scale): cand_hw int32 [N][S][2] the resized (H, W),
+ * cand_inv float64 [N][S] 1.0 / im_scale, cand_scale float32 [N][S] im_scale rounded to float32.  The device only selects
+ * among them.
+ *
+ * frcnn_voc_augment_batch: one thread per slot, the first launch of an augmenting step.
+ *   draw 1: choice[n] (int32 [N][2]: flip, scale index) <- the draw of seeds[n] (uint64 [N]), with s = seeds[n] ^ mix64(3):
+ *             flip  = sample_key(s, 0) >> 63
+ *             index = ((sample_key(s, 1) >> 32) * S) >> 32
+ *           mix64 is the splitmix64 finaliser and sample_key(seed, i) = (mix64(seed ^ i * 0xD6E8FEB86659FD93) &
+ *           0xFFFFFFFF00000000) | i, the hash and key of the device subsampling (frcnn_anchor_targets_batch mode 1) and the
+ *           dropout masks (salts 1 and 2).
+ *   draw 2: the same draw with the flip written as 0 (scale jitter only).
+ *   draw 0: choice is read as the host wrote it (seeds may be NULL).
+ * Then, in every mode, with k = clamp(choice[n][1], 0, S - 1): extents[n] and im_info[n] (int32 [N][2], the raw header's
+ * FRCNN_RAW_EXTENTS / FRCNN_RAW_IM_INFO) <- cand_hw[n][k], inv_scale[n] (FRCNN_RAW_INV_SCALE) <- cand_inv[n][k], scale[n] (the
+ * ground-truth section's float32 im_scale) <- cand_scale[n][k] and flip[n] (int32 [N]) <- (choice[n][0] != 0).  A slot whose
+ * src_hw[n] (int32 [N][2]) is not positive stays empty: extents and im_info 0 x 0, inv_scale, scale and flip 0.  NULL
+ * pointers (seeds only when draw != 0), draw outside 0..2, N outside [1, 65535] or S outside [1, 8] -> FRCNN_ERR_ARG. */
+int frcnn_voc_augment_batch(const unsigned long long* seeds, int N, int S, const int* cand_hw, const double* cand_inv,
+                            const float* cand_scale, const int* src_hw, int draw, int* choice, int* flip, int* extents, int* im_info,
+                            double* inv_scale, float* scale, void* stream);
+/* frcnn_preprocess_voc_canvas_im2col with a per-slot horizontal flip: flip (device int32 [N]) nonzero resizes slot n from its
+ * mirrored photo p[:, ::-1], bit for bit cubic_resize(mean_subtract(p)[:, ::-1]) -- each horizontal tap's column i is read as
+ * w0 - 1 - i, and the weights, the border rule and the summation order are those of the mirrored image's own columns.  A
+ * slot whose flip is 0 equals frcnn_preprocess_voc_canvas_im2col bit for bit.  Every other argument and error as
+ * frcnn_preprocess_voc_canvas_im2col; a NULL flip -> FRCNN_ERR_ARG. */
+int frcnn_preprocess_voc_canvas_im2col_flip(const unsigned char* arena, long long arena_bytes, const long long* src_off,
+                                            const int* src_hw, const double* inv_scale, const int* extents, const int* flip, int N,
+                                            int Hc, int Wc, double mean_b, double mean_g, double mean_r, int ksize, int stride,
+                                            int pad, int K_pad, void* y_hi, void* y_lo, void* stream);
+/* frcnn_voc_scale_gt_batch with a per-slot horizontal flip: where flip[n] (device int32 [N]) is nonzero, the rows g < c of
+ * slot n are first mirrored in its photo's w0 = src_hw[2n+1] columns (py-faster-rcnn's inclusive-pixel flip, float32):
+ * x1' = (f32(w0) - x2) - 1, x2' = (f32(w0) - x1) - 1, y1 and y2 unchanged; then every coordinate times f32(im_scale).  The
+ * same kernel as frcnn_voc_scale_gt_batch (counts clamped, rows past the count zeroed).  NULL pointers, N outside
+ * [1, 65535] or max_gt outside [1, 2^20] -> FRCNN_ERR_ARG. */
+int frcnn_voc_flip_scale_gt_batch(const float* scale, const int* count, const float* raw_gt, const int* src_hw, const int* flip,
+                                  int N, int max_gt, float* gt, int* gt_counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * RPN training targets and losses (SURVEY.md 8f rank 1, the train_rpn.py step).  Box arithmetic is
