@@ -33,6 +33,11 @@ cls_score | bbox_pred -> losses -> backward through the head, the RoI pooling an
 MomentumSGD.  The head, its losses and backward are RcnnTrainer's step (_RcnnStep) with feat_ch = 2048; the trunk
 (_ResNetTrunk) is ResNetRpnTrainer's, launch for launch.  Trainable: every trunk convolution's W, trunk/conv1/b, fc6, fc7,
 cls_score and bbox_pred; the RPN is packed once and gets no gradient, the BN entries stay constant.
+
+ResNetJointTrainer / CanvasResNetJointTrainer -- JointTrainer's and CanvasJointTrainer's approximate joint training step
+(train_engine._JointStep) on the same trunk: the RPN and the head trained together, the feature map's two gradients joined in
+the epilogue of the RPN conv's data gradient, then every bottleneck; export_params() adds the BN constants, so it is a
+whole detector.
 """
 import numpy as np
 import torch
@@ -40,7 +45,7 @@ import torch
 from . import ops, train_ops
 from ._lib import FrcnnError
 from .resnet_engine import BN_EPS, CONV1_KPAD, RESNET_BLOCKS, block_list, fold_batchnorm
-from .train_engine import _CanvasRcnnStep, _CanvasRpnStep, _RcnnStep, _RpnStep
+from .train_engine import _CanvasJointStep, _CanvasRcnnStep, _CanvasRpnStep, _JointStep, _RcnnStep, _RpnStep
 
 SUBSAMPLE_MODES = ("device", "numpy", "none")
 BN_FIELDS = ("gamma", "beta", "avg_mean", "avg_var")
@@ -375,3 +380,53 @@ class CanvasResNetRcnnTrainer(_ResNetTrunk, _CanvasRcnnStep):
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
                                process_group, raw_input, optimizer=optimizer, augment=augment, scales=scales, flip=flip)
+
+
+def _export_detector(self):
+    """export_params() with the frozen BatchNorm constants: a whole detector, which ResNetEngine loads as it stands."""
+    return dict(self.bn_params, **_JointStep.export_params(self))
+
+
+class ResNetJointTrainer(_ResNetTrunk, _JointStep):
+    """JointTrainer's approximate joint training step with the ResNet trunk for one image shape: one trunk forward, the
+    trained RPN (2048 -> 512 3x3, twin heads) once, rpn_loss and ProposalLayer from its output, the head on res5's RoIs and
+    loss_rcnn; backward of their sum, the feature map's two gradients joined in the epilogue of the RPN conv's data
+    gradient, through every bottleneck.  The surface is JointTrainer's (forward(x, gt, im_info, disable_pos, keep_inds,
+    masks) -> float32[8], backward(debug), update, step, export_params), with folded_params(); the arguments are
+    ResNetRpnTrainer's and ResNetRcnnTrainer's, rpn_delta and rcnn_delta being their deltas.  The BN entries stay constant;
+    export_params() holds every parameter of the detector: the trunk's, the RPN's, the head's and the BN constants."""
+    export_params = _export_detector
+
+    def __init__(self, params, H, W, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=32, loss_lambda=1.0, rpn_delta=3.0, subsample="device", num_classes=21, rcnn_delta=1.0,
+                 post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16, sample="numpy", seed=0, dropout=True, device="cuda",
+                 process_group=None, optimizer=None):
+        self.n_layers = n_layers
+        self._init_joint(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                         loss_lambda, rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size,
+                         sample, seed, dropout, optimizer=optimizer)
+
+    def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None, keep_inds=None, masks=None):
+        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA.  Returns losses float32[8] (device), as JointTrainer."""
+        self._check_input(x_chw, gt_boxes)
+        return super(ResNetJointTrainer, self).forward(x_chw, gt_boxes, im_info, disable_pos, keep_inds, masks)
+
+
+class CanvasResNetJointTrainer(_ResNetTrunk, _CanvasJointStep):
+    """CanvasJointTrainer's step with the ResNet trunk: N images of different sizes per update, per-slot losses [N, 8], one
+    set of weights with ResNetJointTrainer's parameters, frozen BatchNorm and folded_params().  The trunk runs as in
+    CanvasResNetRpnTrainer, the RPN half as there and the head half as in CanvasResNetRcnnTrainer; draws, pins, raw input
+    and augmentation are CanvasJointTrainer's.  A multi-rank run stays eager with one exchange bucket after backward.
+    export_params() is ResNetJointTrainer's."""
+    export_params = _export_detector
+
+    def __init__(self, params, N, Hc, Wc, anchors, n_layers=101, precision="bf16x3", lr=0.001, momentum=0.9,
+                 weight_decay=0.0005, feat_stride=32, loss_lambda=1.0, rpn_delta=3.0, subsample="device", num_classes=21,
+                 rcnn_delta=1.0, post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16, sample="device", dropout="device",
+                 seed=0, max_gt=256, device="cuda", process_group=None, raw_input=False, optimizer=None, augment=None,
+                 scales=(600,), flip=True):
+        self.n_layers = n_layers
+        self._init_canvas_joint(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                                rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size, sample,
+                                dropout, seed, max_gt, device, process_group, raw_input, optimizer=optimizer, augment=augment,
+                                scales=scales, flip=flip)

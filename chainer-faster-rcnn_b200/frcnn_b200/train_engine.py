@@ -7,10 +7,16 @@ RcnnTrainer -- one train_rcnn.py step: trunk -> frozen test-mode RPN -> Proposal
 dropout -> head losses -> backward through the head, the RoI pooling and the trunk -> the same optimizer.
 CanvasRpnTrainer -- RpnTrainer's step on N images of different sizes per update (an N-slot canvas), one captured graph.
 CanvasRcnnTrainer -- RcnnTrainer's step on such a canvas, with device-side RoI sampling and dropout masks.
+JointTrainer -- approximate joint training (py-faster-rcnn's end2end): one trunk forward, the trained RPN once, rpn_loss and
+ProposalLayer from its output, RcnnTrainer's head and loss_rcnn; one backward of rpn_loss + loss_rcnn, the feature map's two
+gradients joined in the epilogue of the RPN conv's data gradient; one update of every parameter.
+CanvasJointTrainer -- JointTrainer's step on a canvas, one captured graph.
 
 Every trainer, here and in resnet_train, is one trunk (_Vgg16Trunk, _ResNetTrunk: layers, forward, backward from the
-feature map's gradient, repacking) and one step (_RpnStep, _RcnnStep, or on a canvas _CanvasRpnStep, _CanvasRcnnStep), both
-launching through _ConvTrainer's launch layer over one image, which _CanvasSteps overrides for a canvas.
+feature map's gradient, repacking) and one step (_RpnStep, _RcnnStep, _JointStep, or on a canvas _CanvasRpnStep,
+_CanvasRcnnStep, _CanvasJointStep), all launching through _ConvTrainer's launch layer over one image, which _CanvasSteps
+overrides for a canvas.  _JointStep runs the RPN and RCNN steps' own halves (forward after the trunk, backward down to the
+feature map's gradient).
 
 Mirrors /root/reference train_rpn.py:144-179 with `model.rpn_train = True`: FasterRCNN.__call__ takes the RPN training
 branch (models/faster_rcnn.py:114-116 -> models/region_proposal_network.py:117-156), the optimizer is
@@ -496,14 +502,23 @@ class _Vgg16Trunk(object):
 
 class _RpnStep(_ConvTrainer):
     """The RPN step over any trunk: the RPN 3x3 conv and its twin heads, AnchorTargetLayer, rpn_loss and the backward
-    through the heads and the RPN conv into the trunk's."""
+    through the heads and the RPN conv into the trunk's.
+
+    The names the RCNN step also uses for its own head -- the twin heads' `packed` key, head_ld, n_heads, head_out,
+    head_grad, delta and targets -- live on `_rpn`: the trainer itself, or in _JointStep, which holds both steps, an
+    _RpnNames beside the RCNN step's."""
+    heads_key = "heads"         # the twin heads' entry in `packed`
+
+    @property
+    def _rpn(self):
+        return self
 
     def _init_rpn(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                   loss_lambda, delta, subsample, seed, optimizer=None):
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           optimizer=optimizer)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
-        self.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
+        self._rpn.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
         self.repack()
 
     def _step_table(self, A):
@@ -515,27 +530,32 @@ class _RpnStep(_ConvTrainer):
 
     def _init_rpn_head(self, loss_lambda, delta, subsample, seed):
         """The RPN step's loss settings, its 3x3 conv (the last layer) at the feature map and the twin heads' output."""
-        self.loss_lambda, self.delta, self.subsample, self.seed = loss_lambda, delta, subsample, seed
-        self.n_heads = 6 * self.A
-        self.head_ld = ops.round_up(self.n_heads, 32)
+        r = self._rpn
+        self.loss_lambda, self.subsample, self.seed = loss_lambda, subsample, seed
+        r.delta = delta
+        r.n_heads = 6 * self.A
+        r.head_ld = ops.round_up(r.n_heads, 32)
         R = self.rpn_layer = self.layers[-1]
         R["H"], R["W"], R["pool"], R["halvings"] = self.fh, self.fw, False, self.halvings
         R["y"] = self._act(self.fh, self.fw, 512)
-        self.head_out = torch.empty((self._slots * self.fh * self.fw, self.head_ld), dtype=torch.float32, device=self.device)
+        r.head_out = torch.empty((self._slots * self.fh * self.fw, r.head_ld), dtype=torch.float32, device=self.device)
 
-    def _heads_w(self, flat):
+    def _rpn_heads_w(self, flat):
         o, _, _ = self.index["RPN/rpn_cls_score/W"]
-        return flat[o:o + self.n_heads * 512].view(self.n_heads, 512)
+        return flat[o:o + self._rpn.n_heads * 512].view(self._rpn.n_heads, 512)
 
-    def _heads_b(self, flat):
+    def _rpn_heads_b(self, flat):
         o, _, _ = self.index["RPN/rpn_cls_score/b"]
-        return flat[o:o + self.n_heads]
+        return flat[o:o + self._rpn.n_heads]
 
     def repack(self):
         self._repack_trunk()
-        R = self.rpn_layer
+        self._repack_rpn()
+
+    def _repack_rpn(self):
+        R, r = self.rpn_layer, self._rpn
         self._repack(R["name"], self.weights(R["name"] + "/W"), self.weights(R["name"] + "/b"), 512, cin_pad=R["cin"])
-        self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
+        self._repack(r.heads_key, self._rpn_heads_w(self.w_flat), self._rpn_heads_b(self.w_flat), r.head_ld)
 
     # ---------------------------------------------------------------- forward
     def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
@@ -543,9 +563,18 @@ class _RpnStep(_ConvTrainer):
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss.  (The reference also runs the ProposalLayer here,
         region_proposal_network.py:122-124; its output does not enter the RPN loss and is skipped.)"""
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
-        R = self.rpn_layer
-        self._rpn_forward(self._forward_trunk(x_chw), self.packed[R["name"]], self.packed["heads"], R["y"], self.head_ld,
-                          self.head_out)
+        self._rpn_trained_forward(self._forward_trunk(x_chw))
+        self.last_losses = self._rpn_losses(gt_boxes, im_h, im_w, disable_pos)
+        return self.last_losses
+
+    def _rpn_trained_forward(self, feat):
+        """The trained RPN (its `packed` planes) on the feature map: rpn_layer's y and the twin heads' _rpn.head_out."""
+        R, r = self.rpn_layer, self._rpn
+        self._rpn_forward(feat, self.packed[R["name"]], self.packed[r.heads_key], R["y"], r.head_ld, r.head_out)
+
+    def _rpn_losses(self, gt_boxes, im_h, im_w, disable_pos):
+        """AnchorTargetLayer and rpn_loss on _rpn.head_out; sets _rpn.head_grad.  Returns losses float32[4] (device)."""
+        r = self._rpn
         if disable_pos is None and self.subsample == "numpy":
             disable_pos = self._numpy_subsample(gt_boxes, im_h, im_w)
         if disable_pos is not None:
@@ -556,11 +585,10 @@ class _RpnStep(_ConvTrainer):
         else:
             mode, kw = train_ops.SUBSAMPLE_NONE, {}
         train_ops.anchor_targets(self.anchors, self.A, self.fh, self.fw, self.feat_stride, gt_boxes, im_h, im_w, mode=mode,
-                                 work=self.targets, **kw)
-        losses, self.head_grad, _ = train_ops.rpn_loss(self.head_out, None, self.anchors, self.A, self.fh, self.fw,
-                                                       self.feat_stride, im_h, im_w, self.targets, delta=self.delta,
-                                                       loss_lambda=self.loss_lambda, layout="nhwc", ld=self.head_ld)
-        self.last_losses = losses
+                                 work=r.targets, **kw)
+        losses, r.head_grad, _ = train_ops.rpn_loss(r.head_out, None, self.anchors, self.A, self.fh, self.fw,
+                                                    self.feat_stride, im_h, im_w, r.targets, delta=r.delta,
+                                                    loss_lambda=self.loss_lambda, layout="nhwc", ld=r.head_ld)
         return losses
 
     def _numpy_subsample(self, gt_boxes, im_h, im_w):
@@ -568,7 +596,7 @@ class _RpnStep(_ConvTrainer):
         and np.random.choice draws from NumPy's global RNG in the reference's order (a seeded run reproduces the reference's
         labels bit for bit); returns the positions to disable in the inside-compact numbering (int32 CUDA tensor)."""
         w = train_ops.anchor_targets(self.anchors, self.A, self.fh, self.fw, self.feat_stride, gt_boxes, im_h, im_w,
-                                     mode=train_ops.SUBSAMPLE_NONE, work=self.targets)
+                                     mode=train_ops.SUBSAMPLE_NONE, work=self._rpn.targets)
         n_inside = int(w.counts[0].item())
         labels = w.labels_full[w.inds_inside[:n_inside].long()].cpu().numpy()
         num_fg = int(train_ops.RPN_FG_FRACTION * train_ops.RPN_BATCHSIZE)
@@ -590,8 +618,14 @@ class _RpnStep(_ConvTrainer):
         debug: a dict that receives, per layer name, float32 (C,H,W) copies ([N,C,H,W] on a canvas) of the incoming
         gradient ("g_in"), the masked / routed gradient ("dy") and the data gradient the layer passes on ("g_out") -- the
         buffers themselves are reused from layer to layer.  The trunk's entries are those of its _backward_trunk."""
+        self._backward_trunk(self._backward_rpn(debug), debug)
+
+    def _backward_rpn(self, debug=None, res=None, tag=None):
+        """The twin heads' and the RPN 3x3 conv's (feat_ch -> 512, its own bias) gradients; returns the RPN conv's data
+        gradient, the gradient of the feature map, in the _gact of `tag` (default the trunk's feat_grad_tag).  res: a
+        gradient of the feature map from elsewhere (ops.Act, another buffer), added in the data gradient's epilogue
+        (frcnn_conv2d_res)."""
         g = self._backward_heads(debug)
-        # ---- the RPN 3x3 conv (feat_ch -> 512, its own bias), then the trunk from the gradient of the feature map
         R, fh, fw, C = self.rpn_layer, self.fh, self.fw, self.feat_ch
         dy = self._gact(fh, fw, 512)
         dyT = self._tbuf(1, 512, fh, fw)
@@ -602,28 +636,33 @@ class _RpnStep(_ConvTrainer):
         self._prep(fh, fw, C, g=self.feat, tbuf=xT)
         self._wgrad(dyT, xT, 512, C, 9, self.grads(R["name"] + "/W"))
         train_ops.bias_grad(dyT, 512, self.grads(R["name"] + "/b"))
-        g = self._gact(fh, fw, C, tag=self.feat_grad_tag)
-        self._conv(dy, self.packed[R["name"]][2], self.zero_bias, 3, False, self.halvings, out=g)
+        g = self._gact(fh, fw, C, tag=self.feat_grad_tag if tag is None else tag)
+        if res is None:
+            self._conv(dy, self.packed[R["name"]][2], self.zero_bias, 3, False, self.halvings, out=g)
+        else:
+            self._res_conv(dy, self.packed[R["name"]][2], self.zero_bias, 3, False, res, self.halvings, g)
         if debug is not None:
             debug[R["name"]]["g_out"] = self._chw(g)
-        self._backward_trunk(g, debug)
+        return g
 
     def _backward_heads(self, debug=None):
-        """The twin 1x1 heads' weight / bias gradients; returns the gradient w.r.t. the RPN 3x3 conv's post-ReLU output."""
-        fh, fw, ld = self.fh, self.fw, self.head_ld
+        """The twin 1x1 heads' weight / bias gradients; returns the gradient w.r.t. the RPN 3x3 conv's post-ReLU output.
+        debug: the entry under _rpn.heads_key."""
+        r = self._rpn
+        fh, fw, ld = self.fh, self.fw, r.head_ld
         R = self.rpn_layer
         # ---- twin 1x1 heads: dY = head_grad [fh*fw, ld] fp32 (columns >= 6A are zero)
         dyh = self._gact(fh, fw, ld)
         dyhT = self._tbuf(1, ld, fh, fw)
-        self._prep(fh, fw, ld, g_f32=self.head_grad, out=dyh, tbuf=dyhT)
+        self._prep(fh, fw, ld, g_f32=r.head_grad, out=dyh, tbuf=dyhT)
         midT = self._tbuf(3, 512, fh, fw)
         self._prep(fh, fw, 512, g=R["y"], tbuf=midT)
-        self._wgrad(dyhT, midT, ld, 512, 1, self._heads_w(self.g_flat), m_out=self.n_heads)
-        train_ops.bias_grad(dyhT, self.n_heads, self._heads_b(self.g_flat))
+        self._wgrad(dyhT, midT, ld, 512, 1, self._rpn_heads_w(self.g_flat), m_out=r.n_heads)
+        train_ops.bias_grad(dyhT, r.n_heads, self._rpn_heads_b(self.g_flat))
         g = self._gact(fh, fw, 512, tag=1)
-        self._conv(dyh, self.packed["heads"][2], self.zero_bias, 1, False, self.halvings, out=g)
+        self._conv(dyh, self.packed[r.heads_key][2], self.zero_bias, 1, False, self.halvings, out=g)
         if debug is not None:
-            debug["heads"] = dict(dy=self._chw(dyh), g_out=self._chw(g))
+            debug[r.heads_key] = dict(dy=self._chw(dyh), g_out=self._chw(g))
         return g
 
     def step(self, x_chw, gt_boxes, im_info=None, disable_pos=None):
@@ -643,13 +682,18 @@ class _RcnnStep(_ConvTrainer):
         self.num_classes = num_classes
         self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           optimizer=optimizer)
-        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+        self._frozen_rpn(params)
+        self._init_rcnn_head(delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_rcnn_draws(sample, seed, dropout)
+        self.repack()
+
+    def _init_rcnn_draws(self, sample, seed, dropout):
+        """One image's sampling and dropout settings, the masks' generator and the proposal workspace."""
         self.sample, self.dropout = sample, dropout
         self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
         self.prop = ops.ProposalWorkspace(self.A, self.fh, self.fw, self.pre_n, self.post_n, self.device)
         self.roi_ws = None
-        self.repack()
 
     def _step_table(self, A):
         """The step's convolutions (none) and parameters in flat-buffer order (cls_score | bbox_pred adjacent: one
@@ -659,16 +703,13 @@ class _RcnnStep(_ConvTrainer):
         frozen_rpn = _entries(*_RpnStep._step_table(self, A)[:2])
         return [], fc + [(n + "/W", (co, 4096)) for n, co in heads] + [(n + "/b", (co,)) for n, co in heads], frozen_rpn
 
-    def _init_rcnn_head(self, params, delta, post_n, pre_n, nms_thresh, min_size):
-        """The RCNN step's frozen RPN with its outputs, and the head's settings and activations."""
+    def _init_rcnn_head(self, delta, post_n, pre_n, nms_thresh, min_size):
+        """The head's settings and activations."""
         self.delta = delta
         self.post_n, self.pre_n, self.nms_thresh, self.min_size = post_n, pre_n, nms_thresh, min_size
         self.n_heads = 5 * self.num_classes
         self.head_ld = ops.round_up(self.n_heads, 32)
         dev, rows, C = self.device, self._slots * self.fh * self.fw, self.feat_ch
-        self._frozen_rpn(params)
-        self.rpn_mid = self._act(self.fh, self.fw, 512)
-        self.rpn_out = torch.empty((rows, self.rpn_ld), dtype=torch.float32, device=dev)
         self.pool5 = self._act(1, post_n, 49 * C)
         self.fc6 = self._act(1, post_n, 4096)
         self.fc7 = self._act(1, post_n, 4096)
@@ -677,7 +718,7 @@ class _RcnnStep(_ConvTrainer):
 
     def _frozen_rpn(self, params):
         """The RPN's 3x3 and twin-head weights as (planes, bias), packed once (forward only: the RCNN step gives them no
-        gradient)."""
+        gradient), and their outputs."""
         T = lambda k: torch.from_numpy(np.ascontiguousarray(params[k], dtype=np.float32)).to(self.device)     # noqa: E731
         self.rpn3 = (ops.pack_conv_weights(T("RPN/rpn_conv_3x3/W"), cin_pad=self.feat_ch, precision=self.precision),
                      ops.pad_bias(T("RPN/rpn_conv_3x3/b"), 512))
@@ -685,6 +726,8 @@ class _RcnnStep(_ConvTrainer):
         bh = torch.cat([T("RPN/rpn_cls_score/b"), T("RPN/rpn_bbox_pred/b")], dim=0)
         self.rpn_ld = ops.round_up(6 * self.A, 32)
         self.rpn_heads = (ops.pack_conv_weights(wh, precision=self.precision), ops.pad_bias(bh, self.rpn_ld))
+        self.rpn_mid = self._act(self.fh, self.fw, 512)
+        self.rpn_out = torch.empty((self._slots * self.fh * self.fw, self.rpn_ld), dtype=torch.float32, device=self.device)
 
     # ---------------------------------------------------------------- parameters
     def _heads_w(self, flat):
@@ -697,6 +740,9 @@ class _RcnnStep(_ConvTrainer):
 
     def repack(self):
         self._repack_trunk()
+        self._repack_rcnn()
+
+    def _repack_rcnn(self):
         for n in ("fc6", "fc7"):
             self._repack(n, self.weights(n + "/W"), self.weights(n + "/b"), 4096)
         self._repack("heads", self._heads_w(self.w_flat), self._heads_b(self.w_flat), self.head_ld)
@@ -721,8 +767,14 @@ class _RcnnStep(_ConvTrainer):
         im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
         feat = self._forward_trunk(x_chw)
         self._rpn_forward(feat, self.rpn3, self.rpn_heads, self.rpn_mid, self.rpn_ld, self.rpn_out)
-        ops.proposals(self.rpn_out, None, self.anchors, self.A, self.fh, self.fw, self.feat_stride, im_h, im_w, self.min_size,
-                      self.pre_n, self.post_n, self.nms_thresh, layout="nhwc", ld=self.rpn_ld, cls_is_logits=True, work=self.prop)
+        self.last_losses = self._rcnn_losses(feat, self.rpn_out, self.rpn_ld, gt_boxes, im_h, im_w, keep_inds, masks)
+        return self.last_losses
+
+    def _rcnn_losses(self, feat, rpn_out, rpn_ld, gt_boxes, im_h, im_w, keep_inds, masks):
+        """ProposalLayer on an RPN's output (fp32 [fh*fw, rpn_ld]: logits, then deltas), ProposalTargetLayer, RoI pooling,
+        the head and its losses; sets head_grad.  Returns losses float32[4] (device)."""
+        ops.proposals(rpn_out, None, self.anchors, self.A, self.fh, self.fw, self.feat_stride, im_h, im_w, self.min_size,
+                      self.pre_n, self.post_n, self.nms_thresh, layout="nhwc", ld=rpn_ld, cls_is_logits=True, work=self.prop)
         rois, count = self.prop.rois, self.prop.count
         self.max_ov, self.argmax = train_ops.roi_overlaps(rois, count, gt_boxes)
         if keep_inds is None:
@@ -738,7 +790,6 @@ class _RcnnStep(_ConvTrainer):
         self.masks = masks
         self._head_forward()
         losses, self.head_grad = train_ops.rcnn_loss(self.head_out, self.keep, self.labels, self.ext, self.num_classes, self.delta)
-        self.last_losses = losses
         return losses
 
     def _head_forward(self):
@@ -768,6 +819,11 @@ class _RcnnStep(_ConvTrainer):
     def backward(self, debug=None):
         """Fills g_flat with d(loss_rcnn)/d(parameter) for every trainable parameter.  debug: as RpnTrainer.backward, plus
         "roi": the gradient of the pooled RoIs ("dpool5") and of the feature map (fp32 [fh*fw, feat_ch], "dfeat")."""
+        self._backward_trunk(self._backward_rcnn(debug), debug)
+
+    def _backward_rcnn(self, debug=None):
+        """The head's, fc7's and fc6's gradients and the RoI pooling's backward; returns the gradient of the feature map
+        (dfeat split into the gradient activation of tag 3)."""
         R_cap, ld, C = self.post_n, self.head_ld, self.feat_ch
         twice = self.masks is not None               # ratio-0.5 dropout: dz = 2 * g * (y > 0), y = the post-dropout activation
         # ---- cls_score | bbox_pred: dY = head_grad [R_cap, ld] fp32 (zero rows for RoIs that were not kept)
@@ -811,7 +867,7 @@ class _RcnnStep(_ConvTrainer):
         self._prep(self.fh, self.fw, C, g_f32=self.dfeat, out=gfeat)
         if debug is not None:
             debug["roi"] = dict(dpool5=self._chw(gp), dfeat=self.dfeat.clone())
-        self._backward_trunk(gfeat, debug)
+        return gfeat
 
     def _roi_pool_backward(self, g):
         """dfeat = the RoI pooling's backward of g (the gradient of pool5)."""
@@ -823,6 +879,97 @@ class _RcnnStep(_ConvTrainer):
 
     def step(self, x_chw, gt_boxes, im_info=None, keep_inds=None, masks=None):
         losses = self.forward(x_chw, gt_boxes, im_info, keep_inds, masks)
+        self.backward()
+        self.update()
+        return losses
+
+
+class _RpnNames(object):
+    """The RPN step's own head in _JointStep, where the trainer's head_ld, n_heads, head_out, head_grad, delta and
+    packed["heads"] are the RCNN step's: the twin heads' `packed` key, width, output and gradient, rpn_loss's delta and the
+    anchor targets."""
+    heads_key = "RPN/heads"
+
+
+JOIN_TAG = 4        # the _gact tag of the joined feature-map gradient: no trunk's backward uses it, so it is never the
+                    # split dfeat (tag 3) it adds
+
+
+class _JointStep(_RpnStep, _RcnnStep):
+    """Approximate joint training (py-faster-rcnn's end2end recipe) over any trunk: one trunk forward, the trained RPN run
+    once, AnchorTargetLayer and rpn_loss on its output, ProposalLayer on the same logits (the proposals are constants),
+    ProposalTargetLayer, RoI pooling, fc6 / fc7 with dropout and loss_rcnn; the loss is rpn_loss + loss_rcnn.  Backward:
+    the head and the RoI pooling into dfeat, split into a gradient activation; the RPN heads' and conv's weight gradients;
+    the RPN conv's data gradient with the split dfeat added in its epilogue (frcnn_conv2d_res), so the feature map's two
+    gradients meet without a pass of their own; then the trunk.  Each half is _RpnStep's and _RcnnStep's own code; the RPN
+    half's head lives on `rpn` (_RpnNames).
+
+    Flat layout: the trunk, the RPN 3x3 conv, fc6, fc7, cls_score | bbox_pred, then the RPN's twin heads; nothing is frozen
+    and every step parameter lies after the trunk (VGG16's early exchange from conv4_1 covers only finished gradients)."""
+
+    @property
+    def _rpn(self):
+        return self.rpn
+
+    def _step_table(self, A):
+        rpn_layers, rpn_params, _ = _RpnStep._step_table(self, A)
+        _, rcnn_params, _ = _RcnnStep._step_table(self, A)
+        return rpn_layers, rcnn_params + rpn_params, []
+
+    def _joint_options(self, subsample, sample, dropout, post_n):
+        """Raises FrcnnError for a bad one-image option (before anything is allocated)."""
+        who = type(self).__name__
+        if subsample not in ("device", "numpy", "none"):
+            raise FrcnnError("%s: subsample must be one of ['device', 'none', 'numpy'] (got %r)" % (who, subsample))
+        if sample != "numpy":
+            raise FrcnnError("%s: sample must be 'numpy' (keep_inds= pins the kept rows) (got %r)" % (who, sample))
+        if dropout not in (True, False):
+            raise FrcnnError("%s: dropout must be True or False (masks= pins the masks) (got %r)" % (who, dropout))
+        if not 1 <= int(post_n) <= 4096:
+            raise FrcnnError("%s: post_n must be in [1, 4096] (got %r)" % (who, post_n))
+
+    def _init_joint(self, params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                    loss_lambda, rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size, sample,
+                    seed, dropout, optimizer=None):
+        self._joint_options(subsample, sample, dropout, post_n)
+        self.num_classes, self.rpn = num_classes, _RpnNames()
+        self._init_common(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          optimizer=optimizer)
+        self._init_rpn_head(loss_lambda, rpn_delta, subsample, seed)
+        self.rpn.targets = train_ops.AnchorTargets(self.A, self.fh, self.fw, self.device)
+        self._init_rcnn_head(rcnn_delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_rcnn_draws(sample, seed, dropout)
+        self.repack()
+
+    def repack(self):
+        self._repack_trunk()
+        self._repack_rpn()
+        self._repack_rcnn()
+
+    # ---------------------------------------------------------------- forward
+    def forward(self, x_chw, gt_boxes, im_info=None, disable_pos=None, keep_inds=None, masks=None):
+        """x_chw (3,H,W) float32 CUDA; gt_boxes [G,5] float32 CUDA; disable_pos pins the RPN's subsampling, keep_inds the
+        kept rows and masks the dropout masks, as in RpnTrainer / RcnnTrainer.  Returns losses float32[8] (device):
+        rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss, loss_cls, loss_bbox, cls_accuracy, loss_rcnn."""
+        im_h, im_w = (self.H, self.W) if im_info is None else (int(im_info[0]), int(im_info[1]))
+        feat = self._forward_trunk(x_chw)
+        self._rpn_trained_forward(feat)
+        rpn = self._rpn_losses(gt_boxes, im_h, im_w, disable_pos)
+        rcnn = self._rcnn_losses(feat, self.rpn.head_out, self.rpn.head_ld, gt_boxes, im_h, im_w, keep_inds, masks)
+        self.last_losses = torch.cat([rpn, rcnn])
+        return self.last_losses
+
+    # ---------------------------------------------------------------- backward
+    def backward(self, debug=None):
+        """Fills g_flat with d(rpn_loss + loss_rcnn)/d(parameter): the RPN's parameters from rpn_loss, the head's from
+        loss_rcnn, the trunk's from both.  debug: RcnnTrainer's head entries ("heads", "fc7", "fc6", "roi"), RpnTrainer's
+        RPN entries with the twin heads under "RPN/heads" ("RPN/rpn_conv_3x3"'s "g_out" is the joined gradient of the
+        feature map), and the trunk's."""
+        dfeat = self._backward_rcnn(debug)
+        self._backward_trunk(self._backward_rpn(debug, res=dfeat, tag=JOIN_TAG), debug)
+
+    def step(self, x_chw, gt_boxes, im_info=None, disable_pos=None, keep_inds=None, masks=None):
+        losses = self.forward(x_chw, gt_boxes, im_info, disable_pos, keep_inds, masks)
         self.backward()
         self.update()
         return losses
@@ -1009,6 +1156,12 @@ class _CanvasSteps(object):
         offsets.copy_(torch.from_numpy(offs), non_blocking=True)
 
     # ---------------------------------------------------------------- the step
+    def _advance_seeds(self):
+        """The step's last draw-related launch: when the step draws from its seeds (the step's _draws), slot n's seed moves
+        on by N, once per step, so that slot n of step t draws with seed + t*N + n."""
+        if self._draws():
+            self.seeds.add_(self.N)
+
     def run(self):
         """Enqueues forward + backward + update on the current stream, with no host synchronisation."""
         self.forward()
@@ -1055,20 +1208,27 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
         subsampling lists; then the first repack."""
         self._canvas_options(N, max_gt)
         self._augment_options(raw_input, augment, scales, flip)
-        if subsample not in self._MODES:
-            raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
+        self._subsample_options(subsample)
         self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
         self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
                           lead=(N,), optimizer=optimizer)
         self._init_rpn_head(loss_lambda, delta, subsample, seed)
         self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
-        dev = self.device
-        self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rpn_loss_batch
-        self.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, max_gt, dev)
+        self._init_canvas_rpn_targets()
         self.step_losses = self.targets.losses
-        self.disable_pos = torch.zeros((max(N * self.targets.cap, 1),), dtype=torch.int32, device=dev)
-        self.disable_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
         self.repack()
+
+    def _subsample_options(self, subsample):
+        if subsample not in self._MODES:
+            raise FrcnnError("%s: subsample must be one of %s" % (type(self).__name__, sorted(self._MODES)))
+
+    def _init_canvas_rpn_targets(self):
+        """The batched anchor targets, the twin heads' gradient and the subsampling lists."""
+        r, N, dev = self._rpn, self.N, self.device
+        r.head_grad = torch.empty_like(r.head_out)     # every element written by frcnn_rpn_loss_batch
+        r.targets = train_ops.AnchorTargetsBatch(N, self.A, self.fh, self.fw, self.max_gt, dev)
+        self.disable_pos = torch.zeros((max(N * r.targets.cap, 1),), dtype=torch.int32, device=dev)
+        self.disable_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
 
     # ---------------------------------------------------------------- staging
     def put(self, images, gt_boxes, img_infos=None, disable_pos=None):
@@ -1110,27 +1270,32 @@ class _CanvasRpnStep(_CanvasSteps, _RpnStep):
                 raise FrcnnError("%s.%s: disable lists need subsample='list' (the trainer has %r)" % (who, call, self.subsample))
             if len(disable_pos) != n_images:
                 raise FrcnnError("%s.%s: %d images and %d disable lists" % (who, call, n_images, len(disable_pos)))
-            if any(int(d.numel()) > self.targets.cap for d in disable_pos):
-                raise FrcnnError("%s.%s: a disable list is longer than %d anchors" % (who, call, self.targets.cap))
+            cap = self._rpn.targets.cap
+            if any(int(d.numel()) > cap for d in disable_pos):
+                raise FrcnnError("%s.%s: a disable list is longer than %d anchors" % (who, call, cap))
         return disable_pos
 
     # ---------------------------------------------------------------- forward
     def forward(self):
         """Forward over the staged canvas, the anchor targets and the per-slot losses (float32 [N, 4] device buffer:
         rpn_loss_cls, rpn_loss_bbox, rpn_cls_accuracy, rpn_loss; zeros for an empty slot)."""
-        (ext, k), R = self._level(self.halvings), self.rpn_layer
-        self._rpn_forward(self._forward_trunk(), self.packed[R["name"]], self.packed["heads"], R["y"], self.head_ld, self.head_out)
-        mode = self._MODES[self.subsample]
+        self._rpn_trained_forward(self._forward_trunk())
+        self.last_losses = self._rpn_losses_batch()
+        self._advance_seeds()
+        return self.last_losses
+
+    def _rpn_losses_batch(self):
+        """The batched anchor targets and rpn_loss on _rpn.head_out, with the step's seeds; fills _rpn.head_grad.  Returns
+        the per-slot losses, float32 [N, 4]."""
+        (ext, k), r = self._level(self.halvings), self._rpn
         train_ops.anchor_targets_batch(self.anchors, self.A, self.feat_stride, ext, self.im_info, self.gt, self.gt_counts,
-                                       self.targets, halvings=k, mode=mode, seeds=self.seeds, disable_pos=self.disable_pos,
-                                       disable_offsets=self.disable_offsets)
-        if mode == train_ops.SUBSAMPLE_DEVICE or self.augment == "device":
-            self.seeds.add_(self.N)
-        losses = train_ops.rpn_loss_batch(self.head_out, self.head_ld, self.anchors, self.A, self.feat_stride, ext, self.im_info,
-                                          self.targets, halvings=k, delta=self.delta, loss_lambda=self.loss_lambda,
-                                          dhead=self.head_grad)
-        self.last_losses = losses
-        return losses
+                                       r.targets, halvings=k, mode=self._MODES[self.subsample], seeds=self.seeds,
+                                       disable_pos=self.disable_pos, disable_offsets=self.disable_offsets)
+        return train_ops.rpn_loss_batch(r.head_out, r.head_ld, self.anchors, self.A, self.feat_stride, ext, self.im_info,
+                                        r.targets, halvings=k, delta=r.delta, loss_lambda=self.loss_lambda, dhead=r.head_grad)
+
+    def _draws(self):
+        return self.subsample == "device" or self.augment == "device"
 
     def step(self, images, gt_boxes, img_infos=None, disable_pos=None):
         """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
@@ -1156,21 +1321,34 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
                           raw_input, optimizer=None, augment=None, scales=(600,), flip=True):
         """Checks the options, then builds the trunk, the canvas input, the frozen RPN and the head, the batched proposals,
         targets, kept lists and masks; then the first repack."""
-        who = type(self).__name__
         self._canvas_options(N, max_gt)
         self._augment_options(raw_input, augment, scales, flip)
+        self._sampling_options(sample, dropout, post_n)
+        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
+        self.num_classes = num_classes
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          lead=(N,), optimizer=optimizer)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
+        self._frozen_rpn(params)
+        self._init_rcnn_head(delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_canvas_rcnn_targets(sample, dropout)
+        self.step_losses = self.ptargets.losses
+        self.repack()
+
+    def _sampling_options(self, sample, dropout, post_n):
+        who = type(self).__name__
         if sample not in self._SAMPLE:
             raise FrcnnError("%s: sample must be one of %s" % (who, sorted(self._SAMPLE)))
         if dropout not in self._DROPOUT:
             raise FrcnnError("%s: dropout must be one of %s" % (who, self._DROPOUT))
         if not 1 <= int(post_n) <= 4096:
             raise FrcnnError("%s: post_n must be in [1, 4096] (got %r)" % (who, post_n))
-        self.N, self.max_gt, self.num_classes = N, max_gt, nc = int(N), int(max_gt), num_classes
-        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
-                          lead=(N,), optimizer=optimizer)
-        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
-        self._init_rcnn_head(params, delta, post_n, pre_n, nms_thresh, min_size)
+
+    def _init_canvas_rcnn_targets(self, sample, dropout):
+        """The head's extents, the batched proposals, targets, kept lists and masks, the head's gradient and the RoI
+        pooling backward's workspace."""
         self.sample, self.dropout = sample, dropout
+        N, nc, pre_n, post_n = self.N, self.num_classes, self.pre_n, self.post_n
         dev, fh, fw = self.device, self.fh, self.fw
         # the head's extents (1, R_n): column 1 is the proposal count frcnn_proposals_batch_ext writes
         self.head_ext = torch.ones((N, 2), dtype=torch.int32, device=dev)
@@ -1178,14 +1356,12 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
             torch.zeros((N, post_n, 4), dtype=torch.float32, device=dev), torch.zeros((N, post_n), dtype=torch.float32, device=dev),
             self.head_ext[:, 1]))
         self.ptargets = train_ops.ProposalTargetsBatch(N, post_n, nc, dev)
-        self.step_losses = self.ptargets.losses
         self.keep_list = torch.zeros((N * train_ops.ROIS_PER_IMAGE,), dtype=torch.int32, device=dev)
         self.keep_offsets = torch.zeros((N + 1,), dtype=torch.int32, device=dev)
         self.masks = torch.zeros((2, N, post_n, 4096), dtype=torch.uint8, device=dev) if dropout is not None else None
         self.head_grad = torch.empty_like(self.head_out)     # every element written by frcnn_rcnn_loss_batch
         self.roi_ws = torch.empty((ops._lib.load().frcnn_roi_pool_backward_batch_workspace_bytes(N, fh, fw, self.feat_ch),),
                                   dtype=torch.uint8, device=dev)
-        self.repack()
 
     # ---------------------------------------------------------------- staging
     def put(self, images, gt_boxes, img_infos=None, keep_inds=None, masks=None):
@@ -1251,12 +1427,20 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
     def forward(self):
         """Forward over the staged canvas, the proposal targets and the per-slot losses (float32 [N, 4] device buffer:
         loss_cls, loss_bbox, cls_accuracy, loss_rcnn; zeros for a slot that kept nothing)."""
-        N, (ext, k), R_cap = self.N, self._level(self.halvings), self.post_n
         feat = self._forward_trunk()
         self._rpn_forward(feat, self.rpn3, self.rpn_heads, self.rpn_mid, self.rpn_ld, self.rpn_out)
-        ops.proposals_batch(self.rpn_out.view(N, self.fh * self.fw, self.rpn_ld), None, self.anchors, self.A, self.fh, self.fw,
+        self.last_losses = self._rcnn_losses_batch(feat, self.rpn_out, self.rpn_ld)
+        self._advance_seeds()
+        return self.last_losses
+
+    def _rcnn_losses_batch(self, feat, rpn_out, rpn_ld):
+        """The batched ProposalLayer on an RPN's output (fp32 [N*fh*fw, rpn_ld]), proposal targets, RoI pooling, dropout
+        masks, the head and its losses, with the step's seeds; fills head_grad.  Returns the per-slot losses, float32
+        [N, 4]."""
+        N, (ext, k), R_cap = self.N, self._level(self.halvings), self.post_n
+        ops.proposals_batch(rpn_out.view(N, self.fh * self.fw, rpn_ld), None, self.anchors, self.A, self.fh, self.fw,
                             self.feat_stride, 0, 0, self.min_size, self.pre_n, R_cap, self.nms_thresh, layout="nhwc",
-                            ld=self.rpn_ld, cls_is_logits=True, work=self.prop, extents=ext, halvings=k, im_info=self.im_info)
+                            ld=rpn_ld, cls_is_logits=True, work=self.prop, extents=ext, halvings=k, im_info=self.im_info)
         rois, count = self.prop.rois, self.head_ext[:, 1]
         train_ops.proposal_targets_batch(rois, count, self.gt, self.gt_counts, self.ptargets, mode=self._SAMPLE[self.sample],
                                          seeds=self.seeds, keep_list=self.keep_list, list_offsets=self.keep_offsets)
@@ -1265,12 +1449,11 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
         if self.dropout == "device":
             for j in range(2):
                 train_ops.dropout_masks_batch(self.seeds, j + 1, self.masks[j])
-        if self.sample == "device" or self.dropout == "device" or self.augment == "device":
-            self.seeds.add_(N)
         self._head_forward()
-        losses = train_ops.rcnn_loss_batch(self.head_out, self.ptargets, delta=self.delta, dhead=self.head_grad)
-        self.last_losses = losses
-        return losses
+        return train_ops.rcnn_loss_batch(self.head_out, self.ptargets, delta=self.delta, dhead=self.head_grad)
+
+    def _draws(self):
+        return self.sample == "device" or self.dropout == "device" or self.augment == "device"
 
     def _roi_pool_backward(self, g):
         ext, k = self._level(self.halvings)
@@ -1286,6 +1469,91 @@ class _CanvasRcnnStep(_CanvasSteps, _RcnnStep):
     def step_raw(self, photos, boxes, labels, keep_inds=None, masks=None, flips=None, scale_index=None):
         """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 4] on the device."""
         self.put_raw(photos, boxes, labels, keep_inds, masks, flips, scale_index)
+        return self._step()
+
+
+class _CanvasJointStep(_CanvasRpnStep, _CanvasRcnnStep, _JointStep):
+    """_JointStep on a canvas (CanvasJointTrainer describes it): _CanvasRpnStep's anchor targets and loss and
+    _CanvasRcnnStep's proposals, targets, RoI pooling and loss on the one RPN output, with both steps' staging."""
+
+    def _init_canvas_joint(self, params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                           rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size, sample, dropout,
+                           seed, max_gt, device, process_group, raw_input, optimizer=None, augment=None, scales=(600,),
+                           flip=True):
+        """Checks both steps' options, then builds the trunk, the RPN head, the canvas input, the head, both steps'
+        batched targets and lists; then the first repack."""
+        self._canvas_options(N, max_gt)
+        self._augment_options(raw_input, augment, scales, flip)
+        self._subsample_options(subsample)
+        self._sampling_options(sample, dropout, post_n)
+        self.N, self.max_gt = N, max_gt = int(N), int(max_gt)
+        self.num_classes, self.rpn = num_classes, _RpnNames()
+        self._init_common(params, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                          lead=(N,), optimizer=optimizer)
+        self._init_rpn_head(loss_lambda, rpn_delta, subsample, seed)
+        self._canvas_init(N, Hc, Wc, max_gt, seed, raw_input, augment, scales, flip)
+        self._init_rcnn_head(rcnn_delta, post_n, pre_n, nms_thresh, min_size)
+        self._init_canvas_rpn_targets()
+        self._init_canvas_rcnn_targets(sample, dropout)
+        self.repack()
+
+    @property
+    def step_losses(self):
+        """The last step's per-slot losses, float32 [N, 8]: the RPN step's four, then the RCNN step's."""
+        return torch.cat([self.rpn.targets.losses, self.ptargets.losses], dim=1)
+
+    # ---------------------------------------------------------------- staging
+    def put(self, images, gt_boxes, img_infos=None, disable_pos=None, keep_inds=None, masks=None):
+        """Stages up to N images with their ground truth and clip bounds, as CanvasRpnTrainer.put, with both steps' pins:
+        disable lists (subsample="list"), kept lists (sample="list") and masks (dropout="explicit").  Raises FrcnnError
+        before anything is queued when something does not fit."""
+        self._need_input("put")
+        images, gt_boxes = list(images), list(gt_boxes)
+        self._check_gt(images, gt_boxes)
+        disable_pos = self._check_disable("put", len(images), disable_pos)
+        keep_inds, masks = self._check_extras("put", len(images), keep_inds, masks)
+        self._stage(images, gt_boxes, img_infos)
+        self._stage_pins(disable_pos, keep_inds, masks)
+
+    def put_raw(self, photos, boxes, labels, disable_pos=None, keep_inds=None, masks=None, flips=None, scale_index=None):
+        """put() for a trainer built with raw_input=True, as CanvasRpnTrainer.put_raw.  Returns [im_scale] (with augment:
+        each photo's candidate im_scale tuple)."""
+        self._need_input("put_raw")
+        photos = list(photos)
+        disable_pos = self._check_disable("put_raw", len(photos), disable_pos)
+        keep_inds, masks = self._check_extras("put_raw", len(photos), keep_inds, masks)
+        scales = self._stage_raw(photos, boxes, labels, flips, scale_index)
+        self._stage_pins(disable_pos, keep_inds, masks)
+        return scales
+
+    def _stage_pins(self, disable_pos, keep_inds, masks):
+        if self.subsample == "list":
+            self._stage_lists(disable_pos, self.N, self.disable_pos, self.disable_offsets)
+        self._stage_extras(keep_inds, masks)
+
+    # ---------------------------------------------------------------- forward
+    def forward(self):
+        """Forward over the staged canvas and both steps' per-slot losses, float32 [N, 8] (step_losses)."""
+        feat = self._forward_trunk()
+        self._rpn_trained_forward(feat)
+        self._rpn_losses_batch()
+        self._rcnn_losses_batch(feat, self.rpn.head_out, self.rpn.head_ld)
+        self._advance_seeds()
+        self.last_losses = self.step_losses
+        return self.last_losses
+
+    def _draws(self):
+        return _CanvasRpnStep._draws(self) or _CanvasRcnnStep._draws(self)
+
+    def step(self, images, gt_boxes, img_infos=None, disable_pos=None, keep_inds=None, masks=None):
+        """put() + run(), captured into a CUDA graph after the first call (_CanvasSteps._step).  Returns the per-slot
+        losses, float32 [N, 8] on the device."""
+        self.put(images, gt_boxes, img_infos, disable_pos, keep_inds, masks)
+        return self._step()
+
+    def step_raw(self, photos, boxes, labels, disable_pos=None, keep_inds=None, masks=None, flips=None, scale_index=None):
+        """put_raw() + run(), captured like step().  Returns the per-slot losses, float32 [N, 8] on the device."""
+        self.put_raw(photos, boxes, labels, disable_pos, keep_inds, masks, flips, scale_index)
         return self._step()
 
 
@@ -1376,3 +1644,51 @@ class CanvasRcnnTrainer(_Vgg16Trunk, _CanvasRcnnStep):
         self._init_canvas_rcnn(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, num_classes,
                                delta, post_n, pre_n, nms_thresh, min_size, sample, dropout, seed, max_gt, device,
                                process_group, raw_input, optimizer=optimizer, augment=augment, scales=scales, flip=flip)
+
+
+class JointTrainer(_Vgg16Trunk, _JointStep):
+    """One approximate-joint-training step (py-faster-rcnn's end2end recipe; the four losses the reference's train.py
+    reports together): trunk -> the trained RPN, once -> AnchorTargetLayer + rpn_loss, and ProposalLayer on the same logits
+    -> ProposalTargetLayer -> RoI pooling -> fc6 / fc7 with dropout -> cls_score | bbox_pred -> loss_rcnn; backward of
+    rpn_loss + loss_rcnn (the RPN's parameters from rpn_loss, the head's from loss_rcnn, the trunk's from both; no gradient
+    through the proposals' coordinates) -> WeightDecay + the optimizer's rule on every parameter.  export_params() is a
+    whole detector, which Engine loads.
+
+    The arguments are RpnTrainer's and RcnnTrainer's, rpn_delta and rcnn_delta being their two deltas.  Draws: the RPN's
+    subsampling as RpnTrainer's (its seed counter, or NumPy's global RNG with subsample="numpy"), the kept rows as
+    RcnnTrainer's (NumPy, after the RPN's draws) and the masks from a torch generator seeded with `seed`; disable_pos,
+    keep_inds and masks pin them.  The proposal counts default to RcnnTrainer's test-mode ones; pass pre_n=12000,
+    post_n=2000 for py-faster-rcnn's training counts."""
+
+    def __init__(self, params, H, W, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, loss_lambda=1.0, rpn_delta=3.0, subsample="device", num_classes=21, rcnn_delta=1.0,
+                 post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16, sample="numpy", seed=0, dropout=True, device="cuda",
+                 process_group=None, optimizer=None):
+        self._init_joint(params, H, W, anchors, precision, lr, momentum, weight_decay, feat_stride, device, process_group,
+                         loss_lambda, rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size,
+                         sample, seed, dropout, optimizer=optimizer)
+
+
+class CanvasJointTrainer(_Vgg16Trunk, _CanvasJointStep):
+    """JointTrainer's step on N images of different sizes per update, with one set of weights and optimizer state and one
+    captured CUDA graph (a multi-rank run stays eager, with the trunk's gradient exchange).
+
+    The forward is CanvasRpnTrainer's trunk and RPN, run once, its batched anchor targets and loss, then
+    CanvasRcnnTrainer's batched proposals (on the same RPN output), targets, RoI pooling, head and loss; the backward is
+    the head's, then the RPN's with the split dfeat added in the RPN conv's data gradient, then the trunk's.  The gradient
+    is the sum over the slots.  Inside each image everything equals JointTrainer's on that image alone with the same draws.
+    Per-slot losses, float32 [N, 8]: the RPN's four, then the RCNN's.
+
+    Draws: slot n of step t uses seed + t*N + n for the anchor subsampling, the RoI sampling, both dropout masks and the
+    augmentation, and the step advances the seeds once, so step 0 draws the labels CanvasRpnTrainer(seed=seed) draws and the
+    kept rows and masks CanvasRcnnTrainer(seed=seed) draws on the same proposals.  subsample / sample / dropout / augment
+    and their pins (disable_pos, keep_inds, masks, flips, scale_index) are those two trainers'."""
+
+    def __init__(self, params, N, Hc, Wc, anchors, precision="bf16x3", lr=0.001, momentum=0.9, weight_decay=0.0005,
+                 feat_stride=16, loss_lambda=1.0, rpn_delta=3.0, subsample="device", num_classes=21, rcnn_delta=1.0,
+                 post_n=300, pre_n=6000, nms_thresh=0.7, min_size=16, sample="device", dropout="device", seed=0, max_gt=256,
+                 device="cuda", process_group=None, raw_input=False, optimizer=None, augment=None, scales=(600,), flip=True):
+        self._init_canvas_joint(params, N, Hc, Wc, anchors, precision, lr, momentum, weight_decay, feat_stride, loss_lambda,
+                                rpn_delta, subsample, num_classes, rcnn_delta, post_n, pre_n, nms_thresh, min_size, sample,
+                                dropout, seed, max_gt, device, process_group, raw_input, optimizer=optimizer, augment=augment,
+                                scales=scales, flip=flip)
